@@ -196,9 +196,36 @@ int s3b_gemm_bench(int64_t m, int32_t n, int32_t k, int32_t gelu, int32_t force_
 /* y = LayerNorm_D(x) (eps 1e-5), optional GELU; D in {512,768,1024,1280} */
 int s3b_layernorm_f32(const float* x, int64_t m, int32_t d, const float* gamma, const float* beta, int32_t gelu,
                       float* out, void* stream);
-/* softmax(q k^T / 8 + key padding mask) v per (batch, head); q,k,v: [batch][T][heads*64] fp32 */
+/* softmax(q k^T / 8 + key padding mask) v per (batch, head); q,k,v: [batch][T][heads*64] fp32; valid_frames: host,
+ * [batch], each in [1, t]. The context comes back from bf16 hi/lo planes. = s3b_attention_ex with opts NULL. */
 int s3b_attention_f32(const float* q, const float* k, const float* v, const int32_t* valid_frames, int32_t batch,
                       int32_t t, int32_t heads, float* out, void* stream);
+/* Options of s3b_attention_ex (zero-initialise, set struct_size = sizeof(s3b_attention_opts)).
+ *  rel_emb      : optional DEVICE fp32 [num_buckets][heads] (relative_attention_bias.weight, wavlm/modules.py:450-462):
+ *                 scores get gate[b][h][q] * rel_emb[bucket(k - q)][h] before the key mask, through the table the
+ *                 model builds (Toeplitz table for table_frames frames)
+ *  table_frames : frames the table is built for (0 = 4096, as s3b_model_finalize); must be >= t
+ *  gate         : optional DEVICE fp32 [batch][heads][t] (needs rel_emb); NULL = 1
+ *  ctx_format   : operand format the kernel writes the context in: 0 = bf16 hi/lo, 1 = f16q8 (fp16 + e4m3 residual);
+ *                 out is decoded from those planes with the arithmetic the library's kernels read an operand back with */
+typedef struct s3b_attention_opts {
+    int32_t struct_size;
+    int32_t ctx_format;
+    const float* rel_emb;
+    int32_t num_buckets;
+    int32_t max_distance;
+    const float* gate;
+    int32_t table_frames;
+    int32_t reserved32;
+    int64_t reserved[2];
+} s3b_attention_opts;
+int s3b_attention_ex(const float* q, const float* k, const float* v, const int32_t* valid_frames, int32_t batch,
+                     int32_t t, int32_t heads, const s3b_attention_opts* opts, float* out, void* stream);
+/* WavLM gate (wavlm/modules.py:534-551) through the model's kernel: x [batch][t][heads*64] fp32 is first written into
+ * operand planes of x_format (0 = bf16 hi/lo, 1 = f16q8) like a LayerNorm output; grep_w [8][64], grep_b [8],
+ * grep_a [heads] (grep_w NULL = gru_rel_pos off: gate 1). gate_out: DEVICE [batch][heads][t] fp32. */
+int s3b_wavlm_gate_f32(const float* x, int32_t batch, int32_t t, int32_t heads, const float* grep_w,
+                       const float* grep_b, const float* grep_a, int32_t x_format, float* gate_out, void* stream);
 
 #ifdef __cplusplus
 }

@@ -392,6 +392,14 @@ static int build_rel_table(s3b_model* m, int Tmax) {
     return 0;
 }
 
+// The attention kernel's view of a table built for Tmax frames: row h starts at h * (2 Tmax - 1), and k - q = 0 sits
+// at column Tmax - 1. The model's plans and s3b_attention_ex both go through here.
+static void set_rel_bias(AttnParams& ap, const float* table, int Tmax, const float* gate) {
+    ap.bias_table = table;
+    ap.bias_stride = 2 * Tmax - 1, ap.bias_center = Tmax - 1;
+    ap.gate = gate;
+}
+
 extern "C" int s3b_model_finalize(s3b_model* m) {
     if (!m) return fail("null model");
     if (m->finalized) return 0;
@@ -1183,11 +1191,7 @@ int Fwd::build_plan(Plan& pl) {
             TMAP_OK(encode_tmap_bf16_3d(&ap.vt_lo, w->vt_s.l(), T, 64, BH, Tp, (uint64_t)64 * Tp, 64, 64));
             ap.B = B, ap.H = H, ap.T = T, ap.D = D;
             ap.kv_len = d_kv;
-            if (c.relative_position) {
-                ap.bias_table = m->rel_table.as<float>();
-                ap.bias_stride = 2 * m->rel_table_T - 1, ap.bias_center = m->rel_table_T - 1;
-                ap.gate = w->gate.as<float>();
-            }
+            if (c.relative_position) set_rel_bias(ap, m->rel_table.as<float>(), m->rel_table_T, w->gate.as<float>());
             ap.ctx = w->ctx_s.planes(m->scheme);
         }
         {   // out_proj + residual (residual = hidden state l, patched per call)
@@ -1959,16 +1963,36 @@ extern "C" int s3b_layernorm_f32(const float* x, int64_t M, int32_t D, const flo
     return 0;
 }
 
-extern "C" int s3b_attention_f32(const float* q, const float* k, const float* v, const int32_t* valid_frames,
-                                 int32_t B, int32_t T, int32_t H, float* out, void* stream) {
+extern "C" int s3b_attention_ex(const float* q, const float* k, const float* v, const int32_t* valid_frames,
+                                int32_t B, int32_t T, int32_t H, const s3b_attention_opts* opts, float* out,
+                                void* stream) {
     // Runs the production path: identity "QKV GEMM" is replaced by a scatter of the given q/k/v, then the
-    // attention kernel, then ctx hi+lo is recombined to fp32.
+    // attention kernel (WavLM bias table built by the model's own launcher), then the context planes are decoded to fp32.
     if (!q || !k || !v || !valid_frames || !out) return fail("null argument");
+    if (B < 1 || T < 1 || H < 1) return fail("bad sizes");
+    s3b_attention_opts o;
+    memset(&o, 0, sizeof(o));
+    if (opts != nullptr) {
+        if (opts->struct_size != (int32_t)sizeof(s3b_attention_opts))
+            return fail("s3b_attention_opts.struct_size %d != %d (header / library mismatch)", opts->struct_size,
+                        (int)sizeof(s3b_attention_opts));
+        o = *opts;
+    }
+    if (o.ctx_format != 0 && o.ctx_format != 1) return fail("ctx_format must be 0 (bf16 hi/lo) or 1 (f16q8)");
+    if (o.gate != nullptr && o.rel_emb == nullptr) return fail("a gate needs rel_emb");
+    const int table_T = o.table_frames != 0 ? o.table_frames : 4096;  // s3b_model_finalize's table
+    if (o.rel_emb != nullptr) {
+        if (o.num_buckets < 4 || o.max_distance <= o.num_buckets / 4)
+            return fail("num_buckets %d / max_distance %d out of range", o.num_buckets, o.max_distance);
+        if (table_T < T) return fail("table_frames %d is below t = %d", table_T, T);
+    }
+    for (int b = 0; b < B; ++b)
+        if (valid_frames[b] < 1 || valid_frames[b] > T) return fail("valid_frames[%d] = %d not in [1, %d]", b, valid_frames[b], T);
     cudaStream_t st = (cudaStream_t)stream;
     const int D = H * 64, Tp = (T + 7) & ~7;
     const size_t M = (size_t)B * T;
     SplitBuf qs, ks, vts, ctx;
-    DevBuf kv;
+    DevBuf kv, table;
     S3B_OK(qs.ensure(M * D));
     S3B_OK(ks.ensure(M * D));
     S3B_OK(vts.ensure((size_t)B * H * 64 * Tp));
@@ -1986,7 +2010,12 @@ extern "C" int s3b_attention_f32(const float* q, const float* k, const float* v,
     TMAP_OK(encode_tmap_bf16_3d(&ap.vt_hi, vts.h(), T, 64, BH, Tp, (uint64_t)64 * Tp, 64, 64));
     TMAP_OK(encode_tmap_bf16_3d(&ap.vt_lo, vts.l(), T, 64, BH, Tp, (uint64_t)64 * Tp, 64, 64));
     ap.B = B, ap.H = H, ap.T = T, ap.D = D, ap.kv_len = kv.as<int>();
-    ap.ctx = ctx.planes(0);
+    if (o.rel_emb != nullptr) {
+        S3B_OK(table.ensure((size_t)H * (2 * (size_t)table_T - 1) * 4));
+        CUDA_OK(launch_wavlm_rel_table(o.rel_emb, o.num_buckets, o.max_distance, H, table_T, table.as<float>(), st));
+        set_rel_bias(ap, table.as<float>(), table_T, o.gate);
+    }
+    ap.ctx = ctx.planes(o.ctx_format);
     DevBuf trace;
     const char* tb = getenv("S3B_ATTN_TRACE_BLOCK");  // debug: dump a clock64 timeline of one CTA to stderr
     if (tb != nullptr) {
@@ -2010,10 +2039,37 @@ extern "C" int s3b_attention_f32(const float* q, const float* k, const float* v,
             }
         trace.release();
     }
-    CUDA_OK(launch_unsplit(ctx.h(), ctx.l(), M * D, out, st));
+    CUDA_OK(launch_planes_to_f32(ctx.planes(o.ctx_format), M * D, out, st));
     cudaError_t se = cudaStreamSynchronize(st);
-    qs.release(), ks.release(), vts.release(), ctx.release(), kv.release();
+    qs.release(), ks.release(), vts.release(), ctx.release(), kv.release(), table.release();
     if (se != cudaSuccess) return fail("attention execution failed: %s", cudaGetErrorString(se));
+    return 0;
+}
+
+extern "C" int s3b_attention_f32(const float* q, const float* k, const float* v, const int32_t* valid_frames,
+                                 int32_t B, int32_t T, int32_t H, float* out, void* stream) {
+    return s3b_attention_ex(q, k, v, valid_frames, B, T, H, nullptr, out, stream);
+}
+
+extern "C" int s3b_wavlm_gate_f32(const float* x, int32_t B, int32_t T, int32_t H, const float* grep_w,
+                                  const float* grep_b, const float* grep_a, int32_t x_format, float* gate_out,
+                                  void* stream) {
+    // x goes into operand planes the way the model's producers write them (activation split, e4m3 residual scaled by
+    // 2^11 in f16q8), then the production gate kernel reads it back from there
+    if (!x || !gate_out || (grep_w && (!grep_b || !grep_a))) return fail("null argument");
+    if (B < 1 || T < 1 || H < 1) return fail("bad sizes");
+    if (x_format != 0 && x_format != 1) return fail("x_format must be 0 (bf16 hi/lo) or 1 (f16q8)");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int D = H * 64;
+    const size_t M = (size_t)B * T;
+    SplitBuf xs;
+    S3B_OK(xs.ensure(M * D));
+    if (x_format != 0) CUDA_OK(launch_split_q8(x, xs.h(), xs.h8(), xs.l8(), M * D, 0, st));
+    else CUDA_OK(launch_split(x, xs.h(), xs.l(), M * D, st));
+    CUDA_OK(launch_wavlm_gate(xs.planes(x_format), M, B, T, H, D, grep_w, grep_b, grep_a, gate_out, st));
+    cudaError_t se = cudaStreamSynchronize(st);
+    xs.release();
+    if (se != cudaSuccess) return fail("gate execution failed: %s", cudaGetErrorString(se));
     return 0;
 }
 

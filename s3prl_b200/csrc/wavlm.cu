@@ -151,14 +151,17 @@ cudaError_t launch_qkv_scatter(const float* q, const float* k, const float* v, i
     return cudaGetLastError();
 }
 
-__global__ void unsplit_kernel(const __nv_bfloat16* __restrict__ hi, const __nv_bfloat16* __restrict__ lo, size_t n,
-                               float* __restrict__ out) {
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-        out[i] = __bfloat162float(hi[i]) + __bfloat162float(lo[i]);
+// the value a consumer of the operand sees: the same decode as load_planes2, element pairs
+__global__ void planes_to_f32_kernel(const OutPlanes p, size_t n2, float* __restrict__ out) {
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n2; i += (size_t)gridDim.x * blockDim.x) {
+        const float2 v = load_planes2(p, 2 * i);
+        out[2 * i] = v.x, out[2 * i + 1] = v.y;
+    }
 }
 
-cudaError_t launch_unsplit(const __nv_bfloat16* hi, const __nv_bfloat16* lo, size_t n, float* out, cudaStream_t s) {
-    unsplit_kernel<<<132 * 4, 256, 0, s>>>(hi, lo, n, out);
+cudaError_t launch_planes_to_f32(const OutPlanes& p, size_t n, float* out, cudaStream_t s) {
+    if (n & 1) return cudaErrorInvalidValue;
+    planes_to_f32_kernel<<<132 * 4, 256, 0, s>>>(p, n / 2, out);
     return cudaGetLastError();
 }
 

@@ -47,6 +47,8 @@ EXPORTED_SYMBOLS = [
     "s3b_layernorm_f32",
     "s3b_gemm_bench",
     "s3b_attention_f32",
+    "s3b_attention_ex",
+    "s3b_wavlm_gate_f32",
     "s3b_fbank",
     "s3b_fbank_num_frames",
     "s3b_trimmed_lengths",
@@ -100,6 +102,26 @@ class S3BForwardOpts(C.Structure):
     def __init__(self, **kw):
         super().__init__(**kw)
         self.struct_size = C.sizeof(S3BForwardOpts)
+
+
+class S3BAttentionOpts(C.Structure):
+    """Mirror of ``struct s3b_attention_opts``."""
+
+    _fields_ = [
+        ("struct_size", C.c_int32),
+        ("ctx_format", C.c_int32),
+        ("rel_emb", C.c_void_p),
+        ("num_buckets", C.c_int32),
+        ("max_distance", C.c_int32),
+        ("gate", C.c_void_p),
+        ("table_frames", C.c_int32),
+        ("reserved32", C.c_int32),
+        ("reserved", C.c_int64 * 2),
+    ]
+
+    def __init__(self, **kw):
+        super().__init__(**kw)
+        self.struct_size = C.sizeof(S3BAttentionOpts)
 
 
 FAMILY_HUBERT, FAMILY_WAV2VEC2, FAMILY_WAVLM, FAMILY_DISTILLER = 0, 1, 2, 3
@@ -161,6 +183,9 @@ def load() -> C.CDLL:
     lib.s3b_gemm_bench.argtypes = [i64, i32, i32, i32, i32, i32, C.POINTER(C.c_float)]
     lib.s3b_layernorm_f32.argtypes = [f32p, i64, i32, f32p, f32p, i32, f32p, vp]
     lib.s3b_attention_f32.argtypes = [f32p, f32p, f32p, C.POINTER(i32), i32, i32, i32, f32p, vp]
+    lib.s3b_attention_ex.argtypes = [f32p, f32p, f32p, C.POINTER(i32), i32, i32, i32, C.POINTER(S3BAttentionOpts),
+                                     f32p, vp]
+    lib.s3b_wavlm_gate_f32.argtypes = [f32p, i32, i32, i32, f32p, f32p, f32p, i32, f32p, vp]
     lib.s3b_fbank_num_frames.argtypes = [i64]
     lib.s3b_fbank_num_frames.restype = i64
     lib.s3b_fbank.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, f32p, vp]

@@ -1,6 +1,7 @@
-"""GPU parity tests of the building-block entry points of the C ABI (GEMM, LayerNorm, attention)
-against fp64 torch math on the same inputs. Tolerance: the north_star bar is 1e-3 relative on hidden
-states; single blocks are held to 1e-4 relative Frobenius / 2e-4 of the output scale elementwise."""
+"""GPU parity tests of the building-block entry points of the C ABI (GEMM, LayerNorm, attention with and without
+WavLM's gated relative-position bias, the WavLM gate) against fp64 torch math on the same inputs. Tolerance: the
+north_star bar is 1e-3 relative on hidden states; single blocks are held to 1e-4 relative Frobenius / 2e-4 of the
+output scale elementwise, or to a bound derived from the inputs where that bar does not apply (stated per test)."""
 import ctypes as C
 
 import pytest
@@ -120,3 +121,318 @@ def test_attention(s3b_lib, B, T, H, valid):
     rel = _rel(out, ref)
     print(f"attention B={B} T={T} H={H}: rel={rel:.3e}")
     assert rel < 1e-4, rel
+
+
+# ------------------------------------------------------------------------------------------------
+# WavLM gated relative-position bias, context operand formats, softmax edges (s3b_attention_ex) and the
+# gate kernel (s3b_wavlm_gate_f32), against fp64 torch on the same inputs
+# ------------------------------------------------------------------------------------------------
+NUM_BUCKETS, MAX_DISTANCE = 320, 800  # WavLM base / large
+# c of the score error budget (_attention_ref): the softmax normalisation carries a score error twice (numerator and
+# denominator)
+C_SCORE = 2.0
+
+
+def _oracle():
+    import sys
+    from pathlib import Path
+
+    root = str(Path(__file__).resolve().parents[1] / "oracle")
+    if root not in sys.path:
+        sys.path.insert(0, root)
+    import upstream_oracle
+
+    return upstream_oracle
+
+
+def _attention_ex(q, k, v, valid, H, emb=None, gate=None, table_frames=0, ctx_format=0):
+    from s3prl_b200 import lib
+
+    B, T, _ = q.shape
+    out = torch.full_like(q, float("nan"))
+    opts = lib.S3BAttentionOpts(ctx_format=ctx_format, table_frames=table_frames)
+    if emb is not None:
+        opts.rel_emb, opts.num_buckets, opts.max_distance = emb.data_ptr(), NUM_BUCKETS, MAX_DISTANCE
+    if gate is not None:
+        opts.gate = gate.data_ptr()
+    vf = (C.c_int32 * B)(*valid)
+    lib.check(lib.load().s3b_attention_ex(_ptr(q), _ptr(k), _ptr(v), vf, B, T, H, C.byref(opts), _ptr(out), _stream()))
+    torch.cuda.synchronize()
+    return out
+
+
+def _attention_ref(q, k, v, valid, H, emb=None, gate=None):
+    """fp64: softmax(q k^T / 8 + gate[b, h, q] * emb[bucket(k - q), h] + key mask) v, plus the per-element error budget
+    of the kernel (see _row_bound)."""
+    B, T, D = q.shape
+    qh, kh, vh = (t.double().view(B, T, H, 64).transpose(1, 2) for t in (q, k, v))
+    s = qh @ kh.transpose(-1, -2) * 0.125
+    if emb is not None:
+        pos = torch.arange(T)
+        bucket = _oracle().wavlm_relative_bucket(pos[None, :] - pos[:, None], NUM_BUCKETS, MAX_DISTANCE)  # [q, k]
+        bias = emb.double()[bucket.to(emb.device)].permute(2, 0, 1)  # [H, q, k]
+        g = torch.ones(B, H, T, dtype=torch.float64, device=q.device) if gate is None else gate.double()
+        s = s + g[..., None] * bias[None]
+    mask = torch.arange(T, device=q.device)[None, :] >= torch.tensor(valid, device=q.device)[:, None]
+    s = s.masked_fill(mask[:, None, None, :], float("-inf"))
+    p = s.softmax(-1)
+    ref = (p @ vh).transpose(1, 2).reshape(B, T, D)
+    # score error budget of the bf16 hi/lo products: eps_row = C_SCORE * 2^-15 * max_k sum_d |q_d k_d| / 8 (natural-log
+    # units, valid keys only); the output error then stays below (eps_row + 2^-15) * sum_k p_k |v_k| (2^-15: P and O
+    # rounded through bf16 hi/lo planes, exp2.approx)
+    qk_abs = (qh.abs() @ kh.abs().transpose(-1, -2) * 0.125).masked_fill(mask[:, None, None, :], 0.0)
+    eps_row = C_SCORE * 2.0**-15 * qk_abs.amax(-1, keepdim=True)
+    budget = ((eps_row + 2.0**-15) * (p @ vh.abs())).transpose(1, 2).reshape(B, T, D)
+    return ref, budget
+
+
+def _check_fp32(out, ref, what, budget=None):
+    """N(0, 1)-scale logits: 1e-4 relative Frobenius and 2e-4 of the output scale elementwise (the block bar above);
+    with `budget`, every element also within the derived per-row bound."""
+    assert torch.isfinite(out).all(), what
+    rel = _rel(out, ref)
+    err = (out.double() - ref).abs()
+    assert rel < 1e-4, (what, rel)
+    assert err.max().item() < 2e-4 * ref.abs().max().item() + 1e-6, (what, err.max().item())
+    ratio = 0.0
+    if budget is not None:
+        ratio = (err / budget).max().item()
+        assert ratio < 1.0, (what, ratio)
+    return rel, ratio
+
+
+def _ulp16(x):
+    """fp16 ulp of |x| (normal range; 2^-24 below it)."""
+    e = torch.floor(torch.log2(x.abs().clamp_min(2.0**-14)))
+    return torch.exp2(e - 10)
+
+
+def _emulate_f16q8(x):
+    """The activation f16q8 operand as the GEMMs read it: h16 + e4m3((x - h16) * 2^11) * 2^-11."""
+    h16 = x.half()
+    l8 = ((x - h16.double()) * 2.0**11).float().to(torch.float8_e4m3fn)
+    return h16.double() + l8.double() * 2.0**-11
+
+
+def _check_f16q8(out1, out0, ref, what):
+    """Context written as fp16 + e4m3 residual (ctx_format 1), decoded like load_planes2.
+    Against fp64: the same bar as format 0. Against the reference emulated through the format: the kernel's own fp32
+    error (measured through the bf16 hi/lo planes of the same run, out0; those hold 16 significand bits: 2^-16) plus
+    one e4m3 rounding on each side (the kernel's and the emulation's), each <= 2^-5 fp16 ulp (3 bits kept of a
+    residual <= half an ulp) + 2^-21 (below e4m3's normal range, 2^-6 at scale 2^11, its step is 2^-9: half of it
+    unscaled). Above |x| ~ 2^-9 that is well under the half ulp a dropped residual costs."""
+    _check_fp32(out1, ref, what)
+    emu = _emulate_f16q8(ref)
+    ulp = _ulp16(torch.maximum(ref.abs(), out0.double().abs()))
+    bound = (out0.double() - ref).abs() + 2.0**-16 * ref.abs() + 2 * (2.0**-5 * ulp + 2.0**-21)
+    ratio = ((out1.double() - emu).abs() / bound).max().item()
+    assert ratio < 1.0, (what, ratio)
+    return ratio
+
+
+def _run_both_formats(q, k, v, valid, H, ref, what, budget=None, **kw):
+    out0 = _attention_ex(q, k, v, valid, H, ctx_format=0, **kw)
+    rel, r_row = _check_fp32(out0, ref, what + " ctx bf16x2", budget)
+    out1 = _attention_ex(q, k, v, valid, H, ctx_format=1, **kw)
+    r_fmt = _check_f16q8(out1, out0, ref, what + " ctx f16q8")
+    return rel, r_row, r_fmt
+
+
+BIAS_CASES = {  # T -> ragged valid_frames (incl. 1, 64, 65 and T); 999 / 1025 reach |k - q| > 800: the clamp bucket
+    2: [2, 1],
+    37: [37, 1, 30],
+    130: [130, 64, 65],
+    499: [499, 1, 64, 65],
+    999: [999, 640, 65],
+    1025: [1025, 64, 1],
+}
+
+
+@pytest.mark.parametrize("emb_std", [0.5, 4.0])
+@pytest.mark.parametrize("gate_kind", ["none", "const", "random"])
+@pytest.mark.parametrize("T", sorted(BIAS_CASES))
+@pytest.mark.parametrize("H", [12, 16])
+def test_attention_wavlm_bias(s3b_lib, H, T, gate_kind, emb_std):
+    """WavLM relative-position bias through the model's table (launch_wavlm_rel_table, centre / stride as in the model's
+    plans), gated per (b, h, q), for a table built for exactly T frames (centre T - 1) and for the model's 4096, with the
+    context in both operand formats. emb std 0.5 is fabricate_state_dict's; std 4 makes the bias dominate the softmax.
+    The bias is added in fp32 after the products, so the N(0, 1) bar needs no widening."""
+    valid = BIAS_CASES[T]
+    B, D = len(valid), H * 64
+    g = torch.Generator(device="cuda").manual_seed(H * 10007 + T * 31 + int(emb_std * 8) + len(gate_kind))
+    q, k, v = (torch.randn(B, T, D, device="cuda", generator=g) for _ in range(3))
+    emb = torch.randn(NUM_BUCKETS, H, device="cuda", generator=g) * emb_std
+    gate = None
+    if gate_kind == "const":
+        gate = torch.full((B, H, T), 1.75, device="cuda")
+    elif gate_kind == "random":  # the gate's range: (1, max(2, 1 + grep_a)), grep_a ~ 1.3
+        gate = 1.0 + 1.3 * torch.rand(B, H, T, device="cuda", generator=g)
+    ref, _ = _attention_ref(q, k, v, valid, H, emb, gate)
+    worst = [0.0, 0.0]
+    for tf in (T, 0):
+        rel, _, r_fmt = _run_both_formats(q, k, v, valid, H, ref, f"H={H} T={T} table={tf}", emb=emb, gate=gate,
+                                          table_frames=tf)
+        worst = [max(worst[0], rel), max(worst[1], r_fmt)]
+    print(f"biased attention H={H} T={T} gate={gate_kind} std={emb_std}: rel={worst[0]:.3e} f16q8/bound={worst[1]:.3f}")
+
+
+@pytest.mark.parametrize("bias", [False, True])
+@pytest.mark.parametrize("T", [1, 2, 3, 7, 8, 9])
+def test_attention_tiny_tiles(s3b_lib, T, bias):
+    """T != Tp and TMA boxes that hang off the end of every tensor: one key block, one partial query tile."""
+    H = 12
+    valid = sorted({T, max(1, T // 2), 1}, reverse=True)
+    B, D = len(valid), H * 64
+    g = torch.Generator(device="cuda").manual_seed(T * 2 + bias)
+    q, k, v = (torch.randn(B, T, D, device="cuda", generator=g) for _ in range(3))
+    emb = torch.randn(NUM_BUCKETS, H, device="cuda", generator=g) if bias else None
+    gate = 1.0 + torch.rand(B, H, T, device="cuda", generator=g) if bias else None
+    ref, budget = _attention_ref(q, k, v, valid, H, emb, gate)
+    _, r_row, r_fmt = _run_both_formats(q, k, v, valid, H, ref, f"T={T} bias={bias}", budget, emb=emb, gate=gate)
+    print(f"tiny tile T={T} bias={bias}: row bound ratio {r_row:.3f}, f16q8/bound {r_fmt:.3f}")
+
+
+def _dominant_inputs(B, T, H, where, g):
+    """q = N(0, 1) + 4u, keys N(0, 1) except one key 40u (|u| = 1): its logit is ~20, the others ~N(0, 1.1)."""
+    D = H * 64
+    u = torch.full((64,), 0.125, device="cuda")
+    q = torch.randn(B, T, H, 64, device="cuda", generator=g) + 4 * u
+    k = torch.randn(B, T, H, 64, device="cuda", generator=g)
+    v = torch.randn(B, T, H, 64, device="cuda", generator=g)
+    k[:, where] = 40 * u
+    return q.reshape(B, T, D), k.reshape(B, T, D), v.reshape(B, T, D)
+
+
+@pytest.mark.parametrize("bias", [False, True])
+def test_attention_dominant_key(s3b_lib, bias):
+    """One key that outweighs all others: in the first key block, in the last, and at masked positions (inside the
+    last partial block and beyond it). A masked key gets exactly zero weight even with the largest logit and bias:
+    its value is 1e30, which any weight above zero would show."""
+    H, T = 12, 300
+    g = torch.Generator(device="cuda").manual_seed(17 + bias)
+    emb = gate = None
+    if bias:  # later keys (k - q > 0: buckets 160..319) get the largest bias, so the masked tail tops every row
+        emb = torch.randn(NUM_BUCKETS, H, device="cuda", generator=g)
+        emb[NUM_BUCKETS // 2 :] += 6.0
+        gate = 1.0 + torch.rand(1, H, T, device="cuda", generator=g)
+    for where, valid in ((3, [T]), (T - 2, [T]), ([150, 190, 260], [150]), ([200, 140], [130])):
+        q, k, v = _dominant_inputs(1, T, H, where, g)
+        v[:, valid[0] :] = 1e30
+        gb = None if gate is None else gate
+        ref, budget = _attention_ref(q, k, v, valid, H, emb, gb)
+        _, r_row, r_fmt = _run_both_formats(q, k, v, valid, H, ref, f"dominant at {where} valid={valid}", budget,
+                                            emb=emb, gate=gb)
+        print(f"dominant key at {where} valid={valid} bias={bias}: row bound ratio {r_row:.3f}, f16q8/bound {r_fmt:.3f}")
+
+
+@pytest.mark.parametrize("bias", [False, True])
+def test_attention_rising_max(s3b_lib, bias):
+    """Every row's running max rises block after block (logits grow with the key index, by the scores or by the bias),
+    so every block rescales O by alpha < 1; the last block holds most of the weight."""
+    H, T = 12, 320
+    B, D = 2, H * 64
+    g = torch.Generator(device="cuda").manual_seed(5 + bias)
+    u = torch.full((64,), 0.125, device="cuda")
+    v = torch.randn(B, T, D, device="cuda", generator=g)
+    emb = gate = None
+    if bias:  # emb grows with the bucket on the k > q side; q, k small noise
+        q = 0.1 * torch.randn(B, T, D, device="cuda", generator=g)
+        k = 0.1 * torch.randn(B, T, D, device="cuda", generator=g)
+        emb = torch.zeros(NUM_BUCKETS, H, device="cuda")
+        emb[NUM_BUCKETS // 2 :] = torch.linspace(0.0, 8.0, NUM_BUCKETS // 2, device="cuda")[:, None]
+        emb[: NUM_BUCKETS // 2] = -torch.linspace(0.0, 8.0, NUM_BUCKETS // 2, device="cuda")[:, None]
+        gate = 1.0 + torch.rand(B, H, T, device="cuda", generator=g)
+    else:  # score(q, t) ~ 8 t / T
+        q = (4 * u + 0.05 * torch.randn(B, T, H, 64, device="cuda", generator=g)).reshape(B, T, D)
+        ramp = torch.arange(T, device="cuda", dtype=torch.float32)[:, None, None] * 16.0 / T
+        k = (ramp * u + 0.05 * torch.randn(B, T, H, 64, device="cuda", generator=g)).reshape(B, T, D)
+    valid = [T, 200]
+    ref, budget = _attention_ref(q, k, v, valid, H, emb, gate)
+    _, r_row, r_fmt = _run_both_formats(q, k, v, valid, H, ref, f"rising max bias={bias}", budget, emb=emb, gate=gate)
+    print(f"rising max bias={bias}: row bound ratio {r_row:.3f}, f16q8/bound {r_fmt:.3f}")
+
+
+@pytest.mark.parametrize("bias", [False, True])
+@pytest.mark.parametrize("q_scale", [4.0, 8.0])
+def test_attention_large_logits(s3b_lib, q_scale, bias):
+    """q x4 / x8: logits of std 4 / 8, peaked softmax rows. The score error grows with sum_d |q_d k_d|, not with |s|,
+    so the bound is the per-row budget derived from the inputs (_attention_ref); no fixed relative bar."""
+    H, T = 12, 499
+    valid = [499, 65, 1]
+    B, D = len(valid), H * 64
+    g = torch.Generator(device="cuda").manual_seed(int(q_scale) * 3 + bias)
+    q = torch.randn(B, T, D, device="cuda", generator=g) * q_scale
+    k, v = (torch.randn(B, T, D, device="cuda", generator=g) for _ in range(2))
+    emb = torch.randn(NUM_BUCKETS, H, device="cuda", generator=g) * 0.5 if bias else None
+    gate = 1.0 + 1.3 * torch.rand(B, H, T, device="cuda", generator=g) if bias else None
+    ref, budget = _attention_ref(q, k, v, valid, H, emb, gate)
+    worst = [0.0, 0.0]
+    for fmt in (0, 1):
+        out = _attention_ex(q, k, v, valid, H, emb=emb, gate=gate, ctx_format=fmt)
+        assert torch.isfinite(out).all()
+        err = (out.double() - ref).abs()
+        if fmt == 1:  # plus the format's own rounding (see _check_f16q8)
+            err = (err - 2.0**-4 * _ulp16(ref) - 2.0**-21).clamp_min(0.0)
+        worst[fmt] = (err / budget).max().item()
+        assert worst[fmt] < 1.0, (q_scale, bias, fmt, worst[fmt])
+    print(f"q x{q_scale} bias={bias}: measured / row bound = {worst[0]:.3f} (bf16x2), {worst[1]:.3f} (f16q8)")
+
+
+def test_attention_ex_validates_options(s3b_lib):
+    from s3prl_b200 import lib
+
+    B, T, H = 1, 100, 12
+    q = torch.randn(B, T, H * 64, device="cuda")
+    emb = torch.randn(NUM_BUCKETS, H, device="cuda")
+    for kw in ({"emb": emb, "table_frames": T - 1}, {"ctx_format": 2},
+               {"gate": torch.ones(B, H, T, device="cuda")}):
+        with pytest.raises(lib.S3BError):
+            _attention_ex(q, q, q, [T], H, **kw)
+    with pytest.raises(lib.S3BError):
+        _attention_ex(q, q, q, [0], H)
+
+
+def _gate_ref(x, H, w, b, a):
+    """oracle formula (upstream_oracle.wavlm_gated_bias, modules.py:534-551) in fp64 -> gate [B, H, T]."""
+    B, T, _ = x.shape
+    sd = {"p.grep_linear.weight": w.double(), "p.grep_linear.bias": b.double(), "p.grep_a": a.double().view(1, H, 1, 1)}
+    ones = torch.ones(H, T, 1, dtype=torch.float64, device=x.device)
+    return _oracle().wavlm_gated_bias(x.double(), sd, "p", H, ones)[..., 0]
+
+
+@pytest.mark.parametrize("x_scale", [1.0, 1e-3])
+@pytest.mark.parametrize("x_format", [0, 1])
+@pytest.mark.parametrize("B,T,H", [(2, 37, 12), (1, 37, 16), (3, 499, 12), (2, 130, 16)])
+def test_wavlm_gate(s3b_lib, B, T, H, x_format, x_scale):
+    """The gate kernel from operand planes (both formats) vs the oracle formula. M * H * 8 lanes: 74 * 96 and 37 * 128
+    are not multiples of the 256-thread block (tail lanes). x at LayerNorm-output scale, and x1e-3, which puts the
+    f16q8 residual into e4m3's subnormals.
+    Bound: |dg| <= 0.25 * max(1, grep_a) * (sum_c (|W_a,c| + |W_b,c|) |dx_c|) + 2^-20 (sigmoid slopes <= 1/4 times the
+    summed-row inputs' read error dx: 2^-16 |x| for bf16 hi/lo, 2^-15 |x| + 2^-21 for f16q8, plus 2^-20 |x| for the
+    fp32 row sums and dot products; 2^-20 for expf and the division)."""
+    from s3prl_b200 import lib
+
+    D = H * 64
+    g = torch.Generator(device="cuda").manual_seed(B * 1000 + T + H + x_format)
+    x = torch.randn(B, T, D, device="cuda", generator=g) * x_scale
+    w = torch.randn(8, 64, device="cuda", generator=g) * 0.2
+    bias = torch.randn(8, device="cuda", generator=g) * 0.2
+    a = 1.0 + 0.3 * torch.randn(H, device="cuda", generator=g)
+    out = torch.full((B, H, T), float("nan"), device="cuda")
+    lib.check(s3b_lib.s3b_wavlm_gate_f32(_ptr(x), B, T, H, _ptr(w), _ptr(bias), _ptr(a), x_format, _ptr(out), _stream()))
+    torch.cuda.synchronize()
+    ref = _gate_ref(x, H, w, bias, a)
+    assert torch.isfinite(out).all()
+    dx = x.double().abs() * 2.0**-16 if x_format == 0 else x.double().abs() * 2.0**-15 + 2.0**-21
+    dx = dx + x.double().abs() * 2.0**-20
+    wsum = w.double().abs().view(2, 4, 64).sum(1).sum(0)  # |W_a| + |W_b| per input channel (upper bound)
+    slope = 0.25 * a.double().abs().clamp_min(1.0)
+    bound = slope[None, :, None] * (dx.view(B, T, H, 64) @ wsum).permute(0, 2, 1) + 2.0**-20
+    ratio = ((out.double() - ref).abs() / bound).max().item()
+    print(f"gate B={B} T={T} H={H} fmt={x_format} x*{x_scale}: measured / bound = {ratio:.3f}")
+    assert ratio < 1.0, ratio
+
+    off = torch.full_like(out, float("nan"))  # grep_w NULL (gru_rel_pos off): gate 1
+    lib.check(s3b_lib.s3b_wavlm_gate_f32(_ptr(x), B, T, H, None, None, None, x_format, _ptr(off), _stream()))
+    torch.cuda.synchronize()
+    assert torch.equal(off, torch.ones_like(off))

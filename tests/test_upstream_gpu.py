@@ -140,6 +140,37 @@ def test_positional_conv_block_variants(s3b_lib, depth, conv_pos, dim):
         _compare(h.cpu(), r, f"pos_conv depth={depth} conv_pos={conv_pos} D={dim} layer {l}")
 
 
+@pytest.mark.slow
+def test_wavlm_rel_table_rebuild(s3b_lib):
+    """WavLM's relative-position table is built at finalize for 4096 frames (82 s) and rebuilt for 2T frames when a
+    longer batch arrives. A two-layer wavlm_base_plus: one 82.5 s utterance (T = 4124 > 4096) against the oracle,
+    then, on the same model and its rebuilt table (centre 2 * 4124 - 1), a short ragged batch. The oracle's
+    [H, T, T] bias and scores take a few GB of host memory at this length."""
+    import dataclasses
+
+    import upstream_oracle as O
+    from s3prl_b200.upstream.configs import ARCHS
+    from s3prl_b200.upstream.expert import UpstreamExpert
+    from s3prl_b200.upstream.weights import fabricate_state_dict
+
+    cfg = dataclasses.replace(ARCHS["wavlm_base_plus"], encoder_layers=2)
+    sd = fabricate_state_dict(cfg, seed=11)
+    _EXPERTS.clear()
+    expert = UpstreamExpert(arch=cfg, state_dict=sd, name="wavlm_two_layers").to("cuda")
+    for lens in ([1_320_000], [40000, 33333, 900]):
+        wavs = _wavs(lens, seed=len(lens))
+        assert len(lens) > 1 or O.conv_output_length(lens[0]) > 4096
+        with torch.no_grad():
+            ref, _pad = O.upstream_forward(wavs, sd, cfg)
+        hs = expert([w.cuda() for w in wavs])["hidden_states"]
+        assert len(hs) == len(ref) == 3
+        worst = 0.0
+        for l, (h, r) in enumerate(zip(hs, ref)):
+            worst = max(worst, _compare(h.cpu(), r, f"wavlm two layers lens={lens} layer {l}"))
+        del ref, hs
+        print(f"wavlm two layers lens={lens}: worst per-layer relative error vs oracle = {worst:.3e}")
+
+
 def test_forward_host_matches_device(s3b_lib):
     expert = _expert("hubert_base")
     wavs = _wavs([16000, 9000], seed=5)
