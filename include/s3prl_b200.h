@@ -185,9 +185,59 @@ int s3b_melspec(const float* const* wavs, const int64_t* trimmed_lens, int32_t b
                 const int32_t* feats_len, const int32_t* final_len, int32_t t_out, float* out, void* stream);
 
 /* Building blocks exposed for parity tests (device pointers, fp32) -------------------------------------- */
-/* out[M][N] = act(A[M][K] * W[N][K]^T + bias[N]) (+ residual[M][N]); K % 64 == 0, N % 16 == 0 */
+/* out[M][N] = act(A[M][K] * W[N][K]^T + bias[N]) (+ residual[M][N]); K % 64 == 0, N % 16 == 0.
+ * = s3b_linear_ex with opts NULL: the default operand scheme (S3B_GEMM_SCHEME) where it applies, else bf16x3. */
 int s3b_linear_f32(const float* a, const float* w, const float* bias, const float* residual, int64_t m, int32_t n,
                    int32_t k, int32_t gelu, float* out, void* stream);
+/* Options of s3b_linear_ex (zero-initialise, set struct_size = sizeof(s3b_linear_opts), scheme = out_fmt = -1).
+ *  scheme      : -1 = the library default where it applies (else bf16x3), 0 = bf16x3, 1 = f16q8 (needs K % 128 == 0
+ *                and N % 128 == 0; an impossible request is an error)
+ *  tile_n      : 0 = the library's choice, 128 or 256 = that tile width (must divide N)
+ *  out_fmt     : -1 = fp32 output; 0 / 1 = the output is written as operand planes (0 = bf16 hi/lo, 1 = f16q8) like
+ *                fc1's, and out is decoded from them
+ *  row_mask    : optional DEVICE uint8 [M]: rows != 0 are written as zero (post_extract_proj's padding mask)
+ *  out_pre     : optional DEVICE fp32 [M][N]: the value before the residual add (fc2's ffn output)
+ *  lda, a_off  : A is the [M][K] column slice starting at column a_off of a [M][lda] matrix (0, 0 = dense [M][K]);
+ *                lda and a_off multiples of 16 (the distiller's SplitLinear)
+ *  scheme_used, tile_n_used : filled in with the operand scheme and the tile width that ran */
+typedef struct s3b_linear_opts {
+    int32_t struct_size;
+    int32_t scheme;
+    int32_t tile_n;
+    int32_t out_fmt;
+    const uint8_t* row_mask;
+    float* out_pre;
+    int64_t lda;
+    int64_t a_off;
+    int32_t scheme_used;
+    int32_t tile_n_used;
+    int64_t reserved[2];
+} s3b_linear_opts;
+int s3b_linear_ex(const float* a, const float* w, const float* bias, const float* residual, int64_t m, int32_t n,
+                  int32_t k, int32_t gelu, s3b_linear_opts* opts, float* out, void* stream);
+/* The QKV projection as a layer runs it: x [batch][t][heads*64] times w [3D][D]^T + b [3D] through the GEMM's QKV
+ * epilogue (q scaled by 1/8 * log2(e), per-head layout, v transposed), in operand scheme `scheme` (-1 / 0 / 1 as in
+ * s3b_linear_opts). The bf16 hi/lo planes it writes are decoded to q_out, k_out [batch][heads][t][64] and
+ * vt_out [batch][heads][64][(t + 7) & ~7]. The epilogue writes columns [0, t) of each vt_out row; the padding columns
+ * t.. are never written by it and come back as the zero of a freshly allocated plane. */
+int s3b_qkv_f32(const float* x, const float* w, const float* b, int32_t batch, int32_t t, int32_t heads, int32_t scheme,
+                float* q_out, float* k_out, float* vt_out, void* stream);
+/* One conv of the feature extractor (Conv1d(512, 512, kw, stride 2), kw in {2, 3}) as the model runs it: implicit GEMM on
+ * channels-last x [batch][lin][512], weight w [512][512][kw] (torch layout), optional bias [512], optional GELU, in
+ * operand scheme `scheme`; out_fmt -1 = fp32 output, 0 / 1 = operand planes decoded to fp32.
+ * out: [batch][(lin - kw) / 2 + 1][512]. */
+int s3b_conv_gemm_f32(const float* x, const float* w, const float* bias, int32_t batch, int64_t lin, int32_t kw,
+                      int32_t gelu, int32_t scheme, int32_t out_fmt, float* out, void* stream);
+/* The positional conv as the model runs it (bf16x3): x [batch][t][d], folded weight w [d][d / groups][k], bias [d].
+ *  taps_per_kblock 1: one k-block per tap, bias + GELU + residual in the GEMM epilogue, fp32 (then LayerNorm if gamma:
+ *    as in the model, operand planes come only from that LayerNorm, so out_fmt >= 0 needs gamma);
+ *  taps_per_kblock 4: four taps per k-block (zero taps appended up to a multiple of 4) + the combine kernel, mode
+ *    0 = x + GELU(conv + bias); 1 = data2vec block GELU(LayerNorm_noaffine(conv + bias)); 2 = x + the mode-1 value.
+ *  gamma, beta: optional LayerNorm(d) of the result (post-LN models' encoder LayerNorm); NULL = none.
+ *  out_fmt -1 = fp32 output, 0 / 1 = operand planes decoded to fp32. out: [batch][t][d]. */
+int s3b_posconv_f32(const float* x, const float* w, const float* bias, int32_t batch, int32_t t, int32_t d,
+                    int32_t groups, int32_t k, int32_t taps_per_kblock, int32_t mode, const float* gamma,
+                    const float* beta, int32_t out_fmt, float* out, void* stream);
 /* micro-benchmark of the production GEMM kernel: `iters` back-to-back launches of [M][K] x [N][K]^T with the fc1-style
  * epilogue (gelu != 0: bias + GELU + bf16 hi/lo output) or the out_proj-style one (bias + residual + fp32 output).
  * force_un in {0 = the library's choice, 128, 256} forces the CTA-pair tile width. out[0] = ms per launch,

@@ -91,8 +91,6 @@ struct GemmParams {
     // loads 64-wide boxes but only the first 3 k-steps carry non-zero weights.
     int k_steps;
 
-    // debug timeline (tools/gemm_trace.py): 16 clock64 stamps of CTA 0, or nullptr
-    unsigned long long* trace;
 };
 
 // k-block width the kernel instantiation for this tile width uses (tensor-map boxes must match)

@@ -400,6 +400,44 @@ static void set_rel_bias(AttnParams& ap, const float* table, int Tmax, const flo
     ap.gate = gate;
 }
 
+// ---- weight relayouts shared by s3b_model_finalize and the building-block entry points ----------------------------
+// conv 1..6: [out][in][tap] -> [out][tap*512 + in] (K index of the channels-last im2col row)
+static std::vector<float> conv_weight_layout(const float* w, int kw) {
+    const int C = kConvDim;
+    std::vector<float> r((size_t)C * C * kw);
+    for (int o = 0; o < C; ++o)
+        for (int ci = 0; ci < C; ++ci)
+            for (int j = 0; j < kw; ++j) r[((size_t)o * kw + j) * C + ci] = w[((size_t)o * C + ci) * kw + j];
+    return r;
+}
+// grouped positional conv, folded weight w [D][cpg][Kp]. One tap per k-block (posconv_params):
+// B operand [group*Kp + tap][n = cpg][64 (zero padded)]
+static std::vector<float> posconv_weight_layout(const float* w, int D, int G, int Kp) {
+    const int cpg = D / G;
+    std::vector<float> wb((size_t)G * Kp * cpg * 64, 0.0f);
+    for (int g = 0; g < G; ++g)
+        for (int k = 0; k < Kp; ++k)
+            for (int n = 0; n < cpg; ++n)
+                for (int ci = 0; ci < cpg; ++ci)
+                    wb[(((size_t)g * Kp + k) * cpg + n) * 64 + ci] = w[((size_t)(g * cpg + n) * cpg + ci) * Kp + k];
+    return wb;
+}
+// four taps per k-block (tap = 4q + j, posconv4_params), the tap count rounded up to K4 = a multiple of four with zero
+// taps: B operand [group*K4/4 + q][n = j*cpg + co][64 (zero padded)]
+static std::vector<float> posconv4_weight_layout(const float* w, int D, int G, int Kp) {
+    const int cpg = D / G, K4 = (Kp + 3) / 4 * 4;
+    std::vector<float> w4((size_t)G * K4 * cpg * 64, 0.0f);
+    for (int g = 0; g < G; ++g)
+        for (int k = 0; k < Kp; ++k)
+            for (int n = 0; n < cpg; ++n)
+                for (int ci = 0; ci < cpg; ++ci) {
+                    const int q = k / 4, j = k % 4;
+                    w4[((((size_t)g * (K4 / 4) + q) * 4 + j) * cpg + n) * 64 + ci] =
+                        w[((size_t)(g * cpg + n) * cpg + ci) * Kp + k];
+                }
+    return w4;
+}
+
 extern "C" int s3b_model_finalize(s3b_model* m) {
     if (!m) return fail("null model");
     if (m->finalized) return 0;
@@ -434,10 +472,7 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
         const std::string p = fe + std::to_string(i);
         const int kw = kConvK[i];
         S3B_OK(need(m, p + ".0.weight", {C, C, kw}, &t));
-        std::vector<float> r((size_t)C * C * kw);
-        for (int o = 0; o < C; ++o)
-            for (int ci = 0; ci < C; ++ci)
-                for (int j = 0; j < kw; ++j) r[((size_t)o * kw + j) * C + ci] = t->data[((size_t)o * C + ci) * kw + j];
+        const std::vector<float> r = conv_weight_layout(t->data.data(), kw);
         S3B_OK(upload_split(m->conv_w[i], r.data(), r.size(), m->scheme));
         if (c.conv_bias) S3B_OK(upload_vec(m, p + ".0.bias", C, m->conv_b[i]));
         if (c.extractor_layer_norm) {
@@ -454,32 +489,23 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
     S3B_OK(upload_split(m->proj_w, t->data.data(), t->numel(), m->scheme));
     S3B_OK(upload_vec(m, "post_extract_proj.bias", D, m->proj_b));
     // ---- data2vec pos_conv: pos_conv_depth plain Conv1d(k, padding k/2, groups) blocks (make_conv_block,
-    //      wav2vec2_model.py:2995-3026). Four taps per k-block like pos_w4 below, the tap count rounded up to a
-    //      multiple of four with zero taps: B operand [group*K4/4 + q][n = j*cpg + co][64 (zero padded)], tap = 4q + j
+    //      wav2vec2_model.py:2995-3026). Four taps per k-block like pos_w4 below (posconv4_weight_layout)
     if (c.pos_conv_depth > 1) {
         if (!pairs_enabled()) return fail("pos_conv_depth > 1 runs on the CTA-pair GEMM only (S3B_GEMM_PAIR=0 is set)");
-        const int G = c.pos_conv_groups, cpg = D / G, Kp = pos_taps(c), K4 = pos_taps4(c);
+        const int G = c.pos_conv_groups, cpg = D / G, Kp = pos_taps(c);
         m->posd_w4.resize(c.pos_conv_depth);
         m->posd_b.resize(c.pos_conv_depth);
         for (int i = 0; i < c.pos_conv_depth; ++i) {
             const std::string pre = "encoder.pos_conv." + std::to_string(i) + ".0.";
             const HostTensor* tw;
             S3B_OK(need(m, pre + "weight", {D, cpg, Kp}, &tw));
-            std::vector<float> w4((size_t)G * K4 * cpg * 64, 0.0f);
-            for (int g = 0; g < G; ++g)
-                for (int k = 0; k < Kp; ++k)
-                    for (int n = 0; n < cpg; ++n)
-                        for (int ci = 0; ci < cpg; ++ci) {
-                            const int o = g * cpg + n, q = k / 4, j = k % 4;
-                            w4[((((size_t)g * (K4 / 4) + q) * 4 + j) * cpg + n) * 64 + ci] =
-                                tw->data[((size_t)o * cpg + ci) * Kp + k];
-                        }
+            const std::vector<float> w4 = posconv4_weight_layout(tw->data.data(), D, G, Kp);
             S3B_OK(upload_split(m->posd_w4[i], w4.data(), w4.size()));
             S3B_OK(upload_vec(m, pre + "bias", D, m->posd_b[i]));
         }
     } else {
     // ---- pos_conv: fold weight_norm(dim=2): W[o][c][k] = g[k] * v[o][c][k] / ||v[:,:,k]||  ---------------
-    //      (make_conv_pos, wav2vec2_model.py:2937-2953). GEMM B operand: [group*Kp + tap][n = cpg][64 (zero padded)]
+    //      (make_conv_pos, wav2vec2_model.py:2937-2953), then the one-tap and (Kp % 4 == 0) four-tap layouts
         const int G = c.pos_conv_groups, cpg = D / G, Kp = c.pos_conv_kernel;
         const HostTensor *tg, *tv;
         S3B_OK(need(m, "encoder.pos_conv.0.weight_g", {1, 1, Kp}, &tg));
@@ -492,27 +518,13 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
             }
         std::vector<float> scale(Kp);
         for (int k = 0; k < Kp; ++k) scale[k] = (float)((double)tg->data[k] / sqrt(nrm[k]));
-        std::vector<float> wb((size_t)G * Kp * cpg * 64, 0.0f);
-        for (int g = 0; g < G; ++g)
-            for (int k = 0; k < Kp; ++k)
-                for (int n = 0; n < cpg; ++n)
-                    for (int ci = 0; ci < cpg; ++ci) {
-                        const int o = g * cpg + n;
-                        // fp32 product like torch's _weight_norm (v * (g / norm))
-                        wb[(((size_t)g * Kp + k) * cpg + n) * 64 + ci] = tv->data[((size_t)o * cpg + ci) * Kp + k] * scale[k];
-                    }
+        std::vector<float> wf((size_t)D * cpg * Kp);
+        for (size_t oc = 0; oc < (size_t)D * cpg; ++oc)
+            for (int k = 0; k < Kp; ++k) wf[oc * Kp + k] = tv->data[oc * Kp + k] * scale[k];  // fp32, like torch's _weight_norm
+        const std::vector<float> wb = posconv_weight_layout(wf.data(), D, G, Kp);
         S3B_OK(upload_split(m->pos_w, wb.data(), wb.size()));
-        // four taps per k-block (tap = 4q + j): B operand [group*Kp/4 + q][n = j*cpg + co][64 (zero padded)]
         if (Kp % 4 == 0) {
-            std::vector<float> w4((size_t)G * Kp * cpg * 64, 0.0f);
-            for (int g = 0; g < G; ++g)
-                for (int k = 0; k < Kp; ++k)
-                    for (int n = 0; n < cpg; ++n)
-                        for (int ci = 0; ci < cpg; ++ci) {
-                            const int q = k / 4, j = k % 4;
-                            w4[((((size_t)g * (Kp / 4) + q) * 4 + j) * cpg + n) * 64 + ci] =
-                                wb[(((size_t)g * Kp + k) * cpg + n) * 64 + ci];
-                        }
+            const std::vector<float> w4 = posconv4_weight_layout(wf.data(), D, G, Kp);
             S3B_OK(upload_split(m->pos_w4, w4.data(), w4.size()));
         }
         S3B_OK(upload_vec(m, "encoder.pos_conv.0.bias", D, m->pos_b));
@@ -674,6 +686,22 @@ static void set_epi(GemmParams& p, const Epi& e, int ldo) {
     p.out_f32 = e.out_f32, p.out_hi = e.op.hi, p.out_lo = e.op.lo, p.out_h8 = e.op.h8, p.out_l8 = e.op.l8;
     p.out_fmt = e.op.fmt, p.ldo = ldo;
     p.qkv_mode = 0;
+}
+
+// q pre-scaled by head_dim^-0.5 (exact power of two) and log2(e): the attention kernel's softmax runs on exp2
+static const float kQScale = 0.125f * 1.4426950408889634f;
+
+// QKV epilogue of a [B*T][3D] linear: bias, then q (scaled), k as [B][H][T][64] and v transposed as [B][H][64][Tp]
+// (Tp = T rounded up to 8), all as bf16 hi/lo planes
+static void set_qkv_epi(GemmParams& p, const float* bias, int T, int H, const SplitBuf& q, const SplitBuf& k,
+                        const SplitBuf& vt) {
+    const int D = H * 64;
+    Epi e;
+    e.bias = bias;
+    set_epi(p, e, 3 * D);
+    p.qkv_mode = 1, p.T = T, p.Tp = (T + 7) & ~7, p.H = H, p.D = D, p.q_scale = kQScale;
+    p.q_hi = q.h(), p.q_lo = q.l(), p.k_hi = k.h(), p.k_lo = k.l();
+    p.vt_hi = vt.h(), p.vt_lo = vt.l();
 }
 
 // The paired tile layout (gemm.cuh: two_cta) serves the 256- and 128-column tiles: 64-wide k-blocks (128-byte
@@ -1170,15 +1198,10 @@ int Fwd::build_plan(Plan& pl) {
     for (int l = 0; l < NL; ++l) {
         LayerW& W = m->layers[l];
         LayerPlan& lp = pl.layers[l];
-        {   // QKV projection, scattered per head; q pre-scaled by head_dim^-0.5 (exact power of two) and log2(e)
+        {   // QKV projection, scattered per head
             GemmParams& p = lp.qkv;
             S3B_OK(linear_params(p, w->xs_s, W.qkv, M, 3 * D, D, 1, m->scheme));
-            Epi e;
-            e.bias = W.qkv_b.as<float>();
-            set_epi(p, e, 3 * D);
-            p.qkv_mode = 1, p.T = T, p.Tp = Tp, p.H = H, p.D = D, p.q_scale = 0.125f * 1.4426950408889634f;
-            p.q_hi = w->q_s.h(), p.q_lo = w->q_s.l(), p.k_hi = w->k_s.h(), p.k_lo = w->k_s.l();
-            p.vt_hi = w->vt_s.h(), p.vt_lo = w->vt_s.l();
+            set_qkv_epi(p, W.qkv_b.as<float>(), T, H, w->q_s, w->k_s, w->vt_s);
         }
         {
             AttnParams& ap = lp.attn;
@@ -1847,62 +1870,245 @@ static int device_sm_count(int* out) {
     return 0;
 }
 
-extern "C" int s3b_linear_f32(const float* a, const float* w, const float* bias, const float* residual, int64_t M,
-                              int32_t N, int32_t K, int32_t gelu, float* out, void* stream) {
+// Operand scheme of a building-block call: -1 = the library default where the shape allows it (else bf16x3), 0 / 1 =
+// exactly that scheme (linear_params / conv_params refuse an f16q8 request the shape cannot take)
+static int resolve_scheme(int scheme, int K, int N, int* out) {
+    if (scheme < -1 || scheme > 1) return fail("scheme must be -1 (default), 0 (bf16x3) or 1 (f16q8), not %d", scheme);
+    if (scheme == -1) scheme = (K % 128 == 0 && N % 128 == 0 && pairs_enabled()) ? default_scheme() : 0;
+    *out = scheme;
+    return 0;
+}
+
+// fp32 -> operand planes of `scheme`, on the stream (weight != 0: the weight split of the f16q8 format)
+static int split_operand(const float* x, SplitBuf& s, size_t n, int scheme, int weight, cudaStream_t st) {
+    S3B_OK(s.ensure(n));
+    if (scheme != 0) CUDA_OK(launch_split_q8(x, s.h(), s.h8(), s.l8(), n, weight, st));
+    else CUDA_OK(launch_split(x, s.h(), s.l(), n, st));
+    return 0;
+}
+
+// a device fp32 tensor of the caller (written on `st`) to the host, for the weight relayouts of s3b_model_finalize
+static int download_f32(const float* src, size_t n, cudaStream_t st, std::vector<float>& dst) {
+    dst.resize(n);
+    CUDA_OK(cudaStreamSynchronize(st));
+    CUDA_OK(cudaMemcpy(dst.data(), src, n * 4, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+static int check_out_fmt(int out_fmt) {
+    if (out_fmt < -1 || out_fmt > 1) return fail("out_fmt must be -1 (fp32), 0 (bf16 hi/lo) or 1 (f16q8), not %d", out_fmt);
+    return 0;
+}
+
+extern "C" int s3b_linear_ex(const float* a, const float* w, const float* bias, const float* residual, int64_t M,
+                             int32_t N, int32_t K, int32_t gelu, s3b_linear_opts* opts, float* out, void* stream) {
     if (!a || !w || !out) return fail("null argument");
+    if (M < 1 || N < 1 || K < 1) return fail("bad sizes");
+    s3b_linear_opts o;
+    memset(&o, 0, sizeof(o));
+    o.scheme = -1, o.out_fmt = -1;
+    if (opts != nullptr) {
+        if (opts->struct_size != (int32_t)sizeof(s3b_linear_opts))
+            return fail("s3b_linear_opts.struct_size %d != %d (header / library mismatch)", opts->struct_size,
+                        (int)sizeof(s3b_linear_opts));
+        o = *opts;
+    }
+    int scheme = 0;
+    S3B_OK(resolve_scheme(o.scheme, K, N, &scheme));
+    S3B_OK(check_out_fmt(o.out_fmt));
+    if (o.tile_n != 0 && o.tile_n != 128 && o.tile_n != 256) return fail("tile_n must be 0, 128 or 256, not %d", o.tile_n);
+    if (o.tile_n != 0 && N % o.tile_n != 0) return fail("tile_n %d does not divide N = %d", o.tile_n, N);
+    if (o.tile_n != 0 && !pairs_enabled()) return fail("tile_n needs the paired tile layout (S3B_GEMM_PAIR=0 is set)");
+    const int64_t lda = o.lda != 0 ? o.lda : K;
+    if (o.a_off < 0 || o.a_off + K > lda || (o.lda != 0 && (lda % 16 != 0 || o.a_off % 16 != 0)))
+        return fail("A slice [%lld, %lld) of rows of %lld elements: out of range or not a multiple of 16",
+                    (long long)o.a_off, (long long)(o.a_off + K), (long long)lda);
     cudaStream_t st = (cudaStream_t)stream;
     int sms = 0;
     S3B_OK(device_sm_count(&sms));
-    SplitBuf as, ws;
-    S3B_OK(as.ensure((size_t)M * K));
-    S3B_OK(ws.ensure((size_t)N * K));
-    // the operand scheme under test: S3B_GEMM_SCHEME (like a model would pick it), bf16x3 when f16q8 cannot apply
-    int scheme = default_scheme();
-    if (K % 128 != 0 || N % 128 != 0 || !pairs_enabled()) scheme = 0;
-    if (scheme != 0) {
-        CUDA_OK(launch_split_q8(a, as.h(), as.h8(), as.l8(), (size_t)M * K, 0, st));
-        CUDA_OK(launch_split_q8(w, ws.h(), ws.h8(), ws.l8(), (size_t)N * K, 1, st));
-    } else {
-        CUDA_OK(launch_split(a, as.h(), as.l(), (size_t)M * K, st));
-        CUDA_OK(launch_split(w, ws.h(), ws.l(), (size_t)N * K, st));
-    }
+    g_sm_count = sms;  // the tile-width choice a model finalized on this device makes
+    SplitBuf as, ws, os;
     GemmParams p;
-    int r = linear_params(p, as, ws, M, N, K, 0, scheme);
-    if (r == 0) {
+    const int r = [&]() -> int {
+        S3B_OK(split_operand(a, as, (size_t)M * lda, scheme, 0, st));
+        S3B_OK(split_operand(w, ws, (size_t)N * K, scheme, 1, st));
+        const int epi_kind = o.out_fmt < 0 ? 0 : (gelu ? 2 : 1);
+        g_force_pair_un = o.tile_n;
+        const int rp = linear_params(p, as, ws, M, N, K, epi_kind, scheme, lda, (size_t)o.a_off);
+        g_force_pair_un = 0;
+        S3B_OK(rp);
+        if (o.tile_n != 0 && p.umma_n != o.tile_n) return fail("tile_n %d requested, %d chosen", o.tile_n, p.umma_n);
         Epi e;
-        e.bias = bias, e.residual = residual, e.gelu = gelu, e.out_f32 = out;
+        e.bias = bias, e.residual = residual, e.gelu = gelu, e.row_mask = o.row_mask;
+        if (o.out_fmt < 0) {
+            e.out_f32 = out;
+        } else {
+            S3B_OK(os.ensure((size_t)M * N));
+            e.op = os.planes(o.out_fmt);
+        }
         set_epi(p, e, N);
-        // S3B_GEMM_TRACE=1: clock64 timeline of CTA 0 to stderr (tools/gemm_trace.py); 3 launches, last one traced
-        const bool trace = getenv("S3B_GEMM_TRACE") != nullptr;
-        unsigned long long* tr = nullptr;
-        if (trace && cudaMalloc(&tr, 16 * sizeof(unsigned long long)) == cudaSuccess) {
-            cudaMemsetAsync(tr, 0, 16 * sizeof(unsigned long long), st);
-            launch_gemm_bf16x3(p, sms, st);
-            launch_gemm_bf16x3(p, sms, st);
-            p.trace = tr;
+        p.out_pre = o.out_pre;
+        CUDA_OK(launch_gemm_bf16x3(p, sms, st));
+        if (o.out_fmt >= 0) CUDA_OK(launch_planes_to_f32(os.planes(o.out_fmt), (size_t)M * N, out, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+        return 0;
+    }();
+    as.release(), ws.release(), os.release();
+    if (r == 0 && opts != nullptr) opts->scheme_used = scheme, opts->tile_n_used = p.umma_n;
+    return r;
+}
+
+extern "C" int s3b_linear_f32(const float* a, const float* w, const float* bias, const float* residual, int64_t M,
+                              int32_t N, int32_t K, int32_t gelu, float* out, void* stream) {
+    return s3b_linear_ex(a, w, bias, residual, M, N, K, gelu, nullptr, out, stream);
+}
+
+extern "C" int s3b_qkv_f32(const float* x, const float* w, const float* b, int32_t B, int32_t T, int32_t H,
+                           int32_t scheme, float* q_out, float* k_out, float* vt_out, void* stream) {
+    if (!x || !w || !b || !q_out || !k_out || !vt_out) return fail("null argument");
+    if (B < 1 || T < 1 || H < 1) return fail("bad sizes");
+    const int D = H * 64, Tp = (T + 7) & ~7;
+    const int64_t M = (int64_t)B * T;
+    int sch = 0;
+    S3B_OK(resolve_scheme(scheme, D, 3 * D, &sch));
+    cudaStream_t st = (cudaStream_t)stream;
+    int sms = 0;
+    S3B_OK(device_sm_count(&sms));
+    g_sm_count = sms;
+    SplitBuf xs, ws, qs, ks, vts;
+    const int r = [&]() -> int {
+        S3B_OK(split_operand(x, xs, (size_t)M * D, sch, 0, st));
+        S3B_OK(split_operand(w, ws, (size_t)3 * D * D, sch, 1, st));
+        S3B_OK(qs.ensure((size_t)M * D));
+        S3B_OK(ks.ensure((size_t)M * D));
+        S3B_OK(vts.ensure((size_t)B * H * 64 * Tp));
+        GemmParams p;
+        S3B_OK(linear_params(p, xs, ws, M, 3 * D, D, 1, sch));
+        set_qkv_epi(p, b, T, H, qs, ks, vts);
+        CUDA_OK(launch_gemm_bf16x3(p, sms, st));
+        CUDA_OK(launch_planes_to_f32(qs.planes(0), (size_t)M * D, q_out, st));
+        CUDA_OK(launch_planes_to_f32(ks.planes(0), (size_t)M * D, k_out, st));
+        CUDA_OK(launch_planes_to_f32(vts.planes(0), (size_t)B * H * 64 * Tp, vt_out, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+        return 0;
+    }();
+    xs.release(), ws.release(), qs.release(), ks.release(), vts.release();
+    return r;
+}
+
+extern "C" int s3b_conv_gemm_f32(const float* x, const float* w, const float* bias, int32_t B, int64_t Lin, int32_t kw,
+                                 int32_t gelu, int32_t scheme, int32_t out_fmt, float* out, void* stream) {
+    if (!x || !w || !out) return fail("null argument");
+    if (kw != 2 && kw != 3) return fail("kw must be 2 or 3, not %d", kw);
+    if (B < 1 || Lin < kw) return fail("bad sizes (batch %d, lin %lld, kw %d)", B, (long long)Lin, kw);
+    S3B_OK(check_out_fmt(out_fmt));
+    const int C = kConvDim;
+    const int64_t Lout = (Lin - kw) / 2 + 1;
+    int sch = 0;
+    S3B_OK(resolve_scheme(scheme, kw * C, C, &sch));
+    cudaStream_t st = (cudaStream_t)stream;
+    int sms = 0;
+    S3B_OK(device_sm_count(&sms));
+    SplitBuf xs, ws, os;
+    const int r = [&]() -> int {
+        std::vector<float> wh;
+        S3B_OK(download_f32(w, (size_t)C * C * kw, st, wh));
+        const std::vector<float> wl = conv_weight_layout(wh.data(), kw);
+        S3B_OK(upload_split(ws, wl.data(), wl.size(), sch));
+        S3B_OK(split_operand(x, xs, (size_t)B * Lin * C, sch, 0, st));
+        GemmParams p;
+        S3B_OK(conv_params(p, xs, ws, B, Lin, Lout, kw, sch));
+        Epi e;
+        e.bias = bias, e.gelu = gelu;
+        if (out_fmt < 0) {
+            e.out_f32 = out;
+        } else {
+            S3B_OK(os.ensure((size_t)B * Lout * C));
+            e.op = os.planes(out_fmt);
         }
-        cudaEvent_t e0 = nullptr, e1 = nullptr;
-        if (trace) cudaEventCreate(&e0), cudaEventCreate(&e1), cudaEventRecord(e0, st);
-        cudaError_t ce = launch_gemm_bf16x3(p, sms, st);
-        if (ce != cudaSuccess) r = fail("gemm launch failed: %s", cudaGetErrorString(ce));
-        if (trace) {
-            cudaEventRecord(e1, st);
-            cudaStreamSynchronize(st);
-            float ms = 0.f;
-            cudaEventElapsedTime(&ms, e0, e1);
-            unsigned long long h[16] = {0};
-            if (tr) cudaMemcpy(h, tr, sizeof(h), cudaMemcpyDeviceToHost), cudaFree(tr);
-            fprintf(stderr, "gemm_trace M=%lld N=%d K=%d two_cta=%d umma_n=%d event_us=%.2f tiles_cta0=%llu :", (long long)M, N, K,
-                    p.two_cta, p.umma_n, ms * 1000.f, h[10]);
-            for (int i = 1; i < 14; ++i)
-                if (i != 10) fprintf(stderr, " t%d=%lld", i, h[i] ? (long long)(h[i] - h[0]) : -1LL);
-            fprintf(stderr, "\n");
-            cudaEventDestroy(e0), cudaEventDestroy(e1);
+        set_epi(p, e, C);
+        CUDA_OK(launch_gemm_bf16x3(p, sms, st));
+        if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), (size_t)B * Lout * C, out, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+        return 0;
+    }();
+    xs.release(), ws.release(), os.release();
+    return r;
+}
+
+extern "C" int s3b_posconv_f32(const float* x, const float* w, const float* bias, int32_t B, int32_t T, int32_t D,
+                               int32_t G, int32_t k, int32_t taps, int32_t mode, const float* gamma, const float* beta,
+                               int32_t out_fmt, float* out, void* stream) {
+    if (!x || !w || !bias || !out || (gamma == nullptr) != (beta == nullptr)) return fail("null argument");
+    if (B < 1 || T < 1) return fail("bad sizes");
+    if (D != 512 && D != 768 && D != 1024 && D != 1280) return fail("d must be 512, 768, 1024 or 1280, not %d", D);
+    if (G < 1 || D % G != 0) return fail("d %d is not a multiple of groups %d", D, G);
+    const int cpg = D / G;
+    if (cpg % 16 != 0 || cpg > 64) return fail("channels per group must be a multiple of 16, <= 64 (got %d)", cpg);
+    if (taps != 1 && taps != 4) return fail("taps_per_kblock must be 1 or 4, not %d", taps);
+    if (mode < 0 || mode > 2) return fail("mode must be 0, 1 or 2, not %d", mode);
+    if (k < 2) return fail("kernel size %d < 2", k);
+    if (mode == 0 && k % (taps == 4 ? 4 : 2) != 0) return fail("conv_pos kernel %d: must be even (a multiple of 4 with "
+                                                               "four taps per k-block)", k);
+    if (taps == 4 && 4 * cpg != 192 && 4 * cpg != 256) return fail("four taps per k-block need 48 or 64 channels per group");
+    if (taps == 1 && mode != 0) return fail("the data2vec blocks (mode 1, 2) run four taps per k-block only");
+    if (taps == 1 && gamma == nullptr && out_fmt >= 0)  // Fwd::stage(8): the one-tap epilogue writes fp32 only
+        return fail("one tap per k-block writes operand planes only through the LayerNorm (gamma)");
+    if (!pairs_enabled() && taps == 4) return fail("four taps per k-block need the paired tile layout (S3B_GEMM_PAIR=0)");
+    S3B_OK(check_out_fmt(out_fmt));
+    // one conv block of k taps: pos_taps(c) = k (the data2vec blocks' k = max(3, conv_pos / depth) is the caller's)
+    s3b_config c;
+    memset(&c, 0, sizeof(c));
+    c.embed_dim = D, c.pos_conv_groups = G, c.pos_conv_kernel = k, c.pos_conv_depth = 1;
+    const size_t M = (size_t)B * T;
+    cudaStream_t st = (cudaStream_t)stream;
+    int sms = 0;
+    S3B_OK(device_sm_count(&sms));
+    SplitBuf xs, ws, os;
+    DevBuf z;
+    const int r = [&]() -> int {
+        std::vector<float> wh;
+        S3B_OK(download_f32(w, (size_t)D * cpg * k, st, wh));
+        const std::vector<float> wl =
+            taps == 4 ? posconv4_weight_layout(wh.data(), D, G, k) : posconv_weight_layout(wh.data(), D, G, k);
+        S3B_OK(upload_split(ws, wl.data(), wl.size()));
+        S3B_OK(split_operand(x, xs, M * D, 0, 0, st));
+        OutPlanes op = no_planes();
+        if (out_fmt >= 0) {
+            S3B_OK(os.ensure(M * D));
+            op = os.planes(out_fmt);
         }
-    }
-    cudaError_t se = cudaStreamSynchronize(st);
-    as.release(), ws.release();
-    if (r == 0 && se != cudaSuccess) return fail("gemm execution failed: %s", cudaGetErrorString(se));
+        float* out_f32 = out_fmt < 0 ? out : nullptr;
+        GemmParams p;
+        Epi e;
+        if (taps == 4) {
+            // Fwd::stage(8): Z = the four-tap GEMM, then the combine kernel (+ LayerNorm)
+            S3B_OK(z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
+            S3B_OK(posconv4_params(p, c, xs.h(), xs.l(), ws.h(), ws.l(), B, T));
+            e.out_f32 = z.as<float>();
+            set_epi(p, e, 4 * D);
+            CUDA_OK(launch_gemm_bf16x3(p, sms, st));
+            CUDA_OK(launch_posconv_combine(z.as<float>(), x, bias, B, T, D, cpg, gamma, beta, gamma ? 1 : 0, mode,
+                                           out_f32, op, st));
+        } else {
+            // Fwd::stage(8), one tap per k-block: x + GELU(conv + bias) in the epilogue, then the LayerNorm
+            S3B_OK(posconv_params(p, c, xs.h(), xs.l(), ws.h(), ws.l(), B, T));
+            e.bias = bias, e.gelu = 1, e.residual = x;
+            if (gamma != nullptr) {
+                S3B_OK(z.ensure(M * D * sizeof(float)));
+                e.out_f32 = z.as<float>();
+            } else {
+                e.out_f32 = out_f32;
+            }
+            set_epi(p, e, D);
+            CUDA_OK(launch_gemm_bf16x3(p, sms, st));
+            if (gamma != nullptr) CUDA_OK(launch_layernorm(z.as<float>(), M, D, gamma, beta, 0, out_f32, op, st));
+        }
+        if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(op, M * D, out, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+        return 0;
+    }();
+    xs.release(), ws.release(), os.release(), z.release();
     return r;
 }
 
@@ -1999,7 +2205,7 @@ extern "C" int s3b_attention_ex(const float* q, const float* k, const float* v, 
     S3B_OK(ctx.ensure(M * D));
     S3B_OK(kv.ensure(B * sizeof(int)));
     CUDA_OK(cudaMemcpyAsync(kv.p, valid_frames, B * sizeof(int), cudaMemcpyHostToDevice, st));
-    CUDA_OK(launch_qkv_scatter(q, k, v, B, T, Tp, H, 0.125f * 1.4426950408889634f, qs.h(), qs.l(), ks.h(), ks.l(), vts.h(), vts.l(), st));
+    CUDA_OK(launch_qkv_scatter(q, k, v, B, T, Tp, H, kQScale, qs.h(), qs.l(), ks.h(), ks.l(), vts.h(), vts.l(), st));
     AttnParams ap;
     memset(&ap, 0, sizeof(ap));
     const uint64_t BH = (uint64_t)B * H;

@@ -44,6 +44,10 @@ EXPORTED_SYMBOLS = [
     "s3b_weighted_sum",
     "s3b_weighted_sum_backward",
     "s3b_linear_f32",
+    "s3b_linear_ex",
+    "s3b_qkv_f32",
+    "s3b_conv_gemm_f32",
+    "s3b_posconv_f32",
     "s3b_layernorm_f32",
     "s3b_gemm_bench",
     "s3b_attention_f32",
@@ -124,6 +128,30 @@ class S3BAttentionOpts(C.Structure):
         self.struct_size = C.sizeof(S3BAttentionOpts)
 
 
+class S3BLinearOpts(C.Structure):
+    """Mirror of ``struct s3b_linear_opts`` (scheme and out_fmt default to -1: the library's scheme, fp32 output)."""
+
+    _fields_ = [
+        ("struct_size", C.c_int32),
+        ("scheme", C.c_int32),
+        ("tile_n", C.c_int32),
+        ("out_fmt", C.c_int32),
+        ("row_mask", C.c_void_p),
+        ("out_pre", C.c_void_p),
+        ("lda", C.c_int64),
+        ("a_off", C.c_int64),
+        ("scheme_used", C.c_int32),
+        ("tile_n_used", C.c_int32),
+        ("reserved", C.c_int64 * 2),
+    ]
+
+    def __init__(self, **kw):
+        kw.setdefault("scheme", -1)
+        kw.setdefault("out_fmt", -1)
+        super().__init__(**kw)
+        self.struct_size = C.sizeof(S3BLinearOpts)
+
+
 FAMILY_HUBERT, FAMILY_WAV2VEC2, FAMILY_WAVLM, FAMILY_DISTILLER = 0, 1, 2, 3
 
 _lib: Optional[C.CDLL] = None
@@ -180,6 +208,10 @@ def load() -> C.CDLL:
     lib.s3b_weighted_sum.argtypes = [f32p, i32, i64, f32p, f32p, vp]
     lib.s3b_weighted_sum_backward.argtypes = [f32p, i32, i64, f32p, f32p, vp]
     lib.s3b_linear_f32.argtypes = [f32p, f32p, f32p, f32p, i64, i32, i32, i32, f32p, vp]
+    lib.s3b_linear_ex.argtypes = [f32p, f32p, f32p, f32p, i64, i32, i32, i32, C.POINTER(S3BLinearOpts), f32p, vp]
+    lib.s3b_qkv_f32.argtypes = [f32p, f32p, f32p, i32, i32, i32, i32, f32p, f32p, f32p, vp]
+    lib.s3b_conv_gemm_f32.argtypes = [f32p, f32p, f32p, i32, i64, i32, i32, i32, i32, f32p, vp]
+    lib.s3b_posconv_f32.argtypes = [f32p, f32p, f32p, i32, i32, i32, i32, i32, i32, i32, f32p, f32p, i32, f32p, vp]
     lib.s3b_gemm_bench.argtypes = [i64, i32, i32, i32, i32, i32, C.POINTER(C.c_float)]
     lib.s3b_layernorm_f32.argtypes = [f32p, i64, i32, f32p, f32p, i32, f32p, vp]
     lib.s3b_attention_f32.argtypes = [f32p, f32p, f32p, C.POINTER(i32), i32, i32, i32, f32p, vp]

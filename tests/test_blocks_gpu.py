@@ -36,7 +36,10 @@ def _stream():
         (2000, 768, 3072, True, False, True),
     ],
 )
-def test_linear_bf16x3(s3b_lib, M, N, K, bias, gelu, res):
+@pytest.mark.parametrize("scheme", [None, 0, 1])
+def test_linear(s3b_lib, scheme, M, N, K, bias, gelu, res):
+    """Both operand schemes, requested explicitly (s3b_linear_ex); f16q8 needs K % 128 == 0 and N % 128 == 0, and a
+    shape without them is refused instead of falling back to bf16x3. None: s3b_linear_f32, the library's default."""
     from s3prl_b200 import lib
 
     g = torch.Generator(device="cuda").manual_seed(M * 7 + N)
@@ -45,12 +48,19 @@ def test_linear_bf16x3(s3b_lib, M, N, K, bias, gelu, res):
     b = torch.randn(N, device="cuda", generator=g) if bias else None
     r = torch.randn(M, N, device="cuda", generator=g) if res else None
     out = torch.full((M, N), float("nan"), device="cuda")
-    lib.check(
-        s3b_lib.s3b_linear_f32(
-            _ptr(a), _ptr(w), _ptr(b) if bias else None, _ptr(r) if res else None, M, N, K, int(gelu), _ptr(out), _stream()
-        )
-    )
+    opts = lib.S3BLinearOpts(scheme=-1 if scheme is None else scheme)
+    args = (_ptr(a), _ptr(w), _ptr(b) if bias else None, _ptr(r) if res else None, M, N, K, int(gelu), C.byref(opts),
+            _ptr(out), _stream())
+    if scheme == 1 and (K % 128 != 0 or N % 128 != 0):
+        with pytest.raises(lib.S3BError, match="f16q8"):
+            lib.check(s3b_lib.s3b_linear_ex(*args))
+        return
+    if scheme is None:
+        lib.check(s3b_lib.s3b_linear_f32(*args[:8], args[9], args[10]))
+    else:
+        lib.check(s3b_lib.s3b_linear_ex(*args))
     torch.cuda.synchronize()
+    assert scheme is None or opts.scheme_used == scheme
     ref = a.double() @ w.double().t()
     if bias:
         ref = ref + b.double()
@@ -61,7 +71,7 @@ def test_linear_bf16x3(s3b_lib, M, N, K, bias, gelu, res):
     assert torch.isfinite(out).all()
     rel = _rel(out, ref)
     mx = (out.double() - ref).abs().max().item()
-    print(f"linear M={M} N={N} K={K}: rel={rel:.3e} maxabs={mx:.3e}")
+    print(f"linear scheme={scheme} tile={opts.tile_n_used} M={M} N={N} K={K}: rel={rel:.3e} maxabs={mx:.3e}")
     assert rel < 1e-4, rel
     assert mx < 2e-4 * ref.abs().max().item() + 1e-5
 
