@@ -17,11 +17,11 @@ struct GemmParams {
     CUtensorMap b_hi, b_lo;
 
     // scheme 1 ("f16q8", CTA-pair kernel only): fp16 main product + two e4m3 correction products.
-    //   a_hi / b_hi are the fp16 planes (box {64, rows}), a_h8 / a_l8 / b_h8 / b_l8 the e4m3 planes (box {128, rows});
-    //   k-blocks are 128 elements wide: block_k == 128, K % 128 == 0; a_lo / b_lo are unused.
+    //   a_hi / b_hi are the fp16 planes (box {64, rows}, SWIZZLE_128B), a_h8 / a_l8 / b_h8 / b_l8 the e4m3 planes
+    //   (box {64, rows}, SWIZZLE_64B); a_lo / b_lo are unused. k-blocks are 64 elements wide (block_k == 64, K % 128 == 0)
+    //   and the kernel walks them twice: num_k_blocks stages of e4m3 corrections, then num_k_blocks of fp16 products.
+    //   num_k_blocks and kb_per_row therefore count 64-element blocks, as in the bf16x3 CTA-pair layout.
     int scheme;
-    int q8_debug;  // s3b_gemm_bench only (timing experiments, wrong numerics): 1 = corrections issued as kind::f16,
-                   // 2 = no scale-input-d, 3 = correction MMAs skipped, 4 = main MMAs skipped
     CUtensorMap a_h8, a_l8, b_h8, b_l8;
 
     // ---- tiling -------------------------------------------------------------------------------
@@ -31,7 +31,7 @@ struct GemmParams {
     int n_tiles;            // output column tiles
     int umma_n;             // columns per tile (multiple of 16, <= 256)
     int two_cta;            // 1: CTA-pair kernel (umma_n == 256, block_k == 64, B boxes hold umma_n/2 rows)
-    int block_k;            // bf16 elements per k-block: gemm_block_k(umma_n) (32 for 128x256 tiles, else 64)
+    int block_k;            // K elements per k-block: gemm_block_k(umma_n) (32 for 128x256 tiles, else 64); f16q8: 64
     int num_k_blocks;       // k-blocks per output tile
     // k-block kb reads   A box at (a_k_per_ntile*n_tile + (kb % kb_per_row)*block_k,
     //                              row0 + (kb / kb_per_row)*a_row_step + a_row_off, batch)
@@ -103,7 +103,7 @@ cudaError_t launch_gemm_bf16x3(const GemmParams& p, int sm_count, cudaStream_t s
 // Returns 0 on success, else a CUresult / -1 (driver entry point missing).
 int encode_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1,
                         uint64_t stride2, uint32_t box0, uint32_t box1);
-// Same for a 1-byte (e4m3) plane: box0 must be 128 elements (one 128-byte swizzle row).
+// Same for a 1-byte (e4m3) plane: box0 is 128 elements (SWIZZLE_128B) or 64 elements (SWIZZLE_64B), one swizzle row.
 int encode_tmap_u8_3d(CUtensorMap* out, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1,
                       uint64_t stride2, uint32_t box0, uint32_t box1);
 

@@ -26,7 +26,10 @@ static constexpr int kBlockM = 128;
 static constexpr int kThreads = 288;
 static constexpr int kSmemBudget = 220 * 1024;
 
-// RB: bytes of one K row of a stage = the swizzle span (128: 64 bf16 / 128 e4m3 elements, 64: 32 bf16 elements)
+// RB: bytes of one K row of a stage plane = the swizzle span (128: 64 bf16 elements, 64: 32 bf16 / 64 e4m3 elements).
+// f16q8 uses RB = 64 with 64 elements of K per stage: pass 0 fills the four planes with 64-byte e4m3 rows
+// [A_l8 A_h8 W_h8 W_l8], pass 1 fills [A16 | W16] with 128-byte fp16 rows (each spanning two planes). Both are
+// 48 KB at BN = 256, which makes the ring four deep there (six at BN = 128).
 template <int BN, int RB>
 struct GemmCfg {
     static constexpr int kAPlane = kBlockM * RB;
@@ -120,7 +123,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
     // two_cta layout: the W boxes hold BN/2 rows and a stage takes two of them (gemm.cuh)
     const int b_boxes = p.two_cta ? 2 : 1;
     const int b_box_rows = BN / b_boxes;
-    const int passes = kScheme == 0 ? 1 : 2;
+    constexpr int kPasses = kScheme == 0 ? 1 : 2;
 
     if (warp == 8) {
         // ===================== TMA producer =====================
@@ -135,7 +138,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
                 const int a_k0 = p.a_k_per_ntile * n_tile;
                 const int b_n0 = p.b_n_tiled ? n_tile * BN : 0;
                 const int b_z0 = n_tile * p.b_z_per_ntile;
-                for (int pass = 0; pass < passes; ++pass) {
+                for (int pass = 0; pass < kPasses; ++pass) {
                     for (int kb = 0; kb < p.num_k_blocks; ++kb) {
                         const int kq = kb / p.kb_per_row;
                         const int kr = kb - kq * p.kb_per_row;
@@ -147,23 +150,24 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
                         const int a_k = a_k0 + kr * p.block_k;
                         const int b_k = (p.b_k_linear ? kb : kr) * p.block_k;
                         const int b_z = p.b_k_linear ? 0 : b_z0 + kq;
-                        // planes: scheme 0 [A_hi A_lo W_hi W_lo]; scheme 1 pass 0 [A_l8 A_h8 W_h8 W_l8],
-                        // pass 1 [A16 k, A16 k+64, W16 k, W16 k+64] (128 elements of K per stage)
-                        const CUtensorMap* ma0 = &p.a_hi;
-                        const CUtensorMap* ma1 = &p.a_lo;
-                        const CUtensorMap* mb0 = &p.b_hi;
-                        const CUtensorMap* mb1 = &p.b_lo;
-                        int ak1 = a_k, bk1 = b_k;
-                        if (kScheme == 1) {
-                            if (pass == 0) ma0 = &p.a_l8, ma1 = &p.a_h8, mb0 = &p.b_h8, mb1 = &p.b_l8;
-                            else ma1 = &p.a_hi, mb1 = &p.b_hi, ak1 = a_k + 64, bk1 = b_k + 64;
-                        }
-                        tma_load_3d(st, ma0, &full_bar[stage], a_k, a_row, batch);
-                        tma_load_3d(st + Cfg::kAPlane, ma1, &full_bar[stage], ak1, a_row, batch);
-                        for (int h = 0; h < b_boxes; ++h) {
-                            const int rows = b_n0 + h * b_box_rows;
-                            tma_load_3d(sb + h * b_box_rows * RB, mb0, &full_bar[stage], b_k, rows, b_z);
-                            tma_load_3d(sb + Cfg::kBPlane + h * b_box_rows * RB, mb1, &full_bar[stage], bk1, rows, b_z);
+                        if (kScheme == 1 && pass == 1) {
+                            // [A16 | W16]: one fp16 box of 128-byte rows each, spanning both planes of the stage
+                            tma_load_3d(st, &p.a_hi, &full_bar[stage], a_k, a_row, batch);
+                            for (int h = 0; h < b_boxes; ++h)
+                                tma_load_3d(sb + h * b_box_rows * 128, &p.b_hi, &full_bar[stage], b_k, b_n0 + h * b_box_rows, b_z);
+                        } else {
+                            // planes: scheme 0 [A_hi A_lo W_hi W_lo]; scheme 1 pass 0 [A_l8 A_h8 W_h8 W_l8] (64-byte rows)
+                            const CUtensorMap* ma0 = kScheme == 0 ? &p.a_hi : &p.a_l8;
+                            const CUtensorMap* ma1 = kScheme == 0 ? &p.a_lo : &p.a_h8;
+                            const CUtensorMap* mb0 = kScheme == 0 ? &p.b_hi : &p.b_h8;
+                            const CUtensorMap* mb1 = kScheme == 0 ? &p.b_lo : &p.b_l8;
+                            tma_load_3d(st, ma0, &full_bar[stage], a_k, a_row, batch);
+                            tma_load_3d(st + Cfg::kAPlane, ma1, &full_bar[stage], a_k, a_row, batch);
+                            for (int h = 0; h < b_boxes; ++h) {
+                                const int rows = b_n0 + h * b_box_rows;
+                                tma_load_3d(sb + h * b_box_rows * RB, mb0, &full_bar[stage], b_k, rows, b_z);
+                                tma_load_3d(sb + Cfg::kBPlane + h * b_box_rows * RB, mb1, &full_bar[stage], b_k, rows, b_z);
+                            }
                         }
                         if (++stage == kStages) stage = 0, phase ^= 1u;
                     }
@@ -192,7 +196,10 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
         // tensor pipe is fed while this warpgroup waits for the next stage.
         int pending = -1;
         bool first = true;
-        for (int pass = 0; pass < passes; ++pass) {
+        // The pass loop is unrolled so that every wgmma sits in straight-line code: with a runtime pass index the
+        // rescale below is a branch ptxas treats as divergent, and it then serialises every wgmma of the kernel.
+#pragma unroll
+        for (int pass = 0; pass < kPasses; ++pass) {
             if (kScheme == 1 && pass == 1) {
                 // the corrections carry 2^kQ8Scale: scale them back before the main product accumulates (exact)
                 wgmma_wait<0>();
@@ -204,6 +211,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
                 const float s = 1.0f / (float)(1 << kQ8Scale);
 #pragma unroll
                 for (int i = 0; i < kNR; ++i) acc[i] *= s;
+                wgmma_fence();
             }
             for (int kb = 0; kb < p.num_k_blocks; ++kb) {
                 mbar_wait(&full_bar[stage], phase);
@@ -225,24 +233,23 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
                             first = false;
                         }
                     }
-                } else if (pass == 0) {  // (kScheme == 1 from here on)
-                    // A_l8 x W_h8 and A_h8 x W_l8, K = 32 per MMA (32 bytes)
+                } else if (pass == 0) {  // (kScheme == 1 from here on, RB == 64)
+                    // A_l8 x W_h8 and A_h8 x W_l8, K = 32 per MMA (32 bytes), two k-steps per 64-byte row
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
+                    for (int k = 0; k < 2; ++k) {
                         const uint64_t ko = (uint64_t)(k * 2);
                         Wgmma<BN, 2>::ss(acc, da0 + ko, db0 + ko, first ? 0u : 1u);
                         Wgmma<BN, 2>::ss(acc, da1 + ko, db1 + ko, 1u);
                         first = false;
                     }
                 } else {
-                    // A16[k..k+64) x W16[k..k+64) and the next 64, K = 16 per MMA
+                    // A16[k..k+64) x W16[k..k+64), K = 16 per MMA: one box of 128-byte rows each, spanning both
+                    // 64-byte planes of the stage (the warpgroup's 64 A rows start 64 * 128 bytes apart)
+                    const uint64_t da = make_wgmma_desc<128>(st + wg * 64 * 128), db = make_wgmma_desc<128>(b0);
 #pragma unroll
-                    for (int t = 0; t < 2; ++t) {
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) {
-                            const uint64_t ko = (uint64_t)(k * 2);
-                            Wgmma<BN, 1>::ss(acc, (t == 0 ? da0 : da1) + ko, (t == 0 ? db0 : db1) + ko, 1u);
-                        }
+                    for (int k = 0; k < 4; ++k) {
+                        const uint64_t ko = (uint64_t)(k * 2);
+                        Wgmma<BN, 1>::ss(acc, da + ko, db + ko, 1u);
                     }
                 }
                 wgmma_commit();
@@ -295,7 +302,7 @@ static cudaError_t launch_impl(const GemmParams& p, int sm_count, cudaStream_t s
 template <int BN>
 static cudaError_t launch_n(const GemmParams& p, int sm_count, cudaStream_t stream) {
     if (p.scheme != 0) {
-        if constexpr (BN == 256 || BN == 192 || BN == 128) return launch_impl<BN, 128, 1>(p, sm_count, stream);
+        if constexpr (BN == 256 || BN == 192 || BN == 128) return launch_impl<BN, 64, 1>(p, sm_count, stream);
         return cudaErrorInvalidValue;
     }
     if (p.block_k == 64) return launch_impl<BN, 128, 0>(p, sm_count, stream);
@@ -304,7 +311,7 @@ static cudaError_t launch_n(const GemmParams& p, int sm_count, cudaStream_t stre
 
 cudaError_t launch_gemm_bf16x3(const GemmParams& p, int sm_count, cudaStream_t stream) {
     if (p.ln_gamma != nullptr) return cudaErrorNotSupported;  // LayerNorm is a separate launch (norm.cu)
-    if (p.scheme != 0 ? (p.block_k != 128 || p.k_steps != 0) : (p.block_k != 64 && p.block_k != 32))
+    if (p.scheme != 0 ? (p.block_k != 64 || p.k_steps != 0) : (p.block_k != 64 && p.block_k != 32))
         return cudaErrorInvalidValue;
     if (p.scheme == 0 && p.block_k == 32 && (p.two_cta || p.k_steps != 0)) return cudaErrorInvalidValue;
     if (p.out_fmt != 0 && (p.qkv_mode || (p.out_hi != nullptr && (p.out_h8 == nullptr || p.out_l8 == nullptr))))
@@ -365,13 +372,15 @@ int encode_tmap_u8_3d(CUtensorMap* out, const void* base, uint64_t d0, uint64_t 
                       uint64_t stride2, uint32_t box0, uint32_t box1) {
     PFN_encodeTiled fn = get_encode_fn();
     if (fn == nullptr) return -1;
-    if (box0 != 128) return -2;  // one 128-byte swizzle row of e4m3 elements
+    // the swizzle span equals the box row: 128 e4m3 elements -> 128 B, 64 elements -> 64 B
+    if (box0 != 128 && box0 != 64) return -2;
+    const CUtensorMapSwizzle sw = box0 == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
     cuuint64_t dims[3] = {d0, d1, d2};
     cuuint64_t strides[2] = {stride1, stride2};  // bytes == elements
     cuuint32_t box[3] = {box0, box1, 1};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void*>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return (int)r;
 }

@@ -719,17 +719,24 @@ static int use_cta_pairs(int umma_n) { return ((umma_n == 256 || umma_n == 128) 
 
 static int g_force_pair_un = 0;  // s3b_gemm_bench: force the tile width (tile-shape sweeps)
 
-// Tile width for a flat [M][N] linear layer: 256 columns (one 128 x 256 tile per SM and round) unless the 256-wide
-// tiles would leave more than half of the SMs idle in the last round; then 128 columns (twice the tiles, each
-// re-reading its A rows, but the work spreads over all SMs). Both widths give bit-identical results.
+// Tile width for a flat [M][N] linear layer. Both widths give bit-identical results; the rule comes from
+// tools/gemm_shapes.py on an H100 80GB HBM3 (same ranking at 400 W and 700 W power limits), at the encoder shapes of
+// hubert_base (K = 768, 3072) and wav2vec2_large (K = 1024, 4096), M = 7984..15984:
+//  - bf16x3, and f16q8 with K <= 1024: 128 columns, 1.3x-2x faster than 256 at every measured shape.
+//  - f16q8 with K >= 3072 (fc2): 256 columns are 3-15% faster when their last round of tiles fills at least half of
+//    the SMs (or none is partial); otherwise that round runs half empty and 128 columns are 19% faster (hubert_base
+//    fc2 at M = 7984: 189 tiles of 256 on 132 SMs). The K >= 2048 cut lies between measured Ks (1024 and 3072).
+// The epilogue kind (epi_kind) does not enter the rule: at K <= 1024 the GELU (fc1) and fp32 epilogues ranked the two
+// widths the same way.
 static int pick_pair_umma_n(int64_t M, int N, int K, int epi_kind, int sm_count, int scheme = 0) {
-    (void)K, (void)epi_kind, (void)scheme;
+    (void)epi_kind;
     if (g_force_pair_un != 0 && N % g_force_pair_un == 0) return g_force_pair_un;
     if (N % 256 != 0) return (N % 128 == 0) ? 128 : 0;
+    if (scheme == 0 || K < 2048) return 128;
     const int sms = sm_count > 0 ? sm_count : 1;
     const int64_t tiles = (M + 127) / 128 * (N / 256);
     const int64_t last = tiles % sms;
-    return (last != 0 && last < sms / 2 && tiles < 4 * (int64_t)sms) ? 128 : 256;
+    return (last == 0 || last >= sms / 2) ? 256 : 128;
 }
 
 static int pick_umma_n(int N) {
@@ -764,12 +771,12 @@ static int linear_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, in
     if (scheme != 0) {
         if (!pair || K % 128 != 0) return fail("f16q8 GEMM needs CTA pairs and K %% 128 == 0 (N=%d K=%d)", N, K);
         TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, 128));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8() + a_off, K, M, 1, lda, (uint64_t)M * lda, 128, 128));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8() + a_off, K, M, 1, lda, (uint64_t)M * lda, 128, 128));
+        TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, 128));
+        TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, 128));
         TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, (uint64_t)N * K, 64, un / 2));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, N, 1, K, (uint64_t)N * K, 128, un / 2));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, N, 1, K, (uint64_t)N * K, 128, un / 2));
-        p.scheme = 1, p.two_cta = 1, p.block_k = 128, p.num_k_blocks = K / 128, p.kb_per_row = K / 128;
+        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, N, 1, K, (uint64_t)N * K, 64, un / 2));
+        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, N, 1, K, (uint64_t)N * K, 64, un / 2));
+        p.scheme = 1, p.two_cta = 1, p.block_k = 64, p.num_k_blocks = K / 64, p.kb_per_row = K / 64;
     } else {
         const int bk = pair ? 64 : gemm_block_k(un);
         const int bbox = pair ? un / 2 : un;  // CTA pairs: each CTA loads half of the tile's W rows
@@ -798,12 +805,12 @@ static int conv_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int 
     if (scheme != 0) {
         if (!pair) return fail("f16q8 GEMM needs CTA pairs");
         TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 128, 128));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 128, 128));
+        TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
+        TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
         TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, C, 1, K, (uint64_t)C * K, 64, 128));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, C, 1, K, (uint64_t)C * K, 128, 128));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, C, 1, K, (uint64_t)C * K, 128, 128));
-        p.scheme = 1, p.two_cta = 1, p.block_k = 128, p.num_k_blocks = K / 128, p.kb_per_row = (2 * C) / 128;
+        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, C, 1, K, (uint64_t)C * K, 64, 128));
+        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, C, 1, K, (uint64_t)C * K, 64, 128));
+        p.scheme = 1, p.two_cta = 1, p.block_k = 64, p.num_k_blocks = K / 64, p.kb_per_row = (2 * C) / 64;
     } else {
         const int bk = pair ? 64 : gemm_block_k(256);
         const int bbox = pair ? 128 : 256;
@@ -2137,7 +2144,6 @@ extern "C" int s3b_gemm_bench(int64_t M, int32_t N, int32_t K, int32_t gelu, int
     if (K % 128 != 0 || N % 128 != 0 || !pairs_enabled()) scheme = 0;
     int r = linear_params(p, as, ws, M, N, K, gelu ? 2 : 0, scheme);
     g_force_pair_un = 0;
-    if (const char* dbg = getenv("S3B_Q8_DEBUG")) p.q8_debug = atoi(dbg);
     if (r == 0) {
         Epi e;
         e.bias = bias.as<float>();
