@@ -46,6 +46,8 @@ struct GemmParams {
     int b_z_per_ntile;
 
     // ---- epilogue: v = acc (+bias[n]) ; gelu? ; (+residual[m][n]) ; row_mask[m] ? 0 -----------------
+    // The launch picks one kernel instantiation per output kind: out_f32, operand planes (out_hi ...), both (widths
+    // >= 128 only) or the QKV scatter (widths >= 128 only). A launch with none of them is an error.
     int out_rows_per_batch;  // flat output row m = batch*out_rows_per_batch + row
     int ldo;                 // leading dimension (elements) of out_f32/out_hi/out_lo/residual
     const float* bias;

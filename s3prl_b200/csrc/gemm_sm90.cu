@@ -9,11 +9,15 @@
 //   pos_conv (grouped Conv1d k=128)    s3prl/upstream/wav2vec2/wav2vec2_model.py:2937-2953,3064-3067
 //   q/k/v/out projections, fc1, fc2    s3prl/upstream/wav2vec2/wav2vec2_model.py:1146-1168,3260-3322
 //
-// One CTA per SM, persistent over 128 x BN output tiles; 288 threads:
-//   warps 0..3, 4..7 : two consumer warpgroups, 64 output rows each (wgmma m64nBN, accumulators in registers),
-//                      then the epilogue straight from the accumulator registers
-//   warp 8           : TMA producer (A and W boxes -> swizzled shared-memory ring of kStages stages)
-// With 288 threads ptxas may give every thread up to 224 registers: the 128 accumulators of a 256-wide tile fit.
+// One CTA per SM, persistent over 128 x BN output tiles, one TMA producer warp filling a swizzled shared-memory ring of
+// kStages stages in tile order. Two kernels consume it:
+//   cooperative (every width but 128), 288 threads: warps 0..3 and 4..7 are two consumer warpgroups that share each
+//     tile, 64 rows each (wgmma m64nBN); warp 8 is the producer. ptxas gives these kernels at most 168 registers a
+//     thread, which holds the 128 accumulators of a 256-wide tile.
+//   ping-pong (128-wide tiles), 384 threads: warpgroups 0 and 1 take alternate tiles, each a whole 128 x 128 tile
+//     (two m64n128 wgmmas per k-step, 128 accumulators); warp 8 of warpgroup 2 is the producer. One warpgroup's
+//     epilogue then overlaps the other's MMAs. setmaxnreg moves registers from the producer warpgroup to the consumers.
+// Both run the same k order and f16q8 pass order per output element, so the two widths agree bit for bit.
 #include <stdio.h>
 
 #include "common.cuh"
@@ -24,6 +28,7 @@ namespace s3b {
 
 static constexpr int kBlockM = 128;
 static constexpr int kThreads = 288;
+static constexpr int kPingPongThreads = 384;
 static constexpr int kSmemBudget = 220 * 1024;
 
 // RB: bytes of one K row of a stage plane = the swizzle span (128: 64 bf16 elements, 64: 32 bf16 / 64 e4m3 elements).
@@ -40,58 +45,356 @@ struct GemmCfg {
     static_assert(kStages >= 2, "tile too large for the shared-memory ring");
 };
 
-// Epilogue of one row pair (2 consecutive columns): v = acc (+bias) ; gelu? ; then the output modes of gemm.cuh
-__device__ __forceinline__ void epilogue_pair(const GemmParams& p, size_t m, int col, bool masked, float x0, float x1) {
-    if (p.bias != nullptr) {
-        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-        x0 += b.x, x1 += b.y;
-    }
-    if (p.gelu) x0 = gelu_erf(x0), x1 = gelu_erf(x1);
-    if (p.qkv_mode) {
-        // m = b*T + t ; col = which*D + h*64 + d (column pairs never straddle a head)
-        const int b = (int)(m / (size_t)p.T);
-        const int t = (int)(m - (size_t)b * p.T);
-        const int which = col / p.D;
-        const int within = col - which * p.D;
-        const int h = within >> 6;
-        const int d = within & 63;
-        const size_t bh = (size_t)b * p.H + h;
-        if (which < 2) {
-            if (which == 0) x0 *= p.q_scale, x1 *= p.q_scale;
-            uint32_t hi, lo;
-            split_pack2(x0, x1, hi, lo);
-            const size_t o = (bh * p.T + t) * 64 + d;
-            *reinterpret_cast<uint32_t*>((which == 0 ? p.q_hi : p.k_hi) + o) = hi;
-            *reinterpret_cast<uint32_t*>((which == 0 ? p.q_lo : p.k_lo) + o) = lo;
-        } else {
-            __nv_bfloat16 h0, l0, h1, l1;
-            split_bf16(x0, h0, l0);
-            split_bf16(x1, h1, l1);
-            const size_t o = (bh * 64 + d) * (size_t)p.Tp + t;
-            p.vt_hi[o] = h0, p.vt_lo[o] = l0;
-            p.vt_hi[o + p.Tp] = h1, p.vt_lo[o + p.Tp] = l1;
+// Epilogue kinds, one kernel instantiation each (chosen per launch in launch_gemm_bf16x3). Every non-QKV kind computes
+//   v = acc (+bias) ; gelu? ; out_pre = v? ; (+residual) ; row_mask ? 0
+// and stores v as fp32, as operand planes, or both.
+enum EpiKind { kEpiF32 = 1, kEpiPlanes = 2, kEpiBoth = 3, kEpiQkv = 4 };
+
+__device__ __forceinline__ void setmaxnreg_dec40() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+__device__ __forceinline__ void setmaxnreg_inc232() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
+
+// ===================== TMA producer: every tile of this CTA, kPasses * num_k_blocks stages each, in tile order ====
+template <int BN, int RB, int kScheme>
+__device__ __forceinline__ void produce(const GemmParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar) {
+    using Cfg = GemmCfg<BN, RB>;
+    constexpr int kPasses = kScheme == 0 ? 1 : 2;
+    const int num_tiles = p.batches * p.tiles_m_per_batch * p.n_tiles;
+    // two_cta layout: the W boxes hold BN/2 rows and a stage takes two of them (gemm.cuh)
+    const int b_boxes = p.two_cta ? 2 : 1;
+    const int b_box_rows = BN / b_boxes;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int n_tile = tile % p.n_tiles;
+        const int mt = tile / p.n_tiles;
+        const int batch = mt / p.tiles_m_per_batch;
+        const int row0 = (mt - batch * p.tiles_m_per_batch) * kBlockM;
+        const int a_k0 = p.a_k_per_ntile * n_tile;
+        const int b_n0 = p.b_n_tiled ? n_tile * BN : 0;
+        const int b_z0 = n_tile * p.b_z_per_ntile;
+        for (int pass = 0; pass < kPasses; ++pass) {
+            for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+                const int kq = kb / p.kb_per_row;
+                const int kr = kb - kq * p.kb_per_row;
+                mbar_wait(&empty_bar[stage], phase ^ 1u);
+                uint8_t* st = smem + stage * Cfg::kStageBytes;
+                uint8_t* sb = st + 2 * Cfg::kAPlane;
+                mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)Cfg::kStageBytes);
+                const int a_row = row0 + kq * p.a_row_step + p.a_row_off;
+                const int a_k = a_k0 + kr * p.block_k;
+                const int b_k = (p.b_k_linear ? kb : kr) * p.block_k;
+                const int b_z = p.b_k_linear ? 0 : b_z0 + kq;
+                if (kScheme == 1 && pass == 1) {
+                    // [A16 | W16]: one fp16 box of 128-byte rows each, spanning both planes of the stage
+                    tma_load_3d(st, &p.a_hi, &full_bar[stage], a_k, a_row, batch);
+                    for (int h = 0; h < b_boxes; ++h)
+                        tma_load_3d(sb + h * b_box_rows * 128, &p.b_hi, &full_bar[stage], b_k, b_n0 + h * b_box_rows, b_z);
+                } else {
+                    // planes: scheme 0 [A_hi A_lo W_hi W_lo]; scheme 1 pass 0 [A_l8 A_h8 W_h8 W_l8] (64-byte rows)
+                    const CUtensorMap* ma0 = kScheme == 0 ? &p.a_hi : &p.a_l8;
+                    const CUtensorMap* ma1 = kScheme == 0 ? &p.a_lo : &p.a_h8;
+                    const CUtensorMap* mb0 = kScheme == 0 ? &p.b_hi : &p.b_h8;
+                    const CUtensorMap* mb1 = kScheme == 0 ? &p.b_lo : &p.b_l8;
+                    tma_load_3d(st, ma0, &full_bar[stage], a_k, a_row, batch);
+                    tma_load_3d(st + Cfg::kAPlane, ma1, &full_bar[stage], a_k, a_row, batch);
+                    for (int h = 0; h < b_boxes; ++h) {
+                        const int rows = b_n0 + h * b_box_rows;
+                        tma_load_3d(sb + h * b_box_rows * RB, mb0, &full_bar[stage], b_k, rows, b_z);
+                        tma_load_3d(sb + Cfg::kBPlane + h * b_box_rows * RB, mb1, &full_bar[stage], b_k, rows, b_z);
+                    }
+                }
+                if (++stage == Cfg::kStages) stage = 0, phase ^= 1u;
+            }
         }
-        return;
-    }
-    const size_t off = m * (size_t)p.ldo + col;
-    if (p.out_pre != nullptr) *reinterpret_cast<float2*>(p.out_pre + off) = make_float2(x0, x1);
-    if (p.residual != nullptr) {
-        const float2 r = __ldg(reinterpret_cast<const float2*>(p.residual + off));
-        x0 += r.x, x1 += r.y;
-    }
-    if (masked) x0 = 0.f, x1 = 0.f;
-    if (p.out_f32 != nullptr) *reinterpret_cast<float2*>(p.out_f32 + off) = make_float2(x0, x1);
-    if (p.out_hi != nullptr) {
-        const OutPlanes o{p.out_hi, p.out_lo, p.out_h8, p.out_l8, p.out_fmt};
-        store_planes2(o, x0, x1, off);
     }
 }
 
-template <int BN, int RB, int kScheme>
+// ===================== MMAs of one tile: kHalves 64-row halves of A starting at half `half0`, acc[h] per half ======
+// Stage s is released (one arrive per warp of the warpgroup) once the wgmma group reading it has retired; one group
+// stays in flight so that the tensor pipe is fed while this warpgroup waits for the next stage. Every output element
+// sees the same wgmma sequence whichever kernel, warpgroup or half runs it.
+template <int BN, int RB, int kScheme, int kHalves>
+__device__ __forceinline__ void mma_tile(const GemmParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                         int half0, int lane, int& stage, uint32_t& phase,
+                                         float (&acc)[kHalves][BN / 2]) {
+    using Cfg = GemmCfg<BN, RB>;
+    constexpr int kStages = Cfg::kStages;
+    constexpr int kNR = BN / 2;
+    constexpr int kPasses = kScheme == 0 ? 1 : 2;
+    const int k_steps = p.k_steps > 0 ? p.k_steps : RB / 32;  // 16-wide k-steps per stage (scheme 0)
+#pragma unroll
+    for (int h = 0; h < kHalves; ++h)
+#pragma unroll
+        for (int i = 0; i < kNR; ++i) acc[h][i] = 0.f;
+
+    int pending = -1;
+    bool first = true;
+    // The pass loop is unrolled so that every wgmma sits in straight-line code: with a runtime pass index the
+    // rescale below is a branch ptxas treats as divergent, and it then serialises every wgmma of the kernel.
+#pragma unroll
+    for (int pass = 0; pass < kPasses; ++pass) {
+        if (kScheme == 1 && pass == 1) {
+            // the corrections carry 2^kQ8Scale: scale them back before the main product accumulates (exact)
+            wgmma_wait<0>();
+            if (pending >= 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[pending]);
+                pending = -1;
+            }
+            const float s = 1.0f / (float)(1 << kQ8Scale);
+#pragma unroll
+            for (int h = 0; h < kHalves; ++h)
+#pragma unroll
+                for (int i = 0; i < kNR; ++i) acc[h][i] *= s;
+            wgmma_fence();
+        }
+        for (int kb = 0; kb < p.num_k_blocks; ++kb) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint32_t st = smem_u32(smem + stage * Cfg::kStageBytes);
+            const uint32_t b0 = st + 2 * Cfg::kAPlane, b1 = b0 + Cfg::kBPlane;
+            const uint64_t db0 = make_wgmma_desc<RB>(b0), db1 = make_wgmma_desc<RB>(b1);
+            wgmma_fence();
+            if constexpr (kScheme == 0) {
+#pragma unroll
+                for (int k = 0; k < RB / 32; ++k) {
+                    if (k < k_steps) {
+                        // advance 16 bf16 (= 32 bytes) along K inside the swizzle atom: +2 in (addr >> 4) units
+                        const uint64_t ko = (uint64_t)(k * 2);
+#pragma unroll
+                        for (int h = 0; h < kHalves; ++h) {
+                            const uint32_t a0 = st + (half0 + h) * 64 * RB, a1 = a0 + Cfg::kAPlane;
+                            const uint64_t da0 = make_wgmma_desc<RB>(a0), da1 = make_wgmma_desc<RB>(a1);
+                            Wgmma<BN, 0>::ss(acc[h], da1 + ko, db0 + ko, first ? 0u : 1u);
+                            Wgmma<BN, 0>::ss(acc[h], da0 + ko, db1 + ko, 1u);
+                            Wgmma<BN, 0>::ss(acc[h], da0 + ko, db0 + ko, 1u);
+                        }
+                        first = false;
+                    }
+                }
+            } else if (pass == 0) {  // (kScheme == 1 from here on, RB == 64)
+                // A_l8 x W_h8 and A_h8 x W_l8, K = 32 per MMA (32 bytes), two k-steps per 64-byte row
+#pragma unroll
+                for (int k = 0; k < 2; ++k) {
+                    const uint64_t ko = (uint64_t)(k * 2);
+#pragma unroll
+                    for (int h = 0; h < kHalves; ++h) {
+                        const uint32_t a0 = st + (half0 + h) * 64 * RB, a1 = a0 + Cfg::kAPlane;
+                        const uint64_t da0 = make_wgmma_desc<RB>(a0), da1 = make_wgmma_desc<RB>(a1);
+                        Wgmma<BN, 2>::ss(acc[h], da0 + ko, db0 + ko, first ? 0u : 1u);
+                        Wgmma<BN, 2>::ss(acc[h], da1 + ko, db1 + ko, 1u);
+                    }
+                    first = false;
+                }
+            } else {
+                // A16[k..k+64) x W16[k..k+64), K = 16 per MMA: one box of 128-byte rows each, spanning both
+                // 64-byte planes of the stage (a half's 64 A rows start 64 * 128 bytes apart)
+                const uint64_t db = make_wgmma_desc<128>(b0);
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const uint64_t ko = (uint64_t)(k * 2);
+#pragma unroll
+                    for (int h = 0; h < kHalves; ++h) {
+                        const uint64_t da = make_wgmma_desc<128>(st + (half0 + h) * 64 * 128);
+                        Wgmma<BN, 1>::ss(acc[h], da + ko, db + ko, 1u);
+                    }
+                }
+            }
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (pending >= 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[pending]);
+            }
+            pending = stage;
+            if (++stage == kStages) stage = 0, phase ^= 1u;
+        }
+    }
+    wgmma_wait<0>();
+    if (pending >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[pending]);
+    }
+}
+
+// two consecutive columns of one operand-plane format (the arithmetic of store_planes2)
+template <int kFmt>
+__device__ __forceinline__ void store_plane_pair(const GemmParams& p, float x0, float x1, size_t off) {
+    if constexpr (kFmt != 0) {
+        uint32_t h;
+        uint16_t a, b;
+        split_q8_pack2(x0, x1, h, a, b);
+        *reinterpret_cast<uint32_t*>(p.out_hi + off) = h;
+        *reinterpret_cast<uint16_t*>(p.out_h8 + off) = a;
+        *reinterpret_cast<uint16_t*>(p.out_l8 + off) = b;
+    } else {
+        uint32_t h, l;
+        split_pack2(x0, x1, h, l);
+        *reinterpret_cast<uint32_t*>(p.out_hi + off) = h;
+        *reinterpret_cast<uint32_t*>(p.out_lo + off) = l;
+    }
+}
+
+// ===================== epilogue of one tile, straight from the accumulator registers ===============================
+// acc[h] holds rows row_base + 64 h + {0, 8} (register 4j + 2i + {0,1}: row + 8i, columns col0 + 8j + {0,1}).
+// Per-row work (flat row, mask, offsets, QKV's b and t) is done once per row, the bias once per chunk of kCh column
+// pairs for all rows, and every load of a chunk is issued before any of its stores. Mode tests are uniform branches
+// around whole chunks, never per pair.
+template <int BN, int kEpi, int kHalves>
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, float (&acc)[kHalves][BN / 2], int batch,
+                                              int row_base, int col0) {
+    constexpr int kJ = BN / 8;               // column pairs per row
+    // pairs per chunk: 8, but 2 next to the 128 accumulators of a 256-wide cooperative tile (168 registers at most)
+    constexpr int kCh = BN * kHalves >= 256 && kHalves == 1 ? 2 : (kJ < 8 ? kJ : 8);
+    constexpr int kRows = 2 * kHalves;       // rows per thread
+    static_assert(kJ % kCh == 0, "chunking");
+    bool ok[kRows];
+    size_t m[kRows];
+#pragma unroll
+    for (int s = 0; s < kRows; ++s) {
+        const int row = row_base + 64 * (s >> 1) + 8 * (s & 1);
+        ok[s] = row < p.rows_per_batch;
+        m[s] = (size_t)batch * p.out_rows_per_batch + row;
+    }
+    const bool has_bias = p.bias != nullptr;
+
+    if constexpr (kEpi == kEpiQkv) {
+        // m = b*T + t ; col = which*D + h*64 + d (column pairs never straddle a head)
+        //   q, k: [B][H][T][64] at (b*H*T + t)*64 + h*T*64 + d      v^T: [B][H][64][Tp] at b*H*64*Tp + t + (h*64 + d)*Tp
+        const int T = p.T, D = p.D;
+        size_t base_qk[kRows], base_v[kRows];
+#pragma unroll
+        for (int s = 0; s < kRows; ++s) {
+            const int b = (int)m[s] / T;
+            const int t = (int)m[s] - b * T;
+            base_qk[s] = ((size_t)b * p.H * T + t) * 64;
+            base_v[s] = (size_t)b * p.H * 64 * p.Tp + t;
+        }
+        int which = col0 / D;
+        int within = col0 - which * D;
+#pragma unroll
+        for (int c = 0; c < kJ; c += kCh) {
+            float2 bv[kCh];
+            if (has_bias) {
+#pragma unroll
+                for (int jj = 0; jj < kCh; ++jj) bv[jj] = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 8 * (c + jj)));
+            }
+#pragma unroll
+            for (int jj = 0; jj < kCh; ++jj) {
+                const int j = c + jj;
+                const int h = within >> 6, d = within & 63;
+                if (which < 2) {
+                    __nv_bfloat16* dst_hi = which == 0 ? p.q_hi : p.k_hi;
+                    __nv_bfloat16* dst_lo = which == 0 ? p.q_lo : p.k_lo;
+                    const int o_col = h * T * 64 + d;
+#pragma unroll
+                    for (int s = 0; s < kRows; ++s) {
+                        if (!ok[s]) continue;
+                        float x0 = acc[s >> 1][4 * j + 2 * (s & 1)], x1 = acc[s >> 1][4 * j + 2 * (s & 1) + 1];
+                        if (has_bias) x0 += bv[jj].x, x1 += bv[jj].y;
+                        if (which == 0) x0 *= p.q_scale, x1 *= p.q_scale;
+                        uint32_t hi, lo;
+                        split_pack2(x0, x1, hi, lo);
+                        *reinterpret_cast<uint32_t*>(dst_hi + base_qk[s] + o_col) = hi;
+                        *reinterpret_cast<uint32_t*>(dst_lo + base_qk[s] + o_col) = lo;
+                    }
+                } else {
+                    const int o_col = within * p.Tp;
+#pragma unroll
+                    for (int s = 0; s < kRows; ++s) {
+                        if (!ok[s]) continue;
+                        float x0 = acc[s >> 1][4 * j + 2 * (s & 1)], x1 = acc[s >> 1][4 * j + 2 * (s & 1) + 1];
+                        if (has_bias) x0 += bv[jj].x, x1 += bv[jj].y;
+                        __nv_bfloat16 h0, l0, h1, l1;
+                        split_bf16(x0, h0, l0);
+                        split_bf16(x1, h1, l1);
+                        const size_t o = base_v[s] + o_col;
+                        p.vt_hi[o] = h0, p.vt_lo[o] = l0;
+                        p.vt_hi[o + p.Tp] = h1, p.vt_lo[o + p.Tp] = l1;
+                    }
+                }
+                within += 8;
+                if (within >= D) within -= D, ++which;
+            }
+        }
+        return;
+    } else {
+        const bool gelu = p.gelu != 0, has_res = p.residual != nullptr, has_pre = p.out_pre != nullptr;
+        const int fmt = p.out_fmt;
+        size_t off[kRows];
+        bool zero[kRows];
+#pragma unroll
+        for (int s = 0; s < kRows; ++s) {
+            off[s] = m[s] * (size_t)p.ldo + col0;
+            zero[s] = ok[s] && p.row_mask != nullptr && p.row_mask[m[s]] != 0;
+        }
+#pragma unroll
+        for (int c = 0; c < kJ; c += kCh) {
+            float2 bv[kCh];
+            if (has_bias) {
+#pragma unroll
+                for (int jj = 0; jj < kCh; ++jj) bv[jj] = __ldg(reinterpret_cast<const float2*>(p.bias + col0 + 8 * (c + jj)));
+            }
+#pragma unroll
+            for (int s = 0; s < kRows; ++s) {
+                if (!ok[s]) continue;
+                float(&a)[BN / 2] = acc[s >> 1];
+                const int r2 = 2 * (s & 1);
+                float2 rv[kCh];
+                if (has_res) {
+#pragma unroll
+                    for (int jj = 0; jj < kCh; ++jj)
+                        rv[jj] = __ldg(reinterpret_cast<const float2*>(p.residual + off[s] + 8 * (c + jj)));
+                }
+                if (has_bias) {
+#pragma unroll
+                    for (int jj = 0; jj < kCh; ++jj) a[4 * (c + jj) + r2] += bv[jj].x, a[4 * (c + jj) + r2 + 1] += bv[jj].y;
+                }
+                if (gelu) {
+#pragma unroll
+                    for (int jj = 0; jj < kCh; ++jj)
+                        a[4 * (c + jj) + r2] = gelu_erf(a[4 * (c + jj) + r2]),
+                        a[4 * (c + jj) + r2 + 1] = gelu_erf(a[4 * (c + jj) + r2 + 1]);
+                }
+                if (has_pre) {
+#pragma unroll
+                    for (int jj = 0; jj < kCh; ++jj)
+                        *reinterpret_cast<float2*>(p.out_pre + off[s] + 8 * (c + jj)) =
+                            make_float2(a[4 * (c + jj) + r2], a[4 * (c + jj) + r2 + 1]);
+                }
+                if (has_res) {
+#pragma unroll
+                    for (int jj = 0; jj < kCh; ++jj) a[4 * (c + jj) + r2] += rv[jj].x, a[4 * (c + jj) + r2 + 1] += rv[jj].y;
+                }
+                if (zero[s]) {
+#pragma unroll
+                    for (int jj = 0; jj < kCh; ++jj) a[4 * (c + jj) + r2] = 0.f, a[4 * (c + jj) + r2 + 1] = 0.f;
+                }
+                if constexpr ((kEpi & kEpiF32) != 0) {
+#pragma unroll
+                    for (int jj = 0; jj < kCh; ++jj)
+                        *reinterpret_cast<float2*>(p.out_f32 + off[s] + 8 * (c + jj)) =
+                            make_float2(a[4 * (c + jj) + r2], a[4 * (c + jj) + r2 + 1]);
+                }
+                if constexpr ((kEpi & kEpiPlanes) != 0) {
+                    if (fmt != 0) {
+#pragma unroll
+                        for (int jj = 0; jj < kCh; ++jj)
+                            store_plane_pair<1>(p, a[4 * (c + jj) + r2], a[4 * (c + jj) + r2 + 1], off[s] + 8 * (c + jj));
+                    } else {
+#pragma unroll
+                        for (int jj = 0; jj < kCh; ++jj)
+                            store_plane_pair<0>(p, a[4 * (c + jj) + r2], a[4 * (c + jj) + r2 + 1], off[s] + 8 * (c + jj));
+                    }
+                }
+            }
+        }
+    }
+}
+
+template <int BN, int RB, int kScheme, int kEpi>
 __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_constant__ GemmParams p) {
     using Cfg = GemmCfg<BN, RB>;
     constexpr int kStages = Cfg::kStages;
-    constexpr int kNR = BN / 2;  // accumulator registers per thread
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment is required by the 128B swizzle atoms (8 rows x 128 B)
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -118,195 +421,147 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
     pdl_wait();  // everything above overlapped the previous kernel's tail; global memory is touched only below
     pdl_launch_dependents();
 
-    const int tiles_m = p.batches * p.tiles_m_per_batch;
-    const int num_tiles = tiles_m * p.n_tiles;
-    // two_cta layout: the W boxes hold BN/2 rows and a stage takes two of them (gemm.cuh)
-    const int b_boxes = p.two_cta ? 2 : 1;
-    const int b_box_rows = BN / b_boxes;
-    constexpr int kPasses = kScheme == 0 ? 1 : 2;
-
     if (warp == 8) {
-        // ===================== TMA producer =====================
-        if (elect_one()) {
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                const int n_tile = tile % p.n_tiles;
-                const int mt = tile / p.n_tiles;
-                const int batch = mt / p.tiles_m_per_batch;
-                const int row0 = (mt - batch * p.tiles_m_per_batch) * kBlockM;
-                const int a_k0 = p.a_k_per_ntile * n_tile;
-                const int b_n0 = p.b_n_tiled ? n_tile * BN : 0;
-                const int b_z0 = n_tile * p.b_z_per_ntile;
-                for (int pass = 0; pass < kPasses; ++pass) {
-                    for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-                        const int kq = kb / p.kb_per_row;
-                        const int kr = kb - kq * p.kb_per_row;
-                        mbar_wait(&empty_bar[stage], phase ^ 1u);
-                        uint8_t* st = smem + stage * Cfg::kStageBytes;
-                        uint8_t* sb = st + 2 * Cfg::kAPlane;
-                        mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)Cfg::kStageBytes);
-                        const int a_row = row0 + kq * p.a_row_step + p.a_row_off;
-                        const int a_k = a_k0 + kr * p.block_k;
-                        const int b_k = (p.b_k_linear ? kb : kr) * p.block_k;
-                        const int b_z = p.b_k_linear ? 0 : b_z0 + kq;
-                        if (kScheme == 1 && pass == 1) {
-                            // [A16 | W16]: one fp16 box of 128-byte rows each, spanning both planes of the stage
-                            tma_load_3d(st, &p.a_hi, &full_bar[stage], a_k, a_row, batch);
-                            for (int h = 0; h < b_boxes; ++h)
-                                tma_load_3d(sb + h * b_box_rows * 128, &p.b_hi, &full_bar[stage], b_k, b_n0 + h * b_box_rows, b_z);
-                        } else {
-                            // planes: scheme 0 [A_hi A_lo W_hi W_lo]; scheme 1 pass 0 [A_l8 A_h8 W_h8 W_l8] (64-byte rows)
-                            const CUtensorMap* ma0 = kScheme == 0 ? &p.a_hi : &p.a_l8;
-                            const CUtensorMap* ma1 = kScheme == 0 ? &p.a_lo : &p.a_h8;
-                            const CUtensorMap* mb0 = kScheme == 0 ? &p.b_hi : &p.b_h8;
-                            const CUtensorMap* mb1 = kScheme == 0 ? &p.b_lo : &p.b_l8;
-                            tma_load_3d(st, ma0, &full_bar[stage], a_k, a_row, batch);
-                            tma_load_3d(st + Cfg::kAPlane, ma1, &full_bar[stage], a_k, a_row, batch);
-                            for (int h = 0; h < b_boxes; ++h) {
-                                const int rows = b_n0 + h * b_box_rows;
-                                tma_load_3d(sb + h * b_box_rows * RB, mb0, &full_bar[stage], b_k, rows, b_z);
-                                tma_load_3d(sb + Cfg::kBPlane + h * b_box_rows * RB, mb1, &full_bar[stage], b_k, rows, b_z);
-                            }
-                        }
-                        if (++stage == kStages) stage = 0, phase ^= 1u;
-                    }
-                }
-            }
-        }
+        if (elect_one()) produce<BN, RB, kScheme>(p, smem, full_bar, empty_bar);
         return;
     }
 
-    // ===================== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile =====================
+    // ===================== consumers: warpgroup wg owns rows [64 wg, 64 wg + 64) of every tile =====================
     const int wg = warp >> 2;
     const int wq = warp & 3;
-    const int k_steps = p.k_steps > 0 ? p.k_steps : RB / 32;  // 16-wide k-steps per stage (scheme 0)
+    const int num_tiles = p.batches * p.tiles_m_per_batch * p.n_tiles;
     int stage = 0;
     uint32_t phase = 0;
-    float acc[kNR];
+    float acc[1][BN / 2];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int n_tile = tile % p.n_tiles;
         const int mt = tile / p.n_tiles;
         const int batch = mt / p.tiles_m_per_batch;
         const int row0 = (mt - batch * p.tiles_m_per_batch) * kBlockM;
-#pragma unroll
-        for (int i = 0; i < kNR; ++i) acc[i] = 0.f;
-
-        // Stage s is released once the wgmma group reading it has retired; one group stays in flight so that the
-        // tensor pipe is fed while this warpgroup waits for the next stage.
-        int pending = -1;
-        bool first = true;
-        // The pass loop is unrolled so that every wgmma sits in straight-line code: with a runtime pass index the
-        // rescale below is a branch ptxas treats as divergent, and it then serialises every wgmma of the kernel.
-#pragma unroll
-        for (int pass = 0; pass < kPasses; ++pass) {
-            if (kScheme == 1 && pass == 1) {
-                // the corrections carry 2^kQ8Scale: scale them back before the main product accumulates (exact)
-                wgmma_wait<0>();
-                if (pending >= 0) {
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&empty_bar[pending]);
-                    pending = -1;
-                }
-                const float s = 1.0f / (float)(1 << kQ8Scale);
-#pragma unroll
-                for (int i = 0; i < kNR; ++i) acc[i] *= s;
-                wgmma_fence();
-            }
-            for (int kb = 0; kb < p.num_k_blocks; ++kb) {
-                mbar_wait(&full_bar[stage], phase);
-                const uint32_t st = smem_u32(smem + stage * Cfg::kStageBytes);
-                const uint32_t a0 = st + wg * 64 * RB, a1 = a0 + Cfg::kAPlane;
-                const uint32_t b0 = st + 2 * Cfg::kAPlane, b1 = b0 + Cfg::kBPlane;
-                const uint64_t da0 = make_wgmma_desc<RB>(a0), da1 = make_wgmma_desc<RB>(a1);
-                const uint64_t db0 = make_wgmma_desc<RB>(b0), db1 = make_wgmma_desc<RB>(b1);
-                wgmma_fence();
-                if constexpr (kScheme == 0) {
-#pragma unroll
-                    for (int k = 0; k < RB / 32; ++k) {
-                        if (k < k_steps) {
-                            // advance 16 bf16 (= 32 bytes) along K inside the swizzle atom: +2 in (addr >> 4) units
-                            const uint64_t ko = (uint64_t)(k * 2);
-                            Wgmma<BN, 0>::ss(acc, da1 + ko, db0 + ko, first ? 0u : 1u);
-                            Wgmma<BN, 0>::ss(acc, da0 + ko, db1 + ko, 1u);
-                            Wgmma<BN, 0>::ss(acc, da0 + ko, db0 + ko, 1u);
-                            first = false;
-                        }
-                    }
-                } else if (pass == 0) {  // (kScheme == 1 from here on, RB == 64)
-                    // A_l8 x W_h8 and A_h8 x W_l8, K = 32 per MMA (32 bytes), two k-steps per 64-byte row
-#pragma unroll
-                    for (int k = 0; k < 2; ++k) {
-                        const uint64_t ko = (uint64_t)(k * 2);
-                        Wgmma<BN, 2>::ss(acc, da0 + ko, db0 + ko, first ? 0u : 1u);
-                        Wgmma<BN, 2>::ss(acc, da1 + ko, db1 + ko, 1u);
-                        first = false;
-                    }
-                } else {
-                    // A16[k..k+64) x W16[k..k+64), K = 16 per MMA: one box of 128-byte rows each, spanning both
-                    // 64-byte planes of the stage (the warpgroup's 64 A rows start 64 * 128 bytes apart)
-                    const uint64_t da = make_wgmma_desc<128>(st + wg * 64 * 128), db = make_wgmma_desc<128>(b0);
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const uint64_t ko = (uint64_t)(k * 2);
-                        Wgmma<BN, 1>::ss(acc, da + ko, db + ko, 1u);
-                    }
-                }
-                wgmma_commit();
-                wgmma_wait<1>();
-                if (pending >= 0) {
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&empty_bar[pending]);
-                }
-                pending = stage;
-                if (++stage == kStages) stage = 0, phase ^= 1u;
-            }
-        }
-        wgmma_wait<0>();
-        if (pending >= 0) {
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty_bar[pending]);
-        }
-
-        // ===================== epilogue: thread holds rows r, r + 8 and columns 8j + 2(lane%4) + {0,1} ==========
-        const int col0 = n_tile * BN + 2 * (lane & 3);
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            const int row = row0 + wg * 64 + wq * 16 + (lane >> 2) + 8 * i;
-            if (row >= p.rows_per_batch) continue;
-            const size_t m = (size_t)batch * p.out_rows_per_batch + row;
-            const bool masked = (p.row_mask != nullptr) && (p.row_mask[m] != 0);
-#pragma unroll
-            for (int j = 0; j < BN / 8; ++j) epilogue_pair(p, m, col0 + 8 * j, masked, acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-        }
+        mma_tile<BN, RB, kScheme, 1>(p, smem, full_bar, empty_bar, wg, lane, stage, phase, acc);
+        epilogue_tile<BN, kEpi, 1>(p, acc, batch, row0 + wg * 64 + wq * 16 + (lane >> 2), n_tile * BN + 2 * (lane & 3));
     }
 }
 
-template <int BN, int RB, int kScheme>
-static cudaError_t launch_impl(const GemmParams& p, int sm_count, cudaStream_t stream) {
+template <int RB, int kScheme, int kEpi>
+__global__ void __launch_bounds__(kPingPongThreads, 1) gemm_sm90_pingpong_kernel(const __grid_constant__ GemmParams p) {
+    constexpr int BN = 128;
     using Cfg = GemmCfg<BN, RB>;
-    auto kernel = gemm_sm90_kernel<BN, RB, kScheme>;
-    static PerDeviceOnce attr_once;
+    constexpr int kStages = Cfg::kStages;
+    constexpr int kPasses = kScheme == 0 ? 1 : 2;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * Cfg::kStageBytes);  // [kStages]
+    uint64_t* empty_bar = full_bar + kStages;                                              // [kStages]
+    uint64_t* order_bar = empty_bar + kStages;  // [2]: order_bar[wg] = the other warpgroup finished its mainloop
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+
+    if (warp == 8 && elect_one()) {
+        tma_prefetch_desc(&p.a_hi);
+        tma_prefetch_desc(&p.b_hi);
+        if (kScheme == 0) {
+            tma_prefetch_desc(&p.a_lo);
+            tma_prefetch_desc(&p.b_lo);
+        }
+        for (int s = 0; s < kStages; ++s) {
+            mbar_init(&full_bar[s], 1);
+            mbar_init(&empty_bar[s], 4);  // each stage is consumed by ONE warpgroup: one arrive per warp
+        }
+        mbar_init(&order_bar[0], 4);
+        mbar_init(&order_bar[1], 4);
+        fence_mbar_init();
+    }
+    __syncthreads();
+    pdl_wait();
+    pdl_launch_dependents();
+
+    if (warp >= 8) {
+        setmaxnreg_dec40();
+        if (warp == 8 && elect_one()) produce<BN, RB, kScheme>(p, smem, full_bar, empty_bar);
+        return;
+    }
+    setmaxnreg_inc232();
+
+    // ===================== consumers: warpgroup wg takes this CTA's tiles of ordinal wg, wg + 2, ... =============
+    // The mainloops run in tile order, one warpgroup at a time: tile ordinal `ord` starts its MMAs once the other
+    // warpgroup has finished those of ordinal ord - 1, and its epilogue then overlaps the other's MMAs of ord + 1.
+    // The order also keeps every full-barrier wait at most one phase ahead of the producer: a warpgroup that waited
+    // on a stage two ring laps ahead would see the parity of the earlier phase and read a stage not yet loaded.
+    const int wg = warp >> 2;
+    const int wq = warp & 3;
+    const int num_tiles = p.batches * p.tiles_m_per_batch * p.n_tiles;
+    const int stages_per_tile = kPasses * p.num_k_blocks;
+    float acc[2][BN / 2];
+    int j = 0;  // tiles this warpgroup has done
+    for (int tile = blockIdx.x + wg * gridDim.x, ord = wg; tile < num_tiles; tile += 2 * gridDim.x, ord += 2, ++j) {
+        // the producer fills the ring in tile order: tile ordinal `ord` starts at ring position ord * stages_per_tile
+        const int g = ord * stages_per_tile;
+        int stage = g % kStages;
+        uint32_t phase = (uint32_t)(g / kStages) & 1u;
+        const int n_tile = tile % p.n_tiles;
+        const int mt = tile / p.n_tiles;
+        const int batch = mt / p.tiles_m_per_batch;
+        const int row0 = (mt - batch * p.tiles_m_per_batch) * kBlockM;
+        if (ord > 0) mbar_wait(&order_bar[wg], (uint32_t)(j - (wg == 0 ? 1 : 0)) & 1u);
+        mma_tile<BN, RB, kScheme, 2>(p, smem, full_bar, empty_bar, 0, lane, stage, phase, acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&order_bar[wg ^ 1]);
+        epilogue_tile<BN, kEpi, 2>(p, acc, batch, row0 + wq * 16 + (lane >> 2), n_tile * BN + 2 * (lane & 3));
+    }
+}
+
+template <typename Kernel>
+static cudaError_t launch_persistent(Kernel kernel, PerDeviceOnce& attr_once, int threads, int smem_bytes,
+                                     const GemmParams& p, int sm_count, cudaStream_t stream) {
     bool& attr_set = attr_once.current();
     if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes);
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
         if (e != cudaSuccess) return e;
         attr_set = true;
     }
     const int num_tiles = p.batches * p.tiles_m_per_batch * p.n_tiles;
     if (num_tiles <= 0) return cudaSuccess;
     const int grid = num_tiles < sm_count ? num_tiles : sm_count;
-    return launch_pdl(kernel, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, stream, p);
+    return launch_pdl(kernel, dim3(grid), dim3(threads), smem_bytes, stream, p);
+}
+
+template <int BN, int RB, int kScheme, int kEpi>
+static cudaError_t launch_impl(const GemmParams& p, int sm_count, cudaStream_t stream) {
+    static PerDeviceOnce attr_once;
+    if constexpr (BN == 128)
+        return launch_persistent(gemm_sm90_pingpong_kernel<RB, kScheme, kEpi>, attr_once, kPingPongThreads,
+                                 GemmCfg<BN, RB>::kSmemBytes, p, sm_count, stream);
+    else
+        return launch_persistent(gemm_sm90_kernel<BN, RB, kScheme, kEpi>, attr_once, kThreads,
+                                 GemmCfg<BN, RB>::kSmemBytes, p, sm_count, stream);
+}
+
+// QKV scatter and the fp32 + planes output run at the widths of the encoder's linears only (>= 128 columns)
+template <int BN, int RB, int kScheme>
+static cudaError_t launch_epi(const GemmParams& p, int sm_count, cudaStream_t stream) {
+    const bool f32 = p.out_f32 != nullptr, planes = p.out_hi != nullptr;
+    if constexpr (BN >= 128) {
+        if (p.qkv_mode) return launch_impl<BN, RB, kScheme, kEpiQkv>(p, sm_count, stream);
+        if (f32 && planes) return launch_impl<BN, RB, kScheme, kEpiBoth>(p, sm_count, stream);
+    }
+    if (p.qkv_mode || (f32 && planes)) return cudaErrorInvalidValue;
+    if (planes) return launch_impl<BN, RB, kScheme, kEpiPlanes>(p, sm_count, stream);
+    if (f32) return launch_impl<BN, RB, kScheme, kEpiF32>(p, sm_count, stream);
+    return cudaErrorInvalidValue;  // no output
 }
 
 template <int BN>
 static cudaError_t launch_n(const GemmParams& p, int sm_count, cudaStream_t stream) {
     if (p.scheme != 0) {
-        if constexpr (BN == 256 || BN == 192 || BN == 128) return launch_impl<BN, 64, 1>(p, sm_count, stream);
+        if constexpr (BN == 256 || BN == 192 || BN == 128) return launch_epi<BN, 64, 1>(p, sm_count, stream);
         return cudaErrorInvalidValue;
     }
-    if (p.block_k == 64) return launch_impl<BN, 128, 0>(p, sm_count, stream);
-    return launch_impl<BN, 64, 0>(p, sm_count, stream);
+    if (p.block_k == 64) return launch_epi<BN, 128, 0>(p, sm_count, stream);
+    // 32-wide k-blocks: only the unpaired 192- and 256-column tiles use them (gemm_block_k)
+    if constexpr (BN > 128) return launch_epi<BN, 64, 0>(p, sm_count, stream);
+    return cudaErrorInvalidValue;
 }
 
 cudaError_t launch_gemm_bf16x3(const GemmParams& p, int sm_count, cudaStream_t stream) {

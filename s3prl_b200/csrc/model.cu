@@ -720,14 +720,16 @@ static int use_cta_pairs(int umma_n) { return ((umma_n == 256 || umma_n == 128) 
 static int g_force_pair_un = 0;  // s3b_gemm_bench: force the tile width (tile-shape sweeps)
 
 // Tile width for a flat [M][N] linear layer. Both widths give bit-identical results; the rule comes from
-// tools/gemm_shapes.py on an H100 80GB HBM3 (same ranking at 400 W and 700 W power limits), at the encoder shapes of
-// hubert_base (K = 768, 3072) and wav2vec2_large (K = 1024, 4096), M = 7984..15984:
-//  - bf16x3, and f16q8 with K <= 1024: 128 columns, 1.3x-2x faster than 256 at every measured shape.
-//  - f16q8 with K >= 3072 (fc2): 256 columns are 3-15% faster when their last round of tiles fills at least half of
-//    the SMs (or none is partial); otherwise that round runs half empty and 128 columns are 19% faster (hubert_base
+// tools/gemm_shapes.py on an H100 80GB HBM3 at 400 W, at the encoder shapes of hubert_base (K = 768, 3072) and
+// wav2vec2_large (K = 1024, 4096), M = 7984..15984, with the ping-pong kernel at 128 columns:
+//  - bf16x3: 128 columns, 1.4x-2.2x faster than 256 at every measured shape.
+//  - f16q8 with K <= 1024: 128 columns, 1.04x-1.5x faster than 256, except wav2vec2_large's fc1 (N = 4096), where
+//    256 is 3-6% faster; hubert_base's fc1 (N = 3072) prefers 128 by 4%, so N does not make a clean cut.
+//  - f16q8 with K >= 3072 (fc2): 256 columns are 21-28% faster when their last round of tiles fills at least half of
+//    the SMs (or none is partial); otherwise that round runs half empty and 128 columns are 17% faster (hubert_base
 //    fc2 at M = 7984: 189 tiles of 256 on 132 SMs). The K >= 2048 cut lies between measured Ks (1024 and 3072).
 // The epilogue kind (epi_kind) does not enter the rule: at K <= 1024 the GELU (fc1) and fp32 epilogues ranked the two
-// widths the same way.
+// widths the same way, but for the one shape above.
 static int pick_pair_umma_n(int64_t M, int N, int K, int epi_kind, int sm_count, int scheme = 0) {
     (void)epi_kind;
     if (g_force_pair_un != 0 && N % g_force_pair_un == 0) return g_force_pair_un;
@@ -801,19 +803,23 @@ static int conv_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int 
     memset(&p, 0, sizeof(p));
     const int C = kConvDim, K = kw * C;
     const uint64_t rows = (uint64_t)((Lin + 1) / 2);
-    const int pair = use_cta_pairs(256);
+    // Tile width: tools/gemm_shapes.py times the linear with conv i's M, N = 512 and K as a proxy (H100 80GB HBM3,
+    // 400 W, both models' conv stacks): f16q8 256 columns are 4-20% faster than 128 at every conv, bf16x3 128 columns
+    // 25-40% faster than 256.
+    const int un = scheme != 0 ? 256 : 128;
+    const int pair = use_cta_pairs(un);
     if (scheme != 0) {
         if (!pair) return fail("f16q8 GEMM needs CTA pairs");
         TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
         TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
         TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, C, 1, K, (uint64_t)C * K, 64, 128));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, C, 1, K, (uint64_t)C * K, 64, 128));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, C, 1, K, (uint64_t)C * K, 64, 128));
+        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, C, 1, K, (uint64_t)C * K, 64, un / 2));
+        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, C, 1, K, (uint64_t)C * K, 64, un / 2));
+        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, C, 1, K, (uint64_t)C * K, 64, un / 2));
         p.scheme = 1, p.two_cta = 1, p.block_k = 64, p.num_k_blocks = K / 64, p.kb_per_row = (2 * C) / 64;
     } else {
-        const int bk = pair ? 64 : gemm_block_k(256);
-        const int bbox = pair ? 128 : 256;
+        const int bk = pair ? 64 : gemm_block_k(un);
+        const int bbox = pair ? un / 2 : un;
         TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, bk, 128));
         TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, bk, 128));
         // weights [512][K], K index = tap*512 + channel, read linearly along K
@@ -822,7 +828,7 @@ static int conv_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int 
         p.two_cta = pair, p.block_k = bk, p.num_k_blocks = K / bk, p.kb_per_row = (2 * C) / bk;
     }
     p.batches = B, p.rows_per_batch = (int)Lout, p.tiles_m_per_batch = (int)((Lout + 127) / 128);
-    p.n_tiles = C / 256, p.umma_n = 256;
+    p.n_tiles = C / un, p.umma_n = un;
     p.a_row_step = 1, p.a_row_off = 0, p.a_k_per_ntile = 0, p.b_n_tiled = 1, p.b_z_per_ntile = 0, p.b_k_linear = 1;
     p.out_rows_per_batch = (int)Lout;
     p.alg_flops = 2.0 * (double)B * Lout * C * K;
