@@ -276,6 +276,15 @@ int s3b_attention_ex(const float* q, const float* k, const float* v, const int32
  * grep_a [heads] (grep_w NULL = gru_rel_pos off: gate 1). gate_out: DEVICE [batch][heads][t] fp32. */
 int s3b_wavlm_gate_f32(const float* x, int32_t batch, int32_t t, int32_t heads, const float* grep_w,
                        const float* grep_b, const float* grep_a, int32_t x_format, float* gate_out, void* stream);
+/* The feature extractor's front end as a forward runs it: ragged DEVICE waveforms (host array of pointers, lengths
+ * lens[b] in [1, max_len]) packed into [batch][max_len] (normalize: per-utterance F.layer_norm over lens[b] samples),
+ * then conv 0 (w [512][1][10], optional bias [512]) with GroupNorm(512, 512) over all L0 = (max_len - 10) / 5 + 1
+ * frames (layer_norm 0; a bias is dropped as the model drops it) or per-frame LayerNorm(512) (layer_norm 1),
+ * gamma / beta [512], GELU, written as operand planes of out_fmt (0 = bf16 hi/lo, 1 = f16q8) and decoded to
+ * out [batch][L0][512]. max_len >= 10. wav_out (optional DEVICE [batch][max_len]): the packed waveform. */
+int s3b_frontend_f32(const float* const* wavs, const int64_t* lens, int32_t batch, int64_t max_len, int32_t normalize,
+                     const float* w, const float* bias, const float* gamma, const float* beta, int32_t layer_norm,
+                     int32_t out_fmt, float* wav_out, float* out, void* stream);
 
 #ifdef __cplusplus
 }

@@ -178,40 +178,45 @@ __device__ __forceinline__ void conv0_quad(const float* xs, int tl, const float 
 //   sum_t z_t[c]^2 = sum_jk w[c][j] w[c][k] R_jk,  R_jk = sum_t x[5t+j] x[5t+k]
 // so the GroupNorm statistics of all 512 channels follow from 10 + 55 numbers per utterance: one cheap pass over
 // the waveform instead of a full conv pass (the previous conv0_stats_kernel took 0.29 ms at C2).
+// The moments are summed in fp64 (a product of two fp32 samples is exact there): var = w^T R w / L0 - mean^2 cancels
+// by the channel's conditioning (sum_j |w_j| |x|)^2 / var(z), large where a filter rejects most of the signal (a
+// high-pass filter on band-limited or DC-offset audio), and fp32 sums lose conditioning^2 * 2^-24 of var there.
 static constexpr int kNMom = kC0K + kC0K * (kC0K + 1) / 2;  // 65
+static constexpr int kMomSplit = 3;                          // threads per moment, each summing every third frame
+static_assert(kMomSplit * kNMom <= 256, "one thread per (moment, frame phase)");
 
 __global__ void __launch_bounds__(256) conv0_moments_kernel(const float* __restrict__ x, long long L, int L0,
-                                                            float* __restrict__ part /*[B][nchunk][65]*/,
+                                                            double* __restrict__ part /*[B][nchunk][65]*/,
                                                             int nchunk) {
     __shared__ __align__(16) float xs[kXTile];
-    __shared__ float red[8][kNMom];
+    __shared__ double red[kMomSplit][kNMom];
     const int b = blockIdx.y, chunk = blockIdx.x;
     const int t0 = chunk * kTCH;
     conv0_load_tile(x + (size_t)b * L, L, (long long)t0 * kC0S, xs);
     __syncthreads();
-    const int t = t0 + threadIdx.x;
-    float xv[kC0K];
-#pragma unroll
-    for (int j = 0; j < kC0K; ++j) xv[j] = (t < L0) ? xs[threadIdx.x * kC0S + j] : 0.0f;
-    float mom[kNMom];
-    int idx = 0;
-#pragma unroll
-    for (int j = 0; j < kC0K; ++j) mom[idx++] = xv[j];
-#pragma unroll
-    for (int j = 0; j < kC0K; ++j)
-#pragma unroll
-        for (int k = j; k < kC0K; ++k) mom[idx++] = xv[j] * xv[k];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-#pragma unroll
-    for (int i = 0; i < kNMom; ++i) {
-        const float v = warp_sum(mom[i]);
-        if (lane == 0) red[warp][i] = v;
+    const int nt = min(kTCH, L0 - t0);  // frames of this chunk inside [0, L0)
+    if (threadIdx.x < kMomSplit * kNMom) {
+        const int i = threadIdx.x % kNMom, phase = threadIdx.x / kNMom;
+        // moment i: m_j (i = j < 10), then R_jk for j <= k in row order (the order conv0_finalize_kernel reads)
+        int j = i, k = -1;
+        if (i >= kC0K) {
+            int r = i - kC0K;
+            for (j = 0; r >= kC0K - j; ++j) r -= kC0K - j;
+            k = j + r;
+        }
+        const int kk = k < 0 ? j : k;
+        double acc = 0.0;
+        for (int t = phase; t < nt; t += kMomSplit) {
+            const double a = (double)xs[t * kC0S + j];
+            acc = fma(a, k < 0 ? 1.0 : (double)xs[t * kC0S + kk], acc);
+        }
+        red[phase][i] = acc;
     }
     __syncthreads();
     if (threadIdx.x < kNMom) {
-        float v = 0.f;
+        double v = 0.0;
 #pragma unroll
-        for (int wv = 0; wv < 8; ++wv) v += red[wv][threadIdx.x];
+        for (int p = 0; p < kMomSplit; ++p) v += red[p][threadIdx.x];
         part[((size_t)b * nchunk + chunk) * kNMom + threadIdx.x] = v;
     }
 }
@@ -219,7 +224,7 @@ __global__ void __launch_bounds__(256) conv0_moments_kernel(const float* __restr
 // finalize: GroupNorm(512 groups == per channel) statistics over ALL L0 frames of the padded batch
 // (Fp32GroupNorm, eps 1e-5, biased variance; wav2vec2_model.py:1841-1853, 2898-2904), in double:
 //   y = (z - mean) * rstd * gamma + beta  =  z * scale + shift
-__global__ void __launch_bounds__(kC0) conv0_finalize_kernel(const float* __restrict__ part, int nchunk, int L0,
+__global__ void __launch_bounds__(kC0) conv0_finalize_kernel(const double* __restrict__ part, int nchunk, int L0,
                                                              const float* __restrict__ w,
                                                              const float* __restrict__ gamma,
                                                              const float* __restrict__ beta,
@@ -228,7 +233,7 @@ __global__ void __launch_bounds__(kC0) conv0_finalize_kernel(const float* __rest
     const int b = blockIdx.x, c = threadIdx.x;
     if (c < kNMom) {
         double acc = 0.0;
-        for (int k = 0; k < nchunk; ++k) acc += (double)part[((size_t)b * nchunk + k) * kNMom + c];
+        for (int k = 0; k < nchunk; ++k) acc += part[((size_t)b * nchunk + k) * kNMom + c];
         mom[c] = acc;
     }
     __syncthreads();
@@ -356,7 +361,7 @@ __global__ void __launch_bounds__(256) conv0_apply_ln_kernel(const float* __rest
 }
 
 cudaError_t launch_conv0_groupnorm(const float* x, int B, long long L, int L0, const float* w, const float* gamma,
-                                   const float* beta, float* ws_part /*[B][nchunk][65]*/,
+                                   const float* beta, double* ws_part /*[B][nchunk][65]*/,
                                    float* ws_scale_shift /*[2][B][512]*/, const OutPlanes& op, cudaStream_t s) {
     const int nchunk = (L0 + kTCH - 1) / kTCH;
     float* scale = ws_scale_shift;
@@ -376,6 +381,6 @@ cudaError_t launch_conv0_layernorm(const float* x, int B, long long L, int L0, c
     return cudaGetLastError();
 }
 
-size_t conv0_ws_part_floats(int B, int L0) { return (size_t)B * ((L0 + kTCH - 1) / kTCH) * kNMom; }
+size_t conv0_ws_part_bytes(int B, int L0) { return (size_t)B * ((L0 + kTCH - 1) / kTCH) * kNMom * sizeof(double); }
 
 }  // namespace s3b

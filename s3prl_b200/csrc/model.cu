@@ -892,12 +892,14 @@ static int posconv4_params(GemmParams& p, const s3b_config& c, const __nv_bfloat
 // ------------------------------------------------------------------------------------------------
 // launch accounting / profiling
 // ------------------------------------------------------------------------------------------------
+// (m == nullptr: a building-block entry point, nothing to account)
 static inline void prof_begin(s3b_model* m, cudaStream_t st) {
-    if (!m->prof.on) return;
+    if (m == nullptr || !m->prof.on) return;
     m->prof.pending = m->prof.get();
     cudaEventRecord(m->prof.pending, st);
 }
 static inline void prof_end(s3b_model* m, cudaStream_t st, int cat, int nkernels, double flops) {
+    if (m == nullptr) return;
     m->launches_total += nkernels;
     if (!m->prof.on) return;
     cudaEvent_t b = m->prof.get();
@@ -917,6 +919,26 @@ static inline void prof_end(s3b_model* m, cudaStream_t st, int cat, int nkernels
 #define KNORM(expr) KLAUNCH(CAT_NORM, 1, 0.0, expr)
 #define KCONV0(nk, expr) KLAUNCH(CAT_CONV0, nk, conv0_flops, expr)
 #define KMISC(expr) KLAUNCH(CAT_MISC, 1, 0.0, expr)
+
+// The feature extractor's front end (Fwd::stage(0), s3b_frontend_f32): B ragged waveforms packed into
+// wav_pad [B][Lmax] (+ per-utterance normalisation), then conv 0 (w [512][10]) with GroupNorm(512, 512) over all
+// L0 frames (layer_norm 0) or per-frame LayerNorm(512) (layer_norm 1), GELU, written to operand planes `op`.
+// Workspaces: wav_stats [B][2], c0_part conv0_ws_part_bytes(B, L0), c0_ss [2][B][512] (GroupNorm only).
+static int launch_frontend(s3b_model* m, cudaStream_t st, const float* const* d_wavs, const long long* d_lens, int B,
+                           long long Lmax, int L0, int normalize, const float* w, const float* bias, const float* gamma,
+                           const float* beta, int layer_norm, float* wav_pad, float* wav_stats, double* c0_part,
+                           float* c0_ss, const OutPlanes& op) {
+    const double conv0_flops = 2.0 * kConvK[0] * kConvDim * (double)B * L0;
+    KMISC(launch_wav_pack(d_wavs, d_lens, B, Lmax, normalize, wav_stats, wav_pad, st));
+    if (layer_norm) {
+        KCONV0(1, launch_conv0_layernorm(wav_pad, B, Lmax, L0, w, bias, gamma, beta, op, st));
+    } else {
+        // a conv-0 bias (conv_bias with extractor_mode "default") is removed again by the per-channel GroupNorm
+        // mean: it cancels exactly in (z + b) - mean(z + b), so the kernel never adds it
+        KCONV0(3, launch_conv0_groupnorm(wav_pad, B, Lmax, L0, w, gamma, beta, c0_part, c0_ss, op, st));
+    }
+    return 0;
+}
 
 // LayerNorm fused into the producing GEMM (gemm.cuh: ln_*): on unless S3B_FUSE_LN=0 (kept for A/B measurements)
 // S3B_FUSE_LN: 0 = never, 1 = wherever possible, unset = only where the tile's MMAs (K >= 2048: fc2) leave the epilogue
@@ -1091,7 +1113,7 @@ int Fwd::prepare() {
     // ---- workspace ------------------------------------------------------------------------------------------
     S3B_OK(w->wav_pad.ensure((size_t)B * Lmax * 4));
     S3B_OK(w->wav_stats.ensure((size_t)B * 2 * 4));
-    S3B_OK(w->c0_part.ensure(conv0_ws_part_floats(B, (int)L[0]) * 4));
+    S3B_OK(w->c0_part.ensure(conv0_ws_part_bytes(B, (int)L[0])));
     S3B_OK(w->c0_ss.ensure((size_t)2 * B * C * 4));
     for (int i = 0; i < kNumConv - 1; ++i) S3B_OK(w->act[i].ensure((size_t)B * L[i] * C));
     S3B_OK(w->conv_f32.ensure((size_t)B * (c.extractor_layer_norm ? L[1] : L[6]) * C * 4));
@@ -1307,27 +1329,17 @@ int Fwd::stage(int s) {
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, H = c.num_heads, NL = c.num_layers, C = kConvDim;
     const double attn_flops = 4.0 * (double)T * T * D * B;
-    const double conv0_flops = 2.0 * kConvK[0] * C * (double)B * L[0];
 
     if (s == 0) {
         // ---- bookkeeping copy, waveform packing (+ normalisation), conv 0 + norm + GELU -> act[0] ------------------
         const size_t book_bytes = (size_t)(reinterpret_cast<char*>(d_mask) - w->book.as<char>()) + (size_t)M;
         CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host, book_bytes, cudaMemcpyHostToDevice, st));
         if (!capturing) CUDA_OK(cudaEventRecord(w->book_copied, st));  // (graph replay: recorded after the launch)
-        KMISC(launch_wav_pack(d_wavs, d_lens, B, Lmax, c.normalize_wav, w->wav_stats.as<float>(),
-                              w->wav_pad.as<float>(), st));
-        if (c.extractor_layer_norm) {
-            KCONV0(1, launch_conv0_layernorm(w->wav_pad.as<float>(), B, Lmax, (int)L[0], m->conv0_w.as<float>(),
-                                             c.conv_bias ? m->conv0_b.as<float>() : nullptr, m->norm0_g.as<float>(),
-                                             m->norm0_b.as<float>(), w->act[0].planes(m->scheme), st));
-        } else {
-            // a conv-0 bias (conv_bias with extractor_mode "default") is removed again by the per-channel GroupNorm
-            // mean: it cancels exactly in (z + b) - mean(z + b), so the kernel never adds it
-            KCONV0(3, launch_conv0_groupnorm(w->wav_pad.as<float>(), B, Lmax, (int)L[0], m->conv0_w.as<float>(),
-                                             m->norm0_g.as<float>(), m->norm0_b.as<float>(), w->c0_part.as<float>(),
-                                             w->c0_ss.as<float>(), w->act[0].planes(m->scheme), st));
-        }
-        return 0;
+        return launch_frontend(m, st, d_wavs, d_lens, B, Lmax, (int)L[0], c.normalize_wav, m->conv0_w.as<float>(),
+                               c.conv_bias ? m->conv0_b.as<float>() : nullptr, m->norm0_g.as<float>(),
+                               m->norm0_b.as<float>(), c.extractor_layer_norm, w->wav_pad.as<float>(),
+                               w->wav_stats.as<float>(), w->c0_part.as<double>(), w->c0_ss.as<float>(),
+                               w->act[0].planes(m->scheme));
     }
     if (s >= 1 && s <= 6) {
         // ---- conv s as implicit GEMM (+ per-frame LayerNorm + GELU in "layer_norm" mode) ----------------------------
@@ -2289,6 +2301,54 @@ extern "C" int s3b_wavlm_gate_f32(const float* x, int32_t B, int32_t T, int32_t 
     xs.release();
     if (se != cudaSuccess) return fail("gate execution failed: %s", cudaGetErrorString(se));
     return 0;
+}
+
+extern "C" int s3b_frontend_f32(const float* const* wavs, const int64_t* lens, int32_t B, int64_t max_len,
+                                int32_t normalize, const float* w, const float* bias, const float* gamma,
+                                const float* beta, int32_t layer_norm, int32_t out_fmt, float* wav_out, float* out,
+                                void* stream) {
+    // the launches of Fwd::stage(0) (launch_frontend) on workspaces of this call; the conv-0 planes decoded to fp32
+    if (!wavs || !lens || !w || !gamma || !beta || !out) return fail("null argument");
+    if (B < 1) return fail("bad batch %d", B);
+    if (max_len < kConvK[0]) return fail("max_len %lld is below the conv-0 window of %d samples", (long long)max_len,
+                                         kConvK[0]);
+    for (int b = 0; b < B; ++b) {
+        if (wavs[b] == nullptr) return fail("null argument: wavs[%d]", b);
+        if (lens[b] < 1 || lens[b] > max_len)
+            return fail("lens[%d] = %lld not in [1, %lld]", b, (long long)lens[b], (long long)max_len);
+    }
+    if (normalize != 0 && normalize != 1) return fail("normalize must be 0 or 1, not %d", normalize);
+    if (layer_norm != 0 && layer_norm != 1) return fail("layer_norm must be 0 (GroupNorm) or 1 (LayerNorm), not %d", layer_norm);
+    if (out_fmt != 0 && out_fmt != 1) return fail("out_fmt must be 0 (bf16 hi/lo) or 1 (f16q8), not %d", out_fmt);
+    const int64_t L0 = conv_out_len(max_len, 0);
+    if ((int64_t)B * L0 > 2000000000LL) return fail("batch too large for 32-bit tile indexing");
+    cudaStream_t st = (cudaStream_t)stream;
+    DevBuf book, pad, stats, part, ss;
+    SplitBuf os;
+    const int r = [&]() -> int {
+        S3B_OK(book.ensure((size_t)B * (sizeof(void*) + sizeof(long long))));
+        std::vector<long long> hl(lens, lens + B);
+        CUDA_OK(cudaMemcpyAsync(book.p, wavs, (size_t)B * sizeof(void*), cudaMemcpyHostToDevice, st));
+        long long* d_lens = reinterpret_cast<long long*>(book.as<char>() + (size_t)B * sizeof(void*));
+        CUDA_OK(cudaMemcpyAsync(d_lens, hl.data(), (size_t)B * sizeof(long long), cudaMemcpyHostToDevice, st));
+        float* wav_pad = wav_out;
+        if (wav_pad == nullptr) {
+            S3B_OK(pad.ensure((size_t)B * max_len * 4));
+            wav_pad = pad.as<float>();
+        }
+        S3B_OK(stats.ensure((size_t)B * 2 * 4));
+        S3B_OK(part.ensure(conv0_ws_part_bytes(B, (int)L0)));
+        S3B_OK(ss.ensure((size_t)2 * B * kConvDim * 4));
+        S3B_OK(os.ensure((size_t)B * L0 * kConvDim));
+        S3B_OK(launch_frontend(nullptr, st, book.as<const float*>(), d_lens, B, max_len, (int)L0, normalize, w, bias,
+                               gamma, beta, layer_norm, wav_pad, stats.as<float>(), part.as<double>(), ss.as<float>(),
+                               os.planes(out_fmt)));
+        CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), (size_t)B * L0 * kConvDim, out, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+        return 0;
+    }();
+    book.release(), pad.release(), stats.release(), part.release(), ss.release(), os.release();
+    return r;
 }
 
 // ------------------------------------------------------------------------------------------------

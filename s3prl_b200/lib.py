@@ -53,6 +53,7 @@ EXPORTED_SYMBOLS = [
     "s3b_attention_f32",
     "s3b_attention_ex",
     "s3b_wavlm_gate_f32",
+    "s3b_frontend_f32",
     "s3b_fbank",
     "s3b_fbank_num_frames",
     "s3b_trimmed_lengths",
@@ -218,6 +219,8 @@ def load() -> C.CDLL:
     lib.s3b_attention_ex.argtypes = [f32p, f32p, f32p, C.POINTER(i32), i32, i32, i32, C.POINTER(S3BAttentionOpts),
                                      f32p, vp]
     lib.s3b_wavlm_gate_f32.argtypes = [f32p, i32, i32, i32, f32p, f32p, f32p, i32, f32p, vp]
+    lib.s3b_frontend_f32.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i64, i32, f32p, f32p, f32p, f32p, i32, i32,
+                                     f32p, f32p, vp]
     lib.s3b_fbank_num_frames.argtypes = [i64]
     lib.s3b_fbank_num_frames.restype = i64
     lib.s3b_fbank.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, f32p, vp]
