@@ -43,7 +43,12 @@ typedef struct s3b_config {
     int32_t pos_conv_depth;        /* 0 / 1: one weight-normed conv of pos_conv_kernel taps (make_conv_pos); > 1 (data2vec):
                                       that many blocks Conv1d(k) -> LayerNorm(no affine) -> GELU with
                                       k = max(3, pos_conv_kernel / pos_conv_depth) (wav2vec2_model.py:2995-3026) */
-    int32_t reserved[5];
+    /* wav2vec 2.0 Conformer (layer_type "conformer", attn_type "espnet", pos_enc_type "rope";
+     * ConformerEncoder wav2vec2_model.py:3132-3211, ConformerEncoderLayer :441-578). 1 needs family 1; the positional
+     * conv fields are then unused (the encoder has no pos_conv) and rotary attention is implied. */
+    int32_t conformer;            /* 0: transformer layers; 1: Conformer layers */
+    int32_t depthwise_kernel;     /* depthwise_conv_kernel_size of the convolution module: odd, 1..63 (conformer only) */
+    int32_t reserved[3];
 } s3b_config;
 
 /* Library / error ------------------------------------------------------------------------------ */
@@ -102,7 +107,9 @@ int s3b_forward_host(s3b_model* m, const float* const* wavs, const int64_t* lens
  *                     the residual add = layer_results[i][2] of the reference (wav2vec2/expert.py:87-93,
  *                     feature_selection "fairseq_layers_before_residual"); ffn_layer_stride like layer_stride
  *  last_residual    : optional DEVICE [batch][T][embed_dim], layer_norm_first models only: output of the last layer
- *                     before encoder.layer_norm = layer_results[-1][0] ("fairseq_layers", wav2vec2/expert.py:81-86) */
+ *                     before encoder.layer_norm = layer_results[-1][0] ("fairseq_layers", wav2vec2/expert.py:81-86)
+ *  A Conformer model refuses ffn_out and last_residual: its encoder collects no layer_results
+ *  (wav2vec2_model.py:3199-3200), so the reference has no such outputs. */
 typedef struct s3b_forward_opts {
     int32_t struct_size;
     int32_t lanes;
@@ -129,7 +136,8 @@ int s3b_wavlm_buckets(int32_t num_buckets, int32_t max_distance, const int32_t* 
 
 /* Accounting --------------------------------------------------------------------------------------
  * Kernel categories: 0 = GEMM, 1 = attention, 2 = conv-0 (+GroupNorm/LayerNorm+GELU),
- * 3 = LayerNorm kernels, 4 = misc (waveform packing, WavLM gate). With profiling enabled every launch of
+ * 3 = LayerNorm kernels (Conformer: LayerNorm + RoPE included), 4 = misc (waveform packing, WavLM gate, the
+ * Conformer's GLU + depthwise conv). With profiling enabled every launch of
  * s3b_forward is bracketed by CUDA events on the launching stream; s3b_profile_read synchronises the device and
  * returns, per category, accumulated device milliseconds, ALGORITHMIC flops (2*M*N*K of the un-padded
  * contraction; 4*T^2*D per utterance and layer for attention) and kernel launches. Arrays have 5 entries. */
@@ -186,6 +194,7 @@ int s3b_melspec(const float* const* wavs, const int64_t* trimmed_lens, int32_t b
 
 /* Building blocks exposed for parity tests (device pointers, fp32) -------------------------------------- */
 /* out[M][N] = act(A[M][K] * W[N][K]^T + bias[N]) (+ residual[M][N]); K % 64 == 0, N % 16 == 0.
+ * gelu selects act: 0 = none, 1 = GELU (exact erf), 2 = SiLU (x * sigmoid(x), the Conformer's Swish).
  * = s3b_linear_ex with opts NULL: the default operand scheme (S3B_GEMM_SCHEME) where it applies, else bf16x3. */
 int s3b_linear_f32(const float* a, const float* w, const float* bias, const float* residual, int64_t m, int32_t n,
                    int32_t k, int32_t gelu, float* out, void* stream);
@@ -285,6 +294,20 @@ int s3b_wavlm_gate_f32(const float* x, int32_t batch, int32_t t, int32_t heads, 
 int s3b_frontend_f32(const float* const* wavs, const int64_t* lens, int32_t batch, int64_t max_len, int32_t normalize,
                      const float* w, const float* bias, const float* gamma, const float* beta, int32_t layer_norm,
                      int32_t out_fmt, float* wav_out, float* out, void* stream);
+/* The Conformer convolution module between its pointwise convs, as a forward runs it (wav2vec2_model.py:383-389):
+ * x [batch][t][2d] (pointwise_conv1 output, channels-last) -> GLU (x[..., :d] * sigmoid(x[..., d:])) -> depthwise
+ * Conv1d(k, padding k / 2, groups d, no bias; dw_w [d][1][k]) over each utterance's t frames -> BatchNorm1d (eval, eps
+ * 1e-5; bn_gamma, bn_beta, bn_mean, bn_var [d], folded into the taps as the model folds them) -> SiLU, written as
+ * operand planes of out_fmt (0 = bf16 hi/lo, 1 = f16q8) and decoded to out [batch][t][d]. d % 64 == 0, k odd <= 63. */
+int s3b_conformer_conv_f32(const float* x, int32_t batch, int32_t t, int32_t d, int32_t k, const float* dw_w,
+                           const float* bn_gamma, const float* bn_beta, const float* bn_mean, const float* bn_var,
+                           int32_t out_fmt, float* out, void* stream);
+/* The Conformer's attention input (wav2vec2_model.py:541, 255-310): y = LayerNorm_d(x) * gamma + beta (eps 1e-5) and
+ * rope(y) per 64-wide head at frame index row % t, angles fp32(frame) * inv_freq[j] (inv_freq: host [32], NULL =
+ * 1 / 10000^(2j / 64)), both written as operand planes of out_fmt and decoded to out [m][d] and out_rope [m][d].
+ * x: [m][d] (m a multiple of t: rows of utterances of t frames); d in {512, 768, 1024, 1280}. */
+int s3b_layernorm_rope_f32(const float* x, int64_t m, int32_t t, int32_t d, const float* gamma, const float* beta,
+                           const float* inv_freq, int32_t out_fmt, float* out, float* out_rope, void* stream);
 
 #ifdef __cplusplus
 }

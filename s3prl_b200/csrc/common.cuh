@@ -45,6 +45,16 @@ __device__ __forceinline__ float gelu_erf(float x) {
 #endif
 }
 
+// sigmoid(x) = 1 / (1 + e^-x) and SiLU(x) = x * sigmoid(x) (the Conformer's Swish, torch.nn.SiLU); two MUFU ops,
+// relative error a few ulp. x -> -inf: e^-x = inf, rcp = 0, so both go to 0 without a NaN.
+__device__ __forceinline__ float sigmoid_fast(float x) {
+    float e, r;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * -1.4426950408889634f));
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
+    return r;
+}
+__device__ __forceinline__ float silu(float x) { return x * sigmoid_fast(x); }
+
 // hi/lo split of an fp32 value into two bf16 values (round-to-nearest-even both times)
 __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {
     hi = __float2bfloat16_rn(x);

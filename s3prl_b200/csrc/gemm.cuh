@@ -45,7 +45,8 @@ struct GemmParams {
     int b_k_linear;
     int b_z_per_ntile;
 
-    // ---- epilogue: v = acc (+bias[n]) ; gelu? ; (+residual[m][n]) ; row_mask[m] ? 0 -----------------
+    // ---- epilogue: v = acc (+bias[n]) ; act ; (+residual[m][n]) ; row_mask[m] ? 0 -----------------
+    // gelu: 0 = no activation, 1 = GELU (exact erf), 2 = SiLU (x * sigmoid(x), the Conformer's Swish)
     // The launch picks one kernel instantiation per output kind: out_f32, operand planes (out_hi ...), both (widths
     // >= 128 only) or the QKV scatter (widths >= 128 only). A launch with none of them is an error.
     int out_rows_per_batch;  // flat output row m = batch*out_rows_per_batch + row
@@ -66,9 +67,12 @@ struct GemmParams {
 
     // ---- epilogue, QKV scatter mode (qkv_mode != 0): columns [0,D) -> q*scale, [D,2D) -> k, [2D,3D) -> v
     // q,k: [B][H][T][64] split bf16 ; v transposed: [B][H][64][Tp] split bf16. Flat row m = b*T + t.
+    // qkv_col0: the scatter column of GEMM column 0 (the Conformer runs [q | k] with 0 and v alone with 2D; `bias` then
+    // points at the launch's own columns)
     int qkv_mode;
     int T, Tp, H, D;
     float q_scale;
+    int qkv_col0;
     __nv_bfloat16 *q_hi, *q_lo, *k_hi, *k_lo, *vt_hi, *vt_lo;
 
     // ---- optional fused LayerNorm over the whole output row (CTA-pair kernel, N == ldo == 128 * ln_v4) ------------

@@ -46,7 +46,7 @@ struct GemmCfg {
 };
 
 // Epilogue kinds, one kernel instantiation each (chosen per launch in launch_gemm_bf16x3). Every non-QKV kind computes
-//   v = acc (+bias) ; gelu? ; out_pre = v? ; (+residual) ; row_mask ? 0
+//   v = acc (+bias) ; GELU or SiLU? ; out_pre = v? ; (+residual) ; row_mask ? 0
 // and stores v as fp32, as operand planes, or both.
 enum EpiKind { kEpiF32 = 1, kEpiPlanes = 2, kEpiBoth = 3, kEpiQkv = 4 };
 
@@ -269,8 +269,9 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float (&acc)[
             base_qk[s] = ((size_t)b * p.H * T + t) * 64;
             base_v[s] = (size_t)b * p.H * 64 * p.Tp + t;
         }
-        int which = col0 / D;
-        int within = col0 - which * D;
+        const int qcol = col0 + p.qkv_col0;
+        int which = qcol / D;
+        int within = qcol - which * D;
 #pragma unroll
         for (int c = 0; c < kJ; c += kCh) {
             float2 bv[kCh];
@@ -318,7 +319,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float (&acc)[
         }
         return;
     } else {
-        const bool gelu = p.gelu != 0, has_res = p.residual != nullptr, has_pre = p.out_pre != nullptr;
+        const int act = p.gelu;
+        const bool has_res = p.residual != nullptr, has_pre = p.out_pre != nullptr;
         const int fmt = p.out_fmt;
         size_t off[kRows];
         bool zero[kRows];
@@ -349,11 +351,16 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float (&acc)[
 #pragma unroll
                     for (int jj = 0; jj < kCh; ++jj) a[4 * (c + jj) + r2] += bv[jj].x, a[4 * (c + jj) + r2 + 1] += bv[jj].y;
                 }
-                if (gelu) {
+                if (act == 1) {
 #pragma unroll
                     for (int jj = 0; jj < kCh; ++jj)
                         a[4 * (c + jj) + r2] = gelu_erf(a[4 * (c + jj) + r2]),
                         a[4 * (c + jj) + r2 + 1] = gelu_erf(a[4 * (c + jj) + r2 + 1]);
+                } else if (act == 2) {
+#pragma unroll
+                    for (int jj = 0; jj < kCh; ++jj)
+                        a[4 * (c + jj) + r2] = silu(a[4 * (c + jj) + r2]),
+                        a[4 * (c + jj) + r2 + 1] = silu(a[4 * (c + jj) + r2 + 1]);
                 }
                 if (has_pre) {
 #pragma unroll

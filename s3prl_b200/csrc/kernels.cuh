@@ -27,6 +27,9 @@ cudaError_t launch_conv0_layernorm(const float* x, int B, long long L, int L0, c
 // Any of out_f32 / (out_hi,out_lo) may be null. x and out_f32 may alias.
 cudaError_t launch_layernorm(const float* x, size_t M, int D, const float* gamma, const float* beta, int gelu,
                              float* out_f32, const OutPlanes& op, cudaStream_t s);
+// Conformer: y = LayerNorm_D(x) -> op, rope(y) -> op_rope; frame t = row % T, cs [>= T][64] = cos | sin of the 32 angles
+cudaError_t launch_layernorm_rope(const float* x, size_t M, int T, int D, const float* gamma, const float* beta,
+                                  const float* cs, const OutPlanes& op, const OutPlanes& op_rope, cudaStream_t s);
 // out[m] = sum_l w[l] * hs[l][m]   (Featurizer._weighted_sum, interfaces.py:217-248; w already softmaxed)
 cudaError_t launch_posconv_combine(const float* z, const float* x, const float* bias, int B, int T, int D, int cpg,
                                    const float* gamma, const float* beta, int do_ln, int mode, float* out_f32,
@@ -36,6 +39,13 @@ cudaError_t launch_weighted_sum(const float* hs, int NL, size_t n_per_layer, con
 // grad_w[l] = sum_m hs[l][m] * gout[m]
 cudaError_t launch_weighted_sum_bwd(const float* hs, int NL, size_t n_per_layer, const float* gout, float* grad_w,
                                     cudaStream_t s);
+
+// ---- conformer.cu --------------------------------------------------------------------------------
+// out = SiLU(depthwise_conv_k(GLU(x)) + bias) per utterance, zero padding outside [0, T); x [B][T][2D] fp32,
+// w [D][k] (BatchNorm folded in), bias [D]; D % 64 == 0, k odd, k <= kDwMaxKernel. out: operand planes [B][T][D].
+static constexpr int kDwMaxKernel = 63;
+cudaError_t launch_depthwise_glu(const float* x, int B, int T, int D, int k, const float* w, const float* bias,
+                                 const OutPlanes& op, cudaStream_t s);
 
 // ---- peer.cu: fused weighted sum + push all-gather over peer memory --------------------------------------------------
 cudaError_t launch_weighted_sum_push(const float* hs, int NL, size_t n_per_layer, size_t layer_stride, const float* w,

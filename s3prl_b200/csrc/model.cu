@@ -7,6 +7,7 @@
 //   TransformerEncoder.extract_features         s3prl/upstream/wav2vec2/wav2vec2_model.py:3054-3121
 //   TransformerSentenceEncoderLayer.forward     s3prl/upstream/wav2vec2/wav2vec2_model.py:3260-3322
 //   WavLM TransformerEncoder / layer            s3prl/upstream/wavlm/WavLM.py:599-645,709-774
+//   ConformerEncoder / ConformerEncoderLayer    s3prl/upstream/wav2vec2/wav2vec2_model.py:3132-3211,441-578 (rope)
 // Data layout in HBM: every activation is token-major / channels-last ([B][L][C]); GEMM operands are kept as
 // two bf16 planes (hi, lo); hidden states are written once, in fp32, straight into the caller's
 // [NL+1][B][T][D] buffer (the reference's forward hooks become plain views of that buffer).
@@ -136,6 +137,11 @@ struct LayerW {
     SplitBuf qkv, out, fc1, fc2;
     DevBuf qkv_b, out_b, fc1_b, fc2_b, ln1_g, ln1_b, ln2_g, ln2_b;
     DevBuf grep_w, grep_b, grep_a;  // WavLM gate
+    // Conformer (finalize_conformer_layer): qkv holds [linear_q; linear_k] ([2D][D]), v linear_v, qkv_b the three
+    // biases; fc1 / fc2 are ffn2.w_1 / w_2 and ffn1_* the first half-step FFN (w_2 and its bias pre-scaled by 0.5);
+    // ln1 = self_attn_layer_norm, ln2 = final_layer_norm; dw_w / dw_b the depthwise taps with BatchNorm folded in
+    SplitBuf v, ffn1_w1, ffn1_w2, pw1, pw2;
+    DevBuf ffn1_b1, ffn1_b2, ffn1_ln_g, ffn1_ln_b, ffn2_ln_g, ffn2_ln_b, conv_ln_g, conv_ln_b, dw_w, dw_b;
 };
 
 // per-category device-time profile (CUDA events around each launch on the launching stream)
@@ -177,6 +183,7 @@ struct Workspace {
     size_t book_valid = 0;  // bytes of the mirror that hold the last call's block
     cudaEvent_t book_copied = nullptr;  // the previous call's H2D copy has been consumed: the mirror may be rewritten
     DevBuf wav_stats, wav_pad, c0_part, c0_ss, conv_f32, tmp_f32, x_f32, x1_f32, gate, pos_z, ln_counters, hs0;
+    DevBuf glu_f32;  // Conformer: pointwise_conv1 output [M][2D]
     SplitBuf act[kNumConv], ln512_s, x_s, xs_s, q_s, k_s, vt_s, ctx_s, x1_s, h_s;
     cudaStream_t stream = nullptr;  // lane stream (lane 1; lane 0 runs on the caller's stream)
     cudaEvent_t done = nullptr;
@@ -210,6 +217,10 @@ struct s3b_model {
     DevBuf rel_table_src;  // WavLM relative_attention_bias.weight [num_buckets][H]
     DevBuf rel_table;      // [H][2*rel_table_T - 1] gathered table (x log2 e), built at finalize for rel_table_T frames
     int rel_table_T = 0;
+    // Conformer rotary embedding: rope_cs [rope_T][64] = cos | sin of fp32(t) * inv_freq[j], j < 32 (build_rope_table)
+    DevBuf rope_cs;
+    int rope_T = 0;
+    std::vector<float> rope_inv_freq;
     std::vector<LayerW> layers;
 
     Workspace ws[2];
@@ -330,6 +341,15 @@ extern "C" int s3b_model_create(const s3b_config* cfg, s3b_model** out) {
         return fail("no_feature_layer_norm with extractor_mode layer_norm is not supported");
     if ((cfg->family == 3) != (cfg->no_feature_layer_norm != 0))
         return fail("the distiller family (3) and no_feature_layer_norm go together");
+    if (cfg->conformer != 0 && cfg->conformer != 1) return fail("conformer must be 0 or 1");
+    if (cfg->conformer) {
+        if (cfg->family != 1) return fail("the Conformer encoder goes with the wav2vec2 family (1)");
+        if (cfg->relative_position || cfg->pred_heads) return fail("the Conformer encoder has no WavLM bias or prediction heads");
+        if (cfg->depthwise_kernel < 1 || cfg->depthwise_kernel > kDwMaxKernel || cfg->depthwise_kernel % 2 == 0)
+            return fail("depthwise_kernel %d: must be odd, 1..%d", cfg->depthwise_kernel, kDwMaxKernel);
+    } else if (cfg->depthwise_kernel != 0) {
+        return fail("depthwise_kernel is a Conformer field (conformer = 0)");
+    }
     s3b_model* m = new s3b_model();
     m->cfg = *cfg;
     m->scheme = default_scheme();
@@ -353,7 +373,7 @@ extern "C" void s3b_model_destroy(s3b_model* m) {
     if (!m) return;
     DevBuf* bufs[] = {&m->conv0_w, &m->conv0_b, &m->norm0_g, &m->norm0_b, &m->ln512_g, &m->ln512_b, &m->proj_b,
                       &m->pos_b, &m->enc_ln_g, &m->enc_ln_b, &m->rel_table_src, &m->rel_table, &m->stage_wav,
-                      &m->stage_out};
+                      &m->stage_out, &m->rope_cs};
     for (DevBuf* b : bufs) b->release();
     for (int i = 0; i < kNumConv; ++i)
         m->conv_w[i].release(), m->conv_b[i].release(), m->conv_ln_g[i].release(), m->conv_ln_b[i].release();
@@ -365,8 +385,11 @@ extern "C" void s3b_model_destroy(s3b_model* m) {
     m->pred1_b.release(), m->pred2_b.release();
     for (LayerW& l : m->layers) {
         l.qkv.release(), l.out.release(), l.fc1.release(), l.fc2.release();
-        DevBuf* lb[] = {&l.qkv_b, &l.out_b, &l.fc1_b, &l.fc2_b, &l.ln1_g, &l.ln1_b, &l.ln2_g, &l.ln2_b,
-                        &l.grep_w, &l.grep_b, &l.grep_a};
+        l.v.release(), l.ffn1_w1.release(), l.ffn1_w2.release(), l.pw1.release(), l.pw2.release();
+        DevBuf* lb[] = {&l.qkv_b,     &l.out_b,     &l.fc1_b,     &l.fc2_b,     &l.ln1_g,     &l.ln1_b,
+                        &l.ln2_g,     &l.ln2_b,     &l.grep_w,    &l.grep_b,    &l.grep_a,    &l.ffn1_b1,
+                        &l.ffn1_b2,   &l.ffn1_ln_g, &l.ffn1_ln_b, &l.ffn2_ln_g, &l.ffn2_ln_b, &l.conv_ln_g,
+                        &l.conv_ln_b, &l.dw_w,      &l.dw_b};
         for (DevBuf* b : lb) b->release();
     }
     for (Workspace& w : m->ws) w.release();
@@ -398,6 +421,120 @@ static void set_rel_bias(AttnParams& ap, const float* table, int Tmax, const flo
     ap.bias_table = table;
     ap.bias_stride = 2 * Tmax - 1, ap.bias_center = Tmax - 1;
     ap.gate = gate;
+}
+
+// Conformer rotary table for frames [0, Tmax): the reference's angle fp32(t) * inv_freq[j] is an fp32 product
+// (RotaryPositionalEmbedding.forward, wav2vec2_model.py:66-70); its cos / sin are taken in double and rounded to fp32.
+// inv_freq: the checkpoint's buffer, else 1 / 10000^(2j / 64) rounded to fp32.
+static std::vector<float> rope_table(const std::vector<float>& inv_freq, int Tmax) {
+    std::vector<float> cs((size_t)Tmax * 64);
+    for (int t = 0; t < Tmax; ++t)
+        for (int j = 0; j < 32; ++j) {
+            const float a = (float)t * inv_freq[j];
+            cs[(size_t)t * 64 + j] = (float)cos((double)a);
+            cs[(size_t)t * 64 + 32 + j] = (float)sin((double)a);
+        }
+    return cs;
+}
+static std::vector<float> default_inv_freq() {
+    std::vector<float> f(32);
+    for (int j = 0; j < 32; ++j) f[j] = (float)(1.0 / pow(10000.0, (2.0 * j) / 64.0));
+    return f;
+}
+// grown (synchronously) like rel_table when a batch has more frames; a forward reads m->rope_cs at launch time
+static int build_rope_table(s3b_model* m, int Tmax) {
+    const std::vector<float> cs = rope_table(m->rope_inv_freq, Tmax);
+    CUDA_OK(cudaDeviceSynchronize());  // the previous table may still be read by enqueued work
+    S3B_OK(upload_f32(m->rope_cs, cs.data(), cs.size()));
+    m->rope_T = Tmax;
+    return 0;
+}
+
+// BatchNorm1d (eval, eps 1e-5) folded into the depthwise conv (wav2vec2_model.py:387-388), in double:
+// w' = w * s, b' = beta - mean * s, s = gamma / sqrt(var + eps). w: [D][k].
+static void fold_depthwise_bn(const float* w, const float* gamma, const float* beta, const float* mean,
+                              const float* var, int D, int k, std::vector<float>& wf, std::vector<float>& bf) {
+    wf.resize((size_t)D * k), bf.resize(D);
+    for (int c = 0; c < D; ++c) {
+        const double s = (double)gamma[c] / sqrt((double)var[c] + 1e-5);
+        for (int j = 0; j < k; ++j) wf[(size_t)c * k + j] = (float)((double)w[(size_t)c * k + j] * s);
+        bf[c] = (float)((double)beta[c] - (double)mean[c] * s);
+    }
+}
+
+// One ConformerEncoderLayer (wav2vec2_model.py:441-578) of a layer_type "conformer", pos_enc_type "rope" checkpoint.
+static int finalize_conformer_layer(s3b_model* m, int l) {
+    const s3b_config& c = m->cfg;
+    const int D = c.embed_dim, F = c.ffn_dim, k = c.depthwise_kernel;
+    LayerW& L = m->layers[l];
+    const std::string p = "encoder.layers." + std::to_string(l) + ".";
+    const HostTensor* t;
+    // x = x + 0.5 * ffn(x): the 0.5 goes into w_2 and its bias (a power of two: exact in fp32 and in both operand
+    // schemes), so that w_2 runs the plain bias + residual epilogue
+    auto ffn = [&](const std::string& f, SplitBuf& w1, DevBuf& b1, SplitBuf& w2, DevBuf& b2, DevBuf& lg, DevBuf& lb) {
+        S3B_OK(upload_vec(m, f + "layer_norm.weight", D, lg));
+        S3B_OK(upload_vec(m, f + "layer_norm.bias", D, lb));
+        S3B_OK(need(m, f + "w_1.weight", {F, D}, &t));
+        S3B_OK(upload_split(w1, t->data.data(), t->numel(), m->scheme));
+        S3B_OK(upload_vec(m, f + "w_1.bias", F, b1));
+        S3B_OK(need(m, f + "w_2.weight", {D, F}, &t));
+        std::vector<float> h(t->data);
+        for (float& v : h) v *= 0.5f;
+        S3B_OK(upload_split(w2, h.data(), h.size(), m->scheme));
+        S3B_OK(need(m, f + "w_2.bias", {D}, &t));
+        h = t->data;
+        for (float& v : h) v *= 0.5f;
+        return upload_f32(b2, h.data(), h.size());
+    };
+    S3B_OK(ffn(p + "ffn1.", L.ffn1_w1, L.ffn1_b1, L.ffn1_w2, L.ffn1_b2, L.ffn1_ln_g, L.ffn1_ln_b));
+    S3B_OK(ffn(p + "ffn2.", L.fc1, L.fc1_b, L.fc2, L.fc2_b, L.ffn2_ln_g, L.ffn2_ln_b));
+    // attention: [q | k] from rope(LN(x)) in one GEMM, v from LN(x) in another; biases [bq | bk | bv]
+    const std::string a = p + "self_attn.";
+    const HostTensor *wq, *wk, *wv, *bq, *bk, *bv;
+    S3B_OK(need(m, a + "linear_q.weight", {D, D}, &wq));
+    S3B_OK(need(m, a + "linear_k.weight", {D, D}, &wk));
+    S3B_OK(need(m, a + "linear_v.weight", {D, D}, &wv));
+    S3B_OK(need(m, a + "linear_q.bias", {D}, &bq));
+    S3B_OK(need(m, a + "linear_k.bias", {D}, &bk));
+    S3B_OK(need(m, a + "linear_v.bias", {D}, &bv));
+    std::vector<float> w((size_t)2 * D * D), b((size_t)3 * D);
+    memcpy(w.data(), wq->data.data(), (size_t)D * D * 4);
+    memcpy(w.data() + (size_t)D * D, wk->data.data(), (size_t)D * D * 4);
+    memcpy(b.data(), bq->data.data(), D * 4), memcpy(b.data() + D, bk->data.data(), D * 4);
+    memcpy(b.data() + 2 * D, bv->data.data(), D * 4);
+    S3B_OK(upload_split(L.qkv, w.data(), w.size(), m->scheme));
+    S3B_OK(upload_split(L.v, wv->data.data(), wv->numel(), m->scheme));
+    S3B_OK(upload_f32(L.qkv_b, b.data(), b.size()));
+    S3B_OK(need(m, a + "linear_out.weight", {D, D}, &t));
+    S3B_OK(upload_split(L.out, t->data.data(), t->numel(), m->scheme));
+    S3B_OK(upload_vec(m, a + "linear_out.bias", D, L.out_b));
+    if ((t = find(m, a + "rotary_emb.inv_freq")) != nullptr) {
+        if (t->numel() != 32) return fail("'%srotary_emb.inv_freq' has %zu entries, expected 32", a.c_str(), t->numel());
+        if (l == 0) m->rope_inv_freq = t->data;
+        else if (t->data != m->rope_inv_freq) return fail("layer %d's rotary inv_freq differs from layer 0's", l);
+    }
+    S3B_OK(upload_vec(m, p + "self_attn_layer_norm.weight", D, L.ln1_g));
+    S3B_OK(upload_vec(m, p + "self_attn_layer_norm.bias", D, L.ln1_b));
+    S3B_OK(upload_vec(m, p + "final_layer_norm.weight", D, L.ln2_g));
+    S3B_OK(upload_vec(m, p + "final_layer_norm.bias", D, L.ln2_b));
+    // convolution module
+    const std::string cm = p + "conv_module.";
+    S3B_OK(upload_vec(m, cm + "layer_norm.weight", D, L.conv_ln_g));
+    S3B_OK(upload_vec(m, cm + "layer_norm.bias", D, L.conv_ln_b));
+    S3B_OK(need(m, cm + "pointwise_conv1.weight", {2 * D, D, 1}, &t));
+    S3B_OK(upload_split(L.pw1, t->data.data(), t->numel(), m->scheme));
+    S3B_OK(need(m, cm + "pointwise_conv2.weight", {D, D, 1}, &t));
+    S3B_OK(upload_split(L.pw2, t->data.data(), t->numel(), m->scheme));
+    const HostTensor *dw, *g, *be, *mu, *var;
+    S3B_OK(need(m, cm + "depthwise_conv.weight", {D, 1, k}, &dw));
+    S3B_OK(need(m, cm + "batch_norm.weight", {D}, &g));
+    S3B_OK(need(m, cm + "batch_norm.bias", {D}, &be));
+    S3B_OK(need(m, cm + "batch_norm.running_mean", {D}, &mu));
+    S3B_OK(need(m, cm + "batch_norm.running_var", {D}, &var));
+    std::vector<float> wf, bf;
+    fold_depthwise_bn(dw->data.data(), g->data.data(), be->data.data(), mu->data.data(), var->data.data(), D, k, wf, bf);
+    S3B_OK(upload_f32(L.dw_w, wf.data(), wf.size()));
+    return upload_f32(L.dw_b, bf.data(), bf.size());
 }
 
 // ---- weight relayouts shared by s3b_model_finalize and the building-block entry points ----------------------------
@@ -490,7 +627,9 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
     S3B_OK(upload_vec(m, "post_extract_proj.bias", D, m->proj_b));
     // ---- data2vec pos_conv: pos_conv_depth plain Conv1d(k, padding k/2, groups) blocks (make_conv_block,
     //      wav2vec2_model.py:2995-3026). Four taps per k-block like pos_w4 below (posconv4_weight_layout)
-    if (c.pos_conv_depth > 1) {
+    if (c.conformer) {
+        // ConformerEncoder.extract_features never calls pos_conv (wav2vec2_model.py:3171-3211): its weights are unused
+    } else if (c.pos_conv_depth > 1) {
         if (!pairs_enabled()) return fail("pos_conv_depth > 1 runs on the CTA-pair GEMM only (S3B_GEMM_PAIR=0 is set)");
         const int G = c.pos_conv_groups, cpg = D / G, Kp = pos_taps(c);
         m->posd_w4.resize(c.pos_conv_depth);
@@ -533,7 +672,12 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
     S3B_OK(upload_vec(m, "encoder.layer_norm.bias", D, m->enc_ln_b));
     // ---- transformer layers ------------------------------------------------------------------------
     m->layers.resize(c.num_layers);
-    for (int l = 0; l < c.num_layers; ++l) {
+    if (c.conformer) {
+        m->rope_inv_freq = default_inv_freq();
+        for (int l = 0; l < c.num_layers; ++l) S3B_OK(finalize_conformer_layer(m, l));
+        S3B_OK(build_rope_table(m, 4096));  // utterances up to 82 s; rebuilt (synchronously) for longer batches
+    }
+    for (int l = 0; l < c.num_layers && !c.conformer; ++l) {
         LayerW& L = m->layers[l];
         const std::string p = "encoder.layers." + std::to_string(l) + ".";
         const HostTensor *wq, *wk, *wv, *bq, *bk, *bv;
@@ -692,14 +836,15 @@ static void set_epi(GemmParams& p, const Epi& e, int ldo) {
 static const float kQScale = 0.125f * 1.4426950408889634f;
 
 // QKV epilogue of a [B*T][3D] linear: bias, then q (scaled), k as [B][H][T][64] and v transposed as [B][H][64][Tp]
-// (Tp = T rounded up to 8), all as bf16 hi/lo planes
+// (Tp = T rounded up to 8), all as bf16 hi/lo planes. col0: the QKV column of the launch's first column (a launch
+// covering only [k | v] or v), `bias` then starts at that column.
 static void set_qkv_epi(GemmParams& p, const float* bias, int T, int H, const SplitBuf& q, const SplitBuf& k,
-                        const SplitBuf& vt) {
+                        const SplitBuf& vt, int col0 = 0) {
     const int D = H * 64;
     Epi e;
     e.bias = bias;
     set_epi(p, e, 3 * D);
-    p.qkv_mode = 1, p.T = T, p.Tp = (T + 7) & ~7, p.H = H, p.D = D, p.q_scale = kQScale;
+    p.qkv_mode = 1, p.T = T, p.Tp = (T + 7) & ~7, p.H = H, p.D = D, p.q_scale = kQScale, p.qkv_col0 = col0;
     p.q_hi = q.h(), p.q_lo = q.l(), p.k_hi = k.h(), p.k_lo = k.l();
     p.vt_hi = vt.h(), p.vt_lo = vt.l();
 }
@@ -971,6 +1116,7 @@ static void set_ln(GemmParams& p, const float* gamma, const float* beta, int gel
 struct LayerPlan {
     GemmParams qkv, out, fc1, fc2;
     AttnParams attn;
+    GemmParams v, ffn1_a, ffn1_b, pw1, pw2;  // Conformer (qkv = [q | k], fc1 / fc2 = ffn2)
 };
 struct Plan {
     int B = 0;
@@ -987,7 +1133,7 @@ struct Plan {
 
 void Workspace::release() {
     DevBuf* bufs[] = {&book, &wav_stats, &wav_pad, &c0_part, &c0_ss, &conv_f32, &tmp_f32, &x_f32, &x1_f32, &gate, &pos_z,
-                      &ln_counters, &hs0};
+                      &ln_counters, &hs0, &glu_f32};
     for (DevBuf* b : bufs) b->release();
     for (int i = 0; i < kNumConv; ++i) act[i].release();
     SplitBuf* sb[] = {&ln512_s, &x_s, &xs_s, &q_s, &k_s, &vt_s, &ctx_s, &x1_s, &h_s};
@@ -1037,17 +1183,24 @@ struct Fwd {
     int fuse_ln = 0;  // fuse_ln_mode()
     unsigned int* cnt[2] = {nullptr, nullptr};  // two alternating row-block counter arrays of the fused LayerNorm
 
+    static constexpr int kConformerStages = 10;  // stages per Conformer layer (conformer_stage)
     int num_stages() const {
+        if (m->cfg.conformer) return 9 + kConformerStages * m->cfg.num_layers;
         return 9 + 5 * m->cfg.num_layers + (m->cfg.pred_heads > 0 ? 1 + m->cfg.pred_heads : 0);
     }
     bool distil() const { return m->cfg.family == 3; }
     // Output slot i of the caller's buffer. Hidden state l (the input of layer l / the encoder output) lives in slot l —
     // except for the distiller, whose slot 0 is feat_final and whose layer-0 input is not exposed (internal scratch).
     float* slot(int i) const { return hidden + (size_t)i * layer_stride; }
-    float* proj_out() const { return distil() ? slot(0) : w->x_f32.as<float>(); }
+    // post_extract_proj output; a pre-LN Conformer's hidden state 0 is that output itself (no pos_conv)
+    float* proj_out() const {
+        return (distil() || (m->cfg.conformer && m->cfg.layer_norm_first)) ? slot(0) : w->x_f32.as<float>();
+    }
     int prepare();
     int build_plan(Plan& pl);
+    int build_conformer_layer(LayerPlan& lp, int l);
     int stage(int s);
+    int conformer_stage(int l, int sub);
     float* hs(int l) const { return (distil() && l == 0) ? w->hs0.as<float>() : slot(l); }
 };
 
@@ -1068,6 +1221,7 @@ int Fwd::prepare() {
     if (layer_stride == 0) layer_stride = (size_t)M * D;
     if (ffn_out != nullptr && ffn_stride == 0) ffn_stride = (size_t)M * D;
     if (c.relative_position && T > m->rel_table_T) S3B_OK(build_rel_table(m, 2 * T));
+    if (c.conformer && T > m->rope_T) S3B_OK(build_rope_table(m, 2 * T));
 
     // ---- bookkeeping block: pinned host mirror -> one async copy ---------------------------------------------
     const size_t off_lens = (size_t)B * sizeof(void*);
@@ -1129,7 +1283,8 @@ int Fwd::prepare() {
     S3B_OK(w->k_s.ensure((size_t)M * D));
     S3B_OK(w->vt_s.ensure((size_t)B * H * 64 * Tp));
     S3B_OK(w->h_s.ensure((size_t)M * F));
-    if (posconv4_ok(c)) S3B_OK(w->pos_z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
+    if (c.conformer) S3B_OK(w->glu_f32.ensure((size_t)M * 2 * D * sizeof(float)));
+    else if (posconv4_ok(c)) S3B_OK(w->pos_z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
     if (c.relative_position) S3B_OK(w->gate.ensure((size_t)B * H * T * 4));
     if (c.family == 3) S3B_OK(w->hs0.ensure((size_t)M * D * 4));
     fuse_ln = fuse_ln_mode();
@@ -1169,6 +1324,91 @@ int Fwd::prepare() {
     return 0;
 }
 
+// the attention kernel's view of a lane's q / k / v^T planes (QKV scatter epilogue) and its context output
+static int attn_params(AttnParams& ap, const Workspace* w, int B, int T, int H, const int* d_kv, int scheme) {
+    const uint64_t BH = (uint64_t)B * H;
+    const int Tp = (T + 7) & ~7;
+    memset(&ap, 0, sizeof(ap));
+    TMAP_OK(encode_tmap_bf16_3d(&ap.q_hi, w->q_s.h(), 64, T, BH, 64, (uint64_t)T * 64, 64, 128));
+    TMAP_OK(encode_tmap_bf16_3d(&ap.q_lo, w->q_s.l(), 64, T, BH, 64, (uint64_t)T * 64, 64, 128));
+    TMAP_OK(encode_tmap_bf16_3d(&ap.k_hi, w->k_s.h(), 64, T, BH, 64, (uint64_t)T * 64, 64, 64));
+    TMAP_OK(encode_tmap_bf16_3d(&ap.k_lo, w->k_s.l(), 64, T, BH, 64, (uint64_t)T * 64, 64, 64));
+    TMAP_OK(encode_tmap_bf16_3d(&ap.vt_hi, w->vt_s.h(), T, 64, BH, Tp, (uint64_t)64 * Tp, 64, 64));
+    TMAP_OK(encode_tmap_bf16_3d(&ap.vt_lo, w->vt_s.l(), T, 64, BH, Tp, (uint64_t)64 * Tp, 64, 64));
+    ap.B = B, ap.H = H, ap.T = T, ap.D = H * 64;
+    ap.kv_len = d_kv;
+    ap.ctx = w->ctx_s.planes(scheme);
+    return 0;
+}
+
+// One Conformer layer (wav2vec2_model.py:537-578) as nine GEMMs. Residual stream: hidden state l -> r1 (x1_f32, after
+// ffn1) -> r2 (x_f32, after attention) -> r3 (x1_f32, after the conv module) -> r4 (tmp_f32, after ffn2) ->
+// final_layer_norm -> hidden state l+1. Operand planes: xs_s = LayerNorm outputs, x1_s = rope(LN) / depthwise output.
+int Fwd::build_conformer_layer(LayerPlan& lp, int l) {
+    const s3b_config& c = m->cfg;
+    const int D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, sch = m->scheme;
+    LayerW& W = m->layers[l];
+    {   // ffn1.w_1 + SiLU
+        GemmParams& p = lp.ffn1_a;
+        S3B_OK(linear_params(p, w->xs_s, W.ffn1_w1, M, F, D, 2, sch));
+        Epi e;
+        e.bias = W.ffn1_b1.as<float>(), e.gelu = 2, e.op = w->h_s.planes(sch);
+        set_epi(p, e, F);
+    }
+    {   // r1 = x + 0.5 ffn1 (0.5 folded into w_2; residual = hidden state l, patched per call)
+        GemmParams& p = lp.ffn1_b;
+        S3B_OK(linear_params(p, w->h_s, W.ffn1_w2, M, D, F, 0, sch));
+        Epi e;
+        e.bias = W.ffn1_b2.as<float>(), e.out_f32 = w->x1_f32.as<float>();
+        set_epi(p, e, D);
+    }
+    {   // [q | k] from rope(LN(r1)), v from LN(r1)
+        GemmParams& p = lp.qkv;
+        S3B_OK(linear_params(p, w->x1_s, W.qkv, M, 2 * D, D, 1, sch));
+        set_qkv_epi(p, W.qkv_b.as<float>(), T, H, w->q_s, w->k_s, w->vt_s, 0);
+        GemmParams& pv = lp.v;
+        S3B_OK(linear_params(pv, w->xs_s, W.v, M, D, D, 1, sch));
+        set_qkv_epi(pv, W.qkv_b.as<float>() + 2 * D, T, H, w->q_s, w->k_s, w->vt_s, 2 * D);
+    }
+    S3B_OK(attn_params(lp.attn, w, B, T, H, d_kv, sch));
+    {   // r2 = r1 + linear_out(attn)
+        GemmParams& p = lp.out;
+        S3B_OK(linear_params(p, w->ctx_s, W.out, M, D, D, 0, sch));
+        Epi e;
+        e.bias = W.out_b.as<float>(), e.residual = w->x1_f32.as<float>(), e.out_f32 = w->x_f32.as<float>();
+        set_epi(p, e, D);
+    }
+    {   // pointwise_conv1 (no bias) -> fp32 [M][2D], the depthwise kernel's input
+        GemmParams& p = lp.pw1;
+        S3B_OK(linear_params(p, w->xs_s, W.pw1, M, 2 * D, D, 0, sch));
+        Epi e;
+        e.out_f32 = w->glu_f32.as<float>();
+        set_epi(p, e, 2 * D);
+    }
+    {   // r3 = r2 + pointwise_conv2 (no bias)
+        GemmParams& p = lp.pw2;
+        S3B_OK(linear_params(p, w->x1_s, W.pw2, M, D, D, 0, sch));
+        Epi e;
+        e.residual = w->x_f32.as<float>(), e.out_f32 = w->x1_f32.as<float>();
+        set_epi(p, e, D);
+    }
+    {   // ffn2.w_1 + SiLU
+        GemmParams& p = lp.fc1;
+        S3B_OK(linear_params(p, w->xs_s, W.fc1, M, F, D, 2, sch));
+        Epi e;
+        e.bias = W.fc1_b.as<float>(), e.gelu = 2, e.op = w->h_s.planes(sch);
+        set_epi(p, e, F);
+    }
+    {   // r4 = r3 + 0.5 ffn2
+        GemmParams& p = lp.fc2;
+        S3B_OK(linear_params(p, w->h_s, W.fc2, M, D, F, 0, sch));
+        Epi e;
+        e.bias = W.fc2_b.as<float>(), e.residual = w->x1_f32.as<float>(), e.out_f32 = w->tmp_f32.as<float>();
+        set_epi(p, e, D);
+    }
+    return 0;
+}
+
 int Fwd::build_plan(Plan& pl) {
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, NL = c.num_layers, C = kConvDim;
@@ -1197,9 +1437,14 @@ int Fwd::build_plan(Plan& pl) {
         Epi e;
         e.bias = m->proj_b.as<float>();
         e.row_mask = d_mask;  // x[padding_mask] = 0 (wav2vec2_model.py:3061-3062)
-        e.out_f32 = w->x_f32.as<float>();
-        e.op = w->x_s.planes(0);  // operand of pos_conv, which stays on the bf16x3 kernel (48-channel groups)
+        e.out_f32 = w->x_f32.as<float>();  // patched per call (proj_out)
+        if (!c.conformer) e.op = w->x_s.planes(0);  // operand of pos_conv, which stays on the bf16x3 kernel (48-channel groups)
         set_epi(p, e, D);
+    }
+    if (c.conformer) {
+        pl.layers.resize(NL);
+        for (int l = 0; l < NL; ++l) S3B_OK(build_conformer_layer(pl.layers[l], l));
+        return 0;
     }
     if (c.pos_conv_depth > 1) {
         // block i reads the operand planes block i-1 wrote (x_s -> x1_s -> ctx_s -> x1_s ...; both are free here)
@@ -1229,7 +1474,6 @@ int Fwd::build_plan(Plan& pl) {
         }
     }
     pl.layers.resize(NL);
-    const uint64_t BH = (uint64_t)B * H;
     for (int l = 0; l < NL; ++l) {
         LayerW& W = m->layers[l];
         LayerPlan& lp = pl.layers[l];
@@ -1238,20 +1482,8 @@ int Fwd::build_plan(Plan& pl) {
             S3B_OK(linear_params(p, w->xs_s, W.qkv, M, 3 * D, D, 1, m->scheme));
             set_qkv_epi(p, W.qkv_b.as<float>(), T, H, w->q_s, w->k_s, w->vt_s);
         }
-        {
-            AttnParams& ap = lp.attn;
-            memset(&ap, 0, sizeof(ap));
-            TMAP_OK(encode_tmap_bf16_3d(&ap.q_hi, w->q_s.h(), 64, T, BH, 64, (uint64_t)T * 64, 64, 128));
-            TMAP_OK(encode_tmap_bf16_3d(&ap.q_lo, w->q_s.l(), 64, T, BH, 64, (uint64_t)T * 64, 64, 128));
-            TMAP_OK(encode_tmap_bf16_3d(&ap.k_hi, w->k_s.h(), 64, T, BH, 64, (uint64_t)T * 64, 64, 64));
-            TMAP_OK(encode_tmap_bf16_3d(&ap.k_lo, w->k_s.l(), 64, T, BH, 64, (uint64_t)T * 64, 64, 64));
-            TMAP_OK(encode_tmap_bf16_3d(&ap.vt_hi, w->vt_s.h(), T, 64, BH, Tp, (uint64_t)64 * Tp, 64, 64));
-            TMAP_OK(encode_tmap_bf16_3d(&ap.vt_lo, w->vt_s.l(), T, 64, BH, Tp, (uint64_t)64 * Tp, 64, 64));
-            ap.B = B, ap.H = H, ap.T = T, ap.D = D;
-            ap.kv_len = d_kv;
-            if (c.relative_position) set_rel_bias(ap, m->rel_table.as<float>(), m->rel_table_T, w->gate.as<float>());
-            ap.ctx = w->ctx_s.planes(m->scheme);
-        }
+        S3B_OK(attn_params(lp.attn, w, B, T, H, d_kv, m->scheme));
+        if (c.relative_position) set_rel_bias(lp.attn, m->rel_table.as<float>(), m->rel_table_T, w->gate.as<float>());
         {   // out_proj + residual (residual = hidden state l, patched per call)
             GemmParams& p = lp.out;
             S3B_OK(linear_params(p, w->ctx_s, W.out, M, D, D, 0, m->scheme));
@@ -1365,6 +1597,19 @@ int Fwd::stage(int s) {
         KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
         if (distil() && layer_done) S3B_OK(layer_done(m, 0, st, user));
         return 0;
+    }
+    if (s == 8 && c.conformer) {
+        // ---- Conformer: no pos_conv; post-LN models: encoder.layer_norm -> hidden state 0 (wav2vec2_model.py:3183-3184)
+        if (!c.layer_norm_first)
+            KNORM(launch_layernorm(w->x_f32.as<float>(), (size_t)M, D, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(), 0,
+                                   hs(0), no_planes(), st));
+        if (layer_done) S3B_OK(layer_done(m, 0, st, user));
+        return 0;
+    }
+    if (c.conformer) {
+        const int l = (s - 9) / kConformerStages;
+        if (l >= NL) return fail("internal: stage %d out of range", s);
+        return conformer_stage(l, (s - 9) % kConformerStages);
     }
     if (s == 8) {
         // ---- x = x + GELU(pos_conv(x)) ; post-LN models: LayerNorm -> hidden state 0 -------------------------------
@@ -1487,6 +1732,88 @@ int Fwd::stage(int s) {
         }
     }
     return 0;
+}
+
+// Conformer layer l, stage `sub` of kConformerStages (buffers: build_conformer_layer)
+int Fwd::conformer_stage(int l, int sub) {
+    s3b_model* m = this->m;  // the launch macros expect `m` and `st`
+    cudaStream_t st = this->st;
+    const s3b_config& c = m->cfg;
+    const int D = c.embed_dim;
+    const double attn_flops = 4.0 * (double)T * T * D * B;
+    LayerW& W = m->layers[l];
+    LayerPlan& lp = plan->layers[l];
+    const OutPlanes xs = w->xs_s.planes(m->scheme);
+    switch (sub) {
+        case 0: {  // ffn1: LayerNorm -> w_1 + SiLU
+            KNORM(launch_layernorm(hs(l), (size_t)M, D, W.ffn1_ln_g.as<float>(), W.ffn1_ln_b.as<float>(), 0, nullptr, xs, st));
+            GemmParams p = lp.ffn1_a;
+            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            return 0;
+        }
+        case 1: {  // r1 = x + 0.5 w_2(...)
+            GemmParams p = lp.ffn1_b;
+            p.residual = hs(l);
+            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            return 0;
+        }
+        case 2: {  // self_attn_layer_norm + RoPE -> [q | k] and v
+            KNORM(launch_layernorm_rope(w->x1_f32.as<float>(), (size_t)M, T, D, W.ln1_g.as<float>(), W.ln1_b.as<float>(),
+                                        m->rope_cs.as<float>(), xs, w->x1_s.planes(m->scheme), st));
+            {
+                GemmParams p = lp.qkv;
+                KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            }
+            GemmParams p = lp.v;
+            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            return 0;
+        }
+        case 3:
+            KATTN(launch_attention(lp.attn, st));
+            return 0;
+        case 4: {  // r2 = r1 + linear_out
+            GemmParams p = lp.out;
+            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            return 0;
+        }
+        case 5: {  // conv_module: LayerNorm -> pointwise_conv1
+            KNORM(launch_layernorm(w->x_f32.as<float>(), (size_t)M, D, W.conv_ln_g.as<float>(), W.conv_ln_b.as<float>(), 0,
+                                   nullptr, xs, st));
+            GemmParams p = lp.pw1;
+            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            return 0;
+        }
+        case 6:  // GLU -> depthwise conv -> BatchNorm -> SiLU
+            KMISC(launch_depthwise_glu(w->glu_f32.as<float>(), B, T, D, c.depthwise_kernel, W.dw_w.as<float>(),
+                                       W.dw_b.as<float>(), w->x1_s.planes(m->scheme), st));
+            return 0;
+        case 7: {  // r3 = r2 + pointwise_conv2
+            GemmParams p = lp.pw2;
+            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            return 0;
+        }
+        case 8: {  // ffn2: LayerNorm -> w_1 + SiLU
+            KNORM(launch_layernorm(w->x1_f32.as<float>(), (size_t)M, D, W.ffn2_ln_g.as<float>(), W.ffn2_ln_b.as<float>(), 0,
+                                   nullptr, xs, st));
+            GemmParams p = lp.fc1;
+            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            return 0;
+        }
+        default: {  // r4 = r3 + 0.5 w_2(...) -> final_layer_norm -> hidden state l+1 (pre-LN: encoder.layer_norm after
+                    // the last layer, wav2vec2_model.py:3049-3050)
+            GemmParams p = lp.fc2;
+            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            float* r4 = w->tmp_f32.as<float>();
+            const bool enc_ln = c.layer_norm_first && l == c.num_layers - 1;
+            KNORM(launch_layernorm(r4, (size_t)M, D, W.ln2_g.as<float>(), W.ln2_b.as<float>(), 0, enc_ln ? r4 : hs(l + 1),
+                                   no_planes(), st));
+            if (enc_ln)
+                KNORM(launch_layernorm(r4, (size_t)M, D, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(), 0, hs(l + 1),
+                                       no_planes(), st));
+            if (layer_done) S3B_OK(layer_done(m, l + 1, st, user));
+            return 0;
+        }
+    }
 }
 
 // Number of lanes for a batch: S3B_LANES overrides; otherwise two lanes when the batch can be split AND carries at
@@ -1651,6 +1978,8 @@ extern "C" int s3b_forward_ex(s3b_model* m, const float* const* wavs, const int6
                     (int)sizeof(s3b_forward_opts));
     for (int b = 0; b < batch; ++b)
         if (lens[b] > max_len) return fail("lens[%d]=%lld exceeds max_len", b, (long long)lens[b]);
+    if (m->cfg.conformer && opts != nullptr && (opts->ffn_out != nullptr || opts->last_residual != nullptr))
+        return fail("ffn_out / last_residual: a Conformer encoder collects no layer results (wav2vec2_model.py:3199-3200)");
     return forward_lanes(m, wavs, lens, batch, max_len, hidden_out, (cudaStream_t)stream, opts);
 }
 
@@ -1941,6 +2270,7 @@ extern "C" int s3b_linear_ex(const float* a, const float* w, const float* bias, 
     int scheme = 0;
     S3B_OK(resolve_scheme(o.scheme, K, N, &scheme));
     S3B_OK(check_out_fmt(o.out_fmt));
+    if (gelu < 0 || gelu > 2) return fail("gelu must be 0 (none), 1 (GELU) or 2 (SiLU), not %d", gelu);
     if (o.tile_n != 0 && o.tile_n != 128 && o.tile_n != 256) return fail("tile_n must be 0, 128 or 256, not %d", o.tile_n);
     if (o.tile_n != 0 && N % o.tile_n != 0) return fail("tile_n %d does not divide N = %d", o.tile_n, N);
     if (o.tile_n != 0 && !pairs_enabled()) return fail("tile_n needs the paired tile layout (S3B_GEMM_PAIR=0 is set)");
@@ -2348,6 +2678,68 @@ extern "C" int s3b_frontend_f32(const float* const* wavs, const int64_t* lens, i
         return 0;
     }();
     book.release(), pad.release(), stats.release(), part.release(), ss.release(), os.release();
+    return r;
+}
+
+extern "C" int s3b_conformer_conv_f32(const float* x, int32_t B, int32_t T, int32_t D, int32_t k, const float* dw_w,
+                                      const float* bn_gamma, const float* bn_beta, const float* bn_mean,
+                                      const float* bn_var, int32_t out_fmt, float* out, void* stream) {
+    // Fwd::conformer_stage(6) on this call's buffers: BatchNorm folded on the host like s3b_model_finalize does it
+    if (!x || !dw_w || !bn_gamma || !bn_beta || !bn_mean || !bn_var || !out) return fail("null argument");
+    if (B < 1 || T < 1) return fail("bad sizes (batch %d, t %d)", B, T);
+    if (D < 64 || D % 64 != 0) return fail("d must be a positive multiple of 64, not %d", D);
+    if (k < 1 || k > kDwMaxKernel || k % 2 == 0) return fail("kernel size %d: must be odd, 1..%d", k, kDwMaxKernel);
+    if (out_fmt != 0 && out_fmt != 1) return fail("out_fmt must be 0 (bf16 hi/lo) or 1 (f16q8), not %d", out_fmt);
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t M = (size_t)B * T;
+    DevBuf wb, bb;
+    SplitBuf os;
+    const int r = [&]() -> int {
+        std::vector<float> w, g, be, mu, var, wf, bf;
+        S3B_OK(download_f32(dw_w, (size_t)D * k, st, w));
+        S3B_OK(download_f32(bn_gamma, D, st, g));
+        S3B_OK(download_f32(bn_beta, D, st, be));
+        S3B_OK(download_f32(bn_mean, D, st, mu));
+        S3B_OK(download_f32(bn_var, D, st, var));
+        fold_depthwise_bn(w.data(), g.data(), be.data(), mu.data(), var.data(), D, k, wf, bf);
+        S3B_OK(upload_f32(wb, wf.data(), wf.size()));
+        S3B_OK(upload_f32(bb, bf.data(), bf.size()));
+        S3B_OK(os.ensure(M * D));
+        CUDA_OK(launch_depthwise_glu(x, B, T, D, k, wb.as<float>(), bb.as<float>(), os.planes(out_fmt), st));
+        CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), M * D, out, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+        return 0;
+    }();
+    wb.release(), bb.release(), os.release();
+    return r;
+}
+
+extern "C" int s3b_layernorm_rope_f32(const float* x, int64_t M, int32_t T, int32_t D, const float* gamma,
+                                      const float* beta, const float* inv_freq, int32_t out_fmt, float* out,
+                                      float* out_rope, void* stream) {
+    // Fwd::conformer_stage(2)'s LayerNorm + RoPE kernel, with a table built for the t frames like build_rope_table
+    if (!x || !gamma || !beta || !out || !out_rope) return fail("null argument");
+    if (M < 1 || T < 1 || M % T != 0) return fail("m = %lld must be a positive multiple of t = %d", (long long)M, T);
+    if (D != 512 && D != 768 && D != 1024 && D != 1280) return fail("d must be 512, 768, 1024 or 1280, not %d", D);
+    if (out_fmt != 0 && out_fmt != 1) return fail("out_fmt must be 0 (bf16 hi/lo) or 1 (f16q8), not %d", out_fmt);
+    cudaStream_t st = (cudaStream_t)stream;
+    const std::vector<float> f = inv_freq ? std::vector<float>(inv_freq, inv_freq + 32) : default_inv_freq();
+    const std::vector<float> cs = rope_table(f, T);
+    DevBuf table;
+    SplitBuf y, yr;
+    const int r = [&]() -> int {
+        S3B_OK(table.ensure(cs.size() * 4));
+        CUDA_OK(cudaMemcpyAsync(table.p, cs.data(), cs.size() * 4, cudaMemcpyHostToDevice, st));
+        S3B_OK(y.ensure((size_t)M * D));
+        S3B_OK(yr.ensure((size_t)M * D));
+        CUDA_OK(launch_layernorm_rope(x, (size_t)M, T, D, gamma, beta, table.as<float>(), y.planes(out_fmt),
+                                      yr.planes(out_fmt), st));
+        CUDA_OK(launch_planes_to_f32(y.planes(out_fmt), (size_t)M * D, out, st));
+        CUDA_OK(launch_planes_to_f32(yr.planes(out_fmt), (size_t)M * D, out_rope, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+        return 0;
+    }();
+    table.release(), y.release(), yr.release();
     return r;
 }
 

@@ -69,6 +69,88 @@ cudaError_t launch_layernorm(const float* x, size_t M, int D, const float* gamma
 }
 
 // ------------------------------------------------------------------------------------------------
+// Conformer attention input (wav2vec2_model.py:255-310, 541): y = self_attn_layer_norm(x) and its rotary embedding
+//   rope(y)_t = y_t * cos_t + rotate_half(y_t) * sin_t,  rotate_half(u) = cat(-u[32:], u[:32]) per 64-wide head,
+// t = frame index in the padded batch (row % T). y feeds linear_v, rope(y) linear_q / linear_k; both are written as
+// operand planes. cs: [>= T][64] fp32, cos of the 32 angles then their sin. Lane l holds channels 4 (l + 32 i) + 0..3,
+// i.e. head offset 4 (l & 15): its rotate_half partner (offset +- 32) is lane l ^ 8 with the same i.
+// ------------------------------------------------------------------------------------------------
+template <int V4>
+__global__ void __launch_bounds__(256) layernorm_rope_kernel(const float* __restrict__ x, size_t M, int T,
+                                                             const float* __restrict__ gamma,
+                                                             const float* __restrict__ beta,
+                                                             const float* __restrict__ cs, const OutPlanes op,
+                                                             const OutPlanes op_rope) {
+    constexpr int D = V4 * 128;
+    const int lane = threadIdx.x & 31;
+    const size_t row = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    pdl_wait();
+    pdl_launch_dependents();
+    if (row >= M) return;  // warp-uniform: the shuffles below see full warps
+    const float4* xr = reinterpret_cast<const float4*>(x + row * D);
+    float4 v[V4];
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < V4; ++i) {
+        v[i] = xr[lane + 32 * i];
+        s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
+    }
+    const float mean = warp_sum(s) * (1.0f / D);
+    float q = 0.f;
+#pragma unroll
+    for (int i = 0; i < V4; ++i) {
+        const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
+        q += (a * a + b * b) + (c * c + d * d);
+    }
+    const float rstd = rsqrtf(warp_sum(q) * (1.0f / D) + 1e-5f);
+    const int t = (int)(row % (size_t)T);
+    const float4 co = __ldg(reinterpret_cast<const float4*>(cs + (size_t)t * 64) + (lane & 7));
+    const float4 si = __ldg(reinterpret_cast<const float4*>(cs + (size_t)t * 64 + 32) + (lane & 7));
+    const float sgn = (lane & 8) ? 1.0f : -1.0f;  // first half of a head takes -u[d + 32], second half +u[d - 32]
+    const float4* g4 = reinterpret_cast<const float4*>(gamma);
+    const float4* b4 = reinterpret_cast<const float4*>(beta);
+#pragma unroll
+    for (int i = 0; i < V4; ++i) {
+        const int c4 = lane + 32 * i;
+        const float4 g = __ldg(g4 + c4), b = __ldg(b4 + c4);
+        float4 y;
+        y.x = (v[i].x - mean) * rstd * g.x + b.x;
+        y.y = (v[i].y - mean) * rstd * g.y + b.y;
+        y.z = (v[i].z - mean) * rstd * g.z + b.z;
+        y.w = (v[i].w - mean) * rstd * g.w + b.w;
+        float4 u;
+        u.x = sgn * __shfl_xor_sync(0xffffffffu, y.x, 8);
+        u.y = sgn * __shfl_xor_sync(0xffffffffu, y.y, 8);
+        u.z = sgn * __shfl_xor_sync(0xffffffffu, y.z, 8);
+        u.w = sgn * __shfl_xor_sync(0xffffffffu, y.w, 8);
+        float4 r;
+        r.x = y.x * co.x + u.x * si.x;
+        r.y = y.y * co.y + u.y * si.y;
+        r.z = y.z * co.z + u.z * si.z;
+        r.w = y.w * co.w + u.w * si.w;
+        store_planes4(op, y, row * D + 4 * (size_t)c4);
+        store_planes4(op_rope, r, row * D + 4 * (size_t)c4);
+    }
+}
+
+cudaError_t launch_layernorm_rope(const float* x, size_t M, int T, int D, const float* gamma, const float* beta,
+                                  const float* cs, const OutPlanes& op, const OutPlanes& op_rope, cudaStream_t s) {
+    if (M == 0) return cudaSuccess;
+    if (T < 1 || op.hi == nullptr || op_rope.hi == nullptr) return cudaErrorInvalidValue;
+    const unsigned blocks = (unsigned)((M + 7) / 8);
+#define S3B_LR(V) \
+    return launch_pdl(layernorm_rope_kernel<V>, dim3(blocks), dim3(256), 0, s, x, M, T, gamma, beta, cs, op, op_rope)
+    switch (D) {
+        case 512: S3B_LR(4);
+        case 768: S3B_LR(6);
+        case 1024: S3B_LR(8);
+        case 1280: S3B_LR(10);
+        default: return cudaErrorInvalidValue;
+    }
+#undef S3B_LR
+}
+
+// ------------------------------------------------------------------------------------------------
 // pos_conv combine: the grouped k=128 convolution is computed as a GEMM over FOUR taps per k-block,
 //   Z_j[u] = sum_q x[u + 4q - 64] . W[4q + j]   (j = 0..3, N = 4 * cpg columns per group; model.cu posconv4_params)
 // and the four column blocks are re-aligned here:  conv[t] = sum_j Z_j[t + j]. One warp per frame:

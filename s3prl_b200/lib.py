@@ -54,6 +54,8 @@ EXPORTED_SYMBOLS = [
     "s3b_attention_ex",
     "s3b_wavlm_gate_f32",
     "s3b_frontend_f32",
+    "s3b_conformer_conv_f32",
+    "s3b_layernorm_rope_f32",
     "s3b_fbank",
     "s3b_fbank_num_frames",
     "s3b_trimmed_lengths",
@@ -87,7 +89,9 @@ class S3BConfig(C.Structure):
         ("no_feature_layer_norm", C.c_int32),
         ("pred_heads", C.c_int32),
         ("pos_conv_depth", C.c_int32),
-        ("reserved", C.c_int32 * 5),
+        ("conformer", C.c_int32),
+        ("depthwise_kernel", C.c_int32),
+        ("reserved", C.c_int32 * 3),
     ]
 
 
@@ -221,6 +225,8 @@ def load() -> C.CDLL:
     lib.s3b_wavlm_gate_f32.argtypes = [f32p, i32, i32, i32, f32p, f32p, f32p, i32, f32p, vp]
     lib.s3b_frontend_f32.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i64, i32, f32p, f32p, f32p, f32p, i32, i32,
                                      f32p, f32p, vp]
+    lib.s3b_conformer_conv_f32.argtypes = [f32p, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, i32, f32p, vp]
+    lib.s3b_layernorm_rope_f32.argtypes = [f32p, i64, i32, i32, f32p, f32p, C.POINTER(C.c_float), i32, f32p, f32p, vp]
     lib.s3b_fbank_num_frames.argtypes = [i64]
     lib.s3b_fbank_num_frames.restype = i64
     lib.s3b_fbank.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, f32p, vp]

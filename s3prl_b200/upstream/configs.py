@@ -38,6 +38,13 @@ class ArchConfig:
     # post_extract_proj, and `pred_heads` prediction heads (Linear -> GELU -> SplitLinear) on the encoder output
     feature_layer_norm: bool = True
     pred_heads: int = 0
+    # wav2vec 2.0 Conformer (Wav2Vec2Config.layer_type / attn_type / pos_enc_type / depthwise_conv_kernel_size,
+    # wav2vec2_model.py:2448, 3132-3211): ConformerEncoderLayer instead of the transformer layer, no pos_conv. Served:
+    # attn_type "espnet" with rotary position encoding ("rope") only.
+    layer_type: str = "transformer"  # "transformer" | "conformer"
+    pos_enc_type: str = "abs"  # "abs" | "rope" | "rel_pos"
+    attn_type: str = ""  # "" (fairseq MultiheadAttention) | "espnet"
+    depthwise_conv_kernel_size: int = 31
 
     @property
     def family_id(self) -> int:
@@ -48,6 +55,10 @@ class ArchConfig:
     def pos_conv_kernel(self) -> int:
         """Taps of one positional conv (wav2vec2_model.py:2996-2998)."""
         return max(3, self.conv_pos // self.pos_conv_depth) if self.pos_conv_depth > 1 else self.conv_pos
+
+    @property
+    def conformer(self) -> bool:
+        return self.layer_type == "conformer"
 
     @property
     def num_outputs(self) -> int:
@@ -108,6 +119,13 @@ for _alias, _arch in {
     "ms_hubert": "hubert_base",
 }.items():
     ARCHS[_alias] = ARCHS[_arch]
+# wav2vec 2.0 Conformer with rotary attention (s3prl/upstream/wav2vec2/hubconf.py wav2vec2_conformer_rope). The values
+# are those of fairseq's Conformer-large LibriLight pre-training config as far as they are public; they were NOT checked
+# against the released checkpoint (not reachable offline). They only shape the fabricated checkpoint: a real checkpoint
+# loaded through wav2vec2_local carries its own cfg (arch_from_reference_cfg).
+ARCHS["wav2vec2_conformer_rope"] = replace(
+    _BASE, family="wav2vec2", **_LL60K, layer_type="conformer", pos_enc_type="rope", attn_type="espnet"
+)
 ALIASES = {
     "hubert": "hubert_base",
     "hubert_large": "hubert_large_ll60k",
@@ -155,6 +173,24 @@ def arch_from_reference_cfg(family: str, model_cfg: dict, task_cfg: dict | None 
             feature_layer_norm=False,
             pred_heads=int(g("n_tasks", 12)),
         )
+    layer_type = g("layer_type", "transformer") or "transformer"
+    conformer = {}
+    if layer_type == "conformer":
+        pos_enc, attn, k = g("pos_enc_type", "abs"), g("attn_type", ""), int(g("depthwise_conv_kernel_size", 31))
+        if family != "wav2vec2":
+            raise ValueError(f"a Conformer encoder is a wav2vec2 model, not family '{family}'")
+        if pos_enc == "rel_pos":
+            raise ValueError("Conformer with pos_enc_type 'rel_pos' (Transformer-XL attention) is not supported; "
+                             "only the rotary variant ('rope') is")
+        if pos_enc != "rope":
+            raise ValueError(f"Conformer with pos_enc_type {pos_enc!r} is not supported; only 'rope' is")
+        if attn != "espnet":
+            raise ValueError(f"Conformer with attn_type {attn!r} is not supported; only 'espnet' is")
+        if k % 2 == 0 or not 1 <= k <= 63:
+            raise ValueError(f"depthwise_conv_kernel_size {k}: must be odd and at most 63")
+        conformer = dict(layer_type="conformer", pos_enc_type=pos_enc, attn_type=attn, depthwise_conv_kernel_size=k)
+    elif layer_type != "transformer":
+        raise ValueError(f"unsupported layer_type {layer_type!r}")
     return ArchConfig(
         family=family,
         extractor_mode=g("extractor_mode", "default"),
@@ -172,4 +208,5 @@ def arch_from_reference_cfg(family: str, model_cfg: dict, task_cfg: dict | None 
         num_buckets=int(g("num_buckets", 320)),
         max_distance=int(g("max_distance", 800)),
         gru_rel_pos=bool(g("gru_rel_pos", False)),
+        **conformer,
     )

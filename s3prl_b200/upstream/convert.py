@@ -47,6 +47,9 @@ def reference_model_cfg(cfg: ArchConfig) -> Dict:
     )
     if cfg.pos_conv_depth > 1:
         d.update(pos_conv_depth=cfg.pos_conv_depth)
+    if cfg.conformer:
+        d.update(layer_type="conformer", pos_enc_type=cfg.pos_enc_type, attn_type=cfg.attn_type,
+                 depthwise_conv_kernel_size=cfg.depthwise_conv_kernel_size)
     if cfg.family == "wavlm":
         d.update(
             normalize=cfg.normalize,

@@ -56,7 +56,16 @@ def _c_config(cfg: ArchConfig) -> _lib.S3BConfig:
     c.no_feature_layer_norm = int(not cfg.feature_layer_norm)
     c.pred_heads = int(cfg.pred_heads)
     c.pos_conv_depth = int(cfg.pos_conv_depth)
+    if cfg.conformer:
+        c.conformer = 1
+        c.depthwise_kernel = int(cfg.depthwise_conv_kernel_size)
     return c
+
+
+def _rotary_inv_freq() -> torch.Tensor:
+    """RotaryPositionalEmbedding's buffer for 64-wide heads, computed as the reference computes it
+    (wav2vec2_model.py:51): a checkpoint without the buffer gets the value the reference model would hold."""
+    return 1.0 / (10000 ** (torch.arange(0, 64, 2).float() / 64))
 
 
 class _NativeModel:
@@ -70,6 +79,10 @@ class _NativeModel:
         self.handle = C.c_void_p()
         cc = _c_config(cfg)
         _lib.check(self.lib.s3b_model_create(C.byref(cc), C.byref(self.handle)))
+        if cfg.conformer:
+            state_dict = dict(state_dict)
+            for l in range(cfg.encoder_layers):
+                state_dict.setdefault(f"encoder.layers.{l}.self_attn.rotary_emb.inv_freq", _rotary_inv_freq())
         try:
             for name, t in state_dict.items():
                 if not torch.is_tensor(t) or not t.is_floating_point():
@@ -133,6 +146,11 @@ class UpstreamExpert(nn.Module):
             raise AssertionError(f"feature_selection must be one of {_FEATURE_SELECTIONS}, got {feature_selection!r}")
         if self.arch.family == "distiller" and (hooks or feature_selection is not None):
             raise TypeError("the Distiller expert takes neither hooks nor feature_selection (distiller/expert.py:18-40)")
+        if self.arch.conformer and (hooks or feature_selection is not None):
+            raise TypeError(
+                "feature_selection and hooks are not available for a Conformer model: its encoder collects no layer "
+                "results (wav2vec2_model.py:3199-3200); use the default hidden_states"
+            )
         if feature_selection is not None and self.arch.family != "wav2vec2":
             raise TypeError(f"feature_selection is an option of the wav2vec2 experts only (got family {self.arch.family})")
         self.feature_selection = feature_selection

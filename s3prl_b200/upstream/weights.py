@@ -47,6 +47,8 @@ def fabricate_state_dict(cfg: ArchConfig, seed: int = 0) -> Dict[str, torch.Tens
     sd["post_extract_proj.weight"] = randn(D, in_d, std=1.0 / math.sqrt(in_d))
     sd["post_extract_proj.bias"] = randn(D, std=0.05)
     cpg = D // cfg.conv_pos_groups
+    if cfg.conformer:
+        return _fabricate_conformer(cfg, sd, randn, g)
     if cfg.pos_conv_depth > 1:
         # data2vec: plain Conv1d blocks (make_conv_block, wav2vec2_model.py:3000-3022; every block is followed by a LayerNorm, so the scale is immaterial)
         k = cfg.pos_conv_kernel
@@ -86,6 +88,44 @@ def fabricate_state_dict(cfg: ArchConfig, seed: int = 0) -> Dict[str, torch.Tens
         sd["output_layer.0.bias"] = randn(N * D, std=0.05)
         sd["output_layer.2.weight"] = randn(N, D, D, std=1.0 / math.sqrt(D))  # [task][in][out]
         sd["output_layer.2.bias"] = randn(1, 1, N, D, std=0.05)
+    return sd
+
+
+def _fabricate_conformer(cfg: ArchConfig, sd: Dict[str, torch.Tensor], randn, g) -> Dict[str, torch.Tensor]:
+    """The encoder of a rotary Conformer (ConformerEncoder / ConformerEncoderLayer, wav2vec2_model.py:441-578,
+    3132-3211): no pos_conv; per layer two half-step FFNs, rotary attention, the convolution module and the final
+    LayerNorm. BatchNorm statistics are non-trivial (running_var in [0.5, 1.5], non-zero running_mean) so that the
+    folding of eval-mode BatchNorm into the depthwise taps is exercised. The rotary inv_freq buffer is left to the
+    model (it is not a learned parameter)."""
+    D, F, k = cfg.encoder_embed_dim, cfg.encoder_ffn_embed_dim, cfg.depthwise_conv_kernel_size
+
+    def ln(name):
+        sd[f"{name}.weight"] = randn(D, std=0.1, mean=1.0)
+        sd[f"{name}.bias"] = randn(D, std=0.1)
+
+    ln("encoder.layer_norm")
+    for l in range(cfg.encoder_layers):
+        p = f"encoder.layers.{l}"
+        for f in ("ffn1", "ffn2"):
+            ln(f"{p}.{f}.layer_norm")
+            sd[f"{p}.{f}.w_1.weight"] = randn(F, D, std=1.0 / math.sqrt(D))
+            sd[f"{p}.{f}.w_1.bias"] = randn(F, std=0.05)
+            sd[f"{p}.{f}.w_2.weight"] = randn(D, F, std=1.0 / math.sqrt(F))
+            sd[f"{p}.{f}.w_2.bias"] = randn(D, std=0.05)
+        ln(f"{p}.self_attn_layer_norm")
+        for name in ("linear_q", "linear_k", "linear_v", "linear_out"):
+            sd[f"{p}.self_attn.{name}.weight"] = randn(D, D, std=1.0 / math.sqrt(D))
+            sd[f"{p}.self_attn.{name}.bias"] = randn(D, std=0.05)
+        c = f"{p}.conv_module"
+        ln(f"{c}.layer_norm")
+        sd[f"{c}.pointwise_conv1.weight"] = randn(2 * D, D, 1, std=1.0 / math.sqrt(D))
+        sd[f"{c}.depthwise_conv.weight"] = randn(D, 1, k, std=1.0 / math.sqrt(k))
+        sd[f"{c}.batch_norm.weight"] = randn(D, std=0.1, mean=1.0)
+        sd[f"{c}.batch_norm.bias"] = randn(D, std=0.1)
+        sd[f"{c}.batch_norm.running_mean"] = randn(D, std=0.1)
+        sd[f"{c}.batch_norm.running_var"] = torch.rand(D, generator=g) + 0.5
+        sd[f"{c}.pointwise_conv2.weight"] = randn(D, D, 1, std=1.0 / math.sqrt(D))
+        ln(f"{p}.final_layer_norm")
     return sd
 
 
