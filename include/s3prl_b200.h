@@ -30,7 +30,8 @@ typedef struct s3b_config {
     int32_t num_layers;           /* encoder_layers */
     int32_t embed_dim;            /* encoder_embed_dim (multiple of 128) */
     int32_t ffn_dim;              /* encoder_ffn_embed_dim */
-    int32_t num_heads;            /* encoder_attention_heads; head dim must be 64 */
+    int32_t num_heads;            /* encoder_attention_heads; head dim embed_dim / num_heads: 64, 80 or 120 (64 for a
+                                   * Conformer or the wavlm family) */
     int32_t pos_conv_kernel;      /* conv_pos (128; data2vec 95) */
     int32_t pos_conv_groups;      /* conv_pos_groups (16) */
     int32_t relative_position;    /* WavLM relative_position_embedding */
@@ -231,6 +232,11 @@ int s3b_linear_ex(const float* a, const float* w, const float* bias, const float
  * t.. are never written by it and come back as the zero of a freshly allocated plane. */
 int s3b_qkv_f32(const float* x, const float* w, const float* b, int32_t batch, int32_t t, int32_t heads, int32_t scheme,
                 float* q_out, float* k_out, float* vt_out, void* stream);
+/* s3b_qkv_f32 for heads of head_dim (64, 80 or 120) channels: x [batch][t][heads*head_dim]; q scaled by
+ * head_dim^-0.5 * log2(e) (one fp32 constant); q_out, k_out [batch][heads][t][head_dim],
+ * vt_out [batch][heads][head_dim][(t + 7) & ~7]. */
+int s3b_qkv_hd_f32(const float* x, const float* w, const float* b, int32_t batch, int32_t t, int32_t heads,
+                   int32_t head_dim, int32_t scheme, float* q_out, float* k_out, float* vt_out, void* stream);
 /* One conv of the feature extractor (Conv1d(512, 512, kw, stride 2), kw in {2, 3}) as the model runs it: implicit GEMM on
  * channels-last x [batch][lin][512], weight w [512][512][kw] (torch layout), optional bias [512], optional GELU, in
  * operand scheme `scheme`; out_fmt -1 = fp32 output, 0 / 1 = operand planes decoded to fp32.
@@ -238,7 +244,8 @@ int s3b_qkv_f32(const float* x, const float* w, const float* b, int32_t batch, i
 int s3b_conv_gemm_f32(const float* x, const float* w, const float* bias, int32_t batch, int64_t lin, int32_t kw,
                       int32_t gelu, int32_t scheme, int32_t out_fmt, float* out, void* stream);
 /* The positional conv as the model runs it (bf16x3): x [batch][t][d], folded weight w [d][d / groups][k], bias [d].
- *  taps_per_kblock 1: one k-block per tap, bias + GELU + residual in the GEMM epilogue, fp32 (then LayerNorm if gamma:
+ * d in {512, 768, 1024, 1280, 1920}; d / groups in {16, 32, 48, 64, 80, 120} (80 and 120: taps_per_kblock 1 only).
+ *  taps_per_kblock 1: one k-block per tap (two above 64 channels per group), bias + GELU + residual in the GEMM epilogue, fp32 (then LayerNorm if gamma:
  *    as in the model, operand planes come only from that LayerNorm, so out_fmt >= 0 needs gamma);
  *  taps_per_kblock 4: four taps per k-block (zero taps appended up to a multiple of 4) + the combine kernel, mode
  *    0 = x + GELU(conv + bias); 1 = data2vec block GELU(LayerNorm_noaffine(conv + bias)); 2 = x + the mode-1 value.
@@ -252,7 +259,7 @@ int s3b_posconv_f32(const float* x, const float* w, const float* bias, int32_t b
  * force_un in {0 = the library's choice, 128, 256} forces the CTA-pair tile width. out[0] = ms per launch,
  * out[1] = tile width used. (tools/gemm_tile_sweep.py) */
 int s3b_gemm_bench(int64_t m, int32_t n, int32_t k, int32_t gelu, int32_t force_un, int32_t iters, float* out);
-/* y = LayerNorm_D(x) (eps 1e-5), optional GELU; D in {512,768,1024,1280} */
+/* y = LayerNorm_D(x) (eps 1e-5), optional GELU; D in {512,768,1024,1280,1920} */
 int s3b_layernorm_f32(const float* x, int64_t m, int32_t d, const float* gamma, const float* beta, int32_t gelu,
                       float* out, void* stream);
 /* softmax(q k^T / 8 + key padding mask) v per (batch, head); q,k,v: [batch][T][heads*64] fp32; valid_frames: host,
@@ -266,7 +273,9 @@ int s3b_attention_f32(const float* q, const float* k, const float* v, const int3
  *  table_frames : frames the table is built for (0 = 4096, as s3b_model_finalize); must be >= t
  *  gate         : optional DEVICE fp32 [batch][heads][t] (needs rel_emb); NULL = 1
  *  ctx_format   : operand format the kernel writes the context in: 0 = bf16 hi/lo, 1 = f16q8 (fp16 + e4m3 residual);
- *                 out is decoded from those planes with the arithmetic the library's kernels read an operand back with */
+ *                 out is decoded from those planes with the arithmetic the library's kernels read an operand back with
+ *  head_dim     : channels per head, 64, 80 or 120 (0 = 64): q, k, v are [batch][t][heads*head_dim] and the scores are
+ *                 scaled by head_dim^-0.5; rel_emb needs 64 */
 typedef struct s3b_attention_opts {
     int32_t struct_size;
     int32_t ctx_format;
@@ -275,7 +284,7 @@ typedef struct s3b_attention_opts {
     int32_t max_distance;
     const float* gate;
     int32_t table_frames;
-    int32_t reserved32;
+    int32_t head_dim;
     int64_t reserved[2];
 } s3b_attention_opts;
 int s3b_attention_ex(const float* q, const float* k, const float* v, const int32_t* valid_frames, int32_t batch,

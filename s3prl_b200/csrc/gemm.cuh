@@ -29,7 +29,7 @@ struct GemmParams {
     int rows_per_batch;     // valid output rows per batch
     int tiles_m_per_batch;  // ceil(rows_per_batch / 128)
     int n_tiles;            // output column tiles
-    int umma_n;             // columns per tile (multiple of 16, <= 256)
+    int umma_n;             // columns per tile (multiple of 16, <= 256; 80 or 120 for the pos_conv's wide groups)
     int two_cta;            // 1: CTA-pair kernel (umma_n == 256, block_k == 64, B boxes hold umma_n/2 rows)
     int block_k;            // K elements per k-block: gemm_block_k(umma_n) (32 for 128x256 tiles, else 64); f16q8: 64
     int num_k_blocks;       // k-blocks per output tile
@@ -66,7 +66,8 @@ struct GemmParams {
     float* out_pre;  // optional: v BEFORE the residual add (fc2 output, "fairseq_layers_before_residual"), same layout
 
     // ---- epilogue, QKV scatter mode (qkv_mode != 0): columns [0,D) -> q*scale, [D,2D) -> k, [2D,3D) -> v
-    // q,k: [B][H][T][64] split bf16 ; v transposed: [B][H][64][Tp] split bf16. Flat row m = b*T + t.
+    // q,k: [B][H][T][hd] split bf16 ; v transposed: [B][H][hd][Tp] split bf16. Flat row m = b*T + t. hd (below) is
+    // the head width, 64, 80 or 120 (D = H * hd).
     // qkv_col0: the scatter column of GEMM column 0 (the Conformer runs [q | k] with 0 and v alone with 2D; `bias` then
     // points at the launch's own columns)
     int qkv_mode;
@@ -97,6 +98,9 @@ struct GemmParams {
     // loads 64-wide boxes but only the first 3 k-steps carry non-zero weights.
     int k_steps;
 
+    int hd;                 // QKV scatter: head width
+    unsigned int hd_magic;  // 2^32 / hd rounded up: column / hd = __umulhi(column, hd_magic) for columns < 2^16
+    int qk_head_step;       // (T - 1) * hd
 };
 
 // k-block width the kernel instantiation for this tile width uses (tensor-map boxes must match)

@@ -243,8 +243,9 @@ template <int BN, int kEpi, int kHalves>
 __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float (&acc)[kHalves][BN / 2], int batch,
                                               int row_base, int col0) {
     constexpr int kJ = BN / 8;               // column pairs per row
-    // pairs per chunk: 8, but 2 next to the 128 accumulators of a 256-wide cooperative tile (168 registers at most)
-    constexpr int kCh = BN * kHalves >= 256 && kHalves == 1 ? 2 : (kJ < 8 ? kJ : 8);
+    // pairs per chunk: 8, but 2 next to the 128 accumulators of a 256-wide cooperative tile (168 registers at most),
+    // and 5 at the pos_conv's 80- and 120-column tiles
+    constexpr int kCh = BN * kHalves >= 256 && kHalves == 1 ? 2 : (kJ < 8 ? kJ : (kJ % 8 == 0 ? 8 : 5));
     constexpr int kRows = 2 * kHalves;       // rows per thread
     static_assert(kJ % kCh == 0, "chunking");
     bool ok[kRows];
@@ -258,16 +259,18 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float (&acc)[
     const bool has_bias = p.bias != nullptr;
 
     if constexpr (kEpi == kEpiQkv) {
-        // m = b*T + t ; col = which*D + h*64 + d (column pairs never straddle a head)
-        //   q, k: [B][H][T][64] at (b*H*T + t)*64 + h*T*64 + d      v^T: [B][H][64][Tp] at b*H*64*Tp + t + (h*64 + d)*Tp
-        const int T = p.T, D = p.D;
+        // m = b*T + t ; col = which*D + h*hd + d (column pairs never straddle a head: hd is even)
+        //   q, k: [B][H][T][hd] at (b*H*T + t)*hd + h*T*hd + d      v^T: [B][H][hd][Tp] at b*H*hd*Tp + t + (h*hd + d)*Tp
+        // q / k column offset h*T*hd + d = within + h*(T-1)*hd, h = within / hd by a multiply-high with p.hd_magic
+        // (exact for within < 2^16), once per column pair; (T-1)*hd is the host's p.qk_head_step
+        const int T = p.T, D = p.D, hd = p.hd;
         size_t base_qk[kRows], base_v[kRows];
 #pragma unroll
         for (int s = 0; s < kRows; ++s) {
             const int b = (int)m[s] / T;
             const int t = (int)m[s] - b * T;
-            base_qk[s] = ((size_t)b * p.H * T + t) * 64;
-            base_v[s] = (size_t)b * p.H * 64 * p.Tp + t;
+            base_qk[s] = (size_t)(unsigned)(b * p.H * T + t) * (unsigned)hd;  // (b*H*T + t) <= B*T*H < 2^31
+            base_v[s] = (size_t)(unsigned)(b * D) * (unsigned)p.Tp + t;
         }
         const int qcol = col0 + p.qkv_col0;
         int which = qcol / D;
@@ -282,11 +285,11 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float (&acc)[
 #pragma unroll
             for (int jj = 0; jj < kCh; ++jj) {
                 const int j = c + jj;
-                const int h = within >> 6, d = within & 63;
+                const int h = (int)__umulhi((unsigned)within, p.hd_magic);
                 if (which < 2) {
                     __nv_bfloat16* dst_hi = which == 0 ? p.q_hi : p.k_hi;
                     __nv_bfloat16* dst_lo = which == 0 ? p.q_lo : p.k_lo;
-                    const int o_col = h * T * 64 + d;
+                    const int o_col = within + h * p.qk_head_step;
 #pragma unroll
                     for (int s = 0; s < kRows; ++s) {
                         if (!ok[s]) continue;
@@ -582,6 +585,8 @@ cudaError_t launch_gemm_bf16x3(const GemmParams& p, int sm_count, cudaStream_t s
         case 256: return launch_n<256>(p, sm_count, stream);
         case 192: return launch_n<192>(p, sm_count, stream);
         case 128: return launch_n<128>(p, sm_count, stream);
+        case 120: return p.two_cta ? cudaErrorInvalidValue : launch_n<120>(p, sm_count, stream);
+        case 80: return p.two_cta ? cudaErrorInvalidValue : launch_n<80>(p, sm_count, stream);
         case 64: return p.two_cta ? cudaErrorInvalidValue : launch_n<64>(p, sm_count, stream);
         case 48: return p.two_cta ? cudaErrorInvalidValue : launch_n<48>(p, sm_count, stream);
         case 32: return p.two_cta ? cudaErrorInvalidValue : launch_n<32>(p, sm_count, stream);

@@ -23,7 +23,7 @@ cudaError_t launch_conv0_layernorm(const float* x, int B, long long L, int L0, c
                                    const float* gamma, const float* beta, const OutPlanes& op, cudaStream_t s);
 
 // ---- norm.cu -------------------------------------------------------------------------------------
-// y = LayerNorm_D(x) * gamma + beta (eps 1e-5, biased var), optional GELU; D in {512, 768, 1024}.
+// y = LayerNorm_D(x) * gamma + beta (eps 1e-5, biased var), optional GELU; D in {512, 768, 1024, 1280, 1920}.
 // Any of out_f32 / (out_hi,out_lo) may be null. x and out_f32 may alias.
 cudaError_t launch_layernorm(const float* x, size_t M, int D, const float* gamma, const float* beta, int gelu,
                              float* out_f32, const OutPlanes& op, cudaStream_t s);
@@ -55,9 +55,9 @@ cudaError_t launch_wait_flags(const uint32_t* flags, int n, uint32_t seq, cudaSt
 
 // ---- attention.cu --------------------------------------------------------------------------------
 struct AttnParams {
-    CUtensorMap q_hi, q_lo;    // [B*H][T][64]  box {64, 128, 1}
-    CUtensorMap k_hi, k_lo;    // [B*H][T][64]  box {64,  64, 1}
-    CUtensorMap vt_hi, vt_lo;  // [B*H][64][Tp] (dim0 = T valid keys) box {64, 64, 1}
+    CUtensorMap q_hi, q_lo;    // [B*H][T][hd]  box {64, 128, 1}
+    CUtensorMap k_hi, k_lo;    // [B*H][T][hd]  box {64,  64, 1}
+    CUtensorMap vt_hi, vt_lo;  // [B*H][hd][Tp] (dim0 = T valid keys) box {64, hd, 1}
     int B, H, T, D;
     const int* kv_len;          // [B] valid (un-padded) key count, >= 1
     // optional WavLM gated relative position bias: S[q][k] += gate[b][h][q] * table[h][k - q + bias_center]
@@ -68,6 +68,7 @@ struct AttnParams {
     // optional timeline (debug): clock64 stamps of CTA `trace_block`, [2 roles][16 blocks][8 slots]
     long long* trace;
     int trace_block;
+    int hd;  // head width: 64, 80 or 120 (D = H * hd); the bias above needs 64
 };
 cudaError_t launch_attention(const AttnParams& p, cudaStream_t s);
 

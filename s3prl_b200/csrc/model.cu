@@ -316,17 +316,27 @@ static int default_scheme() {
     return S3B_DEFAULT_SCHEME;
 }
 
+// attention head widths the kernel is built for (attention.cu), and pos_conv group widths: multiples of 16 up to 64
+// (one 64-wide k-block per tap, or four taps per k-block), 80 and 120 (two k-blocks per tap, one tap per k-block)
+static bool head_dim_ok(int hd) { return hd == 64 || hd == 80 || hd == 120; }
+static bool posconv_cpg_ok(int cpg) { return (cpg % 16 == 0 && cpg >= 16 && cpg <= 64) || cpg == 80 || cpg == 120; }
+static int head_dim(const s3b_config& c) { return c.embed_dim / c.num_heads; }
+
 // ------------------------------------------------------------------------------------------------
 // C ABI: model lifetime
 // ------------------------------------------------------------------------------------------------
 extern "C" int s3b_model_create(const s3b_config* cfg, s3b_model** out) {
     if (!cfg || !out) return fail("null argument");
-    if (cfg->embed_dim % 128 != 0 || cfg->embed_dim > 1280) return fail("embed_dim must be a multiple of 128, <= 1280");
-    if (cfg->num_heads * 64 != cfg->embed_dim) return fail("head dim must be 64");
+    if (cfg->embed_dim % 128 != 0 || cfg->embed_dim > 1920) return fail("embed_dim must be a multiple of 128, <= 1920");
+    if (cfg->num_heads < 1 || cfg->embed_dim % cfg->num_heads != 0 || !head_dim_ok(cfg->embed_dim / cfg->num_heads))
+        return fail("head dim (embed_dim / num_heads = %d / %d) must be 64, 80 or 120", cfg->embed_dim, cfg->num_heads);
+    const int hd = cfg->embed_dim / cfg->num_heads;
     if (cfg->ffn_dim % 256 != 0) return fail("ffn_dim must be a multiple of 256");
-    if (cfg->embed_dim % cfg->pos_conv_groups != 0) return fail("embed_dim %% pos_conv_groups != 0");
+    if (cfg->pos_conv_groups < 1 || cfg->embed_dim % cfg->pos_conv_groups != 0)
+        return fail("embed_dim %% pos_conv_groups != 0");
     const int cpg = cfg->embed_dim / cfg->pos_conv_groups;
-    if (cpg % 16 != 0 || cpg > 64) return fail("channels per pos_conv group must be a multiple of 16, <= 64");
+    if (!posconv_cpg_ok(cpg))
+        return fail("channels per pos_conv group (embed_dim / pos_conv_groups = %d) must be 16, 32, 48, 64, 80 or 120", cpg);
     if (cfg->pos_conv_depth < 0 || cfg->pos_conv_depth > 8) return fail("pos_conv_depth out of range (0..8)");
     if (cfg->pos_conv_depth <= 1 && cfg->pos_conv_kernel % 2 != 0) return fail("pos_conv_kernel must be even");
     if (cfg->pos_conv_depth > 1 && (cfg->pos_conv_kernel < 3 || (4 * cpg != 192 && 4 * cpg != 256)))
@@ -342,6 +352,11 @@ extern "C" int s3b_model_create(const s3b_config* cfg, s3b_model** out) {
     if ((cfg->family == 3) != (cfg->no_feature_layer_norm != 0))
         return fail("the distiller family (3) and no_feature_layer_norm go together");
     if (cfg->conformer != 0 && cfg->conformer != 1) return fail("conformer must be 0 or 1");
+    // the rotary table, the WavLM gate (grep_linear [8][64]) and the relative bias are 64-wide per head
+    if (cfg->conformer && hd != 64)
+        return fail("conformer = 1 needs 64-wide heads: head dim (embed_dim / num_heads) is %d", hd);
+    if (cfg->family == 2 && hd != 64)
+        return fail("family 2 (wavlm) needs 64-wide heads: head dim (embed_dim / num_heads) is %d", hd);
     if (cfg->conformer) {
         if (cfg->family != 1) return fail("the Conformer encoder goes with the wav2vec2 family (1)");
         if (cfg->relative_position || cfg->pred_heads) return fail("the Conformer encoder has no WavLM bias or prediction heads");
@@ -547,20 +562,21 @@ static std::vector<float> conv_weight_layout(const float* w, int kw) {
             for (int j = 0; j < kw; ++j) r[((size_t)o * kw + j) * C + ci] = w[((size_t)o * C + ci) * kw + j];
     return r;
 }
-// grouped positional conv, folded weight w [D][cpg][Kp]. One tap per k-block (posconv_params):
-// B operand [group*Kp + tap][n = cpg][64 (zero padded)]
+// grouped positional conv, folded weight w [D][cpg][Kp]. One tap per k-block, or per two k-blocks above 64 channels
+// per group (posconv_params): B operand [group*Kp + tap][n = cpg][Kc = cpg rounded up to 64 (zero padded)]
+static int posconv_kc(int cpg) { return (cpg + 63) / 64 * 64; }
 static std::vector<float> posconv_weight_layout(const float* w, int D, int G, int Kp) {
-    const int cpg = D / G;
-    std::vector<float> wb((size_t)G * Kp * cpg * 64, 0.0f);
+    const int cpg = D / G, Kc = posconv_kc(cpg);
+    std::vector<float> wb((size_t)G * Kp * cpg * Kc, 0.0f);
     for (int g = 0; g < G; ++g)
         for (int k = 0; k < Kp; ++k)
             for (int n = 0; n < cpg; ++n)
                 for (int ci = 0; ci < cpg; ++ci)
-                    wb[(((size_t)g * Kp + k) * cpg + n) * 64 + ci] = w[((size_t)(g * cpg + n) * cpg + ci) * Kp + k];
+                    wb[(((size_t)g * Kp + k) * cpg + n) * Kc + ci] = w[((size_t)(g * cpg + n) * cpg + ci) * Kp + k];
     return wb;
 }
 // four taps per k-block (tap = 4q + j, posconv4_params), the tap count rounded up to K4 = a multiple of four with zero
-// taps: B operand [group*K4/4 + q][n = j*cpg + co][64 (zero padded)]
+// taps: B operand [group*K4/4 + q][n = j*cpg + co][64 (zero padded)]; cpg <= 64 (48 or 64 where it runs)
 static std::vector<float> posconv4_weight_layout(const float* w, int D, int G, int Kp) {
     const int cpg = D / G, K4 = (Kp + 3) / 4 * 4;
     std::vector<float> w4((size_t)G * K4 * cpg * 64, 0.0f);
@@ -662,7 +678,7 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
             for (int k = 0; k < Kp; ++k) wf[oc * Kp + k] = tv->data[oc * Kp + k] * scale[k];  // fp32, like torch's _weight_norm
         const std::vector<float> wb = posconv_weight_layout(wf.data(), D, G, Kp);
         S3B_OK(upload_split(m->pos_w, wb.data(), wb.size()));
-        if (Kp % 4 == 0) {
+        if (Kp % 4 == 0 && (4 * cpg == 192 || 4 * cpg == 256)) {  // the groups posconv4_ok can run four taps on
             const std::vector<float> w4 = posconv4_weight_layout(wf.data(), D, G, Kp);
             S3B_OK(upload_split(m->pos_w4, w4.data(), w4.size()));
         }
@@ -832,19 +848,22 @@ static void set_epi(GemmParams& p, const Epi& e, int ldo) {
     p.qkv_mode = 0;
 }
 
-// q pre-scaled by head_dim^-0.5 (exact power of two) and log2(e): the attention kernel's softmax runs on exp2
+// q pre-scaled by head_dim^-0.5 and log2(e): the attention kernel's softmax runs on exp2. For 64-wide heads that is
+// log2(e) / 8, exact but for the rounding of log2(e); for 80 and 120 the product is rounded to one fp32 constant.
 static const float kQScale = 0.125f * 1.4426950408889634f;
+static float q_scale(int hd) { return hd == 64 ? kQScale : (float)(1.4426950408889634 / sqrt((double)hd)); }
 
-// QKV epilogue of a [B*T][3D] linear: bias, then q (scaled), k as [B][H][T][64] and v transposed as [B][H][64][Tp]
+// QKV epilogue of a [B*T][3D] linear: bias, then q (scaled), k as [B][H][T][hd] and v transposed as [B][H][hd][Tp]
 // (Tp = T rounded up to 8), all as bf16 hi/lo planes. col0: the QKV column of the launch's first column (a launch
 // covering only [k | v] or v), `bias` then starts at that column.
-static void set_qkv_epi(GemmParams& p, const float* bias, int T, int H, const SplitBuf& q, const SplitBuf& k,
+static void set_qkv_epi(GemmParams& p, const float* bias, int T, int H, int hd, const SplitBuf& q, const SplitBuf& k,
                         const SplitBuf& vt, int col0 = 0) {
-    const int D = H * 64;
+    const int D = H * hd;
     Epi e;
     e.bias = bias;
     set_epi(p, e, 3 * D);
-    p.qkv_mode = 1, p.T = T, p.Tp = (T + 7) & ~7, p.H = H, p.D = D, p.q_scale = kQScale, p.qkv_col0 = col0;
+    p.qkv_mode = 1, p.T = T, p.Tp = (T + 7) & ~7, p.H = H, p.D = D, p.q_scale = q_scale(hd), p.qkv_col0 = col0;
+    p.hd = hd, p.hd_magic = 0xFFFFFFFFu / (unsigned)hd + 1u, p.qk_head_step = (T - 1) * hd;
     p.q_hi = q.h(), p.q_lo = q.l(), p.k_hi = k.h(), p.k_lo = k.l();
     p.vt_hi = vt.h(), p.vt_lo = vt.l();
 }
@@ -987,17 +1006,20 @@ static int pos_taps(const s3b_config& c) {
 }
 static int pos_taps4(const s3b_config& c) { return (pos_taps(c) + 3) / 4 * 4; }
 
-// grouped positional conv: one k-block per tap; A row coordinate = t + tap - K/2 (TMA zero-fills t<0, t>=T)
+// grouped positional conv: one k-block per tap; A row coordinate = t + tap - K/2 (TMA zero-fills t<0, t>=T).
+// Groups of 80 and 120 channels take two 64-wide k-blocks per tap: the A box of the second reads on into the next
+// group's channels (or, for the last group, past D: TMA zero fill), which meet the zero-padded weights of posconv_kc.
+// The tile is exactly the group's cpg columns wide, so no output column lands in a neighbouring group.
 static int posconv_params(GemmParams& p, const s3b_config& c, const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo,
                           const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, int B, int T) {
     memset(&p, 0, sizeof(p));
-    const int D = c.embed_dim, G = c.pos_conv_groups, cpg = D / G, Kp = c.pos_conv_kernel;
+    const int D = c.embed_dim, G = c.pos_conv_groups, cpg = D / G, Kp = c.pos_conv_kernel, Kc = posconv_kc(cpg);
     TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, x_hi, D, T, B, D, (uint64_t)T * D, 64, 128));
     TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, x_lo, D, T, B, D, (uint64_t)T * D, 64, 128));
-    TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, w_hi, 64, cpg, (uint64_t)G * Kp, 64, (uint64_t)cpg * 64, 64, cpg));
-    TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, w_lo, 64, cpg, (uint64_t)G * Kp, 64, (uint64_t)cpg * 64, 64, cpg));
+    TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, w_hi, Kc, cpg, (uint64_t)G * Kp, Kc, (uint64_t)cpg * Kc, 64, cpg));
+    TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, w_lo, Kc, cpg, (uint64_t)G * Kp, Kc, (uint64_t)cpg * Kc, 64, cpg));
     p.batches = B, p.rows_per_batch = T, p.tiles_m_per_batch = (T + 127) / 128;
-    p.n_tiles = G, p.umma_n = cpg, p.block_k = 64, p.num_k_blocks = Kp, p.kb_per_row = 1;
+    p.n_tiles = G, p.umma_n = cpg, p.block_k = 64, p.num_k_blocks = Kp * (Kc / 64), p.kb_per_row = Kc / 64;
     p.a_row_step = 1, p.a_row_off = -(Kp / 2), p.a_k_per_ntile = cpg, p.b_n_tiled = 0, p.b_z_per_ntile = Kp;
     p.out_rows_per_batch = T;
     p.alg_flops = 2.0 * (double)B * T * D * cpg * Kp;
@@ -1281,7 +1303,7 @@ int Fwd::prepare() {
     S3B_OK(w->ctx_s.ensure((size_t)M * D));
     S3B_OK(w->q_s.ensure((size_t)M * D));
     S3B_OK(w->k_s.ensure((size_t)M * D));
-    S3B_OK(w->vt_s.ensure((size_t)B * H * 64 * Tp));
+    S3B_OK(w->vt_s.ensure((size_t)D * B * Tp));
     S3B_OK(w->h_s.ensure((size_t)M * F));
     if (c.conformer) S3B_OK(w->glu_f32.ensure((size_t)M * 2 * D * sizeof(float)));
     else if (posconv4_ok(c)) S3B_OK(w->pos_z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
@@ -1324,18 +1346,26 @@ int Fwd::prepare() {
     return 0;
 }
 
-// the attention kernel's view of a lane's q / k / v^T planes (QKV scatter epilogue) and its context output
-static int attn_params(AttnParams& ap, const Workspace* w, int B, int T, int H, const int* d_kv, int scheme) {
+// The attention kernel's view of q / k / v^T planes as the QKV scatter writes them (q, k [B*H][T][hd], v^T
+// [B*H][hd][Tp]): Q and K rows as 64-wide boxes, the last one reading past hd into TMA zero fill.
+static int attn_tmaps(AttnParams& ap, const SplitBuf& q, const SplitBuf& k, const SplitBuf& vt, int B, int T, int H,
+                      int hd) {
     const uint64_t BH = (uint64_t)B * H;
     const int Tp = (T + 7) & ~7;
+    TMAP_OK(encode_tmap_bf16_3d(&ap.q_hi, q.h(), hd, T, BH, hd, (uint64_t)T * hd, 64, 128));
+    TMAP_OK(encode_tmap_bf16_3d(&ap.q_lo, q.l(), hd, T, BH, hd, (uint64_t)T * hd, 64, 128));
+    TMAP_OK(encode_tmap_bf16_3d(&ap.k_hi, k.h(), hd, T, BH, hd, (uint64_t)T * hd, 64, 64));
+    TMAP_OK(encode_tmap_bf16_3d(&ap.k_lo, k.l(), hd, T, BH, hd, (uint64_t)T * hd, 64, 64));
+    TMAP_OK(encode_tmap_bf16_3d(&ap.vt_hi, vt.h(), T, hd, BH, Tp, (uint64_t)hd * Tp, 64, hd));
+    TMAP_OK(encode_tmap_bf16_3d(&ap.vt_lo, vt.l(), T, hd, BH, Tp, (uint64_t)hd * Tp, 64, hd));
+    ap.B = B, ap.H = H, ap.T = T, ap.D = H * hd, ap.hd = hd;
+    return 0;
+}
+
+// the attention kernel's view of a lane's q / k / v^T planes (QKV scatter epilogue) and its context output
+static int attn_params(AttnParams& ap, const Workspace* w, int B, int T, int H, int hd, const int* d_kv, int scheme) {
     memset(&ap, 0, sizeof(ap));
-    TMAP_OK(encode_tmap_bf16_3d(&ap.q_hi, w->q_s.h(), 64, T, BH, 64, (uint64_t)T * 64, 64, 128));
-    TMAP_OK(encode_tmap_bf16_3d(&ap.q_lo, w->q_s.l(), 64, T, BH, 64, (uint64_t)T * 64, 64, 128));
-    TMAP_OK(encode_tmap_bf16_3d(&ap.k_hi, w->k_s.h(), 64, T, BH, 64, (uint64_t)T * 64, 64, 64));
-    TMAP_OK(encode_tmap_bf16_3d(&ap.k_lo, w->k_s.l(), 64, T, BH, 64, (uint64_t)T * 64, 64, 64));
-    TMAP_OK(encode_tmap_bf16_3d(&ap.vt_hi, w->vt_s.h(), T, 64, BH, Tp, (uint64_t)64 * Tp, 64, 64));
-    TMAP_OK(encode_tmap_bf16_3d(&ap.vt_lo, w->vt_s.l(), T, 64, BH, Tp, (uint64_t)64 * Tp, 64, 64));
-    ap.B = B, ap.H = H, ap.T = T, ap.D = H * 64;
+    S3B_OK(attn_tmaps(ap, w->q_s, w->k_s, w->vt_s, B, T, H, hd));
     ap.kv_len = d_kv;
     ap.ctx = w->ctx_s.planes(scheme);
     return 0;
@@ -1365,12 +1395,12 @@ int Fwd::build_conformer_layer(LayerPlan& lp, int l) {
     {   // [q | k] from rope(LN(r1)), v from LN(r1)
         GemmParams& p = lp.qkv;
         S3B_OK(linear_params(p, w->x1_s, W.qkv, M, 2 * D, D, 1, sch));
-        set_qkv_epi(p, W.qkv_b.as<float>(), T, H, w->q_s, w->k_s, w->vt_s, 0);
+        set_qkv_epi(p, W.qkv_b.as<float>(), T, H, 64, w->q_s, w->k_s, w->vt_s, 0);
         GemmParams& pv = lp.v;
         S3B_OK(linear_params(pv, w->xs_s, W.v, M, D, D, 1, sch));
-        set_qkv_epi(pv, W.qkv_b.as<float>() + 2 * D, T, H, w->q_s, w->k_s, w->vt_s, 2 * D);
+        set_qkv_epi(pv, W.qkv_b.as<float>() + 2 * D, T, H, 64, w->q_s, w->k_s, w->vt_s, 2 * D);
     }
-    S3B_OK(attn_params(lp.attn, w, B, T, H, d_kv, sch));
+    S3B_OK(attn_params(lp.attn, w, B, T, H, 64, d_kv, sch));
     {   // r2 = r1 + linear_out(attn)
         GemmParams& p = lp.out;
         S3B_OK(linear_params(p, w->ctx_s, W.out, M, D, D, 0, sch));
@@ -1480,9 +1510,9 @@ int Fwd::build_plan(Plan& pl) {
         {   // QKV projection, scattered per head
             GemmParams& p = lp.qkv;
             S3B_OK(linear_params(p, w->xs_s, W.qkv, M, 3 * D, D, 1, m->scheme));
-            set_qkv_epi(p, W.qkv_b.as<float>(), T, H, w->q_s, w->k_s, w->vt_s);
+            set_qkv_epi(p, W.qkv_b.as<float>(), T, H, head_dim(c), w->q_s, w->k_s, w->vt_s);
         }
-        S3B_OK(attn_params(lp.attn, w, B, T, H, d_kv, m->scheme));
+        S3B_OK(attn_params(lp.attn, w, B, T, H, head_dim(c), d_kv, m->scheme));
         if (c.relative_position) set_rel_bias(lp.attn, m->rel_table.as<float>(), m->rel_table_T, w->gate.as<float>());
         {   // out_proj + residual (residual = hidden state l, patched per call)
             GemmParams& p = lp.out;
@@ -2318,11 +2348,12 @@ extern "C" int s3b_linear_f32(const float* a, const float* w, const float* bias,
     return s3b_linear_ex(a, w, bias, residual, M, N, K, gelu, nullptr, out, stream);
 }
 
-extern "C" int s3b_qkv_f32(const float* x, const float* w, const float* b, int32_t B, int32_t T, int32_t H,
-                           int32_t scheme, float* q_out, float* k_out, float* vt_out, void* stream) {
+extern "C" int s3b_qkv_hd_f32(const float* x, const float* w, const float* b, int32_t B, int32_t T, int32_t H,
+                              int32_t hd, int32_t scheme, float* q_out, float* k_out, float* vt_out, void* stream) {
     if (!x || !w || !b || !q_out || !k_out || !vt_out) return fail("null argument");
     if (B < 1 || T < 1 || H < 1) return fail("bad sizes");
-    const int D = H * 64, Tp = (T + 7) & ~7;
+    if (!head_dim_ok(hd)) return fail("head_dim must be 64, 80 or 120, not %d", hd);
+    const int D = H * hd, Tp = (T + 7) & ~7;
     const int64_t M = (int64_t)B * T;
     int sch = 0;
     S3B_OK(resolve_scheme(scheme, D, 3 * D, &sch));
@@ -2336,19 +2367,24 @@ extern "C" int s3b_qkv_f32(const float* x, const float* w, const float* b, int32
         S3B_OK(split_operand(w, ws, (size_t)3 * D * D, sch, 1, st));
         S3B_OK(qs.ensure((size_t)M * D));
         S3B_OK(ks.ensure((size_t)M * D));
-        S3B_OK(vts.ensure((size_t)B * H * 64 * Tp));
+        S3B_OK(vts.ensure((size_t)B * D * Tp));
         GemmParams p;
         S3B_OK(linear_params(p, xs, ws, M, 3 * D, D, 1, sch));
-        set_qkv_epi(p, b, T, H, qs, ks, vts);
+        set_qkv_epi(p, b, T, H, hd, qs, ks, vts);
         CUDA_OK(launch_gemm_bf16x3(p, sms, st));
         CUDA_OK(launch_planes_to_f32(qs.planes(0), (size_t)M * D, q_out, st));
         CUDA_OK(launch_planes_to_f32(ks.planes(0), (size_t)M * D, k_out, st));
-        CUDA_OK(launch_planes_to_f32(vts.planes(0), (size_t)B * H * 64 * Tp, vt_out, st));
+        CUDA_OK(launch_planes_to_f32(vts.planes(0), (size_t)B * D * Tp, vt_out, st));
         CUDA_OK(cudaStreamSynchronize(st));
         return 0;
     }();
     xs.release(), ws.release(), qs.release(), ks.release(), vts.release();
     return r;
+}
+
+extern "C" int s3b_qkv_f32(const float* x, const float* w, const float* b, int32_t B, int32_t T, int32_t H,
+                           int32_t scheme, float* q_out, float* k_out, float* vt_out, void* stream) {
+    return s3b_qkv_hd_f32(x, w, b, B, T, H, 64, scheme, q_out, k_out, vt_out, stream);
 }
 
 extern "C" int s3b_conv_gemm_f32(const float* x, const float* w, const float* bias, int32_t B, int64_t Lin, int32_t kw,
@@ -2396,10 +2432,11 @@ extern "C" int s3b_posconv_f32(const float* x, const float* w, const float* bias
                                int32_t out_fmt, float* out, void* stream) {
     if (!x || !w || !bias || !out || (gamma == nullptr) != (beta == nullptr)) return fail("null argument");
     if (B < 1 || T < 1) return fail("bad sizes");
-    if (D != 512 && D != 768 && D != 1024 && D != 1280) return fail("d must be 512, 768, 1024 or 1280, not %d", D);
+    if (D != 512 && D != 768 && D != 1024 && D != 1280 && D != 1920)
+        return fail("d must be 512, 768, 1024, 1280 or 1920, not %d", D);
     if (G < 1 || D % G != 0) return fail("d %d is not a multiple of groups %d", D, G);
     const int cpg = D / G;
-    if (cpg % 16 != 0 || cpg > 64) return fail("channels per group must be a multiple of 16, <= 64 (got %d)", cpg);
+    if (!posconv_cpg_ok(cpg)) return fail("channels per group must be 16, 32, 48, 64, 80 or 120 (got %d)", cpg);
     if (taps != 1 && taps != 4) return fail("taps_per_kblock must be 1 or 4, not %d", taps);
     if (mode < 0 || mode > 2) return fail("mode must be 0, 1 or 2, not %d", mode);
     if (k < 2) return fail("kernel size %d < 2", k);
@@ -2540,6 +2577,9 @@ extern "C" int s3b_attention_ex(const float* q, const float* k, const float* v, 
     }
     if (o.ctx_format != 0 && o.ctx_format != 1) return fail("ctx_format must be 0 (bf16 hi/lo) or 1 (f16q8)");
     if (o.gate != nullptr && o.rel_emb == nullptr) return fail("a gate needs rel_emb");
+    const int hd = o.head_dim != 0 ? o.head_dim : 64;
+    if (!head_dim_ok(hd)) return fail("head_dim must be 64, 80 or 120 (0 = 64), not %d", o.head_dim);
+    if (hd != 64 && o.rel_emb != nullptr) return fail("the relative position bias (rel_emb) needs head_dim 64");
     const int table_T = o.table_frames != 0 ? o.table_frames : 4096;  // s3b_model_finalize's table
     if (o.rel_emb != nullptr) {
         if (o.num_buckets < 4 || o.max_distance <= o.num_buckets / 4)
@@ -2549,27 +2589,22 @@ extern "C" int s3b_attention_ex(const float* q, const float* k, const float* v, 
     for (int b = 0; b < B; ++b)
         if (valid_frames[b] < 1 || valid_frames[b] > T) return fail("valid_frames[%d] = %d not in [1, %d]", b, valid_frames[b], T);
     cudaStream_t st = (cudaStream_t)stream;
-    const int D = H * 64, Tp = (T + 7) & ~7;
+    const int D = H * hd, Tp = (T + 7) & ~7;
     const size_t M = (size_t)B * T;
     SplitBuf qs, ks, vts, ctx;
     DevBuf kv, table;
     S3B_OK(qs.ensure(M * D));
     S3B_OK(ks.ensure(M * D));
-    S3B_OK(vts.ensure((size_t)B * H * 64 * Tp));
+    S3B_OK(vts.ensure((size_t)B * D * Tp));
     S3B_OK(ctx.ensure(M * D));
     S3B_OK(kv.ensure(B * sizeof(int)));
     CUDA_OK(cudaMemcpyAsync(kv.p, valid_frames, B * sizeof(int), cudaMemcpyHostToDevice, st));
-    CUDA_OK(launch_qkv_scatter(q, k, v, B, T, Tp, H, kQScale, qs.h(), qs.l(), ks.h(), ks.l(), vts.h(), vts.l(), st));
+    CUDA_OK(launch_qkv_scatter(q, k, v, B, T, Tp, H, hd, q_scale(hd), qs.h(), qs.l(), ks.h(), ks.l(), vts.h(), vts.l(),
+                               st));
     AttnParams ap;
     memset(&ap, 0, sizeof(ap));
-    const uint64_t BH = (uint64_t)B * H;
-    TMAP_OK(encode_tmap_bf16_3d(&ap.q_hi, qs.h(), 64, T, BH, 64, (uint64_t)T * 64, 64, 128));
-    TMAP_OK(encode_tmap_bf16_3d(&ap.q_lo, qs.l(), 64, T, BH, 64, (uint64_t)T * 64, 64, 128));
-    TMAP_OK(encode_tmap_bf16_3d(&ap.k_hi, ks.h(), 64, T, BH, 64, (uint64_t)T * 64, 64, 64));
-    TMAP_OK(encode_tmap_bf16_3d(&ap.k_lo, ks.l(), 64, T, BH, 64, (uint64_t)T * 64, 64, 64));
-    TMAP_OK(encode_tmap_bf16_3d(&ap.vt_hi, vts.h(), T, 64, BH, Tp, (uint64_t)64 * Tp, 64, 64));
-    TMAP_OK(encode_tmap_bf16_3d(&ap.vt_lo, vts.l(), T, 64, BH, Tp, (uint64_t)64 * Tp, 64, 64));
-    ap.B = B, ap.H = H, ap.T = T, ap.D = D, ap.kv_len = kv.as<int>();
+    S3B_OK(attn_tmaps(ap, qs, ks, vts, B, T, H, hd));
+    ap.kv_len = kv.as<int>();
     if (o.rel_emb != nullptr) {
         S3B_OK(table.ensure((size_t)H * (2 * (size_t)table_T - 1) * 4));
         CUDA_OK(launch_wavlm_rel_table(o.rel_emb, o.num_buckets, o.max_distance, H, table_T, table.as<float>(), st));

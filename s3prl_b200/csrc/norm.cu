@@ -63,6 +63,7 @@ cudaError_t launch_layernorm(const float* x, size_t M, int D, const float* gamma
         case 768: e = launch_pdl(layernorm_kernel<6>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
         case 1024: e = launch_pdl(layernorm_kernel<8>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
         case 1280: e = launch_pdl(layernorm_kernel<10>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
+        case 1920: e = launch_pdl(layernorm_kernel<15>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
         default: return cudaErrorInvalidValue;
     }
     return e;

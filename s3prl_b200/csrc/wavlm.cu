@@ -123,31 +123,31 @@ cudaError_t launch_wavlm_gate(const OutPlanes& xp, size_t M, int B, int T, int H
 }
 
 __global__ void qkv_scatter_kernel(const float* __restrict__ q, const float* __restrict__ k,
-                                   const float* __restrict__ v, int B, int T, int Tp, int H, float q_scale,
+                                   const float* __restrict__ v, int B, int T, int Tp, int H, int hd, float q_scale,
                                    __nv_bfloat16* q_hi, __nv_bfloat16* q_lo, __nv_bfloat16* k_hi,
                                    __nv_bfloat16* k_lo, __nv_bfloat16* vt_hi, __nv_bfloat16* vt_lo) {
-    const int D = H * 64;
+    const int D = H * hd;
     const size_t n = (size_t)B * T * D;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
         const size_t m = i / D;
         const int col = (int)(i - m * D);
         const int b = (int)(m / T), t = (int)(m - (size_t)b * T);
-        const int h = col >> 6, d = col & 63;
+        const int h = col / hd, d = col - h * hd;
         const size_t bh = (size_t)b * H + h;
         __nv_bfloat16 hi, lo;
         split_bf16(q[i] * q_scale, hi, lo);
-        q_hi[(bh * T + t) * 64 + d] = hi, q_lo[(bh * T + t) * 64 + d] = lo;
+        q_hi[(bh * T + t) * hd + d] = hi, q_lo[(bh * T + t) * hd + d] = lo;
         split_bf16(k[i], hi, lo);
-        k_hi[(bh * T + t) * 64 + d] = hi, k_lo[(bh * T + t) * 64 + d] = lo;
+        k_hi[(bh * T + t) * hd + d] = hi, k_lo[(bh * T + t) * hd + d] = lo;
         split_bf16(v[i], hi, lo);
-        vt_hi[(bh * 64 + d) * (size_t)Tp + t] = hi, vt_lo[(bh * 64 + d) * (size_t)Tp + t] = lo;
+        vt_hi[(bh * hd + d) * (size_t)Tp + t] = hi, vt_lo[(bh * hd + d) * (size_t)Tp + t] = lo;
     }
 }
 
-cudaError_t launch_qkv_scatter(const float* q, const float* k, const float* v, int B, int T, int Tp, int H,
+cudaError_t launch_qkv_scatter(const float* q, const float* k, const float* v, int B, int T, int Tp, int H, int hd,
                                float q_scale, __nv_bfloat16* q_hi, __nv_bfloat16* q_lo, __nv_bfloat16* k_hi,
                                __nv_bfloat16* k_lo, __nv_bfloat16* vt_hi, __nv_bfloat16* vt_lo, cudaStream_t s) {
-    qkv_scatter_kernel<<<132 * 4, 256, 0, s>>>(q, k, v, B, T, Tp, H, q_scale, q_hi, q_lo, k_hi, k_lo, vt_hi, vt_lo);
+    qkv_scatter_kernel<<<132 * 4, 256, 0, s>>>(q, k, v, B, T, Tp, H, hd, q_scale, q_hi, q_lo, k_hi, k_lo, vt_hi, vt_lo);
     return cudaGetLastError();
 }
 

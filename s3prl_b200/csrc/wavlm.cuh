@@ -21,9 +21,9 @@ cudaError_t launch_wavlm_rel_table(const float* emb /*[num_buckets][H] device*/,
 cudaError_t launch_wavlm_gate(const OutPlanes& xp, size_t M, int B, int T, int H, int D, const float* grep_w,
                               const float* grep_b, const float* grep_a, float* gate, cudaStream_t s);
 
-// test helpers: fp32 [B][T][H*64] q/k/v -> the attention kernel's operand layout; n (even) elements of an operand in
+// test helpers: fp32 [B][T][H*hd] q/k/v -> the attention kernel's operand layout; n (even) elements of an operand in
 // either format -> fp32
-cudaError_t launch_qkv_scatter(const float* q, const float* k, const float* v, int B, int T, int Tp, int H,
+cudaError_t launch_qkv_scatter(const float* q, const float* k, const float* v, int B, int T, int Tp, int H, int hd,
                                float q_scale, __nv_bfloat16* q_hi, __nv_bfloat16* q_lo, __nv_bfloat16* k_hi,
                                __nv_bfloat16* k_lo, __nv_bfloat16* vt_hi, __nv_bfloat16* vt_lo, cudaStream_t s);
 cudaError_t launch_planes_to_f32(const OutPlanes& p, size_t n, float* out, cudaStream_t s);

@@ -46,6 +46,7 @@ EXPORTED_SYMBOLS = [
     "s3b_linear_f32",
     "s3b_linear_ex",
     "s3b_qkv_f32",
+    "s3b_qkv_hd_f32",
     "s3b_conv_gemm_f32",
     "s3b_posconv_f32",
     "s3b_layernorm_f32",
@@ -124,7 +125,7 @@ class S3BAttentionOpts(C.Structure):
         ("max_distance", C.c_int32),
         ("gate", C.c_void_p),
         ("table_frames", C.c_int32),
-        ("reserved32", C.c_int32),
+        ("head_dim", C.c_int32),
         ("reserved", C.c_int64 * 2),
     ]
 
@@ -215,6 +216,7 @@ def load() -> C.CDLL:
     lib.s3b_linear_f32.argtypes = [f32p, f32p, f32p, f32p, i64, i32, i32, i32, f32p, vp]
     lib.s3b_linear_ex.argtypes = [f32p, f32p, f32p, f32p, i64, i32, i32, i32, C.POINTER(S3BLinearOpts), f32p, vp]
     lib.s3b_qkv_f32.argtypes = [f32p, f32p, f32p, i32, i32, i32, i32, f32p, f32p, f32p, vp]
+    lib.s3b_qkv_hd_f32.argtypes = [f32p, f32p, f32p, i32, i32, i32, i32, i32, f32p, f32p, f32p, vp]
     lib.s3b_conv_gemm_f32.argtypes = [f32p, f32p, f32p, i32, i64, i32, i32, i32, i32, f32p, vp]
     lib.s3b_posconv_f32.argtypes = [f32p, f32p, f32p, i32, i32, i32, i32, i32, i32, i32, f32p, f32p, i32, f32p, vp]
     lib.s3b_gemm_bench.argtypes = [i64, i32, i32, i32, i32, i32, C.POINTER(C.c_float)]

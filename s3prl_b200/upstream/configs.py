@@ -126,6 +126,18 @@ for _alias, _arch in {
 ARCHS["wav2vec2_conformer_rope"] = replace(
     _BASE, family="wav2vec2", **_LL60K, layer_type="conformer", pos_enc_type="rope", attn_type="espnet"
 )
+# XLS-R 1B and 2B (s3prl/upstream/wav2vec2/hubconf.py xls_r_1b / xls_r_2b: wav2vec2_custom on the released files):
+# the LibriLight-large options with 48 layers and 80- / 120-wide heads. The values are those of fairseq's public XLS-R
+# configs; they were NOT checked against the released checkpoints (not reachable offline). A real checkpoint loaded
+# through wav2vec2_local / wav2vec2_custom carries its own cfg (arch_from_reference_cfg); this table shapes fabricated
+# checkpoints. It is kept apart from ARCHS, whose every key is a hub entry: these models are reached through
+# wav2vec2_local / wav2vec2_custom / wav2vec2_url, or UpstreamExpert(arch=XLS_R[...]).
+XLS_R: Dict[str, ArchConfig] = {
+    "xls_r_1b": replace(_BASE, family="wav2vec2", **dict(_LL60K, encoder_layers=48, encoder_embed_dim=1280,
+                                                         encoder_ffn_embed_dim=5120, encoder_attention_heads=16)),
+    "xls_r_2b": replace(_BASE, family="wav2vec2", **dict(_LL60K, encoder_layers=48, encoder_embed_dim=1920,
+                                                         encoder_ffn_embed_dim=7680, encoder_attention_heads=16)),
+}
 ALIASES = {
     "hubert": "hubert_base",
     "hubert_large": "hubert_large_ll60k",
