@@ -178,9 +178,24 @@ void s3b_peer_destroy(s3b_peer* p);
 /* fbank baseline upstream (s3prl/upstream/baseline/expert.py:69-79 over torchaudio.compliance.kaldi.fbank,
  * fbank.yaml: 80 mel bins, 25 ms / 10 ms, log; + 2 x ComputeDeltas(5) + per-utterance CMVN).
  *  wavs : host array of `batch` DEVICE pointers (fp32, un-padded), lens : host array of lengths
- *  out  : DEVICE buffer [batch][s3b_fbank_num_frames(max(lens))][240] fp32, zero beyond each utterance's frames */
+ *  out  : DEVICE buffer [batch][s3b_fbank_num_frames(max(lens))][240] fp32, zero beyond each utterance's frames
+ *  Every lens[b] must be >= 0. */
 int64_t s3b_fbank_num_frames(int64_t len);
 int s3b_fbank(const float* const* wavs, const int64_t* lens, int32_t batch, float* out, void* stream);
+
+/* Options of s3b_fbank_ex / s3b_melspec_ex (zero-initialise, set struct_size = sizeof(s3b_spectral_opts)).
+ *  cmvn : 1 = per-utterance CMVN, as s3b_fbank / s3b_melspec (the fbank, mel and linear entries);
+ *         0 = the features before CMVN (fbank: the fbank_no_cmvn entry, s3prl/upstream/baseline/fbank_no_cmvn.yaml)
+ *  opts NULL is cmvn = 1. */
+typedef struct s3b_spectral_opts {
+    int32_t struct_size;
+    int32_t cmvn;
+    int64_t reserved[3];
+} s3b_spectral_opts;
+/* s3b_fbank with options. cmvn = 0: out holds [log-mel | delta | delta-delta] before CMVN, zero beyond each
+ * utterance's frames. */
+int s3b_fbank_ex(const float* const* wavs, const int64_t* lens, int32_t batch, const s3b_spectral_opts* opts,
+                 float* out, void* stream);
 
 /* mel / linear baseline upstreams (s3prl/upstream/baseline/expert.py:52-79 over OnlinePreprocessor.forward,
  * s3prl/upstream/baseline/preprocessor.py:150-223; mel.yaml / linear.yaml). The host side (Python, like the
@@ -188,10 +203,18 @@ int s3b_fbank(const float* const* wavs, const int64_t* lens, int32_t batch, floa
  *  s3b_trimmed_lengths: out[b] = (index of the last non-zero sample) + 1, or lens[b] if all zero (synchronous).
  *  s3b_melspec: STFT power (n_fft 400, hop 160, hann, center/reflect over the row padded to `padded_len`) ->
  *    mel != 0: 80-bin HTK mel, else 201 linear bins -> log(x + 1e-10) -> CMVN over the first feats_len[b] frames
- *    -> first final_len[b] frames kept, zero up to t_out. out: DEVICE [batch][t_out][80 | 201] fp32. */
+ *    -> first final_len[b] frames kept, zero up to t_out. out: DEVICE [batch][t_out][80 | 201] fp32.
+ *    Refused: lens[b] < 0 (s3b_trimmed_lengths); trimmed_lens[b] outside [0, padded_len], feats_len[b] outside
+ *    [0, 1 + padded_len / 160], final_len[b] outside [0, t_out] (s3b_melspec). */
 int s3b_trimmed_lengths(const float* const* wavs, const int64_t* lens, int32_t batch, int64_t* out);
 int s3b_melspec(const float* const* wavs, const int64_t* trimmed_lens, int32_t batch, int64_t padded_len, int32_t mel,
                 const int32_t* feats_len, const int32_t* final_len, int32_t t_out, float* out, void* stream);
+/* s3b_melspec with options. cmvn = 0: out is DEVICE [batch][1 + padded_len / 160][80 | 201], the log features of
+ * every frame of the padded batch (the reference's feat before the per-utterance cut); feats_len, final_len and t_out
+ * are then unused and may be NULL / 0. */
+int s3b_melspec_ex(const float* const* wavs, const int64_t* trimmed_lens, int32_t batch, int64_t padded_len,
+                   int32_t mel, const int32_t* feats_len, const int32_t* final_len, int32_t t_out,
+                   const s3b_spectral_opts* opts, float* out, void* stream);
 
 /* Building blocks exposed for parity tests (device pointers, fp32) -------------------------------------- */
 /* out[M][N] = act(A[M][K] * W[N][K]^T + bias[N]) (+ residual[M][N]); K % 64 == 0, N % 16 == 0.

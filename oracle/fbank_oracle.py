@@ -99,7 +99,9 @@ def spectrogram_forward(wavs: Sequence[torch.Tensor], feat_type: str = "mel") ->
     for w in wavs:  # last non-zero sample + 1 (the whole thing if all zero), preprocessor.py:166-175
         nz = w.nonzero()
         trimmed.append(len(w) if len(nz) == 0 else int(nz[:, -1].max()) + 1)
-    x = torch.nn.utils.rnn.pad_sequence([w[:n].float() for w, n in zip(wavs, trimmed)], batch_first=True)
+    # the reference's trim slices the channel axis of a [1, L] row (preprocessor.py:176-182): the batch keeps its
+    # original padding, and only feats_len below sees the trimmed lengths
+    x = torch.nn.utils.rnn.pad_sequence([w.float() for w in wavs], batch_first=True)
     spec = torch.stft(x, n_fft=400, hop_length=160, win_length=400, window=torch.hann_window(400), center=True,
                       pad_mode="reflect", normalized=False, onesided=True, return_complex=True)
     feat = spec.abs().pow(2)  # [B, 201, n_frames]

@@ -194,6 +194,43 @@ def make_spectrogram_fixture():
     torch.save(out, GOLDEN / "spectrogram.pt")
 
 
+# structured inputs (recipes in tests/spectral_ref.py): each keeps a specific error alive through CMVN
+SPECTRAL_FBANK = [("chirp", 6400, "none"), ("pink", 6401, "none"), ("bursts", 4800, "none"), ("dc", 2000, "none"),
+                  ("tone_fbank_half", 720, "none"), ("impulses", 560, "none"), ("brown", 401, "none"),
+                  ("int16", 400, "none")]
+SPECTRAL_STFT = [("tone_stft_half", 4321, "none"), ("chirp", 6400, "zeros"), ("pink", 6000, "negzeros"),
+                 ("brown", 5000, "none"), ("tone_25", 3000, "first_only")]
+
+
+def spectral_wavs(spec):
+    sys.path.insert(0, str(ROOT / "tests"))
+    import spectral_ref as R
+
+    return [R.with_tail(R.structured_wav(kind, n), tail) for kind, n, tail in spec]
+
+
+def make_spectral_fixture():
+    """fbank, fbank_no_cmvn, mel and linear of the reference on structured audio (tones, chirp, bursts, tilted noise,
+    DC, impulses, int16 scale, trailing zeros / -0.0, 1-frame utterances). The waveforms are stored as recipes plus
+    their fp32 checksums."""
+    from s3prl.upstream.baseline.hubconf import fbank, fbank_no_cmvn, linear, mel
+
+    out = {"fbank_spec": SPECTRAL_FBANK, "stft_spec": SPECTRAL_STFT, "cases": {}}
+    for spec, entries in ((SPECTRAL_FBANK, (("fbank", fbank), ("fbank_no_cmvn", fbank_no_cmvn))),
+                          (SPECTRAL_STFT, (("mel", mel), ("linear", linear)))):
+        wavs = spectral_wavs(spec)
+        out["checksum_" + ("fbank" if spec is SPECTRAL_FBANK else "stft")] = torch.stack(
+            [w.double().sum() for w in wavs] + [w.double().abs().sum() for w in wavs])
+        for name, factory in entries:
+            expert = factory()
+            expert.eval()
+            with torch.no_grad():
+                hs = expert(wavs)["hidden_states"][0]
+            out["cases"][name] = hs.float().clone()
+            print(f"spectral {name}: {tuple(hs.shape)}")
+    torch.save(out, GOLDEN / "spectral_structured.pt")
+
+
 class _FakeLayers:
     """Only the layer facts a Featurizer reads (five 16-wide layers, stride 320)."""
 
@@ -291,6 +328,8 @@ def main():
         make_fbank_fixture()
     if args.only in (None, "spectrogram"):
         make_spectrogram_fixture()
+    if args.only in (None, "spectral"):
+        make_spectral_fixture()
     if args.only in (None, "nn"):
         make_nn_fixture()
     for name in CASES:

@@ -202,17 +202,22 @@ __global__ void __launch_bounds__(256) cmvn_kernel(float* __restrict__ feat, con
     for (int t = m; t < max_frames; ++t) c[(size_t)t * kFeat] = 0.f;
 }
 
-cudaError_t launch_fbank(const float* const* wavs_dev, const long long* lens_dev, int B, int max_frames, float* out,
-                         cudaStream_t s) {
+cudaError_t launch_fbank(const float* const* wavs_dev, const long long* lens_dev, int B, int max_frames, int cmvn,
+                         float* out, cudaStream_t s) {
     cudaError_t e = ensure_tables(s);
     if (e != cudaSuccess) return e;
     if (max_frames <= 0 || B <= 0) return cudaSuccess;
+    // without CMVN nothing else writes the rows past each utterance's frames
+    if (!cmvn) {
+        e = cudaMemsetAsync(out, 0, (size_t)B * max_frames * kFeat * sizeof(float), s);
+        if (e != cudaSuccess) return e;
+    }
     dim3 g1((max_frames + 3) / 4, B);
     fbank_frames_kernel<<<g1, 128, 0, s>>>(wavs_dev, lens_dev, max_frames, out);
     dim3 g2((max_frames * kMel + 255) / 256, B);
     delta_kernel<<<g2, 256, 0, s>>>(out, lens_dev, max_frames, 0);
     delta_kernel<<<g2, 256, 0, s>>>(out, lens_dev, max_frames, kMel);
-    cmvn_kernel<<<B, 256, 0, s>>>(out, lens_dev, max_frames);
+    if (cmvn) cmvn_kernel<<<B, 256, 0, s>>>(out, lens_dev, max_frames);
     return cudaGetLastError();
 }
 

@@ -172,14 +172,17 @@ __global__ void __launch_bounds__(256) mel_cmvn_kernel(const float* __restrict__
 }
 
 cudaError_t launch_melspec(const float* const* wavs_dev, const long long* trim_lens_dev, int B, long long Lp,
-                           int mel, const int* feats_len_dev, const int* final_len_dev, int t_out, float* tmp,
+                           int mel, int cmvn, const int* feats_len_dev, const int* final_len_dev, int t_out, float* tmp,
                            float* out, cudaStream_t s) {
     cudaError_t e = ensure_mel_tables(s);
     if (e != cudaSuccess) return e;
     const int n_frames = (int)(1 + Lp / kHop);
     dim3 g1((n_frames + 3) / 4, B);
-    stft_mel_kernel<<<g1, 128, 0, s>>>(wavs_dev, trim_lens_dev, Lp, n_frames, mel, tmp);
-    mel_cmvn_kernel<<<B, 256, 0, s>>>(tmp, n_frames, mel ? kNmel : kNbin, feats_len_dev, final_len_dev, t_out, out);
+    // without CMVN the log features of every frame of the padded batch are the output
+    stft_mel_kernel<<<g1, 128, 0, s>>>(wavs_dev, trim_lens_dev, Lp, n_frames, mel, cmvn ? tmp : out);
+    if (cmvn)
+        mel_cmvn_kernel<<<B, 256, 0, s>>>(tmp, n_frames, mel ? kNmel : kNbin, feats_len_dev, final_len_dev, t_out,
+                                          out);
     return cudaGetLastError();
 }
 

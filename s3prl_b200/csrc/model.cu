@@ -2785,24 +2785,72 @@ extern "C" int s3b_layernorm_rope_f32(const float* x, int64_t M, int32_t T, int3
 
 extern "C" int64_t s3b_fbank_num_frames(int64_t len) { return len < 400 ? 0 : 1 + (len - 400) / 160; }
 
-extern "C" int s3b_fbank(const float* const* wavs, const int64_t* lens, int32_t batch, float* out, void* stream) {
+// Device memory owned by one call and released in the order of that call's stream (stream-ordered allocator). Every
+// call stages its pointers and lengths, and keeps its intermediates, in blocks of its own, so a later call on another
+// stream cannot overwrite what a call still queued will read.
+struct StreamBuf {
+    void* p = nullptr;
+    cudaStream_t s;
+    explicit StreamBuf(cudaStream_t st) : s(st) {}
+    StreamBuf(const StreamBuf&) = delete;
+    StreamBuf& operator=(const StreamBuf&) = delete;
+    ~StreamBuf() {
+        if (p) cudaFreeAsync(p, s);
+    }
+    int alloc(size_t n) {
+        cudaError_t e = cudaMallocAsync(&p, n, s);
+        if (e != cudaSuccess) {
+            p = nullptr;
+            return fail("cudaMallocAsync(%zu) failed: %s", n, cudaGetErrorString(e));
+        }
+        return 0;
+    }
+    template <class T>
+    T* as() const {
+        return reinterpret_cast<T*>(p);
+    }
+};
+
+static int check_spectral_opts(const s3b_spectral_opts* opts) {
+    if (opts != nullptr && opts->struct_size != (int32_t)sizeof(s3b_spectral_opts))
+        return fail("s3b_spectral_opts.struct_size %d != %d (header / library mismatch)", opts->struct_size,
+                    (int)sizeof(s3b_spectral_opts));
+    if (opts != nullptr && opts->cmvn != 0 && opts->cmvn != 1) return fail("cmvn must be 0 or 1, not %d", opts->cmvn);
+    return 0;
+}
+
+static int check_lengths(const int64_t* lens, int32_t batch) {
+    for (int b = 0; b < batch; ++b)
+        if (lens[b] < 0) return fail("lens[%d] = %lld is negative", b, (long long)lens[b]);
+    return 0;
+}
+
+extern "C" int s3b_fbank_ex(const float* const* wavs, const int64_t* lens, int32_t batch,
+                            const s3b_spectral_opts* opts, float* out, void* stream) {
     if (!wavs || !lens || !out) return fail("null argument");
     if (batch < 1) return fail("empty batch");
+    S3B_OK(check_spectral_opts(opts));
+    S3B_OK(check_lengths(lens, batch));
     if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
+    const int cmvn = opts ? opts->cmvn : 1;
     cudaStream_t st = (cudaStream_t)stream;
     int64_t max_len = 0;
     for (int b = 0; b < batch; ++b) max_len = lens[b] > max_len ? lens[b] : max_len;
     const int64_t max_frames = s3b_fbank_num_frames(max_len);
     if (max_frames < 1) return fail("waveforms shorter than one 25 ms frame");
-    static thread_local DevBuf scratch;
-    S3B_OK(scratch.ensure((size_t)batch * (sizeof(void*) + sizeof(long long))));
+    StreamBuf scratch(st);
+    S3B_OK(scratch.alloc((size_t)batch * (sizeof(void*) + sizeof(long long))));
     std::vector<long long> l64(lens, lens + batch);
     const float** d_ptrs = scratch.as<const float*>();
     long long* d_lens = reinterpret_cast<long long*>(scratch.as<char>() + (size_t)batch * sizeof(void*));
     CUDA_OK(cudaMemcpyAsync(d_ptrs, wavs, batch * sizeof(void*), cudaMemcpyHostToDevice, st));
     CUDA_OK(cudaMemcpyAsync(d_lens, l64.data(), batch * sizeof(long long), cudaMemcpyHostToDevice, st));
-    CUDA_OK(launch_fbank(d_ptrs, d_lens, batch, (int)max_frames, out, st));
+    CUDA_OK(launch_fbank(d_ptrs, d_lens, batch, (int)max_frames, cmvn, out, st));
     return 0;
+}
+
+extern "C" int s3b_fbank(const float* const* wavs, const int64_t* lens, int32_t batch, float* out, void* stream) {
+    return s3b_fbank_ex(wavs, lens, batch, nullptr, out, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2810,6 +2858,7 @@ extern "C" int s3b_fbank(const float* const* wavs, const int64_t* lens, int32_t 
 // ------------------------------------------------------------------------------------------------
 extern "C" int s3b_trimmed_lengths(const float* const* wavs, const int64_t* lens, int32_t batch, int64_t* out) {
     if (!wavs || !lens || !out) return fail("null argument");
+    S3B_OK(check_lengths(lens, batch));
     if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
     DevBuf scratch;
     S3B_OK(scratch.ensure((size_t)batch * (sizeof(void*) + 2 * sizeof(long long))));
@@ -2826,18 +2875,32 @@ extern "C" int s3b_trimmed_lengths(const float* const* wavs, const int64_t* lens
     return 0;
 }
 
-extern "C" int s3b_melspec(const float* const* wavs, const int64_t* trimmed_lens, int32_t batch, int64_t padded_len,
-                           int32_t mel, const int32_t* feats_len, const int32_t* final_len, int32_t t_out, float* out,
-                           void* stream) {
-    if (!wavs || !trimmed_lens || !feats_len || !final_len || !out) return fail("null argument");
-    if (batch < 1 || padded_len < 1 || t_out < 1) return fail("bad sizes");
+extern "C" int s3b_melspec_ex(const float* const* wavs, const int64_t* trimmed_lens, int32_t batch,
+                              int64_t padded_len, int32_t mel, const int32_t* feats_len, const int32_t* final_len,
+                              int32_t t_out, const s3b_spectral_opts* opts, float* out, void* stream) {
+    S3B_OK(check_spectral_opts(opts));
+    const int cmvn = opts ? opts->cmvn : 1;
+    if (!wavs || !trimmed_lens || !out || (cmvn && (!feats_len || !final_len))) return fail("null argument");
+    if (batch < 1 || padded_len < 1 || (cmvn && t_out < 1)) return fail("bad sizes");
+    const int64_t n_frames = 1 + padded_len / 160;
+    for (int b = 0; b < batch; ++b) {
+        if (trimmed_lens[b] < 0 || trimmed_lens[b] > padded_len)
+            return fail("trimmed_lens[%d] = %lld outside [0, padded_len = %lld]", b, (long long)trimmed_lens[b],
+                        (long long)padded_len);
+        if (!cmvn) continue;
+        // mel_cmvn_kernel reads feats_len[b] rows of utterance b's n_frames-row block of tmp
+        if (feats_len[b] < 0 || feats_len[b] > n_frames)
+            return fail("feats_len[%d] = %d outside [0, 1 + padded_len / 160 = %lld]", b, feats_len[b],
+                        (long long)n_frames);
+        if (final_len[b] < 0 || final_len[b] > t_out)
+            return fail("final_len[%d] = %d outside [0, t_out = %d]", b, final_len[b], t_out);
+    }
     if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
     cudaStream_t st = (cudaStream_t)stream;
     const int dim = mel ? 80 : 201;
-    const int64_t n_frames = 1 + padded_len / 160;
-    static thread_local DevBuf scratch, tmp;
-    S3B_OK(scratch.ensure((size_t)batch * (sizeof(void*) + sizeof(long long) + 2 * sizeof(int))));
-    S3B_OK(tmp.ensure((size_t)batch * n_frames * dim * 4));
+    StreamBuf scratch(st), tmp(st);
+    S3B_OK(scratch.alloc((size_t)batch * (sizeof(void*) + sizeof(long long) + 2 * sizeof(int))));
+    if (cmvn) S3B_OK(tmp.alloc((size_t)batch * n_frames * dim * 4));
     const float** d_ptrs = scratch.as<const float*>();
     long long* d_lens = reinterpret_cast<long long*>(scratch.as<char>() + (size_t)batch * sizeof(void*));
     int* d_fl = reinterpret_cast<int*>(d_lens + batch);
@@ -2845,8 +2908,17 @@ extern "C" int s3b_melspec(const float* const* wavs, const int64_t* trimmed_lens
     std::vector<long long> l64(trimmed_lens, trimmed_lens + batch);
     CUDA_OK(cudaMemcpyAsync(d_ptrs, wavs, batch * sizeof(void*), cudaMemcpyHostToDevice, st));
     CUDA_OK(cudaMemcpyAsync(d_lens, l64.data(), batch * sizeof(long long), cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaMemcpyAsync(d_fl, feats_len, batch * sizeof(int), cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaMemcpyAsync(d_kl, final_len, batch * sizeof(int), cudaMemcpyHostToDevice, st));
-    CUDA_OK(launch_melspec(d_ptrs, d_lens, batch, padded_len, mel, d_fl, d_kl, t_out, tmp.as<float>(), out, st));
+    if (cmvn) {
+        CUDA_OK(cudaMemcpyAsync(d_fl, feats_len, batch * sizeof(int), cudaMemcpyHostToDevice, st));
+        CUDA_OK(cudaMemcpyAsync(d_kl, final_len, batch * sizeof(int), cudaMemcpyHostToDevice, st));
+    }
+    CUDA_OK(launch_melspec(d_ptrs, d_lens, batch, padded_len, mel, cmvn, d_fl, d_kl, t_out, tmp.as<float>(), out, st));
     return 0;
+}
+
+extern "C" int s3b_melspec(const float* const* wavs, const int64_t* trimmed_lens, int32_t batch, int64_t padded_len,
+                           int32_t mel, const int32_t* feats_len, const int32_t* final_len, int32_t t_out, float* out,
+                           void* stream) {
+    return s3b_melspec_ex(wavs, trimmed_lens, batch, padded_len, mel, feats_len, final_len, t_out, nullptr, out,
+                          stream);
 }

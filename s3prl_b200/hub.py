@@ -66,7 +66,16 @@ def fbank(*args, **kwargs):
     return FbankExpert(**kwargs)
 
 
+def fbank_no_cmvn(*args, **kwargs):
+    """The fbank baseline's log-mel + deltas without CMVN (s3prl/upstream/baseline/hubconf.py:51-58, fbank_no_cmvn.yaml)."""
+    from .upstream.baseline import FbankExpert
+
+    kwargs["cmvn"] = False
+    return FbankExpert(**kwargs)
+
+
 ENTRIES["fbank"] = fbank
+ENTRIES["fbank_no_cmvn"] = fbank_no_cmvn
 
 
 def mel(*args, **kwargs):

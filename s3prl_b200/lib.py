@@ -58,9 +58,11 @@ EXPORTED_SYMBOLS = [
     "s3b_conformer_conv_f32",
     "s3b_layernorm_rope_f32",
     "s3b_fbank",
+    "s3b_fbank_ex",
     "s3b_fbank_num_frames",
     "s3b_trimmed_lengths",
     "s3b_melspec",
+    "s3b_melspec_ex",
 ]
 
 
@@ -158,6 +160,21 @@ class S3BLinearOpts(C.Structure):
         self.struct_size = C.sizeof(S3BLinearOpts)
 
 
+class S3BSpectralOpts(C.Structure):
+    """Mirror of ``struct s3b_spectral_opts`` (cmvn defaults to 1, as s3b_fbank / s3b_melspec)."""
+
+    _fields_ = [
+        ("struct_size", C.c_int32),
+        ("cmvn", C.c_int32),
+        ("reserved", C.c_int64 * 3),
+    ]
+
+    def __init__(self, **kw):
+        kw.setdefault("cmvn", 1)
+        super().__init__(**kw)
+        self.struct_size = C.sizeof(S3BSpectralOpts)
+
+
 FAMILY_HUBERT, FAMILY_WAV2VEC2, FAMILY_WAVLM, FAMILY_DISTILLER = 0, 1, 2, 3
 
 _lib: Optional[C.CDLL] = None
@@ -232,8 +249,11 @@ def load() -> C.CDLL:
     lib.s3b_fbank_num_frames.argtypes = [i64]
     lib.s3b_fbank_num_frames.restype = i64
     lib.s3b_fbank.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, f32p, vp]
+    lib.s3b_fbank_ex.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, C.POINTER(S3BSpectralOpts), f32p, vp]
     lib.s3b_trimmed_lengths.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, C.POINTER(i64)]
     lib.s3b_melspec.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i64, i32, C.POINTER(i32), C.POINTER(i32), i32, f32p, vp]
+    lib.s3b_melspec_ex.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i64, i32, C.POINTER(i32), C.POINTER(i32), i32,
+                                   C.POINTER(S3BSpectralOpts), f32p, vp]
     _lib = lib
     return lib
 

@@ -3,6 +3,7 @@
     expert = FbankExpert()
     out = expert([wav_0, wav_1, ...])      # list of 1-D fp32 CUDA tensors
     out["hidden_states"] == [X],  X: [B, max_frames, 240]  (80 log-mel + delta + delta-delta, CMVN)
+    FbankExpert(cmvn=False) is the ``fbank_no_cmvn`` entry (fbank_no_cmvn.yaml): the same features without CMVN.
     expert.get_downsample_rates("hidden_states") == 160
 """
 from __future__ import annotations
@@ -20,8 +21,9 @@ class FbankExpert(nn.Module):
     output_dim = 240
     downsample_rate = 160
 
-    def __init__(self, model_config=None, **kwargs):
+    def __init__(self, model_config=None, cmvn: bool = True, **kwargs):
         super().__init__()
+        self.cmvn = bool(cmvn)
         self.register_buffer("_device_anchor", torch.zeros(1), persistent=False)
 
     def get_downsample_rates(self, key: str) -> int:
@@ -43,9 +45,10 @@ class FbankExpert(nn.Module):
             out = torch.empty((B, m, self.output_dim), dtype=torch.float32, device=device)
             ptrs = (C.c_void_p * B)(*[w.data_ptr() for w in wavs])
             lens_c = (C.c_int64 * B)(*lens)
+            opts = _lib.S3BSpectralOpts(cmvn=int(self.cmvn))
             _lib.check(
-                lib.s3b_fbank(ptrs, lens_c, B, C.c_void_p(out.data_ptr()),
-                              C.c_void_p(torch.cuda.current_stream(device).cuda_stream))
+                lib.s3b_fbank_ex(ptrs, lens_c, B, C.byref(opts), C.c_void_p(out.data_ptr()),
+                                 C.c_void_p(torch.cuda.current_stream(device).cuda_stream))
             )
         return {"last_hidden_state": out, "hidden_states": [out]}
 
@@ -53,9 +56,11 @@ class FbankExpert(nn.Module):
 class SpectrogramExpert(nn.Module):
     """``mel`` / ``linear`` baselines (s3prl/upstream/baseline/expert.py:52-79 with mel.yaml / linear.yaml).
 
-    The length bookkeeping is the reference's, quirks included: trailing exact zeros are trimmed
-    (preprocessor.py:166-175), CMVN runs over ``round(len / (Lmax / n_frames))`` frames (:203-204) and the final
-    cut uses the ratio of the FIRST utterance (expert.py:62-64)."""
+    The length bookkeeping is the reference's, quirks included: the lengths after dropping trailing exact zeros
+    (preprocessor.py:166-175) set how many frames CMVN runs over, ``round(len / (Lmax / n_frames))`` (:203-204), but
+    the STFT still sees the batch padded to the longest ORIGINAL length (the trim there slices the channel axis, so
+    Lmax and n_frames come from the untrimmed padding), and the final cut uses the ratio of the FIRST utterance
+    (expert.py:62-64)."""
 
     downsample_rate = 160
 
@@ -72,7 +77,7 @@ class SpectrogramExpert(nn.Module):
     @staticmethod
     def plan_lengths(orig_lens: List[int], trimmed_lens: List[int]):
         """(padded_len, feats_len, final_len, t_out) exactly as the reference's Python arithmetic yields them."""
-        lp = max(trimmed_lens)
+        lp = max(orig_lens)
         n_frames = 1 + lp // 160
         downsample_rate = lp / n_frames
         feats_len = [round(n / downsample_rate) for n in trimmed_lens]
