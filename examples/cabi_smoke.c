@@ -29,7 +29,7 @@ int main(void) {
         (const void*)s3b_wavlm_gate_f32, (const void*)s3b_linear_ex,      (const void*)s3b_qkv_f32,
         (const void*)s3b_conv_gemm_f32,  (const void*)s3b_posconv_f32,    (const void*)s3b_frontend_f32,
         (const void*)s3b_conformer_conv_f32, (const void*)s3b_layernorm_rope_f32, (const void*)s3b_qkv_hd_f32,
-        (const void*)s3b_fbank_ex,       (const void*)s3b_melspec_ex,
+        (const void*)s3b_fbank_ex,       (const void*)s3b_melspec_ex,     (const void*)s3b_decoar2_features_f32,
     };
     s3b_config cfg;
     int64_t lens[2] = {16000, 800};

@@ -49,7 +49,14 @@ typedef struct s3b_config {
      * conv fields are then unused (the encoder has no pos_conv) and rotary attention is implied. */
     int32_t conformer;            /* 0: transformer layers; 1: Conformer layers */
     int32_t depthwise_kernel;     /* depthwise_conv_kernel_size of the convolution module: odd, 1..63 (conformer only) */
-    int32_t reserved[3];
+    /* 0: the waveform conv stack (feature_extractor.*, layer_norm.*) in front of post_extract_proj [D][512].
+     * 1: DeCoAR 2.0 (s3prl/upstream/decoar2/{audio,decoar2,expert}.py): per utterance kaldi fbank (80 mel bins, 25 ms /
+     *    10 ms, hamming window, snip_edges) -> CMVN over all m frames (unbiased std) -> every second frame, T_b =
+     *    (m_b + 1) / 2, into post_extract_proj [D][80]; frame t of utterance b is padding iff t >= T_b. Needs family 1 and
+     *    a transformer encoder with pos_conv_depth <= 1; the conv-stack fields (extractor_layer_norm, conv_bias,
+     *    normalize_wav, no_feature_layer_norm) must be 0. Utterances need >= 560 samples (2 fbank frames). */
+    int32_t frontend;
+    int32_t reserved[2];
 } s3b_config;
 
 /* Library / error ------------------------------------------------------------------------------ */
@@ -72,11 +79,13 @@ void s3b_model_destroy(s3b_model* m);
 
 /* Frame bookkeeping (bit-exact integer rules) ------------------------------------
  * T = conv-stack output length for a padded batch of max length max_len
- * (ConvFeatureExtractionModel, wav2vec2_model.py:2857-2934). Returns -1 if max_len is too short. */
+ * (ConvFeatureExtractionModel, wav2vec2_model.py:2857-2934); m may be NULL. For a DeCoAR 2.0 model (frontend 1)
+ * T = (1 + (max_len - 400) / 160 + 1) / 2. Returns -1 if max_len is too short (below 400 samples for DeCoAR 2.0). */
 int64_t s3b_num_frames(const s3b_model* m, int64_t max_len);
 /* valid_frames[b] = number of un-padded frames of utterance b inside a batch padded to max_len:
  * HuBERT/WavLM chunk-all rule (hubert_model.py:454-464, WavLM.py:339-349) or the wav2vec2 conv-length
- * rule (wav2vec2_model.py:2610-2625,2652-2671). frame t of utterance b is padding iff t >= valid_frames[b]. */
+ * rule (wav2vec2_model.py:2610-2625,2652-2671); DeCoAR 2.0: (1 + (lens[b] - 400) / 160 + 1) / 2, lens[b] >= 560.
+ * frame t of utterance b is padding iff t >= valid_frames[b]. */
 int s3b_valid_frames(const s3b_model* m, const int64_t* lens, int32_t batch, int64_t max_len, int32_t* valid_frames);
 
 /* The hot path ------------------------------------------------------------------------------------
@@ -136,7 +145,8 @@ int s3b_forward_host_ex(s3b_model* m, const float* const* wavs, const int64_t* l
 int s3b_wavlm_buckets(int32_t num_buckets, int32_t max_distance, const int32_t* rel, int32_t n, int32_t* out);
 
 /* Accounting --------------------------------------------------------------------------------------
- * Kernel categories: 0 = GEMM, 1 = attention, 2 = conv-0 (+GroupNorm/LayerNorm+GELU),
+ * Kernel categories: 0 = GEMM, 1 = attention, 2 = the front end before the GEMMs: conv-0 (+GroupNorm/LayerNorm+GELU), or
+ * for a DeCoAR 2.0 model the fbank frame kernel and the CMVN / decimation kernel,
  * 3 = LayerNorm kernels (Conformer: LayerNorm + RoPE included), 4 = misc (waveform packing, WavLM gate, the
  * Conformer's GLU + depthwise conv). With profiling enabled every launch of
  * s3b_forward is bracketed by CUDA events on the launching stream; s3b_profile_read synchronises the device and
@@ -326,6 +336,12 @@ int s3b_wavlm_gate_f32(const float* x, int32_t batch, int32_t t, int32_t heads, 
 int s3b_frontend_f32(const float* const* wavs, const int64_t* lens, int32_t batch, int64_t max_len, int32_t normalize,
                      const float* w, const float* bias, const float* gamma, const float* beta, int32_t layer_norm,
                      int32_t out_fmt, float* wav_out, float* out, void* stream);
+/* The DeCoAR 2.0 front end as a forward runs it (frontend = 1 of s3b_config): ragged DEVICE waveforms (host array of
+ * pointers, host lengths lens[b] >= 560) -> kaldi fbank with the hamming window -> CMVN over each utterance's frames ->
+ * every second frame, written as operand planes of out_fmt (0 = bf16 hi/lo, 1 = f16q8) and decoded to
+ * out [batch][T][80], T = (1 + (max(lens) - 400) / 160 + 1) / 2, rows t >= T_b zero. */
+int s3b_decoar2_features_f32(const float* const* wavs, const int64_t* lens, int32_t batch, int32_t out_fmt, float* out,
+                             void* stream);
 /* The Conformer convolution module between its pointwise convs, as a forward runs it (wav2vec2_model.py:383-389):
  * x [batch][t][2d] (pointwise_conv1 output, channels-last) -> GLU (x[..., :d] * sigmoid(x[..., d:])) -> depthwise
  * Conv1d(k, padding k / 2, groups d, no bias; dw_w [d][1][k]) over each utterance's t frames -> BatchNorm1d (eval, eps

@@ -6,12 +6,16 @@
 //   per-utterance CMVN with unbiased std                    s3prl/upstream/baseline/extracter.py:78-90
 // One warp computes one 25 ms frame: DC removal, pre-emphasis, povey window, 512-point radix-2 FFT in shared
 // memory, power spectrum, sparse triangular mel projection (the "matmul"), log. All fp32.
+// The same frame kernel with a hamming window is the front end of DeCoAR 2.0 (s3prl/upstream/decoar2/audio.py:41-86),
+// followed by decoar2_cmvn_kernel: per-utterance CMVN over all frames, every second frame kept, written as the
+// operand planes of post_extract_proj.
 #include <math.h>
 
 #include <vector>
 
 #include "common.cuh"
 #include "fbank.cuh"
+#include "kernels.cuh"
 
 namespace s3b {
 
@@ -26,6 +30,10 @@ struct FbankTables {
 };
 __device__ FbankTables g_tab;
 static bool g_tab_ready[64] = {false};
+// DeCoAR 2.0's window, torch.hamming_window(400, periodic=False, alpha=0.54, beta=0.46) (kaldi.py _get_window). A table
+// of its own: g_tab.window stays the povey window of the fbank baseline, and both models can live in one process.
+__device__ float g_hamming[kWin];
+static bool g_hamming_ready[64] = {false};
 
 static void build_tables(FbankTables& t) {
     // povey window: hann(400, periodic=False) ** 0.85   (kaldi.py:98-100)
@@ -77,9 +85,27 @@ static cudaError_t ensure_tables(cudaStream_t s) {
     return e;
 }
 
+// Synchronous: the shared tables and the hamming window of the current device, built once. DeCoAR 2.0 models call it
+// at finalize, so that their forwards (asynchronous, graph-capturable) never build tables.
+cudaError_t init_fbank_tables() {
+    cudaError_t e = ensure_tables(0);
+    if (e != cudaSuccess) return e;
+    int dev = 0;
+    e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    if (dev < 64 && g_hamming_ready[dev]) return cudaSuccess;
+    float h[kWin];
+    for (int n = 0; n < kWin; ++n) h[n] = (float)(0.54 - 0.46 * cos(2.0 * M_PI * n / (kWin - 1)));
+    e = cudaMemcpyToSymbol(g_hamming, h, sizeof(h));
+    if (e == cudaSuccess && dev < 64) g_hamming_ready[dev] = true;
+    return e;
+}
+
 __device__ __forceinline__ int bitrev9(int x) { return (int)(__brev((unsigned)x) >> 23); }
 
-// grid: (ceil(max_frames / 4), B); block: 128 threads = 4 warps = 4 frames
+// grid: (ceil(max_frames / 4), B); block: 128 threads = 4 warps = 4 frames. kHamming: hamming instead of povey window;
+// kLd: floats between consecutive frames of `out` (the log-mel goes to columns [0, 80))
+template <bool kHamming, int kLd>
 __global__ void __launch_bounds__(128) fbank_frames_kernel(const float* const* __restrict__ wavs,
                                                            const long long* __restrict__ lens, int max_frames,
                                                            float* __restrict__ out) {
@@ -116,7 +142,7 @@ __global__ void __launch_bounds__(128) fbank_frames_kernel(const float* const* _
     for (int i = 0; i < 16; ++i) {
         const int n = lane + 32 * i;
         float v = 0.f;
-        if (n < kWin) v = (re[n] - 0.97f * re[n > 0 ? n - 1 : 0]) * g_tab.window[n];
+        if (n < kWin) v = (re[n] - 0.97f * re[n > 0 ? n - 1 : 0]) * (kHamming ? g_hamming[n] : g_tab.window[n]);
         y[i] = v;
     }
     __syncwarp();
@@ -154,7 +180,7 @@ __global__ void __launch_bounds__(128) fbank_frames_kernel(const float* const* _
     }
     __syncwarp();
     // mel projection + log(max(e, eps))
-    float* o = out + ((size_t)b * max_frames + t) * kFeat;
+    float* o = out + ((size_t)b * max_frames + t) * kLd;
     for (int j = lane; j < kMel; j += 32) {
         const int st = g_tab.mel_start[j], cnt = g_tab.mel_count[j];
         const float* mw = g_tab.mel_w + g_tab.mel_off[j];
@@ -213,11 +239,83 @@ cudaError_t launch_fbank(const float* const* wavs_dev, const long long* lens_dev
         if (e != cudaSuccess) return e;
     }
     dim3 g1((max_frames + 3) / 4, B);
-    fbank_frames_kernel<<<g1, 128, 0, s>>>(wavs_dev, lens_dev, max_frames, out);
+    fbank_frames_kernel<false, kFeat><<<g1, 128, 0, s>>>(wavs_dev, lens_dev, max_frames, out);
     dim3 g2((max_frames * kMel + 255) / 256, B);
     delta_kernel<<<g2, 256, 0, s>>>(out, lens_dev, max_frames, 0);
     delta_kernel<<<g2, 256, 0, s>>>(out, lens_dev, max_frames, kMel);
     if (cmvn) cmvn_kernel<<<B, 256, 0, s>>>(out, lens_dev, max_frames);
+    return cudaGetLastError();
+}
+
+// DeCoAR 2.0 CMVN + decimation (audio.py:13-38, 77-84): y = (x - mean_t) / (1e-10 + std_t) per utterance and mel bin
+// over all m_b frames (unbiased std; the odd frames that y[::2] drops count too), then rows t < T_b = (m_b + 1) / 2
+// take frame 2t. Written as operand planes [B * T][128] of post_extract_proj: columns 80..127 and rows t >= T_b zero.
+// grid (B, 8): blockIdx.y is a 16-column slice of the operand rows (slices 5..7 only write zeros); block 256 threads.
+// The statistics are a two-pass fp64 reduction over 16 frame lanes x 16 bins.
+__global__ void __launch_bounds__(256) decoar2_cmvn_kernel(const float* __restrict__ feat,
+                                                           const long long* __restrict__ lens, int max_frames, int T,
+                                                           OutPlanes op) {
+    __shared__ double s_part[16][17];
+    __shared__ float s_mean[16], s_sd[16];
+    const int b = blockIdx.x, col0 = blockIdx.y * 16;
+    const long long L = lens[b];
+    const int m = L < kWin ? 0 : (int)(1 + (L - kWin) / kShift);
+    const int tb = (m + 1) / 2;
+    const bool mel = col0 < kMel;  // block-uniform
+    const float* base = feat + (size_t)b * max_frames * kMel + col0;
+    if (mel) {
+        const int j = threadIdx.x & 15, r = threadIdx.x >> 4;
+        double s = 0.0;
+        for (int t = r; t < m; t += 16) s += (double)base[(size_t)t * kMel + j];
+        s_part[r][j] = s;
+        __syncthreads();
+        if (threadIdx.x < 16) {
+            double a = 0.0;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) a += s_part[i][threadIdx.x];
+            s_mean[threadIdx.x] = (float)(a / m);
+        }
+        __syncthreads();
+        const float mean = s_mean[j];
+        double q = 0.0;
+        for (int t = r; t < m; t += 16) {
+            const float d = base[(size_t)t * kMel + j] - mean;
+            q += (double)d * (double)d;
+        }
+        s_part[r][j] = q;
+        __syncthreads();
+        if (threadIdx.x < 16) {
+            double a = 0.0;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) a += s_part[i][threadIdx.x];
+            s_sd[threadIdx.x] = (float)sqrt(a / (double)(m - 1));  // m == 1 -> NaN, as torch.std does
+        }
+        __syncthreads();
+    }
+    // 8 column pairs x 32 row lanes
+    const int p = threadIdx.x & 7, r = threadIdx.x >> 3;
+    float mean0 = 0.f, mean1 = 0.f, den0 = 1.f, den1 = 1.f;
+    if (mel) {
+        mean0 = s_mean[2 * p], mean1 = s_mean[2 * p + 1];
+        den0 = 1e-10f + s_sd[2 * p], den1 = 1e-10f + s_sd[2 * p + 1];
+    }
+    for (int t = r; t < T; t += 32) {
+        float y0 = 0.f, y1 = 0.f;
+        if (mel && t < tb) {
+            const float2 x = *reinterpret_cast<const float2*>(base + (size_t)(2 * t) * kMel + 2 * p);
+            y0 = (x.x - mean0) / den0;
+            y1 = (x.y - mean1) / den1;
+        }
+        store_planes2(op, y0, y1, ((size_t)b * T + t) * kDecoar2K + col0 + 2 * p);
+    }
+}
+
+cudaError_t launch_decoar2_features(const float* const* wavs_dev, const long long* lens_dev, int B, int max_frames,
+                                    int T, float* fb, const OutPlanes& op, cudaStream_t s) {
+    if (max_frames <= 0 || B <= 0 || T <= 0) return cudaSuccess;
+    dim3 g1((max_frames + 3) / 4, B);
+    fbank_frames_kernel<true, kMel><<<g1, 128, 0, s>>>(wavs_dev, lens_dev, max_frames, fb);
+    decoar2_cmvn_kernel<<<dim3(B, kDecoar2K / 16), 256, 0, s>>>(fb, lens_dev, max_frames, T, op);
     return cudaGetLastError();
 }
 

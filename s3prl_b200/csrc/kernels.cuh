@@ -47,6 +47,17 @@ static constexpr int kDwMaxKernel = 63;
 cudaError_t launch_depthwise_glu(const float* x, int B, int T, int D, int k, const float* w, const float* bias,
                                  const OutPlanes& op, cudaStream_t s);
 
+// ---- fbank.cu: the DeCoAR 2.0 front end -------------------------------------------------------------------------
+// K of DeCoAR 2.0's post_extract_proj GEMM: the 80 mel bins, zero-padded to the f16q8 GEMM's K % 128 rule
+static constexpr int kDecoar2K = 128;
+// builds the fbank tables and the hamming window on the current device (synchronous; once per device)
+cudaError_t init_fbank_tables();
+// kaldi fbank with the hamming window into fb [B][max_frames][80] (frames t < m_b of each utterance), then CMVN over
+// each utterance's m_b frames and y[::2] into operand planes op [B * T][kDecoar2K] (zero beyond 80 columns and T_b rows).
+// Needs init_fbank_tables() on this device first. m_b >= 2 (m_b == 1 gives NaN, as the reference's unbiased std).
+cudaError_t launch_decoar2_features(const float* const* wavs_dev, const long long* lens_dev, int B, int max_frames,
+                                    int T, float* fb, const OutPlanes& op, cudaStream_t s);
+
 // ---- peer.cu: fused weighted sum + push all-gather over peer memory --------------------------------------------------
 cudaError_t launch_weighted_sum_push(const float* hs, int NL, size_t n_per_layer, size_t layer_stride, const float* w,
                                      float* const* peer_dst, uint32_t* const* peer_flag, int n_peers, uint32_t seq,

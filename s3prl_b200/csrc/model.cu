@@ -184,6 +184,7 @@ struct Workspace {
     cudaEvent_t book_copied = nullptr;  // the previous call's H2D copy has been consumed: the mirror may be rewritten
     DevBuf wav_stats, wav_pad, c0_part, c0_ss, conv_f32, tmp_f32, x_f32, x1_f32, gate, pos_z, ln_counters, hs0;
     DevBuf glu_f32;  // Conformer: pointwise_conv1 output [M][2D]
+    DevBuf fb_f32;   // DeCoAR 2.0: log-mel frames [B][m(Lmax)][80]
     SplitBuf act[kNumConv], ln512_s, x_s, xs_s, q_s, k_s, vt_s, ctx_s, x1_s, h_s;
     cudaStream_t stream = nullptr;  // lane stream (lane 1; lane 0 runs on the caller's stream)
     cudaEvent_t done = nullptr;
@@ -294,6 +295,14 @@ static int64_t num_frames(int64_t L) {
     return L;
 }
 
+// DeCoAR 2.0 (frontend 1): kaldi fbank frames m = 1 + (L - 400) / 160 (snip_edges), y[::2] keeps (m + 1) / 2 of them
+static const int64_t kDecoar2MinLen = 560;  // two fbank frames: the unbiased std of one frame is NaN
+static int64_t decoar2_frames(int64_t L) { return L < 400 ? 0 : (1 + (L - 400) / 160 + 1) / 2; }
+static int64_t fbank_frames(int64_t L) { return L < 400 ? 0 : 1 + (L - 400) / 160; }
+static bool decoar2(const s3b_model* m) { return m != nullptr && m->cfg.frontend == 1; }
+// frames of a batch padded to L for this model's front end (m NULL: the conv stack)
+static int64_t model_frames(const s3b_model* m, int64_t L) { return decoar2(m) ? decoar2_frames(L) : num_frames(L); }
+
 // ------------------------------------------------------------------------------------------------
 // C ABI: library
 // ------------------------------------------------------------------------------------------------
@@ -364,6 +373,16 @@ extern "C" int s3b_model_create(const s3b_config* cfg, s3b_model** out) {
             return fail("depthwise_kernel %d: must be odd, 1..%d", cfg->depthwise_kernel, kDwMaxKernel);
     } else if (cfg->depthwise_kernel != 0) {
         return fail("depthwise_kernel is a Conformer field (conformer = 0)");
+    }
+    if (cfg->frontend != 0 && cfg->frontend != 1) return fail("frontend must be 0 (conv stack) or 1 (DeCoAR 2.0 fbank)");
+    if (cfg->frontend == 1) {
+        // DeCoAR 2.0 = fbank features into the wav2vec 2.0 TransformerEncoder (decoar2/decoar2.py:27-59)
+        if (cfg->family != 1) return fail("frontend 1 (DeCoAR 2.0) goes with the wav2vec2 family (1), not %d", cfg->family);
+        if (cfg->conformer) return fail("frontend 1 (DeCoAR 2.0) runs a transformer encoder, not a Conformer");
+        if (cfg->pos_conv_depth > 1) return fail("frontend 1 (DeCoAR 2.0) needs pos_conv_depth <= 1");
+        if (cfg->extractor_layer_norm || cfg->conv_bias || cfg->normalize_wav || cfg->no_feature_layer_norm)
+            return fail("frontend 1 (DeCoAR 2.0) has no conv stack: extractor_layer_norm, conv_bias, normalize_wav and "
+                        "no_feature_layer_norm must be 0");
     }
     s3b_model* m = new s3b_model();
     m->cfg = *cfg;
@@ -609,38 +628,48 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
     const HostTensor* t;
     const std::string fe = "feature_extractor.conv_layers.";
 
-    // ---- conv 0 ------------------------------------------------------------------------------
-    S3B_OK(need(m, fe + "0.0.weight", {C, 1, kConvK[0]}, &t));
-    S3B_OK(upload_f32(m->conv0_w, t->data.data(), t->numel()));
-    if (c.conv_bias) S3B_OK(upload_vec(m, fe + "0.0.bias", C, m->conv0_b));
-    if (c.extractor_layer_norm) {
-        S3B_OK(upload_vec(m, fe + "0.2.1.weight", C, m->norm0_g));
-        S3B_OK(upload_vec(m, fe + "0.2.1.bias", C, m->norm0_b));
+    if (decoar2(m)) {
+        // ---- DeCoAR 2.0: post_extract_proj [D][80] zero-padded to K = 128; fbank tables built here, not in a forward --
+        S3B_OK(need(m, "post_extract_proj.weight", {D, 80}, &t));
+        std::vector<float> wp((size_t)D * kDecoar2K, 0.f);
+        for (int o = 0; o < D; ++o) memcpy(&wp[(size_t)o * kDecoar2K], &t->data[(size_t)o * 80], 80 * sizeof(float));
+        S3B_OK(upload_split(m->proj_w, wp.data(), wp.size(), m->scheme));
+        S3B_OK(upload_vec(m, "post_extract_proj.bias", D, m->proj_b));
+        CUDA_OK(init_fbank_tables());
     } else {
-        S3B_OK(upload_vec(m, fe + "0.2.weight", C, m->norm0_g));
-        S3B_OK(upload_vec(m, fe + "0.2.bias", C, m->norm0_b));
-    }
-    // ---- conv 1..6: [out][in][tap] -> [out][tap*512 + in] (K index of the channels-last im2col row) ----
-    for (int i = 1; i < kNumConv; ++i) {
-        const std::string p = fe + std::to_string(i);
-        const int kw = kConvK[i];
-        S3B_OK(need(m, p + ".0.weight", {C, C, kw}, &t));
-        const std::vector<float> r = conv_weight_layout(t->data.data(), kw);
-        S3B_OK(upload_split(m->conv_w[i], r.data(), r.size(), m->scheme));
-        if (c.conv_bias) S3B_OK(upload_vec(m, p + ".0.bias", C, m->conv_b[i]));
+        // ---- conv 0 ------------------------------------------------------------------------------
+        S3B_OK(need(m, fe + "0.0.weight", {C, 1, kConvK[0]}, &t));
+        S3B_OK(upload_f32(m->conv0_w, t->data.data(), t->numel()));
+        if (c.conv_bias) S3B_OK(upload_vec(m, fe + "0.0.bias", C, m->conv0_b));
         if (c.extractor_layer_norm) {
-            S3B_OK(upload_vec(m, p + ".2.1.weight", C, m->conv_ln_g[i]));
-            S3B_OK(upload_vec(m, p + ".2.1.bias", C, m->conv_ln_b[i]));
+            S3B_OK(upload_vec(m, fe + "0.2.1.weight", C, m->norm0_g));
+            S3B_OK(upload_vec(m, fe + "0.2.1.bias", C, m->norm0_b));
+        } else {
+            S3B_OK(upload_vec(m, fe + "0.2.weight", C, m->norm0_g));
+            S3B_OK(upload_vec(m, fe + "0.2.bias", C, m->norm0_b));
         }
+        // ---- conv 1..6: [out][in][tap] -> [out][tap*512 + in] (K index of the channels-last im2col row) ----
+        for (int i = 1; i < kNumConv; ++i) {
+            const std::string p = fe + std::to_string(i);
+            const int kw = kConvK[i];
+            S3B_OK(need(m, p + ".0.weight", {C, C, kw}, &t));
+            const std::vector<float> r = conv_weight_layout(t->data.data(), kw);
+            S3B_OK(upload_split(m->conv_w[i], r.data(), r.size(), m->scheme));
+            if (c.conv_bias) S3B_OK(upload_vec(m, p + ".0.bias", C, m->conv_b[i]));
+            if (c.extractor_layer_norm) {
+                S3B_OK(upload_vec(m, p + ".2.1.weight", C, m->conv_ln_g[i]));
+                S3B_OK(upload_vec(m, p + ".2.1.bias", C, m->conv_ln_b[i]));
+            }
+        }
+        // ---- LayerNorm(512) + post_extract_proj ----------------------------------------------------------
+        if (!c.no_feature_layer_norm) {
+            S3B_OK(upload_vec(m, "layer_norm.weight", C, m->ln512_g));
+            S3B_OK(upload_vec(m, "layer_norm.bias", C, m->ln512_b));
+        }
+        S3B_OK(need(m, "post_extract_proj.weight", {D, C}, &t));
+        S3B_OK(upload_split(m->proj_w, t->data.data(), t->numel(), m->scheme));
+        S3B_OK(upload_vec(m, "post_extract_proj.bias", D, m->proj_b));
     }
-    // ---- LayerNorm(512) + post_extract_proj ----------------------------------------------------------
-    if (!c.no_feature_layer_norm) {
-        S3B_OK(upload_vec(m, "layer_norm.weight", C, m->ln512_g));
-        S3B_OK(upload_vec(m, "layer_norm.bias", C, m->ln512_b));
-    }
-    S3B_OK(need(m, "post_extract_proj.weight", {D, C}, &t));
-    S3B_OK(upload_split(m->proj_w, t->data.data(), t->numel(), m->scheme));
-    S3B_OK(upload_vec(m, "post_extract_proj.bias", D, m->proj_b));
     // ---- data2vec pos_conv: pos_conv_depth plain Conv1d(k, padding k/2, groups) blocks (make_conv_block,
     //      wav2vec2_model.py:2995-3026). Four taps per k-block like pos_w4 below (posconv4_weight_layout)
     if (c.conformer) {
@@ -764,8 +793,8 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
 // ------------------------------------------------------------------------------------------------
 // frame bookkeeping
 // ------------------------------------------------------------------------------------------------
-extern "C" int64_t s3b_num_frames(const s3b_model*, int64_t max_len) {
-    const int64_t T = num_frames(max_len);
+extern "C" int64_t s3b_num_frames(const s3b_model* m, int64_t max_len) {
+    const int64_t T = model_frames(m, max_len);
     return T > 0 ? T : -1;
 }
 
@@ -776,16 +805,21 @@ extern "C" int32_t s3b_num_outputs(const s3b_model* m) {
 extern "C" int s3b_valid_frames(const s3b_model* m, const int64_t* lens, int32_t batch, int64_t max_len,
                                 int32_t* valid) {
     if (!m || !lens || !valid) return fail("null argument");
-    const int64_t T = num_frames(max_len);
-    if (T <= 0) return fail("max_len %lld too short for the conv stack", (long long)max_len);
+    const int64_t T = model_frames(m, max_len);
+    if (T <= 0) return fail("max_len %lld too short for the %s", (long long)max_len, decoar2(m) ? "fbank" : "conv stack");
     bool any_pad = false;
     for (int b = 0; b < batch; ++b) {
         if (lens[b] < 1 || lens[b] > max_len) return fail("lens[%d]=%lld out of range", b, (long long)lens[b]);
+        if (decoar2(m) && lens[b] < kDecoar2MinLen)
+            return fail("lens[%d]=%lld: DeCoAR 2.0 needs >= %lld samples (2 fbank frames; the CMVN std of one frame is NaN)",
+                        b, (long long)lens[b], (long long)kDecoar2MinLen);
         any_pad |= lens[b] < max_len;
     }
     for (int b = 0; b < batch; ++b) {
         int64_t v;
-        if (m->cfg.family == 1) {
+        if (decoar2(m)) {
+            v = decoar2_frames(lens[b]);  // pad_sequence of the per-utterance features (decoar2/expert.py:81-92)
+        } else if (m->cfg.family == 1) {
             // wav2vec2: conv-length rule, only when the batch has any padding (wav2vec2_model.py:2652-2671). The
             // reference evaluates floor((n - k) / s + 1) in fp32 WITHOUT clamping, so an utterance shorter than the
             // receptive field yields 0 or a negative length and `mask[b, length - 1] = 1` wraps around like any
@@ -1155,7 +1189,7 @@ struct Plan {
 
 void Workspace::release() {
     DevBuf* bufs[] = {&book, &wav_stats, &wav_pad, &c0_part, &c0_ss, &conv_f32, &tmp_f32, &x_f32, &x1_f32, &gate, &pos_z,
-                      &ln_counters, &hs0, &glu_f32};
+                      &ln_counters, &hs0, &glu_f32, &fb_f32};
     for (DevBuf* b : bufs) b->release();
     for (int i = 0; i < kNumConv; ++i) act[i].release();
     SplitBuf* sb[] = {&ln512_s, &x_s, &xs_s, &q_s, &k_s, &vt_s, &ctx_s, &x1_s, &h_s};
@@ -1230,13 +1264,14 @@ int Fwd::prepare() {
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, C = kConvDim;
     if (B < 1) return fail("empty batch");
+    const bool fb = decoar2(m);
     {
         int64_t cur = Lmax;
-        for (int i = 0; i < kNumConv; ++i) cur = L[i] = conv_out_len(cur, i);
+        for (int i = 0; i < kNumConv; ++i) cur = L[i] = fb ? 0 : conv_out_len(cur, i);
     }
-    const int64_t T64 = L[kNumConv - 1];
-    if (T64 < 1) return fail("max_len %lld too short: the conv stack yields no frame", (long long)Lmax);
-    if ((int64_t)B * L[0] > 2000000000LL) return fail("batch too large for 32-bit tile indexing");
+    const int64_t T64 = model_frames(m, Lmax);
+    if (T64 < 1) return fail("max_len %lld too short: the %s yields no frame", (long long)Lmax, fb ? "fbank" : "conv stack");
+    if ((int64_t)B * (fb ? fbank_frames(Lmax) : L[0]) > 2000000000LL) return fail("batch too large for 32-bit tile indexing");
     T = (int)T64;
     M = (int64_t)B * T;
     Tp = (T + 7) & ~7;
@@ -1287,13 +1322,18 @@ int Fwd::prepare() {
     d_mask = reinterpret_cast<uint8_t*>(db + off_mask);
 
     // ---- workspace ------------------------------------------------------------------------------------------
-    S3B_OK(w->wav_pad.ensure((size_t)B * Lmax * 4));
-    S3B_OK(w->wav_stats.ensure((size_t)B * 2 * 4));
-    S3B_OK(w->c0_part.ensure(conv0_ws_part_bytes(B, (int)L[0])));
-    S3B_OK(w->c0_ss.ensure((size_t)2 * B * C * 4));
-    for (int i = 0; i < kNumConv - 1; ++i) S3B_OK(w->act[i].ensure((size_t)B * L[i] * C));
-    S3B_OK(w->conv_f32.ensure((size_t)B * (c.extractor_layer_norm ? L[1] : L[6]) * C * 4));
-    S3B_OK(w->ln512_s.ensure((size_t)M * C));
+    if (fb) {
+        S3B_OK(w->fb_f32.ensure((size_t)B * fbank_frames(Lmax) * 80 * 4));
+        S3B_OK(w->ln512_s.ensure((size_t)M * kDecoar2K));  // post_extract_proj's A operand: the CMVN kernel's planes
+    } else {
+        S3B_OK(w->wav_pad.ensure((size_t)B * Lmax * 4));
+        S3B_OK(w->wav_stats.ensure((size_t)B * 2 * 4));
+        S3B_OK(w->c0_part.ensure(conv0_ws_part_bytes(B, (int)L[0])));
+        S3B_OK(w->c0_ss.ensure((size_t)2 * B * C * 4));
+        for (int i = 0; i < kNumConv - 1; ++i) S3B_OK(w->act[i].ensure((size_t)B * L[i] * C));
+        S3B_OK(w->conv_f32.ensure((size_t)B * (c.extractor_layer_norm ? L[1] : L[6]) * C * 4));
+        S3B_OK(w->ln512_s.ensure((size_t)M * C));
+    }
     S3B_OK(w->tmp_f32.ensure((size_t)M * D * 4));
     S3B_OK(w->x_f32.ensure((size_t)M * D * 4));
     S3B_OK(w->x1_f32.ensure((size_t)M * D * 4));
@@ -1442,7 +1482,7 @@ int Fwd::build_conformer_layer(LayerPlan& lp, int l) {
 int Fwd::build_plan(Plan& pl) {
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, NL = c.num_layers, C = kConvDim;
-    for (int i = 1; i < kNumConv; ++i) {
+    for (int i = 1; i < kNumConv && !decoar2(m); ++i) {
         GemmParams& p = pl.conv[i];
         S3B_OK(conv_params(p, w->act[i - 1], m->conv_w[i], B, L[i - 1], L[i], kConvK[i], m->scheme));
         Epi e;
@@ -1463,7 +1503,7 @@ int Fwd::build_plan(Plan& pl) {
     }
     {
         GemmParams& p = pl.proj;
-        S3B_OK(linear_params(p, w->ln512_s, m->proj_w, M, D, C, 1, m->scheme));
+        S3B_OK(linear_params(p, w->ln512_s, m->proj_w, M, D, decoar2(m) ? kDecoar2K : C, 1, m->scheme));
         Epi e;
         e.bias = m->proj_b.as<float>();
         e.row_mask = d_mask;  // x[padding_mask] = 0 (wav2vec2_model.py:3061-3062)
@@ -1597,6 +1637,11 @@ int Fwd::stage(int s) {
         const size_t book_bytes = (size_t)(reinterpret_cast<char*>(d_mask) - w->book.as<char>()) + (size_t)M;
         CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host, book_bytes, cudaMemcpyHostToDevice, st));
         if (!capturing) CUDA_OK(cudaEventRecord(w->book_copied, st));  // (graph replay: recorded after the launch)
+        if (decoar2(m)) {  // fbank frames + CMVN / y[::2] -> post_extract_proj's operand planes (profile category 2)
+            KLAUNCH(CAT_CONV0, 2, 0.0, launch_decoar2_features(d_wavs, d_lens, B, (int)fbank_frames(Lmax), T,
+                                                               w->fb_f32.as<float>(), w->ln512_s.planes(m->scheme), st));
+            return 0;
+        }
         return launch_frontend(m, st, d_wavs, d_lens, B, Lmax, (int)L[0], c.normalize_wav, m->conv0_w.as<float>(),
                                c.conv_bias ? m->conv0_b.as<float>() : nullptr, m->norm0_g.as<float>(),
                                m->norm0_b.as<float>(), c.extractor_layer_norm, w->wav_pad.as<float>(),
@@ -1605,6 +1650,7 @@ int Fwd::stage(int s) {
     }
     if (s >= 1 && s <= 6) {
         // ---- conv s as implicit GEMM (+ per-frame LayerNorm + GELU in "layer_norm" mode) ----------------------------
+        if (decoar2(m)) return 0;  // no conv stack
         const int i = s;
         GemmParams p = plan->conv[i];
         KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
@@ -1618,7 +1664,7 @@ int Fwd::stage(int s) {
     }
     if (s == 7) {
         // ---- LayerNorm(512) -> post_extract_proj (+ zero padded frames) --------------------------------------------
-        if (!c.no_feature_layer_norm)
+        if (!c.no_feature_layer_norm && !decoar2(m))
             KNORM(launch_layernorm(w->conv_f32.as<float>(), (size_t)M, C, m->ln512_g.as<float>(), m->ln512_b.as<float>(),
                                    0, nullptr, w->ln512_s.planes(m->scheme), st));
         GemmParams p = plan->proj;
@@ -1864,8 +1910,8 @@ static int default_lanes(int B, int64_t T) {
     return (long long)B * T >= min_frames ? 2 : 1;
 }
 
-extern "C" int32_t s3b_default_lanes(const s3b_model*, int32_t batch, int64_t max_len) {
-    const int64_t T = num_frames(max_len);
+extern "C" int32_t s3b_default_lanes(const s3b_model* m, int32_t batch, int64_t max_len) {
+    const int64_t T = model_frames(m, max_len);
     return (batch < 1 || T < 1) ? -1 : default_lanes(batch, T);
 }
 
@@ -1873,8 +1919,9 @@ static int forward_lanes(s3b_model* m, const float* const* wavs, const int64_t* 
                          float* hidden_out, cudaStream_t st, const s3b_forward_opts* o) {
     const s3b_config& c = m->cfg;
     if (B < 1) return fail("empty batch");
-    const int64_t T = num_frames(Lmax);
-    if (T < 1) return fail("max_len %lld too short: the conv stack yields no frame", (long long)Lmax);
+    const int64_t T = model_frames(m, Lmax);
+    if (T < 1) return fail("max_len %lld too short: the %s yields no frame", (long long)Lmax,
+                           decoar2(m) ? "fbank" : "conv stack");
     int lanes = (o && o->lanes > 0) ? o->lanes : default_lanes(B, T);
     if (lanes > 2) lanes = 2;
     if (lanes > B) lanes = B;
@@ -2015,7 +2062,7 @@ extern "C" int s3b_forward_ex(s3b_model* m, const float* const* wavs, const int6
 
 static int forward_host_impl(s3b_model* m, const float* const* wavs, const int64_t* lens, int32_t batch,
                              int64_t max_len, float* hidden_out, float* hidden_dev) {
-    const int64_t T = num_frames(max_len);
+    const int64_t T = model_frames(m, max_len);
     if (T < 1) return fail("max_len too short");
     size_t total = 0;
     for (int b = 0; b < batch; ++b) total += (size_t)lens[b];
@@ -2713,6 +2760,49 @@ extern "C" int s3b_frontend_f32(const float* const* wavs, const int64_t* lens, i
         return 0;
     }();
     book.release(), pad.release(), stats.release(), part.release(), ss.release(), os.release();
+    return r;
+}
+
+extern "C" int s3b_decoar2_features_f32(const float* const* wavs, const int64_t* lens, int32_t B, int32_t out_fmt,
+                                        float* out, void* stream) {
+    // Fwd::stage(0) of a DeCoAR 2.0 model on workspaces of this call; the operand planes decoded, columns 0..79 kept
+    if (!wavs || !lens || !out) return fail("null argument");
+    if (B < 1) return fail("bad batch %d", B);
+    if (out_fmt != 0 && out_fmt != 1) return fail("out_fmt must be 0 (bf16 hi/lo) or 1 (f16q8), not %d", out_fmt);
+    int64_t max_len = 0;
+    for (int b = 0; b < B; ++b) {
+        if (wavs[b] == nullptr) return fail("null argument: wavs[%d]", b);
+        if (lens[b] < kDecoar2MinLen)
+            return fail("lens[%d] = %lld: DeCoAR 2.0 needs >= %lld samples (2 fbank frames)", b, (long long)lens[b],
+                        (long long)kDecoar2MinLen);
+        max_len = lens[b] > max_len ? lens[b] : max_len;
+    }
+    const int64_t mf = fbank_frames(max_len), T = decoar2_frames(max_len);
+    if ((int64_t)B * mf > 2000000000LL) return fail("batch too large for 32-bit indexing");
+    if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
+    CUDA_OK(init_fbank_tables());
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t rows = (size_t)B * T;
+    DevBuf book, fbuf, dec;
+    SplitBuf os;
+    const int r = [&]() -> int {
+        S3B_OK(book.ensure((size_t)B * (sizeof(void*) + sizeof(long long))));
+        std::vector<long long> hl(lens, lens + B);
+        CUDA_OK(cudaMemcpyAsync(book.p, wavs, (size_t)B * sizeof(void*), cudaMemcpyHostToDevice, st));
+        long long* d_lens = reinterpret_cast<long long*>(book.as<char>() + (size_t)B * sizeof(void*));
+        CUDA_OK(cudaMemcpyAsync(d_lens, hl.data(), (size_t)B * sizeof(long long), cudaMemcpyHostToDevice, st));
+        S3B_OK(fbuf.ensure((size_t)B * mf * 80 * 4));
+        S3B_OK(os.ensure(rows * kDecoar2K));
+        S3B_OK(dec.ensure(rows * kDecoar2K * 4));
+        CUDA_OK(launch_decoar2_features(book.as<const float*>(), d_lens, B, (int)mf, (int)T, fbuf.as<float>(),
+                                        os.planes(out_fmt), st));
+        CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), rows * kDecoar2K, dec.as<float>(), st));
+        CUDA_OK(cudaMemcpy2DAsync(out, 80 * sizeof(float), dec.p, kDecoar2K * sizeof(float), 80 * sizeof(float), rows,
+                                  cudaMemcpyDeviceToDevice, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+        return 0;
+    }();
+    book.release(), fbuf.release(), dec.release(), os.release();
     return r;
 }
 

@@ -96,6 +96,37 @@ ENTRIES["mel"] = mel
 ENTRIES["linear"] = linear
 
 
+def decoar2(ckpt=None, model_config=None, refresh=False, *args, **kwargs):
+    """DeCoAR 2.0 (s3prl/upstream/decoar2/hubconf.py:34-42): the fabricated checkpoint without ``ckpt``, else the
+    local ``{"model": state_dict}`` file."""
+    from .upstream.decoar2 import Decoar2Expert
+
+    if isinstance(ckpt, str) and ckpt.startswith("http"):
+        raise ValueError("decoar2: remote checkpoints are not reachable here; pass a local checkpoint file")
+    return Decoar2Expert(ckpt=ckpt, **kwargs)
+
+
+def _make_decoar2_file_entry(suffix: str) -> Callable:
+    """decoar2_local / decoar2_url / decoar2_custom (decoar2/hubconf.py:10-31): a local checkpoint file; a URL is refused."""
+
+    def entry(ckpt, *args, **kwargs):
+        from .upstream.decoar2 import Decoar2Expert
+
+        assert isinstance(ckpt, str), "a checkpoint path is required"
+        if ckpt.startswith("http"):
+            raise ValueError(f"decoar2_{suffix}: remote checkpoints are not reachable here; download {ckpt} and pass the file")
+        kwargs.pop("refresh", None)
+        return Decoar2Expert(ckpt=ckpt, **kwargs)
+
+    entry.__name__ = f"decoar2_{suffix}"
+    return entry
+
+
+ENTRIES["decoar2"] = decoar2
+for _suffix in ("local", "url", "custom"):
+    ENTRIES[f"decoar2_{_suffix}"] = _make_decoar2_file_entry(_suffix)
+
+
 def options() -> List[str]:
     """Names of the available entries (cf. s3prl.hub.options, s3prl/hub.py:40-54)."""
     return sorted(ENTRIES)

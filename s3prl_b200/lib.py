@@ -56,6 +56,7 @@ EXPORTED_SYMBOLS = [
     "s3b_wavlm_gate_f32",
     "s3b_frontend_f32",
     "s3b_conformer_conv_f32",
+    "s3b_decoar2_features_f32",
     "s3b_layernorm_rope_f32",
     "s3b_fbank",
     "s3b_fbank_ex",
@@ -94,7 +95,8 @@ class S3BConfig(C.Structure):
         ("pos_conv_depth", C.c_int32),
         ("conformer", C.c_int32),
         ("depthwise_kernel", C.c_int32),
-        ("reserved", C.c_int32 * 3),
+        ("frontend", C.c_int32),
+        ("reserved", C.c_int32 * 2),
     ]
 
 
@@ -176,6 +178,7 @@ class S3BSpectralOpts(C.Structure):
 
 
 FAMILY_HUBERT, FAMILY_WAV2VEC2, FAMILY_WAVLM, FAMILY_DISTILLER = 0, 1, 2, 3
+FRONTEND_CONV, FRONTEND_DECOAR2 = 0, 1
 
 _lib: Optional[C.CDLL] = None
 
@@ -245,6 +248,7 @@ def load() -> C.CDLL:
     lib.s3b_frontend_f32.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i64, i32, f32p, f32p, f32p, f32p, i32, i32,
                                      f32p, f32p, vp]
     lib.s3b_conformer_conv_f32.argtypes = [f32p, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, i32, f32p, vp]
+    lib.s3b_decoar2_features_f32.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i32, f32p, vp]
     lib.s3b_layernorm_rope_f32.argtypes = [f32p, i64, i32, i32, f32p, f32p, C.POINTER(C.c_float), i32, f32p, f32p, vp]
     lib.s3b_fbank_num_frames.argtypes = [i64]
     lib.s3b_fbank_num_frames.restype = i64

@@ -45,6 +45,9 @@ class ArchConfig:
     pos_enc_type: str = "abs"  # "abs" | "rope" | "rel_pos"
     attn_type: str = ""  # "" (fairseq MultiheadAttention) | "espnet"
     depthwise_conv_kernel_size: int = 31
+    # What feeds post_extract_proj: "conv" = the waveform conv stack + LayerNorm(512); "fbank" = DeCoAR 2.0's kaldi
+    # fbank (hamming window) + per-utterance CMVN + every second frame (s3prl/upstream/decoar2/audio.py:41-86)
+    frontend: str = "conv"
 
     @property
     def family_id(self) -> int:

@@ -59,6 +59,7 @@ def _c_config(cfg: ArchConfig) -> _lib.S3BConfig:
     if cfg.conformer:
         c.conformer = 1
         c.depthwise_kernel = int(cfg.depthwise_conv_kernel_size)
+    c.frontend = {"conv": _lib.FRONTEND_CONV, "fbank": _lib.FRONTEND_DECOAR2}[cfg.frontend]
     return c
 
 
