@@ -30,6 +30,8 @@ int main(void) {
         (const void*)s3b_conv_gemm_f32,  (const void*)s3b_posconv_f32,    (const void*)s3b_frontend_f32,
         (const void*)s3b_conformer_conv_f32, (const void*)s3b_layernorm_rope_f32, (const void*)s3b_qkv_hd_f32,
         (const void*)s3b_fbank_ex,       (const void*)s3b_melspec_ex,     (const void*)s3b_decoar2_features_f32,
+        (const void*)s3b_apc_model_create, (const void*)s3b_profile_read_ex, (const void*)s3b_apc_features_f32,
+        (const void*)s3b_gru_f32,        (const void*)s3b_gru_max_active_clusters,
     };
     s3b_config cfg;
     int64_t lens[2] = {16000, 800};
@@ -55,6 +57,24 @@ int main(void) {
         printf("valid frames of (16000, 800) samples: %d %d\n", (int)valid[0], (int)valid[1]);
         s3b_model_destroy(m);
         if (valid[0] != 49 || valid[1] != 3) return 4; /* 800 samples cover frames 0..2 (chunks of 326 samples) */
+    }
+    {
+        /* APC: one frame per kaldi fbank frame, 1 + (n - 400) / 160 */
+        s3b_apc_config acfg;
+        s3b_model* m = NULL;
+        memset(&acfg, 0, sizeof(acfg));
+        acfg.struct_size = (int32_t)sizeof(acfg), acfg.num_layers = 3, acfg.hidden = 512, acfg.residual = 1;
+        if (s3b_apc_model_create(&acfg, &m) != 0) {
+            printf("s3b_apc_model_create: %s\n", s3b_last_error());
+            return 5;
+        }
+        if (s3b_valid_frames(m, lens, 2, 16000, valid) != 0 || s3b_num_outputs(m) != 3) {
+            printf("APC bookkeeping: %s\n", s3b_last_error());
+            return 6;
+        }
+        printf("APC frames of (16000, 800) samples: %d %d\n", (int)valid[0], (int)valid[1]);
+        s3b_model_destroy(m);
+        if (valid[0] != 98 || valid[1] != 3) return 7;
     }
     return 0;
 }

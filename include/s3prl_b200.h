@@ -74,6 +74,26 @@ int s3b_device_count(void);
  * splits every GEMM weight into bf16 hi/lo, uploads to the current CUDA device. */
 int s3b_model_create(const s3b_config* cfg, s3b_model** out);
 int s3b_model_set_tensor(s3b_model* m, const char* name, const float* data, const int64_t* shape, int32_t ndim);
+
+/* APC / VQ-APC (s3prl/upstream/apc/{expert,apc,audio}.py, vq_apc/expert.py). Per utterance kaldi fbank (80 mel bins,
+ * 25 ms / 10 ms, hamming window, snip_edges), CMVN over all m frames (unbiased std), pad_sequence to T = max m, then
+ * num_layers single-layer GRUs (gate order r, z, n; h_0 = 0) over the packed sequences; layer l > 0 adds its input when
+ * residual is set. Frame t of utterance b is padding iff t >= m_b, and every output there is exactly 0.
+ * Tensors (s3b_model_set_tensor, reference key names): rnn_layers.{l}.weight_ih_l0 [3H][80 or H], .weight_hh_l0
+ * [3H][H], .bias_ih_l0 [3H], .bias_hh_l0 [3H]; other keys (postnet.*, vq_layers.*) are ignored.
+ * The model then works with s3b_model_finalize, s3b_forward / _ex / _host / _host_ex, s3b_num_frames (m of max_len),
+ * s3b_valid_frames (m_b; lens[b] >= 560 samples, since the std of one frame is NaN), s3b_default_lanes and the
+ * profile calls. s3b_num_outputs = num_layers: hidden_out holds the output of every layer ([num_layers][batch][T][H]).
+ * s3b_forward_ex refuses ffn_out and last_residual. Served: num_layers 3, hidden 512; finalize fails when the device
+ * cannot hold one cluster of the recurrence kernel (16 CTAs, 209 KB of shared memory each). */
+typedef struct s3b_apc_config {
+    int32_t struct_size; /* sizeof(s3b_apc_config) */
+    int32_t num_layers;  /* config["model"]["paras"]["num_layers"] */
+    int32_t hidden;      /* hidden_size */
+    int32_t residual;    /* residual: 0 or 1 */
+    int32_t reserved[4]; /* 0 */
+} s3b_apc_config;
+int s3b_apc_model_create(const s3b_apc_config* cfg, s3b_model** out);
 int s3b_model_finalize(s3b_model* m);
 void s3b_model_destroy(s3b_model* m);
 
@@ -151,9 +171,13 @@ int s3b_wavlm_buckets(int32_t num_buckets, int32_t max_distance, const int32_t* 
  * Conformer's GLU + depthwise conv). With profiling enabled every launch of
  * s3b_forward is bracketed by CUDA events on the launching stream; s3b_profile_read synchronises the device and
  * returns, per category, accumulated device milliseconds, ALGORITHMIC flops (2*M*N*K of the un-padded
- * contraction; 4*T^2*D per utterance and layer for attention) and kernel launches. Arrays have 5 entries. */
+ * contraction; 4*T^2*D per utterance and layer for attention) and kernel launches. Arrays have 5 entries.
+ * s3b_profile_read_ex reads the first num_categories (1..6) categories; category 5 is APC's GRU recurrence kernel
+ * (flops: 6*H*H per frame of the padded batch). reset clears all six. */
 int s3b_profile_enable(s3b_model* m, int32_t enable);
 int s3b_profile_read(s3b_model* m, double* ms, double* flops, int64_t* launches, int32_t reset);
+int s3b_profile_read_ex(s3b_model* m, int32_t num_categories, double* ms, double* flops, int64_t* launches,
+                        int32_t reset);
 /* kernels launched by s3b_forward / s3b_forward_host on this model since creation */
 int64_t s3b_launch_count(const s3b_model* m);
 
@@ -342,6 +366,20 @@ int s3b_frontend_f32(const float* const* wavs, const int64_t* lens, int32_t batc
  * out [batch][T][80], T = (1 + (max(lens) - 400) / 160 + 1) / 2, rows t >= T_b zero. */
 int s3b_decoar2_features_f32(const float* const* wavs, const int64_t* lens, int32_t batch, int32_t out_fmt, float* out,
                              void* stream);
+/* The APC front end as a forward runs it: s3b_decoar2_features_f32 without the decimation, every frame kept:
+ * out [batch][T][80], T = 1 + (max(lens) - 400) / 160, rows t >= m_b zero; lens[b] >= 560. */
+int s3b_apc_features_f32(const float* const* wavs, const int64_t* lens, int32_t batch, int32_t out_fmt, float* out,
+                         void* stream);
+/* One APC GRU layer's recurrence as a forward runs it (the model's kernel): xg [batch][t][3H] DEVICE = W_ih x + b_ih
+ * (gate order r, z, n), whh [3H][H] and bhh [3H] DEVICE (weight_hh_l0, bias_hh_l0), optional residual [batch][t][H]
+ * DEVICE added to the output, lens HOST [batch] valid frames in [0, t]. out [batch][t][H] DEVICE: h_t + residual for
+ * t < lens[b], 0 beyond. out_fmt -1 = no operand planes; 0 / 1 = the planes the model feeds the next layer's GEMM
+ * (bf16 hi/lo or f16q8), decoded to planes_out [batch][t][H]. hidden must be 512. */
+/* cudaOccupancyMaxActiveClusters of the recurrence kernel on the current device: clusters of 16 CTAs (32 hidden units
+ * and 209 KB of shared memory each) that can run at once; each runs 4 utterances. */
+int s3b_gru_max_active_clusters(int32_t* out);
+int s3b_gru_f32(const float* xg, const float* whh, const float* bhh, const float* residual, const int32_t* lens,
+                int32_t batch, int32_t t, int32_t hidden, int32_t out_fmt, float* out, float* planes_out, void* stream);
 /* The Conformer convolution module between its pointwise convs, as a forward runs it (wav2vec2_model.py:383-389):
  * x [batch][t][2d] (pointwise_conv1 output, channels-last) -> GLU (x[..., :d] * sigmoid(x[..., d:])) -> depthwise
  * Conv1d(k, padding k / 2, groups d, no bias; dw_w [d][1][k]) over each utterance's t frames -> BatchNorm1d (eval, eps

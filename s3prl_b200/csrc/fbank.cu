@@ -247,20 +247,21 @@ cudaError_t launch_fbank(const float* const* wavs_dev, const long long* lens_dev
     return cudaGetLastError();
 }
 
-// DeCoAR 2.0 CMVN + decimation (audio.py:13-38, 77-84): y = (x - mean_t) / (1e-10 + std_t) per utterance and mel bin
-// over all m_b frames (unbiased std; the odd frames that y[::2] drops count too), then rows t < T_b = (m_b + 1) / 2
-// take frame 2t. Written as operand planes [B * T][128] of post_extract_proj: columns 80..127 and rows t >= T_b zero.
+// DeCoAR 2.0 / APC CMVN (+ decimation) (decoar2/audio.py:13-38, 77-84; apc/audio.py:25-96): y = (x - mean_t) /
+// (1e-10 + std_t) per utterance and mel bin over all m_b frames (unbiased std; the frames that y[::2] drops count too),
+// then rows t < T_b = ceil(m_b / step) take frame step * t (step 2: DeCoAR 2.0's y[::2]; step 1: APC keeps every
+// frame). Written as operand planes [B * T][128] of the first GEMM: columns 80..127 and rows t >= T_b zero.
 // grid (B, 8): blockIdx.y is a 16-column slice of the operand rows (slices 5..7 only write zeros); block 256 threads.
 // The statistics are a two-pass fp64 reduction over 16 frame lanes x 16 bins.
 __global__ void __launch_bounds__(256) decoar2_cmvn_kernel(const float* __restrict__ feat,
                                                            const long long* __restrict__ lens, int max_frames, int T,
-                                                           OutPlanes op) {
+                                                           int step, OutPlanes op) {
     __shared__ double s_part[16][17];
     __shared__ float s_mean[16], s_sd[16];
     const int b = blockIdx.x, col0 = blockIdx.y * 16;
     const long long L = lens[b];
     const int m = L < kWin ? 0 : (int)(1 + (L - kWin) / kShift);
-    const int tb = (m + 1) / 2;
+    const int tb = (m + step - 1) / step;
     const bool mel = col0 < kMel;  // block-uniform
     const float* base = feat + (size_t)b * max_frames * kMel + col0;
     if (mel) {
@@ -302,7 +303,7 @@ __global__ void __launch_bounds__(256) decoar2_cmvn_kernel(const float* __restri
     for (int t = r; t < T; t += 32) {
         float y0 = 0.f, y1 = 0.f;
         if (mel && t < tb) {
-            const float2 x = *reinterpret_cast<const float2*>(base + (size_t)(2 * t) * kMel + 2 * p);
+            const float2 x = *reinterpret_cast<const float2*>(base + (size_t)(step * t) * kMel + 2 * p);
             y0 = (x.x - mean0) / den0;
             y1 = (x.y - mean1) / den1;
         }
@@ -311,11 +312,12 @@ __global__ void __launch_bounds__(256) decoar2_cmvn_kernel(const float* __restri
 }
 
 cudaError_t launch_decoar2_features(const float* const* wavs_dev, const long long* lens_dev, int B, int max_frames,
-                                    int T, float* fb, const OutPlanes& op, cudaStream_t s) {
+                                    int T, int frame_step, float* fb, const OutPlanes& op, cudaStream_t s) {
+    if (frame_step != 1 && frame_step != 2) return cudaErrorInvalidValue;
     if (max_frames <= 0 || B <= 0 || T <= 0) return cudaSuccess;
     dim3 g1((max_frames + 3) / 4, B);
     fbank_frames_kernel<true, kMel><<<g1, 128, 0, s>>>(wavs_dev, lens_dev, max_frames, fb);
-    decoar2_cmvn_kernel<<<dim3(B, kDecoar2K / 16), 256, 0, s>>>(fb, lens_dev, max_frames, T, op);
+    decoar2_cmvn_kernel<<<dim3(B, kDecoar2K / 16), 256, 0, s>>>(fb, lens_dev, max_frames, T, frame_step, op);
     return cudaGetLastError();
 }
 

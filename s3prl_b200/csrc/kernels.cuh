@@ -53,10 +53,34 @@ static constexpr int kDecoar2K = 128;
 // builds the fbank tables and the hamming window on the current device (synchronous; once per device)
 cudaError_t init_fbank_tables();
 // kaldi fbank with the hamming window into fb [B][max_frames][80] (frames t < m_b of each utterance), then CMVN over
-// each utterance's m_b frames and y[::2] into operand planes op [B * T][kDecoar2K] (zero beyond 80 columns and T_b rows).
-// Needs init_fbank_tables() on this device first. m_b >= 2 (m_b == 1 gives NaN, as the reference's unbiased std).
+// each utterance's m_b frames and y[::frame_step] into operand planes op [B * T][kDecoar2K] (zero beyond 80 columns and
+// T_b = ceil(m_b / frame_step) rows). frame_step: 2 for DeCoAR 2.0, 1 for APC. Needs init_fbank_tables() on this
+// device first. m_b >= 2 (m_b == 1 gives NaN, as the reference's unbiased std).
 cudaError_t launch_decoar2_features(const float* const* wavs_dev, const long long* lens_dev, int B, int max_frames,
-                                    int T, float* fb, const OutPlanes& op, cudaStream_t s);
+                                    int T, int frame_step, float* fb, const OutPlanes& op, cudaStream_t s);
+
+// ---- gru.cu: the GRU recurrence of APC / VQ-APC (cluster-resident W_hh) ------------------------------------------
+static constexpr int kGruHidden = 512;  // hidden size the kernel is built for
+static constexpr int kGruGroup = 4;     // utterances per cluster
+static constexpr int kGruCtas = 16;     // CTAs per cluster (non-portable cluster size), 32 hidden units each
+struct GruParams {
+    const float* xg;   // [B][T][3H]: W_i x + b_i, with b_hr / b_hz added to the r / z columns (gate order r, z, n)
+    const float* whh;  // [3H][H] weight_hh_l0
+    const float* bhn;  // [H] the n third of bias_hh_l0
+    const float* res;  // optional [B][T][H]: added to the layer output (the residual), not to the state
+    const int* len;    // [B] valid frames; frames t >= len[b] are written as zero
+    const int* order;  // [B] utterance indices, longest first: cluster g runs order[4g .. 4g + 3]
+    int B, T;
+    float* out;        // [B][T][H] layer output (fp32)
+    OutPlanes op;      // optional [B * T][H] operand planes of the same values (op.hi null: none)
+};
+cudaError_t launch_gru(const GruParams& p, cudaStream_t s);
+// clusters of the recurrence kernel that can be co-resident on the current device (0: the kernel cannot run)
+cudaError_t gru_max_active_clusters(int* n);
+size_t gru_smem_bytes();
+// xg[r][q * H + u] += bhh[q * H + u] for q in {0, 1} (r, z) and rows r < rows: the bias folding the model does in its
+// GEMM epilogue, for the building-block entry point
+cudaError_t launch_gru_fold_bias(float* xg, const float* bhh, size_t rows, cudaStream_t s);
 
 // ---- peer.cu: fused weighted sum + push all-gather over peer memory --------------------------------------------------
 cudaError_t launch_weighted_sum_push(const float* hs, int NL, size_t n_per_layer, size_t layer_stride, const float* w,

@@ -17,6 +17,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <map>
 #include <string>
 #include <vector>
@@ -142,10 +143,15 @@ struct LayerW {
     // ln1 = self_attn_layer_norm, ln2 = final_layer_norm; dw_w / dw_b the depthwise taps with BatchNorm folded in
     SplitBuf v, ffn1_w1, ffn1_w2, pw1, pw2;
     DevBuf ffn1_b1, ffn1_b2, ffn1_ln_g, ffn1_ln_b, ffn2_ln_g, ffn2_ln_b, conv_ln_g, conv_ln_b, dw_w, dw_b;
+    // APC GRU layer: wih = weight_ih_l0 [3H][K] (layer 0: K = 80 zero-padded to kDecoar2K), gru_b = bias_ih_l0 with
+    // bias_hh_l0's r and z thirds added (the input GEMM's bias), whh = weight_hh_l0 [3H][H] fp32, bhn = bias_hh_l0[2H:]
+    SplitBuf wih;
+    DevBuf gru_b, whh, bhn;
 };
 
 // per-category device-time profile (CUDA events around each launch on the launching stream)
-enum { CAT_GEMM = 0, CAT_ATTN = 1, CAT_CONV0 = 2, CAT_NORM = 3, CAT_MISC = 4, CAT_COUNT = 5 };
+// CAT_GRU (APC's recurrence) is read through s3b_profile_read_ex only: s3b_profile_read fills five entries
+enum { CAT_GEMM = 0, CAT_ATTN = 1, CAT_CONV0 = 2, CAT_NORM = 3, CAT_MISC = 4, CAT_GRU = 5, CAT_COUNT = 6 };
 struct ProfRec {
     int cat;
     cudaEvent_t a, b;
@@ -155,9 +161,9 @@ struct Profiler {
     std::vector<cudaEvent_t> pool;
     std::vector<ProfRec> recs;
     cudaEvent_t pending = nullptr;
-    double ms[CAT_COUNT] = {0, 0, 0, 0, 0};
-    double flops[CAT_COUNT] = {0, 0, 0, 0, 0};
-    long long launches[CAT_COUNT] = {0, 0, 0, 0, 0};
+    double ms[CAT_COUNT] = {};
+    double flops[CAT_COUNT] = {};
+    long long launches[CAT_COUNT] = {};
     cudaEvent_t get() {
         if (!pool.empty()) {
             cudaEvent_t e = pool.back();
@@ -184,7 +190,8 @@ struct Workspace {
     cudaEvent_t book_copied = nullptr;  // the previous call's H2D copy has been consumed: the mirror may be rewritten
     DevBuf wav_stats, wav_pad, c0_part, c0_ss, conv_f32, tmp_f32, x_f32, x1_f32, gate, pos_z, ln_counters, hs0;
     DevBuf glu_f32;  // Conformer: pointwise_conv1 output [M][2D]
-    DevBuf fb_f32;   // DeCoAR 2.0: log-mel frames [B][m(Lmax)][80]
+    DevBuf fb_f32;   // DeCoAR 2.0 / APC: log-mel frames [B][m(Lmax)][80]
+    DevBuf xg_f32;   // APC: the input GEMM's output [M][3H]
     SplitBuf act[kNumConv], ln512_s, x_s, xs_s, q_s, k_s, vt_s, ctx_s, x1_s, h_s;
     cudaStream_t stream = nullptr;  // lane stream (lane 1; lane 0 runs on the caller's stream)
     cudaEvent_t done = nullptr;
@@ -194,6 +201,9 @@ struct Workspace {
 
 struct s3b_model {
     s3b_config cfg;
+    // APC / VQ-APC (s3b_apc_model_create): cfg then holds num_layers and embed_dim = hidden, everything else zero
+    bool apc = false;
+    int apc_residual = 0;
     std::map<std::string, HostTensor> host;
     bool finalized = false;
     int sm_count = 132;
@@ -300,8 +310,11 @@ static const int64_t kDecoar2MinLen = 560;  // two fbank frames: the unbiased st
 static int64_t decoar2_frames(int64_t L) { return L < 400 ? 0 : (1 + (L - 400) / 160 + 1) / 2; }
 static int64_t fbank_frames(int64_t L) { return L < 400 ? 0 : 1 + (L - 400) / 160; }
 static bool decoar2(const s3b_model* m) { return m != nullptr && m->cfg.frontend == 1; }
+static bool apc(const s3b_model* m) { return m != nullptr && m->apc; }
 // frames of a batch padded to L for this model's front end (m NULL: the conv stack)
-static int64_t model_frames(const s3b_model* m, int64_t L) { return decoar2(m) ? decoar2_frames(L) : num_frames(L); }
+static int64_t model_frames(const s3b_model* m, int64_t L) {
+    return apc(m) ? fbank_frames(L) : decoar2(m) ? decoar2_frames(L) : num_frames(L);
+}
 
 // ------------------------------------------------------------------------------------------------
 // C ABI: library
@@ -391,6 +404,25 @@ extern "C" int s3b_model_create(const s3b_config* cfg, s3b_model** out) {
     return 0;
 }
 
+extern "C" int s3b_apc_model_create(const s3b_apc_config* cfg, s3b_model** out) {
+    if (!cfg || !out) return fail("null argument");
+    if (cfg->struct_size != (int32_t)sizeof(s3b_apc_config))
+        return fail("s3b_apc_config.struct_size %d != %d (header / library mismatch)", cfg->struct_size,
+                    (int)sizeof(s3b_apc_config));
+    if (cfg->num_layers != 3) return fail("num_layers %d: the APC model is served with 3 GRU layers", cfg->num_layers);
+    if (cfg->hidden != kGruHidden) return fail("hidden %d: the APC model is served with hidden size %d", cfg->hidden, kGruHidden);
+    if (cfg->residual != 0 && cfg->residual != 1) return fail("residual must be 0 or 1, not %d", cfg->residual);
+    for (int i = 0; i < 4; ++i)
+        if (cfg->reserved[i] != 0) return fail("s3b_apc_config.reserved[%d] must be 0", i);
+    s3b_model* m = new s3b_model();
+    memset(&m->cfg, 0, sizeof(m->cfg));
+    m->cfg.num_layers = cfg->num_layers, m->cfg.embed_dim = cfg->hidden;
+    m->apc = true, m->apc_residual = cfg->residual;
+    m->scheme = default_scheme();
+    *out = m;
+    return 0;
+}
+
 extern "C" int s3b_model_set_tensor(s3b_model* m, const char* name, const float* data, const int64_t* shape,
                                     int32_t ndim) {
     if (!m || !name || !data || (!shape && ndim > 0)) return fail("null argument");
@@ -419,11 +451,11 @@ extern "C" void s3b_model_destroy(s3b_model* m) {
     m->pred1_b.release(), m->pred2_b.release();
     for (LayerW& l : m->layers) {
         l.qkv.release(), l.out.release(), l.fc1.release(), l.fc2.release();
-        l.v.release(), l.ffn1_w1.release(), l.ffn1_w2.release(), l.pw1.release(), l.pw2.release();
+        l.v.release(), l.ffn1_w1.release(), l.ffn1_w2.release(), l.pw1.release(), l.pw2.release(), l.wih.release();
         DevBuf* lb[] = {&l.qkv_b,     &l.out_b,     &l.fc1_b,     &l.fc2_b,     &l.ln1_g,     &l.ln1_b,
                         &l.ln2_g,     &l.ln2_b,     &l.grep_w,    &l.grep_b,    &l.grep_a,    &l.ffn1_b1,
                         &l.ffn1_b2,   &l.ffn1_ln_g, &l.ffn1_ln_b, &l.ffn2_ln_g, &l.ffn2_ln_b, &l.conv_ln_g,
-                        &l.conv_ln_b, &l.dw_w,      &l.dw_b};
+                        &l.conv_ln_b, &l.dw_w,      &l.dw_b,      &l.gru_b,     &l.whh,       &l.bhn};
         for (DevBuf* b : lb) b->release();
     }
     for (Workspace& w : m->ws) w.release();
@@ -610,6 +642,41 @@ static std::vector<float> posconv4_weight_layout(const float* w, int D, int G, i
     return w4;
 }
 
+// APC (apc.py:36-48): rnn_layers.{l} = nn.GRU(in, H) with in = 80 for layer 0 and H after it. The recurrence kernel
+// must be able to run at all: clusters of 16 CTAs with 209 KB of shared memory each.
+static int finalize_apc(s3b_model* m) {
+    const int NL = m->cfg.num_layers, H = m->cfg.embed_dim;
+    m->layers.resize(NL);
+    for (int l = 0; l < NL; ++l) {
+        LayerW& L = m->layers[l];
+        const std::string p = "rnn_layers." + std::to_string(l) + ".";
+        const int in = l == 0 ? 80 : H, K = l == 0 ? kDecoar2K : H;
+        const HostTensor *wih, *whh, *bih, *bhh;
+        S3B_OK(need(m, p + "weight_ih_l0", {3 * H, in}, &wih));
+        S3B_OK(need(m, p + "weight_hh_l0", {3 * H, H}, &whh));
+        S3B_OK(need(m, p + "bias_ih_l0", {3 * H}, &bih));
+        S3B_OK(need(m, p + "bias_hh_l0", {3 * H}, &bhh));
+        std::vector<float> w((size_t)3 * H * K, 0.f);
+        for (int o = 0; o < 3 * H; ++o) memcpy(&w[(size_t)o * K], &wih->data[(size_t)o * in], in * sizeof(float));
+        S3B_OK(upload_split(L.wih, w.data(), w.size(), m->scheme));
+        // b_hr, b_hz sit outside r * (.) and fold into the GEMM's bias; b_hn does not
+        std::vector<float> b(bih->data);
+        for (int i = 0; i < 2 * H; ++i) b[i] += bhh->data[i];
+        S3B_OK(upload_f32(L.gru_b, b.data(), b.size()));
+        S3B_OK(upload_f32(L.whh, whh->data.data(), whh->numel()));
+        S3B_OK(upload_f32(L.bhn, bhh->data.data() + 2 * H, H));
+    }
+    int clusters = 0;
+    CUDA_OK(gru_max_active_clusters(&clusters));
+    if (clusters < 1)
+        return fail("the GRU recurrence kernel cannot run on this device: cudaOccupancyMaxActiveClusters reports 0 "
+                    "clusters of %d CTAs with %zu bytes of shared memory each", kGruCtas, gru_smem_bytes());
+    CUDA_OK(init_fbank_tables());
+    m->host.clear();
+    m->finalized = true;
+    return 0;
+}
+
 extern "C" int s3b_model_finalize(s3b_model* m) {
     if (!m) return fail("null model");
     if (m->finalized) return 0;
@@ -622,6 +689,7 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
         return fail("device is sm_%d%d; this library contains sm_90a code only", prop.major, prop.minor);
     m->sm_count = prop.multiProcessorCount;
     g_sm_count = m->sm_count;
+    if (apc(m)) return finalize_apc(m);
 
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, F = c.ffn_dim, C = kConvDim;
@@ -799,6 +867,7 @@ extern "C" int64_t s3b_num_frames(const s3b_model* m, int64_t max_len) {
 }
 
 extern "C" int32_t s3b_num_outputs(const s3b_model* m) {
+    if (apc(m)) return m->cfg.num_layers;  // the output of every GRU layer (+ residual)
     return m ? m->cfg.num_layers + 1 + m->cfg.pred_heads : -1;
 }
 
@@ -806,10 +875,14 @@ extern "C" int s3b_valid_frames(const s3b_model* m, const int64_t* lens, int32_t
                                 int32_t* valid) {
     if (!m || !lens || !valid) return fail("null argument");
     const int64_t T = model_frames(m, max_len);
-    if (T <= 0) return fail("max_len %lld too short for the %s", (long long)max_len, decoar2(m) ? "fbank" : "conv stack");
+    if (T <= 0)
+        return fail("max_len %lld too short for the %s", (long long)max_len, decoar2(m) || apc(m) ? "fbank" : "conv stack");
     bool any_pad = false;
     for (int b = 0; b < batch; ++b) {
         if (lens[b] < 1 || lens[b] > max_len) return fail("lens[%d]=%lld out of range", b, (long long)lens[b]);
+        if (apc(m) && lens[b] < kDecoar2MinLen)
+            return fail("lens[%d]=%lld: APC needs >= %lld samples (2 fbank frames; the CMVN std of one frame is NaN)", b,
+                        (long long)lens[b], (long long)kDecoar2MinLen);
         if (decoar2(m) && lens[b] < kDecoar2MinLen)
             return fail("lens[%d]=%lld: DeCoAR 2.0 needs >= %lld samples (2 fbank frames; the CMVN std of one frame is NaN)",
                         b, (long long)lens[b], (long long)kDecoar2MinLen);
@@ -817,7 +890,9 @@ extern "C" int s3b_valid_frames(const s3b_model* m, const int64_t* lens, int32_t
     }
     for (int b = 0; b < batch; ++b) {
         int64_t v;
-        if (decoar2(m)) {
+        if (apc(m)) {
+            v = fbank_frames(lens[b]);  // pad_sequence of the per-utterance features (apc/expert.py:47-51)
+        } else if (decoar2(m)) {
             v = decoar2_frames(lens[b]);  // pad_sequence of the per-utterance features (decoar2/expert.py:81-92)
         } else if (m->cfg.family == 1) {
             // wav2vec2: conv-length rule, only when the batch has any padding (wav2vec2_model.py:2652-2671). The
@@ -1185,11 +1260,12 @@ struct Plan {
     std::vector<LayerPlan> layers;
     GemmParams pred1;                // Distiller: Linear(D, N*D) + GELU
     std::vector<GemmParams> pred2;   // Distiller: SplitLinear, one [D][D] GEMM per task
+    std::vector<GemmParams> gru_in;  // APC: the input projection of every GRU layer
 };
 
 void Workspace::release() {
     DevBuf* bufs[] = {&book, &wav_stats, &wav_pad, &c0_part, &c0_ss, &conv_f32, &tmp_f32, &x_f32, &x1_f32, &gate, &pos_z,
-                      &ln_counters, &hs0, &glu_f32, &fb_f32};
+                      &ln_counters, &hs0, &glu_f32, &fb_f32, &xg_f32};
     for (DevBuf* b : bufs) b->release();
     for (int i = 0; i < kNumConv; ++i) act[i].release();
     SplitBuf* sb[] = {&ln512_s, &x_s, &xs_s, &q_s, &k_s, &vt_s, &ctx_s, &x1_s, &h_s};
@@ -1235,12 +1311,14 @@ struct Fwd {
     const float** d_wavs = nullptr;
     long long* d_lens = nullptr;
     int* d_kv = nullptr;
+    int* d_ord = nullptr;  // APC: utterances longest first (the recurrence kernel's grouping)
     uint8_t* d_mask = nullptr;
     int fuse_ln = 0;  // fuse_ln_mode()
     unsigned int* cnt[2] = {nullptr, nullptr};  // two alternating row-block counter arrays of the fused LayerNorm
 
     static constexpr int kConformerStages = 10;  // stages per Conformer layer (conformer_stage)
     int num_stages() const {
+        if (apc(m)) return 1 + 2 * m->cfg.num_layers;  // front end, then per layer: input GEMM, recurrence
         if (m->cfg.conformer) return 9 + kConformerStages * m->cfg.num_layers;
         return 9 + 5 * m->cfg.num_layers + (m->cfg.pred_heads > 0 ? 1 + m->cfg.pred_heads : 0);
     }
@@ -1257,6 +1335,7 @@ struct Fwd {
     int build_conformer_layer(LayerPlan& lp, int l);
     int stage(int s);
     int conformer_stage(int l, int sub);
+    int apc_stage(int s);
     float* hs(int l) const { return (distil() && l == 0) ? w->hs0.as<float>() : slot(l); }
 };
 
@@ -1264,7 +1343,7 @@ int Fwd::prepare() {
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, C = kConvDim;
     if (B < 1) return fail("empty batch");
-    const bool fb = decoar2(m);
+    const bool fb = decoar2(m) || apc(m);
     {
         int64_t cur = Lmax;
         for (int i = 0; i < kNumConv; ++i) cur = L[i] = fb ? 0 : conv_out_len(cur, i);
@@ -1283,7 +1362,8 @@ int Fwd::prepare() {
     // ---- bookkeeping block: pinned host mirror -> one async copy ---------------------------------------------
     const size_t off_lens = (size_t)B * sizeof(void*);
     const size_t off_kv = off_lens + (size_t)B * sizeof(long long);
-    const size_t off_mask = (off_kv + (size_t)B * sizeof(int) + 15) & ~(size_t)15;
+    const size_t off_ord = off_kv + (size_t)B * sizeof(int);
+    const size_t off_mask = (off_ord + (apc(m) ? (size_t)B * sizeof(int) : 0) + 15) & ~(size_t)15;
     const size_t book_bytes = off_mask + (size_t)M;
     S3B_OK(w->book.ensure(book_bytes));
     if (w->book_host_bytes < book_bytes) {
@@ -1309,6 +1389,13 @@ int Fwd::prepare() {
         for (int b = 0; b < B; ++b) hl[b] = (long long)lens[b];
         for (int b = 0; b < B; ++b)
             for (int t = hk[b]; t < T; ++t) hm[(size_t)b * T + t] = 1;
+        if (apc(m)) {  // group utterances of similar length: a recurrence cluster stops at its own longest
+            int* ho = reinterpret_cast<int*>(hb + off_ord);
+            std::vector<int> ord(B);
+            for (int b = 0; b < B; ++b) ord[b] = b;
+            std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return hk[a] > hk[b]; });
+            memcpy(ho, ord.data(), (size_t)B * sizeof(int));
+        }
         if (w->book_valid != book_bytes || memcmp(w->book_host, hb, book_bytes) != 0) {
             CUDA_OK(cudaEventSynchronize(w->book_copied));  // normally long complete
             memcpy(w->book_host, hb, book_bytes);
@@ -1319,10 +1406,16 @@ int Fwd::prepare() {
     d_wavs = reinterpret_cast<const float**>(db);
     d_lens = reinterpret_cast<long long*>(db + off_lens);
     d_kv = reinterpret_cast<int*>(db + off_kv);
+    d_ord = reinterpret_cast<int*>(db + off_ord);
     d_mask = reinterpret_cast<uint8_t*>(db + off_mask);
 
     // ---- workspace ------------------------------------------------------------------------------------------
-    if (fb) {
+    if (apc(m)) {
+        S3B_OK(w->fb_f32.ensure((size_t)B * T * 80 * 4));
+        S3B_OK(w->ln512_s.ensure((size_t)M * kDecoar2K));  // layer 0's GEMM operand: the CMVN kernel's planes
+        S3B_OK(w->x_s.ensure((size_t)M * D));             // layers 1..: the recurrence kernel's planes
+        S3B_OK(w->xg_f32.ensure((size_t)M * 3 * D * 4));
+    } else if (fb) {
         S3B_OK(w->fb_f32.ensure((size_t)B * fbank_frames(Lmax) * 80 * 4));
         S3B_OK(w->ln512_s.ensure((size_t)M * kDecoar2K));  // post_extract_proj's A operand: the CMVN kernel's planes
     } else {
@@ -1334,21 +1427,23 @@ int Fwd::prepare() {
         S3B_OK(w->conv_f32.ensure((size_t)B * (c.extractor_layer_norm ? L[1] : L[6]) * C * 4));
         S3B_OK(w->ln512_s.ensure((size_t)M * C));
     }
-    S3B_OK(w->tmp_f32.ensure((size_t)M * D * 4));
-    S3B_OK(w->x_f32.ensure((size_t)M * D * 4));
-    S3B_OK(w->x1_f32.ensure((size_t)M * D * 4));
-    S3B_OK(w->x_s.ensure((size_t)M * D));
-    S3B_OK(w->xs_s.ensure((size_t)M * D));
-    S3B_OK(w->x1_s.ensure((size_t)M * D));
-    S3B_OK(w->ctx_s.ensure((size_t)M * D));
-    S3B_OK(w->q_s.ensure((size_t)M * D));
-    S3B_OK(w->k_s.ensure((size_t)M * D));
-    S3B_OK(w->vt_s.ensure((size_t)D * B * Tp));
-    S3B_OK(w->h_s.ensure((size_t)M * F));
-    if (c.conformer) S3B_OK(w->glu_f32.ensure((size_t)M * 2 * D * sizeof(float)));
-    else if (posconv4_ok(c)) S3B_OK(w->pos_z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
-    if (c.relative_position) S3B_OK(w->gate.ensure((size_t)B * H * T * 4));
-    if (c.family == 3) S3B_OK(w->hs0.ensure((size_t)M * D * 4));
+    if (!apc(m)) {  // the encoder's buffers
+        S3B_OK(w->tmp_f32.ensure((size_t)M * D * 4));
+        S3B_OK(w->x_f32.ensure((size_t)M * D * 4));
+        S3B_OK(w->x1_f32.ensure((size_t)M * D * 4));
+        S3B_OK(w->x_s.ensure((size_t)M * D));
+        S3B_OK(w->xs_s.ensure((size_t)M * D));
+        S3B_OK(w->x1_s.ensure((size_t)M * D));
+        S3B_OK(w->ctx_s.ensure((size_t)M * D));
+        S3B_OK(w->q_s.ensure((size_t)M * D));
+        S3B_OK(w->k_s.ensure((size_t)M * D));
+        S3B_OK(w->vt_s.ensure((size_t)D * B * Tp));
+        S3B_OK(w->h_s.ensure((size_t)M * F));
+        if (c.conformer) S3B_OK(w->glu_f32.ensure((size_t)M * 2 * D * sizeof(float)));
+        else if (posconv4_ok(c)) S3B_OK(w->pos_z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
+        if (c.relative_position) S3B_OK(w->gate.ensure((size_t)B * H * T * 4));
+        if (c.family == 3) S3B_OK(w->hs0.ensure((size_t)M * D * 4));
+    }
     fuse_ln = fuse_ln_mode();
     {
         const size_t n_cnt = (size_t)B * (L[1] / 128 + 2) + (size_t)M / 128 + 16;
@@ -1482,6 +1577,20 @@ int Fwd::build_conformer_layer(LayerPlan& lp, int l) {
 int Fwd::build_plan(Plan& pl) {
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, NL = c.num_layers, C = kConvDim;
+    if (apc(m)) {
+        // x_g = x W_ih^T + (b_ih + [b_hr, b_hz, 0]) over all B * T rows, fp32 [M][3D] (the recurrence ignores t >= m_b)
+        pl.gru_in.resize(NL);
+        for (int l = 0; l < NL; ++l) {
+            GemmParams& p = pl.gru_in[l];
+            S3B_OK(linear_params(p, l == 0 ? w->ln512_s : w->x_s, m->layers[l].wih, M, 3 * D, l == 0 ? kDecoar2K : D, 0,
+                                 m->scheme));
+            Epi e;
+            e.bias = m->layers[l].gru_b.as<float>();
+            e.out_f32 = w->xg_f32.as<float>();
+            set_epi(p, e, 3 * D);
+        }
+        return 0;
+    }
     for (int i = 1; i < kNumConv && !decoar2(m); ++i) {
         GemmParams& p = pl.conv[i];
         S3B_OK(conv_params(p, w->act[i - 1], m->conv_w[i], B, L[i - 1], L[i], kConvK[i], m->scheme));
@@ -1625,7 +1734,41 @@ int Fwd::build_plan(Plan& pl) {
     return 0;
 }
 
+// APC: stage 0 = fbank + CMVN into layer 0's operand planes; stage 1 + 2l = layer l's input GEMM; stage 2 + 2l = its
+// recurrence, which writes hidden state l (+ layer l's input when residual, l > 0) and layer l + 1's operand planes
+int Fwd::apc_stage(int s) {
+    s3b_model* m = this->m;  // the launch macros expect `m` and `st`
+    cudaStream_t st = this->st;
+    const int D = m->cfg.embed_dim, NL = m->cfg.num_layers;
+    if (s == 0) {
+        const size_t book_bytes = (size_t)(reinterpret_cast<char*>(d_mask) - w->book.as<char>()) + (size_t)M;
+        CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host, book_bytes, cudaMemcpyHostToDevice, st));
+        if (!capturing) CUDA_OK(cudaEventRecord(w->book_copied, st));
+        KLAUNCH(CAT_CONV0, 2, 0.0, launch_decoar2_features(d_wavs, d_lens, B, T, T, 1, w->fb_f32.as<float>(),
+                                                           w->ln512_s.planes(m->scheme), st));
+        return 0;
+    }
+    const int l = (s - 1) / 2;
+    if (l >= NL) return fail("internal: stage %d out of range", s);
+    if ((s - 1) % 2 == 0) {
+        GemmParams p = plan->gru_in[l];
+        KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+        return 0;
+    }
+    const LayerW& W = m->layers[l];
+    GruParams g;
+    g.xg = w->xg_f32.as<float>(), g.whh = W.whh.as<float>(), g.bhn = W.bhn.as<float>();
+    g.res = (m->apc_residual && l > 0) ? slot(l - 1) : nullptr;
+    g.len = d_kv, g.order = d_ord, g.B = B, g.T = T;
+    g.out = slot(l);
+    g.op = l + 1 < NL ? w->x_s.planes(m->scheme) : no_planes();
+    KLAUNCH(CAT_GRU, 1, 2.0 * 3 * D * D * (double)M, launch_gru(g, st));
+    if (layer_done) S3B_OK(layer_done(m, l, st, user));
+    return 0;
+}
+
 int Fwd::stage(int s) {
+    if (apc(m)) return apc_stage(s);
     s3b_model* m = this->m;  // the launch macros expect `m` and `st`
     cudaStream_t st = this->st;
     const s3b_config& c = m->cfg;
@@ -1638,7 +1781,7 @@ int Fwd::stage(int s) {
         CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host, book_bytes, cudaMemcpyHostToDevice, st));
         if (!capturing) CUDA_OK(cudaEventRecord(w->book_copied, st));  // (graph replay: recorded after the launch)
         if (decoar2(m)) {  // fbank frames + CMVN / y[::2] -> post_extract_proj's operand planes (profile category 2)
-            KLAUNCH(CAT_CONV0, 2, 0.0, launch_decoar2_features(d_wavs, d_lens, B, (int)fbank_frames(Lmax), T,
+            KLAUNCH(CAT_CONV0, 2, 0.0, launch_decoar2_features(d_wavs, d_lens, B, (int)fbank_frames(Lmax), T, 2,
                                                                w->fb_f32.as<float>(), w->ln512_s.planes(m->scheme), st));
             return 0;
         }
@@ -1921,7 +2064,7 @@ static int forward_lanes(s3b_model* m, const float* const* wavs, const int64_t* 
     if (B < 1) return fail("empty batch");
     const int64_t T = model_frames(m, Lmax);
     if (T < 1) return fail("max_len %lld too short: the %s yields no frame", (long long)Lmax,
-                           decoar2(m) ? "fbank" : "conv stack");
+                           decoar2(m) || apc(m) ? "fbank" : "conv stack");
     int lanes = (o && o->lanes > 0) ? o->lanes : default_lanes(B, T);
     if (lanes > 2) lanes = 2;
     if (lanes > B) lanes = B;
@@ -2057,6 +2200,8 @@ extern "C" int s3b_forward_ex(s3b_model* m, const float* const* wavs, const int6
         if (lens[b] > max_len) return fail("lens[%d]=%lld exceeds max_len", b, (long long)lens[b]);
     if (m->cfg.conformer && opts != nullptr && (opts->ffn_out != nullptr || opts->last_residual != nullptr))
         return fail("ffn_out / last_residual: a Conformer encoder collects no layer results (wav2vec2_model.py:3199-3200)");
+    if (apc(m) && opts != nullptr && (opts->ffn_out != nullptr || opts->last_residual != nullptr))
+        return fail("ffn_out / last_residual: an APC model is a GRU stack, it has no feed-forward blocks or layer results");
     return forward_lanes(m, wavs, lens, batch, max_len, hidden_out, (cudaStream_t)stream, opts);
 }
 
@@ -2155,8 +2300,10 @@ extern "C" int s3b_profile_enable(s3b_model* m, int32_t enable) {
     return 0;
 }
 
-extern "C" int s3b_profile_read(s3b_model* m, double* ms, double* flops, int64_t* launches, int32_t reset) {
+extern "C" int s3b_profile_read_ex(s3b_model* m, int32_t num_categories, double* ms, double* flops, int64_t* launches,
+                                   int32_t reset) {
     if (!m || !ms || !flops || !launches) return fail("null argument");
+    if (num_categories < 1 || num_categories > CAT_COUNT) return fail("num_categories must be 1..%d", (int)CAT_COUNT);
     CUDA_OK(cudaDeviceSynchronize());
     for (ProfRec& r : m->prof.recs) {
         float t = 0.f;
@@ -2167,10 +2314,14 @@ extern "C" int s3b_profile_read(s3b_model* m, double* ms, double* flops, int64_t
     }
     m->prof.recs.clear();
     for (int c = 0; c < CAT_COUNT; ++c) {
-        ms[c] = m->prof.ms[c], flops[c] = m->prof.flops[c], launches[c] = m->prof.launches[c];
+        if (c < num_categories) ms[c] = m->prof.ms[c], flops[c] = m->prof.flops[c], launches[c] = m->prof.launches[c];
         if (reset) m->prof.ms[c] = 0, m->prof.flops[c] = 0, m->prof.launches[c] = 0;
     }
     return 0;
+}
+
+extern "C" int s3b_profile_read(s3b_model* m, double* ms, double* flops, int64_t* launches, int32_t reset) {
+    return s3b_profile_read_ex(m, 5, ms, flops, launches, reset);
 }
 
 extern "C" int64_t s3b_launch_count(const s3b_model* m) { return m ? m->launches_total : -1; }
@@ -2763,9 +2914,10 @@ extern "C" int s3b_frontend_f32(const float* const* wavs, const int64_t* lens, i
     return r;
 }
 
-extern "C" int s3b_decoar2_features_f32(const float* const* wavs, const int64_t* lens, int32_t B, int32_t out_fmt,
-                                        float* out, void* stream) {
-    // Fwd::stage(0) of a DeCoAR 2.0 model on workspaces of this call; the operand planes decoded, columns 0..79 kept
+// Fwd::stage(0) of a DeCoAR 2.0 (step 2) or APC (step 1) model on workspaces of this call; the operand planes
+// decoded, columns 0..79 kept
+static int fbank_cmvn_features(const float* const* wavs, const int64_t* lens, int32_t B, int step, int32_t out_fmt,
+                               float* out, void* stream) {
     if (!wavs || !lens || !out) return fail("null argument");
     if (B < 1) return fail("bad batch %d", B);
     if (out_fmt != 0 && out_fmt != 1) return fail("out_fmt must be 0 (bf16 hi/lo) or 1 (f16q8), not %d", out_fmt);
@@ -2773,11 +2925,12 @@ extern "C" int s3b_decoar2_features_f32(const float* const* wavs, const int64_t*
     for (int b = 0; b < B; ++b) {
         if (wavs[b] == nullptr) return fail("null argument: wavs[%d]", b);
         if (lens[b] < kDecoar2MinLen)
-            return fail("lens[%d] = %lld: DeCoAR 2.0 needs >= %lld samples (2 fbank frames)", b, (long long)lens[b],
+            return fail("lens[%d] = %lld: %s needs >= %lld samples (2 fbank frames)", b, (long long)lens[b],
+                        step == 1 ? "APC" : "DeCoAR 2.0",
                         (long long)kDecoar2MinLen);
         max_len = lens[b] > max_len ? lens[b] : max_len;
     }
-    const int64_t mf = fbank_frames(max_len), T = decoar2_frames(max_len);
+    const int64_t mf = fbank_frames(max_len), T = step == 1 ? mf : decoar2_frames(max_len);
     if ((int64_t)B * mf > 2000000000LL) return fail("batch too large for 32-bit indexing");
     if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
     CUDA_OK(init_fbank_tables());
@@ -2794,7 +2947,7 @@ extern "C" int s3b_decoar2_features_f32(const float* const* wavs, const int64_t*
         S3B_OK(fbuf.ensure((size_t)B * mf * 80 * 4));
         S3B_OK(os.ensure(rows * kDecoar2K));
         S3B_OK(dec.ensure(rows * kDecoar2K * 4));
-        CUDA_OK(launch_decoar2_features(book.as<const float*>(), d_lens, B, (int)mf, (int)T, fbuf.as<float>(),
+        CUDA_OK(launch_decoar2_features(book.as<const float*>(), d_lens, B, (int)mf, (int)T, step, fbuf.as<float>(),
                                         os.planes(out_fmt), st));
         CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), rows * kDecoar2K, dec.as<float>(), st));
         CUDA_OK(cudaMemcpy2DAsync(out, 80 * sizeof(float), dec.p, kDecoar2K * sizeof(float), 80 * sizeof(float), rows,
@@ -2803,6 +2956,73 @@ extern "C" int s3b_decoar2_features_f32(const float* const* wavs, const int64_t*
         return 0;
     }();
     book.release(), fbuf.release(), dec.release(), os.release();
+    return r;
+}
+
+extern "C" int s3b_decoar2_features_f32(const float* const* wavs, const int64_t* lens, int32_t B, int32_t out_fmt,
+                                        float* out, void* stream) {
+    return fbank_cmvn_features(wavs, lens, B, 2, out_fmt, out, stream);
+}
+
+extern "C" int s3b_apc_features_f32(const float* const* wavs, const int64_t* lens, int32_t B, int32_t out_fmt,
+                                    float* out, void* stream) {
+    return fbank_cmvn_features(wavs, lens, B, 1, out_fmt, out, stream);
+}
+
+extern "C" int s3b_gru_max_active_clusters(int32_t* out) {
+    if (!out) return fail("null argument");
+    if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
+    int n = 0;
+    CUDA_OK(gru_max_active_clusters(&n));
+    *out = n;
+    return 0;
+}
+
+extern "C" int s3b_gru_f32(const float* xg, const float* whh, const float* bhh, const float* residual,
+                           const int32_t* lens, int32_t B, int32_t T, int32_t hidden, int32_t out_fmt, float* out,
+                           float* planes_out, void* stream) {
+    // Fwd::apc_stage(2 + 2l) on this call's buffers: b_hr / b_hz added to a copy of xg as the model's GEMM bias adds
+    // them, utterances grouped longest first as the model groups them
+    if (!xg || !whh || !bhh || !lens || !out) return fail("null argument");
+    if (hidden != kGruHidden) return fail("hidden %d: the recurrence kernel is built for %d", hidden, kGruHidden);
+    if (B < 1 || T < 1) return fail("bad sizes (batch %d, t %d)", B, T);
+    if (out_fmt < -1 || out_fmt > 1) return fail("out_fmt must be -1 (none), 0 (bf16 hi/lo) or 1 (f16q8), not %d", out_fmt);
+    if (out_fmt >= 0 && planes_out == nullptr) return fail("out_fmt %d needs planes_out", out_fmt);
+    for (int b = 0; b < B; ++b)
+        if (lens[b] < 0 || lens[b] > T) return fail("lens[%d] = %d outside [0, %d]", b, lens[b], T);
+    if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int H = hidden;
+    const size_t M = (size_t)B * T;
+    DevBuf xgc, bk;
+    SplitBuf os;
+    const int r = [&]() -> int {
+        std::vector<int> host(2 * (size_t)B);
+        memcpy(host.data(), lens, (size_t)B * sizeof(int));
+        std::vector<int> ord(B);
+        for (int b = 0; b < B; ++b) ord[b] = b;
+        std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return lens[a] > lens[b]; });
+        memcpy(host.data() + B, ord.data(), (size_t)B * sizeof(int));
+        S3B_OK(bk.ensure(host.size() * sizeof(int)));
+        CUDA_OK(cudaMemcpyAsync(bk.p, host.data(), host.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+        S3B_OK(xgc.ensure(M * 3 * H * 4));
+        CUDA_OK(cudaMemcpyAsync(xgc.p, xg, M * 3 * H * 4, cudaMemcpyDeviceToDevice, st));
+        CUDA_OK(launch_gru_fold_bias(xgc.as<float>(), bhh, M, st));
+        GruParams g;
+        g.xg = xgc.as<float>(), g.whh = whh, g.bhn = bhh + 2 * H, g.res = residual;
+        g.len = bk.as<int>(), g.order = bk.as<int>() + B, g.B = B, g.T = T;
+        g.out = out;
+        g.op = no_planes();
+        if (out_fmt >= 0) {
+            S3B_OK(os.ensure(M * H));
+            g.op = os.planes(out_fmt);
+        }
+        CUDA_OK(launch_gru(g, st));
+        if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(g.op, M * H, planes_out, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+        return 0;
+    }();
+    xgc.release(), bk.release(), os.release();
     return r;
 }
 

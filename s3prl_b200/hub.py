@@ -127,6 +127,34 @@ for _suffix in ("local", "url", "custom"):
     ENTRIES[f"decoar2_{_suffix}"] = _make_decoar2_file_entry(_suffix)
 
 
+def _make_apc_entry(name: str, vq: bool, needs_ckpt: bool) -> Callable:
+    """APC / VQ-APC (apc/hubconf.py, vq_apc/hubconf.py): the fabricated checkpoint without ``ckpt``, else the local
+    ``{"config", "model"}`` file; a URL is refused (remote checkpoints cannot be reached offline)."""
+
+    def entry(ckpt=None, *args, **kwargs):
+        from .upstream.apc import ApcExpert
+
+        if needs_ckpt:
+            assert isinstance(ckpt, str), "a checkpoint path is required"
+        if isinstance(ckpt, str) and ckpt.startswith("http"):
+            raise ValueError(f"{name}: remote checkpoints are not reachable here; download {ckpt} and pass the file")
+        kwargs.pop("refresh", None)
+        kwargs.pop("model_config", None)
+        return ApcExpert(ckpt=ckpt, name=name, vq=vq, **kwargs)
+
+    entry.__name__ = name
+    return entry
+
+
+for _name in ("apc", "apc_360hr", "apc_960hr"):
+    ENTRIES[_name] = _make_apc_entry(_name, False, False)
+for _name in ("vq_apc", "vq_apc_360hr", "vq_apc_960hr"):
+    ENTRIES[_name] = _make_apc_entry(_name, True, False)
+ENTRIES["apc_local"] = _make_apc_entry("apc_local", False, True)
+ENTRIES["apc_url"] = _make_apc_entry("apc_url", False, True)
+ENTRIES["vq_apc_url"] = _make_apc_entry("vq_apc_url", True, True)
+
+
 def options() -> List[str]:
     """Names of the available entries (cf. s3prl.hub.options, s3prl/hub.py:40-54)."""
     return sorted(ENTRIES)

@@ -23,6 +23,7 @@ EXPORTED_SYMBOLS = [
     "s3b_model_set_tensor",
     "s3b_model_finalize",
     "s3b_model_destroy",
+    "s3b_apc_model_create",
     "s3b_num_frames",
     "s3b_valid_frames",
     "s3b_num_outputs",
@@ -40,6 +41,7 @@ EXPORTED_SYMBOLS = [
     "s3b_peer_destroy",
     "s3b_profile_enable",
     "s3b_profile_read",
+    "s3b_profile_read_ex",
     "s3b_launch_count",
     "s3b_weighted_sum",
     "s3b_weighted_sum_backward",
@@ -57,6 +59,9 @@ EXPORTED_SYMBOLS = [
     "s3b_frontend_f32",
     "s3b_conformer_conv_f32",
     "s3b_decoar2_features_f32",
+    "s3b_apc_features_f32",
+    "s3b_gru_f32",
+    "s3b_gru_max_active_clusters",
     "s3b_layernorm_rope_f32",
     "s3b_fbank",
     "s3b_fbank_ex",
@@ -98,6 +103,22 @@ class S3BConfig(C.Structure):
         ("frontend", C.c_int32),
         ("reserved", C.c_int32 * 2),
     ]
+
+
+class S3BApcConfig(C.Structure):
+    """Mirror of ``struct s3b_apc_config``."""
+
+    _fields_ = [
+        ("struct_size", C.c_int32),
+        ("num_layers", C.c_int32),
+        ("hidden", C.c_int32),
+        ("residual", C.c_int32),
+        ("reserved", C.c_int32 * 4),
+    ]
+
+    def __init__(self, **kw):
+        super().__init__(**kw)
+        self.struct_size = C.sizeof(S3BApcConfig)
 
 
 class S3BForwardOpts(C.Structure):
@@ -204,6 +225,7 @@ def load() -> C.CDLL:
     lib.s3b_device_count.restype = C.c_int
     lib.s3b_model_create.argtypes = [C.POINTER(S3BConfig), C.POINTER(vp)]
     lib.s3b_model_set_tensor.argtypes = [vp, C.c_char_p, vp, C.POINTER(i64), i32]
+    lib.s3b_apc_model_create.argtypes = [C.POINTER(S3BApcConfig), C.POINTER(vp)]
     lib.s3b_model_finalize.argtypes = [vp]
     lib.s3b_model_destroy.argtypes = [vp]
     lib.s3b_model_destroy.restype = None
@@ -229,6 +251,7 @@ def load() -> C.CDLL:
     lib.s3b_peer_destroy.restype = None
     lib.s3b_profile_enable.argtypes = [vp, i32]
     lib.s3b_profile_read.argtypes = [vp, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(i64), i32]
+    lib.s3b_profile_read_ex.argtypes = [vp, i32, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(i64), i32]
     lib.s3b_launch_count.argtypes = [vp]
     lib.s3b_launch_count.restype = i64
     lib.s3b_weighted_sum.argtypes = [f32p, i32, i64, f32p, f32p, vp]
@@ -249,6 +272,9 @@ def load() -> C.CDLL:
                                      f32p, f32p, vp]
     lib.s3b_conformer_conv_f32.argtypes = [f32p, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, i32, f32p, vp]
     lib.s3b_decoar2_features_f32.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i32, f32p, vp]
+    lib.s3b_apc_features_f32.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i32, f32p, vp]
+    lib.s3b_gru_max_active_clusters.argtypes = [C.POINTER(i32)]
+    lib.s3b_gru_f32.argtypes = [f32p, f32p, f32p, f32p, C.POINTER(i32), i32, i32, i32, i32, f32p, f32p, vp]
     lib.s3b_layernorm_rope_f32.argtypes = [f32p, i64, i32, i32, f32p, f32p, C.POINTER(C.c_float), i32, f32p, f32p, vp]
     lib.s3b_fbank_num_frames.argtypes = [i64]
     lib.s3b_fbank_num_frames.restype = i64
