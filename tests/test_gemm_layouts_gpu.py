@@ -132,9 +132,11 @@ def _epilogue(pre, e, bias=None, gelu=False, res=None):
     return out, eo + 2.0**-24 * out.abs()
 
 
-def _check(what, out, ref1, b1, ref2, b2, gemm, scheme, frob=True):
+def _check(what, out, ref1, b1, ref2, b2, gemm, scheme, frob=True, apart_check=True):
     """out within b1 of ref1 and b2 of ref2 everywhere; the GEMM's bounds gemm = (e1, e2) apart by the factor the
-    module docstring states (median); 1e-4 relative Frobenius vs ref1 where the operands are N(0, 1)-scaled (frob)."""
+    module docstring states (median), unless the caller checks the property that factor stands for itself
+    (apart_check=False: tests/test_port_shapes_gpu.py at K >= 5120); 1e-4 relative Frobenius vs ref1 where the
+    operands are N(0, 1)-scaled (frob)."""
     assert torch.isfinite(out).all(), what
     o = out.double()
     r1 = ((o - ref1).abs() / b1).max().item()
@@ -144,7 +146,8 @@ def _check(what, out, ref1, b1, ref2, b2, gemm, scheme, frob=True):
     print(f"{what}: measured/bound fp64 {r1:.3f}, emulated {r2:.3f} (bounds {apart:.0f}x apart); rel {rel:.2e}")
     assert r1 < 1.0, (what, "fp64", r1)
     assert r2 < 1.0, (what, "emulated", r2)
-    assert apart >= (50.0 if scheme == 1 else 4.0), (what, apart)
+    if apart_check:
+        assert apart >= (50.0 if scheme == 1 else 4.0), (what, apart)
     if frob:
         assert rel < 1e-4, (what, rel)
 
