@@ -182,7 +182,8 @@ int s3b_profile_read_ex(s3b_model* m, int32_t num_categories, double* ms, double
 int64_t s3b_launch_count(const s3b_model* m);
 
 /* Featurizer (s3prl/upstream/interfaces.py:217-248) --------------------------------------------------
- * out[i] = sum_l w[l] * hs[l][i], hs = [num][n_per_layer] fp32 device, w = device (already softmaxed). */
+ * out[i] = sum_l w[l] * hs[l][i], hs = [num][n_per_layer] fp32 device, w = device (already softmaxed).
+ * num in [1, 64]; n_per_layer a non-negative multiple of 4; hs, out and grad_out 16-byte aligned. */
 int s3b_weighted_sum(const float* hs, int32_t num, int64_t n_per_layer, const float* w, float* out, void* stream);
 /* grad_w[l] = sum_i hs[l][i] * grad_out[i] */
 int s3b_weighted_sum_backward(const float* hs, int32_t num, int64_t n_per_layer, const float* grad_out,
@@ -191,10 +192,11 @@ int s3b_weighted_sum_backward(const float* hs, int32_t num, int64_t n_per_layer,
 /* Fused Featurizer + all-gather over NVLink peer memory (multi-GPU step ---------------------------
  * One process per GPU on one NVSwitch node. Every rank creates an exchange object (the library cudaMalloc's
  * [slots][world][block_elems] floats + flags and exports them as a 64-byte CUDA IPC handle), the host side exchanges
- * the handles (torch.distributed.all_gather in s3prl_b200/parallel.py) and calls s3b_peer_connect with all of them.
+ * the handles (torch.distributed.all_gather_object in s3prl_b200/parallel.py) and calls s3b_peer_connect with all of them.
  *  s3b_peer_push(step): ONE kernel computes sum_l w[l] * hs[l][i] over this rank's block (hs layers layer_stride
  *    elements apart) and stores it into slot step % slots of EVERY rank's buffer at this rank's position, then
- *    releases a per-(slot, rank) flag = step + 1 at system scope.
+ *    releases a per-(slot, rank) flag = step + 1 at system scope. num in [1, 64], layer_stride a multiple of 4 and
+ *    >= block_elems, hs 16-byte aligned. Steps count from 0 and stay below 2^32 - 1: the flags are uint32 step + 1.
  *  s3b_peer_wait(step): stream-ordered wait until every rank's flag of that slot has reached step + 1: the local
  *    gathered buffer s3b_peer_slot(step) = [world][block_elems] is then complete.
  * Contract: a slot is rewritten `slots` steps later; the host protocol (parallel.FeatureGatherer) waits for step s-1

@@ -2329,15 +2329,35 @@ extern "C" int64_t s3b_launch_count(const s3b_model* m) { return m ? m->launches
 // ------------------------------------------------------------------------------------------------
 // Featurizer
 // ------------------------------------------------------------------------------------------------
+// The weighted-sum kernels keep the layer weights in a 64-entry shared table and move hs / out / grad_out as float4.
+// Checked before any CUDA call, so a bad argument is refused with its name even on a host without a device.
+static int check_layers(int32_t num) {
+    if (num < 1 || num > 64) return fail("num = %d: the weighted sum takes 1..64 layers", num);
+    return 0;
+}
+static int check_float4(const void* ptr, const char* name) {
+    if (reinterpret_cast<uintptr_t>(ptr) & 15) return fail("%s = %p is not 16-byte aligned (read as float4)", name, ptr);
+    return 0;
+}
+static int check_ws_args(const float* hs, int32_t num, int64_t n_per_layer, const float* other, const char* other_name) {
+    S3B_OK(check_layers(num));
+    if (n_per_layer < 0 || (n_per_layer & 3) != 0)
+        return fail("n_per_layer = %lld must be a non-negative multiple of 4", (long long)n_per_layer);
+    S3B_OK(check_float4(hs, "hs"));
+    return check_float4(other, other_name);
+}
+
 extern "C" int s3b_weighted_sum(const float* hs, int32_t num, int64_t n_per_layer, const float* w, float* out,
                                 void* stream) {
     if (!hs || !w || !out) return fail("null argument");
+    S3B_OK(check_ws_args(hs, num, n_per_layer, out, "out"));
     CUDA_OK(launch_weighted_sum(hs, num, (size_t)n_per_layer, w, out, (cudaStream_t)stream));
     return 0;
 }
 extern "C" int s3b_weighted_sum_backward(const float* hs, int32_t num, int64_t n_per_layer, const float* grad_out,
                                          float* grad_w, void* stream) {
     if (!hs || !grad_out || !grad_w) return fail("null argument");
+    S3B_OK(check_ws_args(hs, num, n_per_layer, grad_out, "grad_out"));
     CUDA_OK(launch_weighted_sum_bwd(hs, num, (size_t)n_per_layer, grad_out, grad_w, (cudaStream_t)stream));
     return 0;
 }
@@ -2412,6 +2432,11 @@ extern "C" int s3b_peer_push(s3b_peer* p, const float* hs, int32_t num, int64_t 
                              uint32_t step, void* stream) {
     if (!p || !hs || !w) return fail("null argument");
     if (!p->connected && p->world > 1) return fail("s3b_peer_connect has not been called");
+    S3B_OK(check_layers(num));
+    if (layer_stride < p->block || (layer_stride & 3) != 0)
+        return fail("layer_stride = %lld must be a multiple of 4 and >= block_elems = %lld", (long long)layer_stride,
+                    (long long)p->block);
+    S3B_OK(check_float4(hs, "hs"));
     const int slot = (int)(step % p->slots);
     float* dst[16];
     uint32_t* flag[16];

@@ -287,7 +287,7 @@ __global__ void __launch_bounds__(256) weighted_sum_kernel(const float4* __restr
                                                            const float* __restrict__ w_dev,
                                                            float4* __restrict__ out) {
     __shared__ float lw[kMaxLayers];
-    if (threadIdx.x < NL) lw[threadIdx.x] = w_dev[threadIdx.x];
+    if ((int)threadIdx.x < NL) lw[threadIdx.x] = w_dev[threadIdx.x];
     __syncthreads();
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);

@@ -32,7 +32,7 @@ struct PushParams {
 __global__ void __launch_bounds__(256) weighted_sum_push_kernel(const __grid_constant__ PushParams p) {
     __shared__ float lw[kMaxLayersP];
     __shared__ bool is_last;
-    if (threadIdx.x < p.NL) lw[threadIdx.x] = p.w[threadIdx.x];
+    if ((int)threadIdx.x < p.NL) lw[threadIdx.x] = p.w[threadIdx.x];
     __syncthreads();
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n4; i += (size_t)gridDim.x * blockDim.x) {
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);

@@ -91,29 +91,24 @@ class FeatureGatherer:
                 block *= x
             handle = C.c_void_p()
             mine = (C.c_ubyte * 64)()
-            ok = 1
+            ok = True
             with torch.cuda.device(device):
                 if lib.s3b_peer_create(self.rank, self.world, block, slots, C.byref(handle), mine) != 0:
-                    ok, self._why = 0, lib.s3b_last_error().decode()
-            # exchange the 64-byte IPC handles (and whether everybody got this far)
-            t = torch.zeros(65, dtype=torch.uint8, device=device)
-            if ok:
-                t[:64] = torch.tensor(list(bytes(mine)), dtype=torch.uint8, device=device)
-                t[64] = 1
-            allh = torch.empty(self.world * 65, dtype=torch.uint8, device=device)
-            dist.all_gather_into_tensor(allh, t)
-            allh = allh.view(self.world, 65).cpu()
-            if bool((allh[:, 64] == 1).all()):
-                blob = bytes(allh[:, :64].contiguous().view(-1).tolist())
-                buf = (C.c_ubyte * len(blob)).from_buffer_copy(blob)
-                with torch.cuda.device(device):
+                    ok, self._why = False, lib.s3b_last_error().decode()
+                # exchange the 64-byte IPC handles (and whether everybody got this far) as host objects, which NCCL and
+                # gloo both gather (gloo also where several ranks share one device)
+                allh = [None] * self.world
+                dist.all_gather_object(allh, (ok, bytes(mine) if ok else b""))
+                if all(o for o, _ in allh):
+                    blob = b"".join(h for _, h in allh)
+                    buf = (C.c_ubyte * len(blob)).from_buffer_copy(blob)
                     if lib.s3b_peer_connect(handle, buf) != 0:
-                        ok, self._why = 0, lib.s3b_last_error().decode()
-            else:
-                ok = 0
-            flag = torch.tensor([ok], dtype=torch.int32, device=device)
-            dist.all_reduce(flag, op=dist.ReduceOp.MIN)
-            if int(flag.item()) == 1:
+                        ok, self._why = False, lib.s3b_last_error().decode()
+                else:
+                    ok = False
+                status = [None] * self.world
+                dist.all_gather_object(status, ok)
+            if all(status):
                 self.handle, self.lib, self.slots, self.block, self.mode = handle, lib, slots, block, "push"
             else:
                 if handle:

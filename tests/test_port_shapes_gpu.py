@@ -325,7 +325,11 @@ def test_weighted_sum(s3b_lib, NL, B, T, D):
 
 
 def test_weighted_sum_refusals(s3b_lib):
-    """More layers than the kernel's shared table (65 > kMaxLayers), and a layer size that is not whole float4."""
+    """More layers than the kernel's shared table (65 > kMaxLayers), and a layer size that is not whole float4. Then,
+    forward and backward alike, with the argument named in the message: num < 1 (a negative num passed the old
+    `NL > 64` check and let all 256 threads index the 64-entry table), negative layer sizes (a negative multiple of 4
+    passed as a huge size_t), and hs / out / grad_out off the 16-byte alignment of their float4 accesses. Nothing is
+    written by a refused call."""
     L = _lib().load()
     hs = torch.zeros(65 * 8, device="cuda")
     w = torch.zeros(65, device="cuda")
@@ -336,6 +340,34 @@ def test_weighted_sum_refusals(s3b_lib):
     assert L.s3b_weighted_sum(_ptr(hs), 3, 6, _ptr(w), _ptr(out), _stream()) != 0
     assert L.s3b_weighted_sum_backward(_ptr(hs), 3, 6, _ptr(out), _ptr(grad), _stream()) != 0
     torch.cuda.synchronize()
+
+    def refused(fn, args, what):
+        rc = fn(*args, _stream())
+        msg = L.s3b_last_error().decode()
+        assert rc != 0 and msg.startswith(what + " = "), (fn, what, msg)
+
+    hs.fill_(float("nan"))
+    out_nan = torch.full((12,), float("nan"), device="cuda")
+    grad.fill_(float("nan"))
+    fwd, bwd = L.s3b_weighted_sum, L.s3b_weighted_sum_backward
+    # first the cases a library without these checks would still run harmlessly (empty layers launch nothing), so that
+    # such a library fails here before any of the out-of-bounds launches below
+    refused(fwd, (_ptr(hs), 0, 0, _ptr(w), _ptr(out_nan)), "num")
+    refused(bwd, (_ptr(hs), 0, 0, _ptr(out_nan), _ptr(grad)), "num")
+    for num in (-1, -(2**31), 65):
+        refused(fwd, (_ptr(hs), num, 8, _ptr(w), _ptr(out_nan)), "num")
+        refused(bwd, (_ptr(hs), num, 8, _ptr(out_nan), _ptr(grad)), "num")
+    for n in (-4, -(2**62), 6):
+        refused(fwd, (_ptr(hs), 3, n, _ptr(w), _ptr(out_nan)), "n_per_layer")
+        refused(bwd, (_ptr(hs), 3, n, _ptr(out_nan), _ptr(grad)), "n_per_layer")
+    for off in (1, 2, 3):
+        hs_off, out_off = C.c_void_p(hs.data_ptr() + 4 * off), C.c_void_p(out_nan.data_ptr() + 4 * off)
+        refused(fwd, (hs_off, 3, 8, _ptr(w), _ptr(out_nan)), "hs")
+        refused(bwd, (hs_off, 3, 8, _ptr(out_nan), _ptr(grad)), "hs")
+        refused(fwd, (_ptr(hs), 3, 8, _ptr(w), out_off), "out")
+        refused(bwd, (_ptr(hs), 3, 8, out_off, _ptr(grad)), "grad_out")
+    torch.cuda.synchronize()
+    assert torch.isnan(out_nan).all() and torch.isnan(grad).all()
 
 
 @pytest.mark.parametrize("NL,D", [(13, 768), (49, 1280)])
