@@ -315,8 +315,8 @@ int s3b_posconv_f32(const float* x, const float* w, const float* bias, int32_t b
                     const float* beta, int32_t out_fmt, float* out, void* stream);
 /* micro-benchmark of the production GEMM kernel: `iters` back-to-back launches of [M][K] x [N][K]^T with the fc1-style
  * epilogue (gelu != 0: bias + GELU + bf16 hi/lo output) or the out_proj-style one (bias + residual + fp32 output).
- * force_un in {0 = the library's choice, 128, 256} forces the CTA-pair tile width. out[0] = ms per launch,
- * out[1] = tile width used. (tools/gemm_tile_sweep.py) */
+ * force_un in {0 = the library's choice, 128, 256} forces the tile width (columns per output tile) wherever it divides
+ * n. out[0] = ms per launch, out[1] = tile width used. (tools/gemm_shapes.py) */
 int s3b_gemm_bench(int64_t m, int32_t n, int32_t k, int32_t gelu, int32_t force_un, int32_t iters, float* out);
 /* y = LayerNorm_D(x) (eps 1e-5), optional GELU; D in {512,768,1024,1280,1920} */
 int s3b_layernorm_f32(const float* x, int64_t m, int32_t d, const float* gamma, const float* beta, int32_t gelu,

@@ -13,29 +13,26 @@ namespace s3b {
 struct GemmParams {
     // A operand (activations): bf16 hi / lo, 3-D tensor maps (k, row, batch), box {64, 128, 1}, SWIZZLE_128B
     CUtensorMap a_hi, a_lo;
-    // B operand (weights, [N][K] K-major): bf16 hi / lo, 3-D tensor maps (k, n, z), box {64, umma_n, 1}
+    // B operand (weights, [N][K] K-major): bf16 hi / lo, 3-D tensor maps (k, n, z), box {64, bn, 1}
     CUtensorMap b_hi, b_lo;
 
-    // scheme 1 ("f16q8", CTA-pair kernel only): fp16 main product + two e4m3 correction products.
+    // scheme 1 ("f16q8", bn 128 or 256 only): fp16 main product + two e4m3 correction products.
     //   a_hi / b_hi are the fp16 planes (box {64, rows}, SWIZZLE_128B), a_h8 / a_l8 / b_h8 / b_l8 the e4m3 planes
-    //   (box {64, rows}, SWIZZLE_64B); a_lo / b_lo are unused. k-blocks are 64 elements wide (block_k == 64, K % 128 == 0)
-    //   and the kernel walks them twice: num_k_blocks stages of e4m3 corrections, then num_k_blocks of fp16 products.
-    //   num_k_blocks and kb_per_row therefore count 64-element blocks, as in the bf16x3 CTA-pair layout.
+    //   (box {64, rows}, SWIZZLE_64B); a_lo / b_lo are unused. K % 128 == 0, and the kernel walks the 64-wide
+    //   k-blocks twice: num_k_blocks stages of e4m3 corrections, then num_k_blocks of fp16 products.
     int scheme;
     CUtensorMap a_h8, a_l8, b_h8, b_l8;
 
-    // ---- tiling -------------------------------------------------------------------------------
+    // ---- tiling: every k-block is 64 elements of K wide --------------------------------------------------------
     int batches;            // extent of A's 3rd dim that is tiled over
     int rows_per_batch;     // valid output rows per batch
     int tiles_m_per_batch;  // ceil(rows_per_batch / 128)
     int n_tiles;            // output column tiles
-    int umma_n;             // columns per tile (multiple of 16, <= 256; 80 or 120 for the pos_conv's wide groups)
-    int two_cta;            // 1: CTA-pair kernel (umma_n == 256, block_k == 64, B boxes hold umma_n/2 rows)
-    int block_k;            // K elements per k-block: gemm_block_k(umma_n) (32 for 128x256 tiles, else 64); f16q8: 64
+    int bn;                 // columns per tile, the kernel's BN (multiple of 16 <= 256, or 80 / 120: pos_conv groups)
     int num_k_blocks;       // k-blocks per output tile
-    // k-block kb reads   A box at (a_k_per_ntile*n_tile + (kb % kb_per_row)*block_k,
+    // k-block kb reads   A box at (a_k_per_ntile*n_tile + (kb % kb_per_row)*64,
     //                              row0 + (kb / kb_per_row)*a_row_step + a_row_off, batch)
-    //                    B box at (b_k_linear ? kb*block_k : (kb % kb_per_row)*block_k, b_n_tiled ? n_tile*umma_n : 0,
+    //                    B box at (b_k_linear ? kb*64 : (kb % kb_per_row)*64, b_n_tiled ? n_tile*bn : 0,
     //                              b_k_linear ? 0 : kb / kb_per_row + n_tile*b_z_per_ntile)
     int kb_per_row;
     int a_row_step;
@@ -58,8 +55,8 @@ struct GemmParams {
     float* out_f32;
     __nv_bfloat16* out_hi;
     __nv_bfloat16* out_lo;
-    // out_fmt 1: out_hi is an fp16 plane and out_h8 / out_l8 the two e4m3 planes of the f16q8 operand format (same for
-    // the fused LayerNorm outputs); out_fmt 0: out_hi / out_lo are the bf16 hi / lo planes.
+    // out_fmt 1: out_hi is an fp16 plane and out_h8 / out_l8 the two e4m3 planes of the f16q8 operand format;
+    // out_fmt 0: out_hi / out_lo are the bf16 hi / lo planes.
     int out_fmt;
     uint8_t* out_h8;
     uint8_t* out_l8;
@@ -76,25 +73,9 @@ struct GemmParams {
     int qkv_col0;
     __nv_bfloat16 *q_hi, *q_lo, *k_hi, *k_lo, *vt_hi, *vt_lo;
 
-    // ---- optional fused LayerNorm over the whole output row (CTA-pair kernel, N == ldo == 128 * ln_v4) ------------
-    // The n-tiles of a 128-row block are finished by different CTAs; each counts itself in on ln_counter[row block]
-    // after its stores, and the LAST one to arrive normalises the 128 complete rows of out_f32 (re-read from L2):
-    //   y = LayerNorm(out_f32 row) * ln_gamma + ln_beta (eps 1e-5), optional GELU -> ln_out_f32 / ln_out_hi,lo
-    // The values are the ones the separate layernorm_kernel would produce, bit for bit (same per-row arithmetic), and
-    // the LayerNorm traffic overlaps the MMAs of the CTA's next tile instead of running as its own HBM-bound kernel.
-    const float* ln_gamma;  // null = no fused LayerNorm
-    const float* ln_beta;
-    int ln_gelu;
-    float* ln_out_f32;
-    __nv_bfloat16* ln_out_hi;
-    __nv_bfloat16* ln_out_lo;
-    uint8_t* ln_out_h8;
-    uint8_t* ln_out_l8;
-    unsigned int* ln_counter;  // [batches * tiles_m_per_batch], zero on entry, left zero
-
     double alg_flops;  // host-side accounting only: 2*M*N*K with the un-padded K
 
-    // CTA-pair kernel: 16-wide MMA k-steps issued per 64-wide k-block (0 = all 4). pos_conv with 48 channels per group
+    // bf16x3: 16-wide MMA k-steps issued per 64-wide k-block (0 = all 4). pos_conv with 48 channels per group
     // loads 64-wide boxes but only the first 3 k-steps carry non-zero weights.
     int k_steps;
 
@@ -103,13 +84,10 @@ struct GemmParams {
     int qk_head_step;       // (T - 1) * hd
 };
 
-// k-block width the kernel instantiation for this tile width uses (tensor-map boxes must match)
-inline int gemm_block_k(int umma_n) { return umma_n > 128 ? 32 : 64; }
-
 // Launch on `stream`. Returns cudaGetLastError() of the launch.
-cudaError_t launch_gemm_bf16x3(const GemmParams& p, int sm_count, cudaStream_t stream);
+cudaError_t launch_gemm(const GemmParams& p, int sm_count, cudaStream_t stream);
 
-// Encode a 3-D bf16 tensor map with the 128B swizzle. strides in ELEMENTS for dims 1 and 2.
+// Encode a 3-D bf16 tensor map with the 128B swizzle (box0 = 64 elements). strides in ELEMENTS for dims 1 and 2.
 // Returns 0 on success, else a CUresult / -1 (driver entry point missing).
 int encode_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1,
                         uint64_t stride2, uint32_t box0, uint32_t box1);

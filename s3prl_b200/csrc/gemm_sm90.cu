@@ -27,16 +27,18 @@
 namespace s3b {
 
 static constexpr int kBlockM = 128;
+static constexpr int kBlockK = 64;  // K elements per k-block, every scheme and width
 static constexpr int kThreads = 288;
 static constexpr int kPingPongThreads = 384;
 static constexpr int kSmemBudget = 220 * 1024;
 
-// RB: bytes of one K row of a stage plane = the swizzle span (128: 64 bf16 elements, 64: 32 bf16 / 64 e4m3 elements).
-// f16q8 uses RB = 64 with 64 elements of K per stage: pass 0 fills the four planes with 64-byte e4m3 rows
-// [A_l8 A_h8 W_h8 W_l8], pass 1 fills [A16 | W16] with 128-byte fp16 rows (each spanning two planes). Both are
-// 48 KB at BN = 256, which makes the ring four deep there (six at BN = 128).
-template <int BN, int RB>
+// RB: bytes of one K row of a stage plane = the swizzle span. bf16x3: 128 (64 bf16 elements). f16q8: 64, with 64
+// elements of K per stage: pass 0 fills the four planes with 64-byte e4m3 rows [A_l8 A_h8 W_h8 W_l8], pass 1 fills
+// [A16 | W16] with 128-byte fp16 rows (each spanning two planes). Both are 48 KB at BN = 256, which makes the ring
+// four deep there (six at BN = 128).
+template <int BN, int kScheme>
 struct GemmCfg {
+    static constexpr int RB = kScheme == 0 ? 128 : 64;
     static constexpr int kAPlane = kBlockM * RB;
     static constexpr int kBPlane = BN * RB;
     static constexpr int kStageBytes = 2 * kAPlane + 2 * kBPlane;
@@ -45,7 +47,7 @@ struct GemmCfg {
     static_assert(kStages >= 2, "tile too large for the shared-memory ring");
 };
 
-// Epilogue kinds, one kernel instantiation each (chosen per launch in launch_gemm_bf16x3). Every non-QKV kind computes
+// Epilogue kinds, one kernel instantiation each (chosen per launch in launch_gemm). Every non-QKV kind computes
 //   v = acc (+bias) ; GELU or SiLU? ; out_pre = v? ; (+residual) ; row_mask ? 0
 // and stores v as fp32, as operand planes, or both.
 enum EpiKind { kEpiF32 = 1, kEpiPlanes = 2, kEpiBoth = 3, kEpiQkv = 4 };
@@ -54,14 +56,11 @@ __device__ __forceinline__ void setmaxnreg_dec40() { asm volatile("setmaxnreg.de
 __device__ __forceinline__ void setmaxnreg_inc232() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
 
 // ===================== TMA producer: every tile of this CTA, kPasses * num_k_blocks stages each, in tile order ====
-template <int BN, int RB, int kScheme>
+template <int BN, int kScheme>
 __device__ __forceinline__ void produce(const GemmParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar) {
-    using Cfg = GemmCfg<BN, RB>;
+    using Cfg = GemmCfg<BN, kScheme>;
     constexpr int kPasses = kScheme == 0 ? 1 : 2;
     const int num_tiles = p.batches * p.tiles_m_per_batch * p.n_tiles;
-    // two_cta layout: the W boxes hold BN/2 rows and a stage takes two of them (gemm.cuh)
-    const int b_boxes = p.two_cta ? 2 : 1;
-    const int b_box_rows = BN / b_boxes;
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -81,14 +80,13 @@ __device__ __forceinline__ void produce(const GemmParams& p, uint8_t* smem, uint
                 uint8_t* sb = st + 2 * Cfg::kAPlane;
                 mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)Cfg::kStageBytes);
                 const int a_row = row0 + kq * p.a_row_step + p.a_row_off;
-                const int a_k = a_k0 + kr * p.block_k;
-                const int b_k = (p.b_k_linear ? kb : kr) * p.block_k;
+                const int a_k = a_k0 + kr * kBlockK;
+                const int b_k = (p.b_k_linear ? kb : kr) * kBlockK;
                 const int b_z = p.b_k_linear ? 0 : b_z0 + kq;
                 if (kScheme == 1 && pass == 1) {
                     // [A16 | W16]: one fp16 box of 128-byte rows each, spanning both planes of the stage
                     tma_load_3d(st, &p.a_hi, &full_bar[stage], a_k, a_row, batch);
-                    for (int h = 0; h < b_boxes; ++h)
-                        tma_load_3d(sb + h * b_box_rows * 128, &p.b_hi, &full_bar[stage], b_k, b_n0 + h * b_box_rows, b_z);
+                    tma_load_3d(sb, &p.b_hi, &full_bar[stage], b_k, b_n0, b_z);
                 } else {
                     // planes: scheme 0 [A_hi A_lo W_hi W_lo]; scheme 1 pass 0 [A_l8 A_h8 W_h8 W_l8] (64-byte rows)
                     const CUtensorMap* ma0 = kScheme == 0 ? &p.a_hi : &p.a_l8;
@@ -97,11 +95,8 @@ __device__ __forceinline__ void produce(const GemmParams& p, uint8_t* smem, uint
                     const CUtensorMap* mb1 = kScheme == 0 ? &p.b_lo : &p.b_l8;
                     tma_load_3d(st, ma0, &full_bar[stage], a_k, a_row, batch);
                     tma_load_3d(st + Cfg::kAPlane, ma1, &full_bar[stage], a_k, a_row, batch);
-                    for (int h = 0; h < b_boxes; ++h) {
-                        const int rows = b_n0 + h * b_box_rows;
-                        tma_load_3d(sb + h * b_box_rows * RB, mb0, &full_bar[stage], b_k, rows, b_z);
-                        tma_load_3d(sb + Cfg::kBPlane + h * b_box_rows * RB, mb1, &full_bar[stage], b_k, rows, b_z);
-                    }
+                    tma_load_3d(sb, mb0, &full_bar[stage], b_k, b_n0, b_z);
+                    tma_load_3d(sb + Cfg::kBPlane, mb1, &full_bar[stage], b_k, b_n0, b_z);
                 }
                 if (++stage == Cfg::kStages) stage = 0, phase ^= 1u;
             }
@@ -113,11 +108,12 @@ __device__ __forceinline__ void produce(const GemmParams& p, uint8_t* smem, uint
 // Stage s is released (one arrive per warp of the warpgroup) once the wgmma group reading it has retired; one group
 // stays in flight so that the tensor pipe is fed while this warpgroup waits for the next stage. Every output element
 // sees the same wgmma sequence whichever kernel, warpgroup or half runs it.
-template <int BN, int RB, int kScheme, int kHalves>
+template <int BN, int kScheme, int kHalves>
 __device__ __forceinline__ void mma_tile(const GemmParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
                                          int half0, int lane, int& stage, uint32_t& phase,
                                          float (&acc)[kHalves][BN / 2]) {
-    using Cfg = GemmCfg<BN, RB>;
+    using Cfg = GemmCfg<BN, kScheme>;
+    constexpr int RB = Cfg::RB;
     constexpr int kStages = Cfg::kStages;
     constexpr int kNR = BN / 2;
     constexpr int kPasses = kScheme == 0 ? 1 : 2;
@@ -401,9 +397,9 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float (&acc)[
     }
 }
 
-template <int BN, int RB, int kScheme, int kEpi>
+template <int BN, int kScheme, int kEpi>
 __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_constant__ GemmParams p) {
-    using Cfg = GemmCfg<BN, RB>;
+    using Cfg = GemmCfg<BN, kScheme>;
     constexpr int kStages = Cfg::kStages;
     extern __shared__ uint8_t smem_raw[];
     // 1024-byte alignment is required by the 128B swizzle atoms (8 rows x 128 B)
@@ -432,7 +428,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
     pdl_launch_dependents();
 
     if (warp == 8) {
-        if (elect_one()) produce<BN, RB, kScheme>(p, smem, full_bar, empty_bar);
+        if (elect_one()) produce<BN, kScheme>(p, smem, full_bar, empty_bar);
         return;
     }
 
@@ -448,15 +444,15 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
         const int mt = tile / p.n_tiles;
         const int batch = mt / p.tiles_m_per_batch;
         const int row0 = (mt - batch * p.tiles_m_per_batch) * kBlockM;
-        mma_tile<BN, RB, kScheme, 1>(p, smem, full_bar, empty_bar, wg, lane, stage, phase, acc);
+        mma_tile<BN, kScheme, 1>(p, smem, full_bar, empty_bar, wg, lane, stage, phase, acc);
         epilogue_tile<BN, kEpi, 1>(p, acc, batch, row0 + wg * 64 + wq * 16 + (lane >> 2), n_tile * BN + 2 * (lane & 3));
     }
 }
 
-template <int RB, int kScheme, int kEpi>
+template <int kScheme, int kEpi>
 __global__ void __launch_bounds__(kPingPongThreads, 1) gemm_sm90_pingpong_kernel(const __grid_constant__ GemmParams p) {
     constexpr int BN = 128;
-    using Cfg = GemmCfg<BN, RB>;
+    using Cfg = GemmCfg<BN, kScheme>;
     constexpr int kStages = Cfg::kStages;
     constexpr int kPasses = kScheme == 0 ? 1 : 2;
     extern __shared__ uint8_t smem_raw[];
@@ -489,7 +485,7 @@ __global__ void __launch_bounds__(kPingPongThreads, 1) gemm_sm90_pingpong_kernel
 
     if (warp >= 8) {
         setmaxnreg_dec40();
-        if (warp == 8 && elect_one()) produce<BN, RB, kScheme>(p, smem, full_bar, empty_bar);
+        if (warp == 8 && elect_one()) produce<BN, kScheme>(p, smem, full_bar, empty_bar);
         return;
     }
     setmaxnreg_inc232();
@@ -515,7 +511,7 @@ __global__ void __launch_bounds__(kPingPongThreads, 1) gemm_sm90_pingpong_kernel
         const int batch = mt / p.tiles_m_per_batch;
         const int row0 = (mt - batch * p.tiles_m_per_batch) * kBlockM;
         if (ord > 0) mbar_wait(&order_bar[wg], (uint32_t)(j - (wg == 0 ? 1 : 0)) & 1u);
-        mma_tile<BN, RB, kScheme, 2>(p, smem, full_bar, empty_bar, 0, lane, stage, phase, acc);
+        mma_tile<BN, kScheme, 2>(p, smem, full_bar, empty_bar, 0, lane, stage, phase, acc);
         __syncwarp();
         if (lane == 0) mbar_arrive(&order_bar[wg ^ 1]);
         epilogue_tile<BN, kEpi, 2>(p, acc, batch, row0 + wq * 16 + (lane >> 2), n_tile * BN + 2 * (lane & 3));
@@ -537,60 +533,53 @@ static cudaError_t launch_persistent(Kernel kernel, PerDeviceOnce& attr_once, in
     return launch_pdl(kernel, dim3(grid), dim3(threads), smem_bytes, stream, p);
 }
 
-template <int BN, int RB, int kScheme, int kEpi>
+template <int BN, int kScheme, int kEpi>
 static cudaError_t launch_impl(const GemmParams& p, int sm_count, cudaStream_t stream) {
     static PerDeviceOnce attr_once;
     if constexpr (BN == 128)
-        return launch_persistent(gemm_sm90_pingpong_kernel<RB, kScheme, kEpi>, attr_once, kPingPongThreads,
-                                 GemmCfg<BN, RB>::kSmemBytes, p, sm_count, stream);
+        return launch_persistent(gemm_sm90_pingpong_kernel<kScheme, kEpi>, attr_once, kPingPongThreads,
+                                 GemmCfg<BN, kScheme>::kSmemBytes, p, sm_count, stream);
     else
-        return launch_persistent(gemm_sm90_kernel<BN, RB, kScheme, kEpi>, attr_once, kThreads,
-                                 GemmCfg<BN, RB>::kSmemBytes, p, sm_count, stream);
+        return launch_persistent(gemm_sm90_kernel<BN, kScheme, kEpi>, attr_once, kThreads,
+                                 GemmCfg<BN, kScheme>::kSmemBytes, p, sm_count, stream);
 }
 
 // QKV scatter and the fp32 + planes output run at the widths of the encoder's linears only (>= 128 columns)
-template <int BN, int RB, int kScheme>
+template <int BN, int kScheme>
 static cudaError_t launch_epi(const GemmParams& p, int sm_count, cudaStream_t stream) {
     const bool f32 = p.out_f32 != nullptr, planes = p.out_hi != nullptr;
     if constexpr (BN >= 128) {
-        if (p.qkv_mode) return launch_impl<BN, RB, kScheme, kEpiQkv>(p, sm_count, stream);
-        if (f32 && planes) return launch_impl<BN, RB, kScheme, kEpiBoth>(p, sm_count, stream);
+        if (p.qkv_mode) return launch_impl<BN, kScheme, kEpiQkv>(p, sm_count, stream);
+        if (f32 && planes) return launch_impl<BN, kScheme, kEpiBoth>(p, sm_count, stream);
     }
     if (p.qkv_mode || (f32 && planes)) return cudaErrorInvalidValue;
-    if (planes) return launch_impl<BN, RB, kScheme, kEpiPlanes>(p, sm_count, stream);
-    if (f32) return launch_impl<BN, RB, kScheme, kEpiF32>(p, sm_count, stream);
+    if (planes) return launch_impl<BN, kScheme, kEpiPlanes>(p, sm_count, stream);
+    if (f32) return launch_impl<BN, kScheme, kEpiF32>(p, sm_count, stream);
     return cudaErrorInvalidValue;  // no output
 }
 
+// f16q8 runs at the linears' and convs' widths only (128, 256)
 template <int BN>
 static cudaError_t launch_n(const GemmParams& p, int sm_count, cudaStream_t stream) {
-    if (p.scheme != 0) {
-        if constexpr (BN == 256 || BN == 192 || BN == 128) return launch_epi<BN, 64, 1>(p, sm_count, stream);
-        return cudaErrorInvalidValue;
-    }
-    if (p.block_k == 64) return launch_epi<BN, 128, 0>(p, sm_count, stream);
-    // 32-wide k-blocks: only the unpaired 192- and 256-column tiles use them (gemm_block_k)
-    if constexpr (BN > 128) return launch_epi<BN, 64, 0>(p, sm_count, stream);
+    if (p.scheme == 0) return launch_epi<BN, 0>(p, sm_count, stream);
+    if constexpr (BN == 256 || BN == 128) return launch_epi<BN, 1>(p, sm_count, stream);
     return cudaErrorInvalidValue;
 }
 
-cudaError_t launch_gemm_bf16x3(const GemmParams& p, int sm_count, cudaStream_t stream) {
-    if (p.ln_gamma != nullptr) return cudaErrorNotSupported;  // LayerNorm is a separate launch (norm.cu)
-    if (p.scheme != 0 ? (p.block_k != 64 || p.k_steps != 0) : (p.block_k != 64 && p.block_k != 32))
-        return cudaErrorInvalidValue;
-    if (p.scheme == 0 && p.block_k == 32 && (p.two_cta || p.k_steps != 0)) return cudaErrorInvalidValue;
+cudaError_t launch_gemm(const GemmParams& p, int sm_count, cudaStream_t stream) {
+    if (p.scheme != 0 && p.k_steps != 0) return cudaErrorInvalidValue;
     if (p.out_fmt != 0 && (p.qkv_mode || (p.out_hi != nullptr && (p.out_h8 == nullptr || p.out_l8 == nullptr))))
         return cudaErrorInvalidValue;
-    switch (p.umma_n) {
+    switch (p.bn) {
         case 256: return launch_n<256>(p, sm_count, stream);
         case 192: return launch_n<192>(p, sm_count, stream);
         case 128: return launch_n<128>(p, sm_count, stream);
-        case 120: return p.two_cta ? cudaErrorInvalidValue : launch_n<120>(p, sm_count, stream);
-        case 80: return p.two_cta ? cudaErrorInvalidValue : launch_n<80>(p, sm_count, stream);
-        case 64: return p.two_cta ? cudaErrorInvalidValue : launch_n<64>(p, sm_count, stream);
-        case 48: return p.two_cta ? cudaErrorInvalidValue : launch_n<48>(p, sm_count, stream);
-        case 32: return p.two_cta ? cudaErrorInvalidValue : launch_n<32>(p, sm_count, stream);
-        case 16: return p.two_cta ? cudaErrorInvalidValue : launch_n<16>(p, sm_count, stream);
+        case 120: return launch_n<120>(p, sm_count, stream);
+        case 80: return launch_n<80>(p, sm_count, stream);
+        case 64: return launch_n<64>(p, sm_count, stream);
+        case 48: return launch_n<48>(p, sm_count, stream);
+        case 32: return launch_n<32>(p, sm_count, stream);
+        case 16: return launch_n<16>(p, sm_count, stream);
         default: return cudaErrorInvalidValue;
     }
 }
@@ -625,11 +614,10 @@ int encode_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t d0, uint64_
     cuuint64_t strides[2] = {stride1 * 2, stride2 * 2};  // bytes
     cuuint32_t box[3] = {box0, box1, 1};
     cuuint32_t estr[3] = {1, 1, 1};
-    // the swizzle span equals the box row: 64 elements -> 128 B, 32 elements -> 64 B
-    if (box0 != 64 && box0 != 32) return -2;
-    const CUtensorMapSwizzle sw = box0 == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+    // the swizzle span equals the box row: 64 elements -> 128 B
+    if (box0 != 64) return -2;
     CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return (int)r;
 }

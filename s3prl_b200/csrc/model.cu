@@ -188,7 +188,7 @@ struct Workspace {
     size_t book_host_bytes = 0;
     size_t book_valid = 0;  // bytes of the mirror that hold the last call's block
     cudaEvent_t book_copied = nullptr;  // the previous call's H2D copy has been consumed: the mirror may be rewritten
-    DevBuf wav_stats, wav_pad, c0_part, c0_ss, conv_f32, tmp_f32, x_f32, x1_f32, gate, pos_z, ln_counters, hs0;
+    DevBuf wav_stats, wav_pad, c0_part, c0_ss, conv_f32, tmp_f32, x_f32, x1_f32, gate, pos_z, hs0;
     DevBuf glu_f32;  // Conformer: pointwise_conv1 output [M][2D]
     DevBuf fb_f32;   // DeCoAR 2.0 / APC: log-mel frames [B][m(Lmax)][80]
     DevBuf xg_f32;   // APC: the input GEMM's output [M][3H]
@@ -294,7 +294,7 @@ static int upload_vec(s3b_model* m, const std::string& k, int64_t n, DevBuf& dst
     return upload_f32(dst, t->data.data(), (size_t)n);
 }
 
-static int pairs_enabled();
+static bool posconv4_ok(const s3b_config& c);
 static int pos_taps(const s3b_config& c);
 static int pos_taps4(const s3b_config& c);
 
@@ -743,7 +743,6 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
     if (c.conformer) {
         // ConformerEncoder.extract_features never calls pos_conv (wav2vec2_model.py:3171-3211): its weights are unused
     } else if (c.pos_conv_depth > 1) {
-        if (!pairs_enabled()) return fail("pos_conv_depth > 1 runs on the CTA-pair GEMM only (S3B_GEMM_PAIR=0 is set)");
         const int G = c.pos_conv_groups, cpg = D / G, Kp = pos_taps(c);
         m->posd_w4.resize(c.pos_conv_depth);
         m->posd_b.resize(c.pos_conv_depth);
@@ -757,7 +756,7 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
         }
     } else {
     // ---- pos_conv: fold weight_norm(dim=2): W[o][c][k] = g[k] * v[o][c][k] / ||v[:,:,k]||  ---------------
-    //      (make_conv_pos, wav2vec2_model.py:2937-2953), then the one-tap and (Kp % 4 == 0) four-tap layouts
+    //      (make_conv_pos, wav2vec2_model.py:2937-2953), in the four-tap layout where posconv4_ok, else the one-tap one
         const int G = c.pos_conv_groups, cpg = D / G, Kp = c.pos_conv_kernel;
         const HostTensor *tg, *tv;
         S3B_OK(need(m, "encoder.pos_conv.0.weight_g", {1, 1, Kp}, &tg));
@@ -773,11 +772,12 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
         std::vector<float> wf((size_t)D * cpg * Kp);
         for (size_t oc = 0; oc < (size_t)D * cpg; ++oc)
             for (int k = 0; k < Kp; ++k) wf[oc * Kp + k] = tv->data[oc * Kp + k] * scale[k];  // fp32, like torch's _weight_norm
-        const std::vector<float> wb = posconv_weight_layout(wf.data(), D, G, Kp);
-        S3B_OK(upload_split(m->pos_w, wb.data(), wb.size()));
-        if (Kp % 4 == 0 && (4 * cpg == 192 || 4 * cpg == 256)) {  // the groups posconv4_ok can run four taps on
+        if (posconv4_ok(c)) {
             const std::vector<float> w4 = posconv4_weight_layout(wf.data(), D, G, Kp);
             S3B_OK(upload_split(m->pos_w4, w4.data(), w4.size()));
+        } else {
+            const std::vector<float> wb = posconv_weight_layout(wf.data(), D, G, Kp);
+            S3B_OK(upload_split(m->pos_w, wb.data(), wb.size()));
         }
         S3B_OK(upload_vec(m, "encoder.pos_conv.0.bias", D, m->pos_b));
     }
@@ -977,21 +977,6 @@ static void set_qkv_epi(GemmParams& p, const float* bias, int T, int H, int hd, 
     p.vt_hi = vt.h(), p.vt_lo = vt.l();
 }
 
-// The paired tile layout (gemm.cuh: two_cta) serves the 256- and 128-column tiles: 64-wide k-blocks (128-byte
-// swizzle rows, which the f16q8 scheme and the four-tap pos_conv need) and W boxes of half the tile height.
-// S3B_GEMM_PAIR=0 switches it off (32-wide k-blocks for 256-column tiles, bf16x3 only).
-static int pairs_enabled() {
-    static int enabled = -1;
-    if (enabled < 0) {
-        const char* e = getenv("S3B_GEMM_PAIR");
-        enabled = (e == nullptr || e[0] != '0') ? 1 : 0;
-    }
-    return enabled;
-}
-static int use_cta_pairs(int umma_n) { return ((umma_n == 256 || umma_n == 128) && pairs_enabled()) ? 1 : 0; }
-
-static int g_force_pair_un = 0;  // s3b_gemm_bench: force the tile width (tile-shape sweeps)
-
 // Tile width for a flat [M][N] linear layer. Both widths give bit-identical results; the rule comes from
 // tools/gemm_shapes.py on an H100 80GB HBM3 at 400 W, at the encoder shapes of hubert_base (K = 768, 3072) and
 // wav2vec2_large (K = 1024, 4096), M = 7984..15984, with the ping-pong kernel at 128 columns:
@@ -1001,26 +986,18 @@ static int g_force_pair_un = 0;  // s3b_gemm_bench: force the tile width (tile-s
 //  - f16q8 with K >= 3072 (fc2): 256 columns are 21-28% faster when their last round of tiles fills at least half of
 //    the SMs (or none is partial); otherwise that round runs half empty and 128 columns are 17% faster (hubert_base
 //    fc2 at M = 7984: 189 tiles of 256 on 132 SMs). The K >= 2048 cut lies between measured Ks (1024 and 3072).
-// The epilogue kind (epi_kind) does not enter the rule: at K <= 1024 the GELU (fc1) and fp32 epilogues ranked the two
-// widths the same way, but for the one shape above.
-static int pick_pair_umma_n(int64_t M, int N, int K, int epi_kind, int sm_count, int scheme = 0) {
-    (void)epi_kind;
-    if (g_force_pair_un != 0 && N % g_force_pair_un == 0) return g_force_pair_un;
-    if (N % 256 != 0) return (N % 128 == 0) ? 128 : 0;
-    if (scheme == 0 || K < 2048) return 128;
+// The epilogue kind does not enter the rule: at K <= 1024 the GELU (fc1) and fp32 epilogues ranked the two widths the
+// same way, but for the one shape above.
+// An N that is not a multiple of 128 takes the widest of 192, 64, 32 and 16 that divides it. forced != 0 (the tile
+// width s3b_linear_ex or s3b_gemm_bench asks for) is taken wherever it divides N.
+static int pick_bn(int64_t M, int N, int K, int scheme, int sm_count, int forced) {
+    if (forced != 0 && N % forced == 0) return forced;
+    if (N % 128 != 0) return N % 192 == 0 ? 192 : N % 64 == 0 ? 64 : N % 32 == 0 ? 32 : 16;
+    if (N % 256 != 0 || scheme == 0 || K < 2048) return 128;
     const int sms = sm_count > 0 ? sm_count : 1;
     const int64_t tiles = (M + 127) / 128 * (N / 256);
     const int64_t last = tiles % sms;
     return (last == 0 || last >= sms / 2) ? 256 : 128;
-}
-
-static int pick_umma_n(int N) {
-    if (N % 256 == 0) return 256;
-    if (N % 192 == 0) return 192;
-    if (N % 128 == 0) return 128;
-    if (N % 64 == 0) return 64;
-    if (N % 32 == 0) return 32;
-    return 16;
 }
 
 #define TMAP_OK(expr)                                                                     \
@@ -1030,39 +1007,34 @@ static int pick_umma_n(int N) {
     } while (0)
 
 // out[M][N] = A[M][K] * W[N][K]^T, flat token-major A (hi/lo planes), K % 64 == 0
-// epi_kind: 0 = fp32 output, 1 = bf16 hi/lo output (QKV scatter included), 2 = GELU + hi/lo (tile-width choice only)
-// scheme 1: A and W are f16q8 operands (SplitBuf fmt 1), K % 128 == 0.
+// scheme 1: A and W are f16q8 operands (SplitBuf fmt 1), K % 128 == 0, tile width 128 or 256.
 // lda / a_off: A is the [M][K] column slice starting at element a_off of rows that are lda elements apart (0 = dense).
-static int linear_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int64_t M, int N, int K, int epi_kind = 0,
-                         int scheme = 0, int64_t lda = 0, size_t a_off = 0) {
+// forced_bn: the tile width pick_bn takes wherever it divides N (0 = the rule's choice).
+static int linear_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int64_t M, int N, int K, int scheme = 0,
+                         int64_t lda = 0, size_t a_off = 0, int forced_bn = 0) {
     memset(&p, 0, sizeof(p));
     if (lda == 0) lda = K;
-    if (K % 64 != 0 || N % 16 != 0)  // K % 64 keeps both k-block widths legal
-        return fail("linear: K %% 64 or N %% 16 violated (N=%d K=%d)", N, K);
-    int un = pick_umma_n(N);
-    if (pairs_enabled() && pick_pair_umma_n(M, N, K, epi_kind, g_sm_count, scheme) != 0)
-        un = pick_pair_umma_n(M, N, K, epi_kind, g_sm_count, scheme);
-    const int pair = use_cta_pairs(un);
+    if (K % 64 != 0 || N % 16 != 0) return fail("linear: K %% 64 or N %% 16 violated (N=%d K=%d)", N, K);
+    const int bn = pick_bn(M, N, K, scheme, g_sm_count, forced_bn);
     if (scheme != 0) {
-        if (!pair || K % 128 != 0) return fail("f16q8 GEMM needs CTA pairs and K %% 128 == 0 (N=%d K=%d)", N, K);
+        if ((bn != 128 && bn != 256) || K % 128 != 0)
+            return fail("f16q8 GEMM needs a tile width of 128 or 256 and K %% 128 == 0 (N=%d K=%d)", N, K);
         TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, 128));
         TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, 128));
         TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, 128));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, (uint64_t)N * K, 64, un / 2));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, N, 1, K, (uint64_t)N * K, 64, un / 2));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, N, 1, K, (uint64_t)N * K, 64, un / 2));
-        p.scheme = 1, p.two_cta = 1, p.block_k = 64, p.num_k_blocks = K / 64, p.kb_per_row = K / 64;
+        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, (uint64_t)N * K, 64, bn));
+        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, N, 1, K, (uint64_t)N * K, 64, bn));
+        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, N, 1, K, (uint64_t)N * K, 64, bn));
+        p.scheme = 1;
     } else {
-        const int bk = pair ? 64 : gemm_block_k(un);
-        const int bbox = pair ? un / 2 : un;  // CTA pairs: each CTA loads half of the tile's W rows
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h() + a_off, K, M, 1, lda, (uint64_t)M * lda, bk, 128));
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l() + a_off, K, M, 1, lda, (uint64_t)M * lda, bk, 128));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, (uint64_t)N * K, bk, bbox));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, W.l(), K, N, 1, K, (uint64_t)N * K, bk, bbox));
-        p.two_cta = pair, p.block_k = bk, p.num_k_blocks = K / bk, p.kb_per_row = K / bk;
+        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, 128));
+        TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, 128));
+        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, (uint64_t)N * K, 64, bn));
+        TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, W.l(), K, N, 1, K, (uint64_t)N * K, 64, bn));
     }
+    p.num_k_blocks = K / 64, p.kb_per_row = K / 64;
     p.batches = 1, p.rows_per_batch = (int)M, p.tiles_m_per_batch = (int)((M + 127) / 128);
-    p.n_tiles = N / un, p.umma_n = un;
+    p.n_tiles = N / bn, p.bn = bn;
     p.a_row_step = 0, p.a_row_off = 0, p.a_k_per_ntile = 0, p.b_n_tiled = 1, p.b_z_per_ntile = 0;
     p.out_rows_per_batch = (int)M;
     p.alg_flops = 2.0 * (double)M * N * K;
@@ -1079,29 +1051,25 @@ static int conv_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int 
     // Tile width: tools/gemm_shapes.py times the linear with conv i's M, N = 512 and K as a proxy (H100 80GB HBM3,
     // 400 W, both models' conv stacks): f16q8 256 columns are 4-20% faster than 128 at every conv, bf16x3 128 columns
     // 25-40% faster than 256.
-    const int un = scheme != 0 ? 256 : 128;
-    const int pair = use_cta_pairs(un);
+    const int bn = scheme != 0 ? 256 : 128;
+    // weights [512][K], K index = tap*512 + channel, read linearly along K
     if (scheme != 0) {
-        if (!pair) return fail("f16q8 GEMM needs CTA pairs");
         TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
         TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
         TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, C, 1, K, (uint64_t)C * K, 64, un / 2));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, C, 1, K, (uint64_t)C * K, 64, un / 2));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, C, 1, K, (uint64_t)C * K, 64, un / 2));
-        p.scheme = 1, p.two_cta = 1, p.block_k = 64, p.num_k_blocks = K / 64, p.kb_per_row = (2 * C) / 64;
+        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, C, 1, K, (uint64_t)C * K, 64, bn));
+        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, C, 1, K, (uint64_t)C * K, 64, bn));
+        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, C, 1, K, (uint64_t)C * K, 64, bn));
+        p.scheme = 1;
     } else {
-        const int bk = pair ? 64 : gemm_block_k(un);
-        const int bbox = pair ? un / 2 : un;
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, bk, 128));
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, bk, 128));
-        // weights [512][K], K index = tap*512 + channel, read linearly along K
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, C, 1, K, (uint64_t)C * K, bk, bbox));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, W.l(), K, C, 1, K, (uint64_t)C * K, bk, bbox));
-        p.two_cta = pair, p.block_k = bk, p.num_k_blocks = K / bk, p.kb_per_row = (2 * C) / bk;
+        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
+        TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
+        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, C, 1, K, (uint64_t)C * K, 64, bn));
+        TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, W.l(), K, C, 1, K, (uint64_t)C * K, 64, bn));
     }
+    p.num_k_blocks = K / 64, p.kb_per_row = (2 * C) / 64;
     p.batches = B, p.rows_per_batch = (int)Lout, p.tiles_m_per_batch = (int)((Lout + 127) / 128);
-    p.n_tiles = C / un, p.umma_n = un;
+    p.n_tiles = C / bn, p.bn = bn;
     p.a_row_step = 1, p.a_row_off = 0, p.a_k_per_ntile = 0, p.b_n_tiled = 1, p.b_z_per_ntile = 0, p.b_k_linear = 1;
     p.out_rows_per_batch = (int)Lout;
     p.alg_flops = 2.0 * (double)B * Lout * C * K;
@@ -1128,14 +1096,14 @@ static int posconv_params(GemmParams& p, const s3b_config& c, const __nv_bfloat1
     TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, w_hi, Kc, cpg, (uint64_t)G * Kp, Kc, (uint64_t)cpg * Kc, 64, cpg));
     TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, w_lo, Kc, cpg, (uint64_t)G * Kp, Kc, (uint64_t)cpg * Kc, 64, cpg));
     p.batches = B, p.rows_per_batch = T, p.tiles_m_per_batch = (T + 127) / 128;
-    p.n_tiles = G, p.umma_n = cpg, p.block_k = 64, p.num_k_blocks = Kp * (Kc / 64), p.kb_per_row = Kc / 64;
+    p.n_tiles = G, p.bn = cpg, p.num_k_blocks = Kp * (Kc / 64), p.kb_per_row = Kc / 64;
     p.a_row_step = 1, p.a_row_off = -(Kp / 2), p.a_k_per_ntile = cpg, p.b_n_tiled = 0, p.b_z_per_ntile = Kp;
     p.out_rows_per_batch = T;
     p.alg_flops = 2.0 * (double)B * T * D * cpg * Kp;
     return 0;
 }
 
-// pos_conv with FOUR taps per k-block on CTA pairs: consecutive taps read the same activation rows shifted by one
+// pos_conv with FOUR taps per k-block: consecutive taps read the same activation rows shifted by one
 // frame, so the one-tap formulation (N = cpg = 48 columns) is bound by the shared-memory reads of its A operand
 // (4 KB per 24-cycle MMA). Writing tap = 4q + j,
 //     Z_j[u] = sum_q x[u + 4q - Kp/2] . W[4q + j],      conv[t] = sum_j Z_j[t + j]
@@ -1143,21 +1111,19 @@ static int posconv_params(GemmParams& p, const s3b_config& c, const __nv_bfloat1
 // column blocks are re-aligned by posconv_combine_kernel (norm.cu). Rows u in [0, T+3) per utterance.
 static bool posconv4_ok(const s3b_config& c) {
     const int cpg = c.embed_dim / c.pos_conv_groups;
-    if (c.pos_conv_depth > 1) return true;  // the only formulation of the data2vec blocks (checked at create / finalize)
-    return pairs_enabled() && c.pos_conv_kernel % 4 == 0 && (4 * cpg == 192 || 4 * cpg == 256) &&
-           getenv("S3B_POSCONV1") == nullptr;
+    if (c.pos_conv_depth > 1) return true;  // the only formulation of the data2vec blocks (checked at create)
+    return c.pos_conv_kernel % 4 == 0 && (4 * cpg == 192 || 4 * cpg == 256);
 }
 static int posconv4_params(GemmParams& p, const s3b_config& c, const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo,
                            const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, int B, int T) {
     memset(&p, 0, sizeof(p));
-    const int D = c.embed_dim, G = c.pos_conv_groups, cpg = D / G, Kq = pos_taps4(c) / 4, un = 4 * cpg;
+    const int D = c.embed_dim, G = c.pos_conv_groups, cpg = D / G, Kq = pos_taps4(c) / 4, bn = 4 * cpg;
     TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, x_hi, D, T, B, D, (uint64_t)T * D, 64, 128));
     TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, x_lo, D, T, B, D, (uint64_t)T * D, 64, 128));
-    TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, w_hi, 64, un, (uint64_t)G * Kq, 64, (uint64_t)un * 64, 64, un / 2));
-    TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, w_lo, 64, un, (uint64_t)G * Kq, 64, (uint64_t)un * 64, 64, un / 2));
-    p.two_cta = 1;
+    TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, w_hi, 64, bn, (uint64_t)G * Kq, 64, (uint64_t)bn * 64, 64, bn));
+    TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, w_lo, 64, bn, (uint64_t)G * Kq, 64, (uint64_t)bn * 64, 64, bn));
     p.batches = B, p.rows_per_batch = T + 3, p.tiles_m_per_batch = (T + 3 + 127) / 128;
-    p.n_tiles = G, p.umma_n = un, p.block_k = 64, p.num_k_blocks = Kq, p.kb_per_row = 1;
+    p.n_tiles = G, p.bn = bn, p.num_k_blocks = Kq, p.kb_per_row = 1;
     p.a_row_step = 4, p.a_row_off = -(pos_taps(c) / 2), p.a_k_per_ntile = cpg, p.b_n_tiled = 0, p.b_z_per_ntile = Kq;
     p.out_rows_per_batch = T + 3;
     p.k_steps = (cpg + 15) / 16;  // 48 channels per group: the 4th k-step of every 64-wide box has zero weights
@@ -1216,27 +1182,6 @@ static int launch_frontend(s3b_model* m, cudaStream_t st, const float* const* d_
     return 0;
 }
 
-// LayerNorm fused into the producing GEMM (gemm.cuh: ln_*): on unless S3B_FUSE_LN=0 (kept for A/B measurements)
-// S3B_FUSE_LN: 0 = never, 1 = wherever possible, unset = only where the tile's MMAs (K >= 2048: fc2) leave the epilogue
-// warps the slack to do it
-static int fuse_ln_mode() {
-#ifndef S3B_ENABLE_FUSED_LN
-    return 0;  // not compiled in (see gemm_sm100.cu): every LayerNorm is its own launch
-#endif
-    const char* e = getenv("S3B_FUSE_LN");  // read per call: tests toggle it (the plan cache is keyed on it)
-    if (!pairs_enabled()) return 0;
-    if (e == nullptr) return 2;
-    return e[0] == '0' ? 0 : 1;
-}
-// (the fused LayerNorm's operand output uses the GEMM's out_fmt: callers keep both in the same format)
-static void set_ln(GemmParams& p, const float* gamma, const float* beta, int gelu, float* out_f32, const OutPlanes& op,
-                   unsigned int* counter) {
-    p.ln_gamma = gamma, p.ln_beta = beta, p.ln_gelu = gelu, p.ln_out_f32 = out_f32;
-    p.ln_out_hi = op.hi, p.ln_out_lo = op.lo, p.ln_out_h8 = op.h8, p.ln_out_l8 = op.l8;
-    if (op.hi != nullptr) p.out_fmt = op.fmt;
-    p.ln_counter = counter;
-}
-
 // ------------------------------------------------------------------------------------------------
 // cached launch plan: every tensor map / GEMM descriptor of one forward at a given (B, Lmax)
 // ------------------------------------------------------------------------------------------------
@@ -1253,7 +1198,6 @@ struct Plan {
     int B = 0;
     int64_t Lmax = 0;
     uint64_t gen = 0;
-    int fuse_ln = 0;
     GemmParams conv[kNumConv];
     GemmParams proj, pos;
     GemmParams pos_d[8];             // data2vec: one four-taps GEMM per conv block (pos_conv_depth <= 8)
@@ -1265,7 +1209,7 @@ struct Plan {
 
 void Workspace::release() {
     DevBuf* bufs[] = {&book, &wav_stats, &wav_pad, &c0_part, &c0_ss, &conv_f32, &tmp_f32, &x_f32, &x1_f32, &gate, &pos_z,
-                      &ln_counters, &hs0, &glu_f32, &fb_f32, &xg_f32};
+                      &hs0, &glu_f32, &fb_f32, &xg_f32};
     for (DevBuf* b : bufs) b->release();
     for (int i = 0; i < kNumConv; ++i) act[i].release();
     SplitBuf* sb[] = {&ln512_s, &x_s, &xs_s, &q_s, &k_s, &vt_s, &ctx_s, &x1_s, &h_s};
@@ -1313,8 +1257,6 @@ struct Fwd {
     int* d_kv = nullptr;
     int* d_ord = nullptr;  // APC: utterances longest first (the recurrence kernel's grouping)
     uint8_t* d_mask = nullptr;
-    int fuse_ln = 0;  // fuse_ln_mode()
-    unsigned int* cnt[2] = {nullptr, nullptr};  // two alternating row-block counter arrays of the fused LayerNorm
 
     static constexpr int kConformerStages = 10;  // stages per Conformer layer (conformer_stage)
     int num_stages() const {
@@ -1444,19 +1386,12 @@ int Fwd::prepare() {
         if (c.relative_position) S3B_OK(w->gate.ensure((size_t)B * H * T * 4));
         if (c.family == 3) S3B_OK(w->hs0.ensure((size_t)M * D * 4));
     }
-    fuse_ln = fuse_ln_mode();
-    {
-        const size_t n_cnt = (size_t)B * (L[1] / 128 + 2) + (size_t)M / 128 + 16;
-        S3B_OK(w->ln_counters.ensure(2 * n_cnt * sizeof(unsigned int)));
-        cnt[0] = w->ln_counters.as<unsigned int>();
-        cnt[1] = cnt[0] + n_cnt;
-    }
 
     // ---- launch plan (cached per (B, Lmax) while no buffer has been reallocated) --------------------------------
     plan = nullptr;
     for (size_t i = 0; i < w->plans.size(); ++i) {
         Plan* pl = w->plans[i];
-        if (pl->B == B && pl->Lmax == Lmax && pl->gen == g_alloc_generation && pl->fuse_ln == fuse_ln) {
+        if (pl->B == B && pl->Lmax == Lmax && pl->gen == g_alloc_generation) {
             plan = pl;
             w->plans.erase(w->plans.begin() + i);
             w->plans.insert(w->plans.begin(), pl);
@@ -1470,7 +1405,7 @@ int Fwd::prepare() {
             delete pl;
             return r;
         }
-        pl->B = B, pl->Lmax = Lmax, pl->gen = g_alloc_generation, pl->fuse_ln = fuse_ln;
+        pl->B = B, pl->Lmax = Lmax, pl->gen = g_alloc_generation;
         w->plans.insert(w->plans.begin(), pl);
         while (w->plans.size() > 4) {
             delete w->plans.back();
@@ -1515,58 +1450,58 @@ int Fwd::build_conformer_layer(LayerPlan& lp, int l) {
     LayerW& W = m->layers[l];
     {   // ffn1.w_1 + SiLU
         GemmParams& p = lp.ffn1_a;
-        S3B_OK(linear_params(p, w->xs_s, W.ffn1_w1, M, F, D, 2, sch));
+        S3B_OK(linear_params(p, w->xs_s, W.ffn1_w1, M, F, D, sch));
         Epi e;
         e.bias = W.ffn1_b1.as<float>(), e.gelu = 2, e.op = w->h_s.planes(sch);
         set_epi(p, e, F);
     }
     {   // r1 = x + 0.5 ffn1 (0.5 folded into w_2; residual = hidden state l, patched per call)
         GemmParams& p = lp.ffn1_b;
-        S3B_OK(linear_params(p, w->h_s, W.ffn1_w2, M, D, F, 0, sch));
+        S3B_OK(linear_params(p, w->h_s, W.ffn1_w2, M, D, F, sch));
         Epi e;
         e.bias = W.ffn1_b2.as<float>(), e.out_f32 = w->x1_f32.as<float>();
         set_epi(p, e, D);
     }
     {   // [q | k] from rope(LN(r1)), v from LN(r1)
         GemmParams& p = lp.qkv;
-        S3B_OK(linear_params(p, w->x1_s, W.qkv, M, 2 * D, D, 1, sch));
+        S3B_OK(linear_params(p, w->x1_s, W.qkv, M, 2 * D, D, sch));
         set_qkv_epi(p, W.qkv_b.as<float>(), T, H, 64, w->q_s, w->k_s, w->vt_s, 0);
         GemmParams& pv = lp.v;
-        S3B_OK(linear_params(pv, w->xs_s, W.v, M, D, D, 1, sch));
+        S3B_OK(linear_params(pv, w->xs_s, W.v, M, D, D, sch));
         set_qkv_epi(pv, W.qkv_b.as<float>() + 2 * D, T, H, 64, w->q_s, w->k_s, w->vt_s, 2 * D);
     }
     S3B_OK(attn_params(lp.attn, w, B, T, H, 64, d_kv, sch));
     {   // r2 = r1 + linear_out(attn)
         GemmParams& p = lp.out;
-        S3B_OK(linear_params(p, w->ctx_s, W.out, M, D, D, 0, sch));
+        S3B_OK(linear_params(p, w->ctx_s, W.out, M, D, D, sch));
         Epi e;
         e.bias = W.out_b.as<float>(), e.residual = w->x1_f32.as<float>(), e.out_f32 = w->x_f32.as<float>();
         set_epi(p, e, D);
     }
     {   // pointwise_conv1 (no bias) -> fp32 [M][2D], the depthwise kernel's input
         GemmParams& p = lp.pw1;
-        S3B_OK(linear_params(p, w->xs_s, W.pw1, M, 2 * D, D, 0, sch));
+        S3B_OK(linear_params(p, w->xs_s, W.pw1, M, 2 * D, D, sch));
         Epi e;
         e.out_f32 = w->glu_f32.as<float>();
         set_epi(p, e, 2 * D);
     }
     {   // r3 = r2 + pointwise_conv2 (no bias)
         GemmParams& p = lp.pw2;
-        S3B_OK(linear_params(p, w->x1_s, W.pw2, M, D, D, 0, sch));
+        S3B_OK(linear_params(p, w->x1_s, W.pw2, M, D, D, sch));
         Epi e;
         e.residual = w->x_f32.as<float>(), e.out_f32 = w->x1_f32.as<float>();
         set_epi(p, e, D);
     }
     {   // ffn2.w_1 + SiLU
         GemmParams& p = lp.fc1;
-        S3B_OK(linear_params(p, w->xs_s, W.fc1, M, F, D, 2, sch));
+        S3B_OK(linear_params(p, w->xs_s, W.fc1, M, F, D, sch));
         Epi e;
         e.bias = W.fc1_b.as<float>(), e.gelu = 2, e.op = w->h_s.planes(sch);
         set_epi(p, e, F);
     }
     {   // r4 = r3 + 0.5 ffn2
         GemmParams& p = lp.fc2;
-        S3B_OK(linear_params(p, w->h_s, W.fc2, M, D, F, 0, sch));
+        S3B_OK(linear_params(p, w->h_s, W.fc2, M, D, F, sch));
         Epi e;
         e.bias = W.fc2_b.as<float>(), e.residual = w->x1_f32.as<float>(), e.out_f32 = w->tmp_f32.as<float>();
         set_epi(p, e, D);
@@ -1582,7 +1517,7 @@ int Fwd::build_plan(Plan& pl) {
         pl.gru_in.resize(NL);
         for (int l = 0; l < NL; ++l) {
             GemmParams& p = pl.gru_in[l];
-            S3B_OK(linear_params(p, l == 0 ? w->ln512_s : w->x_s, m->layers[l].wih, M, 3 * D, l == 0 ? kDecoar2K : D, 0,
+            S3B_OK(linear_params(p, l == 0 ? w->ln512_s : w->x_s, m->layers[l].wih, M, 3 * D, l == 0 ? kDecoar2K : D,
                                  m->scheme));
             Epi e;
             e.bias = m->layers[l].gru_b.as<float>();
@@ -1606,13 +1541,10 @@ int Fwd::build_plan(Plan& pl) {
             else e.op = w->act[i].planes(m->scheme);
         }
         set_epi(p, e, C);
-        if (c.extractor_layer_norm && fuse_ln == 1 && p.two_cta)  // per-frame LayerNorm(512) + GELU (wav2vec2_model.py:2887-2897)
-            set_ln(p, m->conv_ln_g[i].as<float>(), m->conv_ln_b[i].as<float>(), 1, last ? w->conv_f32.as<float>() : nullptr,
-                   last ? no_planes() : w->act[i].planes(m->scheme), cnt[i & 1]);
     }
     {
         GemmParams& p = pl.proj;
-        S3B_OK(linear_params(p, w->ln512_s, m->proj_w, M, D, decoar2(m) ? kDecoar2K : C, 1, m->scheme));
+        S3B_OK(linear_params(p, w->ln512_s, m->proj_w, M, D, decoar2(m) ? kDecoar2K : C, m->scheme));
         Epi e;
         e.bias = m->proj_b.as<float>();
         e.row_mask = d_mask;  // x[padding_mask] = 0 (wav2vec2_model.py:3061-3062)
@@ -1658,29 +1590,22 @@ int Fwd::build_plan(Plan& pl) {
         LayerPlan& lp = pl.layers[l];
         {   // QKV projection, scattered per head
             GemmParams& p = lp.qkv;
-            S3B_OK(linear_params(p, w->xs_s, W.qkv, M, 3 * D, D, 1, m->scheme));
+            S3B_OK(linear_params(p, w->xs_s, W.qkv, M, 3 * D, D, m->scheme));
             set_qkv_epi(p, W.qkv_b.as<float>(), T, H, head_dim(c), w->q_s, w->k_s, w->vt_s);
         }
         S3B_OK(attn_params(lp.attn, w, B, T, H, head_dim(c), d_kv, m->scheme));
         if (c.relative_position) set_rel_bias(lp.attn, m->rel_table.as<float>(), m->rel_table_T, w->gate.as<float>());
         {   // out_proj + residual (residual = hidden state l, patched per call)
             GemmParams& p = lp.out;
-            S3B_OK(linear_params(p, w->ctx_s, W.out, M, D, D, 0, m->scheme));
+            S3B_OK(linear_params(p, w->ctx_s, W.out, M, D, D, m->scheme));
             Epi e;
             e.bias = W.out_b.as<float>();
             e.out_f32 = c.layer_norm_first ? w->x1_f32.as<float>() : w->tmp_f32.as<float>();
             set_epi(p, e, D);
-            if (fuse_ln == 1 && p.two_cta) {
-                if (c.layer_norm_first)  // x1_s = LN2(r1), r1 = x1_f32
-                    set_ln(p, W.ln2_g.as<float>(), W.ln2_b.as<float>(), 0, nullptr, w->x1_s.planes(m->scheme), cnt[0]);
-                else  // x1 = LN1(x + attn)
-                    set_ln(p, W.ln1_g.as<float>(), W.ln1_b.as<float>(), 0, w->x1_f32.as<float>(),
-                           w->x1_s.planes(m->scheme), cnt[0]);
-            }
         }
         {   // fc1 + GELU
             GemmParams& p = lp.fc1;
-            S3B_OK(linear_params(p, w->x1_s, W.fc1, M, F, D, 2, m->scheme));
+            S3B_OK(linear_params(p, w->x1_s, W.fc1, M, F, D, m->scheme));
             Epi e;
             e.bias = W.fc1_b.as<float>();
             e.gelu = 1;
@@ -1689,23 +1614,12 @@ int Fwd::build_plan(Plan& pl) {
         }
         {   // fc2 + residual (output patched per call for pre-LN models)
             GemmParams& p = lp.fc2;
-            S3B_OK(linear_params(p, w->h_s, W.fc2, M, D, F, 0, m->scheme));
+            S3B_OK(linear_params(p, w->h_s, W.fc2, M, D, F, m->scheme));
             Epi e;
             e.bias = W.fc2_b.as<float>();
             e.residual = w->x1_f32.as<float>();
             e.out_f32 = w->tmp_f32.as<float>();
             set_epi(p, e, D);
-            if (fuse_ln && p.two_cta) {
-                const bool last = (l == NL - 1);
-                if (!c.layer_norm_first)  // hidden state l+1 = LN2(x1 + ffn) (fp32 output patched per call) + operand of layer l+1
-                    set_ln(p, W.ln2_g.as<float>(), W.ln2_b.as<float>(), 0, nullptr,
-                           last ? no_planes() : w->xs_s.planes(m->scheme), cnt[1]);
-                else if (last)  // encoder.layer_norm on the final output (wav2vec2_model.py:3049-3050), output patched per call
-                    set_ln(p, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(), 0, nullptr, no_planes(), cnt[1]);
-                else  // pre-LN: the NEXT layer's LN1 of the residual stream this GEMM produces
-                    set_ln(p, m->layers[l + 1].ln1_g.as<float>(), m->layers[l + 1].ln1_b.as<float>(), 0, nullptr,
-                           w->xs_s.planes(m->scheme), cnt[1]);
-            }
         }
     }
     if (c.pred_heads > 0) {
@@ -1714,7 +1628,7 @@ int Fwd::build_plan(Plan& pl) {
         const int N = c.pred_heads;
         {
             GemmParams& p = pl.pred1;
-            S3B_OK(linear_params(p, w->xs_s, m->pred1_w, M, N * D, D, 2, m->scheme));
+            S3B_OK(linear_params(p, w->xs_s, m->pred1_w, M, N * D, D, m->scheme));
             Epi e;
             e.bias = m->pred1_b.as<float>();
             e.gelu = 1;
@@ -1724,7 +1638,7 @@ int Fwd::build_plan(Plan& pl) {
         pl.pred2.resize(N);
         for (int k = 0; k < N; ++k) {
             GemmParams& p = pl.pred2[k];
-            S3B_OK(linear_params(p, w->h_s, m->pred2_w[k], M, D, D, 0, m->scheme, (int64_t)N * D, (size_t)k * D));
+            S3B_OK(linear_params(p, w->h_s, m->pred2_w[k], M, D, D, m->scheme, (int64_t)N * D, (size_t)k * D));
             Epi e;
             e.bias = m->pred2_b.as<float>() + (size_t)k * D;
             e.out_f32 = w->tmp_f32.as<float>();  // patched per call: output slot NL + 1 + k
@@ -1752,7 +1666,7 @@ int Fwd::apc_stage(int s) {
     if (l >= NL) return fail("internal: stage %d out of range", s);
     if ((s - 1) % 2 == 0) {
         GemmParams p = plan->gru_in[l];
-        KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+        KGEMM(launch_gemm(p, m->sm_count, st));
         return 0;
     }
     const LayerW& W = m->layers[l];
@@ -1796,8 +1710,8 @@ int Fwd::stage(int s) {
         if (decoar2(m)) return 0;  // no conv stack
         const int i = s;
         GemmParams p = plan->conv[i];
-        KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
-        if (c.extractor_layer_norm && p.ln_gamma == nullptr) {
+        KGEMM(launch_gemm(p, m->sm_count, st));
+        if (c.extractor_layer_norm) {
             const bool last = (i == kNumConv - 1);
             KNORM(launch_layernorm(w->conv_f32.as<float>(), (size_t)B * L[i], C, m->conv_ln_g[i].as<float>(),
                                    m->conv_ln_b[i].as<float>(), 1, last ? w->conv_f32.as<float>() : nullptr,
@@ -1813,7 +1727,7 @@ int Fwd::stage(int s) {
         GemmParams p = plan->proj;
         p.out_f32 = proj_out();  // distiller: feat_final IS output slot 0 (padded frames zeroed, like the reference's
                                  // in-place x[padding_mask] = 0 on the same storage, distiller/module.py:303-304)
-        KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+        KGEMM(launch_gemm(p, m->sm_count, st));
         if (distil() && layer_done) S3B_OK(layer_done(m, 0, st, user));
         return 0;
     }
@@ -1840,7 +1754,7 @@ int Fwd::stage(int s) {
             const bool ln = !c.layer_norm_first;
             for (int i = 0; i < c.pos_conv_depth; ++i) {
                 const bool last = (i == c.pos_conv_depth - 1);
-                KGEMM(launch_gemm_bf16x3(plan->pos_d[i], m->sm_count, st));
+                KGEMM(launch_gemm(plan->pos_d[i], m->sm_count, st));
                 const SplitBuf& nxt = (i & 1) ? w->ctx_s : w->x1_s;  // == the `in` of block i+1 in build_plan
                 KNORM(launch_posconv_combine(w->pos_z.as<float>(), last ? proj_out() : nullptr, m->posd_b[i].as<float>(), B,
                                              T, D, D / c.pos_conv_groups, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(),
@@ -1848,7 +1762,7 @@ int Fwd::stage(int s) {
                                              last ? (ln ? w->xs_s.planes(m->scheme) : no_planes()) : nxt.planes(0), st));
             }
         } else if (posconv4_ok(c)) {
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            KGEMM(launch_gemm(p, m->sm_count, st));
             const bool ln = !c.layer_norm_first;
             KNORM(launch_posconv_combine(w->pos_z.as<float>(), proj_out(), m->pos_b.as<float>(), B, T, D,
                                          D / c.pos_conv_groups, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(),
@@ -1856,7 +1770,7 @@ int Fwd::stage(int s) {
         } else {
             p.residual = proj_out();
             if (c.layer_norm_first) p.out_f32 = hs0;
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            KGEMM(launch_gemm(p, m->sm_count, st));
             if (!c.layer_norm_first)
                 KNORM(launch_layernorm(w->tmp_f32.as<float>(), (size_t)M, D, m->enc_ln_g.as<float>(),
                                        m->enc_ln_b.as<float>(), 0, hs0, w->xs_s.planes(m->scheme), st));
@@ -1870,11 +1784,11 @@ int Fwd::stage(int s) {
         const int k = s - (9 + 5 * NL);  // 0: Linear + GELU, 1..N: SplitLinear task k-1
         if (k == 0) {
             GemmParams p = plan->pred1;
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            KGEMM(launch_gemm(p, m->sm_count, st));
         } else {
             GemmParams p = plan->pred2[k - 1];
             p.out_f32 = slot(NL + k);
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            KGEMM(launch_gemm(p, m->sm_count, st));
             if (layer_done) S3B_OK(layer_done(m, NL + k, st, user));
         }
         return 0;
@@ -1891,12 +1805,12 @@ int Fwd::stage(int s) {
     const bool rel = c.relative_position != 0;
     switch (sub) {
         case 0: {
-            // pre-LN: xs = LN1(residual stream); from layer 1 on it is produced by the previous layer's fc2 epilogue
-            if (c.layer_norm_first && (l == 0 || plan->layers[l - 1].fc2.ln_gamma == nullptr))
+            // pre-LN: xs = LN1(residual stream)
+            if (c.layer_norm_first)
                 KNORM(launch_layernorm(hs_in, (size_t)M, D, W.ln1_g.as<float>(), W.ln1_b.as<float>(), 0, nullptr,
                                        w->xs_s.planes(m->scheme), st));
             GemmParams p = lp.qkv;
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            KGEMM(launch_gemm(p, m->sm_count, st));
             if (rel)  // gate from the layer's attention input (post-LN: hs_in; pre-LN: LN1 output) modules.py:534-551
                 KMISC(launch_wavlm_gate(w->xs_s.planes(m->scheme), (size_t)M, B, T, H, D,
                                         c.gru_rel_pos ? W.grep_w.as<float>() : nullptr, W.grep_b.as<float>(),
@@ -1910,8 +1824,7 @@ int Fwd::stage(int s) {
         case 2: {
             GemmParams p = lp.out;
             p.residual = hs_in;
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
-            if (p.ln_gamma != nullptr) return 0;  // LayerNorm fused into the GEMM
+            KGEMM(launch_gemm(p, m->sm_count, st));
             if (c.layer_norm_first)  // x1_s = LN2(r1), r1 = x1_f32
                 KNORM(launch_layernorm(w->x1_f32.as<float>(), (size_t)M, D, W.ln2_g.as<float>(), W.ln2_b.as<float>(), 0,
                                        nullptr, w->x1_s.planes(m->scheme), st));
@@ -1922,7 +1835,7 @@ int Fwd::stage(int s) {
         }
         case 3: {
             GemmParams p = lp.fc1;
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            KGEMM(launch_gemm(p, m->sm_count, st));
             return 0;
         }
         default: {
@@ -1931,12 +1844,7 @@ int Fwd::stage(int s) {
             float* unnorm = (last && last_res != nullptr) ? last_res : w->tmp_f32.as<float>();
             if (c.layer_norm_first) p.out_f32 = last ? unnorm : hs_out;
             if (ffn_out != nullptr) p.out_pre = ffn_out + (size_t)l * ffn_stride;
-            if (p.ln_gamma != nullptr && (!c.layer_norm_first || last)) p.ln_out_f32 = hs_out;
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
-            if (p.ln_gamma != nullptr) {
-                if (layer_done) S3B_OK(layer_done(m, l + 1, st, user));
-                return 0;
-            }
+            KGEMM(launch_gemm(p, m->sm_count, st));
             const bool want_planes = !last || c.pred_heads > 0;  // the next layer's (or the prediction heads') operand
             if (c.layer_norm_first) {
                 if (last)  // encoder.layer_norm on the final output (wav2vec2_model.py:3049-3050)
@@ -1967,13 +1875,13 @@ int Fwd::conformer_stage(int l, int sub) {
         case 0: {  // ffn1: LayerNorm -> w_1 + SiLU
             KNORM(launch_layernorm(hs(l), (size_t)M, D, W.ffn1_ln_g.as<float>(), W.ffn1_ln_b.as<float>(), 0, nullptr, xs, st));
             GemmParams p = lp.ffn1_a;
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            KGEMM(launch_gemm(p, m->sm_count, st));
             return 0;
         }
         case 1: {  // r1 = x + 0.5 w_2(...)
             GemmParams p = lp.ffn1_b;
             p.residual = hs(l);
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            KGEMM(launch_gemm(p, m->sm_count, st));
             return 0;
         }
         case 2: {  // self_attn_layer_norm + RoPE -> [q | k] and v
@@ -1981,10 +1889,10 @@ int Fwd::conformer_stage(int l, int sub) {
                                         m->rope_cs.as<float>(), xs, w->x1_s.planes(m->scheme), st));
             {
                 GemmParams p = lp.qkv;
-                KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+                KGEMM(launch_gemm(p, m->sm_count, st));
             }
             GemmParams p = lp.v;
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            KGEMM(launch_gemm(p, m->sm_count, st));
             return 0;
         }
         case 3:
@@ -1992,14 +1900,14 @@ int Fwd::conformer_stage(int l, int sub) {
             return 0;
         case 4: {  // r2 = r1 + linear_out
             GemmParams p = lp.out;
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            KGEMM(launch_gemm(p, m->sm_count, st));
             return 0;
         }
         case 5: {  // conv_module: LayerNorm -> pointwise_conv1
             KNORM(launch_layernorm(w->x_f32.as<float>(), (size_t)M, D, W.conv_ln_g.as<float>(), W.conv_ln_b.as<float>(), 0,
                                    nullptr, xs, st));
             GemmParams p = lp.pw1;
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            KGEMM(launch_gemm(p, m->sm_count, st));
             return 0;
         }
         case 6:  // GLU -> depthwise conv -> BatchNorm -> SiLU
@@ -2008,20 +1916,20 @@ int Fwd::conformer_stage(int l, int sub) {
             return 0;
         case 7: {  // r3 = r2 + pointwise_conv2
             GemmParams p = lp.pw2;
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            KGEMM(launch_gemm(p, m->sm_count, st));
             return 0;
         }
         case 8: {  // ffn2: LayerNorm -> w_1 + SiLU
             KNORM(launch_layernorm(w->x1_f32.as<float>(), (size_t)M, D, W.ffn2_ln_g.as<float>(), W.ffn2_ln_b.as<float>(), 0,
                                    nullptr, xs, st));
             GemmParams p = lp.fc1;
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            KGEMM(launch_gemm(p, m->sm_count, st));
             return 0;
         }
         default: {  // r4 = r3 + 0.5 w_2(...) -> final_layer_norm -> hidden state l+1 (pre-LN: encoder.layer_norm after
                     // the last layer, wav2vec2_model.py:3049-3050)
             GemmParams p = lp.fc2;
-            KGEMM(launch_gemm_bf16x3(p, m->sm_count, st));
+            KGEMM(launch_gemm(p, m->sm_count, st));
             float* r4 = w->tmp_f32.as<float>();
             const bool enc_ln = c.layer_norm_first && l == c.num_layers - 1;
             KNORM(launch_layernorm(r4, (size_t)M, D, W.ln2_g.as<float>(), W.ln2_b.as<float>(), 0, enc_ln ? r4 : hs(l + 1),
@@ -2481,7 +2389,7 @@ static int device_sm_count(int* out) {
 // exactly that scheme (linear_params / conv_params refuse an f16q8 request the shape cannot take)
 static int resolve_scheme(int scheme, int K, int N, int* out) {
     if (scheme < -1 || scheme > 1) return fail("scheme must be -1 (default), 0 (bf16x3) or 1 (f16q8), not %d", scheme);
-    if (scheme == -1) scheme = (K % 128 == 0 && N % 128 == 0 && pairs_enabled()) ? default_scheme() : 0;
+    if (scheme == -1) scheme = (K % 128 == 0 && N % 128 == 0) ? default_scheme() : 0;
     *out = scheme;
     return 0;
 }
@@ -2526,7 +2434,6 @@ extern "C" int s3b_linear_ex(const float* a, const float* w, const float* bias, 
     if (gelu < 0 || gelu > 2) return fail("gelu must be 0 (none), 1 (GELU) or 2 (SiLU), not %d", gelu);
     if (o.tile_n != 0 && o.tile_n != 128 && o.tile_n != 256) return fail("tile_n must be 0, 128 or 256, not %d", o.tile_n);
     if (o.tile_n != 0 && N % o.tile_n != 0) return fail("tile_n %d does not divide N = %d", o.tile_n, N);
-    if (o.tile_n != 0 && !pairs_enabled()) return fail("tile_n needs the paired tile layout (S3B_GEMM_PAIR=0 is set)");
     const int64_t lda = o.lda != 0 ? o.lda : K;
     if (o.a_off < 0 || o.a_off + K > lda || (o.lda != 0 && (lda % 16 != 0 || o.a_off % 16 != 0)))
         return fail("A slice [%lld, %lld) of rows of %lld elements: out of range or not a multiple of 16",
@@ -2540,12 +2447,8 @@ extern "C" int s3b_linear_ex(const float* a, const float* w, const float* bias, 
     const int r = [&]() -> int {
         S3B_OK(split_operand(a, as, (size_t)M * lda, scheme, 0, st));
         S3B_OK(split_operand(w, ws, (size_t)N * K, scheme, 1, st));
-        const int epi_kind = o.out_fmt < 0 ? 0 : (gelu ? 2 : 1);
-        g_force_pair_un = o.tile_n;
-        const int rp = linear_params(p, as, ws, M, N, K, epi_kind, scheme, lda, (size_t)o.a_off);
-        g_force_pair_un = 0;
-        S3B_OK(rp);
-        if (o.tile_n != 0 && p.umma_n != o.tile_n) return fail("tile_n %d requested, %d chosen", o.tile_n, p.umma_n);
+        S3B_OK(linear_params(p, as, ws, M, N, K, scheme, lda, (size_t)o.a_off, o.tile_n));
+        if (o.tile_n != 0 && p.bn != o.tile_n) return fail("tile_n %d requested, %d chosen", o.tile_n, p.bn);
         Epi e;
         e.bias = bias, e.residual = residual, e.gelu = gelu, e.row_mask = o.row_mask;
         if (o.out_fmt < 0) {
@@ -2556,13 +2459,13 @@ extern "C" int s3b_linear_ex(const float* a, const float* w, const float* bias, 
         }
         set_epi(p, e, N);
         p.out_pre = o.out_pre;
-        CUDA_OK(launch_gemm_bf16x3(p, sms, st));
+        CUDA_OK(launch_gemm(p, sms, st));
         if (o.out_fmt >= 0) CUDA_OK(launch_planes_to_f32(os.planes(o.out_fmt), (size_t)M * N, out, st));
         CUDA_OK(cudaStreamSynchronize(st));
         return 0;
     }();
     as.release(), ws.release(), os.release();
-    if (r == 0 && opts != nullptr) opts->scheme_used = scheme, opts->tile_n_used = p.umma_n;
+    if (r == 0 && opts != nullptr) opts->scheme_used = scheme, opts->tile_n_used = p.bn;
     return r;
 }
 
@@ -2592,9 +2495,9 @@ extern "C" int s3b_qkv_hd_f32(const float* x, const float* w, const float* b, in
         S3B_OK(ks.ensure((size_t)M * D));
         S3B_OK(vts.ensure((size_t)B * D * Tp));
         GemmParams p;
-        S3B_OK(linear_params(p, xs, ws, M, 3 * D, D, 1, sch));
+        S3B_OK(linear_params(p, xs, ws, M, 3 * D, D, sch));
         set_qkv_epi(p, b, T, H, hd, qs, ks, vts);
-        CUDA_OK(launch_gemm_bf16x3(p, sms, st));
+        CUDA_OK(launch_gemm(p, sms, st));
         CUDA_OK(launch_planes_to_f32(qs.planes(0), (size_t)M * D, q_out, st));
         CUDA_OK(launch_planes_to_f32(ks.planes(0), (size_t)M * D, k_out, st));
         CUDA_OK(launch_planes_to_f32(vts.planes(0), (size_t)B * D * Tp, vt_out, st));
@@ -2641,7 +2544,7 @@ extern "C" int s3b_conv_gemm_f32(const float* x, const float* w, const float* bi
             e.op = os.planes(out_fmt);
         }
         set_epi(p, e, C);
-        CUDA_OK(launch_gemm_bf16x3(p, sms, st));
+        CUDA_OK(launch_gemm(p, sms, st));
         if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), (size_t)B * Lout * C, out, st));
         CUDA_OK(cudaStreamSynchronize(st));
         return 0;
@@ -2669,7 +2572,6 @@ extern "C" int s3b_posconv_f32(const float* x, const float* w, const float* bias
     if (taps == 1 && mode != 0) return fail("the data2vec blocks (mode 1, 2) run four taps per k-block only");
     if (taps == 1 && gamma == nullptr && out_fmt >= 0)  // Fwd::stage(8): the one-tap epilogue writes fp32 only
         return fail("one tap per k-block writes operand planes only through the LayerNorm (gamma)");
-    if (!pairs_enabled() && taps == 4) return fail("four taps per k-block need the paired tile layout (S3B_GEMM_PAIR=0)");
     S3B_OK(check_out_fmt(out_fmt));
     // one conv block of k taps: pos_taps(c) = k (the data2vec blocks' k = max(3, conv_pos / depth) is the caller's)
     s3b_config c;
@@ -2702,7 +2604,7 @@ extern "C" int s3b_posconv_f32(const float* x, const float* w, const float* bias
             S3B_OK(posconv4_params(p, c, xs.h(), xs.l(), ws.h(), ws.l(), B, T));
             e.out_f32 = z.as<float>();
             set_epi(p, e, 4 * D);
-            CUDA_OK(launch_gemm_bf16x3(p, sms, st));
+            CUDA_OK(launch_gemm(p, sms, st));
             CUDA_OK(launch_posconv_combine(z.as<float>(), x, bias, B, T, D, cpg, gamma, beta, gamma ? 1 : 0, mode,
                                            out_f32, op, st));
         } else {
@@ -2716,7 +2618,7 @@ extern "C" int s3b_posconv_f32(const float* x, const float* w, const float* bias
                 e.out_f32 = out_f32;
             }
             set_epi(p, e, D);
-            CUDA_OK(launch_gemm_bf16x3(p, sms, st));
+            CUDA_OK(launch_gemm(p, sms, st));
             if (gamma != nullptr) CUDA_OK(launch_layernorm(z.as<float>(), M, D, gamma, beta, 0, out_f32, op, st));
         }
         if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(op, M * D, out, st));
@@ -2747,11 +2649,9 @@ extern "C" int s3b_gemm_bench(int64_t M, int32_t N, int32_t K, int32_t gelu, int
     CUDA_OK(cudaMemset(as.hi.p, 0x3c, (size_t)M * K * 2));
     CUDA_OK(cudaMemset(ws.hi.p, 0x3c, (size_t)N * K * 2));
     GemmParams p;
-    g_force_pair_un = force_un;
     int scheme = default_scheme();
-    if (K % 128 != 0 || N % 128 != 0 || !pairs_enabled()) scheme = 0;
-    int r = linear_params(p, as, ws, M, N, K, gelu ? 2 : 0, scheme);
-    g_force_pair_un = 0;
+    if (K % 128 != 0 || N % 128 != 0) scheme = 0;
+    int r = linear_params(p, as, ws, M, N, K, scheme, 0, 0, force_un);
     if (r == 0) {
         Epi e;
         e.bias = bias.as<float>();
@@ -2760,9 +2660,9 @@ extern "C" int s3b_gemm_bench(int64_t M, int32_t N, int32_t K, int32_t gelu, int
         set_epi(p, e, N);
         cudaEvent_t e0, e1;
         cudaEventCreate(&e0), cudaEventCreate(&e1);
-        for (int i = 0; i < 3; ++i) launch_gemm_bf16x3(p, sms, 0);
+        for (int i = 0; i < 3; ++i) launch_gemm(p, sms, 0);
         cudaEventRecord(e0, 0);
-        for (int i = 0; i < iters; ++i) launch_gemm_bf16x3(p, sms, 0);
+        for (int i = 0; i < iters; ++i) launch_gemm(p, sms, 0);
         cudaEventRecord(e1, 0);
         cudaError_t ce = cudaDeviceSynchronize();
         float ms = 0.f;
@@ -2770,7 +2670,7 @@ extern "C" int s3b_gemm_bench(int64_t M, int32_t N, int32_t K, int32_t gelu, int
         *ms_per_launch = ms / iters;
         cudaEventDestroy(e0), cudaEventDestroy(e1);
         if (ce != cudaSuccess) r = fail("gemm bench failed: %s", cudaGetErrorString(ce));
-        else if (ms_per_launch[0] >= 0) ms_per_launch[1] = (float)p.umma_n;
+        else if (ms_per_launch[0] >= 0) ms_per_launch[1] = (float)p.bn;
     }
     as.release(), ws.release(), os.release(), bias.release(), res.release(), out.release();
     return r;

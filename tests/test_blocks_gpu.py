@@ -34,6 +34,7 @@ def _stream():
         (130, 64, 128, True, False, False),
         (64, 48, 192, True, True, False),
         (2000, 768, 3072, True, False, True),
+        (300, 576, 256, True, True, True),  # N % 192 == 0, N % 128 != 0: the 192-wide tile
     ],
 )
 @pytest.mark.parametrize("scheme", [None, 0, 1])

@@ -7,7 +7,7 @@
 
 For both operand schemes (f16q8, bf16x3), both row counts of bench.py's step (base, hubert_base 32 x 10 s: M = 7984 =
 16 utterances x 499 frames, one of two lanes, and M = 15968, the whole batch in one lane; large, wav2vec2_large 16 x 20 s:
-M = 7992 and 15984), the four encoder-layer GEMMs and both paired tile widths
+M = 7992 and 15984), the four encoder-layer GEMMs and both tile widths
 (128, 256) plus the library's own choice ("auto"), it prints ms per launch (median of R repeats of N back-to-back
 launches, CUDA events) and algorithmic TFLOP/s (2 M N K over that time). The card name and power limit head the output:
 a time means nothing without them.
