@@ -265,6 +265,30 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
 }
 
+// ----------------------------------------------------------------------------------------------
+// thread-block clusters
+// ----------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_rank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// address of the same shared-memory location in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t peer_addr(const void* p, uint32_t rank) {
+    uint32_t out;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(out) : "r"(smem_u32(p)), "r"(rank));
+    return out;
+}
+// arrive on an mbarrier of any CTA of the cluster (a peer_addr address). The default .release.cta semantics: a
+// .cluster-scoped release compiles to a MEMBAR.ALL.GPU that waits for every outstanding store of the thread (the GEMM
+// epilogue's), and a consumer releasing a shared-memory stage that only wgmma read needs no such fence.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_cluster_addr) {
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar_cluster_addr) : "memory");
+}
+
 // generic-proxy writes to smem -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -282,6 +306,17 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
         "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
         ::"r"(smem_u32(smem_dst)),
         "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+        : "memory");
+}
+// the same box into the same shared-memory offset of every CTA of the cluster in `cta_mask`, each completing the
+// transaction bytes on its own mbarrier at `bar`'s offset
+__device__ __forceinline__ void tma_load_3d_multicast(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0,
+                                                      int c1, int c2, uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%3, %4, %5}], [%2], %6;"
+        ::"r"(smem_u32(smem_dst)),
+        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(cta_mask)
         : "memory");
 }
 
@@ -321,20 +356,36 @@ inline bool pdl_enabled() {
     return v != 0;
 }
 
+// cluster_x > 1: thread-block clusters of cluster_x CTAs along x (grid.x a multiple of it), in the same launch
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                              Args... args) {
+inline cudaError_t launch_pdl_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, int cluster_x,
+                                      cudaStream_t stream, Args... args) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid;
     cfg.blockDim = block;
     cfg.dynamicSmemBytes = smem;
     cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchAttribute attr[2];
+    int n = 0;
+    if (pdl_enabled()) {
+        attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attr[n].val.programmaticStreamSerializationAllowed = 1;
+        ++n;
+    }
+    if (cluster_x > 1) {
+        attr[n].id = cudaLaunchAttributeClusterDimension;
+        attr[n].val.clusterDim.x = (unsigned)cluster_x, attr[n].val.clusterDim.y = 1, attr[n].val.clusterDim.z = 1;
+        ++n;
+    }
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = n;
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
+}
+
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
+                              Args... args) {
+    return launch_pdl_cluster(kernel, grid, block, smem, 1, stream, args...);
 }
 
 // cudaFuncSetAttribute applies to the current device only: one "done" flag per device so that a process that

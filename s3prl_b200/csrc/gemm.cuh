@@ -11,7 +11,7 @@
 namespace s3b {
 
 struct GemmParams {
-    // A operand (activations): bf16 hi / lo, 3-D tensor maps (k, row, batch), box {64, 128, 1}, SWIZZLE_128B
+    // A operand (activations): bf16 hi / lo, 3-D tensor maps (k, row, batch), box {64, 128 / cluster_n, 1}, SWIZZLE_128B
     CUtensorMap a_hi, a_lo;
     // B operand (weights, [N][K] K-major): bf16 hi / lo, 3-D tensor maps (k, n, z), box {64, bn, 1}
     CUtensorMap b_hi, b_lo;
@@ -30,6 +30,10 @@ struct GemmParams {
     int n_tiles;            // output column tiles
     int bn;                 // columns per tile, the kernel's BN (multiple of 16 <= 256, or 80 / 120: pos_conv groups)
     int num_k_blocks;       // k-blocks per output tile
+    // 128-wide tiles: CTAs per thread-block cluster along N (0 or 1: no cluster, 2, 4; divides n_tiles). The CTAs of
+    // a cluster take adjacent column tiles of the same rows, and each loads 128 / cluster_n rows of every A box for
+    // all of them (TMA multicast): the A tensor maps then have box height 128 / cluster_n.
+    int cluster_n;
     // k-block kb reads   A box at (a_k_per_ntile*n_tile + (kb % kb_per_row)*64,
     //                              row0 + (kb / kb_per_row)*a_row_step + a_row_off, batch)
     //                    B box at (b_k_linear ? kb*64 : (kb % kb_per_row)*64, b_n_tiled ? n_tile*bn : 0,

@@ -17,6 +17,7 @@
 //   ping-pong (128-wide tiles), 384 threads: warpgroups 0 and 1 take alternate tiles, each a whole 128 x 128 tile
 //     (two m64n128 wgmmas per k-step, 128 accumulators); warp 8 of warpgroup 2 is the producer. One warpgroup's
 //     epilogue then overlaps the other's MMAs. setmaxnreg moves registers from the producer warpgroup to the consumers.
+//     It may run in clusters of CN = 2 or 4 CTAs along N that load each A box once between them (TMA multicast).
 // Both run the same k order and f16q8 pass order per output element, so the two widths agree bit for bit.
 #include <stdio.h>
 
@@ -55,19 +56,54 @@ enum EpiKind { kEpiF32 = 1, kEpiPlanes = 2, kEpiBoth = 3, kEpiQkv = 4 };
 __device__ __forceinline__ void setmaxnreg_dec40() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
 __device__ __forceinline__ void setmaxnreg_inc232() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
 
+// ===================== the persistent tile walk ======================================================================
+// CTAs walk cluster tiles: CN adjacent column tiles of one 128-row tile, one per CTA of a cluster of CN CTAs along x
+// (cluster c = blockIdx.x / CN, rank = blockIdx.x % CN). Every CTA of a cluster therefore runs the same number of
+// tiles with the same K, in lockstep. CN = 1 is the plain walk over tiles, CTA blockIdx.x taking tiles blockIdx.x,
+// blockIdx.x + gridDim.x, ...
+struct TileCoord {
+    int n_tile, batch, row0;
+};
+template <int CN>
+__device__ __forceinline__ TileCoord tile_coord(const GemmParams& p, int ctile, int rank) {
+    const int groups = p.n_tiles / CN;
+    const int mt = ctile / groups;
+    TileCoord c;
+    c.n_tile = (ctile - mt * groups) * CN + rank;
+    c.batch = mt / p.tiles_m_per_batch;
+    c.row0 = (mt - c.batch * p.tiles_m_per_batch) * kBlockM;
+    return c;
+}
+
+// One A box of a stage. CN > 1: this CTA loads rows [rank * 128 / CN, (rank + 1) * 128 / CN) of the box (the tensor
+// map's box height) into that slice of the plane, in every CTA of the cluster; its peers load the other slices.
+template <int CN, int RB>
+__device__ __forceinline__ void load_a(uint8_t* plane, const CUtensorMap* m, uint64_t* bar, int a_k, int a_row,
+                                       int batch, int rank) {
+    if constexpr (CN == 1) {
+        tma_load_3d(plane, m, bar, a_k, a_row, batch);
+    } else {
+        constexpr int kRows = kBlockM / CN;
+        tma_load_3d_multicast(plane + rank * kRows * RB, m, bar, a_k, a_row + rank * kRows, batch,
+                              (uint16_t)((1u << CN) - 1u));
+    }
+}
+
 // ===================== TMA producer: every tile of this CTA, kPasses * num_k_blocks stages each, in tile order ====
-template <int BN, int kScheme>
+// With CN > 1 a stage is refilled only once every CTA of the cluster has released it (empty_bar counts the consumer
+// warps of all of them): this CTA's A slice lands in the peers' stage too. Each full_bar still expects the whole stage,
+// its own W box plus the CN A slices.
+template <int BN, int kScheme, int CN>
 __device__ __forceinline__ void produce(const GemmParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar) {
     using Cfg = GemmCfg<BN, kScheme>;
     constexpr int kPasses = kScheme == 0 ? 1 : 2;
-    const int num_tiles = p.batches * p.tiles_m_per_batch * p.n_tiles;
+    const int rank = CN == 1 ? 0 : (int)cluster_rank();
+    const int num_ctiles = p.batches * p.tiles_m_per_batch * (p.n_tiles / CN);
     int stage = 0;
     uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int n_tile = tile % p.n_tiles;
-        const int mt = tile / p.n_tiles;
-        const int batch = mt / p.tiles_m_per_batch;
-        const int row0 = (mt - batch * p.tiles_m_per_batch) * kBlockM;
+    for (int ct = blockIdx.x / CN; ct < num_ctiles; ct += gridDim.x / CN) {
+        const TileCoord tc = tile_coord<CN>(p, ct, rank);
+        const int n_tile = tc.n_tile, batch = tc.batch, row0 = tc.row0;
         const int a_k0 = p.a_k_per_ntile * n_tile;
         const int b_n0 = p.b_n_tiled ? n_tile * BN : 0;
         const int b_z0 = n_tile * p.b_z_per_ntile;
@@ -85,7 +121,7 @@ __device__ __forceinline__ void produce(const GemmParams& p, uint8_t* smem, uint
                 const int b_z = p.b_k_linear ? 0 : b_z0 + kq;
                 if (kScheme == 1 && pass == 1) {
                     // [A16 | W16]: one fp16 box of 128-byte rows each, spanning both planes of the stage
-                    tma_load_3d(st, &p.a_hi, &full_bar[stage], a_k, a_row, batch);
+                    load_a<CN, 128>(st, &p.a_hi, &full_bar[stage], a_k, a_row, batch, rank);
                     tma_load_3d(sb, &p.b_hi, &full_bar[stage], b_k, b_n0, b_z);
                 } else {
                     // planes: scheme 0 [A_hi A_lo W_hi W_lo]; scheme 1 pass 0 [A_l8 A_h8 W_h8 W_l8] (64-byte rows)
@@ -93,8 +129,8 @@ __device__ __forceinline__ void produce(const GemmParams& p, uint8_t* smem, uint
                     const CUtensorMap* ma1 = kScheme == 0 ? &p.a_lo : &p.a_h8;
                     const CUtensorMap* mb0 = kScheme == 0 ? &p.b_hi : &p.b_h8;
                     const CUtensorMap* mb1 = kScheme == 0 ? &p.b_lo : &p.b_l8;
-                    tma_load_3d(st, ma0, &full_bar[stage], a_k, a_row, batch);
-                    tma_load_3d(st + Cfg::kAPlane, ma1, &full_bar[stage], a_k, a_row, batch);
+                    load_a<CN, Cfg::RB>(st, ma0, &full_bar[stage], a_k, a_row, batch, rank);
+                    load_a<CN, Cfg::RB>(st + Cfg::kAPlane, ma1, &full_bar[stage], a_k, a_row, batch, rank);
                     tma_load_3d(sb, mb0, &full_bar[stage], b_k, b_n0, b_z);
                     tma_load_3d(sb + Cfg::kBPlane, mb1, &full_bar[stage], b_k, b_n0, b_z);
                 }
@@ -102,13 +138,35 @@ __device__ __forceinline__ void produce(const GemmParams& p, uint8_t* smem, uint
             }
         }
     }
+    // CN > 1: the peers' consumers arrive on this CTA's empty barriers until they have consumed their last stage. The
+    // producer waits for every stage's last release, so that this CTA outlives those remote arrives. (Every peer
+    // multicast into this CTA has landed before its own consumers finish: they wait for whole stages.) A cluster
+    // barrier before exit would do the same, but it makes ptxas spill the consumers' registers.
+    if constexpr (CN > 1) {
+        for (int i = 0; i < Cfg::kStages; ++i) {
+            mbar_wait(&empty_bar[stage], phase ^ 1u);
+            if (++stage == Cfg::kStages) stage = 0, phase ^= 1u;
+        }
+    }
+}
+
+// Stage release by one consumer warp: CN > 1 arrives on the stage's empty barrier in every CTA of the cluster (lane r
+// on CTA r's), as each of them multicasts into this CTA's copy of the stage.
+template <int CN>
+__device__ __forceinline__ void release_stage(uint64_t* empty_bar, int lane) {
+    __syncwarp();
+    if constexpr (CN == 1) {
+        if (lane == 0) mbar_arrive(empty_bar);
+    } else {
+        if (lane < CN) mbar_arrive_cluster(peer_addr(empty_bar, (uint32_t)lane));
+    }
 }
 
 // ===================== MMAs of one tile: kHalves 64-row halves of A starting at half `half0`, acc[h] per half ======
 // Stage s is released (one arrive per warp of the warpgroup) once the wgmma group reading it has retired; one group
 // stays in flight so that the tensor pipe is fed while this warpgroup waits for the next stage. Every output element
 // sees the same wgmma sequence whichever kernel, warpgroup or half runs it.
-template <int BN, int kScheme, int kHalves>
+template <int BN, int kScheme, int kHalves, int CN>
 __device__ __forceinline__ void mma_tile(const GemmParams& p, uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
                                          int half0, int lane, int& stage, uint32_t& phase,
                                          float (&acc)[kHalves][BN / 2]) {
@@ -133,8 +191,7 @@ __device__ __forceinline__ void mma_tile(const GemmParams& p, uint8_t* smem, uin
             // the corrections carry 2^kQ8Scale: scale them back before the main product accumulates (exact)
             wgmma_wait<0>();
             if (pending >= 0) {
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&empty_bar[pending]);
+                release_stage<CN>(&empty_bar[pending], lane);
                 pending = -1;
             }
             const float s = 1.0f / (float)(1 << kQ8Scale);
@@ -197,19 +254,13 @@ __device__ __forceinline__ void mma_tile(const GemmParams& p, uint8_t* smem, uin
             }
             wgmma_commit();
             wgmma_wait<1>();
-            if (pending >= 0) {
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&empty_bar[pending]);
-            }
+            if (pending >= 0) release_stage<CN>(&empty_bar[pending], lane);
             pending = stage;
             if (++stage == kStages) stage = 0, phase ^= 1u;
         }
     }
     wgmma_wait<0>();
-    if (pending >= 0) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[pending]);
-    }
+    if (pending >= 0) release_stage<CN>(&empty_bar[pending], lane);
 }
 
 // two consecutive columns of one operand-plane format (the arithmetic of store_planes2)
@@ -428,7 +479,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
     pdl_launch_dependents();
 
     if (warp == 8) {
-        if (elect_one()) produce<BN, kScheme>(p, smem, full_bar, empty_bar);
+        if (elect_one()) produce<BN, kScheme, 1>(p, smem, full_bar, empty_bar);
         return;
     }
 
@@ -444,12 +495,13 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
         const int mt = tile / p.n_tiles;
         const int batch = mt / p.tiles_m_per_batch;
         const int row0 = (mt - batch * p.tiles_m_per_batch) * kBlockM;
-        mma_tile<BN, kScheme, 1>(p, smem, full_bar, empty_bar, wg, lane, stage, phase, acc);
+        mma_tile<BN, kScheme, 1, 1>(p, smem, full_bar, empty_bar, wg, lane, stage, phase, acc);
         epilogue_tile<BN, kEpi, 1>(p, acc, batch, row0 + wg * 64 + wq * 16 + (lane >> 2), n_tile * BN + 2 * (lane & 3));
     }
 }
 
-template <int kScheme, int kEpi>
+// CN: CTAs per cluster along N, which share every A box (tile_coord, load_a, release_stage); 1 = no cluster
+template <int kScheme, int kEpi, int CN>
 __global__ void __launch_bounds__(kPingPongThreads, 1) gemm_sm90_pingpong_kernel(const __grid_constant__ GemmParams p) {
     constexpr int BN = 128;
     using Cfg = GemmCfg<BN, kScheme>;
@@ -473,19 +525,22 @@ __global__ void __launch_bounds__(kPingPongThreads, 1) gemm_sm90_pingpong_kernel
         }
         for (int s = 0; s < kStages; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 4);  // each stage is consumed by ONE warpgroup: one arrive per warp
+            // each stage is consumed by ONE warpgroup of each CTA of the cluster: one arrive per warp
+            mbar_init(&empty_bar[s], 4 * CN);
         }
         mbar_init(&order_bar[0], 4);
         mbar_init(&order_bar[1], 4);
         fence_mbar_init();
     }
-    __syncthreads();
+    // CN > 1: no peer multicasts into this CTA's ring or arrives on its barriers before they are initialised
+    if constexpr (CN == 1) __syncthreads();
+    else cluster_sync();
     pdl_wait();
     pdl_launch_dependents();
 
     if (warp >= 8) {
         setmaxnreg_dec40();
-        if (warp == 8 && elect_one()) produce<BN, kScheme>(p, smem, full_bar, empty_bar);
+        if (warp == 8 && elect_one()) produce<BN, kScheme, CN>(p, smem, full_bar, empty_bar);
         return;
     }
     setmaxnreg_inc232();
@@ -497,51 +552,95 @@ __global__ void __launch_bounds__(kPingPongThreads, 1) gemm_sm90_pingpong_kernel
     // on a stage two ring laps ahead would see the parity of the earlier phase and read a stage not yet loaded.
     const int wg = warp >> 2;
     const int wq = warp & 3;
-    const int num_tiles = p.batches * p.tiles_m_per_batch * p.n_tiles;
+    const int num_ctiles = p.batches * p.tiles_m_per_batch * (p.n_tiles / CN);
     const int stages_per_tile = kPasses * p.num_k_blocks;
     float acc[2][BN / 2];
     int j = 0;  // tiles this warpgroup has done
-    for (int tile = blockIdx.x + wg * gridDim.x, ord = wg; tile < num_tiles; tile += 2 * gridDim.x, ord += 2, ++j) {
+    for (int ct = (int)(blockIdx.x + wg * gridDim.x) / CN, ord = wg; ct < num_ctiles;
+         ct += 2 * (int)gridDim.x / CN, ord += 2, ++j) {
         // the producer fills the ring in tile order: tile ordinal `ord` starts at ring position ord * stages_per_tile
         const int g = ord * stages_per_tile;
         int stage = g % kStages;
         uint32_t phase = (uint32_t)(g / kStages) & 1u;
-        const int n_tile = tile % p.n_tiles;
-        const int mt = tile / p.n_tiles;
-        const int batch = mt / p.tiles_m_per_batch;
-        const int row0 = (mt - batch * p.tiles_m_per_batch) * kBlockM;
         if (ord > 0) mbar_wait(&order_bar[wg], (uint32_t)(j - (wg == 0 ? 1 : 0)) & 1u);
-        mma_tile<BN, kScheme, 2>(p, smem, full_bar, empty_bar, 0, lane, stage, phase, acc);
+        mma_tile<BN, kScheme, 2, CN>(p, smem, full_bar, empty_bar, 0, lane, stage, phase, acc);
         __syncwarp();
         if (lane == 0) mbar_arrive(&order_bar[wg ^ 1]);
-        epilogue_tile<BN, kEpi, 2>(p, acc, batch, row0 + wq * 16 + (lane >> 2), n_tile * BN + 2 * (lane & 3));
+        const TileCoord tc = tile_coord<CN>(p, ct, CN == 1 ? 0 : (int)cluster_rank());
+        epilogue_tile<BN, kEpi, 2>(p, acc, tc.batch, tc.row0 + wq * 16 + (lane >> 2), tc.n_tile * BN + 2 * (lane & 3));
     }
 }
 
+// Per device and kernel instantiation: the shared-memory attribute is set, and how many clusters of it can be resident
+// at once (cudaOccupancyMaxActiveClusters; not every GPC holds a whole number of clusters of one-CTA-per-SM CTAs)
+struct PersistentLaunch {
+    bool attr_set[64] = {};
+    int max_clusters[64] = {};
+};
+
+// One CTA per SM (cn = 1), or cn x as many clusters as fit at once, capped by the clusters of tiles there are
 template <typename Kernel>
-static cudaError_t launch_persistent(Kernel kernel, PerDeviceOnce& attr_once, int threads, int smem_bytes,
+static cudaError_t launch_persistent(Kernel kernel, PersistentLaunch& state, int threads, int smem_bytes, int cn,
                                      const GemmParams& p, int sm_count, cudaStream_t stream) {
-    bool& attr_set = attr_once.current();
-    if (!attr_set) {
-        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
+    int dev = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    dev &= 63;
+    if (!state.attr_set[dev]) {
+        e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
         if (e != cudaSuccess) return e;
-        attr_set = true;
+        state.attr_set[dev] = true;
     }
-    const int num_tiles = p.batches * p.tiles_m_per_batch * p.n_tiles;
-    if (num_tiles <= 0) return cudaSuccess;
-    const int grid = num_tiles < sm_count ? num_tiles : sm_count;
-    return launch_pdl(kernel, dim3(grid), dim3(threads), smem_bytes, stream, p);
+    const int num_ctiles = p.batches * p.tiles_m_per_batch * (p.n_tiles / cn);
+    if (num_ctiles <= 0) return cudaSuccess;
+    int clusters = sm_count;
+    if (cn > 1) {
+        if (state.max_clusters[dev] == 0) {
+            cudaLaunchConfig_t cfg = {};
+            cfg.gridDim = dim3(cn * (sm_count / cn));
+            cfg.blockDim = dim3(threads);
+            cfg.dynamicSmemBytes = smem_bytes;
+            cudaLaunchAttribute attr;
+            attr.id = cudaLaunchAttributeClusterDimension;
+            attr.val.clusterDim.x = (unsigned)cn, attr.val.clusterDim.y = 1, attr.val.clusterDim.z = 1;
+            cfg.attrs = &attr;
+            cfg.numAttrs = 1;
+            e = cudaOccupancyMaxActiveClusters(&state.max_clusters[dev], kernel, &cfg);
+            if (e != cudaSuccess) return e;
+            if (state.max_clusters[dev] <= 0) return cudaErrorInvalidConfiguration;
+        }
+        clusters = state.max_clusters[dev];
+    }
+    const int grid = cn * (num_ctiles < clusters ? num_ctiles : clusters);
+    return launch_pdl_cluster(kernel, dim3(grid), dim3(threads), smem_bytes, cn, stream, p);
 }
 
 template <int BN, int kScheme, int kEpi>
 static cudaError_t launch_impl(const GemmParams& p, int sm_count, cudaStream_t stream) {
-    static PerDeviceOnce attr_once;
-    if constexpr (BN == 128)
-        return launch_persistent(gemm_sm90_pingpong_kernel<kScheme, kEpi>, attr_once, kPingPongThreads,
-                                 GemmCfg<BN, kScheme>::kSmemBytes, p, sm_count, stream);
-    else
-        return launch_persistent(gemm_sm90_kernel<BN, kScheme, kEpi>, attr_once, kThreads,
-                                 GemmCfg<BN, kScheme>::kSmemBytes, p, sm_count, stream);
+    constexpr int kSmem = GemmCfg<BN, kScheme>::kSmemBytes;
+    if constexpr (BN == 128) {
+        static PersistentLaunch state[3];
+        switch (p.cluster_n) {
+            case 0:
+            case 1:
+                return launch_persistent(gemm_sm90_pingpong_kernel<kScheme, kEpi, 1>, state[0], kPingPongThreads,
+                                         kSmem, 1, p, sm_count, stream);
+            case 2:
+                if (p.n_tiles % 2 != 0) return cudaErrorInvalidValue;
+                return launch_persistent(gemm_sm90_pingpong_kernel<kScheme, kEpi, 2>, state[1], kPingPongThreads,
+                                         kSmem, 2, p, sm_count, stream);
+            case 4:
+                if (p.n_tiles % 4 != 0) return cudaErrorInvalidValue;
+                return launch_persistent(gemm_sm90_pingpong_kernel<kScheme, kEpi, 4>, state[2], kPingPongThreads,
+                                         kSmem, 4, p, sm_count, stream);
+            default:
+                return cudaErrorInvalidValue;
+        }
+    } else {
+        static PersistentLaunch state;
+        if (p.cluster_n > 1) return cudaErrorInvalidValue;
+        return launch_persistent(gemm_sm90_kernel<BN, kScheme, kEpi>, state, kThreads, kSmem, 1, p, sm_count, stream);
+    }
 }
 
 // QKV scatter and the fp32 + planes output run at the widths of the encoder's linears only (>= 128 columns)

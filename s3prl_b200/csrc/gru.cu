@@ -42,20 +42,6 @@ struct GruSmem {
 // one CTA per SM with the opt-in maximum of dynamic shared memory (227 KB on sm_90)
 static_assert(sizeof(GruSmem) <= 227 * 1024, "the recurrence kernel's shared memory exceeds 227 KB");
 
-__device__ __forceinline__ uint32_t cluster_rank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// address of the same shared-memory location in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t peer_addr(const void* p, uint32_t rank) {
-    uint32_t out;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(out) : "r"(smem_u32(p)), "r"(rank));
-    return out;
-}
 __device__ __forceinline__ void st_cluster_f4(uint32_t addr, float4 v) {
     asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z),
                  "f"(v.w)

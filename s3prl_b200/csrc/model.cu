@@ -977,7 +977,7 @@ static void set_qkv_epi(GemmParams& p, const float* bias, int T, int H, int hd, 
     p.vt_hi = vt.h(), p.vt_lo = vt.l();
 }
 
-// Tile width for a flat [M][N] linear layer. Both widths give bit-identical results; the rule comes from
+// Tile width for a flat [M][N] linear layer. Both widths give bit-identical results. The rule comes from
 // tools/gemm_shapes.py on an H100 80GB HBM3 at 400 W, at the encoder shapes of hubert_base (K = 768, 3072) and
 // wav2vec2_large (K = 1024, 4096), M = 7984..15984, with the ping-pong kernel at 128 columns:
 //  - bf16x3: 128 columns, 1.4x-2.2x faster than 256 at every measured shape.
@@ -988,6 +988,10 @@ static void set_qkv_epi(GemmParams& p, const float* bias, int T, int H, int hd, 
 //    fc2 at M = 7984: 189 tiles of 256 on 132 SMs). The K >= 2048 cut lies between measured Ks (1024 and 3072).
 // The epilogue kind does not enter the rule: at K <= 1024 the GELU (fc1) and fp32 epilogues ranked the two widths the
 // same way, but for the one shape above.
+// Since f16q8's 128-wide tiles run in clusters of 2 (pick_cluster_n), hubert_base's shapes were re-measured (H100
+// 80GB HBM3, 700 W) and the rule still holds there: at K = 768, 128 columns are 1.15x-1.65x faster than 256 (QKV,
+// out_proj, fc1); fc2 at M = 7984 takes 128 columns, now 10% faster than 256 (0.146 against 0.161 ms), and at
+// M = 15968 the two tie (256 columns 0.281 ms, 128 columns 0.282). wav2vec2_large's shapes were not re-measured.
 // An N that is not a multiple of 128 takes the widest of 192, 64, 32 and 16 that divides it. forced != 0 (the tile
 // width s3b_linear_ex or s3b_gemm_bench asks for) is taken wherever it divides N.
 static int pick_bn(int64_t M, int N, int K, int scheme, int sm_count, int forced) {
@@ -998,6 +1002,23 @@ static int pick_bn(int64_t M, int N, int K, int scheme, int sm_count, int forced
     const int64_t tiles = (M + 127) / 128 * (N / 256);
     const int64_t last = tiles % sms;
     return (last == 0 || last >= sms / 2) ? 256 : 128;
+}
+
+// CTAs per cluster along N for a launch of n_tiles tiles of bn columns: 128-wide tiles take `preferred` (1, 2 or 4)
+// where it divides n_tiles, every other width 1. The CTAs of a cluster load each A tile once between them (TMA
+// multicast), which cuts the L2 -> SM operand traffic per tile. Results are bit-identical whatever the size.
+// f16q8 linears prefer 2: tools/gemm_shapes.py --k-sweep (H100 80GB HBM3, 700 W; M = 7984, N = 2304) cuts the
+// per-K cost of a round of 128-wide tiles from 18.2 to 14.5 ns and leaves the fixed cost at 2-3 us, and
+// hubert_base's QKV, out_proj, fc1 and fc2 run 8-18% faster (4 helps fc1 by another 1%, the only one it divides).
+// bf16x3 prefers 1: its per-K cost does not drop (15.8 ns, 16.3 in clusters of 2), and three of its four
+// encoder linears run 2-3% slower in clusters of 2.
+// S3B_GEMM_CLUSTER=1 / 2 / 4 replaces `preferred` at every call: 1 turns clusters off, for A/B runs of one build.
+static int pick_cluster_n(int bn, int n_tiles, int preferred) {
+    if (const char* e = getenv("S3B_GEMM_CLUSTER")) {
+        const int v = atoi(e);
+        if (v == 1 || v == 2 || v == 4) preferred = v;
+    }
+    return bn == 128 && n_tiles % preferred == 0 ? preferred : 1;
 }
 
 #define TMAP_OK(expr)                                                                     \
@@ -1016,25 +1037,27 @@ static int linear_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, in
     if (lda == 0) lda = K;
     if (K % 64 != 0 || N % 16 != 0) return fail("linear: K %% 64 or N %% 16 violated (N=%d K=%d)", N, K);
     const int bn = pick_bn(M, N, K, scheme, g_sm_count, forced_bn);
+    const int cn = pick_cluster_n(bn, N / bn, scheme != 0 ? 2 : 1);
+    const uint32_t a_box = 128 / cn;
     if (scheme != 0) {
         if ((bn != 128 && bn != 256) || K % 128 != 0)
             return fail("f16q8 GEMM needs a tile width of 128 or 256 and K %% 128 == 0 (N=%d K=%d)", N, K);
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, 128));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, 128));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, 128));
+        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, a_box));
+        TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, a_box));
+        TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, a_box));
         TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, (uint64_t)N * K, 64, bn));
         TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, N, 1, K, (uint64_t)N * K, 64, bn));
         TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, N, 1, K, (uint64_t)N * K, 64, bn));
         p.scheme = 1;
     } else {
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, 128));
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, 128));
+        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, a_box));
+        TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, a_box));
         TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, (uint64_t)N * K, 64, bn));
         TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, W.l(), K, N, 1, K, (uint64_t)N * K, 64, bn));
     }
     p.num_k_blocks = K / 64, p.kb_per_row = K / 64;
     p.batches = 1, p.rows_per_batch = (int)M, p.tiles_m_per_batch = (int)((M + 127) / 128);
-    p.n_tiles = N / bn, p.bn = bn;
+    p.n_tiles = N / bn, p.bn = bn, p.cluster_n = cn;
     p.a_row_step = 0, p.a_row_off = 0, p.a_k_per_ntile = 0, p.b_n_tiled = 1, p.b_z_per_ntile = 0;
     p.out_rows_per_batch = (int)M;
     p.alg_flops = 2.0 * (double)M * N * K;
@@ -1048,28 +1071,32 @@ static int conv_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int 
     memset(&p, 0, sizeof(p));
     const int C = kConvDim, K = kw * C;
     const uint64_t rows = (uint64_t)((Lin + 1) / 2);
-    // Tile width: tools/gemm_shapes.py times the linear with conv i's M, N = 512 and K as a proxy (H100 80GB HBM3,
-    // 400 W, both models' conv stacks): f16q8 256 columns are 4-20% faster than 128 at every conv, bf16x3 128 columns
-    // 25-40% faster than 256.
-    const int bn = scheme != 0 ? 256 : 128;
+    // Tile: tools/gemm_shapes.py times the linear with conv i's M, N = 512 and K as a proxy (H100 80GB HBM3, 700 W,
+    // hubert_base's conv stack at 32 x 10 s). f16q8 on 128-wide tiles in clusters of 4 (N = 512 is four tiles, which
+    // then share each A tile) runs conv 1..6 in 6.96 ms, against 7.57 in clusters of 2, 7.97 on 256-wide tiles
+    // (10-13% slower at every conv) and 9.49 on unclustered 128-wide tiles. bf16x3 stays on unclustered 128-wide
+    // tiles: clusters of 2 and 4 are 2% and 10% slower there, and 256-wide tiles 70%.
+    const int bn = 128;
+    const int cn = pick_cluster_n(bn, C / bn, scheme != 0 ? 4 : 1);
+    const uint32_t a_box = 128 / cn;
     // weights [512][K], K index = tap*512 + channel, read linearly along K
     if (scheme != 0) {
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
+        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, a_box));
+        TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, a_box));
+        TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, a_box));
         TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, C, 1, K, (uint64_t)C * K, 64, bn));
         TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, C, 1, K, (uint64_t)C * K, 64, bn));
         TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, C, 1, K, (uint64_t)C * K, 64, bn));
         p.scheme = 1;
     } else {
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, 128));
+        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, a_box));
+        TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, a_box));
         TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, C, 1, K, (uint64_t)C * K, 64, bn));
         TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, W.l(), K, C, 1, K, (uint64_t)C * K, 64, bn));
     }
     p.num_k_blocks = K / 64, p.kb_per_row = (2 * C) / 64;
     p.batches = B, p.rows_per_batch = (int)Lout, p.tiles_m_per_batch = (int)((Lout + 127) / 128);
-    p.n_tiles = C / bn, p.bn = bn;
+    p.n_tiles = C / bn, p.bn = bn, p.cluster_n = cn;
     p.a_row_step = 1, p.a_row_off = 0, p.a_k_per_ntile = 0, p.b_n_tiled = 1, p.b_z_per_ntile = 0, p.b_k_linear = 1;
     p.out_rows_per_batch = (int)Lout;
     p.alg_flops = 2.0 * (double)B * Lout * C * K;
