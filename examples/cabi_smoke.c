@@ -32,6 +32,7 @@ int main(void) {
         (const void*)s3b_fbank_ex,       (const void*)s3b_melspec_ex,     (const void*)s3b_decoar2_features_f32,
         (const void*)s3b_apc_model_create, (const void*)s3b_profile_read_ex, (const void*)s3b_apc_features_f32,
         (const void*)s3b_gru_f32,        (const void*)s3b_gru_max_active_clusters,
+        (const void*)s3b_decoar_model_create, (const void*)s3b_lstm_f32, (const void*)s3b_lstm_fits,
     };
     s3b_config cfg;
     int64_t lens[2] = {16000, 800};
@@ -75,6 +76,26 @@ int main(void) {
         printf("APC frames of (16000, 800) samples: %d %d\n", (int)valid[0], (int)valid[1]);
         s3b_model_destroy(m);
         if (valid[0] != 98 || valid[1] != 3) return 7;
+    }
+    {
+        /* DeCoAR: the APC frame rule; decoar outputs the last layer, decoar_layers all four */
+        s3b_decoar_config dcfg;
+        int32_t all;
+        for (all = 0; all < 2; ++all) {
+            s3b_model* m = NULL;
+            memset(&dcfg, 0, sizeof(dcfg));
+            dcfg.struct_size = (int32_t)sizeof(dcfg), dcfg.num_layers = 4, dcfg.hidden = 1024, dcfg.all_layers = all;
+            if (s3b_decoar_model_create(&dcfg, &m) != 0) {
+                printf("s3b_decoar_model_create: %s\n", s3b_last_error());
+                return 8;
+            }
+            if (s3b_valid_frames(m, lens, 2, 16000, valid) != 0 || s3b_num_outputs(m) != (all ? 4 : 1)) {
+                printf("DeCoAR bookkeeping: %s\n", s3b_last_error());
+                return 9;
+            }
+            s3b_model_destroy(m);
+            if (valid[0] != 98 || valid[1] != 3) return 10;
+        }
     }
     return 0;
 }

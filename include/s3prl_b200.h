@@ -94,6 +94,29 @@ typedef struct s3b_apc_config {
     int32_t reserved[4]; /* 0 */
 } s3b_apc_config;
 int s3b_apc_model_create(const s3b_apc_config* cfg, s3b_model** out);
+
+/* DeCoAR (s3prl/upstream/decoar/{expert,decoar,audio}.py, decoar_layers/{expert,decoar}.py). The APC front end
+ * (kaldi fbank, 80 bins, hamming window, CMVN over all m frames with the unbiased std, pad_sequence to T = max m),
+ * post_extract_proj = Linear(80, 1024), then two 4-layer nn.LSTM(1024, 1024) stacks (gate order i, f, g, o; h_0 =
+ * c_0 = 0) over the packed sequences: forward_lstm in time order, backward_lstm over each utterance reversed within
+ * its own length. Layer k's output is cat(forward, backward) [batch][T][2048]; frames t >= m_b are exactly 0.
+ * Tensors (s3b_model_set_tensor, reference key names): post_extract_proj.{weight [1024][80], bias},
+ * {forward,backward}_lstm.{weight_ih_l{k} [4096][1024], weight_hh_l{k} [4096][1024], bias_ih_l{k}, bias_hh_l{k}},
+ * k = 0..3; other keys are ignored. s3b_num_outputs = 1 (all_layers 0, `decoar`: the last layer) or 4 (all_layers 1,
+ * `decoar_layers`: every layer); hidden_out is [num_outputs][batch][T][2048]. The model works with the calls listed
+ * for APC; s3b_forward_ex refuses ffn_out and last_residual. The recurrence is grid-resident: one cooperative launch
+ * of 128 CTAs, one per SM, with 212.5 KiB of shared memory each (s3b_lstm_fits). So finalize fails on a device with
+ * fewer than 128 SMs or less opt-in shared memory, and a forward always runs as one lane (s3b_default_lanes is 1 and
+ * lanes = 2 runs as one): two such launches must never be in flight at once, so do not run two DeCoAR forwards
+ * concurrently on one device. */
+typedef struct s3b_decoar_config {
+    int32_t struct_size; /* sizeof(s3b_decoar_config) */
+    int32_t num_layers;  /* 4 */
+    int32_t hidden;      /* 1024 */
+    int32_t all_layers;  /* 0 = decoar, 1 = decoar_layers */
+    int32_t reserved[4]; /* 0 */
+} s3b_decoar_config;
+int s3b_decoar_model_create(const s3b_decoar_config* cfg, s3b_model** out);
 int s3b_model_finalize(s3b_model* m);
 void s3b_model_destroy(s3b_model* m);
 
@@ -172,8 +195,9 @@ int s3b_wavlm_buckets(int32_t num_buckets, int32_t max_distance, const int32_t* 
  * s3b_forward is bracketed by CUDA events on the launching stream; s3b_profile_read synchronises the device and
  * returns, per category, accumulated device milliseconds, ALGORITHMIC flops (2*M*N*K of the un-padded
  * contraction; 4*T^2*D per utterance and layer for attention) and kernel launches. Arrays have 5 entries.
- * s3b_profile_read_ex reads the first num_categories (1..6) categories; category 5 is APC's GRU recurrence kernel
- * (flops: 6*H*H per frame of the padded batch). reset clears all six. */
+ * s3b_profile_read_ex reads the first num_categories (1..6) categories; category 5 is the recurrence kernels: APC's GRU
+ * (flops: 6*H*H per frame of the padded batch) and DeCoAR's LSTM (8*H*H per frame of the padded batch and direction).
+ * reset clears all six. */
 int s3b_profile_enable(s3b_model* m, int32_t enable);
 int s3b_profile_read(s3b_model* m, double* ms, double* flops, int64_t* launches, int32_t reset);
 int s3b_profile_read_ex(s3b_model* m, int32_t num_categories, double* ms, double* flops, int64_t* launches,
@@ -382,6 +406,17 @@ int s3b_apc_features_f32(const float* const* wavs, const int64_t* lens, int32_t 
 int s3b_gru_max_active_clusters(int32_t* out);
 int s3b_gru_f32(const float* xg, const float* whh, const float* bhh, const float* residual, const int32_t* lens,
                 int32_t batch, int32_t t, int32_t hidden, int32_t out_fmt, float* out, float* planes_out, void* stream);
+/* 1 in *out when the current device can host DeCoAR's LSTM recurrence grid (128 co-resident CTAs, one per SM, with
+ * their shared memory; cooperative launch), else 0. */
+int s3b_lstm_fits(int32_t* out);
+/* One DeCoAR LSTM layer and direction as a forward runs it (the model's kernel, H = 1024): xg [batch][t][4H] DEVICE =
+ * W_ih x + b_ih (gate order i, f, g, o), whh [4H][H] DEVICE (weight_hh_l{k}), optional bhh [4H] DEVICE added to xg
+ * (the model folds it into its GEMM bias), lens HOST [batch] valid frames in [0, t]. direction 0 runs frames 0 ..
+ * lens[b] - 1, direction 1 runs them backwards. out [batch][t][2H] DEVICE: the kernel writes columns [direction * H,
+ * direction * H + H) only: h of frame t for t < lens[b], 0 beyond. out_fmt -1 = no operand planes; 0 / 1 = the planes
+ * the model feeds the next layer's GEMM (bf16 hi/lo or f16q8), decoded to planes_out [batch][t][2H] (same columns). */
+int s3b_lstm_f32(const float* xg, const float* whh, const float* bhh, const int32_t* lens, int32_t batch, int32_t t,
+                 int32_t direction, int32_t out_fmt, float* out, float* planes_out, void* stream);
 /* The Conformer convolution module between its pointwise convs, as a forward runs it (wav2vec2_model.py:383-389):
  * x [batch][t][2d] (pointwise_conv1 output, channels-last) -> GLU (x[..., :d] * sigmoid(x[..., d:])) -> depthwise
  * Conv1d(k, padding k / 2, groups d, no bias; dw_w [d][1][k]) over each utterance's t frames -> BatchNorm1d (eval, eps

@@ -82,6 +82,32 @@ size_t gru_smem_bytes();
 // GEMM epilogue, for the building-block entry point
 cudaError_t launch_gru_fold_bias(float* xg, const float* bhh, size_t rows, cudaStream_t s);
 
+// ---- lstm.cu: the LSTM recurrence of DeCoAR (grid-resident W_hh) --------------------------------------------------
+static constexpr int kLstmHidden = 1024;    // hidden size the kernel is built for
+static constexpr int kLstmGroup = 16;       // utterances staged per group-step
+static constexpr int kLstmCtas = 128;       // CTAs of the cooperative grid (one per SM), 8 hidden units each
+static constexpr int kLstmMaxBatch = 512;   // utterances per launch; launch_lstm splits larger batches
+struct LstmParams {
+    const float* xg;    // [B][T][4H]: W_ih x + b_ih (+ b_hh), gate order i, f, g, o
+    const float* whh;   // [4H][H] weight_hh_l{k}
+    const float* bhh;   // optional [4H], added to xg (null when the GEMM bias already holds it)
+    const int* len;     // [B] valid frames; frames t >= len[b] are written as zero
+    const int* order;   // [B] utterance indices, longest first
+    int B, T;
+    int direction;      // 0: t = 0 .. len - 1; 1: t = len - 1 .. 0 (outputs stay in natural time)
+    float* out;         // optional [B][T][ldo] fp32 layer output, columns col0 .. col0 + H - 1
+    int ldo, col0;
+    OutPlanes op;       // optional operand planes of the same values, same layout (op.hi null: none)
+    float* hbuf;        // [2][min(B, kLstmMaxBatch)][H] state exchange buffer (lstm_hbuf_floats)
+    unsigned int* counter;  // grid-barrier counter, zeroed on the stream before every launch
+};
+cudaError_t launch_lstm(const LstmParams& p, cudaStream_t s);
+size_t lstm_hbuf_floats(int B);
+size_t lstm_smem_bytes();
+// ok = 1 when the device can host the grid: >= kLstmCtas SMs, enough opt-in shared memory, cooperative launch and one
+// CTA per SM; sms / smem_optin report the device's values for messages
+cudaError_t lstm_fits(int* ok, int* sms, int* smem_optin);
+
 // ---- peer.cu: fused weighted sum + push all-gather over peer memory --------------------------------------------------
 cudaError_t launch_weighted_sum_push(const float* hs, int NL, size_t n_per_layer, size_t layer_stride, const float* w,
                                      float* const* peer_dst, uint32_t* const* peer_flag, int n_peers, uint32_t seq,

@@ -145,12 +145,14 @@ struct LayerW {
     DevBuf ffn1_b1, ffn1_b2, ffn1_ln_g, ffn1_ln_b, ffn2_ln_g, ffn2_ln_b, conv_ln_g, conv_ln_b, dw_w, dw_b;
     // APC GRU layer: wih = weight_ih_l0 [3H][K] (layer 0: K = 80 zero-padded to kDecoar2K), gru_b = bias_ih_l0 with
     // bias_hh_l0's r and z thirds added (the input GEMM's bias), whh = weight_hh_l0 [3H][H] fp32, bhn = bias_hh_l0[2H:]
+    // DeCoAR LSTM layer k, direction d (layers[2k + d]): wih = weight_ih_lk [4H][H], gru_b = bias_ih_lk + bias_hh_lk,
+    // whh = weight_hh_lk [4H][H] fp32
     SplitBuf wih;
     DevBuf gru_b, whh, bhn;
 };
 
 // per-category device-time profile (CUDA events around each launch on the launching stream)
-// CAT_GRU (APC's recurrence) is read through s3b_profile_read_ex only: s3b_profile_read fills five entries
+// CAT_GRU (the GRU / LSTM recurrences) is read through s3b_profile_read_ex only: s3b_profile_read fills five entries
 enum { CAT_GEMM = 0, CAT_ATTN = 1, CAT_CONV0 = 2, CAT_NORM = 3, CAT_MISC = 4, CAT_GRU = 5, CAT_COUNT = 6 };
 struct ProfRec {
     int cat;
@@ -191,7 +193,8 @@ struct Workspace {
     DevBuf wav_stats, wav_pad, c0_part, c0_ss, conv_f32, tmp_f32, x_f32, x1_f32, gate, pos_z, hs0;
     DevBuf glu_f32;  // Conformer: pointwise_conv1 output [M][2D]
     DevBuf fb_f32;   // DeCoAR 2.0 / APC: log-mel frames [B][m(Lmax)][80]
-    DevBuf xg_f32;   // APC: the input GEMM's output [M][3H]
+    DevBuf xg_f32;   // APC / DeCoAR: the input GEMM's output [M][3H] / [M][4H]
+    DevBuf lstm_h, lstm_sync;  // DeCoAR: the recurrence's state exchange buffer and grid-barrier counter
     SplitBuf act[kNumConv], ln512_s, x_s, xs_s, q_s, k_s, vt_s, ctx_s, x1_s, h_s;
     cudaStream_t stream = nullptr;  // lane stream (lane 1; lane 0 runs on the caller's stream)
     cudaEvent_t done = nullptr;
@@ -204,6 +207,9 @@ struct s3b_model {
     // APC / VQ-APC (s3b_apc_model_create): cfg then holds num_layers and embed_dim = hidden, everything else zero
     bool apc = false;
     int apc_residual = 0;
+    // DeCoAR (s3b_decoar_model_create): cfg holds num_layers and embed_dim = 2 H (the forward | backward concat)
+    bool decoar_lstm = false;
+    int decoar_all_layers = 0;  // 1: decoar_layers (every layer's output), 0: decoar (the last one)
     std::map<std::string, HostTensor> host;
     bool finalized = false;
     int sm_count = 132;
@@ -311,9 +317,12 @@ static int64_t decoar2_frames(int64_t L) { return L < 400 ? 0 : (1 + (L - 400) /
 static int64_t fbank_frames(int64_t L) { return L < 400 ? 0 : 1 + (L - 400) / 160; }
 static bool decoar2(const s3b_model* m) { return m != nullptr && m->cfg.frontend == 1; }
 static bool apc(const s3b_model* m) { return m != nullptr && m->apc; }
+static bool decoar1(const s3b_model* m) { return m != nullptr && m->decoar_lstm; }
+// the recurrent upstreams: every fbank frame kept (APC's front end)
+static bool fbank_all_frames(const s3b_model* m) { return apc(m) || decoar1(m); }
 // frames of a batch padded to L for this model's front end (m NULL: the conv stack)
 static int64_t model_frames(const s3b_model* m, int64_t L) {
-    return apc(m) ? fbank_frames(L) : decoar2(m) ? decoar2_frames(L) : num_frames(L);
+    return fbank_all_frames(m) ? fbank_frames(L) : decoar2(m) ? decoar2_frames(L) : num_frames(L);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -418,6 +427,26 @@ extern "C" int s3b_apc_model_create(const s3b_apc_config* cfg, s3b_model** out) 
     memset(&m->cfg, 0, sizeof(m->cfg));
     m->cfg.num_layers = cfg->num_layers, m->cfg.embed_dim = cfg->hidden;
     m->apc = true, m->apc_residual = cfg->residual;
+    m->scheme = default_scheme();
+    *out = m;
+    return 0;
+}
+
+extern "C" int s3b_decoar_model_create(const s3b_decoar_config* cfg, s3b_model** out) {
+    if (!cfg || !out) return fail("null argument");
+    if (cfg->struct_size != (int32_t)sizeof(s3b_decoar_config))
+        return fail("s3b_decoar_config.struct_size %d != %d (header / library mismatch)", cfg->struct_size,
+                    (int)sizeof(s3b_decoar_config));
+    if (cfg->num_layers != 4) return fail("num_layers %d: DeCoAR is served with 4 LSTM layers", cfg->num_layers);
+    if (cfg->hidden != kLstmHidden)
+        return fail("hidden %d: DeCoAR is served with hidden size %d", cfg->hidden, kLstmHidden);
+    if (cfg->all_layers != 0 && cfg->all_layers != 1) return fail("all_layers must be 0 or 1, not %d", cfg->all_layers);
+    for (int i = 0; i < 4; ++i)
+        if (cfg->reserved[i] != 0) return fail("s3b_decoar_config.reserved[%d] must be 0", i);
+    s3b_model* m = new s3b_model();
+    memset(&m->cfg, 0, sizeof(m->cfg));
+    m->cfg.num_layers = cfg->num_layers, m->cfg.embed_dim = 2 * cfg->hidden;
+    m->decoar_lstm = true, m->decoar_all_layers = cfg->all_layers;
     m->scheme = default_scheme();
     *out = m;
     return 0;
@@ -677,6 +706,49 @@ static int finalize_apc(s3b_model* m) {
     return 0;
 }
 
+// DeCoAR (decoar.py): post_extract_proj = Linear(80, 1024), then {forward,backward}_lstm = nn.LSTM(1024, 1024,
+// num_layers=4). The recurrence kernel needs the whole device: kLstmCtas co-resident CTAs, one per SM.
+static int finalize_decoar(s3b_model* m) {
+    const int NL = m->cfg.num_layers, H = kLstmHidden;
+    const HostTensor* t;
+    S3B_OK(need(m, "post_extract_proj.weight", {H, 80}, &t));
+    std::vector<float> wp((size_t)H * kDecoar2K, 0.f);
+    for (int o = 0; o < H; ++o) memcpy(&wp[(size_t)o * kDecoar2K], &t->data[(size_t)o * 80], 80 * sizeof(float));
+    S3B_OK(upload_split(m->proj_w, wp.data(), wp.size(), m->scheme));
+    S3B_OK(upload_vec(m, "post_extract_proj.bias", H, m->proj_b));
+    m->layers.resize(2 * NL);
+    for (int l = 0; l < NL; ++l)
+        for (int d = 0; d < 2; ++d) {
+            LayerW& L = m->layers[2 * l + d];
+            const std::string p = std::string(d == 0 ? "forward_lstm." : "backward_lstm."), k = std::to_string(l);
+            const HostTensor *wih, *whh, *bih, *bhh;
+            S3B_OK(need(m, p + "weight_ih_l" + k, {4 * H, H}, &wih));
+            S3B_OK(need(m, p + "weight_hh_l" + k, {4 * H, H}, &whh));
+            S3B_OK(need(m, p + "bias_ih_l" + k, {4 * H}, &bih));
+            S3B_OK(need(m, p + "bias_hh_l" + k, {4 * H}, &bhh));
+            S3B_OK(upload_split(L.wih, wih->data.data(), wih->numel(), m->scheme));
+            std::vector<float> b(bih->data);
+            for (int i = 0; i < 4 * H; ++i) b[i] += bhh->data[i];
+            S3B_OK(upload_f32(L.gru_b, b.data(), b.size()));
+            S3B_OK(upload_f32(L.whh, whh->data.data(), whh->numel()));
+        }
+    int ok = 0, sms = 0, smem = 0;
+    CUDA_OK(lstm_fits(&ok, &sms, &smem));
+    if (sms < kLstmCtas)
+        return fail("the LSTM recurrence kernel needs %d SMs (one CTA each, all co-resident); this device has %d",
+                    kLstmCtas, sms);
+    if ((size_t)smem < lstm_smem_bytes())
+        return fail("the LSTM recurrence kernel needs %zu bytes of shared memory per CTA; this device allows %d",
+                    lstm_smem_bytes(), smem);
+    if (!ok)
+        return fail("the LSTM recurrence kernel cannot run on this device: %d co-resident CTAs with %zu bytes of "
+                    "shared memory each (cooperative launch) do not fit", kLstmCtas, lstm_smem_bytes());
+    CUDA_OK(init_fbank_tables());
+    m->host.clear();
+    m->finalized = true;
+    return 0;
+}
+
 extern "C" int s3b_model_finalize(s3b_model* m) {
     if (!m) return fail("null model");
     if (m->finalized) return 0;
@@ -690,6 +762,7 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
     m->sm_count = prop.multiProcessorCount;
     g_sm_count = m->sm_count;
     if (apc(m)) return finalize_apc(m);
+    if (decoar1(m)) return finalize_decoar(m);
 
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, F = c.ffn_dim, C = kConvDim;
@@ -868,6 +941,7 @@ extern "C" int64_t s3b_num_frames(const s3b_model* m, int64_t max_len) {
 
 extern "C" int32_t s3b_num_outputs(const s3b_model* m) {
     if (apc(m)) return m->cfg.num_layers;  // the output of every GRU layer (+ residual)
+    if (decoar1(m)) return m->decoar_all_layers ? m->cfg.num_layers : 1;  // decoar_layers: every layer; decoar: the last
     return m ? m->cfg.num_layers + 1 + m->cfg.pred_heads : -1;
 }
 
@@ -876,13 +950,17 @@ extern "C" int s3b_valid_frames(const s3b_model* m, const int64_t* lens, int32_t
     if (!m || !lens || !valid) return fail("null argument");
     const int64_t T = model_frames(m, max_len);
     if (T <= 0)
-        return fail("max_len %lld too short for the %s", (long long)max_len, decoar2(m) || apc(m) ? "fbank" : "conv stack");
+        return fail("max_len %lld too short for the %s", (long long)max_len,
+                    decoar2(m) || fbank_all_frames(m) ? "fbank" : "conv stack");
     bool any_pad = false;
     for (int b = 0; b < batch; ++b) {
         if (lens[b] < 1 || lens[b] > max_len) return fail("lens[%d]=%lld out of range", b, (long long)lens[b]);
         if (apc(m) && lens[b] < kDecoar2MinLen)
             return fail("lens[%d]=%lld: APC needs >= %lld samples (2 fbank frames; the CMVN std of one frame is NaN)", b,
                         (long long)lens[b], (long long)kDecoar2MinLen);
+        if (decoar1(m) && lens[b] < kDecoar2MinLen)
+            return fail("lens[%d]=%lld: DeCoAR needs >= %lld samples (2 fbank frames; the CMVN std of one frame is NaN)",
+                        b, (long long)lens[b], (long long)kDecoar2MinLen);
         if (decoar2(m) && lens[b] < kDecoar2MinLen)
             return fail("lens[%d]=%lld: DeCoAR 2.0 needs >= %lld samples (2 fbank frames; the CMVN std of one frame is NaN)",
                         b, (long long)lens[b], (long long)kDecoar2MinLen);
@@ -890,7 +968,7 @@ extern "C" int s3b_valid_frames(const s3b_model* m, const int64_t* lens, int32_t
     }
     for (int b = 0; b < batch; ++b) {
         int64_t v;
-        if (apc(m)) {
+        if (fbank_all_frames(m)) {
             v = fbank_frames(lens[b]);  // pad_sequence of the per-utterance features (apc/expert.py:47-51)
         } else if (decoar2(m)) {
             v = decoar2_frames(lens[b]);  // pad_sequence of the per-utterance features (decoar2/expert.py:81-92)
@@ -1231,12 +1309,12 @@ struct Plan {
     std::vector<LayerPlan> layers;
     GemmParams pred1;                // Distiller: Linear(D, N*D) + GELU
     std::vector<GemmParams> pred2;   // Distiller: SplitLinear, one [D][D] GEMM per task
-    std::vector<GemmParams> gru_in;  // APC: the input projection of every GRU layer
+    std::vector<GemmParams> gru_in;  // APC / DeCoAR: the input projection of every recurrent layer (and direction)
 };
 
 void Workspace::release() {
     DevBuf* bufs[] = {&book, &wav_stats, &wav_pad, &c0_part, &c0_ss, &conv_f32, &tmp_f32, &x_f32, &x1_f32, &gate, &pos_z,
-                      &hs0, &glu_f32, &fb_f32, &xg_f32};
+                      &hs0, &glu_f32, &fb_f32, &xg_f32, &lstm_h, &lstm_sync};
     for (DevBuf* b : bufs) b->release();
     for (int i = 0; i < kNumConv; ++i) act[i].release();
     SplitBuf* sb[] = {&ln512_s, &x_s, &xs_s, &q_s, &k_s, &vt_s, &ctx_s, &x1_s, &h_s};
@@ -1282,12 +1360,13 @@ struct Fwd {
     const float** d_wavs = nullptr;
     long long* d_lens = nullptr;
     int* d_kv = nullptr;
-    int* d_ord = nullptr;  // APC: utterances longest first (the recurrence kernel's grouping)
+    int* d_ord = nullptr;  // APC / DeCoAR: utterances longest first (the recurrence kernels' grouping)
     uint8_t* d_mask = nullptr;
 
     static constexpr int kConformerStages = 10;  // stages per Conformer layer (conformer_stage)
     int num_stages() const {
         if (apc(m)) return 1 + 2 * m->cfg.num_layers;  // front end, then per layer: input GEMM, recurrence
+        if (decoar1(m)) return 2 + 4 * m->cfg.num_layers;  // front end, post_extract_proj, per layer and direction: GEMM, recurrence
         if (m->cfg.conformer) return 9 + kConformerStages * m->cfg.num_layers;
         return 9 + 5 * m->cfg.num_layers + (m->cfg.pred_heads > 0 ? 1 + m->cfg.pred_heads : 0);
     }
@@ -1305,6 +1384,7 @@ struct Fwd {
     int stage(int s);
     int conformer_stage(int l, int sub);
     int apc_stage(int s);
+    int decoar_stage(int s);
     float* hs(int l) const { return (distil() && l == 0) ? w->hs0.as<float>() : slot(l); }
 };
 
@@ -1312,7 +1392,7 @@ int Fwd::prepare() {
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, C = kConvDim;
     if (B < 1) return fail("empty batch");
-    const bool fb = decoar2(m) || apc(m);
+    const bool fb = decoar2(m) || fbank_all_frames(m);
     {
         int64_t cur = Lmax;
         for (int i = 0; i < kNumConv; ++i) cur = L[i] = fb ? 0 : conv_out_len(cur, i);
@@ -1332,7 +1412,7 @@ int Fwd::prepare() {
     const size_t off_lens = (size_t)B * sizeof(void*);
     const size_t off_kv = off_lens + (size_t)B * sizeof(long long);
     const size_t off_ord = off_kv + (size_t)B * sizeof(int);
-    const size_t off_mask = (off_ord + (apc(m) ? (size_t)B * sizeof(int) : 0) + 15) & ~(size_t)15;
+    const size_t off_mask = (off_ord + (fbank_all_frames(m) ? (size_t)B * sizeof(int) : 0) + 15) & ~(size_t)15;
     const size_t book_bytes = off_mask + (size_t)M;
     S3B_OK(w->book.ensure(book_bytes));
     if (w->book_host_bytes < book_bytes) {
@@ -1358,7 +1438,7 @@ int Fwd::prepare() {
         for (int b = 0; b < B; ++b) hl[b] = (long long)lens[b];
         for (int b = 0; b < B; ++b)
             for (int t = hk[b]; t < T; ++t) hm[(size_t)b * T + t] = 1;
-        if (apc(m)) {  // group utterances of similar length: a recurrence cluster stops at its own longest
+        if (fbank_all_frames(m)) {  // group utterances of similar length: a recurrence group stops at its own longest
             int* ho = reinterpret_cast<int*>(hb + off_ord);
             std::vector<int> ord(B);
             for (int b = 0; b < B; ++b) ord[b] = b;
@@ -1384,6 +1464,15 @@ int Fwd::prepare() {
         S3B_OK(w->ln512_s.ensure((size_t)M * kDecoar2K));  // layer 0's GEMM operand: the CMVN kernel's planes
         S3B_OK(w->x_s.ensure((size_t)M * D));             // layers 1..: the recurrence kernel's planes
         S3B_OK(w->xg_f32.ensure((size_t)M * 3 * D * 4));
+    } else if (decoar1(m)) {
+        const int H = kLstmHidden;
+        S3B_OK(w->fb_f32.ensure((size_t)B * T * 80 * 4));
+        S3B_OK(w->ln512_s.ensure((size_t)M * kDecoar2K));  // post_extract_proj's operand: the CMVN kernel's planes
+        S3B_OK(w->x_s.ensure((size_t)M * H));              // layer 0's operand: post_extract_proj's output
+        S3B_OK(w->h_s.ensure((size_t)M * 2 * H));          // layers 1..: the previous layer's [M][2H] output
+        S3B_OK(w->xg_f32.ensure((size_t)M * 4 * H * 4));
+        S3B_OK(w->lstm_h.ensure(lstm_hbuf_floats(B) * 4));
+        S3B_OK(w->lstm_sync.ensure(sizeof(unsigned int)));
     } else if (fb) {
         S3B_OK(w->fb_f32.ensure((size_t)B * fbank_frames(Lmax) * 80 * 4));
         S3B_OK(w->ln512_s.ensure((size_t)M * kDecoar2K));  // post_extract_proj's A operand: the CMVN kernel's planes
@@ -1396,7 +1485,7 @@ int Fwd::prepare() {
         S3B_OK(w->conv_f32.ensure((size_t)B * (c.extractor_layer_norm ? L[1] : L[6]) * C * 4));
         S3B_OK(w->ln512_s.ensure((size_t)M * C));
     }
-    if (!apc(m)) {  // the encoder's buffers
+    if (!fbank_all_frames(m)) {  // the encoder's buffers
         S3B_OK(w->tmp_f32.ensure((size_t)M * D * 4));
         S3B_OK(w->x_f32.ensure((size_t)M * D * 4));
         S3B_OK(w->x1_f32.ensure((size_t)M * D * 4));
@@ -1551,6 +1640,31 @@ int Fwd::build_plan(Plan& pl) {
             e.out_f32 = w->xg_f32.as<float>();
             set_epi(p, e, 3 * D);
         }
+        return 0;
+    }
+    if (decoar1(m)) {
+        // post_extract_proj [M][80 -> 128] x [1024][128]^T + b into layer 0's operand planes
+        const int H = kLstmHidden;
+        S3B_OK(linear_params(pl.proj, w->ln512_s, m->proj_w, M, H, kDecoar2K, m->scheme));
+        Epi e;
+        e.bias = m->proj_b.as<float>();
+        e.op = w->x_s.planes(m->scheme);
+        set_epi(pl.proj, e, H);
+        // x_g = x W_ih^T + (b_ih + b_hh), fp32 [M][4H]; layer k > 0 reads its direction's half of layer k - 1's
+        // [M][2H] output (row stride 2H)
+        pl.gru_in.resize(2 * NL);
+        for (int l = 0; l < NL; ++l)
+            for (int d = 0; d < 2; ++d) {
+                GemmParams& p = pl.gru_in[2 * l + d];
+                if (l == 0) S3B_OK(linear_params(p, w->x_s, m->layers[d].wih, M, 4 * H, H, m->scheme));
+                else
+                    S3B_OK(linear_params(p, w->h_s, m->layers[2 * l + d].wih, M, 4 * H, H, m->scheme, 2 * H,
+                                         (size_t)d * H));
+                Epi ei;
+                ei.bias = m->layers[2 * l + d].gru_b.as<float>();
+                ei.out_f32 = w->xg_f32.as<float>();
+                set_epi(p, ei, 4 * H);
+            }
         return 0;
     }
     for (int i = 1; i < kNumConv && !decoar2(m); ++i) {
@@ -1708,8 +1822,54 @@ int Fwd::apc_stage(int s) {
     return 0;
 }
 
+// DeCoAR: stage 0 = fbank + CMVN; stage 1 = post_extract_proj; stage 2 + 4l + 2d = the input GEMM of layer l,
+// direction d (0 forward, 1 backward); stage 3 + 4l + 2d = its recurrence, which writes columns [d H, d H + H) of
+// layer l's [B][T][2H] output: an output slot (decoar_layers: every layer; decoar: the last) and, below the last
+// layer, the operand planes of layer l + 1's GEMMs. The two directions never run concurrently: each recurrence
+// occupies the whole device.
+int Fwd::decoar_stage(int s) {
+    s3b_model* m = this->m;  // the launch macros expect `m` and `st`
+    cudaStream_t st = this->st;
+    const int NL = m->cfg.num_layers, H = kLstmHidden;
+    if (s == 0) {
+        const size_t book_bytes = (size_t)(reinterpret_cast<char*>(d_mask) - w->book.as<char>()) + (size_t)M;
+        CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host, book_bytes, cudaMemcpyHostToDevice, st));
+        if (!capturing) CUDA_OK(cudaEventRecord(w->book_copied, st));
+        KLAUNCH(CAT_CONV0, 2, 0.0, launch_decoar2_features(d_wavs, d_lens, B, T, T, 1, w->fb_f32.as<float>(),
+                                                           w->ln512_s.planes(m->scheme), st));
+        return 0;
+    }
+    if (s == 1) {
+        GemmParams p = plan->proj;
+        KGEMM(launch_gemm(p, m->sm_count, st));
+        return 0;
+    }
+    const int l = (s - 2) / 4, d = ((s - 2) / 2) % 2;
+    if (l >= NL) return fail("internal: stage %d out of range", s);
+    if ((s - 2) % 2 == 0) {
+        GemmParams p = plan->gru_in[2 * l + d];
+        KGEMM(launch_gemm(p, m->sm_count, st));
+        return 0;
+    }
+    const bool last = l == NL - 1;
+    LstmParams g;
+    g.xg = w->xg_f32.as<float>(), g.whh = m->layers[2 * l + d].whh.as<float>(), g.bhh = nullptr;
+    g.len = d_kv, g.order = d_ord, g.B = B, g.T = T, g.direction = d;
+    g.out = m->decoar_all_layers ? slot(l) : last ? slot(0) : nullptr;
+    g.ldo = 2 * H, g.col0 = d * H;
+    g.op = last ? no_planes() : w->h_s.planes(m->scheme);
+    g.hbuf = w->lstm_h.as<float>(), g.counter = w->lstm_sync.as<unsigned int>();
+    KLAUNCH(CAT_GRU, (B + kLstmMaxBatch - 1) / kLstmMaxBatch, 8.0 * H * H * (double)M, launch_lstm(g, st));
+    if (d == 1 && layer_done != nullptr) {
+        if (m->decoar_all_layers) S3B_OK(layer_done(m, l, st, user));
+        else if (last) S3B_OK(layer_done(m, 0, st, user));
+    }
+    return 0;
+}
+
 int Fwd::stage(int s) {
     if (apc(m)) return apc_stage(s);
+    if (decoar1(m)) return decoar_stage(s);
     s3b_model* m = this->m;  // the launch macros expect `m` and `st`
     cudaStream_t st = this->st;
     const s3b_config& c = m->cfg;
@@ -1990,7 +2150,8 @@ static int default_lanes(int B, int64_t T) {
 
 extern "C" int32_t s3b_default_lanes(const s3b_model* m, int32_t batch, int64_t max_len) {
     const int64_t T = model_frames(m, max_len);
-    return (batch < 1 || T < 1) ? -1 : default_lanes(batch, T);
+    if (batch < 1 || T < 1) return -1;
+    return decoar1(m) ? 1 : default_lanes(batch, T);  // DeCoAR's recurrence occupies the whole device
 }
 
 static int forward_lanes(s3b_model* m, const float* const* wavs, const int64_t* lens, int B, int64_t Lmax,
@@ -1999,9 +2160,11 @@ static int forward_lanes(s3b_model* m, const float* const* wavs, const int64_t* 
     if (B < 1) return fail("empty batch");
     const int64_t T = model_frames(m, Lmax);
     if (T < 1) return fail("max_len %lld too short: the %s yields no frame", (long long)Lmax,
-                           decoar2(m) || apc(m) ? "fbank" : "conv stack");
+                           decoar2(m) || fbank_all_frames(m) ? "fbank" : "conv stack");
     int lanes = (o && o->lanes > 0) ? o->lanes : default_lanes(B, T);
     if (lanes > 2) lanes = 2;
+    // two grid-resident LSTM launches must never be in flight at once: a DeCoAR model runs one lane
+    if (decoar1(m)) lanes = 1;
     if (lanes > B) lanes = B;
     const size_t frame = (size_t)T * c.embed_dim;
     const size_t layer_stride = (o && o->layer_stride > 0) ? (size_t)o->layer_stride : (size_t)B * frame;
@@ -2137,6 +2300,9 @@ extern "C" int s3b_forward_ex(s3b_model* m, const float* const* wavs, const int6
         return fail("ffn_out / last_residual: a Conformer encoder collects no layer results (wav2vec2_model.py:3199-3200)");
     if (apc(m) && opts != nullptr && (opts->ffn_out != nullptr || opts->last_residual != nullptr))
         return fail("ffn_out / last_residual: an APC model is a GRU stack, it has no feed-forward blocks or layer results");
+    if (decoar1(m) && opts != nullptr && (opts->ffn_out != nullptr || opts->last_residual != nullptr))
+        return fail("ffn_out / last_residual: a DeCoAR model is an LSTM stack, it has no feed-forward blocks or layer "
+                    "results");
     return forward_lanes(m, wavs, lens, batch, max_len, hidden_out, (cudaStream_t)stream, opts);
 }
 
@@ -2975,6 +3141,65 @@ extern "C" int s3b_gru_f32(const float* xg, const float* whh, const float* bhh, 
         return 0;
     }();
     xgc.release(), bk.release(), os.release();
+    return r;
+}
+
+extern "C" int s3b_lstm_fits(int32_t* out) {
+    if (!out) return fail("null argument");
+    if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
+    int ok = 0, sms = 0, smem = 0;
+    CUDA_OK(lstm_fits(&ok, &sms, &smem));
+    *out = ok;
+    return 0;
+}
+
+extern "C" int s3b_lstm_f32(const float* xg, const float* whh, const float* bhh, const int32_t* lens, int32_t B,
+                            int32_t T, int32_t direction, int32_t out_fmt, float* out, float* planes_out,
+                            void* stream) {
+    // Fwd::decoar_stage(3 + 4l + 2d) on this call's buffers, utterances ordered longest first as the model orders them
+    if (!xg || !whh || !lens || !out) return fail("null argument");
+    if (B < 1 || T < 1) return fail("bad sizes (batch %d, t %d)", B, T);
+    if (direction != 0 && direction != 1) return fail("direction must be 0 (forward) or 1 (backward), not %d", direction);
+    if (out_fmt < -1 || out_fmt > 1) return fail("out_fmt must be -1 (none), 0 (bf16 hi/lo) or 1 (f16q8), not %d", out_fmt);
+    if (out_fmt >= 0 && planes_out == nullptr) return fail("out_fmt %d needs planes_out", out_fmt);
+    for (int b = 0; b < B; ++b)
+        if (lens[b] < 0 || lens[b] > T) return fail("lens[%d] = %d outside [0, %d]", b, lens[b], T);
+    if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
+    int ok = 0, sms = 0, smem = 0;
+    CUDA_OK(lstm_fits(&ok, &sms, &smem));
+    if (!ok) return fail("the LSTM recurrence kernel cannot run on this device (%d SMs, %d bytes of shared memory)", sms, smem);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int H = kLstmHidden;
+    const size_t M = (size_t)B * T;
+    DevBuf bk, hb, sync;
+    SplitBuf os;
+    const int r = [&]() -> int {
+        std::vector<int> host(2 * (size_t)B);
+        memcpy(host.data(), lens, (size_t)B * sizeof(int));
+        std::vector<int> ord(B);
+        for (int b = 0; b < B; ++b) ord[b] = b;
+        std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return lens[a] > lens[b]; });
+        memcpy(host.data() + B, ord.data(), (size_t)B * sizeof(int));
+        S3B_OK(bk.ensure(host.size() * sizeof(int)));
+        CUDA_OK(cudaMemcpyAsync(bk.p, host.data(), host.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+        S3B_OK(hb.ensure(lstm_hbuf_floats(B) * 4));
+        S3B_OK(sync.ensure(sizeof(unsigned int)));
+        LstmParams g;
+        g.xg = xg, g.whh = whh, g.bhh = bhh;
+        g.len = bk.as<int>(), g.order = bk.as<int>() + B, g.B = B, g.T = T, g.direction = direction;
+        g.out = out, g.ldo = 2 * H, g.col0 = direction * H;
+        g.op = no_planes();
+        if (out_fmt >= 0) {
+            S3B_OK(os.ensure(M * 2 * H));
+            g.op = os.planes(out_fmt);
+        }
+        g.hbuf = hb.as<float>(), g.counter = sync.as<unsigned int>();
+        CUDA_OK(launch_lstm(g, st));
+        if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(g.op, M * 2 * H, planes_out, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+        return 0;
+    }();
+    bk.release(), hb.release(), sync.release(), os.release();
     return r;
 }
 

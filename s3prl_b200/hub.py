@@ -155,6 +155,30 @@ ENTRIES["apc_url"] = _make_apc_entry("apc_url", False, True)
 ENTRIES["vq_apc_url"] = _make_apc_entry("vq_apc_url", True, True)
 
 
+def _make_decoar_entry(name: str, all_layers: bool, needs_ckpt: bool) -> Callable:
+    """DeCoAR (decoar/hubconf.py, decoar_layers/hubconf.py): the fabricated checkpoint without ``ckpt``, else the
+    local ``{"model"}`` file; a URL is refused (remote checkpoints cannot be reached offline)."""
+
+    def entry(ckpt=None, *args, **kwargs):
+        from .upstream.decoar import DecoarExpert
+
+        if needs_ckpt:
+            assert isinstance(ckpt, str), "a checkpoint path is required"
+        if isinstance(ckpt, str) and ckpt.startswith("http"):
+            raise ValueError(f"{name}: remote checkpoints are not reachable here; download {ckpt} and pass the file")
+        kwargs.pop("refresh", None)
+        return DecoarExpert(ckpt=ckpt, all_layers=all_layers, name=name, **kwargs)
+
+    entry.__name__ = name
+    return entry
+
+
+for _family, _all in (("decoar", False), ("decoar_layers", True)):
+    ENTRIES[_family] = _make_decoar_entry(_family, _all, False)
+    for _suffix in ("local", "url", "custom"):
+        ENTRIES[f"{_family}_{_suffix}"] = _make_decoar_entry(f"{_family}_{_suffix}", _all, True)
+
+
 def options() -> List[str]:
     """Names of the available entries (cf. s3prl.hub.options, s3prl/hub.py:40-54)."""
     return sorted(ENTRIES)

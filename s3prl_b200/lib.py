@@ -24,6 +24,7 @@ EXPORTED_SYMBOLS = [
     "s3b_model_finalize",
     "s3b_model_destroy",
     "s3b_apc_model_create",
+    "s3b_decoar_model_create",
     "s3b_num_frames",
     "s3b_valid_frames",
     "s3b_num_outputs",
@@ -62,6 +63,8 @@ EXPORTED_SYMBOLS = [
     "s3b_apc_features_f32",
     "s3b_gru_f32",
     "s3b_gru_max_active_clusters",
+    "s3b_lstm_f32",
+    "s3b_lstm_fits",
     "s3b_layernorm_rope_f32",
     "s3b_fbank",
     "s3b_fbank_ex",
@@ -119,6 +122,22 @@ class S3BApcConfig(C.Structure):
     def __init__(self, **kw):
         super().__init__(**kw)
         self.struct_size = C.sizeof(S3BApcConfig)
+
+
+class S3BDecoarConfig(C.Structure):
+    """Mirror of ``struct s3b_decoar_config``."""
+
+    _fields_ = [
+        ("struct_size", C.c_int32),
+        ("num_layers", C.c_int32),
+        ("hidden", C.c_int32),
+        ("all_layers", C.c_int32),
+        ("reserved", C.c_int32 * 4),
+    ]
+
+    def __init__(self, **kw):
+        super().__init__(**kw)
+        self.struct_size = C.sizeof(S3BDecoarConfig)
 
 
 class S3BForwardOpts(C.Structure):
@@ -226,6 +245,7 @@ def load() -> C.CDLL:
     lib.s3b_model_create.argtypes = [C.POINTER(S3BConfig), C.POINTER(vp)]
     lib.s3b_model_set_tensor.argtypes = [vp, C.c_char_p, vp, C.POINTER(i64), i32]
     lib.s3b_apc_model_create.argtypes = [C.POINTER(S3BApcConfig), C.POINTER(vp)]
+    lib.s3b_decoar_model_create.argtypes = [C.POINTER(S3BDecoarConfig), C.POINTER(vp)]
     lib.s3b_model_finalize.argtypes = [vp]
     lib.s3b_model_destroy.argtypes = [vp]
     lib.s3b_model_destroy.restype = None
@@ -275,6 +295,8 @@ def load() -> C.CDLL:
     lib.s3b_apc_features_f32.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i32, f32p, vp]
     lib.s3b_gru_max_active_clusters.argtypes = [C.POINTER(i32)]
     lib.s3b_gru_f32.argtypes = [f32p, f32p, f32p, f32p, C.POINTER(i32), i32, i32, i32, i32, f32p, f32p, vp]
+    lib.s3b_lstm_fits.argtypes = [C.POINTER(i32)]
+    lib.s3b_lstm_f32.argtypes = [f32p, f32p, f32p, C.POINTER(i32), i32, i32, i32, i32, f32p, f32p, vp]
     lib.s3b_layernorm_rope_f32.argtypes = [f32p, i64, i32, i32, f32p, f32p, C.POINTER(C.c_float), i32, f32p, f32p, vp]
     lib.s3b_fbank_num_frames.argtypes = [i64]
     lib.s3b_fbank_num_frames.restype = i64
