@@ -19,7 +19,9 @@
 
 #include <algorithm>
 #include <map>
+#include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/s3prl_b200.h"
@@ -68,9 +70,25 @@ struct HostTensor {
 // bumped on every (re)allocation: cached launch plans hold raw device pointers and are rebuilt when it moves
 static uint64_t g_alloc_generation = 1;
 
+// Owns one device allocation: freed on destruction, moved but never copied (a copy would free it twice)
 struct DevBuf {
     void* p = nullptr;
     size_t bytes = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    DevBuf(DevBuf&& o) noexcept : p(o.p), bytes(o.bytes) { o.p = nullptr, o.bytes = 0; }
+    DevBuf& operator=(DevBuf&& o) noexcept {
+        if (this != &o) {
+            if (p) cudaFree(p);
+            p = o.p, bytes = o.bytes;
+            o.p = nullptr, o.bytes = 0;
+        }
+        return *this;
+    }
+    ~DevBuf() {
+        if (p) cudaFree(p);
+    }
     int ensure(size_t n) {
         n += 1 << 16;  // slack: TMA boxes may over-read the last rows of a view (never consumed)
         if (n <= bytes) return 0;
@@ -86,15 +104,12 @@ struct DevBuf {
         bytes = n;
         return 0;
     }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr, bytes = 0;
-    }
     template <class T>
     T* as() const {
         return reinterpret_cast<T*>(p);
     }
 };
+static_assert(!std::is_copy_constructible<DevBuf>::value, "DevBuf owns its allocation: a copy would free it twice");
 
 // One GEMM operand in HBM, 4 bytes per element in either format:
 //   fmt 0 (bf16x3 scheme): `hi` = bf16 hi plane, `lo` = bf16 lo plane
@@ -114,8 +129,37 @@ struct SplitBuf {
     uint8_t* h8() const { return lo.as<uint8_t>(); }
     uint8_t* l8() const { return lo.as<uint8_t>() + l8_off; }
     OutPlanes planes(int fmt) const { return OutPlanes{h(), fmt ? nullptr : l(), fmt ? h8() : nullptr, fmt ? l8() : nullptr, fmt}; }
-    void release() { hi.release(), lo.release(), l8_off = 0; }
 };
+
+// Streams, events and pinned host memory, released on destruction
+struct StreamDestroy {
+    void operator()(cudaStream_t s) const { cudaStreamDestroy(s); }
+};
+struct EventDestroy {
+    void operator()(cudaEvent_t e) const { cudaEventDestroy(e); }
+};
+struct PinnedFree {
+    void operator()(char* p) const { cudaFreeHost(p); }
+};
+using Stream = std::unique_ptr<CUstream_st, StreamDestroy>;
+using Event = std::unique_ptr<CUevent_st, EventDestroy>;
+using PinnedBuf = std::unique_ptr<char, PinnedFree>;
+
+// the stream / event on first use: a non-blocking stream, an event without timing
+static int ensure_stream(Stream& s) {
+    if (s) return 0;
+    cudaStream_t h = nullptr;
+    CUDA_OK(cudaStreamCreateWithFlags(&h, cudaStreamNonBlocking));
+    s.reset(h);
+    return 0;
+}
+static int ensure_event(Event& e) {
+    if (e) return 0;
+    cudaEvent_t h = nullptr;
+    CUDA_OK(cudaEventCreateWithFlags(&h, cudaEventDisableTiming));
+    e.reset(h);
+    return 0;
+}
 
 // Default operand scheme: 1 = f16q8 (fp16 product + two e4m3 corrections): parity class of bf16x3 on every golden, and
 // 2 MMA slots per 16 of K instead of 3 (e4m3 wgmma runs at twice the fp16 rate); bf16x3 (0) stays available through
@@ -156,50 +200,71 @@ struct LayerW {
 enum { CAT_GEMM = 0, CAT_ATTN = 1, CAT_CONV0 = 2, CAT_NORM = 3, CAT_MISC = 4, CAT_GRU = 5, CAT_COUNT = 6 };
 struct ProfRec {
     int cat;
-    cudaEvent_t a, b;
+    Event a, b;
 };
 struct Profiler {
     bool on = false;
-    std::vector<cudaEvent_t> pool;
+    std::vector<Event> pool;
     std::vector<ProfRec> recs;
-    cudaEvent_t pending = nullptr;
+    Event pending;
     double ms[CAT_COUNT] = {};
     double flops[CAT_COUNT] = {};
     long long launches[CAT_COUNT] = {};
-    cudaEvent_t get() {
+    Event get() {
         if (!pool.empty()) {
-            cudaEvent_t e = pool.back();
+            Event e = std::move(pool.back());
             pool.pop_back();
             return e;
         }
         cudaEvent_t e = nullptr;
         cudaEventCreate(&e);
-        return e;
+        return Event(e);
     }
+};
+
+// Cached launch plan: every tensor map / GEMM descriptor of one forward at a given (B, Lmax).
+// Encoding the ~22 CUtensorMaps of a layer costs ~300 driver calls per forward; they only depend on the workspace
+// addresses, the weights and (B, T), so they are built once per shape and reused (ragged training batches change
+// Lmax every step and rebuild; fixed-shape serving never does). Pointers into the caller's hidden_out buffer are
+// plain epilogue fields and are patched per call.
+struct LayerPlan {
+    GemmParams qkv, out, fc1, fc2;
+    AttnParams attn;
+    GemmParams v, ffn1_a, ffn1_b, pw1, pw2;  // Conformer (qkv = [q | k], fc1 / fc2 = ffn2)
+};
+struct Plan {
+    int B = 0;
+    int64_t Lmax = 0;
+    uint64_t gen = 0;
+    GemmParams conv[kNumConv];
+    GemmParams proj, pos;
+    GemmParams pos_d[8];             // data2vec: one four-taps GEMM per conv block (pos_conv_depth <= 8)
+    std::vector<LayerPlan> layers;
+    GemmParams pred1;                // Distiller: Linear(D, N*D) + GELU
+    std::vector<GemmParams> pred2;   // Distiller: SplitLinear, one [D][D] GEMM per task
+    std::vector<GemmParams> gru_in;  // APC / DeCoAR: the input projection of every recurrent layer (and direction)
 };
 
 // Per-lane working set. A forward call runs the batch as one or two utterance micro-batches ("lanes"): lane 0 on
 // the caller's stream, lane 1 on an internal stream, every kernel enqueue alternating between the two so that one
 // lane's tails / small kernels fill the SMs the other leaves idle. Utterances are independent given the shared
 // max_len, so the result is bit-identical to the single-lane run (tests/test_properties_gpu.py).
-struct Plan;
 struct Workspace {
     // bookkeeping block (one pinned host mirror, one async H2D copy per call): wav ptrs | lens | kv_len | row mask
     DevBuf book;
-    void* book_host = nullptr;
+    PinnedBuf book_host;
     size_t book_host_bytes = 0;
     size_t book_valid = 0;  // bytes of the mirror that hold the last call's block
-    cudaEvent_t book_copied = nullptr;  // the previous call's H2D copy has been consumed: the mirror may be rewritten
+    Event book_copied;      // the previous call's H2D copy has been consumed: the mirror may be rewritten
     DevBuf wav_stats, wav_pad, c0_part, c0_ss, conv_f32, tmp_f32, x_f32, x1_f32, gate, pos_z, hs0;
     DevBuf glu_f32;  // Conformer: pointwise_conv1 output [M][2D]
     DevBuf fb_f32;   // DeCoAR 2.0 / APC: log-mel frames [B][m(Lmax)][80]
     DevBuf xg_f32;   // APC / DeCoAR: the input GEMM's output [M][3H] / [M][4H]
     DevBuf lstm_h, lstm_sync;  // DeCoAR: the recurrence's state exchange buffer and grid-barrier counter
     SplitBuf act[kNumConv], ln512_s, x_s, xs_s, q_s, k_s, vt_s, ctx_s, x1_s, h_s;
-    cudaStream_t stream = nullptr;  // lane stream (lane 1; lane 0 runs on the caller's stream)
-    cudaEvent_t done = nullptr;
-    std::vector<Plan*> plans;  // small LRU of cached tensor maps / launch descriptors keyed by (B, Lmax)
-    void release();
+    Stream stream;  // lane stream (lane 1; lane 0 runs on the caller's stream)
+    Event done;
+    std::vector<std::unique_ptr<Plan>> plans;  // small LRU of cached tensor maps / launch descriptors keyed by (B, Lmax)
 };
 
 struct s3b_model {
@@ -216,9 +281,9 @@ struct s3b_model {
     int scheme = 0;  // tensor-core operand scheme of the conv / linear GEMMs: 0 = bf16x3, 1 = f16q8 (gemm.cuh)
     Profiler prof;
     long long launches_total = 0;  // kernels launched by this model since creation
-    cudaStream_t copy_stream = nullptr, compute_stream = nullptr;
-    cudaEvent_t fork_event = nullptr;
-    std::vector<cudaEvent_t> layer_events;
+    Stream copy_stream, compute_stream;
+    Event fork_event;
+    std::vector<Event> layer_events;
 
     // weights
     DevBuf conv0_w, conv0_b, norm0_g, norm0_b;           // conv 0 (+ GroupNorm or LN affine)
@@ -242,21 +307,6 @@ struct s3b_model {
 
     Workspace ws[2];
     DevBuf stage_wav, stage_out;  // s3b_forward_host staging
-
-    // CUDA-graph replay of a whole forward (S3B_GRAPHS=1): keyed by everything the captured kernel arguments depend on
-    struct GraphEntry {
-        int B, lanes;
-        int64_t Lmax;
-        float *hidden, *ffn, *last_res;
-        size_t layer_stride, ffn_stride;
-        cudaStream_t st;
-        uint64_t gen;
-        int hits;
-        long long launches;
-        cudaGraphExec_t exec;
-    };
-    std::vector<GraphEntry> graphs;
-    bool graphs_disabled = false;
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -274,7 +324,6 @@ static int upload_split(SplitBuf& dst, const float* src, size_t n, int fmt = 0) 
     if (fmt != 0) CUDA_OK(launch_split_q8(tmp.as<float>(), dst.h(), dst.h8(), dst.l8(), n, 1, 0));
     else CUDA_OK(launch_split(tmp.as<float>(), dst.h(), dst.l(), n, 0));
     CUDA_OK(cudaDeviceSynchronize());
-    tmp.release();
     return 0;
 }
 static const HostTensor* find(const s3b_model* m, const std::string& k) {
@@ -464,38 +513,7 @@ extern "C" int s3b_model_set_tensor(s3b_model* m, const char* name, const float*
     return 0;
 }
 
-extern "C" void s3b_model_destroy(s3b_model* m) {
-    if (!m) return;
-    DevBuf* bufs[] = {&m->conv0_w, &m->conv0_b, &m->norm0_g, &m->norm0_b, &m->ln512_g, &m->ln512_b, &m->proj_b,
-                      &m->pos_b, &m->enc_ln_g, &m->enc_ln_b, &m->rel_table_src, &m->rel_table, &m->stage_wav,
-                      &m->stage_out, &m->rope_cs};
-    for (DevBuf* b : bufs) b->release();
-    for (int i = 0; i < kNumConv; ++i)
-        m->conv_w[i].release(), m->conv_b[i].release(), m->conv_ln_g[i].release(), m->conv_ln_b[i].release();
-    SplitBuf* sb[] = {&m->proj_w, &m->pos_w, &m->pos_w4, &m->pred1_w};
-    for (SplitBuf* b : sb) b->release();
-    for (SplitBuf& b : m->pred2_w) b.release();
-    for (SplitBuf& b : m->posd_w4) b.release();
-    for (DevBuf& b : m->posd_b) b.release();
-    m->pred1_b.release(), m->pred2_b.release();
-    for (LayerW& l : m->layers) {
-        l.qkv.release(), l.out.release(), l.fc1.release(), l.fc2.release();
-        l.v.release(), l.ffn1_w1.release(), l.ffn1_w2.release(), l.pw1.release(), l.pw2.release(), l.wih.release();
-        DevBuf* lb[] = {&l.qkv_b,     &l.out_b,     &l.fc1_b,     &l.fc2_b,     &l.ln1_g,     &l.ln1_b,
-                        &l.ln2_g,     &l.ln2_b,     &l.grep_w,    &l.grep_b,    &l.grep_a,    &l.ffn1_b1,
-                        &l.ffn1_b2,   &l.ffn1_ln_g, &l.ffn1_ln_b, &l.ffn2_ln_g, &l.ffn2_ln_b, &l.conv_ln_g,
-                        &l.conv_ln_b, &l.dw_w,      &l.dw_b,      &l.gru_b,     &l.whh,       &l.bhn};
-        for (DevBuf* b : lb) b->release();
-    }
-    for (Workspace& w : m->ws) w.release();
-    if (m->copy_stream) cudaStreamDestroy(m->copy_stream);
-    if (m->compute_stream) cudaStreamDestroy(m->compute_stream);
-    if (m->fork_event) cudaEventDestroy(m->fork_event);
-    for (cudaEvent_t e : m->layer_events) cudaEventDestroy(e);
-    for (auto& g : m->graphs)
-        if (g.exec) cudaGraphExecDestroy(g.exec);
-    delete m;
-}
+extern "C" void s3b_model_destroy(s3b_model* m) { delete m; }
 
 // WavLM: table[h][r] = log2(e) * emb[bucket(r - (Tmax - 1))][h], r in [0, 2 Tmax - 1). Built once for Tmax frames
 // (the ungated bias is shared by all layers and all calls, WavLM.py:622-632); the attention kernel indexes it with
@@ -1243,15 +1261,15 @@ static int posconv4_params(GemmParams& p, const s3b_config& c, const __nv_bfloat
 static inline void prof_begin(s3b_model* m, cudaStream_t st) {
     if (m == nullptr || !m->prof.on) return;
     m->prof.pending = m->prof.get();
-    cudaEventRecord(m->prof.pending, st);
+    cudaEventRecord(m->prof.pending.get(), st);
 }
 static inline void prof_end(s3b_model* m, cudaStream_t st, int cat, int nkernels, double flops) {
     if (m == nullptr) return;
     m->launches_total += nkernels;
     if (!m->prof.on) return;
-    cudaEvent_t b = m->prof.get();
-    cudaEventRecord(b, st);
-    m->prof.recs.push_back({cat, m->prof.pending, b});
+    Event b = m->prof.get();
+    cudaEventRecord(b.get(), st);
+    m->prof.recs.push_back({cat, std::move(m->prof.pending), std::move(b)});
     m->prof.launches[cat] += nkernels;
     m->prof.flops[cat] += flops;
 }
@@ -1288,48 +1306,6 @@ static int launch_frontend(s3b_model* m, cudaStream_t st, const float* const* d_
 }
 
 // ------------------------------------------------------------------------------------------------
-// cached launch plan: every tensor map / GEMM descriptor of one forward at a given (B, Lmax)
-// ------------------------------------------------------------------------------------------------
-// Encoding the ~22 CUtensorMaps of a layer costs ~300 driver calls per forward; they only depend on the workspace
-// addresses, the weights and (B, T), so they are built once per shape and reused (ragged training batches change
-// Lmax every step and rebuild; fixed-shape serving never does). Pointers into the caller's hidden_out buffer are
-// plain epilogue fields and are patched per call.
-struct LayerPlan {
-    GemmParams qkv, out, fc1, fc2;
-    AttnParams attn;
-    GemmParams v, ffn1_a, ffn1_b, pw1, pw2;  // Conformer (qkv = [q | k], fc1 / fc2 = ffn2)
-};
-struct Plan {
-    int B = 0;
-    int64_t Lmax = 0;
-    uint64_t gen = 0;
-    GemmParams conv[kNumConv];
-    GemmParams proj, pos;
-    GemmParams pos_d[8];             // data2vec: one four-taps GEMM per conv block (pos_conv_depth <= 8)
-    std::vector<LayerPlan> layers;
-    GemmParams pred1;                // Distiller: Linear(D, N*D) + GELU
-    std::vector<GemmParams> pred2;   // Distiller: SplitLinear, one [D][D] GEMM per task
-    std::vector<GemmParams> gru_in;  // APC / DeCoAR: the input projection of every recurrent layer (and direction)
-};
-
-void Workspace::release() {
-    DevBuf* bufs[] = {&book, &wav_stats, &wav_pad, &c0_part, &c0_ss, &conv_f32, &tmp_f32, &x_f32, &x1_f32, &gate, &pos_z,
-                      &hs0, &glu_f32, &fb_f32, &xg_f32, &lstm_h, &lstm_sync};
-    for (DevBuf* b : bufs) b->release();
-    for (int i = 0; i < kNumConv; ++i) act[i].release();
-    SplitBuf* sb[] = {&ln512_s, &x_s, &xs_s, &q_s, &k_s, &vt_s, &ctx_s, &x1_s, &h_s};
-    for (SplitBuf* b : sb) b->release();
-    if (book_host) cudaFreeHost(book_host);
-    book_host = nullptr, book_host_bytes = 0;
-    if (book_copied) cudaEventDestroy(book_copied);
-    if (done) cudaEventDestroy(done);
-    if (stream) cudaStreamDestroy(stream);
-    book_copied = nullptr, done = nullptr, stream = nullptr;
-    for (Plan* p : plans) delete p;
-    plans.clear();
-}
-
-// ------------------------------------------------------------------------------------------------
 // forward (one lane = one utterance micro-batch) as a sequence of stages
 // ------------------------------------------------------------------------------------------------
 // layer_done: optional callback fired (host side) right after hidden state `l` has been enqueued completely
@@ -1351,7 +1327,6 @@ struct Fwd {
     float* last_res = nullptr;  // optional (pre-LN models): un-normalised output of the last layer
     LayerDoneFn layer_done = nullptr;
     void* user = nullptr;
-    bool capturing = false;  // enqueueing into a CUDA-graph capture: no event that the host later synchronises on
     // derived
     int64_t L[kNumConv];
     int T = 0, Tp = 0;
@@ -1416,14 +1391,15 @@ int Fwd::prepare() {
     const size_t book_bytes = off_mask + (size_t)M;
     S3B_OK(w->book.ensure(book_bytes));
     if (w->book_host_bytes < book_bytes) {
-        if (w->book_copied) CUDA_OK(cudaEventSynchronize(w->book_copied));
-        if (w->book_host) cudaFreeHost(w->book_host);
-        w->book_host = nullptr, w->book_host_bytes = 0;
+        if (w->book_copied) CUDA_OK(cudaEventSynchronize(w->book_copied.get()));
+        w->book_host.reset(), w->book_host_bytes = 0;
         const size_t cap = book_bytes * 2 + 4096;
-        CUDA_OK(cudaHostAlloc(&w->book_host, cap, cudaHostAllocDefault));
+        void* hp = nullptr;
+        CUDA_OK(cudaHostAlloc(&hp, cap, cudaHostAllocDefault));
+        w->book_host.reset(static_cast<char*>(hp));
         w->book_host_bytes = cap, w->book_valid = 0;
     }
-    if (w->book_copied == nullptr) CUDA_OK(cudaEventCreateWithFlags(&w->book_copied, cudaEventDisableTiming));
+    S3B_OK(ensure_event(w->book_copied));
     {
         // build the block in a scratch vector first: when nothing changed since the last call (fixed-shape serving
         // loops, the bench) the mirror is left alone and the host never waits for the previous copy to be consumed
@@ -1445,9 +1421,9 @@ int Fwd::prepare() {
             std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return hk[a] > hk[b]; });
             memcpy(ho, ord.data(), (size_t)B * sizeof(int));
         }
-        if (w->book_valid != book_bytes || memcmp(w->book_host, hb, book_bytes) != 0) {
-            CUDA_OK(cudaEventSynchronize(w->book_copied));  // normally long complete
-            memcpy(w->book_host, hb, book_bytes);
+        if (w->book_valid != book_bytes || memcmp(w->book_host.get(), hb, book_bytes) != 0) {
+            CUDA_OK(cudaEventSynchronize(w->book_copied.get()));  // normally long complete
+            memcpy(w->book_host.get(), hb, book_bytes);
             w->book_valid = book_bytes;
         }
     }
@@ -1506,28 +1482,20 @@ int Fwd::prepare() {
     // ---- launch plan (cached per (B, Lmax) while no buffer has been reallocated) --------------------------------
     plan = nullptr;
     for (size_t i = 0; i < w->plans.size(); ++i) {
-        Plan* pl = w->plans[i];
-        if (pl->B == B && pl->Lmax == Lmax && pl->gen == g_alloc_generation) {
-            plan = pl;
-            w->plans.erase(w->plans.begin() + i);
-            w->plans.insert(w->plans.begin(), pl);
+        const Plan& pl = *w->plans[i];
+        if (pl.B == B && pl.Lmax == Lmax && pl.gen == g_alloc_generation) {
+            std::rotate(w->plans.begin(), w->plans.begin() + i, w->plans.begin() + i + 1);  // to the front
+            plan = w->plans.front().get();
             break;
         }
     }
     if (plan == nullptr) {
-        Plan* pl = new Plan();
-        int r = build_plan(*pl);
-        if (r != 0) {
-            delete pl;
-            return r;
-        }
+        std::unique_ptr<Plan> pl(new Plan());
+        S3B_OK(build_plan(*pl));
         pl->B = B, pl->Lmax = Lmax, pl->gen = g_alloc_generation;
-        w->plans.insert(w->plans.begin(), pl);
-        while (w->plans.size() > 4) {
-            delete w->plans.back();
-            w->plans.pop_back();
-        }
-        plan = pl;
+        w->plans.insert(w->plans.begin(), std::move(pl));
+        if (w->plans.size() > 4) w->plans.pop_back();
+        plan = w->plans.front().get();
     }
     return 0;
 }
@@ -1797,8 +1765,8 @@ int Fwd::apc_stage(int s) {
     const int D = m->cfg.embed_dim, NL = m->cfg.num_layers;
     if (s == 0) {
         const size_t book_bytes = (size_t)(reinterpret_cast<char*>(d_mask) - w->book.as<char>()) + (size_t)M;
-        CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host, book_bytes, cudaMemcpyHostToDevice, st));
-        if (!capturing) CUDA_OK(cudaEventRecord(w->book_copied, st));
+        CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host.get(), book_bytes, cudaMemcpyHostToDevice, st));
+        CUDA_OK(cudaEventRecord(w->book_copied.get(), st));
         KLAUNCH(CAT_CONV0, 2, 0.0, launch_decoar2_features(d_wavs, d_lens, B, T, T, 1, w->fb_f32.as<float>(),
                                                            w->ln512_s.planes(m->scheme), st));
         return 0;
@@ -1833,8 +1801,8 @@ int Fwd::decoar_stage(int s) {
     const int NL = m->cfg.num_layers, H = kLstmHidden;
     if (s == 0) {
         const size_t book_bytes = (size_t)(reinterpret_cast<char*>(d_mask) - w->book.as<char>()) + (size_t)M;
-        CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host, book_bytes, cudaMemcpyHostToDevice, st));
-        if (!capturing) CUDA_OK(cudaEventRecord(w->book_copied, st));
+        CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host.get(), book_bytes, cudaMemcpyHostToDevice, st));
+        CUDA_OK(cudaEventRecord(w->book_copied.get(), st));
         KLAUNCH(CAT_CONV0, 2, 0.0, launch_decoar2_features(d_wavs, d_lens, B, T, T, 1, w->fb_f32.as<float>(),
                                                            w->ln512_s.planes(m->scheme), st));
         return 0;
@@ -1879,8 +1847,8 @@ int Fwd::stage(int s) {
     if (s == 0) {
         // ---- bookkeeping copy, waveform packing (+ normalisation), conv 0 + norm + GELU -> act[0] ------------------
         const size_t book_bytes = (size_t)(reinterpret_cast<char*>(d_mask) - w->book.as<char>()) + (size_t)M;
-        CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host, book_bytes, cudaMemcpyHostToDevice, st));
-        if (!capturing) CUDA_OK(cudaEventRecord(w->book_copied, st));  // (graph replay: recorded after the launch)
+        CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host.get(), book_bytes, cudaMemcpyHostToDevice, st));
+        CUDA_OK(cudaEventRecord(w->book_copied.get(), st));
         if (decoar2(m)) {  // fbank frames + CMVN / y[::2] -> post_extract_proj's operand planes (profile category 2)
             KLAUNCH(CAT_CONV0, 2, 0.0, launch_decoar2_features(d_wavs, d_lens, B, (int)fbank_frames(Lmax), T, 2,
                                                                w->fb_f32.as<float>(), w->ln512_s.planes(m->scheme), st));
@@ -2188,96 +2156,29 @@ static int forward_lanes(s3b_model* m, const float* const* wavs, const int64_t* 
     const bool concurrent = lanes == 2 && !m->prof.on;
     if (concurrent) {
         Workspace& w1 = m->ws[1];
-        if (w1.stream == nullptr) CUDA_OK(cudaStreamCreateWithFlags(&w1.stream, cudaStreamNonBlocking));
-        if (w1.done == nullptr) CUDA_OK(cudaEventCreateWithFlags(&w1.done, cudaEventDisableTiming));
-        if (m->fork_event == nullptr) CUDA_OK(cudaEventCreateWithFlags(&m->fork_event, cudaEventDisableTiming));
-        f[1].st = w1.stream;
+        S3B_OK(ensure_stream(w1.stream));
+        S3B_OK(ensure_event(w1.done));
+        S3B_OK(ensure_event(m->fork_event));
+        f[1].st = w1.stream.get();
     }
     for (int i = 0; i < lanes; ++i) S3B_OK(f[i].prepare());
     const int ns = f[0].num_stages();
-    auto enqueue = [&](bool capturing) -> int {
-        for (int i = 0; i < lanes; ++i) f[i].capturing = capturing;
-        if (concurrent) {
-            CUDA_OK(cudaEventRecord(m->fork_event, st));
-            CUDA_OK(cudaStreamWaitEvent(f[1].st, m->fork_event, 0));
-            // lane 1 trails lane 0 by two stages: while one lane runs a GEMM the other tends to be in a different kind
-            // of kernel (attention, LayerNorm, another GEMM shape), which is what lets them share the SMs
-            for (int s = 0; s < ns + 2; ++s) {
-                if (s < ns) S3B_OK(f[0].stage(s));
-                if (s >= 2) S3B_OK(f[1].stage(s - 2));
-            }
-            CUDA_OK(cudaEventRecord(m->ws[1].done, f[1].st));
-            CUDA_OK(cudaStreamWaitEvent(st, m->ws[1].done, 0));
-        } else {
-            for (int i = 0; i < lanes; ++i)
-                for (int s = 0; s < ns; ++s) S3B_OK(f[i].stage(s));
+    if (concurrent) {
+        CUDA_OK(cudaEventRecord(m->fork_event.get(), st));
+        CUDA_OK(cudaStreamWaitEvent(f[1].st, m->fork_event.get(), 0));
+        // lane 1 trails lane 0 by two stages: while one lane runs a GEMM the other tends to be in a different kind
+        // of kernel (attention, LayerNorm, another GEMM shape), which is what lets them share the SMs
+        for (int s = 0; s < ns + 2; ++s) {
+            if (s < ns) S3B_OK(f[0].stage(s));
+            if (s >= 2) S3B_OK(f[1].stage(s - 2));
         }
-        return 0;
-    };
-
-    // ---- CUDA-graph replay (S3B_GRAPHS=1, experimental) ----------------------------------------------------------
-    // A forward is ~100 launches per lane, whose host time can exceed the GPU time of a small per-GPU shard. When the same call (shape, buffers, stream) comes back, the whole two-lane
-    // forward is captured once and replayed with one cudaGraphLaunch; the per-call data (waveform pointers, lengths,
-    // masks) travels through the pinned bookkeeping block, which the graph's copy node re-reads. Any failure while
-    // capturing disables graphs for this model and falls back to plain enqueueing — which is what happens on the
-    // measured driver (580.159 / CUDA 12.9 rejects the capture, presumably the programmatic-dependent-launch
-    // attribute of the first kernel behind a copy node); since the step is GPU-bound even at that size, the mode stays
-    // off by default and was not pursued.
-    static int graphs_env = -1;
-    if (graphs_env < 0) {
-        const char* e = getenv("S3B_GRAPHS");
-        graphs_env = (e != nullptr && e[0] == '1') ? 1 : 0;
+        CUDA_OK(cudaEventRecord(m->ws[1].done.get(), f[1].st));
+        CUDA_OK(cudaStreamWaitEvent(st, m->ws[1].done.get(), 0));
+    } else {
+        for (int i = 0; i < lanes; ++i)
+            for (int s = 0; s < ns; ++s) S3B_OK(f[i].stage(s));
     }
-    if (graphs_env == 1 && !m->graphs_disabled && !m->prof.on) {
-        s3b_model::GraphEntry* ge = nullptr;
-        for (auto& g : m->graphs)
-            if (g.B == B && g.lanes == lanes && g.Lmax == Lmax && g.hidden == hidden_out && g.ffn == ffn_out &&
-                g.last_res == last_res && g.layer_stride == layer_stride && g.ffn_stride == ffn_stride && g.st == st)
-                ge = &g;
-        if (ge == nullptr) {
-            if (m->graphs.size() >= 8) {  // drop the oldest entry
-                if (m->graphs.front().exec) cudaGraphExecDestroy(m->graphs.front().exec);
-                m->graphs.erase(m->graphs.begin());
-            }
-            m->graphs.push_back({B, lanes, Lmax, hidden_out, ffn_out, last_res, layer_stride, ffn_stride, st,
-                                 g_alloc_generation, 0, 0, nullptr});
-            ge = &m->graphs.back();
-        }
-        if (ge->exec != nullptr && ge->gen != g_alloc_generation) {  // a workspace buffer moved: captured pointers are stale
-            cudaGraphExecDestroy(ge->exec);
-            ge->exec = nullptr, ge->hits = 0, ge->gen = g_alloc_generation;
-        }
-        ++ge->hits;
-        if (ge->exec == nullptr && ge->hits >= 3) {  // third identical call: worth capturing
-            const long long before = m->launches_total;
-            cudaGraph_t graph = nullptr;
-            bool ok = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
-            if (ok) {
-                const int r = enqueue(true);
-                const cudaError_t ce = cudaStreamEndCapture(st, &graph);
-                ok = r == 0 && ce == cudaSuccess && graph != nullptr;
-            }
-            if (ok) ok = cudaGraphInstantiate(&ge->exec, graph, 0) == cudaSuccess;
-            if (graph) cudaGraphDestroy(graph);
-            ge->launches = m->launches_total - before;
-            m->launches_total = before;
-            if (!ok) {
-                cudaGetLastError();
-                if (ge->exec) cudaGraphExecDestroy(ge->exec);
-                ge->exec = nullptr;
-                m->graphs_disabled = true;
-                fprintf(stderr, "s3prl_b200: CUDA-graph capture of the forward failed (%s); continuing without graphs\n",
-                        g_last_error.c_str());
-            }
-        }
-        if (ge->exec != nullptr) {
-            CUDA_OK(cudaGraphLaunch(ge->exec, st));
-            for (int i = 0; i < lanes; ++i) CUDA_OK(cudaEventRecord(m->ws[i].book_copied, st));  // mirrors consumed by then
-            m->launches_total += ge->launches;
-            return 0;
-        }
-    }
-    return enqueue(false);
+    return 0;
 }
 
 extern "C" int s3b_forward(s3b_model* m, const float* const* wavs, const int64_t* lens, int32_t batch,
@@ -2319,14 +2220,14 @@ static int forward_host_impl(s3b_model* m, const float* const* wavs, const int64
         S3B_OK(m->stage_out.ensure((size_t)s3b_num_outputs(m) * layer_elems * 4));
         hidden_dev = m->stage_out.as<float>();
     }
-    if (m->copy_stream == nullptr) CUDA_OK(cudaStreamCreateWithFlags(&m->copy_stream, cudaStreamNonBlocking));
-    if (m->compute_stream == nullptr) CUDA_OK(cudaStreamCreateWithFlags(&m->compute_stream, cudaStreamNonBlocking));
+    S3B_OK(ensure_stream(m->copy_stream));
+    S3B_OK(ensure_stream(m->compute_stream));
     while ((int)m->layer_events.size() < s3b_num_outputs(m)) {
-        cudaEvent_t e;
-        CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-        m->layer_events.push_back(e);
+        Event e;
+        S3B_OK(ensure_event(e));
+        m->layer_events.push_back(std::move(e));
     }
-    cudaStream_t st = m->compute_stream;
+    cudaStream_t st = m->compute_stream.get();
     std::vector<const float*> ptrs(batch);
     size_t off = 0;
     for (int b = 0; b < batch; ++b) {
@@ -2349,10 +2250,10 @@ static int forward_host_impl(s3b_model* m, const float* const* wavs, const int64
     };
     auto layer_done = [](s3b_model* mm, int l, cudaStream_t s, void* user) -> int {
         Ctx* c = static_cast<Ctx*>(user);
-        CUDA_OK(cudaEventRecord(mm->layer_events[l], s));
-        CUDA_OK(cudaStreamWaitEvent(mm->copy_stream, mm->layer_events[l], 0));
+        CUDA_OK(cudaEventRecord(mm->layer_events[l].get(), s));
+        CUDA_OK(cudaStreamWaitEvent(mm->copy_stream.get(), mm->layer_events[l].get(), 0));
         CUDA_OK(cudaMemcpyAsync(c->host + (size_t)l * c->layer, c->dev + (size_t)l * c->layer, c->chunk * 4,
-                                cudaMemcpyDeviceToHost, mm->copy_stream));
+                                cudaMemcpyDeviceToHost, mm->copy_stream.get()));
         return 0;
     };
     // default: two chunks from 16 utterances on (first-output latency ~ half, GEMMs at 16 utterances still run at
@@ -2374,7 +2275,7 @@ static int forward_host_impl(s3b_model* m, const float* const* wavs, const int64
         for (int s = 0; s < f.num_stages(); ++s) S3B_OK(f.stage(s));
     }
     CUDA_OK(cudaStreamSynchronize(st));
-    CUDA_OK(cudaStreamSynchronize(m->copy_stream));
+    CUDA_OK(cudaStreamSynchronize(m->copy_stream.get()));
     return 0;
 }
 
@@ -2408,10 +2309,10 @@ extern "C" int s3b_profile_read_ex(s3b_model* m, int32_t num_categories, double*
     CUDA_OK(cudaDeviceSynchronize());
     for (ProfRec& r : m->prof.recs) {
         float t = 0.f;
-        CUDA_OK(cudaEventElapsedTime(&t, r.a, r.b));
+        CUDA_OK(cudaEventElapsedTime(&t, r.a.get(), r.b.get()));
         m->prof.ms[r.cat] += t;
-        m->prof.pool.push_back(r.a);
-        m->prof.pool.push_back(r.b);
+        m->prof.pool.push_back(std::move(r.a));
+        m->prof.pool.push_back(std::move(r.b));
     }
     m->prof.recs.clear();
     for (int c = 0; c < CAT_COUNT; ++c) {
@@ -2473,6 +2374,14 @@ struct s3b_peer {
     size_t bytes = 0, flags_off = 0, counter_off = 0;
     std::vector<void*> peer_base;  // every rank's allocation as mapped in THIS process (own: base)
     bool connected = false;
+    s3b_peer() = default;
+    s3b_peer(const s3b_peer&) = delete;
+    s3b_peer& operator=(const s3b_peer&) = delete;
+    ~s3b_peer() {
+        for (int r = 0; r < (int)peer_base.size(); ++r)
+            if (r != rank && peer_base[r]) cudaIpcCloseMemHandle(peer_base[r]);
+        if (base) cudaFree(base);
+    }
 };
 
 extern "C" int s3b_peer_create(int32_t rank, int32_t world, int64_t block_elems, int32_t slots, s3b_peer** out,
@@ -2495,7 +2404,6 @@ extern "C" int s3b_peer_create(int32_t rank, int32_t world, int64_t block_elems,
     cudaIpcMemHandle_t h;
     if (e == cudaSuccess) e = cudaIpcGetMemHandle(&h, p->base);
     if (e != cudaSuccess) {
-        if (p->base) cudaFree(p->base);
         delete p;
         return fail("peer buffer allocation / IPC export failed: %s", cudaGetErrorString(e));
     }
@@ -2560,13 +2468,7 @@ extern "C" int s3b_peer_wait(s3b_peer* p, uint32_t step, void* stream) {
     return 0;
 }
 
-extern "C" void s3b_peer_destroy(s3b_peer* p) {
-    if (!p) return;
-    for (int r = 0; r < p->world; ++r)
-        if (r != p->rank && p->peer_base[r]) cudaIpcCloseMemHandle(p->peer_base[r]);
-    if (p->base) cudaFree(p->base);
-    delete p;
-}
+extern "C" void s3b_peer_destroy(s3b_peer* p) { delete p; }
 
 // ------------------------------------------------------------------------------------------------
 // building blocks for parity tests
@@ -2636,30 +2538,26 @@ extern "C" int s3b_linear_ex(const float* a, const float* w, const float* bias, 
     S3B_OK(device_sm_count(&sms));
     g_sm_count = sms;  // the tile-width choice a model finalized on this device makes
     SplitBuf as, ws, os;
+    S3B_OK(split_operand(a, as, (size_t)M * lda, scheme, 0, st));
+    S3B_OK(split_operand(w, ws, (size_t)N * K, scheme, 1, st));
     GemmParams p;
-    const int r = [&]() -> int {
-        S3B_OK(split_operand(a, as, (size_t)M * lda, scheme, 0, st));
-        S3B_OK(split_operand(w, ws, (size_t)N * K, scheme, 1, st));
-        S3B_OK(linear_params(p, as, ws, M, N, K, scheme, lda, (size_t)o.a_off, o.tile_n));
-        if (o.tile_n != 0 && p.bn != o.tile_n) return fail("tile_n %d requested, %d chosen", o.tile_n, p.bn);
-        Epi e;
-        e.bias = bias, e.residual = residual, e.gelu = gelu, e.row_mask = o.row_mask;
-        if (o.out_fmt < 0) {
-            e.out_f32 = out;
-        } else {
-            S3B_OK(os.ensure((size_t)M * N));
-            e.op = os.planes(o.out_fmt);
-        }
-        set_epi(p, e, N);
-        p.out_pre = o.out_pre;
-        CUDA_OK(launch_gemm(p, sms, st));
-        if (o.out_fmt >= 0) CUDA_OK(launch_planes_to_f32(os.planes(o.out_fmt), (size_t)M * N, out, st));
-        CUDA_OK(cudaStreamSynchronize(st));
-        return 0;
-    }();
-    as.release(), ws.release(), os.release();
-    if (r == 0 && opts != nullptr) opts->scheme_used = scheme, opts->tile_n_used = p.bn;
-    return r;
+    S3B_OK(linear_params(p, as, ws, M, N, K, scheme, lda, (size_t)o.a_off, o.tile_n));
+    if (o.tile_n != 0 && p.bn != o.tile_n) return fail("tile_n %d requested, %d chosen", o.tile_n, p.bn);
+    Epi e;
+    e.bias = bias, e.residual = residual, e.gelu = gelu, e.row_mask = o.row_mask;
+    if (o.out_fmt < 0) {
+        e.out_f32 = out;
+    } else {
+        S3B_OK(os.ensure((size_t)M * N));
+        e.op = os.planes(o.out_fmt);
+    }
+    set_epi(p, e, N);
+    p.out_pre = o.out_pre;
+    CUDA_OK(launch_gemm(p, sms, st));
+    if (o.out_fmt >= 0) CUDA_OK(launch_planes_to_f32(os.planes(o.out_fmt), (size_t)M * N, out, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    if (opts != nullptr) opts->scheme_used = scheme, opts->tile_n_used = p.bn;
+    return 0;
 }
 
 extern "C" int s3b_linear_f32(const float* a, const float* w, const float* bias, const float* residual, int64_t M,
@@ -2681,24 +2579,20 @@ extern "C" int s3b_qkv_hd_f32(const float* x, const float* w, const float* b, in
     S3B_OK(device_sm_count(&sms));
     g_sm_count = sms;
     SplitBuf xs, ws, qs, ks, vts;
-    const int r = [&]() -> int {
-        S3B_OK(split_operand(x, xs, (size_t)M * D, sch, 0, st));
-        S3B_OK(split_operand(w, ws, (size_t)3 * D * D, sch, 1, st));
-        S3B_OK(qs.ensure((size_t)M * D));
-        S3B_OK(ks.ensure((size_t)M * D));
-        S3B_OK(vts.ensure((size_t)B * D * Tp));
-        GemmParams p;
-        S3B_OK(linear_params(p, xs, ws, M, 3 * D, D, sch));
-        set_qkv_epi(p, b, T, H, hd, qs, ks, vts);
-        CUDA_OK(launch_gemm(p, sms, st));
-        CUDA_OK(launch_planes_to_f32(qs.planes(0), (size_t)M * D, q_out, st));
-        CUDA_OK(launch_planes_to_f32(ks.planes(0), (size_t)M * D, k_out, st));
-        CUDA_OK(launch_planes_to_f32(vts.planes(0), (size_t)B * D * Tp, vt_out, st));
-        CUDA_OK(cudaStreamSynchronize(st));
-        return 0;
-    }();
-    xs.release(), ws.release(), qs.release(), ks.release(), vts.release();
-    return r;
+    S3B_OK(split_operand(x, xs, (size_t)M * D, sch, 0, st));
+    S3B_OK(split_operand(w, ws, (size_t)3 * D * D, sch, 1, st));
+    S3B_OK(qs.ensure((size_t)M * D));
+    S3B_OK(ks.ensure((size_t)M * D));
+    S3B_OK(vts.ensure((size_t)B * D * Tp));
+    GemmParams p;
+    S3B_OK(linear_params(p, xs, ws, M, 3 * D, D, sch));
+    set_qkv_epi(p, b, T, H, hd, qs, ks, vts);
+    CUDA_OK(launch_gemm(p, sms, st));
+    CUDA_OK(launch_planes_to_f32(qs.planes(0), (size_t)M * D, q_out, st));
+    CUDA_OK(launch_planes_to_f32(ks.planes(0), (size_t)M * D, k_out, st));
+    CUDA_OK(launch_planes_to_f32(vts.planes(0), (size_t)B * D * Tp, vt_out, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
 }
 
 extern "C" int s3b_qkv_f32(const float* x, const float* w, const float* b, int32_t B, int32_t T, int32_t H,
@@ -2720,30 +2614,26 @@ extern "C" int s3b_conv_gemm_f32(const float* x, const float* w, const float* bi
     int sms = 0;
     S3B_OK(device_sm_count(&sms));
     SplitBuf xs, ws, os;
-    const int r = [&]() -> int {
-        std::vector<float> wh;
-        S3B_OK(download_f32(w, (size_t)C * C * kw, st, wh));
-        const std::vector<float> wl = conv_weight_layout(wh.data(), kw);
-        S3B_OK(upload_split(ws, wl.data(), wl.size(), sch));
-        S3B_OK(split_operand(x, xs, (size_t)B * Lin * C, sch, 0, st));
-        GemmParams p;
-        S3B_OK(conv_params(p, xs, ws, B, Lin, Lout, kw, sch));
-        Epi e;
-        e.bias = bias, e.gelu = gelu;
-        if (out_fmt < 0) {
-            e.out_f32 = out;
-        } else {
-            S3B_OK(os.ensure((size_t)B * Lout * C));
-            e.op = os.planes(out_fmt);
-        }
-        set_epi(p, e, C);
-        CUDA_OK(launch_gemm(p, sms, st));
-        if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), (size_t)B * Lout * C, out, st));
-        CUDA_OK(cudaStreamSynchronize(st));
-        return 0;
-    }();
-    xs.release(), ws.release(), os.release();
-    return r;
+    std::vector<float> wh;
+    S3B_OK(download_f32(w, (size_t)C * C * kw, st, wh));
+    const std::vector<float> wl = conv_weight_layout(wh.data(), kw);
+    S3B_OK(upload_split(ws, wl.data(), wl.size(), sch));
+    S3B_OK(split_operand(x, xs, (size_t)B * Lin * C, sch, 0, st));
+    GemmParams p;
+    S3B_OK(conv_params(p, xs, ws, B, Lin, Lout, kw, sch));
+    Epi e;
+    e.bias = bias, e.gelu = gelu;
+    if (out_fmt < 0) {
+        e.out_f32 = out;
+    } else {
+        S3B_OK(os.ensure((size_t)B * Lout * C));
+        e.op = os.planes(out_fmt);
+    }
+    set_epi(p, e, C);
+    CUDA_OK(launch_gemm(p, sms, st));
+    if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), (size_t)B * Lout * C, out, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
 }
 
 extern "C" int s3b_posconv_f32(const float* x, const float* w, const float* bias, int32_t B, int32_t T, int32_t D,
@@ -2776,50 +2666,46 @@ extern "C" int s3b_posconv_f32(const float* x, const float* w, const float* bias
     S3B_OK(device_sm_count(&sms));
     SplitBuf xs, ws, os;
     DevBuf z;
-    const int r = [&]() -> int {
-        std::vector<float> wh;
-        S3B_OK(download_f32(w, (size_t)D * cpg * k, st, wh));
-        const std::vector<float> wl =
-            taps == 4 ? posconv4_weight_layout(wh.data(), D, G, k) : posconv_weight_layout(wh.data(), D, G, k);
-        S3B_OK(upload_split(ws, wl.data(), wl.size()));
-        S3B_OK(split_operand(x, xs, M * D, 0, 0, st));
-        OutPlanes op = no_planes();
-        if (out_fmt >= 0) {
-            S3B_OK(os.ensure(M * D));
-            op = os.planes(out_fmt);
-        }
-        float* out_f32 = out_fmt < 0 ? out : nullptr;
-        GemmParams p;
-        Epi e;
-        if (taps == 4) {
-            // Fwd::stage(8): Z = the four-tap GEMM, then the combine kernel (+ LayerNorm)
-            S3B_OK(z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
-            S3B_OK(posconv4_params(p, c, xs.h(), xs.l(), ws.h(), ws.l(), B, T));
+    std::vector<float> wh;
+    S3B_OK(download_f32(w, (size_t)D * cpg * k, st, wh));
+    const std::vector<float> wl =
+        taps == 4 ? posconv4_weight_layout(wh.data(), D, G, k) : posconv_weight_layout(wh.data(), D, G, k);
+    S3B_OK(upload_split(ws, wl.data(), wl.size()));
+    S3B_OK(split_operand(x, xs, M * D, 0, 0, st));
+    OutPlanes op = no_planes();
+    if (out_fmt >= 0) {
+        S3B_OK(os.ensure(M * D));
+        op = os.planes(out_fmt);
+    }
+    float* out_f32 = out_fmt < 0 ? out : nullptr;
+    GemmParams p;
+    Epi e;
+    if (taps == 4) {
+        // Fwd::stage(8): Z = the four-tap GEMM, then the combine kernel (+ LayerNorm)
+        S3B_OK(z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
+        S3B_OK(posconv4_params(p, c, xs.h(), xs.l(), ws.h(), ws.l(), B, T));
+        e.out_f32 = z.as<float>();
+        set_epi(p, e, 4 * D);
+        CUDA_OK(launch_gemm(p, sms, st));
+        CUDA_OK(launch_posconv_combine(z.as<float>(), x, bias, B, T, D, cpg, gamma, beta, gamma ? 1 : 0, mode,
+                                       out_f32, op, st));
+    } else {
+        // Fwd::stage(8), one tap per k-block: x + GELU(conv + bias) in the epilogue, then the LayerNorm
+        S3B_OK(posconv_params(p, c, xs.h(), xs.l(), ws.h(), ws.l(), B, T));
+        e.bias = bias, e.gelu = 1, e.residual = x;
+        if (gamma != nullptr) {
+            S3B_OK(z.ensure(M * D * sizeof(float)));
             e.out_f32 = z.as<float>();
-            set_epi(p, e, 4 * D);
-            CUDA_OK(launch_gemm(p, sms, st));
-            CUDA_OK(launch_posconv_combine(z.as<float>(), x, bias, B, T, D, cpg, gamma, beta, gamma ? 1 : 0, mode,
-                                           out_f32, op, st));
         } else {
-            // Fwd::stage(8), one tap per k-block: x + GELU(conv + bias) in the epilogue, then the LayerNorm
-            S3B_OK(posconv_params(p, c, xs.h(), xs.l(), ws.h(), ws.l(), B, T));
-            e.bias = bias, e.gelu = 1, e.residual = x;
-            if (gamma != nullptr) {
-                S3B_OK(z.ensure(M * D * sizeof(float)));
-                e.out_f32 = z.as<float>();
-            } else {
-                e.out_f32 = out_f32;
-            }
-            set_epi(p, e, D);
-            CUDA_OK(launch_gemm(p, sms, st));
-            if (gamma != nullptr) CUDA_OK(launch_layernorm(z.as<float>(), M, D, gamma, beta, 0, out_f32, op, st));
+            e.out_f32 = out_f32;
         }
-        if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(op, M * D, out, st));
-        CUDA_OK(cudaStreamSynchronize(st));
-        return 0;
-    }();
-    xs.release(), ws.release(), os.release(), z.release();
-    return r;
+        set_epi(p, e, D);
+        CUDA_OK(launch_gemm(p, sms, st));
+        if (gamma != nullptr) CUDA_OK(launch_layernorm(z.as<float>(), M, D, gamma, beta, 0, out_f32, op, st));
+    }
+    if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(op, M * D, out, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
 }
 
 // Times `iters` back-to-back launches of the production GEMM (bias + GELU + split epilogue like fc1 when gelu != 0,
@@ -2844,29 +2730,26 @@ extern "C" int s3b_gemm_bench(int64_t M, int32_t N, int32_t K, int32_t gelu, int
     GemmParams p;
     int scheme = default_scheme();
     if (K % 128 != 0 || N % 128 != 0) scheme = 0;
-    int r = linear_params(p, as, ws, M, N, K, scheme, 0, 0, force_un);
-    if (r == 0) {
-        Epi e;
-        e.bias = bias.as<float>();
-        if (gelu) e.gelu = 1, e.op = os.planes(scheme);
-        else e.residual = res.as<float>(), e.out_f32 = out.as<float>();
-        set_epi(p, e, N);
-        cudaEvent_t e0, e1;
-        cudaEventCreate(&e0), cudaEventCreate(&e1);
-        for (int i = 0; i < 3; ++i) launch_gemm(p, sms, 0);
-        cudaEventRecord(e0, 0);
-        for (int i = 0; i < iters; ++i) launch_gemm(p, sms, 0);
-        cudaEventRecord(e1, 0);
-        cudaError_t ce = cudaDeviceSynchronize();
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, e0, e1);
-        *ms_per_launch = ms / iters;
-        cudaEventDestroy(e0), cudaEventDestroy(e1);
-        if (ce != cudaSuccess) r = fail("gemm bench failed: %s", cudaGetErrorString(ce));
-        else if (ms_per_launch[0] >= 0) ms_per_launch[1] = (float)p.bn;
-    }
-    as.release(), ws.release(), os.release(), bias.release(), res.release(), out.release();
-    return r;
+    S3B_OK(linear_params(p, as, ws, M, N, K, scheme, 0, 0, force_un));
+    Epi e;
+    e.bias = bias.as<float>();
+    if (gelu) e.gelu = 1, e.op = os.planes(scheme);
+    else e.residual = res.as<float>(), e.out_f32 = out.as<float>();
+    set_epi(p, e, N);
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    cudaEventCreate(&e0), cudaEventCreate(&e1);
+    const Event t0(e0), t1(e1);
+    for (int i = 0; i < 3; ++i) launch_gemm(p, sms, 0);
+    cudaEventRecord(e0, 0);
+    for (int i = 0; i < iters; ++i) launch_gemm(p, sms, 0);
+    cudaEventRecord(e1, 0);
+    cudaError_t ce = cudaDeviceSynchronize();
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, e0, e1);
+    *ms_per_launch = ms / iters;
+    if (ce != cudaSuccess) return fail("gemm bench failed: %s", cudaGetErrorString(ce));
+    if (ms_per_launch[0] >= 0) ms_per_launch[1] = (float)p.bn;
+    return 0;
 }
 
 extern "C" int s3b_layernorm_f32(const float* x, int64_t M, int32_t D, const float* gamma, const float* beta,
@@ -2948,11 +2831,9 @@ extern "C" int s3b_attention_ex(const float* q, const float* k, const float* v, 
                 for (int sl = 0; sl < 8; ++sl) fprintf(stderr, " %7lld", h[(role * 16 + j) * 8 + sl] ? h[(role * 16 + j) * 8 + sl] - t0 : -1);
                 fprintf(stderr, "\n");
             }
-        trace.release();
     }
     CUDA_OK(launch_planes_to_f32(ctx.planes(o.ctx_format), M * D, out, st));
-    cudaError_t se = cudaStreamSynchronize(st);
-    qs.release(), ks.release(), vts.release(), ctx.release(), kv.release(), table.release();
+    const cudaError_t se = cudaStreamSynchronize(st);  // before the buffers are freed
     if (se != cudaSuccess) return fail("attention execution failed: %s", cudaGetErrorString(se));
     return 0;
 }
@@ -2978,8 +2859,7 @@ extern "C" int s3b_wavlm_gate_f32(const float* x, int32_t B, int32_t T, int32_t 
     if (x_format != 0) CUDA_OK(launch_split_q8(x, xs.h(), xs.h8(), xs.l8(), M * D, 0, st));
     else CUDA_OK(launch_split(x, xs.h(), xs.l(), M * D, st));
     CUDA_OK(launch_wavlm_gate(xs.planes(x_format), M, B, T, H, D, grep_w, grep_b, grep_a, gate_out, st));
-    cudaError_t se = cudaStreamSynchronize(st);
-    xs.release();
+    const cudaError_t se = cudaStreamSynchronize(st);  // before xs is freed
     if (se != cudaSuccess) return fail("gate execution failed: %s", cudaGetErrorString(se));
     return 0;
 }
@@ -3006,30 +2886,26 @@ extern "C" int s3b_frontend_f32(const float* const* wavs, const int64_t* lens, i
     cudaStream_t st = (cudaStream_t)stream;
     DevBuf book, pad, stats, part, ss;
     SplitBuf os;
-    const int r = [&]() -> int {
-        S3B_OK(book.ensure((size_t)B * (sizeof(void*) + sizeof(long long))));
-        std::vector<long long> hl(lens, lens + B);
-        CUDA_OK(cudaMemcpyAsync(book.p, wavs, (size_t)B * sizeof(void*), cudaMemcpyHostToDevice, st));
-        long long* d_lens = reinterpret_cast<long long*>(book.as<char>() + (size_t)B * sizeof(void*));
-        CUDA_OK(cudaMemcpyAsync(d_lens, hl.data(), (size_t)B * sizeof(long long), cudaMemcpyHostToDevice, st));
-        float* wav_pad = wav_out;
-        if (wav_pad == nullptr) {
-            S3B_OK(pad.ensure((size_t)B * max_len * 4));
-            wav_pad = pad.as<float>();
-        }
-        S3B_OK(stats.ensure((size_t)B * 2 * 4));
-        S3B_OK(part.ensure(conv0_ws_part_bytes(B, (int)L0)));
-        S3B_OK(ss.ensure((size_t)2 * B * kConvDim * 4));
-        S3B_OK(os.ensure((size_t)B * L0 * kConvDim));
-        S3B_OK(launch_frontend(nullptr, st, book.as<const float*>(), d_lens, B, max_len, (int)L0, normalize, w, bias,
-                               gamma, beta, layer_norm, wav_pad, stats.as<float>(), part.as<double>(), ss.as<float>(),
-                               os.planes(out_fmt)));
-        CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), (size_t)B * L0 * kConvDim, out, st));
-        CUDA_OK(cudaStreamSynchronize(st));
-        return 0;
-    }();
-    book.release(), pad.release(), stats.release(), part.release(), ss.release(), os.release();
-    return r;
+    S3B_OK(book.ensure((size_t)B * (sizeof(void*) + sizeof(long long))));
+    std::vector<long long> hl(lens, lens + B);
+    CUDA_OK(cudaMemcpyAsync(book.p, wavs, (size_t)B * sizeof(void*), cudaMemcpyHostToDevice, st));
+    long long* d_lens = reinterpret_cast<long long*>(book.as<char>() + (size_t)B * sizeof(void*));
+    CUDA_OK(cudaMemcpyAsync(d_lens, hl.data(), (size_t)B * sizeof(long long), cudaMemcpyHostToDevice, st));
+    float* wav_pad = wav_out;
+    if (wav_pad == nullptr) {
+        S3B_OK(pad.ensure((size_t)B * max_len * 4));
+        wav_pad = pad.as<float>();
+    }
+    S3B_OK(stats.ensure((size_t)B * 2 * 4));
+    S3B_OK(part.ensure(conv0_ws_part_bytes(B, (int)L0)));
+    S3B_OK(ss.ensure((size_t)2 * B * kConvDim * 4));
+    S3B_OK(os.ensure((size_t)B * L0 * kConvDim));
+    S3B_OK(launch_frontend(nullptr, st, book.as<const float*>(), d_lens, B, max_len, (int)L0, normalize, w, bias,
+                           gamma, beta, layer_norm, wav_pad, stats.as<float>(), part.as<double>(), ss.as<float>(),
+                           os.planes(out_fmt)));
+    CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), (size_t)B * L0 * kConvDim, out, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
 }
 
 // Fwd::stage(0) of a DeCoAR 2.0 (step 2) or APC (step 1) model on workspaces of this call; the operand planes
@@ -3056,25 +2932,21 @@ static int fbank_cmvn_features(const float* const* wavs, const int64_t* lens, in
     const size_t rows = (size_t)B * T;
     DevBuf book, fbuf, dec;
     SplitBuf os;
-    const int r = [&]() -> int {
-        S3B_OK(book.ensure((size_t)B * (sizeof(void*) + sizeof(long long))));
-        std::vector<long long> hl(lens, lens + B);
-        CUDA_OK(cudaMemcpyAsync(book.p, wavs, (size_t)B * sizeof(void*), cudaMemcpyHostToDevice, st));
-        long long* d_lens = reinterpret_cast<long long*>(book.as<char>() + (size_t)B * sizeof(void*));
-        CUDA_OK(cudaMemcpyAsync(d_lens, hl.data(), (size_t)B * sizeof(long long), cudaMemcpyHostToDevice, st));
-        S3B_OK(fbuf.ensure((size_t)B * mf * 80 * 4));
-        S3B_OK(os.ensure(rows * kDecoar2K));
-        S3B_OK(dec.ensure(rows * kDecoar2K * 4));
-        CUDA_OK(launch_decoar2_features(book.as<const float*>(), d_lens, B, (int)mf, (int)T, step, fbuf.as<float>(),
-                                        os.planes(out_fmt), st));
-        CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), rows * kDecoar2K, dec.as<float>(), st));
-        CUDA_OK(cudaMemcpy2DAsync(out, 80 * sizeof(float), dec.p, kDecoar2K * sizeof(float), 80 * sizeof(float), rows,
-                                  cudaMemcpyDeviceToDevice, st));
-        CUDA_OK(cudaStreamSynchronize(st));
-        return 0;
-    }();
-    book.release(), fbuf.release(), dec.release(), os.release();
-    return r;
+    S3B_OK(book.ensure((size_t)B * (sizeof(void*) + sizeof(long long))));
+    std::vector<long long> hl(lens, lens + B);
+    CUDA_OK(cudaMemcpyAsync(book.p, wavs, (size_t)B * sizeof(void*), cudaMemcpyHostToDevice, st));
+    long long* d_lens = reinterpret_cast<long long*>(book.as<char>() + (size_t)B * sizeof(void*));
+    CUDA_OK(cudaMemcpyAsync(d_lens, hl.data(), (size_t)B * sizeof(long long), cudaMemcpyHostToDevice, st));
+    S3B_OK(fbuf.ensure((size_t)B * mf * 80 * 4));
+    S3B_OK(os.ensure(rows * kDecoar2K));
+    S3B_OK(dec.ensure(rows * kDecoar2K * 4));
+    CUDA_OK(launch_decoar2_features(book.as<const float*>(), d_lens, B, (int)mf, (int)T, step, fbuf.as<float>(),
+                                    os.planes(out_fmt), st));
+    CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), rows * kDecoar2K, dec.as<float>(), st));
+    CUDA_OK(cudaMemcpy2DAsync(out, 80 * sizeof(float), dec.p, kDecoar2K * sizeof(float), 80 * sizeof(float), rows,
+                              cudaMemcpyDeviceToDevice, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
 }
 
 extern "C" int s3b_decoar2_features_f32(const float* const* wavs, const int64_t* lens, int32_t B, int32_t out_fmt,
@@ -3114,34 +2986,30 @@ extern "C" int s3b_gru_f32(const float* xg, const float* whh, const float* bhh, 
     const size_t M = (size_t)B * T;
     DevBuf xgc, bk;
     SplitBuf os;
-    const int r = [&]() -> int {
-        std::vector<int> host(2 * (size_t)B);
-        memcpy(host.data(), lens, (size_t)B * sizeof(int));
-        std::vector<int> ord(B);
-        for (int b = 0; b < B; ++b) ord[b] = b;
-        std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return lens[a] > lens[b]; });
-        memcpy(host.data() + B, ord.data(), (size_t)B * sizeof(int));
-        S3B_OK(bk.ensure(host.size() * sizeof(int)));
-        CUDA_OK(cudaMemcpyAsync(bk.p, host.data(), host.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-        S3B_OK(xgc.ensure(M * 3 * H * 4));
-        CUDA_OK(cudaMemcpyAsync(xgc.p, xg, M * 3 * H * 4, cudaMemcpyDeviceToDevice, st));
-        CUDA_OK(launch_gru_fold_bias(xgc.as<float>(), bhh, M, st));
-        GruParams g;
-        g.xg = xgc.as<float>(), g.whh = whh, g.bhn = bhh + 2 * H, g.res = residual;
-        g.len = bk.as<int>(), g.order = bk.as<int>() + B, g.B = B, g.T = T;
-        g.out = out;
-        g.op = no_planes();
-        if (out_fmt >= 0) {
-            S3B_OK(os.ensure(M * H));
-            g.op = os.planes(out_fmt);
-        }
-        CUDA_OK(launch_gru(g, st));
-        if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(g.op, M * H, planes_out, st));
-        CUDA_OK(cudaStreamSynchronize(st));
-        return 0;
-    }();
-    xgc.release(), bk.release(), os.release();
-    return r;
+    std::vector<int> host(2 * (size_t)B);
+    memcpy(host.data(), lens, (size_t)B * sizeof(int));
+    std::vector<int> ord(B);
+    for (int b = 0; b < B; ++b) ord[b] = b;
+    std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return lens[a] > lens[b]; });
+    memcpy(host.data() + B, ord.data(), (size_t)B * sizeof(int));
+    S3B_OK(bk.ensure(host.size() * sizeof(int)));
+    CUDA_OK(cudaMemcpyAsync(bk.p, host.data(), host.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    S3B_OK(xgc.ensure(M * 3 * H * 4));
+    CUDA_OK(cudaMemcpyAsync(xgc.p, xg, M * 3 * H * 4, cudaMemcpyDeviceToDevice, st));
+    CUDA_OK(launch_gru_fold_bias(xgc.as<float>(), bhh, M, st));
+    GruParams g;
+    g.xg = xgc.as<float>(), g.whh = whh, g.bhn = bhh + 2 * H, g.res = residual;
+    g.len = bk.as<int>(), g.order = bk.as<int>() + B, g.B = B, g.T = T;
+    g.out = out;
+    g.op = no_planes();
+    if (out_fmt >= 0) {
+        S3B_OK(os.ensure(M * H));
+        g.op = os.planes(out_fmt);
+    }
+    CUDA_OK(launch_gru(g, st));
+    if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(g.op, M * H, planes_out, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
 }
 
 extern "C" int s3b_lstm_fits(int32_t* out) {
@@ -3173,34 +3041,30 @@ extern "C" int s3b_lstm_f32(const float* xg, const float* whh, const float* bhh,
     const size_t M = (size_t)B * T;
     DevBuf bk, hb, sync;
     SplitBuf os;
-    const int r = [&]() -> int {
-        std::vector<int> host(2 * (size_t)B);
-        memcpy(host.data(), lens, (size_t)B * sizeof(int));
-        std::vector<int> ord(B);
-        for (int b = 0; b < B; ++b) ord[b] = b;
-        std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return lens[a] > lens[b]; });
-        memcpy(host.data() + B, ord.data(), (size_t)B * sizeof(int));
-        S3B_OK(bk.ensure(host.size() * sizeof(int)));
-        CUDA_OK(cudaMemcpyAsync(bk.p, host.data(), host.size() * sizeof(int), cudaMemcpyHostToDevice, st));
-        S3B_OK(hb.ensure(lstm_hbuf_floats(B) * 4));
-        S3B_OK(sync.ensure(sizeof(unsigned int)));
-        LstmParams g;
-        g.xg = xg, g.whh = whh, g.bhh = bhh;
-        g.len = bk.as<int>(), g.order = bk.as<int>() + B, g.B = B, g.T = T, g.direction = direction;
-        g.out = out, g.ldo = 2 * H, g.col0 = direction * H;
-        g.op = no_planes();
-        if (out_fmt >= 0) {
-            S3B_OK(os.ensure(M * 2 * H));
-            g.op = os.planes(out_fmt);
-        }
-        g.hbuf = hb.as<float>(), g.counter = sync.as<unsigned int>();
-        CUDA_OK(launch_lstm(g, st));
-        if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(g.op, M * 2 * H, planes_out, st));
-        CUDA_OK(cudaStreamSynchronize(st));
-        return 0;
-    }();
-    bk.release(), hb.release(), sync.release(), os.release();
-    return r;
+    std::vector<int> host(2 * (size_t)B);
+    memcpy(host.data(), lens, (size_t)B * sizeof(int));
+    std::vector<int> ord(B);
+    for (int b = 0; b < B; ++b) ord[b] = b;
+    std::stable_sort(ord.begin(), ord.end(), [&](int a, int b) { return lens[a] > lens[b]; });
+    memcpy(host.data() + B, ord.data(), (size_t)B * sizeof(int));
+    S3B_OK(bk.ensure(host.size() * sizeof(int)));
+    CUDA_OK(cudaMemcpyAsync(bk.p, host.data(), host.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    S3B_OK(hb.ensure(lstm_hbuf_floats(B) * 4));
+    S3B_OK(sync.ensure(sizeof(unsigned int)));
+    LstmParams g;
+    g.xg = xg, g.whh = whh, g.bhh = bhh;
+    g.len = bk.as<int>(), g.order = bk.as<int>() + B, g.B = B, g.T = T, g.direction = direction;
+    g.out = out, g.ldo = 2 * H, g.col0 = direction * H;
+    g.op = no_planes();
+    if (out_fmt >= 0) {
+        S3B_OK(os.ensure(M * 2 * H));
+        g.op = os.planes(out_fmt);
+    }
+    g.hbuf = hb.as<float>(), g.counter = sync.as<unsigned int>();
+    CUDA_OK(launch_lstm(g, st));
+    if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(g.op, M * 2 * H, planes_out, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
 }
 
 extern "C" int s3b_conformer_conv_f32(const float* x, int32_t B, int32_t T, int32_t D, int32_t k, const float* dw_w,
@@ -3216,24 +3080,20 @@ extern "C" int s3b_conformer_conv_f32(const float* x, int32_t B, int32_t T, int3
     const size_t M = (size_t)B * T;
     DevBuf wb, bb;
     SplitBuf os;
-    const int r = [&]() -> int {
-        std::vector<float> w, g, be, mu, var, wf, bf;
-        S3B_OK(download_f32(dw_w, (size_t)D * k, st, w));
-        S3B_OK(download_f32(bn_gamma, D, st, g));
-        S3B_OK(download_f32(bn_beta, D, st, be));
-        S3B_OK(download_f32(bn_mean, D, st, mu));
-        S3B_OK(download_f32(bn_var, D, st, var));
-        fold_depthwise_bn(w.data(), g.data(), be.data(), mu.data(), var.data(), D, k, wf, bf);
-        S3B_OK(upload_f32(wb, wf.data(), wf.size()));
-        S3B_OK(upload_f32(bb, bf.data(), bf.size()));
-        S3B_OK(os.ensure(M * D));
-        CUDA_OK(launch_depthwise_glu(x, B, T, D, k, wb.as<float>(), bb.as<float>(), os.planes(out_fmt), st));
-        CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), M * D, out, st));
-        CUDA_OK(cudaStreamSynchronize(st));
-        return 0;
-    }();
-    wb.release(), bb.release(), os.release();
-    return r;
+    std::vector<float> w, g, be, mu, var, wf, bf;
+    S3B_OK(download_f32(dw_w, (size_t)D * k, st, w));
+    S3B_OK(download_f32(bn_gamma, D, st, g));
+    S3B_OK(download_f32(bn_beta, D, st, be));
+    S3B_OK(download_f32(bn_mean, D, st, mu));
+    S3B_OK(download_f32(bn_var, D, st, var));
+    fold_depthwise_bn(w.data(), g.data(), be.data(), mu.data(), var.data(), D, k, wf, bf);
+    S3B_OK(upload_f32(wb, wf.data(), wf.size()));
+    S3B_OK(upload_f32(bb, bf.data(), bf.size()));
+    S3B_OK(os.ensure(M * D));
+    CUDA_OK(launch_depthwise_glu(x, B, T, D, k, wb.as<float>(), bb.as<float>(), os.planes(out_fmt), st));
+    CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), M * D, out, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
 }
 
 extern "C" int s3b_layernorm_rope_f32(const float* x, int64_t M, int32_t T, int32_t D, const float* gamma,
@@ -3249,20 +3109,16 @@ extern "C" int s3b_layernorm_rope_f32(const float* x, int64_t M, int32_t T, int3
     const std::vector<float> cs = rope_table(f, T);
     DevBuf table;
     SplitBuf y, yr;
-    const int r = [&]() -> int {
-        S3B_OK(table.ensure(cs.size() * 4));
-        CUDA_OK(cudaMemcpyAsync(table.p, cs.data(), cs.size() * 4, cudaMemcpyHostToDevice, st));
-        S3B_OK(y.ensure((size_t)M * D));
-        S3B_OK(yr.ensure((size_t)M * D));
-        CUDA_OK(launch_layernorm_rope(x, (size_t)M, T, D, gamma, beta, table.as<float>(), y.planes(out_fmt),
-                                      yr.planes(out_fmt), st));
-        CUDA_OK(launch_planes_to_f32(y.planes(out_fmt), (size_t)M * D, out, st));
-        CUDA_OK(launch_planes_to_f32(yr.planes(out_fmt), (size_t)M * D, out_rope, st));
-        CUDA_OK(cudaStreamSynchronize(st));
-        return 0;
-    }();
-    table.release(), y.release(), yr.release();
-    return r;
+    S3B_OK(table.ensure(cs.size() * 4));
+    CUDA_OK(cudaMemcpyAsync(table.p, cs.data(), cs.size() * 4, cudaMemcpyHostToDevice, st));
+    S3B_OK(y.ensure((size_t)M * D));
+    S3B_OK(yr.ensure((size_t)M * D));
+    CUDA_OK(launch_layernorm_rope(x, (size_t)M, T, D, gamma, beta, table.as<float>(), y.planes(out_fmt),
+                                  yr.planes(out_fmt), st));
+    CUDA_OK(launch_planes_to_f32(y.planes(out_fmt), (size_t)M * D, out, st));
+    CUDA_OK(launch_planes_to_f32(yr.planes(out_fmt), (size_t)M * D, out_rope, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -3358,7 +3214,6 @@ extern "C" int s3b_trimmed_lengths(const float* const* wavs, const int64_t* lens
     CUDA_OK(launch_trimmed_lengths(d_ptrs, d_lens, batch, d_out, 0));
     CUDA_OK(cudaMemcpy(res.data(), d_out, batch * sizeof(long long), cudaMemcpyDeviceToHost));
     for (int b = 0; b < batch; ++b) out[b] = res[b];
-    scratch.release();
     return 0;
 }
 

@@ -2,12 +2,11 @@
 frame kept, written as operand planes) against torchaudio's own ``kaldi.fbank``; the GRU recurrence kernel at block
 level (``s3b_gru_f32``) against the oracle's GRU in fp64; the whole model against the executed-reference goldens
 (tests/golden/apc_ref*.pt, vq_apc_ref.pt) and the CPU oracle (tests/apc_oracle.py) in both GEMM operand schemes; and
-bit-identical results across batch composition, lanes, shards, ``forward_host``, CUDA-graph replay and apc / vq_apc.
+bit-identical results across batch composition, lanes, shards, ``forward_host`` and apc / vq_apc.
 Bounds: front end 1e-4 relative per utterance; recurrence block 1e-4 relative Frobenius and 2e-4 of the output scale
 elementwise; model 2e-4 relative per layer. Every check prints measured / bound."""
 import ctypes as C
 import os
-import subprocess
 import sys
 from pathlib import Path
 
@@ -269,32 +268,22 @@ def test_forward_ex_refusals_and_profile(s3b_lib):
     print(f"apc profile ms: gemm {ms[0]:.3f} front end {ms[2]:.3f} recurrence {ms[5]:.3f}")
 
 
-def test_graph_replay_is_bit_identical(s3b_lib):
-    """S3B_GRAPHS=1: repeated identical calls give the eager result. A subprocess: the switch is read once per
-    process."""
-    code = r"""
-import sys, torch
-sys.path.insert(0, %r)
-from s3prl_b200.upstream.apc import ApcExpert
-g = torch.Generator().manual_seed(5)
-wavs = [torch.randn(n, generator=g).cuda() for n in (24000, 16000, 9000, 20000, 7000)]
-e = ApcExpert().to("cuda")
-ref = torch.stack(e(wavs)["hidden_states"]).clone()
-native = e._native
-counts, ok = [], True
-for i in range(10):
-    c0 = native.lib.s3b_launch_count(native.handle)
-    res = e(wavs)
-    counts.append(native.lib.s3b_launch_count(native.handle) - c0)
-    ok &= torch.equal(torch.stack(res["hidden_states"]), ref)
-torch.cuda.synchronize()
-assert ok, "graph replay changed the result"
-assert len(set(counts)) == 1, counts
-print("GRAPH_OK", counts[0])
-""" % str(ROOT)
-    env = dict(os.environ, S3B_GRAPHS="1")
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, timeout=600)
-    assert r.returncode == 0 and "GRAPH_OK" in r.stdout, (r.stdout[-500:], r.stderr[-1500:])
+def test_repeated_calls_are_bit_identical(s3b_lib):
+    """10 identical calls after a first one give its result bit for bit and each adds the same launch count."""
+    from s3prl_b200.upstream.apc import ApcExpert
+
+    g = torch.Generator().manual_seed(5)
+    wavs = [torch.randn(n, generator=g).cuda() for n in (24000, 16000, 9000, 20000, 7000)]
+    e = ApcExpert().to("cuda")
+    ref = torch.stack(e(wavs)["hidden_states"]).clone()
+    native = e._native
+    counts = []
+    for i in range(10):
+        c0 = native.lib.s3b_launch_count(native.handle)
+        res = e(wavs)
+        counts.append(native.lib.s3b_launch_count(native.handle) - c0)
+        assert torch.equal(torch.stack(res["hidden_states"]), ref), f"call {i + 1} changed the result"
+    assert len(set(counts)) == 1, counts
 
 
 def test_occupancy(s3b_lib):

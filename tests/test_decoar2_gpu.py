@@ -1,13 +1,12 @@
 """GPU tests of DeCoAR 2.0 (``decoar2``): the front end (kaldi fbank with the hamming window, CMVN, y[::2], written as
 operand planes) against torchaudio's own ``kaldi.fbank``, and the whole model against the executed-reference goldens
 (tests/golden/decoar2_ref*.pt) and the CPU oracle (tests/decoar2_oracle.py) in both GEMM operand schemes, with
-determinism across lanes, shards, a checkpoint file, ``forward_host`` and CUDA-graph replay.
+determinism across lanes, shards, a checkpoint file and ``forward_host``.
 Bounds: front end 1e-4 relative per utterance; the model the golden bars of tests/test_upstream_gpu.py (2e-4 per layer,
 1e-3 of the layer's abs max). Every check prints measured / bound."""
 import ctypes as C
 import math
 import os
-import subprocess
 import sys
 from pathlib import Path
 
@@ -242,29 +241,19 @@ def test_ffn_out_and_profile(s3b_lib):
           f"misc {ms[4]:.3f}")
 
 
-def test_graph_replay_is_bit_identical(s3b_lib):
-    """S3B_GRAPHS=1: repeated identical calls (captured and replayed, or enqueued when the capture is refused) give the
-    eager result, with the same launch accounting. A subprocess, because the switch is read once per process."""
-    code = r"""
-import sys, torch
-sys.path.insert(0, %r)
-from s3prl_b200.upstream.decoar2 import Decoar2Expert
-g = torch.Generator().manual_seed(5)
-wavs = [torch.randn(n, generator=g).cuda() for n in (24000, 16000, 9000, 20000)]
-e = Decoar2Expert().to("cuda")
-ref = torch.stack(e(wavs)["hidden_states"]).clone()
-native = e._native
-counts, ok = [], True
-for i in range(10):
-    c0 = native.lib.s3b_launch_count(native.handle)
-    res = e(wavs)
-    counts.append(native.lib.s3b_launch_count(native.handle) - c0)
-    ok &= torch.equal(torch.stack(res["hidden_states"]), ref)
-torch.cuda.synchronize()
-assert ok, "graph replay changed the result"
-assert len(set(counts)) == 1, counts
-print("GRAPH_OK", counts[0])
-""" % str(ROOT)
-    env = dict(os.environ, S3B_GRAPHS="1")
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, timeout=600)
-    assert r.returncode == 0 and "GRAPH_OK" in r.stdout, (r.stdout[-500:], r.stderr[-1500:])
+def test_repeated_calls_are_bit_identical(s3b_lib):
+    """10 identical calls after a first one give its result bit for bit and each adds the same launch count."""
+    from s3prl_b200.upstream.decoar2 import Decoar2Expert
+
+    g = torch.Generator().manual_seed(5)
+    wavs = [torch.randn(n, generator=g).cuda() for n in (24000, 16000, 9000, 20000)]
+    e = Decoar2Expert().to("cuda")
+    ref = torch.stack(e(wavs)["hidden_states"]).clone()
+    native = e._native
+    counts = []
+    for i in range(10):
+        c0 = native.lib.s3b_launch_count(native.handle)
+        res = e(wavs)
+        counts.append(native.lib.s3b_launch_count(native.handle) - c0)
+        assert torch.equal(torch.stack(res["hidden_states"]), ref), f"call {i + 1} changed the result"
+    assert len(set(counts)) == 1, counts

@@ -1,12 +1,11 @@
 """GPU tests of DeCoAR (``decoar``, ``decoar_layers``): the grid-resident LSTM recurrence kernel at block level
 (``s3b_lstm_f32``) against an fp64 torch loop in both directions; the whole model against the executed-reference
 goldens (tests/golden/decoar*_ref*.pt) in both GEMM operand schemes; ``decoar`` against ``decoar_layers``; the long
-memory in both directions; bit-identical results across lanes, ``forward_host`` chunks, shards and CUDA-graph replay;
+memory in both directions; bit-identical results across lanes, ``forward_host`` chunks and shards;
 and the refusals. Bounds: recurrence block 1e-4 relative Frobenius and 2e-4 of the output scale elementwise; model
 2e-4 relative per hidden state. Every check prints measured / bound."""
 import ctypes as C
 import os
-import subprocess
 import sys
 from pathlib import Path
 
@@ -261,32 +260,19 @@ def test_forward_ex_refusals_and_profile(s3b_lib):
     print(f"decoar profile ms: gemm {ms[0]:.3f} front end {ms[2]:.3f} recurrence {ms[5]:.3f}")
 
 
-def test_graph_replay_is_bit_identical(s3b_lib):
-    """S3B_GRAPHS=1: repeated identical calls give the eager result, whether the forward (with its cooperative
-    launches) is captured and replayed or the capture is refused and the model says so and runs eagerly. A
-    subprocess: the switch is read once per process."""
-    code = r"""
-import sys, torch
-sys.path.insert(0, %r)
-from s3prl_b200.upstream.decoar import DecoarExpert
-g = torch.Generator().manual_seed(5)
-wavs = [torch.randn(n, generator=g).cuda() for n in (24000, 16000, 9000, 20000, 7000)]
-e = DecoarExpert(all_layers=True).to("cuda")
-ref = torch.stack(e(wavs)["hidden_states"]).clone()
-native = e._native
-counts, ok = [], True
-for i in range(6):
-    c0 = native.lib.s3b_launch_count(native.handle)
-    res = e(wavs)
-    counts.append(native.lib.s3b_launch_count(native.handle) - c0)
-    ok &= torch.equal(torch.stack(res["hidden_states"]), ref)
-torch.cuda.synchronize()
-assert ok, "graph replay changed the result"
-assert len(set(counts)) == 1, counts
-print("GRAPH_OK", counts[0])
-""" % str(ROOT)
-    env = dict(os.environ, S3B_GRAPHS="1")
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, timeout=900)
-    assert r.returncode == 0 and "GRAPH_OK" in r.stdout, (r.stdout[-500:], r.stderr[-1500:])
-    refused = "CUDA-graph capture of the forward failed" in r.stderr
-    print("graph mode:", "capture refused, eager fallback: " + r.stderr.strip()[-300:] if refused else "replayed")
+def test_repeated_calls_are_bit_identical(s3b_lib):
+    """6 identical calls after a first one give its result bit for bit and each adds the same launch count."""
+    from s3prl_b200.upstream.decoar import DecoarExpert
+
+    g = torch.Generator().manual_seed(5)
+    wavs = [torch.randn(n, generator=g).cuda() for n in (24000, 16000, 9000, 20000, 7000)]
+    e = DecoarExpert(all_layers=True).to("cuda")
+    ref = torch.stack(e(wavs)["hidden_states"]).clone()
+    native = e._native
+    counts = []
+    for i in range(6):
+        c0 = native.lib.s3b_launch_count(native.handle)
+        res = e(wavs)
+        counts.append(native.lib.s3b_launch_count(native.handle) - c0)
+        assert torch.equal(torch.stack(res["hidden_states"]), ref), f"call {i + 1} changed the result"
+    assert len(set(counts)) == 1, counts

@@ -347,33 +347,19 @@ def test_operand_schemes_agree(s3b_lib, name):
         assert ((a.double() - b.double()).norm() / b.double().norm()).item() < 1e-4
 
 
-def test_graph_replay_is_bit_identical(s3b_lib):
-    """S3B_GRAPHS=1 (experimental): the third identical call (same shapes, same output buffer, same stream) is captured
-    into a CUDA graph and replayed afterwards — or, when the capture is refused (this driver rejects it: programmatic
-    dependent launches inside a capture), the library says so once and keeps enqueueing normally. Either way results
-    and launch accounting must not change. Runs in a subprocess because the switch is read once per process."""
-    import subprocess
+def test_repeated_calls_are_bit_identical(s3b_lib):
+    """10 identical calls after a first one give its result bit for bit and each adds the same launch count."""
+    from s3prl_b200.upstream.expert import UpstreamExpert
 
-    code = r"""
-import sys, torch
-sys.path.insert(0, %r)
-from s3prl_b200.upstream.expert import UpstreamExpert
-g = torch.Generator().manual_seed(5)
-wavs = [torch.randn(n, generator=g).cuda() for n in (24000, 16000, 9000, 20000)]
-e = UpstreamExpert(name="wavlm_base_plus", seed=0).to("cuda")
-ref = torch.stack(e(wavs)["hidden_states"]).clone()
-native = e._native
-counts, ok = [], True
-for i in range(10):
-    c0 = native.lib.s3b_launch_count(native.handle)
-    res = e(wavs)
-    counts.append(native.lib.s3b_launch_count(native.handle) - c0)
-    ok &= torch.equal(torch.stack(res["hidden_states"]), ref)
-torch.cuda.synchronize()
-assert ok, "graph replay changed the result"
-assert len(set(counts)) == 1, counts
-print("GRAPH_OK", counts[0])
-""" % str(ROOT)
-    env = dict(os.environ, S3B_GRAPHS="1")
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, timeout=600)
-    assert r.returncode == 0 and "GRAPH_OK" in r.stdout, (r.stdout[-500:], r.stderr[-1500:])
+    g = torch.Generator().manual_seed(5)
+    wavs = [torch.randn(n, generator=g).cuda() for n in (24000, 16000, 9000, 20000)]
+    e = UpstreamExpert(name="wavlm_base_plus", seed=0).to("cuda")
+    ref = torch.stack(e(wavs)["hidden_states"]).clone()
+    native = e._native
+    counts = []
+    for i in range(10):
+        c0 = native.lib.s3b_launch_count(native.handle)
+        res = e(wavs)
+        counts.append(native.lib.s3b_launch_count(native.handle) - c0)
+        assert torch.equal(torch.stack(res["hidden_states"]), ref), f"call {i + 1} changed the result"
+    assert len(set(counts)) == 1, counts
