@@ -312,7 +312,16 @@ int s3b_linear_ex(const float* a, const float* w, const float* bias, const float
  * epilogue (q scaled by 1/8 * log2(e), per-head layout, v transposed), in operand scheme `scheme` (-1 / 0 / 1 as in
  * s3b_linear_opts). The bf16 hi/lo planes it writes are decoded to q_out, k_out [batch][heads][t][64] and
  * vt_out [batch][heads][64][(t + 7) & ~7]. The epilogue writes columns [0, t) of each vt_out row; the padding columns
- * t.. are never written by it and come back as the zero of a freshly allocated plane. */
+ * t.. are never written by it and come back as the zero of a freshly allocated plane: this entry point allocates its
+ * planes per call. A model's planes live as long as the model and are zeroed only when they are (re)allocated, so
+ * there the padding columns hold whatever an earlier, differently shaped forward left, NaN included. The model path
+ * does not rely on them: the attention kernel's tensor map of v^T has extent t, not (t + 7) & ~7, so the columns past
+ * t are filled with zeros by the TMA load and the stored ones are never read. The same holds for q / k rows past t
+ * and, for 80- and 120-wide heads, the box columns past head_dim. What the model path does rely on is written on every
+ * call by the kernel that owns it: the CMVN kernel zero-fills columns 80..127 and rows past each utterance's frames of
+ * the fbank models' [M][128] operand, and post_extract_proj's row mask zeroes padded frames.
+ * tests/test_history_gpu.py holds a long-lived model to the result of a fresh one after calls of other shapes and
+ * after a forward on non-finite waveforms. */
 int s3b_qkv_f32(const float* x, const float* w, const float* b, int32_t batch, int32_t t, int32_t heads, int32_t scheme,
                 float* q_out, float* k_out, float* vt_out, void* stream);
 /* s3b_qkv_f32 for heads of head_dim (64, 80 or 120) channels: x [batch][t][heads*head_dim]; q scaled by
