@@ -267,13 +267,20 @@ struct Workspace {
     std::vector<std::unique_ptr<Plan>> plans;  // small LRU of cached tensor maps / launch descriptors keyed by (B, Lmax)
 };
 
+// What a model runs, fixed by the create function that made it
+enum ModelKind {
+    kConvEncoder,   // s3b_model_create, frontend 0: conv stack into the transformer / Conformer encoder
+    kFbankEncoder,  // s3b_model_create, frontend 1 (DeCoAR 2.0): fbank + CMVN, every second frame, into the encoder
+    kGruStack,      // s3b_apc_model_create (APC / VQ-APC): fbank + CMVN into a GRU stack
+    kLstmStack,     // s3b_decoar_model_create (DeCoAR): fbank + CMVN, post_extract_proj, bidirectional LSTM stack
+};
+
 struct s3b_model {
     s3b_config cfg;
-    // APC / VQ-APC (s3b_apc_model_create): cfg then holds num_layers and embed_dim = hidden, everything else zero
-    bool apc = false;
+    ModelKind kind = kConvEncoder;
+    // kGruStack: cfg holds num_layers and embed_dim = hidden, everything else zero
     int apc_residual = 0;
-    // DeCoAR (s3b_decoar_model_create): cfg holds num_layers and embed_dim = 2 H (the forward | backward concat)
-    bool decoar_lstm = false;
+    // kLstmStack: cfg holds num_layers and embed_dim = 2 H (the forward | backward concat)
     int decoar_all_layers = 0;  // 1: decoar_layers (every layer's output), 0: decoar (the last one)
     std::map<std::string, HostTensor> host;
     bool finalized = false;
@@ -364,14 +371,15 @@ static int64_t num_frames(int64_t L) {
 static const int64_t kDecoar2MinLen = 560;  // two fbank frames: the unbiased std of one frame is NaN
 static int64_t decoar2_frames(int64_t L) { return L < 400 ? 0 : (1 + (L - 400) / 160 + 1) / 2; }
 static int64_t fbank_frames(int64_t L) { return L < 400 ? 0 : 1 + (L - 400) / 160; }
-static bool decoar2(const s3b_model* m) { return m != nullptr && m->cfg.frontend == 1; }
-static bool apc(const s3b_model* m) { return m != nullptr && m->apc; }
-static bool decoar1(const s3b_model* m) { return m != nullptr && m->decoar_lstm; }
-// the recurrent upstreams: every fbank frame kept (APC's front end)
-static bool fbank_all_frames(const s3b_model* m) { return apc(m) || decoar1(m); }
-// frames of a batch padded to L for this model's front end (m NULL: the conv stack)
+// frames of a batch padded to L for this model's front end (m NULL: the conv stack); on the fbank kinds also the
+// valid frames of one utterance of L samples
 static int64_t model_frames(const s3b_model* m, int64_t L) {
-    return fbank_all_frames(m) ? fbank_frames(L) : decoar2(m) ? decoar2_frames(L) : num_frames(L);
+    if (m == nullptr || m->kind == kConvEncoder) return num_frames(L);
+    return m->kind == kFbankEncoder ? decoar2_frames(L) : fbank_frames(L);  // the recurrent stacks keep every frame
+}
+static int fail_too_short(const s3b_model* m, int64_t max_len) {
+    return fail("max_len %lld too short: the %s yields no frame", (long long)max_len,
+                m->kind == kConvEncoder ? "conv stack" : "fbank");
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -457,6 +465,7 @@ extern "C" int s3b_model_create(const s3b_config* cfg, s3b_model** out) {
     }
     s3b_model* m = new s3b_model();
     m->cfg = *cfg;
+    m->kind = cfg->frontend == 1 ? kFbankEncoder : kConvEncoder;
     m->scheme = default_scheme();
     *out = m;
     return 0;
@@ -475,7 +484,7 @@ extern "C" int s3b_apc_model_create(const s3b_apc_config* cfg, s3b_model** out) 
     s3b_model* m = new s3b_model();
     memset(&m->cfg, 0, sizeof(m->cfg));
     m->cfg.num_layers = cfg->num_layers, m->cfg.embed_dim = cfg->hidden;
-    m->apc = true, m->apc_residual = cfg->residual;
+    m->kind = kGruStack, m->apc_residual = cfg->residual;
     m->scheme = default_scheme();
     *out = m;
     return 0;
@@ -495,7 +504,7 @@ extern "C" int s3b_decoar_model_create(const s3b_decoar_config* cfg, s3b_model**
     s3b_model* m = new s3b_model();
     memset(&m->cfg, 0, sizeof(m->cfg));
     m->cfg.num_layers = cfg->num_layers, m->cfg.embed_dim = 2 * cfg->hidden;
-    m->decoar_lstm = true, m->decoar_all_layers = cfg->all_layers;
+    m->kind = kLstmStack, m->decoar_all_layers = cfg->all_layers;
     m->scheme = default_scheme();
     *out = m;
     return 0;
@@ -718,22 +727,25 @@ static int finalize_apc(s3b_model* m) {
     if (clusters < 1)
         return fail("the GRU recurrence kernel cannot run on this device: cudaOccupancyMaxActiveClusters reports 0 "
                     "clusters of %d CTAs with %zu bytes of shared memory each", kGruCtas, gru_smem_bytes());
-    CUDA_OK(init_fbank_tables());
-    m->host.clear();
-    m->finalized = true;
     return 0;
+}
+
+// post_extract_proj of DeCoAR and DeCoAR 2.0: [N][80] zero-padded to K = kDecoar2K, the width of the CMVN kernel's
+// operand planes
+static int upload_fbank_proj(s3b_model* m, int N) {
+    const HostTensor* t;
+    S3B_OK(need(m, "post_extract_proj.weight", {N, 80}, &t));
+    std::vector<float> wp((size_t)N * kDecoar2K, 0.f);
+    for (int o = 0; o < N; ++o) memcpy(&wp[(size_t)o * kDecoar2K], &t->data[(size_t)o * 80], 80 * sizeof(float));
+    S3B_OK(upload_split(m->proj_w, wp.data(), wp.size(), m->scheme));
+    return upload_vec(m, "post_extract_proj.bias", N, m->proj_b);
 }
 
 // DeCoAR (decoar.py): post_extract_proj = Linear(80, 1024), then {forward,backward}_lstm = nn.LSTM(1024, 1024,
 // num_layers=4). The recurrence kernel needs the whole device: kLstmCtas co-resident CTAs, one per SM.
 static int finalize_decoar(s3b_model* m) {
     const int NL = m->cfg.num_layers, H = kLstmHidden;
-    const HostTensor* t;
-    S3B_OK(need(m, "post_extract_proj.weight", {H, 80}, &t));
-    std::vector<float> wp((size_t)H * kDecoar2K, 0.f);
-    for (int o = 0; o < H; ++o) memcpy(&wp[(size_t)o * kDecoar2K], &t->data[(size_t)o * 80], 80 * sizeof(float));
-    S3B_OK(upload_split(m->proj_w, wp.data(), wp.size(), m->scheme));
-    S3B_OK(upload_vec(m, "post_extract_proj.bias", H, m->proj_b));
+    S3B_OK(upload_fbank_proj(m, H));
     m->layers.resize(2 * NL);
     for (int l = 0; l < NL; ++l)
         for (int d = 0; d < 2; ++d) {
@@ -761,40 +773,18 @@ static int finalize_decoar(s3b_model* m) {
     if (!ok)
         return fail("the LSTM recurrence kernel cannot run on this device: %d co-resident CTAs with %zu bytes of "
                     "shared memory each (cooperative launch) do not fit", kLstmCtas, lstm_smem_bytes());
-    CUDA_OK(init_fbank_tables());
-    m->host.clear();
-    m->finalized = true;
     return 0;
 }
 
-extern "C" int s3b_model_finalize(s3b_model* m) {
-    if (!m) return fail("null model");
-    if (m->finalized) return 0;
-    if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
-    int dev = 0;
-    CUDA_OK(cudaGetDevice(&dev));
-    cudaDeviceProp prop;
-    CUDA_OK(cudaGetDeviceProperties(&prop, dev));
-    if (prop.major != 9 || prop.minor != 0)
-        return fail("device is sm_%d%d; this library contains sm_90a code only", prop.major, prop.minor);
-    m->sm_count = prop.multiProcessorCount;
-    g_sm_count = m->sm_count;
-    if (apc(m)) return finalize_apc(m);
-    if (decoar1(m)) return finalize_decoar(m);
-
+// The conv-stack and fbank encoders: front end, pos_conv, transformer or Conformer layers, prediction heads
+static int finalize_encoder(s3b_model* m) {
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, F = c.ffn_dim, C = kConvDim;
     const HostTensor* t;
     const std::string fe = "feature_extractor.conv_layers.";
 
-    if (decoar2(m)) {
-        // ---- DeCoAR 2.0: post_extract_proj [D][80] zero-padded to K = 128; fbank tables built here, not in a forward --
-        S3B_OK(need(m, "post_extract_proj.weight", {D, 80}, &t));
-        std::vector<float> wp((size_t)D * kDecoar2K, 0.f);
-        for (int o = 0; o < D; ++o) memcpy(&wp[(size_t)o * kDecoar2K], &t->data[(size_t)o * 80], 80 * sizeof(float));
-        S3B_OK(upload_split(m->proj_w, wp.data(), wp.size(), m->scheme));
-        S3B_OK(upload_vec(m, "post_extract_proj.bias", D, m->proj_b));
-        CUDA_OK(init_fbank_tables());
+    if (m->kind == kFbankEncoder) {
+        S3B_OK(upload_fbank_proj(m, D));
     } else {
         // ---- conv 0 ------------------------------------------------------------------------------
         S3B_OK(need(m, fe + "0.0.weight", {C, 1, kConvK[0]}, &t));
@@ -944,6 +934,28 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
         S3B_OK(upload_f32(m->rel_table_src, t->data.data(), t->numel()));
         S3B_OK(build_rel_table(m, 4096));  // utterances up to 82 s; rebuilt (synchronously) for longer batches
     }
+    return 0;
+}
+
+extern "C" int s3b_model_finalize(s3b_model* m) {
+    if (!m) return fail("null model");
+    if (m->finalized) return 0;
+    if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
+    int dev = 0;
+    CUDA_OK(cudaGetDevice(&dev));
+    cudaDeviceProp prop;
+    CUDA_OK(cudaGetDeviceProperties(&prop, dev));
+    if (prop.major != 9 || prop.minor != 0)
+        return fail("device is sm_%d%d; this library contains sm_90a code only", prop.major, prop.minor);
+    m->sm_count = prop.multiProcessorCount;
+    g_sm_count = m->sm_count;
+    switch (m->kind) {
+    case kGruStack: S3B_OK(finalize_apc(m)); break;
+    case kLstmStack: S3B_OK(finalize_decoar(m)); break;
+    case kConvEncoder:
+    case kFbankEncoder: S3B_OK(finalize_encoder(m)); break;
+    }
+    if (m->kind != kConvEncoder) CUDA_OK(init_fbank_tables());  // built here, not in a forward
     m->host.clear();
     m->finalized = true;
     return 0;
@@ -958,38 +970,36 @@ extern "C" int64_t s3b_num_frames(const s3b_model* m, int64_t max_len) {
 }
 
 extern "C" int32_t s3b_num_outputs(const s3b_model* m) {
-    if (apc(m)) return m->cfg.num_layers;  // the output of every GRU layer (+ residual)
-    if (decoar1(m)) return m->decoar_all_layers ? m->cfg.num_layers : 1;  // decoar_layers: every layer; decoar: the last
-    return m ? m->cfg.num_layers + 1 + m->cfg.pred_heads : -1;
+    if (!m) return -1;
+    switch (m->kind) {
+    case kGruStack: return m->cfg.num_layers;  // the output of every GRU layer (+ residual)
+    case kLstmStack: return m->decoar_all_layers ? m->cfg.num_layers : 1;  // decoar_layers: every layer; decoar: the last
+    default: return m->cfg.num_layers + 1 + m->cfg.pred_heads;
+    }
 }
 
 extern "C" int s3b_valid_frames(const s3b_model* m, const int64_t* lens, int32_t batch, int64_t max_len,
                                 int32_t* valid) {
     if (!m || !lens || !valid) return fail("null argument");
     const int64_t T = model_frames(m, max_len);
-    if (T <= 0)
-        return fail("max_len %lld too short for the %s", (long long)max_len,
-                    decoar2(m) || fbank_all_frames(m) ? "fbank" : "conv stack");
+    if (T <= 0) return fail_too_short(m, max_len);
+    const char* fbank_model = m->kind == kFbankEncoder ? "DeCoAR 2.0"
+                              : m->kind == kGruStack   ? "APC"
+                              : m->kind == kLstmStack  ? "DeCoAR"
+                                                       : nullptr;
     bool any_pad = false;
     for (int b = 0; b < batch; ++b) {
         if (lens[b] < 1 || lens[b] > max_len) return fail("lens[%d]=%lld out of range", b, (long long)lens[b]);
-        if (apc(m) && lens[b] < kDecoar2MinLen)
-            return fail("lens[%d]=%lld: APC needs >= %lld samples (2 fbank frames; the CMVN std of one frame is NaN)", b,
-                        (long long)lens[b], (long long)kDecoar2MinLen);
-        if (decoar1(m) && lens[b] < kDecoar2MinLen)
-            return fail("lens[%d]=%lld: DeCoAR needs >= %lld samples (2 fbank frames; the CMVN std of one frame is NaN)",
-                        b, (long long)lens[b], (long long)kDecoar2MinLen);
-        if (decoar2(m) && lens[b] < kDecoar2MinLen)
-            return fail("lens[%d]=%lld: DeCoAR 2.0 needs >= %lld samples (2 fbank frames; the CMVN std of one frame is NaN)",
-                        b, (long long)lens[b], (long long)kDecoar2MinLen);
+        if (fbank_model != nullptr && lens[b] < kDecoar2MinLen)
+            return fail("lens[%d]=%lld: %s needs >= %lld samples (2 fbank frames; the CMVN std of one frame is NaN)", b,
+                        (long long)lens[b], fbank_model, (long long)kDecoar2MinLen);
         any_pad |= lens[b] < max_len;
     }
     for (int b = 0; b < batch; ++b) {
         int64_t v;
-        if (fbank_all_frames(m)) {
-            v = fbank_frames(lens[b]);  // pad_sequence of the per-utterance features (apc/expert.py:47-51)
-        } else if (decoar2(m)) {
-            v = decoar2_frames(lens[b]);  // pad_sequence of the per-utterance features (decoar2/expert.py:81-92)
+        if (m->kind != kConvEncoder) {
+            // pad_sequence of the per-utterance features (apc/expert.py:47-51, decoar2/expert.py:81-92)
+            v = model_frames(m, lens[b]);
         } else if (m->cfg.family == 1) {
             // wav2vec2: conv-length rule, only when the batch has any padding (wav2vec2_model.py:2652-2671). The
             // reference evaluates floor((n - k) / s + 1) in fp32 WITHOUT clamping, so an utterance shorter than the
@@ -1340,10 +1350,13 @@ struct Fwd {
 
     static constexpr int kConformerStages = 10;  // stages per Conformer layer (conformer_stage)
     int num_stages() const {
-        if (apc(m)) return 1 + 2 * m->cfg.num_layers;  // front end, then per layer: input GEMM, recurrence
-        if (decoar1(m)) return 2 + 4 * m->cfg.num_layers;  // front end, post_extract_proj, per layer and direction: GEMM, recurrence
-        if (m->cfg.conformer) return 9 + kConformerStages * m->cfg.num_layers;
-        return 9 + 5 * m->cfg.num_layers + (m->cfg.pred_heads > 0 ? 1 + m->cfg.pred_heads : 0);
+        switch (m->kind) {
+        case kGruStack: return 1 + 2 * m->cfg.num_layers;  // front end, then per layer: input GEMM, recurrence
+        case kLstmStack: return 2 + 4 * m->cfg.num_layers;  // front end, post_extract_proj, per layer and direction: GEMM, recurrence
+        default:
+            if (m->cfg.conformer) return 9 + kConformerStages * m->cfg.num_layers;
+            return 9 + 5 * m->cfg.num_layers + (m->cfg.pred_heads > 0 ? 1 + m->cfg.pred_heads : 0);
+        }
     }
     bool distil() const { return m->cfg.family == 3; }
     // Output slot i of the caller's buffer. Hidden state l (the input of layer l / the encoder output) lives in slot l —
@@ -1367,13 +1380,14 @@ int Fwd::prepare() {
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, C = kConvDim;
     if (B < 1) return fail("empty batch");
-    const bool fb = decoar2(m) || fbank_all_frames(m);
+    const bool fb = m->kind != kConvEncoder;
+    const bool recurrent = m->kind == kGruStack || m->kind == kLstmStack;
     {
         int64_t cur = Lmax;
         for (int i = 0; i < kNumConv; ++i) cur = L[i] = fb ? 0 : conv_out_len(cur, i);
     }
     const int64_t T64 = model_frames(m, Lmax);
-    if (T64 < 1) return fail("max_len %lld too short: the %s yields no frame", (long long)Lmax, fb ? "fbank" : "conv stack");
+    if (T64 < 1) return fail_too_short(m, Lmax);
     if ((int64_t)B * (fb ? fbank_frames(Lmax) : L[0]) > 2000000000LL) return fail("batch too large for 32-bit tile indexing");
     T = (int)T64;
     M = (int64_t)B * T;
@@ -1387,7 +1401,7 @@ int Fwd::prepare() {
     const size_t off_lens = (size_t)B * sizeof(void*);
     const size_t off_kv = off_lens + (size_t)B * sizeof(long long);
     const size_t off_ord = off_kv + (size_t)B * sizeof(int);
-    const size_t off_mask = (off_ord + (fbank_all_frames(m) ? (size_t)B * sizeof(int) : 0) + 15) & ~(size_t)15;
+    const size_t off_mask = (off_ord + (recurrent ? (size_t)B * sizeof(int) : 0) + 15) & ~(size_t)15;
     const size_t book_bytes = off_mask + (size_t)M;
     S3B_OK(w->book.ensure(book_bytes));
     if (w->book_host_bytes < book_bytes) {
@@ -1414,7 +1428,7 @@ int Fwd::prepare() {
         for (int b = 0; b < B; ++b) hl[b] = (long long)lens[b];
         for (int b = 0; b < B; ++b)
             for (int t = hk[b]; t < T; ++t) hm[(size_t)b * T + t] = 1;
-        if (fbank_all_frames(m)) {  // group utterances of similar length: a recurrence group stops at its own longest
+        if (recurrent) {  // group utterances of similar length: a recurrence group stops at its own longest
             int* ho = reinterpret_cast<int*>(hb + off_ord);
             std::vector<int> ord(B);
             for (int b = 0; b < B; ++b) ord[b] = b;
@@ -1435,23 +1449,10 @@ int Fwd::prepare() {
     d_mask = reinterpret_cast<uint8_t*>(db + off_mask);
 
     // ---- workspace ------------------------------------------------------------------------------------------
-    if (apc(m)) {
-        S3B_OK(w->fb_f32.ensure((size_t)B * T * 80 * 4));
-        S3B_OK(w->ln512_s.ensure((size_t)M * kDecoar2K));  // layer 0's GEMM operand: the CMVN kernel's planes
-        S3B_OK(w->x_s.ensure((size_t)M * D));             // layers 1..: the recurrence kernel's planes
-        S3B_OK(w->xg_f32.ensure((size_t)M * 3 * D * 4));
-    } else if (decoar1(m)) {
-        const int H = kLstmHidden;
-        S3B_OK(w->fb_f32.ensure((size_t)B * T * 80 * 4));
-        S3B_OK(w->ln512_s.ensure((size_t)M * kDecoar2K));  // post_extract_proj's operand: the CMVN kernel's planes
-        S3B_OK(w->x_s.ensure((size_t)M * H));              // layer 0's operand: post_extract_proj's output
-        S3B_OK(w->h_s.ensure((size_t)M * 2 * H));          // layers 1..: the previous layer's [M][2H] output
-        S3B_OK(w->xg_f32.ensure((size_t)M * 4 * H * 4));
-        S3B_OK(w->lstm_h.ensure(lstm_hbuf_floats(B) * 4));
-        S3B_OK(w->lstm_sync.ensure(sizeof(unsigned int)));
-    } else if (fb) {
+    if (fb) {
         S3B_OK(w->fb_f32.ensure((size_t)B * fbank_frames(Lmax) * 80 * 4));
-        S3B_OK(w->ln512_s.ensure((size_t)M * kDecoar2K));  // post_extract_proj's A operand: the CMVN kernel's planes
+        // the CMVN kernel's planes: the A operand of post_extract_proj (APC: of layer 0's input GEMM)
+        S3B_OK(w->ln512_s.ensure((size_t)M * kDecoar2K));
     } else {
         S3B_OK(w->wav_pad.ensure((size_t)B * Lmax * 4));
         S3B_OK(w->wav_stats.ensure((size_t)B * 2 * 4));
@@ -1461,7 +1462,17 @@ int Fwd::prepare() {
         S3B_OK(w->conv_f32.ensure((size_t)B * (c.extractor_layer_norm ? L[1] : L[6]) * C * 4));
         S3B_OK(w->ln512_s.ensure((size_t)M * C));
     }
-    if (!fbank_all_frames(m)) {  // the encoder's buffers
+    if (m->kind == kGruStack) {
+        S3B_OK(w->x_s.ensure((size_t)M * D));  // layers 1..: the recurrence kernel's planes
+        S3B_OK(w->xg_f32.ensure((size_t)M * 3 * D * 4));
+    } else if (m->kind == kLstmStack) {
+        const int H = kLstmHidden;
+        S3B_OK(w->x_s.ensure((size_t)M * H));      // layer 0's operand: post_extract_proj's output
+        S3B_OK(w->h_s.ensure((size_t)M * 2 * H));  // layers 1..: the previous layer's [M][2H] output
+        S3B_OK(w->xg_f32.ensure((size_t)M * 4 * H * 4));
+        S3B_OK(w->lstm_h.ensure(lstm_hbuf_floats(B) * 4));
+        S3B_OK(w->lstm_sync.ensure(sizeof(unsigned int)));
+    } else {  // the encoder's buffers
         S3B_OK(w->tmp_f32.ensure((size_t)M * D * 4));
         S3B_OK(w->x_f32.ensure((size_t)M * D * 4));
         S3B_OK(w->x1_f32.ensure((size_t)M * D * 4));
@@ -1596,7 +1607,7 @@ int Fwd::build_conformer_layer(LayerPlan& lp, int l) {
 int Fwd::build_plan(Plan& pl) {
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, NL = c.num_layers, C = kConvDim;
-    if (apc(m)) {
+    if (m->kind == kGruStack) {
         // x_g = x W_ih^T + (b_ih + [b_hr, b_hz, 0]) over all B * T rows, fp32 [M][3D] (the recurrence ignores t >= m_b)
         pl.gru_in.resize(NL);
         for (int l = 0; l < NL; ++l) {
@@ -1610,7 +1621,7 @@ int Fwd::build_plan(Plan& pl) {
         }
         return 0;
     }
-    if (decoar1(m)) {
+    if (m->kind == kLstmStack) {
         // post_extract_proj [M][80 -> 128] x [1024][128]^T + b into layer 0's operand planes
         const int H = kLstmHidden;
         S3B_OK(linear_params(pl.proj, w->ln512_s, m->proj_w, M, H, kDecoar2K, m->scheme));
@@ -1635,7 +1646,7 @@ int Fwd::build_plan(Plan& pl) {
             }
         return 0;
     }
-    for (int i = 1; i < kNumConv && !decoar2(m); ++i) {
+    for (int i = 1; i < kNumConv && m->kind == kConvEncoder; ++i) {
         GemmParams& p = pl.conv[i];
         S3B_OK(conv_params(p, w->act[i - 1], m->conv_w[i], B, L[i - 1], L[i], kConvK[i], m->scheme));
         Epi e;
@@ -1653,7 +1664,7 @@ int Fwd::build_plan(Plan& pl) {
     }
     {
         GemmParams& p = pl.proj;
-        S3B_OK(linear_params(p, w->ln512_s, m->proj_w, M, D, decoar2(m) ? kDecoar2K : C, m->scheme));
+        S3B_OK(linear_params(p, w->ln512_s, m->proj_w, M, D, m->kind == kFbankEncoder ? kDecoar2K : C, m->scheme));
         Epi e;
         e.bias = m->proj_b.as<float>();
         e.row_mask = d_mask;  // x[padding_mask] = 0 (wav2vec2_model.py:3061-3062)
@@ -1757,20 +1768,13 @@ int Fwd::build_plan(Plan& pl) {
     return 0;
 }
 
-// APC: stage 0 = fbank + CMVN into layer 0's operand planes; stage 1 + 2l = layer l's input GEMM; stage 2 + 2l = its
-// recurrence, which writes hidden state l (+ layer l's input when residual, l > 0) and layer l + 1's operand planes
+// APC: stage 0 (Fwd::stage) = fbank + CMVN into layer 0's operand planes; stage 1 + 2l = layer l's input GEMM;
+// stage 2 + 2l = its recurrence, which writes hidden state l (+ layer l's input when residual, l > 0) and layer l + 1's
+// operand planes
 int Fwd::apc_stage(int s) {
     s3b_model* m = this->m;  // the launch macros expect `m` and `st`
     cudaStream_t st = this->st;
     const int D = m->cfg.embed_dim, NL = m->cfg.num_layers;
-    if (s == 0) {
-        const size_t book_bytes = (size_t)(reinterpret_cast<char*>(d_mask) - w->book.as<char>()) + (size_t)M;
-        CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host.get(), book_bytes, cudaMemcpyHostToDevice, st));
-        CUDA_OK(cudaEventRecord(w->book_copied.get(), st));
-        KLAUNCH(CAT_CONV0, 2, 0.0, launch_decoar2_features(d_wavs, d_lens, B, T, T, 1, w->fb_f32.as<float>(),
-                                                           w->ln512_s.planes(m->scheme), st));
-        return 0;
-    }
     const int l = (s - 1) / 2;
     if (l >= NL) return fail("internal: stage %d out of range", s);
     if ((s - 1) % 2 == 0) {
@@ -1790,23 +1794,15 @@ int Fwd::apc_stage(int s) {
     return 0;
 }
 
-// DeCoAR: stage 0 = fbank + CMVN; stage 1 = post_extract_proj; stage 2 + 4l + 2d = the input GEMM of layer l,
-// direction d (0 forward, 1 backward); stage 3 + 4l + 2d = its recurrence, which writes columns [d H, d H + H) of
-// layer l's [B][T][2H] output: an output slot (decoar_layers: every layer; decoar: the last) and, below the last
+// DeCoAR: stage 0 (Fwd::stage) = fbank + CMVN; stage 1 = post_extract_proj; stage 2 + 4l + 2d = the input GEMM of
+// layer l, direction d (0 forward, 1 backward); stage 3 + 4l + 2d = its recurrence, which writes columns [d H, d H + H)
+// of layer l's [B][T][2H] output: an output slot (decoar_layers: every layer; decoar: the last) and, below the last
 // layer, the operand planes of layer l + 1's GEMMs. The two directions never run concurrently: each recurrence
 // occupies the whole device.
 int Fwd::decoar_stage(int s) {
     s3b_model* m = this->m;  // the launch macros expect `m` and `st`
     cudaStream_t st = this->st;
     const int NL = m->cfg.num_layers, H = kLstmHidden;
-    if (s == 0) {
-        const size_t book_bytes = (size_t)(reinterpret_cast<char*>(d_mask) - w->book.as<char>()) + (size_t)M;
-        CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host.get(), book_bytes, cudaMemcpyHostToDevice, st));
-        CUDA_OK(cudaEventRecord(w->book_copied.get(), st));
-        KLAUNCH(CAT_CONV0, 2, 0.0, launch_decoar2_features(d_wavs, d_lens, B, T, T, 1, w->fb_f32.as<float>(),
-                                                           w->ln512_s.planes(m->scheme), st));
-        return 0;
-    }
     if (s == 1) {
         GemmParams p = plan->proj;
         KGEMM(launch_gemm(p, m->sm_count, st));
@@ -1836,33 +1832,36 @@ int Fwd::decoar_stage(int s) {
 }
 
 int Fwd::stage(int s) {
-    if (apc(m)) return apc_stage(s);
-    if (decoar1(m)) return decoar_stage(s);
     s3b_model* m = this->m;  // the launch macros expect `m` and `st`
     cudaStream_t st = this->st;
     const s3b_config& c = m->cfg;
-    const int D = c.embed_dim, H = c.num_heads, NL = c.num_layers, C = kConvDim;
-    const double attn_flops = 4.0 * (double)T * T * D * B;
-
     if (s == 0) {
-        // ---- bookkeeping copy, waveform packing (+ normalisation), conv 0 + norm + GELU -> act[0] ------------------
+        // ---- bookkeeping copy, then the front end -----------------------------------------------------------------
         const size_t book_bytes = (size_t)(reinterpret_cast<char*>(d_mask) - w->book.as<char>()) + (size_t)M;
         CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host.get(), book_bytes, cudaMemcpyHostToDevice, st));
         CUDA_OK(cudaEventRecord(w->book_copied.get(), st));
-        if (decoar2(m)) {  // fbank frames + CMVN / y[::2] -> post_extract_proj's operand planes (profile category 2)
-            KLAUNCH(CAT_CONV0, 2, 0.0, launch_decoar2_features(d_wavs, d_lens, B, (int)fbank_frames(Lmax), T, 2,
+        if (m->kind != kConvEncoder) {
+            // fbank frames + CMVN (DeCoAR 2.0: y[::2]) -> the first GEMM's operand planes (profile category 2)
+            const int step = m->kind == kFbankEncoder ? 2 : 1;
+            KLAUNCH(CAT_CONV0, 2, 0.0, launch_decoar2_features(d_wavs, d_lens, B, (int)fbank_frames(Lmax), T, step,
                                                                w->fb_f32.as<float>(), w->ln512_s.planes(m->scheme), st));
             return 0;
         }
+        // waveform packing (+ normalisation), conv 0 + norm + GELU -> act[0]
         return launch_frontend(m, st, d_wavs, d_lens, B, Lmax, (int)L[0], c.normalize_wav, m->conv0_w.as<float>(),
                                c.conv_bias ? m->conv0_b.as<float>() : nullptr, m->norm0_g.as<float>(),
                                m->norm0_b.as<float>(), c.extractor_layer_norm, w->wav_pad.as<float>(),
                                w->wav_stats.as<float>(), w->c0_part.as<double>(), w->c0_ss.as<float>(),
                                w->act[0].planes(m->scheme));
     }
+    if (m->kind == kGruStack) return apc_stage(s);
+    if (m->kind == kLstmStack) return decoar_stage(s);
+    const int D = c.embed_dim, H = c.num_heads, NL = c.num_layers, C = kConvDim;
+    const double attn_flops = 4.0 * (double)T * T * D * B;
+
     if (s >= 1 && s <= 6) {
         // ---- conv s as implicit GEMM (+ per-frame LayerNorm + GELU in "layer_norm" mode) ----------------------------
-        if (decoar2(m)) return 0;  // no conv stack
+        if (m->kind == kFbankEncoder) return 0;  // no conv stack
         const int i = s;
         GemmParams p = plan->conv[i];
         KGEMM(launch_gemm(p, m->sm_count, st));
@@ -1876,7 +1875,7 @@ int Fwd::stage(int s) {
     }
     if (s == 7) {
         // ---- LayerNorm(512) -> post_extract_proj (+ zero padded frames) --------------------------------------------
-        if (!c.no_feature_layer_norm && !decoar2(m))
+        if (!c.no_feature_layer_norm && m->kind == kConvEncoder)
             KNORM(launch_layernorm(w->conv_f32.as<float>(), (size_t)M, C, m->ln512_g.as<float>(), m->ln512_b.as<float>(),
                                    0, nullptr, w->ln512_s.planes(m->scheme), st));
         GemmParams p = plan->proj;
@@ -2116,10 +2115,14 @@ static int default_lanes(int B, int64_t T) {
     return (long long)B * T >= min_frames ? 2 : 1;
 }
 
+// Lanes a model can run: two grid-resident LSTM launches must never be in flight at once, so a DeCoAR model runs one
+// (its recurrence occupies the whole device)
+static int max_lanes(const s3b_model* m) { return m != nullptr && m->kind == kLstmStack ? 1 : 2; }
+
 extern "C" int32_t s3b_default_lanes(const s3b_model* m, int32_t batch, int64_t max_len) {
     const int64_t T = model_frames(m, max_len);
     if (batch < 1 || T < 1) return -1;
-    return decoar1(m) ? 1 : default_lanes(batch, T);  // DeCoAR's recurrence occupies the whole device
+    return std::min(default_lanes(batch, T), max_lanes(m));
 }
 
 static int forward_lanes(s3b_model* m, const float* const* wavs, const int64_t* lens, int B, int64_t Lmax,
@@ -2127,12 +2130,8 @@ static int forward_lanes(s3b_model* m, const float* const* wavs, const int64_t* 
     const s3b_config& c = m->cfg;
     if (B < 1) return fail("empty batch");
     const int64_t T = model_frames(m, Lmax);
-    if (T < 1) return fail("max_len %lld too short: the %s yields no frame", (long long)Lmax,
-                           decoar2(m) || fbank_all_frames(m) ? "fbank" : "conv stack");
-    int lanes = (o && o->lanes > 0) ? o->lanes : default_lanes(B, T);
-    if (lanes > 2) lanes = 2;
-    // two grid-resident LSTM launches must never be in flight at once: a DeCoAR model runs one lane
-    if (decoar1(m)) lanes = 1;
+    if (T < 1) return fail_too_short(m, Lmax);
+    int lanes = std::min((o && o->lanes > 0) ? (int)o->lanes : default_lanes(B, T), max_lanes(m));
     if (lanes > B) lanes = B;
     const size_t frame = (size_t)T * c.embed_dim;
     const size_t layer_stride = (o && o->layer_stride > 0) ? (size_t)o->layer_stride : (size_t)B * frame;
@@ -2197,20 +2196,21 @@ extern "C" int s3b_forward_ex(s3b_model* m, const float* const* wavs, const int6
                     (int)sizeof(s3b_forward_opts));
     for (int b = 0; b < batch; ++b)
         if (lens[b] > max_len) return fail("lens[%d]=%lld exceeds max_len", b, (long long)lens[b]);
-    if (m->cfg.conformer && opts != nullptr && (opts->ffn_out != nullptr || opts->last_residual != nullptr))
-        return fail("ffn_out / last_residual: a Conformer encoder collects no layer results (wav2vec2_model.py:3199-3200)");
-    if (apc(m) && opts != nullptr && (opts->ffn_out != nullptr || opts->last_residual != nullptr))
-        return fail("ffn_out / last_residual: an APC model is a GRU stack, it has no feed-forward blocks or layer results");
-    if (decoar1(m) && opts != nullptr && (opts->ffn_out != nullptr || opts->last_residual != nullptr))
-        return fail("ffn_out / last_residual: a DeCoAR model is an LSTM stack, it has no feed-forward blocks or layer "
-                    "results");
+    if (opts != nullptr && (opts->ffn_out != nullptr || opts->last_residual != nullptr)) {
+        const char* why =
+            m->kind == kGruStack    ? "an APC model is a GRU stack, it has no feed-forward blocks or layer results"
+            : m->kind == kLstmStack ? "a DeCoAR model is an LSTM stack, it has no feed-forward blocks or layer results"
+            : m->cfg.conformer      ? "a Conformer encoder collects no layer results (wav2vec2_model.py:3199-3200)"
+                                    : nullptr;
+        if (why != nullptr) return fail("ffn_out / last_residual: %s", why);
+    }
     return forward_lanes(m, wavs, lens, batch, max_len, hidden_out, (cudaStream_t)stream, opts);
 }
 
 static int forward_host_impl(s3b_model* m, const float* const* wavs, const int64_t* lens, int32_t batch,
                              int64_t max_len, float* hidden_out, float* hidden_dev) {
     const int64_t T = model_frames(m, max_len);
-    if (T < 1) return fail("max_len too short");
+    if (T < 1) return fail_too_short(m, max_len);
     size_t total = 0;
     for (int b = 0; b < batch; ++b) total += (size_t)lens[b];
     S3B_OK(m->stage_wav.ensure(total * 4));

@@ -12,50 +12,67 @@ this implementation with the reference tree untouched (see INTEGRATION.md).
 """
 from __future__ import annotations
 
-from typing import Callable, Dict, List
+from functools import partial
+from typing import Callable, Dict, List, Optional
 
+from .upstream.apc import ApcExpert
 from .upstream.configs import ALIASES, ARCHS
+from .upstream.decoar import DecoarExpert
+from .upstream.decoar2 import Decoar2Expert
 from .upstream.expert import UpstreamExpert
 
 
-def _make_entry(name: str) -> Callable:
-    def entry(ckpt=None, model_config=None, refresh=False, *args, **kwargs):
+def _entry(name: str, make: Callable, ckpt_required: bool = False, refuse_legacy: bool = False,
+           url_hint: Optional[str] = None) -> Callable:
+    """The hub entry ``name``: ``entry(ckpt, **kwargs)`` returns ``make(ckpt=ckpt, **kwargs)``. A URL is refused (the
+    reference downloads it; remote checkpoints are not reachable here) and the reference's download options
+    ``refresh`` / ``model_config`` are dropped. ``ckpt_required``: a path must be given (``*_local``, ``*_url``,
+    ``*_custom``). ``refuse_legacy``: the entry reads converted fairseq checkpoints of a conv-stack family, and
+    ``legacy=True`` (``hubert_custom``'s un-converted fairseq file, which needs fairseq itself) is refused."""
+
+    def entry(ckpt=None, *args, **kwargs):
+        if ckpt_required:
+            assert isinstance(ckpt, str), f"a {'converted ' if refuse_legacy else ''}checkpoint path is required"
         if isinstance(ckpt, str) and ckpt.startswith("http"):
-            raise ValueError(f"{name}: remote checkpoints are not reachable here; pass a local converted ckpt")
-        return UpstreamExpert(ckpt=ckpt, name=name, model_config=model_config, **kwargs)
+            hint = url_hint or f"download {ckpt} and pass the file"
+            raise ValueError(f"{name}: remote checkpoints are not reachable here; {hint}")
+        kwargs.pop("refresh", None)
+        kwargs.pop("model_config", None)
+        if refuse_legacy and kwargs.pop("legacy", False):
+            raise ValueError(f"{name}: legacy fairseq checkpoints are not supported; convert first "
+                             "(s3prl_b200.upstream.convert.convert_fairseq_checkpoint)")
+        return make(ckpt=ckpt, **kwargs)
 
     entry.__name__ = name
     entry.__doc__ = f"H100-native {name} upstream (s3prl_b200)."
     return entry
 
 
-def _make_local_entry(family: str, suffix: str = "local") -> Callable:
-    """``*_local`` / ``*_custom`` / ``*_url`` (hubert/hubconf.py:57-78 and its siblings): in the reference the latter two
-    download ``ckpt`` when it is a URL and then behave like ``*_local``; there is no network here, so a URL is refused
-    with a message and a path is read as the converted checkpoint it must be."""
-
-    def entry(ckpt, *args, **kwargs):
-        assert isinstance(ckpt, str), "a converted checkpoint path is required"
-        if ckpt.startswith("http"):
-            raise ValueError(f"{family}_{suffix}: remote checkpoints are not reachable here; download {ckpt} and pass the file")
-        kwargs.pop("refresh", None)
-        if kwargs.pop("legacy", False):  # hubert_custom(legacy=True): un-converted fairseq file, needs fairseq itself
-            raise ValueError(f"{family}_{suffix}: legacy fairseq checkpoints are not supported; convert first "
-                             "(s3prl_b200.upstream.convert.convert_fairseq_checkpoint)")
-        return UpstreamExpert(ckpt=ckpt, name=f"{family}_local", **kwargs)
-
-    entry.__name__ = f"{family}_{suffix}"
-    return entry
-
-
 ENTRIES: Dict[str, Callable] = {}
 for _name in list(ARCHS) + list(ALIASES):
-    ENTRIES[_name] = _make_entry(_name)
+    ENTRIES[_name] = _entry(_name, partial(UpstreamExpert, name=_name), url_hint="pass a local converted ckpt")
+# *_local / *_url / *_custom (hubert/hubconf.py:57-78 and its siblings): in the reference the latter two download
+# ckpt when it is a URL and then behave like *_local; here a path is read as the converted checkpoint it must be
 for _family in ("hubert", "wav2vec2", "wavlm", "unispeech_sat", "distiller", "data2vec"):
-    ENTRIES[f"{_family}_local"] = _make_local_entry(_family)
-    ENTRIES[f"{_family}_url"] = _make_local_entry(_family, "url")
-for _family in ("hubert", "wav2vec2", "data2vec"):  # the families whose hubconf defines *_custom
-    ENTRIES[f"{_family}_custom"] = _make_local_entry(_family, "custom")
+    _suffixes = ("local", "url", "custom") if _family in ("hubert", "wav2vec2", "data2vec") else ("local", "url")
+    for _suffix in _suffixes:
+        ENTRIES[f"{_family}_{_suffix}"] = _entry(f"{_family}_{_suffix}", partial(UpstreamExpert, name=f"{_family}_local"),
+                                                 ckpt_required=True, refuse_legacy=True)
+# DeCoAR 2.0 (decoar2/hubconf.py:10-42): the fabricated checkpoint without ckpt, else the local {"model": ...} file
+ENTRIES["decoar2"] = _entry("decoar2", Decoar2Expert, url_hint="pass a local checkpoint file")
+for _suffix in ("local", "url", "custom"):
+    ENTRIES[f"decoar2_{_suffix}"] = _entry(f"decoar2_{_suffix}", Decoar2Expert, ckpt_required=True)
+# APC / VQ-APC (apc/hubconf.py, vq_apc/hubconf.py): the fabricated checkpoint without ckpt, else the local
+# {"config", "model"} file
+for _name, _vq, _required in (("apc", False, False), ("apc_360hr", False, False), ("apc_960hr", False, False),
+                              ("vq_apc", True, False), ("vq_apc_360hr", True, False), ("vq_apc_960hr", True, False),
+                              ("apc_local", False, True), ("apc_url", False, True), ("vq_apc_url", True, True)):
+    ENTRIES[_name] = _entry(_name, partial(ApcExpert, name=_name, vq=_vq), ckpt_required=_required)
+# DeCoAR (decoar/hubconf.py, decoar_layers/hubconf.py): the fabricated checkpoint without ckpt, else the local
+# {"model"} file
+for _family, _all in (("decoar", False), ("decoar_layers", True)):
+    for _name in (_family, f"{_family}_local", f"{_family}_url", f"{_family}_custom"):
+        ENTRIES[_name] = _entry(_name, partial(DecoarExpert, all_layers=_all, name=_name), ckpt_required=_name != _family)
 globals().update(ENTRIES)
 
 
@@ -94,89 +111,6 @@ def linear(*args, **kwargs):
 
 ENTRIES["mel"] = mel
 ENTRIES["linear"] = linear
-
-
-def decoar2(ckpt=None, model_config=None, refresh=False, *args, **kwargs):
-    """DeCoAR 2.0 (s3prl/upstream/decoar2/hubconf.py:34-42): the fabricated checkpoint without ``ckpt``, else the
-    local ``{"model": state_dict}`` file."""
-    from .upstream.decoar2 import Decoar2Expert
-
-    if isinstance(ckpt, str) and ckpt.startswith("http"):
-        raise ValueError("decoar2: remote checkpoints are not reachable here; pass a local checkpoint file")
-    return Decoar2Expert(ckpt=ckpt, **kwargs)
-
-
-def _make_decoar2_file_entry(suffix: str) -> Callable:
-    """decoar2_local / decoar2_url / decoar2_custom (decoar2/hubconf.py:10-31): a local checkpoint file; a URL is refused."""
-
-    def entry(ckpt, *args, **kwargs):
-        from .upstream.decoar2 import Decoar2Expert
-
-        assert isinstance(ckpt, str), "a checkpoint path is required"
-        if ckpt.startswith("http"):
-            raise ValueError(f"decoar2_{suffix}: remote checkpoints are not reachable here; download {ckpt} and pass the file")
-        kwargs.pop("refresh", None)
-        return Decoar2Expert(ckpt=ckpt, **kwargs)
-
-    entry.__name__ = f"decoar2_{suffix}"
-    return entry
-
-
-ENTRIES["decoar2"] = decoar2
-for _suffix in ("local", "url", "custom"):
-    ENTRIES[f"decoar2_{_suffix}"] = _make_decoar2_file_entry(_suffix)
-
-
-def _make_apc_entry(name: str, vq: bool, needs_ckpt: bool) -> Callable:
-    """APC / VQ-APC (apc/hubconf.py, vq_apc/hubconf.py): the fabricated checkpoint without ``ckpt``, else the local
-    ``{"config", "model"}`` file; a URL is refused (remote checkpoints cannot be reached offline)."""
-
-    def entry(ckpt=None, *args, **kwargs):
-        from .upstream.apc import ApcExpert
-
-        if needs_ckpt:
-            assert isinstance(ckpt, str), "a checkpoint path is required"
-        if isinstance(ckpt, str) and ckpt.startswith("http"):
-            raise ValueError(f"{name}: remote checkpoints are not reachable here; download {ckpt} and pass the file")
-        kwargs.pop("refresh", None)
-        kwargs.pop("model_config", None)
-        return ApcExpert(ckpt=ckpt, name=name, vq=vq, **kwargs)
-
-    entry.__name__ = name
-    return entry
-
-
-for _name in ("apc", "apc_360hr", "apc_960hr"):
-    ENTRIES[_name] = _make_apc_entry(_name, False, False)
-for _name in ("vq_apc", "vq_apc_360hr", "vq_apc_960hr"):
-    ENTRIES[_name] = _make_apc_entry(_name, True, False)
-ENTRIES["apc_local"] = _make_apc_entry("apc_local", False, True)
-ENTRIES["apc_url"] = _make_apc_entry("apc_url", False, True)
-ENTRIES["vq_apc_url"] = _make_apc_entry("vq_apc_url", True, True)
-
-
-def _make_decoar_entry(name: str, all_layers: bool, needs_ckpt: bool) -> Callable:
-    """DeCoAR (decoar/hubconf.py, decoar_layers/hubconf.py): the fabricated checkpoint without ``ckpt``, else the
-    local ``{"model"}`` file; a URL is refused (remote checkpoints cannot be reached offline)."""
-
-    def entry(ckpt=None, *args, **kwargs):
-        from .upstream.decoar import DecoarExpert
-
-        if needs_ckpt:
-            assert isinstance(ckpt, str), "a checkpoint path is required"
-        if isinstance(ckpt, str) and ckpt.startswith("http"):
-            raise ValueError(f"{name}: remote checkpoints are not reachable here; download {ckpt} and pass the file")
-        kwargs.pop("refresh", None)
-        return DecoarExpert(ckpt=ckpt, all_layers=all_layers, name=name, **kwargs)
-
-    entry.__name__ = name
-    return entry
-
-
-for _family, _all in (("decoar", False), ("decoar_layers", True)):
-    ENTRIES[_family] = _make_decoar_entry(_family, _all, False)
-    for _suffix in ("local", "url", "custom"):
-        ENTRIES[f"{_family}_{_suffix}"] = _make_decoar_entry(f"{_family}_{_suffix}", _all, True)
 
 
 def options() -> List[str]:

@@ -79,11 +79,8 @@ class S3PRLUpstream(nn.Module):
         self.normalize = normalize
         # Static facts. The reference finds them with a pseudo forward (nn/upstream.py:124-128); that would need a GPU
         # at construction time, and they follow from the architecture anyway.
-        arch = getattr(self.upstream, "arch", None)
-        if arch is not None:  # NL + 1 hidden states; feat_final + layers + prediction heads for the Distiller
-            count, width = arch.num_outputs, self.upstream.hidden_size
-        elif hasattr(self.upstream, "num_layers"):
-            count, width = self.upstream.num_layers + 1, self.upstream.hidden_size
+        if hasattr(self.upstream, "num_outputs"):  # the hidden states of a model-backed expert
+            count, width = self.upstream.num_outputs, self.upstream.hidden_size
         else:  # fbank / mel / linear: one feature sequence
             count, width = 1, self.upstream.output_dim
         stride = self.upstream.get_downsample_rates("hidden_states")

@@ -20,14 +20,13 @@ use a fabricated checkpoint of that shape.
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 from typing import Dict, List, Optional, Tuple
 
 import torch
-import torch.nn as nn
 
 from .. import lib as _lib
+from .expert import NativeExpert
 
 HIDDEN = 512
 NUM_LAYERS = 3
@@ -136,146 +135,47 @@ def load_apc_checkpoint(path: str) -> Tuple[bool, Dict[str, torch.Tensor]]:
     return residual, {k: weights[k] for k in required_keys()}
 
 
-class _ApcNative:
-    """Owner of one APC ``s3b_model`` handle (weights resident on one CUDA device)."""
-
-    def __init__(self, residual: bool, state_dict: Dict[str, torch.Tensor], device: torch.device):
-        self.lib = _lib.load()
-        _lib.require_gpu()
-        self.device = device
-        self.handle = C.c_void_p()
-        cfg = _lib.S3BApcConfig(num_layers=NUM_LAYERS, hidden=HIDDEN, residual=int(residual))
-        _lib.check(self.lib.s3b_apc_model_create(C.byref(cfg), C.byref(self.handle)))
-        try:
-            for name in required_keys():
-                t = state_dict[name].detach().to("cpu", torch.float32).contiguous()
-                shape = (C.c_int64 * t.dim())(*t.shape)
-                _lib.check(self.lib.s3b_model_set_tensor(self.handle, name.encode(), C.c_void_p(t.data_ptr()), shape,
-                                                         t.dim()))
-            with torch.cuda.device(device):
-                _lib.check(self.lib.s3b_model_finalize(self.handle))
-        except Exception:
-            self.close()
-            raise
-
-    def close(self):
-        if getattr(self, "handle", None) is not None and self.handle:
-            self.lib.s3b_model_destroy(self.handle)
-            self.handle = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class ApcExpert(nn.Module):
+class ApcExpert(NativeExpert):
     """``UpstreamExpert`` of APC / VQ-APC: ``expert(wavs)`` on a list of 1-D fp32 CUDA waveforms of at least 560
-    samples. ``lanes``, ``global_max_len`` (sharding) and ``forward_host`` work as for the other experts. The result
-    dict is the reference's: three hidden states [B, T, 512], ``last_hidden_state``, ``hidden_state_{i}`` and
-    ``_hidden_states_info``."""
+    samples. ``lanes``, ``global_max_len`` (sharding), the inference-only refusal, the training-mode warning and
+    ``forward_host`` (its pinned result reused across calls of the same shape) are those of every expert
+    (``NativeExpert``). The result dict is the reference's: three hidden states [B, T, 512], ``last_hidden_state``,
+    ``hidden_state_{i}`` and ``_hidden_states_info``."""
+
+    min_samples = MIN_SAMPLES
+    model_label = "APC"
+    num_layers = num_outputs = NUM_LAYERS  # the output of every GRU layer is a hidden state
+    hidden_size = HIDDEN
 
     def __init__(self, ckpt: Optional[str] = None, name: str = "apc", vq: bool = False, seed: int = 0,
                  randomize_seed: Optional[int] = None, hooks=None, feature_selection=None, **kwargs):
-        super().__init__()
         if hooks or feature_selection is not None:
             raise TypeError("hooks and feature_selection are not available for APC: the reference expert registers "
                             "its three hooks itself (apc/expert.py:27-42); use the default hidden_states")
-        self.name = name
         if ckpt is not None:
             residual, sd = load_apc_checkpoint(ckpt)
         else:
             residual, sd = True, fabricate_apc_state_dict(seed, vq)
         if randomize_seed is not None:  # S3PRLUpstream(randomize=True): fresh weights of the same shape
             sd = fabricate_apc_state_dict(randomize_seed, vq)
+        super().__init__(sd)
+        self.name = name
         self.residual = residual
-        self._state_dict_host = sd
-        self._native: Optional[_ApcNative] = None
-        self.lanes = 0  # 0 = library default; 1 / 2 = utterance micro-batches on that many streams
-        self.global_max_len: Optional[int] = None  # set when a batch is sharded across ranks
-        self.register_buffer("_device_anchor", torch.zeros(1), persistent=False)
 
-    def _ensure_native(self, device: torch.device) -> _ApcNative:
-        if device.type != "cuda":
-            raise _lib.S3BError("s3prl_b200 runs on CUDA devices only (sm_90a); there is no CPU fallback. "
-                                "Move the expert and the waveforms to an H100: expert.to('cuda').")
-        if self._native is None or self._native.device != device:
-            if self._native is not None:
-                self._native.close()
-            self._native = _ApcNative(self.residual, self._state_dict_host, device)
-        return self._native
+    def _native_args(self):
+        cfg = _lib.S3BApcConfig(num_layers=NUM_LAYERS, hidden=HIDDEN, residual=int(self.residual))
+        return "s3b_apc_model_create", cfg, {k: self._state_dict_host[k] for k in required_keys()}
 
     def get_downsample_rates(self, key: str) -> int:
         return DOWNSAMPLE_RATE
 
-    @property
-    def num_layers(self) -> int:
-        return NUM_LAYERS
-
-    @property
-    def hidden_size(self) -> int:
-        return HIDDEN
-
     def num_frames(self, max_len: int) -> int:
         return num_frames(max_len)
 
-    @staticmethod
-    def _check_lengths(wavs) -> None:
-        if len(wavs) == 0:
-            raise ValueError("empty batch")
-        for i, w in enumerate(wavs):
-            if w.numel() < MIN_SAMPLES:
-                raise ValueError(f"utterance {i} has {w.numel()} samples: APC needs >= {MIN_SAMPLES} (two fbank "
-                                 "frames; the reference's CMVN std of a single frame is NaN)")
-
-    @staticmethod
-    def _result(hidden) -> Dict:
+    def forward(self, wavs: List[torch.Tensor]) -> Dict:
+        out = self._forward_ex(*self._prepare(wavs))
+        hidden = tuple(out[i] for i in range(NUM_LAYERS))
         result = {"_hidden_states_info": HIDDEN_STATES_INFO, "hidden_states": hidden, "last_hidden_state": hidden[-1]}
         for i, h in enumerate(hidden):
             result[f"hidden_state_{i}"] = h
         return result
-
-    def forward(self, wavs: List[torch.Tensor]) -> Dict:
-        self._check_lengths(wavs)
-        if any(w.requires_grad for w in wavs):
-            raise _lib.S3BError("s3prl_b200 upstreams are inference-only (frozen upstream)")
-        device = wavs[0].device
-        native = self._ensure_native(device)
-        wavs = [w.detach().to(torch.float32).contiguous() for w in wavs]
-        lens = [int(w.numel()) for w in wavs]
-        B = len(wavs)
-        max_len = self.global_max_len or max(lens)
-        T = num_frames(max_len)
-        with torch.cuda.device(device):
-            out = torch.empty((NUM_LAYERS, B, T, HIDDEN), dtype=torch.float32, device=device)
-            ptrs = (C.c_void_p * B)(*[w.data_ptr() for w in wavs])
-            lens_c = (C.c_int64 * B)(*lens)
-            opts = _lib.S3BForwardOpts(lanes=int(self.lanes))
-            _lib.check(native.lib.s3b_forward_ex(native.handle, ptrs, lens_c, B, max_len, C.c_void_p(out.data_ptr()),
-                                                 C.c_void_p(torch.cuda.current_stream(device).cuda_stream),
-                                                 C.byref(opts)))
-        return self._result(tuple(out[i] for i in range(NUM_LAYERS)))
-
-    def forward_host(self, wavs_host: List[torch.Tensor], keep_device: bool = False):
-        """End-to-end from HOST buffers through ``s3b_forward_host[_ex]``: a pinned host tensor [3, B, T, 512]; with
-        ``keep_device`` also the device-resident copy."""
-        self._check_lengths(wavs_host)
-        native = self._ensure_native(self._device_anchor.device)
-        wavs = [w.detach().to("cpu", torch.float32).contiguous() for w in wavs_host]
-        lens = [int(w.numel()) for w in wavs]
-        B = len(wavs)
-        max_len = self.global_max_len or max(lens)
-        shape = (NUM_LAYERS, B, num_frames(max_len), HIDDEN)
-        out = torch.empty(shape, dtype=torch.float32).pin_memory()
-        ptrs = (C.c_void_p * B)(*[w.data_ptr() for w in wavs])
-        lens_c = (C.c_int64 * B)(*lens)
-        with torch.cuda.device(native.device):
-            if keep_device:
-                dev = torch.empty(shape, dtype=torch.float32, device=native.device)
-                torch.cuda.current_stream(native.device).synchronize()  # the call runs on the library's own streams
-                _lib.check(native.lib.s3b_forward_host_ex(native.handle, ptrs, lens_c, B, max_len,
-                                                          C.c_void_p(out.data_ptr()), C.c_void_p(dev.data_ptr())))
-                return out, dev
-            _lib.check(native.lib.s3b_forward_host(native.handle, ptrs, lens_c, B, max_len, C.c_void_p(out.data_ptr())))
-        return out

@@ -17,14 +17,13 @@ checkpoint is not reachable offline; without a file the experts use a fabricated
 """
 from __future__ import annotations
 
-import ctypes as C
 import math
 from typing import Dict, List, Optional
 
 import torch
-import torch.nn as nn
 
 from .. import lib as _lib
+from .expert import NativeExpert
 
 HIDDEN = 1024
 NUM_LAYERS = 4
@@ -88,71 +87,32 @@ def load_decoar_checkpoint(path: str) -> Dict[str, torch.Tensor]:
     return {k: weights[k] for k in required_keys()}
 
 
-class _DecoarNative:
-    """Owner of one DeCoAR ``s3b_model`` handle (weights resident on one CUDA device)."""
-
-    def __init__(self, all_layers: bool, state_dict: Dict[str, torch.Tensor], device: torch.device):
-        self.lib = _lib.load()
-        _lib.require_gpu()
-        self.device = device
-        self.handle = C.c_void_p()
-        cfg = _lib.S3BDecoarConfig(num_layers=NUM_LAYERS, hidden=HIDDEN, all_layers=int(all_layers))
-        _lib.check(self.lib.s3b_decoar_model_create(C.byref(cfg), C.byref(self.handle)))
-        try:
-            for name in required_keys():
-                t = state_dict[name].detach().to("cpu", torch.float32).contiguous()
-                shape = (C.c_int64 * t.dim())(*t.shape)
-                _lib.check(self.lib.s3b_model_set_tensor(self.handle, name.encode(), C.c_void_p(t.data_ptr()), shape,
-                                                         t.dim()))
-            with torch.cuda.device(device):
-                _lib.check(self.lib.s3b_model_finalize(self.handle))
-        except Exception:
-            self.close()
-            raise
-
-    def close(self):
-        if getattr(self, "handle", None) is not None and self.handle:
-            self.lib.s3b_model_destroy(self.handle)
-            self.handle = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class DecoarExpert(nn.Module):
+class DecoarExpert(NativeExpert):
     """``UpstreamExpert`` of DeCoAR: ``expert(wavs)`` on a list of 1-D fp32 CUDA waveforms of at least 560 samples.
-    ``global_max_len`` (sharding) and ``forward_host`` work as for the other experts; ``lanes`` is accepted but a
-    forward always runs as one lane. The result dict is the reference's: ``hidden_states`` (``decoar``: the last
-    layer; ``decoar_layers`` with ``all_layers``: all four) of shape [B, T, 2048] and ``last_hidden_state``."""
+    ``global_max_len`` (sharding), the inference-only refusal, the training-mode warning and ``forward_host`` (its
+    pinned result reused across calls of the same shape) are those of every expert (``NativeExpert``); ``lanes`` is
+    accepted but a forward always runs as one lane. The result dict is the reference's: ``hidden_states``
+    (``decoar``: the last layer; ``decoar_layers`` with ``all_layers``: all four) of shape [B, T, 2048] and
+    ``last_hidden_state``."""
+
+    min_samples = MIN_SAMPLES
+    model_label = "DeCoAR"
+    hidden_size = OUTPUT_DIM
 
     def __init__(self, ckpt: Optional[str] = None, all_layers: bool = False, name: Optional[str] = None,
                  seed: int = 0, randomize_seed: Optional[int] = None, hooks=None, feature_selection=None, **kwargs):
-        super().__init__()
         if hooks or feature_selection is not None:
             raise TypeError("hooks and feature_selection are not available for DeCoAR: use the default hidden_states")
-        self.name = name or ("decoar_layers" if all_layers else "decoar")
-        self.all_layers = bool(all_layers)
         sd = load_decoar_checkpoint(ckpt) if ckpt is not None else fabricate_decoar_state_dict(seed)
         if randomize_seed is not None:  # S3PRLUpstream(randomize=True): fresh weights of the same shape
             sd = fabricate_decoar_state_dict(randomize_seed)
-        self._state_dict_host = sd
-        self._native: Optional[_DecoarNative] = None
-        self.lanes = 0  # accepted for symmetry with the other experts; the library runs DeCoAR as one lane
-        self.global_max_len: Optional[int] = None  # set when a batch is sharded across ranks
-        self.register_buffer("_device_anchor", torch.zeros(1), persistent=False)
+        super().__init__(sd)
+        self.name = name or ("decoar_layers" if all_layers else "decoar")
+        self.all_layers = bool(all_layers)
 
-    def _ensure_native(self, device: torch.device) -> _DecoarNative:
-        if device.type != "cuda":
-            raise _lib.S3BError("s3prl_b200 runs on CUDA devices only (sm_90a); there is no CPU fallback. "
-                                "Move the expert and the waveforms to an H100: expert.to('cuda').")
-        if self._native is None or self._native.device != device:
-            if self._native is not None:
-                self._native.close()
-            self._native = _DecoarNative(self.all_layers, self._state_dict_host, device)
-        return self._native
+    def _native_args(self):
+        cfg = _lib.S3BDecoarConfig(num_layers=NUM_LAYERS, hidden=HIDDEN, all_layers=int(self.all_layers))
+        return "s3b_decoar_model_create", cfg, {k: self._state_dict_host[k] for k in required_keys()}
 
     def get_downsample_rates(self, key: str) -> int:
         return DOWNSAMPLE_RATE
@@ -161,67 +121,9 @@ class DecoarExpert(nn.Module):
     def num_outputs(self) -> int:
         return NUM_LAYERS if self.all_layers else 1
 
-    @property
-    def hidden_size(self) -> int:
-        return OUTPUT_DIM
-
     def num_frames(self, max_len: int) -> int:
         return num_frames(max_len)
 
-    @staticmethod
-    def _check_lengths(wavs) -> None:
-        if len(wavs) == 0:
-            raise ValueError("empty batch")
-        for i, w in enumerate(wavs):
-            if w.numel() < MIN_SAMPLES:
-                raise ValueError(f"utterance {i} has {w.numel()} samples: DeCoAR needs >= {MIN_SAMPLES} (two fbank "
-                                 "frames; the reference's CMVN std of a single frame is NaN)")
-
-    @staticmethod
-    def _result(hidden) -> Dict:
-        return {"hidden_states": list(hidden), "last_hidden_state": hidden[-1]}
-
     def forward(self, wavs: List[torch.Tensor]) -> Dict:
-        self._check_lengths(wavs)
-        if any(w.requires_grad for w in wavs):
-            raise _lib.S3BError("s3prl_b200 upstreams are inference-only (frozen upstream)")
-        device = wavs[0].device
-        native = self._ensure_native(device)
-        wavs = [w.detach().to(torch.float32).contiguous() for w in wavs]
-        lens = [int(w.numel()) for w in wavs]
-        B = len(wavs)
-        max_len = self.global_max_len or max(lens)
-        T = num_frames(max_len)
-        n = self.num_outputs
-        with torch.cuda.device(device):
-            out = torch.empty((n, B, T, OUTPUT_DIM), dtype=torch.float32, device=device)
-            ptrs = (C.c_void_p * B)(*[w.data_ptr() for w in wavs])
-            lens_c = (C.c_int64 * B)(*lens)
-            opts = _lib.S3BForwardOpts(lanes=int(self.lanes))
-            _lib.check(native.lib.s3b_forward_ex(native.handle, ptrs, lens_c, B, max_len, C.c_void_p(out.data_ptr()),
-                                                 C.c_void_p(torch.cuda.current_stream(device).cuda_stream),
-                                                 C.byref(opts)))
-        return self._result(tuple(out[i] for i in range(n)))
-
-    def forward_host(self, wavs_host: List[torch.Tensor], keep_device: bool = False):
-        """End-to-end from HOST buffers through ``s3b_forward_host[_ex]``: a pinned host tensor
-        [num_outputs, B, T, 2048]; with ``keep_device`` also the device-resident copy."""
-        self._check_lengths(wavs_host)
-        native = self._ensure_native(self._device_anchor.device)
-        wavs = [w.detach().to("cpu", torch.float32).contiguous() for w in wavs_host]
-        lens = [int(w.numel()) for w in wavs]
-        B = len(wavs)
-        max_len = self.global_max_len or max(lens)
-        shape = (self.num_outputs, B, num_frames(max_len), OUTPUT_DIM)
-        out = torch.empty(shape, dtype=torch.float32).pin_memory()
-        ptrs = (C.c_void_p * B)(*[w.data_ptr() for w in wavs])
-        lens_c = (C.c_int64 * B)(*lens)
-        with torch.cuda.device(native.device):
-            if keep_device:
-                dev = torch.empty(shape, dtype=torch.float32, device=native.device)
-                torch.cuda.current_stream(native.device).synchronize()  # the call runs on the library's own streams
-                _lib.check(native.lib.s3b_forward_host_ex(native.handle, ptrs, lens_c, B, max_len,
-                                                          C.c_void_p(out.data_ptr()), C.c_void_p(dev.data_ptr())))
-                return out, dev
-            _lib.check(native.lib.s3b_forward_host(native.handle, ptrs, lens_c, B, max_len, C.c_void_p(out.data_ptr())))
-        return out
+        out = self._forward_ex(*self._prepare(wavs))
+        return {"hidden_states": [out[i] for i in range(self.num_outputs)], "last_hidden_state": out[-1]}

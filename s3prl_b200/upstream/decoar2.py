@@ -70,6 +70,9 @@ class Decoar2Expert(UpstreamExpert):
     """``UpstreamExpert`` of DeCoAR 2.0: ``expert(wavs)`` on a list of 1-D fp32 CUDA waveforms of at least 560
     samples. ``lanes``, ``global_max_len`` (sharding) and ``forward_host`` work as for the wav2vec 2.0 experts."""
 
+    min_samples = MIN_SAMPLES
+    model_label = "DeCoAR 2.0"
+
     def __init__(self, ckpt: Optional[str] = None, randomize_seed: Optional[int] = None, seed: int = 0, **kwargs):
         # the reference's expert swallows every other keyword (decoar2/expert.py:19); so does this one
         if randomize_seed is not None:  # S3PRLUpstream(randomize=True): fresh weights of the same architecture
@@ -85,20 +88,3 @@ class Decoar2Expert(UpstreamExpert):
 
     def num_frames(self, max_len: int) -> int:
         return num_frames(max_len)
-
-    @staticmethod
-    def _check_lengths(wavs) -> None:
-        for i, w in enumerate(wavs):
-            if w.numel() < MIN_SAMPLES:
-                raise ValueError(
-                    f"utterance {i} has {w.numel()} samples: DeCoAR 2.0 needs >= {MIN_SAMPLES} (two fbank frames; the "
-                    "reference's CMVN std of a single frame is NaN)"
-                )
-
-    def forward(self, wavs: List[torch.Tensor]):
-        self._check_lengths(wavs)
-        return super().forward(wavs)
-
-    def forward_host(self, wavs_host: List[torch.Tensor], keep_device: bool = False):
-        self._check_lengths(wavs_host)
-        return super().forward_host(wavs_host, keep_device)

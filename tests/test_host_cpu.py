@@ -467,13 +467,20 @@ def test_s3prl_upstream_bookkeeping_matches_reference_class():
 
 def test_s3prl_upstream_wrapper_layer_counts():
     """S3PRLUpstream's static facts without a device: NL + 1 entries for the encoders, feat_final + layers + prediction
-    heads for DistilHuBERT (s3prl/upstream/distiller/expert.py:44-63), one for fbank."""
+    heads for DistilHuBERT (s3prl/upstream/distiller/expert.py:44-63), the hidden states the recurrent experts return
+    (APC: three, DeCoAR: the last layer or all four), one for fbank."""
     from s3prl_b200.nn import S3PRLUpstream
 
     assert S3PRLUpstream("hubert_base").num_layers == 13
     assert S3PRLUpstream("data2vec_large_ll60k").num_layers == 25
     d = S3PRLUpstream("distilhubert_base")
     assert d.num_layers == 6 and d.hidden_sizes == [768] * 6 and d.downsample_rates == [320] * 6
+    for name, count, width, stride in (("apc", 3, 512, 160), ("vq_apc", 3, 512, 160), ("decoar", 1, 2048, 160),
+                                       ("decoar_layers", 4, 2048, 160), ("decoar2", 13, 768, 320)):
+        u = S3PRLUpstream(name)
+        assert (u.num_layers, u.hidden_sizes, u.downsample_rates) == (count, [width] * count, [stride] * count), name
+    f = S3PRLUpstream("fbank")
+    assert (f.num_layers, f.hidden_sizes) == (1, [240])
 
 
 def _reference_install():
