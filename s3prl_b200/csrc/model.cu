@@ -18,6 +18,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <functional>
 #include <map>
 #include <memory>
 #include <string>
@@ -35,7 +36,6 @@ using namespace s3b;
 // errors
 // ------------------------------------------------------------------------------------------------
 static thread_local std::string g_last_error;
-static int g_sm_count = 132;  // SM count of the device in use (refreshed by s3b_model_finalize)
 
 static int fail(const char* fmt, ...) {
     char buf[1024];
@@ -222,27 +222,21 @@ struct Profiler {
     }
 };
 
-// Cached launch plan: every tensor map / GEMM descriptor of one forward at a given (B, Lmax).
+// Cached launch plan: the forward of one lane at a given (B, Lmax) as an ordered list of steps (build_steps).
 // Encoding the ~22 CUtensorMaps of a layer costs ~300 driver calls per forward; they only depend on the workspace
 // addresses, the weights and (B, T), so they are built once per shape and reused (ragged training batches change
-// Lmax every step and rebuild; fixed-shape serving never does). Pointers into the caller's hidden_out buffer are
-// plain epilogue fields and are patched per call.
-struct LayerPlan {
-    GemmParams qkv, out, fc1, fc2;
-    AttnParams attn;
-    GemmParams v, ffn1_a, ffn1_b, pw1, pw2;  // Conformer (qkv = [q | k], fc1 / fc2 = ffn2)
-};
+// Lmax every step and rebuild; fixed-shape serving never does).
+struct Fwd;
+using Step = std::function<int(Fwd&)>;
 struct Plan {
     int B = 0;
     int64_t Lmax = 0;
     uint64_t gen = 0;
-    GemmParams conv[kNumConv];
-    GemmParams proj, pos;
-    GemmParams pos_d[8];             // data2vec: one four-taps GEMM per conv block (pos_conv_depth <= 8)
-    std::vector<LayerPlan> layers;
-    GemmParams pred1;                // Distiller: Linear(D, N*D) + GELU
-    std::vector<GemmParams> pred2;   // Distiller: SplitLinear, one [D][D] GEMM per task
-    std::vector<GemmParams> gru_in;  // APC / DeCoAR: the input projection of every recurrent layer (and direction)
+    // A step enqueues its kernels on the stream of the Fwd it is handed. It may capture only what the plan key fixes:
+    // weights, workspace and bookkeeping-block addresses, B, T, M, L[] and the tensor maps built from them. Everything
+    // else it reads per call from that Fwd: the stream, the output slots (slot(), hs(), proj_out()), ffn_out /
+    // ffn_stride, last_res and layer_done / user.
+    std::vector<Step> steps;
 };
 
 // Per-lane working set. A forward call runs the batch as one or two utterance micro-batches ("lanes"): lane 0 on
@@ -948,7 +942,6 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
     if (prop.major != 9 || prop.minor != 0)
         return fail("device is sm_%d%d; this library contains sm_90a code only", prop.major, prop.minor);
     m->sm_count = prop.multiProcessorCount;
-    g_sm_count = m->sm_count;
     switch (m->kind) {
     case kGruStack: S3B_OK(finalize_apc(m)); break;
     case kLstmStack: S3B_OK(finalize_decoar(m)); break;
@@ -1056,6 +1049,18 @@ struct Epi {
     OutPlanes op = no_planes();  // GEMM-operand output (either format)
 };
 
+// the two common epilogues: an fp32 output (+ bias, + residual), or operand planes (+ bias, + activation)
+static Epi epi_f32(float* out, const float* bias = nullptr, const float* residual = nullptr) {
+    Epi e;
+    e.out_f32 = out, e.bias = bias, e.residual = residual;
+    return e;
+}
+static Epi epi_planes(const OutPlanes& op, const float* bias = nullptr, int gelu = 0) {
+    Epi e;
+    e.op = op, e.bias = bias, e.gelu = gelu;
+    return e;
+}
+
 static void set_epi(GemmParams& p, const Epi& e, int ldo) {
     p.bias = e.bias, p.residual = e.residual, p.row_mask = e.row_mask, p.gelu = e.gelu;
     p.out_f32 = e.out_f32, p.out_hi = e.op.hi, p.out_lo = e.op.lo, p.out_h8 = e.op.h8, p.out_l8 = e.op.l8;
@@ -1074,9 +1079,7 @@ static float q_scale(int hd) { return hd == 64 ? kQScale : (float)(1.44269504088
 static void set_qkv_epi(GemmParams& p, const float* bias, int T, int H, int hd, const SplitBuf& q, const SplitBuf& k,
                         const SplitBuf& vt, int col0 = 0) {
     const int D = H * hd;
-    Epi e;
-    e.bias = bias;
-    set_epi(p, e, 3 * D);
+    set_epi(p, epi_f32(nullptr, bias), 3 * D);
     p.qkv_mode = 1, p.T = T, p.Tp = (T + 7) & ~7, p.H = H, p.D = D, p.q_scale = q_scale(hd), p.qkv_col0 = col0;
     p.hd = hd, p.hd_magic = 0xFFFFFFFFu / (unsigned)hd + 1u, p.qk_head_step = (T - 1) * hd;
     p.q_hi = q.h(), p.q_lo = q.l(), p.k_hi = k.h(), p.k_lo = k.l();
@@ -1133,16 +1136,17 @@ static int pick_cluster_n(int bn, int n_tiles, int preferred) {
         if (_r != 0) return fail("cuTensorMapEncodeTiled failed (%d) at %s:%d", _r, __FILE__, __LINE__); \
     } while (0)
 
-// out[M][N] = A[M][K] * W[N][K]^T, flat token-major A (hi/lo planes), K % 64 == 0
+// out[M][N] = A[M][K] * W[N][K]^T with epilogue `e`, flat token-major A (hi/lo planes), K % 64 == 0
 // scheme 1: A and W are f16q8 operands (SplitBuf fmt 1), K % 128 == 0, tile width 128 or 256.
+// sm_count: SMs of the device the GEMM runs on (pick_bn's tile-width rule).
 // lda / a_off: A is the [M][K] column slice starting at element a_off of rows that are lda elements apart (0 = dense).
 // forced_bn: the tile width pick_bn takes wherever it divides N (0 = the rule's choice).
-static int linear_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int64_t M, int N, int K, int scheme = 0,
-                         int64_t lda = 0, size_t a_off = 0, int forced_bn = 0) {
+static int linear_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int64_t M, int N, int K, int scheme,
+                         int sm_count, const Epi& e, int64_t lda = 0, size_t a_off = 0, int forced_bn = 0) {
     memset(&p, 0, sizeof(p));
     if (lda == 0) lda = K;
     if (K % 64 != 0 || N % 16 != 0) return fail("linear: K %% 64 or N %% 16 violated (N=%d K=%d)", N, K);
-    const int bn = pick_bn(M, N, K, scheme, g_sm_count, forced_bn);
+    const int bn = pick_bn(M, N, K, scheme, sm_count, forced_bn);
     const int cn = pick_cluster_n(bn, N / bn, scheme != 0 ? 2 : 1);
     const uint32_t a_box = 128 / cn;
     if (scheme != 0) {
@@ -1167,13 +1171,14 @@ static int linear_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, in
     p.a_row_step = 0, p.a_row_off = 0, p.a_k_per_ntile = 0, p.b_n_tiled = 1, p.b_z_per_ntile = 0;
     p.out_rows_per_batch = (int)M;
     p.alg_flops = 2.0 * (double)M * N * K;
+    set_epi(p, e, N);
     return 0;
 }
 
-// conv i (k in {2,3}, stride 2) over channels-last [B][Lin][512]: row t of the [ceil(Lin/2)][1024] view holds
-// samples (2t, 2t+1); taps 0,1 come from view row t, tap 2 from the first half of view row t+1.
+// conv i (k in {2,3}, stride 2) over channels-last [B][Lin][512] with epilogue `e`: row t of the [ceil(Lin/2)][1024]
+// view holds samples (2t, 2t+1); taps 0,1 come from view row t, tap 2 from the first half of view row t+1.
 static int conv_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int B, int64_t Lin, int64_t Lout, int kw,
-                       int scheme = 0) {
+                       int scheme, const Epi& e) {
     memset(&p, 0, sizeof(p));
     const int C = kConvDim, K = kw * C;
     const uint64_t rows = (uint64_t)((Lin + 1) / 2);
@@ -1206,6 +1211,7 @@ static int conv_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int 
     p.a_row_step = 1, p.a_row_off = 0, p.a_k_per_ntile = 0, p.b_n_tiled = 1, p.b_z_per_ntile = 0, p.b_k_linear = 1;
     p.out_rows_per_batch = (int)Lout;
     p.alg_flops = 2.0 * (double)B * Lout * C * K;
+    set_epi(p, e, C);
     return 0;
 }
 
@@ -1221,7 +1227,7 @@ static int pos_taps4(const s3b_config& c) { return (pos_taps(c) + 3) / 4 * 4; }
 // group's channels (or, for the last group, past D: TMA zero fill), which meet the zero-padded weights of posconv_kc.
 // The tile is exactly the group's cpg columns wide, so no output column lands in a neighbouring group.
 static int posconv_params(GemmParams& p, const s3b_config& c, const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo,
-                          const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, int B, int T) {
+                          const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, int B, int T, const Epi& e) {
     memset(&p, 0, sizeof(p));
     const int D = c.embed_dim, G = c.pos_conv_groups, cpg = D / G, Kp = c.pos_conv_kernel, Kc = posconv_kc(cpg);
     TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, x_hi, D, T, B, D, (uint64_t)T * D, 64, 128));
@@ -1233,6 +1239,7 @@ static int posconv_params(GemmParams& p, const s3b_config& c, const __nv_bfloat1
     p.a_row_step = 1, p.a_row_off = -(Kp / 2), p.a_k_per_ntile = cpg, p.b_n_tiled = 0, p.b_z_per_ntile = Kp;
     p.out_rows_per_batch = T;
     p.alg_flops = 2.0 * (double)B * T * D * cpg * Kp;
+    set_epi(p, e, D);
     return 0;
 }
 
@@ -1248,7 +1255,7 @@ static bool posconv4_ok(const s3b_config& c) {
     return c.pos_conv_kernel % 4 == 0 && (4 * cpg == 192 || 4 * cpg == 256);
 }
 static int posconv4_params(GemmParams& p, const s3b_config& c, const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo,
-                           const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, int B, int T) {
+                           const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, int B, int T, const Epi& e) {
     memset(&p, 0, sizeof(p));
     const int D = c.embed_dim, G = c.pos_conv_groups, cpg = D / G, Kq = pos_taps4(c) / 4, bn = 4 * cpg;
     TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, x_hi, D, T, B, D, (uint64_t)T * D, 64, 128));
@@ -1261,6 +1268,7 @@ static int posconv4_params(GemmParams& p, const s3b_config& c, const __nv_bfloat
     p.out_rows_per_batch = T + 3;
     p.k_steps = (cpg + 15) / 16;  // 48 channels per group: the 4th k-step of every 64-wide box has zero weights
     p.alg_flops = 2.0 * (double)B * T * D * cpg * pos_taps(c);
+    set_epi(p, e, 4 * D);
     return 0;
 }
 
@@ -1283,19 +1291,17 @@ static inline void prof_end(s3b_model* m, cudaStream_t st, int cat, int nkernels
     m->prof.launches[cat] += nkernels;
     m->prof.flops[cat] += flops;
 }
-#define KLAUNCH(cat, nk, fl, expr) \
-    do {                           \
-        prof_begin(m, st);         \
-        CUDA_OK(expr);             \
-        prof_end(m, st, cat, nk, fl); \
+// One launch `expr` on stream st, accounted to model m as nk kernels of category cat and fl FLOPs
+#define KLAUNCH(m, st, cat, nk, fl, expr) \
+    do {                                  \
+        prof_begin(m, st);                \
+        CUDA_OK(expr);                    \
+        prof_end(m, st, cat, nk, fl);     \
     } while (0)
-#define KGEMM(expr) KLAUNCH(CAT_GEMM, 1, p.alg_flops, expr)
-#define KATTN(expr) KLAUNCH(CAT_ATTN, 1, attn_flops, expr)
-#define KNORM(expr) KLAUNCH(CAT_NORM, 1, 0.0, expr)
-#define KCONV0(nk, expr) KLAUNCH(CAT_CONV0, nk, conv0_flops, expr)
-#define KMISC(expr) KLAUNCH(CAT_MISC, 1, 0.0, expr)
+#define KNORM(m, st, expr) KLAUNCH(m, st, CAT_NORM, 1, 0.0, expr)
+#define KMISC(m, st, expr) KLAUNCH(m, st, CAT_MISC, 1, 0.0, expr)
 
-// The feature extractor's front end (Fwd::stage(0), s3b_frontend_f32): B ragged waveforms packed into
+// The feature extractor's front end (add_conv_frontend, s3b_frontend_f32): B ragged waveforms packed into
 // wav_pad [B][Lmax] (+ per-utterance normalisation), then conv 0 (w [512][10]) with GroupNorm(512, 512) over all
 // L0 frames (layer_norm 0) or per-frame LayerNorm(512) (layer_norm 1), GELU, written to operand planes `op`.
 // Workspaces: wav_stats [B][2], c0_part conv0_ws_part_bytes(B, L0), c0_ss [2][B][512] (GroupNorm only).
@@ -1304,32 +1310,51 @@ static int launch_frontend(s3b_model* m, cudaStream_t st, const float* const* d_
                            const float* beta, int layer_norm, float* wav_pad, float* wav_stats, double* c0_part,
                            float* c0_ss, const OutPlanes& op) {
     const double conv0_flops = 2.0 * kConvK[0] * kConvDim * (double)B * L0;
-    KMISC(launch_wav_pack(d_wavs, d_lens, B, Lmax, normalize, wav_stats, wav_pad, st));
+    KMISC(m, st, launch_wav_pack(d_wavs, d_lens, B, Lmax, normalize, wav_stats, wav_pad, st));
     if (layer_norm) {
-        KCONV0(1, launch_conv0_layernorm(wav_pad, B, Lmax, L0, w, bias, gamma, beta, op, st));
+        KLAUNCH(m, st, CAT_CONV0, 1, conv0_flops, launch_conv0_layernorm(wav_pad, B, Lmax, L0, w, bias, gamma, beta, op, st));
     } else {
         // a conv-0 bias (conv_bias with extractor_mode "default") is removed again by the per-channel GroupNorm
         // mean: it cancels exactly in (z + b) - mean(z + b), so the kernel never adds it
-        KCONV0(3, launch_conv0_groupnorm(wav_pad, B, Lmax, L0, w, gamma, beta, c0_part, c0_ss, op, st));
+        KLAUNCH(m, st, CAT_CONV0, 3, conv0_flops,
+                launch_conv0_groupnorm(wav_pad, B, Lmax, L0, w, gamma, beta, c0_part, c0_ss, op, st));
     }
     return 0;
 }
 
 // ------------------------------------------------------------------------------------------------
-// forward (one lane = one utterance micro-batch) as a sequence of stages
+// forward (one lane = one utterance micro-batch) as an ordered list of steps
 // ------------------------------------------------------------------------------------------------
 // layer_done: optional callback fired (host side) right after hidden state `l` has been enqueued completely
 typedef int (*LayerDoneFn)(s3b_model*, int l, cudaStream_t st, void* user);
 
-struct Fwd {
-    // inputs
+// What a lane's plan is built for: the model, the lane's workspace, the shape and what follows from it, and the
+// device addresses of the bookkeeping block. Steps capture these by value.
+struct Lane {
     s3b_model* m = nullptr;
     Workspace* w = nullptr;
+    int B = 0;
+    int64_t Lmax = 0;
+    int64_t L[kNumConv];
+    int T = 0;
+    int64_t M = 0;
+    const float** d_wavs = nullptr;
+    long long* d_lens = nullptr;
+    int* d_kv = nullptr;
+    int* d_ord = nullptr;  // APC / DeCoAR: utterances longest first (the recurrence kernels' grouping)
+    uint8_t* d_mask = nullptr;
+    // a [M][N] linear of the model's operand scheme, tiled for its device
+    int linear(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int N, int K, const Epi& e, int64_t lda = 0,
+               size_t a_off = 0) const {
+        return linear_params(p, A, W, M, N, K, m->scheme, m->sm_count, e, lda, a_off);
+    }
+};
+
+// One forward call of one lane: the Lane, and what may change from call to call
+struct Fwd : Lane {
     cudaStream_t st = nullptr;
     const float* const* wavs = nullptr;  // host array of device pointers (this lane's utterances)
     const int64_t* lens = nullptr;
-    int B = 0;
-    int64_t Lmax = 0;
     float* hidden = nullptr;   // this lane's first utterance inside hidden state 0
     size_t layer_stride = 0;   // elements between consecutive hidden states
     float* ffn_out = nullptr;  // optional: fc2 output (+bias) before the residual add, [NL][...] like hidden
@@ -1337,27 +1362,8 @@ struct Fwd {
     float* last_res = nullptr;  // optional (pre-LN models): un-normalised output of the last layer
     LayerDoneFn layer_done = nullptr;
     void* user = nullptr;
-    // derived
-    int64_t L[kNumConv];
-    int T = 0, Tp = 0;
-    int64_t M = 0;
     Plan* plan = nullptr;
-    const float** d_wavs = nullptr;
-    long long* d_lens = nullptr;
-    int* d_kv = nullptr;
-    int* d_ord = nullptr;  // APC / DeCoAR: utterances longest first (the recurrence kernels' grouping)
-    uint8_t* d_mask = nullptr;
 
-    static constexpr int kConformerStages = 10;  // stages per Conformer layer (conformer_stage)
-    int num_stages() const {
-        switch (m->kind) {
-        case kGruStack: return 1 + 2 * m->cfg.num_layers;  // front end, then per layer: input GEMM, recurrence
-        case kLstmStack: return 2 + 4 * m->cfg.num_layers;  // front end, post_extract_proj, per layer and direction: GEMM, recurrence
-        default:
-            if (m->cfg.conformer) return 9 + kConformerStages * m->cfg.num_layers;
-            return 9 + 5 * m->cfg.num_layers + (m->cfg.pred_heads > 0 ? 1 + m->cfg.pred_heads : 0);
-        }
-    }
     bool distil() const { return m->cfg.family == 3; }
     // Output slot i of the caller's buffer. Hidden state l (the input of layer l / the encoder output) lives in slot l —
     // except for the distiller, whose slot 0 is feat_final and whose layer-0 input is not exposed (internal scratch).
@@ -1366,15 +1372,13 @@ struct Fwd {
     float* proj_out() const {
         return (distil() || (m->cfg.conformer && m->cfg.layer_norm_first)) ? slot(0) : w->x_f32.as<float>();
     }
-    int prepare();
-    int build_plan(Plan& pl);
-    int build_conformer_layer(LayerPlan& lp, int l);
-    int stage(int s);
-    int conformer_stage(int l, int sub);
-    int apc_stage(int s);
-    int decoar_stage(int s);
     float* hs(int l) const { return (distil() && l == 0) ? w->hs0.as<float>() : slot(l); }
+    // hidden state l has been enqueued completely
+    int done(int l) const { return layer_done != nullptr ? layer_done(m, l, st, user) : 0; }
+    int prepare();
 };
+
+static int build_steps(const Lane& lane, std::vector<Step>& steps);
 
 int Fwd::prepare() {
     const s3b_config& c = m->cfg;
@@ -1391,7 +1395,7 @@ int Fwd::prepare() {
     if ((int64_t)B * (fb ? fbank_frames(Lmax) : L[0]) > 2000000000LL) return fail("batch too large for 32-bit tile indexing");
     T = (int)T64;
     M = (int64_t)B * T;
-    Tp = (T + 7) & ~7;
+    const int Tp = (T + 7) & ~7;
     if (layer_stride == 0) layer_stride = (size_t)M * D;
     if (ffn_out != nullptr && ffn_stride == 0) ffn_stride = (size_t)M * D;
     if (c.relative_position && T > m->rel_table_T) S3B_OK(build_rel_table(m, 2 * T));
@@ -1502,7 +1506,7 @@ int Fwd::prepare() {
     }
     if (plan == nullptr) {
         std::unique_ptr<Plan> pl(new Plan());
-        S3B_OK(build_plan(*pl));
+        S3B_OK(build_steps(*this, pl->steps));
         pl->B = B, pl->Lmax = Lmax, pl->gen = g_alloc_generation;
         w->plans.insert(w->plans.begin(), std::move(pl));
         if (w->plans.size() > 4) w->plans.pop_back();
@@ -1536,565 +1540,475 @@ static int attn_params(AttnParams& ap, const Workspace* w, int B, int T, int H, 
     return 0;
 }
 
-// One Conformer layer (wav2vec2_model.py:537-578) as nine GEMMs. Residual stream: hidden state l -> r1 (x1_f32, after
-// ffn1) -> r2 (x_f32, after attention) -> r3 (x1_f32, after the conv module) -> r4 (tmp_f32, after ffn2) ->
-// final_layer_norm -> hidden state l+1. Operand planes: xs_s = LayerNorm outputs, x1_s = rope(LN) / depthwise output.
-int Fwd::build_conformer_layer(LayerPlan& lp, int l) {
+// one GEMM of a step on the call's stream
+static int run_gemm(const Fwd& f, const GemmParams& p) {
+    KLAUNCH(f.m, f.st, CAT_GEMM, 1, p.alg_flops, launch_gemm(p, f.m->sm_count, f.st));
+    return 0;
+}
+
+// the bookkeeping block prepare() left in the pinned mirror, copied ahead of everything else on the lane's stream
+static int copy_book(const Lane& lane, cudaStream_t st) {
+    Workspace* w = lane.w;
+    const size_t book_bytes = (size_t)(reinterpret_cast<char*>(lane.d_mask) - w->book.as<char>()) + (size_t)lane.M;
+    CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host.get(), book_bytes, cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaEventRecord(w->book_copied.get(), st));
+    return 0;
+}
+
+// ConvFeatureExtractionModel.forward: waveform packing (+ normalisation) and conv 0 + norm + GELU -> act[0], then conv
+// 1..6 as implicit GEMMs (+ per-frame LayerNorm + GELU in "layer_norm" mode), one step each
+static int add_conv_frontend(const Lane& lane, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    Workspace* w = lane.w;
     const s3b_config& c = m->cfg;
-    const int D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, sch = m->scheme;
-    LayerW& W = m->layers[l];
-    {   // ffn1.w_1 + SiLU
-        GemmParams& p = lp.ffn1_a;
-        S3B_OK(linear_params(p, w->xs_s, W.ffn1_w1, M, F, D, sch));
-        Epi e;
-        e.bias = W.ffn1_b1.as<float>(), e.gelu = 2, e.op = w->h_s.planes(sch);
-        set_epi(p, e, F);
-    }
-    {   // r1 = x + 0.5 ffn1 (0.5 folded into w_2; residual = hidden state l, patched per call)
-        GemmParams& p = lp.ffn1_b;
-        S3B_OK(linear_params(p, w->h_s, W.ffn1_w2, M, D, F, sch));
-        Epi e;
-        e.bias = W.ffn1_b2.as<float>(), e.out_f32 = w->x1_f32.as<float>();
-        set_epi(p, e, D);
-    }
-    {   // [q | k] from rope(LN(r1)), v from LN(r1)
-        GemmParams& p = lp.qkv;
-        S3B_OK(linear_params(p, w->x1_s, W.qkv, M, 2 * D, D, sch));
-        set_qkv_epi(p, W.qkv_b.as<float>(), T, H, 64, w->q_s, w->k_s, w->vt_s, 0);
-        GemmParams& pv = lp.v;
-        S3B_OK(linear_params(pv, w->xs_s, W.v, M, D, D, sch));
-        set_qkv_epi(pv, W.qkv_b.as<float>() + 2 * D, T, H, 64, w->q_s, w->k_s, w->vt_s, 2 * D);
-    }
-    S3B_OK(attn_params(lp.attn, w, B, T, H, 64, d_kv, sch));
-    {   // r2 = r1 + linear_out(attn)
-        GemmParams& p = lp.out;
-        S3B_OK(linear_params(p, w->ctx_s, W.out, M, D, D, sch));
-        Epi e;
-        e.bias = W.out_b.as<float>(), e.residual = w->x1_f32.as<float>(), e.out_f32 = w->x_f32.as<float>();
-        set_epi(p, e, D);
-    }
-    {   // pointwise_conv1 (no bias) -> fp32 [M][2D], the depthwise kernel's input
-        GemmParams& p = lp.pw1;
-        S3B_OK(linear_params(p, w->xs_s, W.pw1, M, 2 * D, D, sch));
-        Epi e;
-        e.out_f32 = w->glu_f32.as<float>();
-        set_epi(p, e, 2 * D);
-    }
-    {   // r3 = r2 + pointwise_conv2 (no bias)
-        GemmParams& p = lp.pw2;
-        S3B_OK(linear_params(p, w->x1_s, W.pw2, M, D, D, sch));
-        Epi e;
-        e.residual = w->x_f32.as<float>(), e.out_f32 = w->x1_f32.as<float>();
-        set_epi(p, e, D);
-    }
-    {   // ffn2.w_1 + SiLU
-        GemmParams& p = lp.fc1;
-        S3B_OK(linear_params(p, w->xs_s, W.fc1, M, F, D, sch));
-        Epi e;
-        e.bias = W.fc1_b.as<float>(), e.gelu = 2, e.op = w->h_s.planes(sch);
-        set_epi(p, e, F);
-    }
-    {   // r4 = r3 + 0.5 ffn2
-        GemmParams& p = lp.fc2;
-        S3B_OK(linear_params(p, w->h_s, W.fc2, M, D, F, sch));
-        Epi e;
-        e.bias = W.fc2_b.as<float>(), e.residual = w->x1_f32.as<float>(), e.out_f32 = w->tmp_f32.as<float>();
-        set_epi(p, e, D);
+    const int B = lane.B, C = kConvDim, sch = m->scheme;
+    steps.push_back([=](Fwd& f) {
+        S3B_OK(copy_book(lane, f.st));
+        return launch_frontend(m, f.st, lane.d_wavs, lane.d_lens, B, lane.Lmax, (int)lane.L[0], m->cfg.normalize_wav,
+                               m->conv0_w.as<float>(), m->cfg.conv_bias ? m->conv0_b.as<float>() : nullptr,
+                               m->norm0_g.as<float>(), m->norm0_b.as<float>(), m->cfg.extractor_layer_norm,
+                               w->wav_pad.as<float>(), w->wav_stats.as<float>(), w->c0_part.as<double>(),
+                               w->c0_ss.as<float>(), w->act[0].planes(sch));
+    });
+    const bool ln = c.extractor_layer_norm != 0;
+    for (int i = 1; i < kNumConv; ++i) {
+        const bool last = i == kNumConv - 1;
+        const float* bias = c.conv_bias ? m->conv_b[i].as<float>() : nullptr;
+        Epi e = epi_f32(w->conv_f32.as<float>(), bias);  // "layer_norm" mode: the LayerNorm kernel adds the GELU
+        if (!ln) {
+            if (!last) e = epi_planes(w->act[i].planes(sch), bias, 1);
+            else if (c.no_feature_layer_norm) e = epi_planes(w->ln512_s.planes(sch), bias, 1);  // into post_extract_proj
+            else e.gelu = 1;
+        }
+        GemmParams p;
+        S3B_OK(conv_params(p, w->act[i - 1], m->conv_w[i], B, lane.L[i - 1], lane.L[i], kConvK[i], sch, e));
+        const size_t rows = (size_t)B * lane.L[i];
+        steps.push_back([=](Fwd& f) {
+            S3B_OK(run_gemm(f, p));
+            if (ln)
+                KNORM(m, f.st, launch_layernorm(w->conv_f32.as<float>(), rows, C, m->conv_ln_g[i].as<float>(),
+                                                m->conv_ln_b[i].as<float>(), 1, last ? w->conv_f32.as<float>() : nullptr,
+                                                last ? no_planes() : w->act[i].planes(sch), f.st));
+            return 0;
+        });
     }
     return 0;
 }
 
-int Fwd::build_plan(Plan& pl) {
+// kaldi fbank frames + CMVN (DeCoAR 2.0: every second frame) into the first GEMM's operand planes (profile category 2)
+static int add_fbank_frontend(const Lane& lane, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    Workspace* w = lane.w;
+    const int frame_step = m->kind == kFbankEncoder ? 2 : 1;
+    steps.push_back([=](Fwd& f) {
+        S3B_OK(copy_book(lane, f.st));
+        KLAUNCH(m, f.st, CAT_CONV0, 2, 0.0,
+                launch_decoar2_features(lane.d_wavs, lane.d_lens, lane.B, (int)fbank_frames(lane.Lmax), lane.T,
+                                        frame_step, w->fb_f32.as<float>(), w->ln512_s.planes(m->scheme), f.st));
+        return 0;
+    });
+    return 0;
+}
+
+// LayerNorm(512) -> post_extract_proj, padded frames zeroed (x[padding_mask] = 0, wav2vec2_model.py:3061-3062). The
+// distiller's output IS output slot 0, feat_final (zeroed like the reference's in-place x[padding_mask] = 0 on the
+// same storage, distiller/module.py:303-304).
+static int add_post_extract_proj(const Lane& lane, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    Workspace* w = lane.w;
     const s3b_config& c = m->cfg;
-    const int D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, NL = c.num_layers, C = kConvDim;
-    if (m->kind == kGruStack) {
-        // x_g = x W_ih^T + (b_ih + [b_hr, b_hz, 0]) over all B * T rows, fp32 [M][3D] (the recurrence ignores t >= m_b)
-        pl.gru_in.resize(NL);
-        for (int l = 0; l < NL; ++l) {
-            GemmParams& p = pl.gru_in[l];
-            S3B_OK(linear_params(p, l == 0 ? w->ln512_s : w->x_s, m->layers[l].wih, M, 3 * D, l == 0 ? kDecoar2K : D,
-                                 m->scheme));
-            Epi e;
-            e.bias = m->layers[l].gru_b.as<float>();
-            e.out_f32 = w->xg_f32.as<float>();
-            set_epi(p, e, 3 * D);
-        }
-        return 0;
-    }
-    if (m->kind == kLstmStack) {
-        // post_extract_proj [M][80 -> 128] x [1024][128]^T + b into layer 0's operand planes
-        const int H = kLstmHidden;
-        S3B_OK(linear_params(pl.proj, w->ln512_s, m->proj_w, M, H, kDecoar2K, m->scheme));
-        Epi e;
-        e.bias = m->proj_b.as<float>();
-        e.op = w->x_s.planes(m->scheme);
-        set_epi(pl.proj, e, H);
-        // x_g = x W_ih^T + (b_ih + b_hh), fp32 [M][4H]; layer k > 0 reads its direction's half of layer k - 1's
-        // [M][2H] output (row stride 2H)
-        pl.gru_in.resize(2 * NL);
-        for (int l = 0; l < NL; ++l)
-            for (int d = 0; d < 2; ++d) {
-                GemmParams& p = pl.gru_in[2 * l + d];
-                if (l == 0) S3B_OK(linear_params(p, w->x_s, m->layers[d].wih, M, 4 * H, H, m->scheme));
-                else
-                    S3B_OK(linear_params(p, w->h_s, m->layers[2 * l + d].wih, M, 4 * H, H, m->scheme, 2 * H,
-                                         (size_t)d * H));
-                Epi ei;
-                ei.bias = m->layers[2 * l + d].gru_b.as<float>();
-                ei.out_f32 = w->xg_f32.as<float>();
-                set_epi(p, ei, 4 * H);
-            }
-        return 0;
-    }
-    for (int i = 1; i < kNumConv && m->kind == kConvEncoder; ++i) {
-        GemmParams& p = pl.conv[i];
-        S3B_OK(conv_params(p, w->act[i - 1], m->conv_w[i], B, L[i - 1], L[i], kConvK[i], m->scheme));
-        Epi e;
-        e.bias = c.conv_bias ? m->conv_b[i].as<float>() : nullptr;
-        const bool last = (i == kNumConv - 1);
-        if (c.extractor_layer_norm) {
-            e.out_f32 = w->conv_f32.as<float>();
-        } else {
-            e.gelu = 1;
-            if (last && c.no_feature_layer_norm) e.op = w->ln512_s.planes(m->scheme);  // straight into post_extract_proj
-            else if (last) e.out_f32 = w->conv_f32.as<float>();
-            else e.op = w->act[i].planes(m->scheme);
-        }
-        set_epi(p, e, C);
-    }
-    {
-        GemmParams& p = pl.proj;
-        S3B_OK(linear_params(p, w->ln512_s, m->proj_w, M, D, m->kind == kFbankEncoder ? kDecoar2K : C, m->scheme));
-        Epi e;
-        e.bias = m->proj_b.as<float>();
-        e.row_mask = d_mask;  // x[padding_mask] = 0 (wav2vec2_model.py:3061-3062)
-        e.out_f32 = w->x_f32.as<float>();  // patched per call (proj_out)
-        if (!c.conformer) e.op = w->x_s.planes(0);  // operand of pos_conv, which stays on the bf16x3 kernel (48-channel groups)
-        set_epi(p, e, D);
-    }
-    if (c.conformer) {
-        pl.layers.resize(NL);
-        for (int l = 0; l < NL; ++l) S3B_OK(build_conformer_layer(pl.layers[l], l));
-        return 0;
-    }
+    const int C = kConvDim, sch = m->scheme;
+    const int64_t M = lane.M;
+    const bool ln = !c.no_feature_layer_norm && m->kind == kConvEncoder;
+    Epi e = epi_f32(nullptr, m->proj_b.as<float>());
+    e.row_mask = lane.d_mask;
+    if (!c.conformer) e.op = w->x_s.planes(0);  // operand of pos_conv, which stays on the bf16x3 kernel (48-channel groups)
+    GemmParams p;
+    S3B_OK(lane.linear(p, w->ln512_s, m->proj_w, c.embed_dim, m->kind == kFbankEncoder ? kDecoar2K : C, e));
+    steps.push_back([=](Fwd& f) {
+        if (ln)
+            KNORM(m, f.st, launch_layernorm(w->conv_f32.as<float>(), (size_t)M, C, m->ln512_g.as<float>(),
+                                            m->ln512_b.as<float>(), 0, nullptr, w->ln512_s.planes(sch), f.st));
+        GemmParams q = p;
+        q.out_f32 = f.proj_out();
+        S3B_OK(run_gemm(f, q));
+        return f.distil() ? f.done(0) : 0;
+    });
+    return 0;
+}
+
+// x = x + GELU(pos_conv(x)); post-LN models: encoder.layer_norm -> hidden state 0 and layer 0's operand planes
+static int add_pos_conv(const Lane& lane, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    Workspace* w = lane.w;
+    const s3b_config& c = m->cfg;
+    const int B = lane.B, T = lane.T, D = c.embed_dim, cpg = D / c.pos_conv_groups, sch = m->scheme;
+    const int64_t M = lane.M;
+    const bool ln = !c.layer_norm_first;
+    float* z = w->pos_z.as<float>();
     if (c.pos_conv_depth > 1) {
-        // block i reads the operand planes block i-1 wrote (x_s -> x1_s -> ctx_s -> x1_s ...; both are free here)
-        for (int i = 0; i < c.pos_conv_depth; ++i) {
-            const SplitBuf& in = i == 0 ? w->x_s : ((i & 1) ? w->x1_s : w->ctx_s);
-            GemmParams& p = pl.pos_d[i];
-            S3B_OK(posconv4_params(p, c, in.h(), in.l(), m->posd_w4[i].h(), m->posd_w4[i].l(), B, T));
-            Epi e;
-            e.out_f32 = w->pos_z.as<float>();
-            set_epi(p, e, 4 * D);
+        // data2vec: x_{i+1} = GELU(LayerNorm_noaffine(conv_i(x_i) + b_i)), x = x + x_depth (wav2vec2_model.py:3000-3019,
+        // 3064-3067), every block a four-taps GEMM and the combine kernel, all in one step. Block i reads the operand
+        // planes block i-1 wrote: x_s -> x1_s -> ctx_s -> x1_s ... (both are free here). Padded frames are NOT
+        // re-zeroed between the blocks (the reference does not either).
+        const int depth = c.pos_conv_depth;
+        std::vector<const SplitBuf*> x(depth);
+        std::vector<GemmParams> conv(depth);
+        for (int i = 0; i < depth; ++i) {
+            x[i] = i == 0 ? &w->x_s : (i & 1) ? &w->x1_s : &w->ctx_s;
+            S3B_OK(posconv4_params(conv[i], c, x[i]->h(), x[i]->l(), m->posd_w4[i].h(), m->posd_w4[i].l(), B, T,
+                                   epi_f32(z)));
         }
+        steps.push_back([=](Fwd& f) {
+            for (int i = 0; i < depth; ++i) {
+                const bool last = (i == depth - 1);
+                S3B_OK(run_gemm(f, conv[i]));
+                KNORM(m, f.st, launch_posconv_combine(z, last ? f.proj_out() : nullptr, m->posd_b[i].as<float>(), B, T,
+                                                      D, cpg, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(),
+                                                      last && ln ? 1 : 0, last ? 2 : 1, last ? f.hs(0) : nullptr,
+                                                      last ? (ln ? w->xs_s.planes(sch) : no_planes()) : x[i + 1]->planes(0),
+                                                      f.st));
+            }
+            return f.distil() ? 0 : f.done(0);
+        });
+    } else if (posconv4_ok(c)) {
+        // four taps per k-block into pos_z, then the combine kernel (+ LayerNorm)
+        GemmParams p;
+        S3B_OK(posconv4_params(p, c, w->x_s.h(), w->x_s.l(), m->pos_w4.h(), m->pos_w4.l(), B, T, epi_f32(z)));
+        steps.push_back([=](Fwd& f) {
+            S3B_OK(run_gemm(f, p));
+            KNORM(m, f.st, launch_posconv_combine(z, f.proj_out(), m->pos_b.as<float>(), B, T, D, cpg,
+                                                  m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(), ln ? 1 : 0, 0,
+                                                  f.hs(0), ln ? w->xs_s.planes(sch) : no_planes(), f.st));
+            return f.distil() ? 0 : f.done(0);
+        });
     } else {
-        GemmParams& p = pl.pos;
-        if (posconv4_ok(c)) {
-            S3B_OK(posconv4_params(p, c, w->x_s.h(), w->x_s.l(), m->pos_w4.h(), m->pos_w4.l(), B, T));
-            Epi e;
-            e.out_f32 = w->pos_z.as<float>();
-            set_epi(p, e, 4 * D);
-        } else {
-            S3B_OK(posconv_params(p, c, w->x_s.h(), w->x_s.l(), m->pos_w.h(), m->pos_w.l(), B, T));
-            Epi e;
-            e.bias = m->pos_b.as<float>();
-            e.gelu = 1;
-            e.residual = w->x_f32.as<float>();
-            e.out_f32 = w->tmp_f32.as<float>();  // pre-LN: patched to hidden state 0 per call
-            set_epi(p, e, D);
-        }
-    }
-    pl.layers.resize(NL);
-    for (int l = 0; l < NL; ++l) {
-        LayerW& W = m->layers[l];
-        LayerPlan& lp = pl.layers[l];
-        {   // QKV projection, scattered per head
-            GemmParams& p = lp.qkv;
-            S3B_OK(linear_params(p, w->xs_s, W.qkv, M, 3 * D, D, m->scheme));
-            set_qkv_epi(p, W.qkv_b.as<float>(), T, H, head_dim(c), w->q_s, w->k_s, w->vt_s);
-        }
-        S3B_OK(attn_params(lp.attn, w, B, T, H, head_dim(c), d_kv, m->scheme));
-        if (c.relative_position) set_rel_bias(lp.attn, m->rel_table.as<float>(), m->rel_table_T, w->gate.as<float>());
-        {   // out_proj + residual (residual = hidden state l, patched per call)
-            GemmParams& p = lp.out;
-            S3B_OK(linear_params(p, w->ctx_s, W.out, M, D, D, m->scheme));
-            Epi e;
-            e.bias = W.out_b.as<float>();
-            e.out_f32 = c.layer_norm_first ? w->x1_f32.as<float>() : w->tmp_f32.as<float>();
-            set_epi(p, e, D);
-        }
-        {   // fc1 + GELU
-            GemmParams& p = lp.fc1;
-            S3B_OK(linear_params(p, w->x1_s, W.fc1, M, F, D, m->scheme));
-            Epi e;
-            e.bias = W.fc1_b.as<float>();
-            e.gelu = 1;
-            e.op = w->h_s.planes(m->scheme);
-            set_epi(p, e, F);
-        }
-        {   // fc2 + residual (output patched per call for pre-LN models)
-            GemmParams& p = lp.fc2;
-            S3B_OK(linear_params(p, w->h_s, W.fc2, M, D, F, m->scheme));
-            Epi e;
-            e.bias = W.fc2_b.as<float>();
-            e.residual = w->x1_f32.as<float>();
-            e.out_f32 = w->tmp_f32.as<float>();
-            set_epi(p, e, D);
-        }
-    }
-    if (c.pred_heads > 0) {
-        // Distiller output layer on the encoder output (operand planes xs_s): Linear(D, N*D) + GELU -> h_s, then one
-        // [D][D] GEMM per task on its D-column slice of h_s (SplitLinear, distiller/module.py:77-90)
-        const int N = c.pred_heads;
-        {
-            GemmParams& p = pl.pred1;
-            S3B_OK(linear_params(p, w->xs_s, m->pred1_w, M, N * D, D, m->scheme));
-            Epi e;
-            e.bias = m->pred1_b.as<float>();
-            e.gelu = 1;
-            e.op = w->h_s.planes(m->scheme);
-            set_epi(p, e, N * D);
-        }
-        pl.pred2.resize(N);
-        for (int k = 0; k < N; ++k) {
-            GemmParams& p = pl.pred2[k];
-            S3B_OK(linear_params(p, w->h_s, m->pred2_w[k], M, D, D, m->scheme, (int64_t)N * D, (size_t)k * D));
-            Epi e;
-            e.bias = m->pred2_b.as<float>() + (size_t)k * D;
-            e.out_f32 = w->tmp_f32.as<float>();  // patched per call: output slot NL + 1 + k
-            set_epi(p, e, D);
-        }
+        // one tap per k-block: x + GELU(conv + bias) in the epilogue (pre-LN: straight into hidden state 0), then the
+        // LayerNorm
+        Epi e = epi_f32(w->tmp_f32.as<float>(), m->pos_b.as<float>());
+        e.gelu = 1;
+        GemmParams p;
+        S3B_OK(posconv_params(p, c, w->x_s.h(), w->x_s.l(), m->pos_w.h(), m->pos_w.l(), B, T, e));
+        steps.push_back([=](Fwd& f) {
+            GemmParams q = p;
+            q.residual = f.proj_out();
+            if (!ln) q.out_f32 = f.hs(0);
+            S3B_OK(run_gemm(f, q));
+            if (ln)
+                KNORM(m, f.st, launch_layernorm(w->tmp_f32.as<float>(), (size_t)M, D, m->enc_ln_g.as<float>(),
+                                                m->enc_ln_b.as<float>(), 0, f.hs(0), w->xs_s.planes(sch), f.st));
+            return f.distil() ? 0 : f.done(0);
+        });
     }
     return 0;
 }
 
-// APC: stage 0 (Fwd::stage) = fbank + CMVN into layer 0's operand planes; stage 1 + 2l = layer l's input GEMM;
-// stage 2 + 2l = its recurrence, which writes hidden state l (+ layer l's input when residual, l > 0) and layer l + 1's
-// operand planes
-int Fwd::apc_stage(int s) {
-    s3b_model* m = this->m;  // the launch macros expect `m` and `st`
-    cudaStream_t st = this->st;
+// TransformerSentenceEncoderLayer.forward (wav2vec2_model.py:3260-3322; WavLM.py:709-774) in five steps
+static int add_transformer_layer(const Lane& lane, int l, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    Workspace* w = lane.w;
+    const s3b_config& c = m->cfg;
+    const int B = lane.B, T = lane.T, D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, hd = head_dim(c);
+    const int sch = m->scheme;
+    const size_t M = (size_t)lane.M;
+    const LayerW* W = &m->layers[l];
+    const bool pre = c.layer_norm_first != 0, rel = c.relative_position != 0, gru_rel = c.gru_rel_pos != 0;
+    const bool last = l == c.num_layers - 1, heads = c.pred_heads > 0;
+    const double attn_flops = 4.0 * (double)T * T * D * B;
+    float* x1 = w->x1_f32.as<float>();
+    float* tmp = w->tmp_f32.as<float>();
+    GemmParams qkv, out, fc1, fc2;
+    AttnParams attn;
+    S3B_OK(lane.linear(qkv, w->xs_s, W->qkv, 3 * D, D, Epi()));
+    set_qkv_epi(qkv, W->qkv_b.as<float>(), T, H, hd, w->q_s, w->k_s, w->vt_s);
+    S3B_OK(attn_params(attn, w, B, T, H, hd, lane.d_kv, sch));
+    if (rel) set_rel_bias(attn, m->rel_table.as<float>(), m->rel_table_T, w->gate.as<float>());
+    S3B_OK(lane.linear(out, w->ctx_s, W->out, D, D, epi_f32(pre ? x1 : tmp, W->out_b.as<float>())));
+    S3B_OK(lane.linear(fc1, w->x1_s, W->fc1, F, D, epi_planes(w->h_s.planes(sch), W->fc1_b.as<float>(), 1)));
+    S3B_OK(lane.linear(fc2, w->h_s, W->fc2, D, F, epi_f32(tmp, W->fc2_b.as<float>(), x1)));
+    // pre-LN: xs = LN1(hidden state l); QKV projection, scattered per head; WavLM: the gate from the layer's attention
+    // input (post-LN: hidden state l; pre-LN: the LN1 output), modules.py:534-551
+    steps.push_back([=](Fwd& f) {
+        if (pre)
+            KNORM(m, f.st, launch_layernorm(f.hs(l), M, D, W->ln1_g.as<float>(), W->ln1_b.as<float>(), 0, nullptr,
+                                            w->xs_s.planes(sch), f.st));
+        S3B_OK(run_gemm(f, qkv));
+        if (rel)
+            KMISC(m, f.st, launch_wavlm_gate(w->xs_s.planes(sch), M, B, T, H, D, gru_rel ? W->grep_w.as<float>() : nullptr,
+                                             W->grep_b.as<float>(), W->grep_a.as<float>(), w->gate.as<float>(), f.st));
+        return 0;
+    });
+    steps.push_back([=](Fwd& f) {
+        KLAUNCH(m, f.st, CAT_ATTN, 1, attn_flops, launch_attention(attn, f.st));
+        return 0;
+    });
+    // r1 = hidden state l + out_proj(ctx); pre-LN: x1_s = LN2(r1); post-LN: x1 = LN1(r1)
+    steps.push_back([=](Fwd& f) {
+        GemmParams p = out;
+        p.residual = f.hs(l);
+        S3B_OK(run_gemm(f, p));
+        if (pre)
+            KNORM(m, f.st, launch_layernorm(x1, M, D, W->ln2_g.as<float>(), W->ln2_b.as<float>(), 0, nullptr,
+                                            w->x1_s.planes(sch), f.st));
+        else
+            KNORM(m, f.st, launch_layernorm(tmp, M, D, W->ln1_g.as<float>(), W->ln1_b.as<float>(), 0, x1,
+                                            w->x1_s.planes(sch), f.st));
+        return 0;
+    });
+    steps.push_back([=](Fwd& f) { return run_gemm(f, fc1); });
+    // fc2 + residual; the next layer's (or the prediction heads') operand planes
+    steps.push_back([=](Fwd& f) {
+        GemmParams p = fc2;
+        // pre-LN: the sum IS hidden state l+1 (un-normalised residual stream), except after the last layer
+        float* unnorm = (last && f.last_res != nullptr) ? f.last_res : tmp;
+        if (pre) p.out_f32 = last ? unnorm : f.hs(l + 1);
+        if (f.ffn_out != nullptr) p.out_pre = f.ffn_out + (size_t)l * f.ffn_stride;
+        S3B_OK(run_gemm(f, p));
+        if (pre) {
+            if (last)  // encoder.layer_norm on the final output (wav2vec2_model.py:3049-3050)
+                KNORM(m, f.st, launch_layernorm(unnorm, M, D, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(), 0,
+                                                f.hs(l + 1), heads ? w->xs_s.planes(sch) : no_planes(), f.st));
+        } else {
+            KNORM(m, f.st, launch_layernorm(tmp, M, D, W->ln2_g.as<float>(), W->ln2_b.as<float>(), 0, f.hs(l + 1),
+                                            !last || heads ? w->xs_s.planes(sch) : no_planes(), f.st));
+        }
+        return f.done(l + 1);
+    });
+    return 0;
+}
+
+// Distiller output layer on the encoder output (operand planes xs_s): Linear(D, N*D) + GELU -> h_s, then one [D][D]
+// GEMM per task on its D-column slice of h_s into output slot NL + 1 + k (SplitLinear, distiller/module.py:77-90)
+static int add_pred_heads(const Lane& lane, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    Workspace* w = lane.w;
+    const int D = m->cfg.embed_dim, N = m->cfg.pred_heads, NL = m->cfg.num_layers;
+    GemmParams p1;
+    S3B_OK(lane.linear(p1, w->xs_s, m->pred1_w, N * D, D, epi_planes(w->h_s.planes(m->scheme), m->pred1_b.as<float>(), 1)));
+    steps.push_back([=](Fwd& f) { return run_gemm(f, p1); });
+    for (int k = 0; k < N; ++k) {
+        GemmParams p;
+        S3B_OK(lane.linear(p, w->h_s, m->pred2_w[k], D, D, epi_f32(nullptr, m->pred2_b.as<float>() + (size_t)k * D),
+                           (int64_t)N * D, (size_t)k * D));
+        steps.push_back([=](Fwd& f) {
+            GemmParams q = p;
+            q.out_f32 = f.slot(NL + 1 + k);
+            S3B_OK(run_gemm(f, q));
+            return f.done(NL + 1 + k);
+        });
+    }
+    return 0;
+}
+
+// ConformerEncoder before its layers: no pos_conv; post-LN models: encoder.layer_norm -> hidden state 0
+// (wav2vec2_model.py:3183-3184)
+static int add_conformer_input(const Lane& lane, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    float* x = lane.w->x_f32.as<float>();
+    const bool ln = !m->cfg.layer_norm_first;
+    const size_t M = (size_t)lane.M;
+    const int D = m->cfg.embed_dim;
+    steps.push_back([=](Fwd& f) {
+        if (ln)
+            KNORM(m, f.st, launch_layernorm(x, M, D, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(), 0, f.hs(0),
+                                            no_planes(), f.st));
+        return f.done(0);
+    });
+    return 0;
+}
+
+// One Conformer layer (wav2vec2_model.py:537-578) in ten steps, nine GEMMs. Residual stream: hidden state l -> r1
+// (x1_f32, after ffn1) -> r2 (x_f32, after attention) -> r3 (x1_f32, after the conv module) -> r4 (tmp_f32, after
+// ffn2) -> final_layer_norm -> hidden state l+1. Operand planes: xs_s = LayerNorm outputs, x1_s = rope(LN) / depthwise
+// output.
+static int add_conformer_layer(const Lane& lane, int l, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    Workspace* w = lane.w;
+    const s3b_config& c = m->cfg;
+    const int B = lane.B, T = lane.T, D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, kw = c.depthwise_kernel;
+    const int sch = m->scheme;
+    const size_t M = (size_t)lane.M;
+    const LayerW* W = &m->layers[l];
+    const double attn_flops = 4.0 * (double)T * T * D * B;
+    const OutPlanes xs = w->xs_s.planes(sch), x1s = w->x1_s.planes(sch), hs = w->h_s.planes(sch);
+    float* r13 = w->x1_f32.as<float>();
+    float* r2 = w->x_f32.as<float>();
+    float* r4 = w->tmp_f32.as<float>();
+    GemmParams ffn1_a, ffn1_b, qk, v, out, pw1, pw2, fc1, fc2;
+    AttnParams attn;
+    S3B_OK(lane.linear(ffn1_a, w->xs_s, W->ffn1_w1, F, D, epi_planes(hs, W->ffn1_b1.as<float>(), 2)));
+    S3B_OK(lane.linear(ffn1_b, w->h_s, W->ffn1_w2, D, F, epi_f32(r13, W->ffn1_b2.as<float>())));
+    S3B_OK(lane.linear(qk, w->x1_s, W->qkv, 2 * D, D, Epi()));
+    set_qkv_epi(qk, W->qkv_b.as<float>(), T, H, 64, w->q_s, w->k_s, w->vt_s, 0);
+    S3B_OK(lane.linear(v, w->xs_s, W->v, D, D, Epi()));
+    set_qkv_epi(v, W->qkv_b.as<float>() + 2 * D, T, H, 64, w->q_s, w->k_s, w->vt_s, 2 * D);
+    S3B_OK(attn_params(attn, w, B, T, H, 64, lane.d_kv, sch));
+    S3B_OK(lane.linear(out, w->ctx_s, W->out, D, D, epi_f32(r2, W->out_b.as<float>(), r13)));
+    S3B_OK(lane.linear(pw1, w->xs_s, W->pw1, 2 * D, D, epi_f32(w->glu_f32.as<float>())));
+    S3B_OK(lane.linear(pw2, w->x1_s, W->pw2, D, D, epi_f32(r13, nullptr, r2)));
+    S3B_OK(lane.linear(fc1, w->xs_s, W->fc1, F, D, epi_planes(hs, W->fc1_b.as<float>(), 2)));
+    S3B_OK(lane.linear(fc2, w->h_s, W->fc2, D, F, epi_f32(r4, W->fc2_b.as<float>(), r13)));
+    // ffn1: LayerNorm -> w_1 + SiLU
+    steps.push_back([=](Fwd& f) {
+        KNORM(m, f.st, launch_layernorm(f.hs(l), M, D, W->ffn1_ln_g.as<float>(), W->ffn1_ln_b.as<float>(), 0, nullptr,
+                                        xs, f.st));
+        return run_gemm(f, ffn1_a);
+    });
+    // r1 = x + 0.5 w_2(...) (0.5 folded into w_2)
+    steps.push_back([=](Fwd& f) {
+        GemmParams p = ffn1_b;
+        p.residual = f.hs(l);
+        return run_gemm(f, p);
+    });
+    // self_attn_layer_norm + RoPE -> [q | k] from rope(LN(r1)), v from LN(r1)
+    steps.push_back([=](Fwd& f) {
+        KNORM(m, f.st, launch_layernorm_rope(r13, M, T, D, W->ln1_g.as<float>(), W->ln1_b.as<float>(),
+                                             m->rope_cs.as<float>(), xs, x1s, f.st));
+        S3B_OK(run_gemm(f, qk));
+        return run_gemm(f, v);
+    });
+    steps.push_back([=](Fwd& f) {
+        KLAUNCH(m, f.st, CAT_ATTN, 1, attn_flops, launch_attention(attn, f.st));
+        return 0;
+    });
+    // r2 = r1 + linear_out
+    steps.push_back([=](Fwd& f) { return run_gemm(f, out); });
+    // conv_module: LayerNorm -> pointwise_conv1 (no bias) -> fp32 [M][2D]
+    steps.push_back([=](Fwd& f) {
+        KNORM(m, f.st, launch_layernorm(r2, M, D, W->conv_ln_g.as<float>(), W->conv_ln_b.as<float>(), 0, nullptr, xs,
+                                        f.st));
+        return run_gemm(f, pw1);
+    });
+    // GLU -> depthwise conv -> BatchNorm -> SiLU
+    steps.push_back([=](Fwd& f) {
+        KMISC(m, f.st, launch_depthwise_glu(w->glu_f32.as<float>(), B, T, D, kw, W->dw_w.as<float>(),
+                                            W->dw_b.as<float>(), x1s, f.st));
+        return 0;
+    });
+    // r3 = r2 + pointwise_conv2 (no bias)
+    steps.push_back([=](Fwd& f) { return run_gemm(f, pw2); });
+    // ffn2: LayerNorm -> w_1 + SiLU
+    steps.push_back([=](Fwd& f) {
+        KNORM(m, f.st, launch_layernorm(r13, M, D, W->ffn2_ln_g.as<float>(), W->ffn2_ln_b.as<float>(), 0, nullptr, xs,
+                                        f.st));
+        return run_gemm(f, fc1);
+    });
+    // r4 = r3 + 0.5 w_2(...) -> final_layer_norm -> hidden state l+1 (pre-LN: encoder.layer_norm after the last layer,
+    // wav2vec2_model.py:3049-3050)
+    const bool enc_ln = c.layer_norm_first && l == c.num_layers - 1;
+    steps.push_back([=](Fwd& f) {
+        S3B_OK(run_gemm(f, fc2));
+        KNORM(m, f.st, launch_layernorm(r4, M, D, W->ln2_g.as<float>(), W->ln2_b.as<float>(), 0,
+                                        enc_ln ? r4 : f.hs(l + 1), no_planes(), f.st));
+        if (enc_ln)
+            KNORM(m, f.st, launch_layernorm(r4, M, D, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(), 0, f.hs(l + 1),
+                                            no_planes(), f.st));
+        return f.done(l + 1);
+    });
+    return 0;
+}
+
+// APC: per GRU layer l, the input GEMM x_g = x W_ih^T + (b_ih + [b_hr, b_hz, 0]) over all B * T rows, fp32 [M][3D]
+// (the recurrence ignores t >= m_b), then the recurrence, which writes hidden state l (+ layer l's input when
+// residual, l > 0) and layer l + 1's operand planes
+static int add_gru_stack(const Lane& lane, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    Workspace* w = lane.w;
     const int D = m->cfg.embed_dim, NL = m->cfg.num_layers;
-    const int l = (s - 1) / 2;
-    if (l >= NL) return fail("internal: stage %d out of range", s);
-    if ((s - 1) % 2 == 0) {
-        GemmParams p = plan->gru_in[l];
-        KGEMM(launch_gemm(p, m->sm_count, st));
-        return 0;
-    }
-    const LayerW& W = m->layers[l];
-    GruParams g;
-    g.xg = w->xg_f32.as<float>(), g.whh = W.whh.as<float>(), g.bhn = W.bhn.as<float>();
-    g.res = (m->apc_residual && l > 0) ? slot(l - 1) : nullptr;
-    g.len = d_kv, g.order = d_ord, g.B = B, g.T = T;
-    g.out = slot(l);
-    g.op = l + 1 < NL ? w->x_s.planes(m->scheme) : no_planes();
-    KLAUNCH(CAT_GRU, 1, 2.0 * 3 * D * D * (double)M, launch_gru(g, st));
-    if (layer_done) S3B_OK(layer_done(m, l, st, user));
-    return 0;
-}
-
-// DeCoAR: stage 0 (Fwd::stage) = fbank + CMVN; stage 1 = post_extract_proj; stage 2 + 4l + 2d = the input GEMM of
-// layer l, direction d (0 forward, 1 backward); stage 3 + 4l + 2d = its recurrence, which writes columns [d H, d H + H)
-// of layer l's [B][T][2H] output: an output slot (decoar_layers: every layer; decoar: the last) and, below the last
-// layer, the operand planes of layer l + 1's GEMMs. The two directions never run concurrently: each recurrence
-// occupies the whole device.
-int Fwd::decoar_stage(int s) {
-    s3b_model* m = this->m;  // the launch macros expect `m` and `st`
-    cudaStream_t st = this->st;
-    const int NL = m->cfg.num_layers, H = kLstmHidden;
-    if (s == 1) {
-        GemmParams p = plan->proj;
-        KGEMM(launch_gemm(p, m->sm_count, st));
-        return 0;
-    }
-    const int l = (s - 2) / 4, d = ((s - 2) / 2) % 2;
-    if (l >= NL) return fail("internal: stage %d out of range", s);
-    if ((s - 2) % 2 == 0) {
-        GemmParams p = plan->gru_in[2 * l + d];
-        KGEMM(launch_gemm(p, m->sm_count, st));
-        return 0;
-    }
-    const bool last = l == NL - 1;
-    LstmParams g;
-    g.xg = w->xg_f32.as<float>(), g.whh = m->layers[2 * l + d].whh.as<float>(), g.bhh = nullptr;
-    g.len = d_kv, g.order = d_ord, g.B = B, g.T = T, g.direction = d;
-    g.out = m->decoar_all_layers ? slot(l) : last ? slot(0) : nullptr;
-    g.ldo = 2 * H, g.col0 = d * H;
-    g.op = last ? no_planes() : w->h_s.planes(m->scheme);
-    g.hbuf = w->lstm_h.as<float>(), g.counter = w->lstm_sync.as<unsigned int>();
-    KLAUNCH(CAT_GRU, (B + kLstmMaxBatch - 1) / kLstmMaxBatch, 8.0 * H * H * (double)M, launch_lstm(g, st));
-    if (d == 1 && layer_done != nullptr) {
-        if (m->decoar_all_layers) S3B_OK(layer_done(m, l, st, user));
-        else if (last) S3B_OK(layer_done(m, 0, st, user));
+    const int64_t M = lane.M;
+    for (int l = 0; l < NL; ++l) {
+        const LayerW& W = m->layers[l];
+        GemmParams in;
+        S3B_OK(lane.linear(in, l == 0 ? w->ln512_s : w->x_s, W.wih, 3 * D, l == 0 ? kDecoar2K : D,
+                           epi_f32(w->xg_f32.as<float>(), W.gru_b.as<float>())));
+        steps.push_back([=](Fwd& f) { return run_gemm(f, in); });
+        GruParams g;
+        g.xg = w->xg_f32.as<float>(), g.whh = W.whh.as<float>(), g.bhn = W.bhn.as<float>();
+        g.len = lane.d_kv, g.order = lane.d_ord, g.B = lane.B, g.T = lane.T;
+        g.op = l + 1 < NL ? w->x_s.planes(m->scheme) : no_planes();
+        const bool residual = m->apc_residual && l > 0;
+        steps.push_back([=](Fwd& f) {
+            GruParams q = g;
+            q.res = residual ? f.slot(l - 1) : nullptr;
+            q.out = f.slot(l);
+            KLAUNCH(m, f.st, CAT_GRU, 1, 2.0 * 3 * D * D * (double)M, launch_gru(q, f.st));
+            return f.done(l);
+        });
     }
     return 0;
 }
 
-int Fwd::stage(int s) {
-    s3b_model* m = this->m;  // the launch macros expect `m` and `st`
-    cudaStream_t st = this->st;
+// DeCoAR: post_extract_proj [M][80 -> 128] x [1024][128]^T + b into layer 0's operand planes; then per layer l and
+// direction d (0 forward, 1 backward) the input GEMM x_g = x W_ih^T + (b_ih + b_hh), fp32 [M][4H], and the recurrence,
+// which writes columns [d H, d H + H) of layer l's [B][T][2H] output: an output slot (decoar_layers: every layer;
+// decoar: the last) and, below the last layer, the operand planes of layer l + 1's GEMMs, which read their direction's
+// half (row stride 2H). The two directions never run concurrently: each recurrence occupies the whole device.
+static int add_lstm_stack(const Lane& lane, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    Workspace* w = lane.w;
+    const int NL = m->cfg.num_layers, H = kLstmHidden, B = lane.B, sch = m->scheme;
+    const int64_t M = lane.M;
+    const bool all_layers = m->decoar_all_layers != 0;
+    GemmParams proj;
+    S3B_OK(lane.linear(proj, w->ln512_s, m->proj_w, H, kDecoar2K, epi_planes(w->x_s.planes(sch), m->proj_b.as<float>())));
+    steps.push_back([=](Fwd& f) { return run_gemm(f, proj); });
+    for (int l = 0; l < NL; ++l) {
+        const bool last = l == NL - 1;
+        for (int d = 0; d < 2; ++d) {
+            const LayerW& W = m->layers[2 * l + d];
+            GemmParams in;
+            S3B_OK(lane.linear(in, l == 0 ? w->x_s : w->h_s, W.wih, 4 * H, H,
+                               epi_f32(w->xg_f32.as<float>(), W.gru_b.as<float>()), l == 0 ? 0 : 2 * H,
+                               l == 0 ? 0 : (size_t)d * H));
+            steps.push_back([=](Fwd& f) { return run_gemm(f, in); });
+            LstmParams g;
+            g.xg = w->xg_f32.as<float>(), g.whh = W.whh.as<float>(), g.bhh = nullptr;
+            g.len = lane.d_kv, g.order = lane.d_ord, g.B = B, g.T = lane.T, g.direction = d;
+            g.out = nullptr, g.ldo = 2 * H, g.col0 = d * H;
+            g.op = last ? no_planes() : w->h_s.planes(sch);
+            g.hbuf = w->lstm_h.as<float>(), g.counter = w->lstm_sync.as<unsigned int>();
+            steps.push_back([=](Fwd& f) {
+                LstmParams q = g;
+                q.out = all_layers ? f.slot(l) : last ? f.slot(0) : nullptr;
+                KLAUNCH(m, f.st, CAT_GRU, (B + kLstmMaxBatch - 1) / kLstmMaxBatch, 8.0 * H * H * (double)M,
+                        launch_lstm(q, f.st));
+                if (d == 0) return 0;
+                return all_layers ? f.done(l) : last ? f.done(0) : 0;
+            });
+        }
+    }
+    return 0;
+}
+
+// One lane's forward at the lane's shape, in enqueue order
+static int build_steps(const Lane& lane, std::vector<Step>& steps) {
+    const s3b_model* m = lane.m;
     const s3b_config& c = m->cfg;
-    if (s == 0) {
-        // ---- bookkeeping copy, then the front end -----------------------------------------------------------------
-        const size_t book_bytes = (size_t)(reinterpret_cast<char*>(d_mask) - w->book.as<char>()) + (size_t)M;
-        CUDA_OK(cudaMemcpyAsync(w->book.p, w->book_host.get(), book_bytes, cudaMemcpyHostToDevice, st));
-        CUDA_OK(cudaEventRecord(w->book_copied.get(), st));
-        if (m->kind != kConvEncoder) {
-            // fbank frames + CMVN (DeCoAR 2.0: y[::2]) -> the first GEMM's operand planes (profile category 2)
-            const int step = m->kind == kFbankEncoder ? 2 : 1;
-            KLAUNCH(CAT_CONV0, 2, 0.0, launch_decoar2_features(d_wavs, d_lens, B, (int)fbank_frames(Lmax), T, step,
-                                                               w->fb_f32.as<float>(), w->ln512_s.planes(m->scheme), st));
-            return 0;
-        }
-        // waveform packing (+ normalisation), conv 0 + norm + GELU -> act[0]
-        return launch_frontend(m, st, d_wavs, d_lens, B, Lmax, (int)L[0], c.normalize_wav, m->conv0_w.as<float>(),
-                               c.conv_bias ? m->conv0_b.as<float>() : nullptr, m->norm0_g.as<float>(),
-                               m->norm0_b.as<float>(), c.extractor_layer_norm, w->wav_pad.as<float>(),
-                               w->wav_stats.as<float>(), w->c0_part.as<double>(), w->c0_ss.as<float>(),
-                               w->act[0].planes(m->scheme));
+    switch (m->kind) {
+    case kGruStack:
+        S3B_OK(add_fbank_frontend(lane, steps));
+        return add_gru_stack(lane, steps);
+    case kLstmStack:
+        S3B_OK(add_fbank_frontend(lane, steps));
+        return add_lstm_stack(lane, steps);
+    case kFbankEncoder:
+        S3B_OK(add_fbank_frontend(lane, steps));
+        // six empty steps where the conv stack would be: with two lanes they keep lane 1's steps enqueued next to the
+        // same lane-0 steps as in the conv encoder
+        for (int i = 1; i < kNumConv; ++i) steps.push_back([](Fwd&) { return 0; });
+        break;
+    case kConvEncoder: S3B_OK(add_conv_frontend(lane, steps)); break;
     }
-    if (m->kind == kGruStack) return apc_stage(s);
-    if (m->kind == kLstmStack) return decoar_stage(s);
-    const int D = c.embed_dim, H = c.num_heads, NL = c.num_layers, C = kConvDim;
-    const double attn_flops = 4.0 * (double)T * T * D * B;
-
-    if (s >= 1 && s <= 6) {
-        // ---- conv s as implicit GEMM (+ per-frame LayerNorm + GELU in "layer_norm" mode) ----------------------------
-        if (m->kind == kFbankEncoder) return 0;  // no conv stack
-        const int i = s;
-        GemmParams p = plan->conv[i];
-        KGEMM(launch_gemm(p, m->sm_count, st));
-        if (c.extractor_layer_norm) {
-            const bool last = (i == kNumConv - 1);
-            KNORM(launch_layernorm(w->conv_f32.as<float>(), (size_t)B * L[i], C, m->conv_ln_g[i].as<float>(),
-                                   m->conv_ln_b[i].as<float>(), 1, last ? w->conv_f32.as<float>() : nullptr,
-                                   last ? no_planes() : w->act[i].planes(m->scheme), st));
-        }
-        return 0;
-    }
-    if (s == 7) {
-        // ---- LayerNorm(512) -> post_extract_proj (+ zero padded frames) --------------------------------------------
-        if (!c.no_feature_layer_norm && m->kind == kConvEncoder)
-            KNORM(launch_layernorm(w->conv_f32.as<float>(), (size_t)M, C, m->ln512_g.as<float>(), m->ln512_b.as<float>(),
-                                   0, nullptr, w->ln512_s.planes(m->scheme), st));
-        GemmParams p = plan->proj;
-        p.out_f32 = proj_out();  // distiller: feat_final IS output slot 0 (padded frames zeroed, like the reference's
-                                 // in-place x[padding_mask] = 0 on the same storage, distiller/module.py:303-304)
-        KGEMM(launch_gemm(p, m->sm_count, st));
-        if (distil() && layer_done) S3B_OK(layer_done(m, 0, st, user));
-        return 0;
-    }
-    if (s == 8 && c.conformer) {
-        // ---- Conformer: no pos_conv; post-LN models: encoder.layer_norm -> hidden state 0 (wav2vec2_model.py:3183-3184)
-        if (!c.layer_norm_first)
-            KNORM(launch_layernorm(w->x_f32.as<float>(), (size_t)M, D, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(), 0,
-                                   hs(0), no_planes(), st));
-        if (layer_done) S3B_OK(layer_done(m, 0, st, user));
-        return 0;
-    }
+    S3B_OK(add_post_extract_proj(lane, steps));
     if (c.conformer) {
-        const int l = (s - 9) / kConformerStages;
-        if (l >= NL) return fail("internal: stage %d out of range", s);
-        return conformer_stage(l, (s - 9) % kConformerStages);
-    }
-    if (s == 8) {
-        // ---- x = x + GELU(pos_conv(x)) ; post-LN models: LayerNorm -> hidden state 0 -------------------------------
-        GemmParams p = plan->pos;
-        float* hs0 = hs(0);
-        if (c.pos_conv_depth > 1) {
-            // data2vec: x_{i+1} = GELU(LayerNorm_noaffine(conv_i(x_i) + b_i)), x = x + x_depth (wav2vec2_model.py:3000-3019,
-            // 3064-3067). Padded frames are NOT re-zeroed between the blocks (the reference does not either).
-            const bool ln = !c.layer_norm_first;
-            for (int i = 0; i < c.pos_conv_depth; ++i) {
-                const bool last = (i == c.pos_conv_depth - 1);
-                KGEMM(launch_gemm(plan->pos_d[i], m->sm_count, st));
-                const SplitBuf& nxt = (i & 1) ? w->ctx_s : w->x1_s;  // == the `in` of block i+1 in build_plan
-                KNORM(launch_posconv_combine(w->pos_z.as<float>(), last ? proj_out() : nullptr, m->posd_b[i].as<float>(), B,
-                                             T, D, D / c.pos_conv_groups, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(),
-                                             last && ln ? 1 : 0, last ? 2 : 1, last ? hs0 : nullptr,
-                                             last ? (ln ? w->xs_s.planes(m->scheme) : no_planes()) : nxt.planes(0), st));
-            }
-        } else if (posconv4_ok(c)) {
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            const bool ln = !c.layer_norm_first;
-            KNORM(launch_posconv_combine(w->pos_z.as<float>(), proj_out(), m->pos_b.as<float>(), B, T, D,
-                                         D / c.pos_conv_groups, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(),
-                                         ln ? 1 : 0, 0, hs0, ln ? w->xs_s.planes(m->scheme) : no_planes(), st));
-        } else {
-            p.residual = proj_out();
-            if (c.layer_norm_first) p.out_f32 = hs0;
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            if (!c.layer_norm_first)
-                KNORM(launch_layernorm(w->tmp_f32.as<float>(), (size_t)M, D, m->enc_ln_g.as<float>(),
-                                       m->enc_ln_b.as<float>(), 0, hs0, w->xs_s.planes(m->scheme), st));
-        }
-        if (!distil() && layer_done) S3B_OK(layer_done(m, 0, st, user));
+        S3B_OK(add_conformer_input(lane, steps));
+        for (int l = 0; l < c.num_layers; ++l) S3B_OK(add_conformer_layer(lane, l, steps));
         return 0;
     }
-
-    // ---- Distiller prediction heads (after the layers) -------------------------------------------------------------
-    if (s >= 9 + 5 * NL) {
-        const int k = s - (9 + 5 * NL);  // 0: Linear + GELU, 1..N: SplitLinear task k-1
-        if (k == 0) {
-            GemmParams p = plan->pred1;
-            KGEMM(launch_gemm(p, m->sm_count, st));
-        } else {
-            GemmParams p = plan->pred2[k - 1];
-            p.out_f32 = slot(NL + k);
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            if (layer_done) S3B_OK(layer_done(m, NL + k, st, user));
-        }
-        return 0;
-    }
-
-    // ---- transformer layer l, five stages ---------------------------------------------------------------------
-    const int l = (s - 9) / 5, sub = (s - 9) % 5;
-    if (l >= NL) return fail("internal: stage %d out of range", s);
-    LayerW& W = m->layers[l];
-    LayerPlan& lp = plan->layers[l];
-    float* hs_in = hs(l);       // layer input = hidden state l
-    float* hs_out = hs(l + 1);  // hidden state l+1
-    const bool last = (l == NL - 1);
-    const bool rel = c.relative_position != 0;
-    switch (sub) {
-        case 0: {
-            // pre-LN: xs = LN1(residual stream)
-            if (c.layer_norm_first)
-                KNORM(launch_layernorm(hs_in, (size_t)M, D, W.ln1_g.as<float>(), W.ln1_b.as<float>(), 0, nullptr,
-                                       w->xs_s.planes(m->scheme), st));
-            GemmParams p = lp.qkv;
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            if (rel)  // gate from the layer's attention input (post-LN: hs_in; pre-LN: LN1 output) modules.py:534-551
-                KMISC(launch_wavlm_gate(w->xs_s.planes(m->scheme), (size_t)M, B, T, H, D,
-                                        c.gru_rel_pos ? W.grep_w.as<float>() : nullptr, W.grep_b.as<float>(),
-                                        W.grep_a.as<float>(), w->gate.as<float>(), st));
-            return 0;
-        }
-        case 1: {
-            KATTN(launch_attention(lp.attn, st));
-            return 0;
-        }
-        case 2: {
-            GemmParams p = lp.out;
-            p.residual = hs_in;
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            if (c.layer_norm_first)  // x1_s = LN2(r1), r1 = x1_f32
-                KNORM(launch_layernorm(w->x1_f32.as<float>(), (size_t)M, D, W.ln2_g.as<float>(), W.ln2_b.as<float>(), 0,
-                                       nullptr, w->x1_s.planes(m->scheme), st));
-            else  // x1 = LN1(x + attn)
-                KNORM(launch_layernorm(w->tmp_f32.as<float>(), (size_t)M, D, W.ln1_g.as<float>(), W.ln1_b.as<float>(), 0,
-                                       w->x1_f32.as<float>(), w->x1_s.planes(m->scheme), st));
-            return 0;
-        }
-        case 3: {
-            GemmParams p = lp.fc1;
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            return 0;
-        }
-        default: {
-            GemmParams p = lp.fc2;
-            // pre-LN: the sum IS hidden state l+1 (un-normalised residual stream), except after the last layer
-            float* unnorm = (last && last_res != nullptr) ? last_res : w->tmp_f32.as<float>();
-            if (c.layer_norm_first) p.out_f32 = last ? unnorm : hs_out;
-            if (ffn_out != nullptr) p.out_pre = ffn_out + (size_t)l * ffn_stride;
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            const bool want_planes = !last || c.pred_heads > 0;  // the next layer's (or the prediction heads') operand
-            if (c.layer_norm_first) {
-                if (last)  // encoder.layer_norm on the final output (wav2vec2_model.py:3049-3050)
-                    KNORM(launch_layernorm(unnorm, (size_t)M, D, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(), 0,
-                                           hs_out, c.pred_heads > 0 ? w->xs_s.planes(m->scheme) : no_planes(), st));
-            } else {
-                KNORM(launch_layernorm(w->tmp_f32.as<float>(), (size_t)M, D, W.ln2_g.as<float>(), W.ln2_b.as<float>(), 0,
-                                       hs_out, want_planes ? w->xs_s.planes(m->scheme) : no_planes(), st));
-            }
-            if (layer_done) S3B_OK(layer_done(m, l + 1, st, user));
-            return 0;
-        }
-    }
+    S3B_OK(add_pos_conv(lane, steps));
+    for (int l = 0; l < c.num_layers; ++l) S3B_OK(add_transformer_layer(lane, l, steps));
+    if (c.pred_heads > 0) S3B_OK(add_pred_heads(lane, steps));
     return 0;
-}
-
-// Conformer layer l, stage `sub` of kConformerStages (buffers: build_conformer_layer)
-int Fwd::conformer_stage(int l, int sub) {
-    s3b_model* m = this->m;  // the launch macros expect `m` and `st`
-    cudaStream_t st = this->st;
-    const s3b_config& c = m->cfg;
-    const int D = c.embed_dim;
-    const double attn_flops = 4.0 * (double)T * T * D * B;
-    LayerW& W = m->layers[l];
-    LayerPlan& lp = plan->layers[l];
-    const OutPlanes xs = w->xs_s.planes(m->scheme);
-    switch (sub) {
-        case 0: {  // ffn1: LayerNorm -> w_1 + SiLU
-            KNORM(launch_layernorm(hs(l), (size_t)M, D, W.ffn1_ln_g.as<float>(), W.ffn1_ln_b.as<float>(), 0, nullptr, xs, st));
-            GemmParams p = lp.ffn1_a;
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            return 0;
-        }
-        case 1: {  // r1 = x + 0.5 w_2(...)
-            GemmParams p = lp.ffn1_b;
-            p.residual = hs(l);
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            return 0;
-        }
-        case 2: {  // self_attn_layer_norm + RoPE -> [q | k] and v
-            KNORM(launch_layernorm_rope(w->x1_f32.as<float>(), (size_t)M, T, D, W.ln1_g.as<float>(), W.ln1_b.as<float>(),
-                                        m->rope_cs.as<float>(), xs, w->x1_s.planes(m->scheme), st));
-            {
-                GemmParams p = lp.qkv;
-                KGEMM(launch_gemm(p, m->sm_count, st));
-            }
-            GemmParams p = lp.v;
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            return 0;
-        }
-        case 3:
-            KATTN(launch_attention(lp.attn, st));
-            return 0;
-        case 4: {  // r2 = r1 + linear_out
-            GemmParams p = lp.out;
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            return 0;
-        }
-        case 5: {  // conv_module: LayerNorm -> pointwise_conv1
-            KNORM(launch_layernorm(w->x_f32.as<float>(), (size_t)M, D, W.conv_ln_g.as<float>(), W.conv_ln_b.as<float>(), 0,
-                                   nullptr, xs, st));
-            GemmParams p = lp.pw1;
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            return 0;
-        }
-        case 6:  // GLU -> depthwise conv -> BatchNorm -> SiLU
-            KMISC(launch_depthwise_glu(w->glu_f32.as<float>(), B, T, D, c.depthwise_kernel, W.dw_w.as<float>(),
-                                       W.dw_b.as<float>(), w->x1_s.planes(m->scheme), st));
-            return 0;
-        case 7: {  // r3 = r2 + pointwise_conv2
-            GemmParams p = lp.pw2;
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            return 0;
-        }
-        case 8: {  // ffn2: LayerNorm -> w_1 + SiLU
-            KNORM(launch_layernorm(w->x1_f32.as<float>(), (size_t)M, D, W.ffn2_ln_g.as<float>(), W.ffn2_ln_b.as<float>(), 0,
-                                   nullptr, xs, st));
-            GemmParams p = lp.fc1;
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            return 0;
-        }
-        default: {  // r4 = r3 + 0.5 w_2(...) -> final_layer_norm -> hidden state l+1 (pre-LN: encoder.layer_norm after
-                    // the last layer, wav2vec2_model.py:3049-3050)
-            GemmParams p = lp.fc2;
-            KGEMM(launch_gemm(p, m->sm_count, st));
-            float* r4 = w->tmp_f32.as<float>();
-            const bool enc_ln = c.layer_norm_first && l == c.num_layers - 1;
-            KNORM(launch_layernorm(r4, (size_t)M, D, W.ln2_g.as<float>(), W.ln2_b.as<float>(), 0, enc_ln ? r4 : hs(l + 1),
-                                   no_planes(), st));
-            if (enc_ln)
-                KNORM(launch_layernorm(r4, (size_t)M, D, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(), 0, hs(l + 1),
-                                       no_planes(), st));
-            if (layer_done) S3B_OK(layer_done(m, l + 1, st, user));
-            return 0;
-        }
-    }
 }
 
 // Number of lanes for a batch: S3B_LANES overrides; otherwise two lanes when the batch can be split AND carries at
@@ -2161,21 +2075,23 @@ static int forward_lanes(s3b_model* m, const float* const* wavs, const int64_t* 
         f[1].st = w1.stream.get();
     }
     for (int i = 0; i < lanes; ++i) S3B_OK(f[i].prepare());
-    const int ns = f[0].num_stages();
     if (concurrent) {
+        const std::vector<Step>& s0 = f[0].plan->steps;
+        const std::vector<Step>& s1 = f[1].plan->steps;
+        if (s0.size() != s1.size()) return fail("internal: the lanes have %zu and %zu steps", s0.size(), s1.size());
         CUDA_OK(cudaEventRecord(m->fork_event.get(), st));
         CUDA_OK(cudaStreamWaitEvent(f[1].st, m->fork_event.get(), 0));
-        // lane 1 trails lane 0 by two stages: while one lane runs a GEMM the other tends to be in a different kind
+        // lane 1 trails lane 0 by two steps: while one lane runs a GEMM the other tends to be in a different kind
         // of kernel (attention, LayerNorm, another GEMM shape), which is what lets them share the SMs
-        for (int s = 0; s < ns + 2; ++s) {
-            if (s < ns) S3B_OK(f[0].stage(s));
-            if (s >= 2) S3B_OK(f[1].stage(s - 2));
+        for (size_t s = 0; s < s0.size() + 2; ++s) {
+            if (s < s0.size()) S3B_OK(s0[s](f[0]));
+            if (s >= 2) S3B_OK(s1[s - 2](f[1]));
         }
         CUDA_OK(cudaEventRecord(m->ws[1].done.get(), f[1].st));
         CUDA_OK(cudaStreamWaitEvent(st, m->ws[1].done.get(), 0));
     } else {
         for (int i = 0; i < lanes; ++i)
-            for (int s = 0; s < ns; ++s) S3B_OK(f[i].stage(s));
+            for (const Step& step : f[i].plan->steps) S3B_OK(step(f[i]));
     }
     return 0;
 }
@@ -2272,7 +2188,7 @@ static int forward_host_impl(s3b_model* m, const float* const* wavs, const int64
         f.Lmax = max_len, f.hidden = hidden_dev + (size_t)b0 * frame_elems, f.layer_stride = layer_elems;
         f.layer_done = layer_done, f.user = &ctxs[c];
         S3B_OK(f.prepare());
-        for (int s = 0; s < f.num_stages(); ++s) S3B_OK(f.stage(s));
+        for (const Step& step : f.plan->steps) S3B_OK(step(f));
     }
     CUDA_OK(cudaStreamSynchronize(st));
     CUDA_OK(cudaStreamSynchronize(m->copy_stream.get()));
@@ -2536,13 +2452,9 @@ extern "C" int s3b_linear_ex(const float* a, const float* w, const float* bias, 
     cudaStream_t st = (cudaStream_t)stream;
     int sms = 0;
     S3B_OK(device_sm_count(&sms));
-    g_sm_count = sms;  // the tile-width choice a model finalized on this device makes
     SplitBuf as, ws, os;
     S3B_OK(split_operand(a, as, (size_t)M * lda, scheme, 0, st));
     S3B_OK(split_operand(w, ws, (size_t)N * K, scheme, 1, st));
-    GemmParams p;
-    S3B_OK(linear_params(p, as, ws, M, N, K, scheme, lda, (size_t)o.a_off, o.tile_n));
-    if (o.tile_n != 0 && p.bn != o.tile_n) return fail("tile_n %d requested, %d chosen", o.tile_n, p.bn);
     Epi e;
     e.bias = bias, e.residual = residual, e.gelu = gelu, e.row_mask = o.row_mask;
     if (o.out_fmt < 0) {
@@ -2551,7 +2463,9 @@ extern "C" int s3b_linear_ex(const float* a, const float* w, const float* bias, 
         S3B_OK(os.ensure((size_t)M * N));
         e.op = os.planes(o.out_fmt);
     }
-    set_epi(p, e, N);
+    GemmParams p;
+    S3B_OK(linear_params(p, as, ws, M, N, K, scheme, sms, e, lda, (size_t)o.a_off, o.tile_n));
+    if (o.tile_n != 0 && p.bn != o.tile_n) return fail("tile_n %d requested, %d chosen", o.tile_n, p.bn);
     p.out_pre = o.out_pre;
     CUDA_OK(launch_gemm(p, sms, st));
     if (o.out_fmt >= 0) CUDA_OK(launch_planes_to_f32(os.planes(o.out_fmt), (size_t)M * N, out, st));
@@ -2577,7 +2491,6 @@ extern "C" int s3b_qkv_hd_f32(const float* x, const float* w, const float* b, in
     cudaStream_t st = (cudaStream_t)stream;
     int sms = 0;
     S3B_OK(device_sm_count(&sms));
-    g_sm_count = sms;
     SplitBuf xs, ws, qs, ks, vts;
     S3B_OK(split_operand(x, xs, (size_t)M * D, sch, 0, st));
     S3B_OK(split_operand(w, ws, (size_t)3 * D * D, sch, 1, st));
@@ -2585,7 +2498,7 @@ extern "C" int s3b_qkv_hd_f32(const float* x, const float* w, const float* b, in
     S3B_OK(ks.ensure((size_t)M * D));
     S3B_OK(vts.ensure((size_t)B * D * Tp));
     GemmParams p;
-    S3B_OK(linear_params(p, xs, ws, M, 3 * D, D, sch));
+    S3B_OK(linear_params(p, xs, ws, M, 3 * D, D, sch, sms, Epi()));
     set_qkv_epi(p, b, T, H, hd, qs, ks, vts);
     CUDA_OK(launch_gemm(p, sms, st));
     CUDA_OK(launch_planes_to_f32(qs.planes(0), (size_t)M * D, q_out, st));
@@ -2619,8 +2532,6 @@ extern "C" int s3b_conv_gemm_f32(const float* x, const float* w, const float* bi
     const std::vector<float> wl = conv_weight_layout(wh.data(), kw);
     S3B_OK(upload_split(ws, wl.data(), wl.size(), sch));
     S3B_OK(split_operand(x, xs, (size_t)B * Lin * C, sch, 0, st));
-    GemmParams p;
-    S3B_OK(conv_params(p, xs, ws, B, Lin, Lout, kw, sch));
     Epi e;
     e.bias = bias, e.gelu = gelu;
     if (out_fmt < 0) {
@@ -2629,7 +2540,8 @@ extern "C" int s3b_conv_gemm_f32(const float* x, const float* w, const float* bi
         S3B_OK(os.ensure((size_t)B * Lout * C));
         e.op = os.planes(out_fmt);
     }
-    set_epi(p, e, C);
+    GemmParams p;
+    S3B_OK(conv_params(p, xs, ws, B, Lin, Lout, kw, sch, e));
     CUDA_OK(launch_gemm(p, sms, st));
     if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), (size_t)B * Lout * C, out, st));
     CUDA_OK(cudaStreamSynchronize(st));
@@ -2653,7 +2565,7 @@ extern "C" int s3b_posconv_f32(const float* x, const float* w, const float* bias
                                                                "four taps per k-block)", k);
     if (taps == 4 && 4 * cpg != 192 && 4 * cpg != 256) return fail("four taps per k-block need 48 or 64 channels per group");
     if (taps == 1 && mode != 0) return fail("the data2vec blocks (mode 1, 2) run four taps per k-block only");
-    if (taps == 1 && gamma == nullptr && out_fmt >= 0)  // Fwd::stage(8): the one-tap epilogue writes fp32 only
+    if (taps == 1 && gamma == nullptr && out_fmt >= 0)  // add_pos_conv: the one-tap epilogue writes fp32 only
         return fail("one tap per k-block writes operand planes only through the LayerNorm (gamma)");
     S3B_OK(check_out_fmt(out_fmt));
     // one conv block of k taps: pos_taps(c) = k (the data2vec blocks' k = max(3, conv_pos / depth) is the caller's)
@@ -2679,27 +2591,19 @@ extern "C" int s3b_posconv_f32(const float* x, const float* w, const float* bias
     }
     float* out_f32 = out_fmt < 0 ? out : nullptr;
     GemmParams p;
-    Epi e;
     if (taps == 4) {
-        // Fwd::stage(8): Z = the four-tap GEMM, then the combine kernel (+ LayerNorm)
+        // add_pos_conv: Z = the four-tap GEMM, then the combine kernel (+ LayerNorm)
         S3B_OK(z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
-        S3B_OK(posconv4_params(p, c, xs.h(), xs.l(), ws.h(), ws.l(), B, T));
-        e.out_f32 = z.as<float>();
-        set_epi(p, e, 4 * D);
+        S3B_OK(posconv4_params(p, c, xs.h(), xs.l(), ws.h(), ws.l(), B, T, epi_f32(z.as<float>())));
         CUDA_OK(launch_gemm(p, sms, st));
         CUDA_OK(launch_posconv_combine(z.as<float>(), x, bias, B, T, D, cpg, gamma, beta, gamma ? 1 : 0, mode,
                                        out_f32, op, st));
     } else {
-        // Fwd::stage(8), one tap per k-block: x + GELU(conv + bias) in the epilogue, then the LayerNorm
-        S3B_OK(posconv_params(p, c, xs.h(), xs.l(), ws.h(), ws.l(), B, T));
-        e.bias = bias, e.gelu = 1, e.residual = x;
-        if (gamma != nullptr) {
-            S3B_OK(z.ensure(M * D * sizeof(float)));
-            e.out_f32 = z.as<float>();
-        } else {
-            e.out_f32 = out_f32;
-        }
-        set_epi(p, e, D);
+        // add_pos_conv, one tap per k-block: x + GELU(conv + bias) in the epilogue, then the LayerNorm
+        if (gamma != nullptr) S3B_OK(z.ensure(M * D * sizeof(float)));
+        Epi e = epi_f32(gamma != nullptr ? z.as<float>() : out_f32, bias, x);
+        e.gelu = 1;
+        S3B_OK(posconv_params(p, c, xs.h(), xs.l(), ws.h(), ws.l(), B, T, e));
         CUDA_OK(launch_gemm(p, sms, st));
         if (gamma != nullptr) CUDA_OK(launch_layernorm(z.as<float>(), M, D, gamma, beta, 0, out_f32, op, st));
     }
@@ -2715,7 +2619,6 @@ extern "C" int s3b_gemm_bench(int64_t M, int32_t N, int32_t K, int32_t gelu, int
     if (!ms_per_launch || iters < 1) return fail("bad argument");
     int sms = 0;
     S3B_OK(device_sm_count(&sms));
-    g_sm_count = sms;
     SplitBuf as, ws, os;
     DevBuf bias, res, out;
     S3B_OK(as.ensure((size_t)M * K));
@@ -2730,12 +2633,9 @@ extern "C" int s3b_gemm_bench(int64_t M, int32_t N, int32_t K, int32_t gelu, int
     GemmParams p;
     int scheme = default_scheme();
     if (K % 128 != 0 || N % 128 != 0) scheme = 0;
-    S3B_OK(linear_params(p, as, ws, M, N, K, scheme, 0, 0, force_un));
-    Epi e;
-    e.bias = bias.as<float>();
-    if (gelu) e.gelu = 1, e.op = os.planes(scheme);
-    else e.residual = res.as<float>(), e.out_f32 = out.as<float>();
-    set_epi(p, e, N);
+    const Epi e = gelu ? epi_planes(os.planes(scheme), bias.as<float>(), 1)
+                       : epi_f32(out.as<float>(), bias.as<float>(), res.as<float>());
+    S3B_OK(linear_params(p, as, ws, M, N, K, scheme, sms, e, 0, 0, force_un));
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     cudaEventCreate(&e0), cudaEventCreate(&e1);
     const Event t0(e0), t1(e1);
@@ -2868,7 +2768,8 @@ extern "C" int s3b_frontend_f32(const float* const* wavs, const int64_t* lens, i
                                 int32_t normalize, const float* w, const float* bias, const float* gamma,
                                 const float* beta, int32_t layer_norm, int32_t out_fmt, float* wav_out, float* out,
                                 void* stream) {
-    // the launches of Fwd::stage(0) (launch_frontend) on workspaces of this call; the conv-0 planes decoded to fp32
+    // the first step of add_conv_frontend (launch_frontend) on workspaces of this call; the conv-0 planes decoded to
+    // fp32
     if (!wavs || !lens || !w || !gamma || !beta || !out) return fail("null argument");
     if (B < 1) return fail("bad batch %d", B);
     if (max_len < kConvK[0]) return fail("max_len %lld is below the conv-0 window of %d samples", (long long)max_len,
@@ -2908,8 +2809,8 @@ extern "C" int s3b_frontend_f32(const float* const* wavs, const int64_t* lens, i
     return 0;
 }
 
-// Fwd::stage(0) of a DeCoAR 2.0 (step 2) or APC (step 1) model on workspaces of this call; the operand planes
-// decoded, columns 0..79 kept
+// add_fbank_frontend's step for a DeCoAR 2.0 (step 2) or APC (step 1) model on workspaces of this call; the operand
+// planes decoded, columns 0..79 kept
 static int fbank_cmvn_features(const float* const* wavs, const int64_t* lens, int32_t B, int step, int32_t out_fmt,
                                float* out, void* stream) {
     if (!wavs || !lens || !out) return fail("null argument");
@@ -2971,7 +2872,7 @@ extern "C" int s3b_gru_max_active_clusters(int32_t* out) {
 extern "C" int s3b_gru_f32(const float* xg, const float* whh, const float* bhh, const float* residual,
                            const int32_t* lens, int32_t B, int32_t T, int32_t hidden, int32_t out_fmt, float* out,
                            float* planes_out, void* stream) {
-    // Fwd::apc_stage(2 + 2l) on this call's buffers: b_hr / b_hz added to a copy of xg as the model's GEMM bias adds
+    // add_gru_stack's recurrence on this call's buffers: b_hr / b_hz added to a copy of xg as the model's GEMM bias adds
     // them, utterances grouped longest first as the model groups them
     if (!xg || !whh || !bhh || !lens || !out) return fail("null argument");
     if (hidden != kGruHidden) return fail("hidden %d: the recurrence kernel is built for %d", hidden, kGruHidden);
@@ -3024,7 +2925,7 @@ extern "C" int s3b_lstm_fits(int32_t* out) {
 extern "C" int s3b_lstm_f32(const float* xg, const float* whh, const float* bhh, const int32_t* lens, int32_t B,
                             int32_t T, int32_t direction, int32_t out_fmt, float* out, float* planes_out,
                             void* stream) {
-    // Fwd::decoar_stage(3 + 4l + 2d) on this call's buffers, utterances ordered longest first as the model orders them
+    // add_lstm_stack's recurrence on this call's buffers, utterances ordered longest first as the model orders them
     if (!xg || !whh || !lens || !out) return fail("null argument");
     if (B < 1 || T < 1) return fail("bad sizes (batch %d, t %d)", B, T);
     if (direction != 0 && direction != 1) return fail("direction must be 0 (forward) or 1 (backward), not %d", direction);
@@ -3070,7 +2971,7 @@ extern "C" int s3b_lstm_f32(const float* xg, const float* whh, const float* bhh,
 extern "C" int s3b_conformer_conv_f32(const float* x, int32_t B, int32_t T, int32_t D, int32_t k, const float* dw_w,
                                       const float* bn_gamma, const float* bn_beta, const float* bn_mean,
                                       const float* bn_var, int32_t out_fmt, float* out, void* stream) {
-    // Fwd::conformer_stage(6) on this call's buffers: BatchNorm folded on the host like s3b_model_finalize does it
+    // add_conformer_layer's depthwise step on this call's buffers: BatchNorm folded on the host like s3b_model_finalize does it
     if (!x || !dw_w || !bn_gamma || !bn_beta || !bn_mean || !bn_var || !out) return fail("null argument");
     if (B < 1 || T < 1) return fail("bad sizes (batch %d, t %d)", B, T);
     if (D < 64 || D % 64 != 0) return fail("d must be a positive multiple of 64, not %d", D);
@@ -3099,7 +3000,7 @@ extern "C" int s3b_conformer_conv_f32(const float* x, int32_t B, int32_t T, int3
 extern "C" int s3b_layernorm_rope_f32(const float* x, int64_t M, int32_t T, int32_t D, const float* gamma,
                                       const float* beta, const float* inv_freq, int32_t out_fmt, float* out,
                                       float* out_rope, void* stream) {
-    // Fwd::conformer_stage(2)'s LayerNorm + RoPE kernel, with a table built for the t frames like build_rope_table
+    // add_conformer_layer's LayerNorm + RoPE kernel, with a table built for the t frames like build_rope_table
     if (!x || !gamma || !beta || !out || !out_rope) return fail("null argument");
     if (M < 1 || T < 1 || M % T != 0) return fail("m = %lld must be a positive multiple of t = %d", (long long)M, T);
     if (D != 512 && D != 768 && D != 1024 && D != 1280) return fail("d must be 512, 768, 1024 or 1280, not %d", D);

@@ -474,7 +474,7 @@ def _pos_inputs(B, T, D, G, k, seed):
 @pytest.mark.parametrize("T", [1, 2, 3, 64, 65, 128, 129, 499])
 @pytest.mark.parametrize("D,G,k,taps,mode", POS_CONFIGS)
 def test_posconv(s3b_lib, D, G, k, taps, mode, T):
-    """Positional conv as Fwd::stage(8) runs it, B = 2: x + GELU(conv + b) (mode 0), the data2vec blocks (mode 1, and
+    """Positional conv as the model's add_pos_conv runs it, B = 2: x + GELU(conv + b) (mode 0), the data2vec blocks (mode 1, and
     mode 2 with the residual), against F.conv1d(padding k // 2, groups) truncated to T and the mode's arithmetic in
     fp64; the bounds propagate through GELU and the LayerNorms (_ln_bound)."""
     x, w, bias, _ = _pos_inputs(2, T, D, G, k, D + k * 3 + taps + 10 * mode + T * 100)
