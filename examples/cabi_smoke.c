@@ -33,6 +33,7 @@ int main(void) {
         (const void*)s3b_apc_model_create, (const void*)s3b_profile_read_ex, (const void*)s3b_apc_features_f32,
         (const void*)s3b_gru_f32,        (const void*)s3b_gru_max_active_clusters,
         (const void*)s3b_decoar_model_create, (const void*)s3b_lstm_f32, (const void*)s3b_lstm_fits,
+        (const void*)s3b_npc_model_create, (const void*)s3b_npc_conv_f32,
     };
     s3b_config cfg;
     int64_t lens[2] = {16000, 800};
@@ -96,6 +97,24 @@ int main(void) {
             s3b_model_destroy(m);
             if (valid[0] != 98 || valid[1] != 3) return 10;
         }
+    }
+    {
+        /* NPC: the APC frame rule; every block, every masked conv and feat are outputs (4 blocks: 9) */
+        s3b_npc_config ncfg;
+        s3b_model* m = NULL;
+        memset(&ncfg, 0, sizeof(ncfg));
+        ncfg.struct_size = (int32_t)sizeof(ncfg), ncfg.n_blocks = 4, ncfg.hidden = 512;
+        ncfg.kernel_size = 15, ncfg.mask_size = 5, ncfg.residual = 1, ncfg.batch_norm = 1, ncfg.act = 0;
+        if (s3b_npc_model_create(&ncfg, &m) != 0) {
+            printf("s3b_npc_model_create: %s\n", s3b_last_error());
+            return 11;
+        }
+        if (s3b_valid_frames(m, lens, 2, 16000, valid) != 0 || s3b_num_outputs(m) != 9) {
+            printf("NPC bookkeeping: %s\n", s3b_last_error());
+            return 12;
+        }
+        s3b_model_destroy(m);
+        if (valid[0] != 98 || valid[1] != 3) return 13;
     }
     return 0;
 }

@@ -117,6 +117,34 @@ typedef struct s3b_decoar_config {
     int32_t reserved[4]; /* 0 */
 } s3b_decoar_config;
 int s3b_decoar_model_create(const s3b_decoar_config* cfg, s3b_model** out);
+/* NPC (s3prl/upstream/npc/{expert,npc,audio}.py). The APC front end (kaldi fbank, 80 bins, hamming window, CMVN over
+ * all m frames with the unbiased std, pad_sequence to T = max m), then n_blocks blocks: ConvBlock i is
+ * act(bn2(linear(act(bn1(conv(x))))) (+ x when residual and i > 0)), with conv = Conv1d(k 3, padding 1) (80 input
+ * channels in block 0, 512 after) and linear = Conv1d(512, 512, 1); masked conv i is tanh(Conv1d(512, 512,
+ * kernel_size, padding (kernel_size - 1) / 2)) with a centred band of mask_size + 2 (i + 1) taps masked out; feat =
+ * the sum of the masked convs. Frames t >= m_b are NOT zero: they hold the response to the zero padding features, and
+ * valid frames near m_b read them, so an utterance's result depends on T (as in the reference).
+ * Tensors (reference key names): blocks.{i}.conv.{weight [512][80 or 512][3], bias}, blocks.{i}.linear.{weight
+ * [512][512][1], bias}, with batch_norm blocks.{i}.bn{1,2}.{weight, bias, running_mean, running_var};
+ * masked_convs.{i}.conv.{weight [512][512][kernel_size], bias} and masked_convs.{i}.conv_mask (same shape). Other
+ * keys (vq_layers.*, postnet.*, num_batches_tracked) are ignored. Finalize folds each BatchNorm (eps 1e-5) into the
+ * conv before it, multiplies each masked weight by its conv_mask and fails, naming the block, if weight is left on
+ * a tap the config masks; only the unmasked taps are computed.
+ * s3b_num_outputs = 2 n_blocks + 1: hidden_out is [block 0, masked conv 0, block 1, ..., masked conv n-1, feat]
+ * [batch][T][512]. The model works with the calls listed for APC; lens[b] >= 560 samples; s3b_forward_ex refuses
+ * ffn_out and last_residual. Served: hidden 512, odd kernel_size > mask_size + 2 n_blocks, odd mask_size. */
+typedef struct s3b_npc_config {
+    int32_t struct_size; /* sizeof(s3b_npc_config) */
+    int32_t n_blocks;    /* config["model"]["paras"]["n_blocks"], 1..32 */
+    int32_t hidden;      /* hidden_size: 512 */
+    int32_t kernel_size; /* masked conv kernel (odd) */
+    int32_t mask_size;   /* odd; masked conv i masks mask_size + 2 (i + 1) centred taps */
+    int32_t residual;    /* 0 or 1 */
+    int32_t batch_norm;  /* 0 or 1 */
+    int32_t act;         /* activate: 0 = relu, 1 = tanh */
+    int32_t reserved[4]; /* 0 */
+} s3b_npc_config;
+int s3b_npc_model_create(const s3b_npc_config* cfg, s3b_model** out);
 int s3b_model_finalize(s3b_model* m);
 void s3b_model_destroy(s3b_model* m);
 
@@ -346,6 +374,15 @@ int s3b_conv_gemm_f32(const float* x, const float* w, const float* bias, int32_t
 int s3b_posconv_f32(const float* x, const float* w, const float* bias, int32_t batch, int32_t t, int32_t d,
                     int32_t groups, int32_t k, int32_t taps_per_kblock, int32_t mode, const float* gamma,
                     const float* beta, int32_t out_fmt, float* out, void* stream);
+/* One NPC convolution as the model runs it: same padding ((k - 1) / 2), implicit GEMM over channels-last
+ * x [batch][t][c_in] (c_in 80, zero-padded to 128 per tap, or 512), weight w [512][c_in][k] (torch layout, device),
+ * mask: 0 = every tap, else the odd width of a centred band of taps left out (the MaskConvBlock's conv_mask);
+ * out = act(conv + bias) + residual, or act(conv + bias + residual) with res_first (the ConvBlock); act 0 = none,
+ * 1 = ReLU, 2 = tanh; bias, residual ([batch][t][512]) optional; out_pre: optional act(conv + bias) before the
+ * residual (not with res_first). scheme -1 / 0 / 1 as s3b_linear_ex. out: [batch][t][512] fp32. */
+int s3b_npc_conv_f32(const float* x, int32_t batch, int32_t t, int32_t c_in, const float* w, int32_t k, int32_t mask,
+                     const float* bias, const float* residual, int32_t act, int32_t res_first, int32_t scheme,
+                     float* out, float* out_pre, void* stream);
 /* micro-benchmark of the production GEMM kernel: `iters` back-to-back launches of [M][K] x [N][K]^T with the fc1-style
  * epilogue (gelu != 0: bias + GELU + bf16 hi/lo output) or the out_proj-style one (bias + residual + fp32 output).
  * force_un in {0 = the library's choice, 128, 256} forces the tile width (columns per output tile) wherever it divides

@@ -35,7 +35,8 @@ struct GemmParams {
     // all of them (TMA multicast): the A tensor maps then have box height 128 / cluster_n.
     int cluster_n;
     // k-block kb reads   A box at (a_k_per_ntile*n_tile + (kb % kb_per_row)*64,
-    //                              row0 + (kb / kb_per_row)*a_row_step + a_row_off, batch)
+    //                              row0 + kq*a_row_step + a_row_off + (kq >= a_gap_at ? a_gap : 0), batch)
+    //                    with kq = kb / kb_per_row
     //                    B box at (b_k_linear ? kb*64 : (kb % kb_per_row)*64, b_n_tiled ? n_tile*bn : 0,
     //                              b_k_linear ? 0 : kb / kb_per_row + n_tile*b_z_per_ntile)
     int kb_per_row;
@@ -45,9 +46,15 @@ struct GemmParams {
     int b_n_tiled;
     int b_k_linear;
     int b_z_per_ntile;
+    // a tap convolution that skips a band of taps (the NPC masked conv): k-block rows kq >= a_gap_at read a_gap rows
+    // further on. a_gap 0 is the plain walk.
+    int a_gap_at;
+    int a_gap;
 
     // ---- epilogue: v = acc (+bias[n]) ; act ; (+residual[m][n]) ; row_mask[m] ? 0 -----------------
-    // gelu: 0 = no activation, 1 = GELU (exact erf), 2 = SiLU (x * sigmoid(x), the Conformer's Swish)
+    // gelu: the activation: 0 = none, 1 = GELU (exact erf), 2 = SiLU (x * sigmoid(x), the Conformer's Swish),
+    //       3 = ReLU, 4 = tanh
+    // res_first: v = acc (+bias) (+residual) ; act instead (the NPC ConvBlock's act(out + res)); out_pre is then unused
     // The launch picks one kernel instantiation per output kind: out_f32, operand planes (out_hi ...), both (widths
     // >= 128 only) or the QKV scatter (widths >= 128 only). A launch with none of them is an error.
     int out_rows_per_batch;  // flat output row m = batch*out_rows_per_batch + row
@@ -56,6 +63,7 @@ struct GemmParams {
     const float* residual;
     const uint8_t* row_mask;
     int gelu;
+    int res_first;
     float* out_f32;
     __nv_bfloat16* out_hi;
     __nv_bfloat16* out_lo;

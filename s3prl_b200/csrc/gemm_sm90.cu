@@ -49,7 +49,8 @@ struct GemmCfg {
 };
 
 // Epilogue kinds, one kernel instantiation each (chosen per launch in launch_gemm). Every non-QKV kind computes
-//   v = acc (+bias) ; GELU or SiLU? ; out_pre = v? ; (+residual) ; row_mask ? 0
+//   v = acc (+bias) ; GELU, SiLU, ReLU or tanh? ; out_pre = v? ; (+residual) ; row_mask ? 0
+// or, with res_first, v = acc (+bias) (+residual) ; activation ; row_mask ? 0
 // and stores v as fp32, as operand planes, or both.
 enum EpiKind { kEpiF32 = 1, kEpiPlanes = 2, kEpiBoth = 3, kEpiQkv = 4 };
 
@@ -115,7 +116,7 @@ __device__ __forceinline__ void produce(const GemmParams& p, uint8_t* smem, uint
                 uint8_t* st = smem + stage * Cfg::kStageBytes;
                 uint8_t* sb = st + 2 * Cfg::kAPlane;
                 mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)Cfg::kStageBytes);
-                const int a_row = row0 + kq * p.a_row_step + p.a_row_off;
+                const int a_row = row0 + kq * p.a_row_step + p.a_row_off + (kq >= p.a_gap_at ? p.a_gap : 0);
                 const int a_k = a_k0 + kr * kBlockK;
                 const int b_k = (p.b_k_linear ? kb : kr) * kBlockK;
                 const int b_z = p.b_k_linear ? 0 : b_z0 + kq;
@@ -371,6 +372,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float (&acc)[
     } else {
         const int act = p.gelu;
         const bool has_res = p.residual != nullptr, has_pre = p.out_pre != nullptr;
+        const bool res_first = has_res && p.res_first != 0, add_res_after = has_res && p.res_first == 0;
         const int fmt = p.out_fmt;
         size_t off[kRows];
         bool zero[kRows];
@@ -401,6 +403,10 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float (&acc)[
 #pragma unroll
                     for (int jj = 0; jj < kCh; ++jj) a[4 * (c + jj) + r2] += bv[jj].x, a[4 * (c + jj) + r2 + 1] += bv[jj].y;
                 }
+                if (res_first) {
+#pragma unroll
+                    for (int jj = 0; jj < kCh; ++jj) a[4 * (c + jj) + r2] += rv[jj].x, a[4 * (c + jj) + r2 + 1] += rv[jj].y;
+                }
                 if (act == 1) {
 #pragma unroll
                     for (int jj = 0; jj < kCh; ++jj)
@@ -411,6 +417,16 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float (&acc)[
                     for (int jj = 0; jj < kCh; ++jj)
                         a[4 * (c + jj) + r2] = silu(a[4 * (c + jj) + r2]),
                         a[4 * (c + jj) + r2 + 1] = silu(a[4 * (c + jj) + r2 + 1]);
+                } else if (act == 3) {
+#pragma unroll
+                    for (int jj = 0; jj < kCh; ++jj)
+                        a[4 * (c + jj) + r2] = fmaxf(a[4 * (c + jj) + r2], 0.f),
+                        a[4 * (c + jj) + r2 + 1] = fmaxf(a[4 * (c + jj) + r2 + 1], 0.f);
+                } else if (act == 4) {
+#pragma unroll
+                    for (int jj = 0; jj < kCh; ++jj)
+                        a[4 * (c + jj) + r2] = tanhf(a[4 * (c + jj) + r2]),
+                        a[4 * (c + jj) + r2 + 1] = tanhf(a[4 * (c + jj) + r2 + 1]);
                 }
                 if (has_pre) {
 #pragma unroll
@@ -418,7 +434,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float (&acc)[
                         *reinterpret_cast<float2*>(p.out_pre + off[s] + 8 * (c + jj)) =
                             make_float2(a[4 * (c + jj) + r2], a[4 * (c + jj) + r2 + 1]);
                 }
-                if (has_res) {
+                if (add_res_after) {
 #pragma unroll
                     for (int jj = 0; jj < kCh; ++jj) a[4 * (c + jj) + r2] += rv[jj].x, a[4 * (c + jj) + r2 + 1] += rv[jj].y;
                 }
@@ -667,6 +683,7 @@ static cudaError_t launch_n(const GemmParams& p, int sm_count, cudaStream_t stre
 
 cudaError_t launch_gemm(const GemmParams& p, int sm_count, cudaStream_t stream) {
     if (p.scheme != 0 && p.k_steps != 0) return cudaErrorInvalidValue;
+    if (p.gelu < 0 || p.gelu > 4 || (p.res_first != 0 && p.out_pre != nullptr)) return cudaErrorInvalidValue;
     if (p.out_fmt != 0 && (p.qkv_mode || (p.out_hi != nullptr && (p.out_h8 == nullptr || p.out_l8 == nullptr))))
         return cudaErrorInvalidValue;
     switch (p.bn) {

@@ -193,6 +193,9 @@ struct LayerW {
     // whh = weight_hh_lk [4H][H] fp32
     SplitBuf wih;
     DevBuf gru_b, whh, bhn;
+    // NPC block i (finalize_npc): fc1 = blocks.i.conv with bn1 folded in ([512][3 * Cp], tap-major, Cp = 128 for block
+    // 0's 80 channels, 512 after), fc2 = blocks.i.linear with bn2 folded in ([512][512]), out = masked_convs.i's
+    // unmasked taps ([512][u * 512]); fc1_b, fc2_b, out_b their biases
 };
 
 // per-category device-time profile (CUDA events around each launch on the launching stream)
@@ -267,6 +270,7 @@ enum ModelKind {
     kFbankEncoder,  // s3b_model_create, frontend 1 (DeCoAR 2.0): fbank + CMVN, every second frame, into the encoder
     kGruStack,      // s3b_apc_model_create (APC / VQ-APC): fbank + CMVN into a GRU stack
     kLstmStack,     // s3b_decoar_model_create (DeCoAR): fbank + CMVN, post_extract_proj, bidirectional LSTM stack
+    kNpcStack,      // s3b_npc_model_create (NPC): fbank + CMVN into ConvBlocks and masked convs
 };
 
 struct s3b_model {
@@ -276,6 +280,8 @@ struct s3b_model {
     int apc_residual = 0;
     // kLstmStack: cfg holds num_layers and embed_dim = 2 H (the forward | backward concat)
     int decoar_all_layers = 0;  // 1: decoar_layers (every layer's output), 0: decoar (the last one)
+    // kNpcStack: cfg holds num_layers = n_blocks and embed_dim = hidden
+    s3b_npc_config npc = {};
     std::map<std::string, HostTensor> host;
     bool finalized = false;
     int sm_count = 132;
@@ -504,6 +510,36 @@ extern "C" int s3b_decoar_model_create(const s3b_decoar_config* cfg, s3b_model**
     return 0;
 }
 
+// NPC's masked conv i zeroes a centred band of mask_size + 2 (i + 1) of its kernel_size taps (npc.py MaskConvBlock)
+static int npc_mask_width(const s3b_npc_config& c, int i) { return c.mask_size + 2 * (i + 1); }
+
+extern "C" int s3b_npc_model_create(const s3b_npc_config* cfg, s3b_model** out) {
+    if (!cfg || !out) return fail("null argument");
+    if (cfg->struct_size != (int32_t)sizeof(s3b_npc_config))
+        return fail("s3b_npc_config.struct_size %d != %d (header / library mismatch)", cfg->struct_size,
+                    (int)sizeof(s3b_npc_config));
+    if (cfg->n_blocks < 1 || cfg->n_blocks > 32) return fail("n_blocks %d: must be 1..32", cfg->n_blocks);
+    if (cfg->hidden != 512) return fail("hidden %d: NPC is served with hidden size 512", cfg->hidden);
+    if (cfg->kernel_size < 1 || cfg->kernel_size > 127 || cfg->kernel_size % 2 == 0)
+        return fail("kernel_size %d: must be odd, 1..127", cfg->kernel_size);
+    if (cfg->mask_size < 1 || cfg->mask_size % 2 == 0) return fail("mask_size %d: must be odd and >= 1", cfg->mask_size);
+    if (cfg->kernel_size <= cfg->mask_size + 2 * cfg->n_blocks)
+        return fail("kernel_size %d must exceed mask_size + 2 n_blocks = %d (the widest mask leaves no tap)",
+                    cfg->kernel_size, cfg->mask_size + 2 * cfg->n_blocks);
+    if (cfg->residual != 0 && cfg->residual != 1) return fail("residual must be 0 or 1, not %d", cfg->residual);
+    if (cfg->batch_norm != 0 && cfg->batch_norm != 1) return fail("batch_norm must be 0 or 1, not %d", cfg->batch_norm);
+    if (cfg->act != 0 && cfg->act != 1) return fail("act must be 0 (relu) or 1 (tanh), not %d", cfg->act);
+    for (int i = 0; i < 4; ++i)
+        if (cfg->reserved[i] != 0) return fail("s3b_npc_config.reserved[%d] must be 0", i);
+    s3b_model* m = new s3b_model();
+    memset(&m->cfg, 0, sizeof(m->cfg));
+    m->cfg.num_layers = cfg->n_blocks, m->cfg.embed_dim = cfg->hidden;
+    m->kind = kNpcStack, m->npc = *cfg;
+    m->scheme = default_scheme();
+    *out = m;
+    return 0;
+}
+
 extern "C" int s3b_model_set_tensor(s3b_model* m, const char* name, const float* data, const int64_t* shape,
                                     int32_t ndim) {
     if (!m || !name || !data || (!shape && ndim > 0)) return fail("null argument");
@@ -721,6 +757,76 @@ static int finalize_apc(s3b_model* m) {
     if (clusters < 1)
         return fail("the GRU recurrence kernel cannot run on this device: cudaOccupancyMaxActiveClusters reports 0 "
                     "clusters of %d CTAs with %zu bytes of shared memory each", kGruCtas, gru_smem_bytes());
+    return 0;
+}
+
+// NPC tap conv weight w [512][cin][k] (fp64) -> the GEMM's B operand [512][u * Cp]: the u = k - mask taps outside the
+// centred band of `mask` taps, in tap order, each zero-padded from cin to Cp channels (tapconv_params)
+static std::vector<float> npc_weight_layout(const std::vector<double>& w, int cin, int k, int mask, int Cp) {
+    const int N = 512, u = k - mask, head = (k - mask) / 2;
+    std::vector<float> r((size_t)N * u * Cp, 0.f);
+    for (int o = 0; o < N; ++o)
+        for (int q = 0; q < u; ++q) {
+            const int tap = q < head ? q : q + mask;
+            for (int c = 0; c < cin; ++c) r[((size_t)o * u + q) * Cp + c] = (float)w[((size_t)o * cin + c) * k + tap];
+        }
+    return r;
+}
+
+// NPC (npc.py): per block i, ConvBlock conv [512][cin][3] -> bn1 -> act -> linear [512][512][1] -> bn2 (+ input) -> act,
+// then MaskConvBlock tanh(conv1d(x, W * conv_mask)). BatchNorm (eval, eps 1e-5) folds into the conv in front of it in
+// fp64: W' = W g / sqrt(v + eps), b' = (b - mu) g / sqrt(v + eps) + beta. The masked weight is multiplied by the file's
+// conv_mask; weight left on a tap the config masks means the file's mask is not the config's, and the model is refused.
+static int finalize_npc(s3b_model* m) {
+    const s3b_npc_config& c = m->npc;
+    const int NB = c.n_blocks, H = 512, k = c.kernel_size;
+    m->layers.resize(NB);
+    for (int i = 0; i < NB; ++i) {
+        LayerW& L = m->layers[i];
+        const std::string b = "blocks." + std::to_string(i) + ".";
+        const int cin = i == 0 ? 80 : H, Cp = i == 0 ? kDecoar2K : H;
+        for (int j = 0; j < 2; ++j) {
+            const std::string conv = b + (j == 0 ? "conv." : "linear."), bn = b + (j == 0 ? "bn1." : "bn2.");
+            const int kin = j == 0 ? cin : H, kw = j == 0 ? 3 : 1;
+            const HostTensor *w, *bias;
+            S3B_OK(need(m, conv + "weight", {H, kin, kw}, &w));
+            S3B_OK(need(m, conv + "bias", {H}, &bias));
+            std::vector<double> wd(w->data.begin(), w->data.end()), bd(bias->data.begin(), bias->data.end());
+            if (c.batch_norm) {
+                const HostTensor *g, *be, *mu, *var;
+                S3B_OK(need(m, bn + "weight", {H}, &g));
+                S3B_OK(need(m, bn + "bias", {H}, &be));
+                S3B_OK(need(m, bn + "running_mean", {H}, &mu));
+                S3B_OK(need(m, bn + "running_var", {H}, &var));
+                for (int o = 0; o < H; ++o) {
+                    const double sc = (double)g->data[o] / sqrt((double)var->data[o] + 1e-5);
+                    for (size_t e = 0; e < (size_t)kin * kw; ++e) wd[(size_t)o * kin * kw + e] *= sc;
+                    bd[o] = (bd[o] - (double)mu->data[o]) * sc + (double)be->data[o];
+                }
+            }
+            const std::vector<float> wl = npc_weight_layout(wd, kin, kw, 0, j == 0 ? Cp : H);
+            const std::vector<float> bl(bd.begin(), bd.end());
+            S3B_OK(upload_split(j == 0 ? L.fc1 : L.fc2, wl.data(), wl.size(), m->scheme));
+            S3B_OK(upload_f32(j == 0 ? L.fc1_b : L.fc2_b, bl.data(), bl.size()));
+        }
+        const std::string mc = "masked_convs." + std::to_string(i) + ".";
+        const HostTensor *w, *mask;
+        S3B_OK(need(m, mc + "conv.weight", {H, H, k}, &w));
+        S3B_OK(need(m, mc + "conv_mask", {H, H, k}, &mask));
+        const int mw = npc_mask_width(c, i), head = (k - mw) / 2;
+        std::vector<double> wd(w->numel());
+        for (size_t e = 0; e < wd.size(); ++e) {
+            wd[e] = (double)(w->data[e] * mask->data[e]);  // fp32, like the reference's conv_mask * weight
+            const int tap = (int)(e % k);
+            if (tap >= head && tap < head + mw && wd[e] != 0.0)
+                return fail("%sconv_mask leaves weight on tap %d, which kernel_size %d and mask_size %d mask in block "
+                            "%d (taps %d..%d): the checkpoint's mask is not the config's", mc.c_str(), tap, k,
+                            c.mask_size, i, head, head + mw - 1);
+        }
+        const std::vector<float> wl = npc_weight_layout(wd, H, k, mw, H);
+        S3B_OK(upload_split(L.out, wl.data(), wl.size(), m->scheme));
+        S3B_OK(upload_vec(m, mc + "conv.bias", H, L.out_b));
+    }
     return 0;
 }
 
@@ -945,6 +1051,7 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
     switch (m->kind) {
     case kGruStack: S3B_OK(finalize_apc(m)); break;
     case kLstmStack: S3B_OK(finalize_decoar(m)); break;
+    case kNpcStack: S3B_OK(finalize_npc(m)); break;
     case kConvEncoder:
     case kFbankEncoder: S3B_OK(finalize_encoder(m)); break;
     }
@@ -967,6 +1074,7 @@ extern "C" int32_t s3b_num_outputs(const s3b_model* m) {
     switch (m->kind) {
     case kGruStack: return m->cfg.num_layers;  // the output of every GRU layer (+ residual)
     case kLstmStack: return m->decoar_all_layers ? m->cfg.num_layers : 1;  // decoar_layers: every layer; decoar: the last
+    case kNpcStack: return 2 * m->cfg.num_layers + 1;  // every block, every masked conv, then feat
     default: return m->cfg.num_layers + 1 + m->cfg.pred_heads;
     }
 }
@@ -979,6 +1087,7 @@ extern "C" int s3b_valid_frames(const s3b_model* m, const int64_t* lens, int32_t
     const char* fbank_model = m->kind == kFbankEncoder ? "DeCoAR 2.0"
                               : m->kind == kGruStack   ? "APC"
                               : m->kind == kLstmStack  ? "DeCoAR"
+                              : m->kind == kNpcStack   ? "NPC"
                                                        : nullptr;
     bool any_pad = false;
     for (int b = 0; b < batch; ++b) {
@@ -1045,6 +1154,7 @@ struct Epi {
     const float* residual = nullptr;
     const uint8_t* row_mask = nullptr;
     int gelu = 0;
+    int res_first = 0;  // the activation after the residual add (gemm.cuh)
     float* out_f32 = nullptr;
     OutPlanes op = no_planes();  // GEMM-operand output (either format)
 };
@@ -1062,7 +1172,7 @@ static Epi epi_planes(const OutPlanes& op, const float* bias = nullptr, int gelu
 }
 
 static void set_epi(GemmParams& p, const Epi& e, int ldo) {
-    p.bias = e.bias, p.residual = e.residual, p.row_mask = e.row_mask, p.gelu = e.gelu;
+    p.bias = e.bias, p.residual = e.residual, p.row_mask = e.row_mask, p.gelu = e.gelu, p.res_first = e.res_first;
     p.out_f32 = e.out_f32, p.out_hi = e.op.hi, p.out_lo = e.op.lo, p.out_h8 = e.op.h8, p.out_l8 = e.op.l8;
     p.out_fmt = e.op.fmt, p.ldo = ldo;
     p.qkv_mode = 0;
@@ -1212,6 +1322,44 @@ static int conv_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int 
     p.out_rows_per_batch = (int)Lout;
     p.alg_flops = 2.0 * (double)B * Lout * C * K;
     set_epi(p, e, C);
+    return 0;
+}
+
+// NPC's same-padded convolutions over channels-last operand planes A [B][T][Cp] (Cp = 128 or 512): output row t of
+// utterance b takes taps j of a k-wide kernel from input row t + j - (k - 1) / 2, TMA zero-filling rows outside
+// [0, T) of its own utterance (padding = (k - 1) / 2). Only the u = k - mask taps outside the centred band of `mask`
+// taps are contracted: one k-block row per tap (Cp / 64 k-blocks), and the rows after the left run of (k - mask) / 2
+// taps skip the band (a_gap). W: [512][u * Cp], npc_weight_layout. alg_flops counts cin, the channels before padding.
+static int tapconv_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int B, int T, int Cp, int cin, int k,
+                          int mask, int scheme, const Epi& e) {
+    memset(&p, 0, sizeof(p));
+    const int N = 512, u = k - mask, K = u * Cp;
+    // 128-wide tiles, clustered like conv_params: f16q8 in fours (N = 512 is four tiles sharing each A box), bf16x3 alone
+    const int bn = 128;
+    const int cn = pick_cluster_n(bn, N / bn, scheme != 0 ? 4 : 1);
+    const uint32_t a_box = 128 / cn;
+    if (scheme != 0) {
+        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), Cp, T, B, Cp, (uint64_t)T * Cp, 64, a_box));
+        TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8(), Cp, T, B, Cp, (uint64_t)T * Cp, 64, a_box));
+        TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8(), Cp, T, B, Cp, (uint64_t)T * Cp, 64, a_box));
+        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, (uint64_t)N * K, 64, bn));
+        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, N, 1, K, (uint64_t)N * K, 64, bn));
+        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, N, 1, K, (uint64_t)N * K, 64, bn));
+        p.scheme = 1;
+    } else {
+        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), Cp, T, B, Cp, (uint64_t)T * Cp, 64, a_box));
+        TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l(), Cp, T, B, Cp, (uint64_t)T * Cp, 64, a_box));
+        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, (uint64_t)N * K, 64, bn));
+        TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, W.l(), K, N, 1, K, (uint64_t)N * K, 64, bn));
+    }
+    p.num_k_blocks = K / 64, p.kb_per_row = Cp / 64;
+    p.batches = B, p.rows_per_batch = T, p.tiles_m_per_batch = (T + 127) / 128;
+    p.n_tiles = N / bn, p.bn = bn, p.cluster_n = cn;
+    p.a_row_step = 1, p.a_row_off = -((k - 1) / 2), p.a_gap_at = (k - mask) / 2, p.a_gap = mask;
+    p.a_k_per_ntile = 0, p.b_n_tiled = 1, p.b_z_per_ntile = 0, p.b_k_linear = 1;
+    p.out_rows_per_batch = T;
+    p.alg_flops = 2.0 * (double)B * T * N * cin * u;
+    set_epi(p, e, N);
     return 0;
 }
 
@@ -1469,6 +1617,9 @@ int Fwd::prepare() {
     if (m->kind == kGruStack) {
         S3B_OK(w->x_s.ensure((size_t)M * D));  // layers 1..: the recurrence kernel's planes
         S3B_OK(w->xg_f32.ensure((size_t)M * 3 * D * 4));
+    } else if (m->kind == kNpcStack) {
+        S3B_OK(w->x_s.ensure((size_t)M * D));  // a block's output: the next block's and its masked conv's operand
+        S3B_OK(w->h_s.ensure((size_t)M * D));  // a block's conv output: its linear's operand
     } else if (m->kind == kLstmStack) {
         const int H = kLstmHidden;
         S3B_OK(w->x_s.ensure((size_t)M * H));      // layer 0's operand: post_extract_proj's output
@@ -1980,6 +2131,51 @@ static int add_lstm_stack(const Lane& lane, std::vector<Step>& steps) {
     return 0;
 }
 
+// NPC: per block i, the ConvBlock's conv (k = 3) into the linear's operand planes, the linear into hidden state 2i (fp32)
+// and the operand planes that block i + 1 and masked conv i read, then masked conv i: tanh(conv + b) is hidden state
+// 2i + 1 (out_pre), and that plus the running feat is feat, accumulated in place in the last output slot (the
+// epilogue reads each residual element before it writes the same element). No row mask anywhere: frames t >= m_b hold
+// the response to the zero features, as in the reference.
+static int add_npc_stack(const Lane& lane, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    Workspace* w = lane.w;
+    const s3b_npc_config& c = m->npc;
+    const int NB = c.n_blocks, B = lane.B, T = lane.T, sch = m->scheme, H = 512;
+    const int act = c.act == 0 ? 3 : 4;  // ReLU or tanh (gemm.cuh)
+    for (int i = 0; i < NB; ++i) {
+        const LayerW& L = m->layers[i];
+        const bool first = i == 0;
+        GemmParams conv, lin, mc;
+        S3B_OK(tapconv_params(conv, first ? w->ln512_s : w->x_s, L.fc1, B, T, first ? kDecoar2K : H, first ? 80 : H, 3,
+                              0, sch, epi_planes(w->h_s.planes(sch), L.fc1_b.as<float>(), act)));
+        Epi el = epi_f32(nullptr, L.fc2_b.as<float>());
+        el.op = w->x_s.planes(sch), el.gelu = act, el.res_first = 1;
+        S3B_OK(tapconv_params(lin, w->h_s, L.fc2, B, T, H, H, 1, 0, sch, el));
+        Epi em = epi_f32(nullptr, L.out_b.as<float>());
+        em.gelu = 4;
+        S3B_OK(tapconv_params(mc, w->x_s, L.out, B, T, H, H, c.kernel_size, npc_mask_width(c, i), sch, em));
+        const bool residual = c.residual && !first;
+        steps.push_back([=](Fwd& f) { return run_gemm(f, conv); });
+        steps.push_back([=](Fwd& f) {
+            GemmParams q = lin;
+            q.out_f32 = f.slot(2 * i);
+            q.residual = residual ? f.slot(2 * i - 2) : nullptr;
+            S3B_OK(run_gemm(f, q));
+            return f.done(2 * i);
+        });
+        steps.push_back([=](Fwd& f) {
+            GemmParams q = mc;
+            q.out_pre = f.slot(2 * i + 1);
+            q.out_f32 = f.slot(2 * NB);
+            q.residual = first ? nullptr : f.slot(2 * NB);
+            S3B_OK(run_gemm(f, q));
+            S3B_OK(f.done(2 * i + 1));
+            return i == NB - 1 ? f.done(2 * NB) : 0;
+        });
+    }
+    return 0;
+}
+
 // One lane's forward at the lane's shape, in enqueue order
 static int build_steps(const Lane& lane, std::vector<Step>& steps) {
     const s3b_model* m = lane.m;
@@ -1991,6 +2187,9 @@ static int build_steps(const Lane& lane, std::vector<Step>& steps) {
     case kLstmStack:
         S3B_OK(add_fbank_frontend(lane, steps));
         return add_lstm_stack(lane, steps);
+    case kNpcStack:
+        S3B_OK(add_fbank_frontend(lane, steps));
+        return add_npc_stack(lane, steps);
     case kFbankEncoder:
         S3B_OK(add_fbank_frontend(lane, steps));
         // six empty steps where the conv stack would be: with two lanes they keep lane 1's steps enqueued next to the
@@ -2116,6 +2315,7 @@ extern "C" int s3b_forward_ex(s3b_model* m, const float* const* wavs, const int6
         const char* why =
             m->kind == kGruStack    ? "an APC model is a GRU stack, it has no feed-forward blocks or layer results"
             : m->kind == kLstmStack ? "a DeCoAR model is an LSTM stack, it has no feed-forward blocks or layer results"
+            : m->kind == kNpcStack  ? "an NPC model is a conv stack, it has no feed-forward blocks or layer results"
             : m->cfg.conformer      ? "a Conformer encoder collects no layer results (wav2vec2_model.py:3199-3200)"
                                     : nullptr;
         if (why != nullptr) return fail("ffn_out / last_residual: %s", why);
@@ -2608,6 +2808,46 @@ extern "C" int s3b_posconv_f32(const float* x, const float* w, const float* bias
         if (gamma != nullptr) CUDA_OK(launch_layernorm(z.as<float>(), M, D, gamma, beta, 0, out_f32, op, st));
     }
     if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(op, M * D, out, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+extern "C" int s3b_npc_conv_f32(const float* x, int32_t B, int32_t T, int32_t c_in, const float* w, int32_t k,
+                                int32_t mask, const float* bias, const float* residual, int32_t act, int32_t res_first,
+                                int32_t scheme, float* out, float* out_pre, void* stream) {
+    if (!x || !w || !out) return fail("null argument");
+    if (B < 1 || T < 1) return fail("bad sizes (batch %d, t %d)", B, T);
+    if (c_in != 80 && c_in != 512) return fail("c_in must be 80 or 512, not %d", c_in);
+    if (k < 1 || k > 127 || k % 2 == 0) return fail("k %d: must be odd, 1..127", k);
+    if (mask < 0 || (mask > 0 && (mask % 2 == 0 || mask >= k))) return fail("mask %d: must be 0 or odd and < k %d", mask, k);
+    if (act < 0 || act > 2) return fail("act must be 0 (none), 1 (ReLU) or 2 (tanh), not %d", act);
+    if (res_first != 0 && res_first != 1) return fail("res_first must be 0 or 1, not %d", res_first);
+    if (res_first && out_pre != nullptr) return fail("out_pre is the value before the residual add: not with res_first");
+    const int N = 512, Cp = c_in == 80 ? kDecoar2K : 512, u = k - mask;
+    const size_t M = (size_t)B * T;
+    int sch = 0;
+    S3B_OK(resolve_scheme(scheme, u * Cp, N, &sch));
+    cudaStream_t st = (cudaStream_t)stream;
+    int sms = 0;
+    S3B_OK(device_sm_count(&sms));
+    std::vector<float> wh;
+    S3B_OK(download_f32(w, (size_t)N * c_in * k, st, wh));
+    const std::vector<float> wl = npc_weight_layout(std::vector<double>(wh.begin(), wh.end()), c_in, k, mask, Cp);
+    SplitBuf xs, ws;
+    S3B_OK(upload_split(ws, wl.data(), wl.size(), sch));
+    DevBuf xpad;
+    if (Cp != c_in) {  // 80 channels zero-padded to 128 per row, as the CMVN kernel writes them
+        S3B_OK(xpad.ensure(M * Cp * 4));
+        CUDA_OK(cudaMemcpy2DAsync(xpad.p, (size_t)Cp * 4, x, (size_t)c_in * 4, (size_t)c_in * 4, M,
+                                  cudaMemcpyDeviceToDevice, st));
+    }
+    S3B_OK(split_operand(Cp != c_in ? xpad.as<float>() : x, xs, M * Cp, sch, 0, st));
+    Epi e = epi_f32(out, bias, residual);
+    e.gelu = act == 0 ? 0 : act == 1 ? 3 : 4, e.res_first = res_first;
+    GemmParams p;
+    S3B_OK(tapconv_params(p, xs, ws, B, T, Cp, c_in, k, mask, sch, e));
+    p.out_pre = out_pre;
+    CUDA_OK(launch_gemm(p, sms, st));
     CUDA_OK(cudaStreamSynchronize(st));
     return 0;
 }

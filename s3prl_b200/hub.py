@@ -20,6 +20,7 @@ from .upstream.configs import ALIASES, ARCHS
 from .upstream.decoar import DecoarExpert
 from .upstream.decoar2 import Decoar2Expert
 from .upstream.expert import UpstreamExpert
+from .upstream.npc import NpcExpert
 
 
 def _entry(name: str, make: Callable, ckpt_required: bool = False, refuse_legacy: bool = False,
@@ -73,6 +74,10 @@ for _name, _vq, _required in (("apc", False, False), ("apc_360hr", False, False)
 for _family, _all in (("decoar", False), ("decoar_layers", True)):
     for _name in (_family, f"{_family}_local", f"{_family}_url", f"{_family}_custom"):
         ENTRIES[_name] = _entry(_name, partial(DecoarExpert, all_layers=_all, name=_name), ckpt_required=_name != _family)
+# NPC (npc/hubconf.py): the fabricated checkpoint without ckpt, else the local {"config", "model"} file
+for _name, _required in (("npc", False), ("npc_360hr", False), ("npc_960hr", False), ("npc_local", True),
+                         ("npc_url", True)):
+    ENTRIES[_name] = _entry(_name, partial(NpcExpert, name=_name), ckpt_required=_required)
 globals().update(ENTRIES)
 
 

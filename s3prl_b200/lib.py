@@ -25,6 +25,7 @@ EXPORTED_SYMBOLS = [
     "s3b_model_destroy",
     "s3b_apc_model_create",
     "s3b_decoar_model_create",
+    "s3b_npc_model_create",
     "s3b_num_frames",
     "s3b_valid_frames",
     "s3b_num_outputs",
@@ -65,6 +66,7 @@ EXPORTED_SYMBOLS = [
     "s3b_gru_max_active_clusters",
     "s3b_lstm_f32",
     "s3b_lstm_fits",
+    "s3b_npc_conv_f32",
     "s3b_layernorm_rope_f32",
     "s3b_fbank",
     "s3b_fbank_ex",
@@ -138,6 +140,26 @@ class S3BDecoarConfig(C.Structure):
     def __init__(self, **kw):
         super().__init__(**kw)
         self.struct_size = C.sizeof(S3BDecoarConfig)
+
+
+class S3BNpcConfig(C.Structure):
+    """Mirror of ``struct s3b_npc_config`` (act: 0 = relu, 1 = tanh)."""
+
+    _fields_ = [
+        ("struct_size", C.c_int32),
+        ("n_blocks", C.c_int32),
+        ("hidden", C.c_int32),
+        ("kernel_size", C.c_int32),
+        ("mask_size", C.c_int32),
+        ("residual", C.c_int32),
+        ("batch_norm", C.c_int32),
+        ("act", C.c_int32),
+        ("reserved", C.c_int32 * 4),
+    ]
+
+    def __init__(self, **kw):
+        super().__init__(**kw)
+        self.struct_size = C.sizeof(S3BNpcConfig)
 
 
 class S3BForwardOpts(C.Structure):
@@ -246,6 +268,7 @@ def load() -> C.CDLL:
     lib.s3b_model_set_tensor.argtypes = [vp, C.c_char_p, vp, C.POINTER(i64), i32]
     lib.s3b_apc_model_create.argtypes = [C.POINTER(S3BApcConfig), C.POINTER(vp)]
     lib.s3b_decoar_model_create.argtypes = [C.POINTER(S3BDecoarConfig), C.POINTER(vp)]
+    lib.s3b_npc_model_create.argtypes = [C.POINTER(S3BNpcConfig), C.POINTER(vp)]
     lib.s3b_model_finalize.argtypes = [vp]
     lib.s3b_model_destroy.argtypes = [vp]
     lib.s3b_model_destroy.restype = None
@@ -296,6 +319,7 @@ def load() -> C.CDLL:
     lib.s3b_gru_max_active_clusters.argtypes = [C.POINTER(i32)]
     lib.s3b_gru_f32.argtypes = [f32p, f32p, f32p, f32p, C.POINTER(i32), i32, i32, i32, i32, f32p, f32p, vp]
     lib.s3b_lstm_fits.argtypes = [C.POINTER(i32)]
+    lib.s3b_npc_conv_f32.argtypes = [f32p, i32, i32, i32, f32p, i32, i32, f32p, f32p, i32, i32, i32, f32p, f32p, vp]
     lib.s3b_lstm_f32.argtypes = [f32p, f32p, f32p, C.POINTER(i32), i32, i32, i32, i32, f32p, f32p, vp]
     lib.s3b_layernorm_rope_f32.argtypes = [f32p, i64, i32, i32, f32p, f32p, C.POINTER(C.c_float), i32, f32p, f32p, vp]
     lib.s3b_fbank_num_frames.argtypes = [i64]

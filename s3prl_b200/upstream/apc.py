@@ -87,12 +87,11 @@ def required_keys() -> List[str]:
             for n in ("weight_ih_l0", "weight_hh_l0", "bias_ih_l0", "bias_hh_l0")]
 
 
-def validate_config(config: dict, where: str = "config") -> bool:
-    """Checks that a checkpoint's config is of the served shape; returns ``residual``. Anything else raises
-    ``ValueError`` naming the field."""
+def validate_audio(config: dict, where: str = "config") -> None:
+    """Checks that a checkpoint's ``data.audio`` is the served front end (shared by APC and NPC, whose audio.py is
+    APC's); anything else raises ``ValueError`` naming the field."""
     try:
         audio = dict(config["data"]["audio"])
-        paras = dict(config["model"]["paras"])
     except (KeyError, TypeError) as e:
         raise ValueError(f"{where}: expected config['data']['audio'] and config['model']['paras'] ({e!r} missing)")
     if audio.pop("feat_type", None) != "fbank":
@@ -108,6 +107,17 @@ def validate_config(config: dict, where: str = "config") -> bool:
     if audio:
         raise ValueError(f"{where}: data.audio.{sorted(audio)[0]} is not served (fbank kwargs other than "
                          "frame_length / frame_shift at their defaults)")
+
+
+def validate_config(config: dict, where: str = "config") -> bool:
+    """Checks that a checkpoint's config is of the served shape; returns ``residual``. Anything else raises
+    ``ValueError`` naming the field."""
+    try:
+        config["data"]["audio"]
+        paras = dict(config["model"]["paras"])
+    except (KeyError, TypeError) as e:
+        raise ValueError(f"{where}: expected config['data']['audio'] and config['model']['paras'] ({e!r} missing)")
+    validate_audio(config, where)
     if paras.pop("hidden_size", None) != HIDDEN:
         raise ValueError(f"{where}: model.paras.hidden_size must be {HIDDEN}")
     if paras.pop("num_layers", None) != NUM_LAYERS:
