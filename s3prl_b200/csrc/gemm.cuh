@@ -13,7 +13,7 @@ namespace s3b {
 struct GemmParams {
     // A operand (activations): bf16 hi / lo, 3-D tensor maps (k, row, batch), box {64, 128 / cluster_n, 1}, SWIZZLE_128B
     CUtensorMap a_hi, a_lo;
-    // B operand (weights, [N][K] K-major): bf16 hi / lo, 3-D tensor maps (k, n, z), box {64, bn, 1}
+    // B operand (weights, one [N][K] K-major matrix): bf16 hi / lo, tensor maps (k, n, 1), box {64, bn, 1}
     CUtensorMap b_hi, b_lo;
 
     // scheme 1 ("f16q8", bn 128 or 256 only): fp16 main product + two e4m3 correction products.
@@ -37,15 +37,11 @@ struct GemmParams {
     // k-block kb reads   A box at (a_k_per_ntile*n_tile + (kb % kb_per_row)*64,
     //                              row0 + kq*a_row_step + a_row_off + (kq >= a_gap_at ? a_gap : 0), batch)
     //                    with kq = kb / kb_per_row
-    //                    B box at (b_k_linear ? kb*64 : (kb % kb_per_row)*64, b_n_tiled ? n_tile*bn : 0,
-    //                              b_k_linear ? 0 : kb / kb_per_row + n_tile*b_z_per_ntile)
+    //                    B box at (kb*64, n_tile*bn, 0)
     int kb_per_row;
     int a_row_step;
     int a_row_off;
     int a_k_per_ntile;
-    int b_n_tiled;
-    int b_k_linear;
-    int b_z_per_ntile;
     // a tap convolution that skips a band of taps (the NPC masked conv): k-block rows kq >= a_gap_at read a_gap rows
     // further on. a_gap 0 is the plain walk.
     int a_gap_at;

@@ -106,8 +106,7 @@ __device__ __forceinline__ void produce(const GemmParams& p, uint8_t* smem, uint
         const TileCoord tc = tile_coord<CN>(p, ct, rank);
         const int n_tile = tc.n_tile, batch = tc.batch, row0 = tc.row0;
         const int a_k0 = p.a_k_per_ntile * n_tile;
-        const int b_n0 = p.b_n_tiled ? n_tile * BN : 0;
-        const int b_z0 = n_tile * p.b_z_per_ntile;
+        const int b_n0 = n_tile * BN;
         for (int pass = 0; pass < kPasses; ++pass) {
             for (int kb = 0; kb < p.num_k_blocks; ++kb) {
                 const int kq = kb / p.kb_per_row;
@@ -118,12 +117,11 @@ __device__ __forceinline__ void produce(const GemmParams& p, uint8_t* smem, uint
                 mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)Cfg::kStageBytes);
                 const int a_row = row0 + kq * p.a_row_step + p.a_row_off + (kq >= p.a_gap_at ? p.a_gap : 0);
                 const int a_k = a_k0 + kr * kBlockK;
-                const int b_k = (p.b_k_linear ? kb : kr) * kBlockK;
-                const int b_z = p.b_k_linear ? 0 : b_z0 + kq;
+                const int b_k = kb * kBlockK;
                 if (kScheme == 1 && pass == 1) {
                     // [A16 | W16]: one fp16 box of 128-byte rows each, spanning both planes of the stage
                     load_a<CN, 128>(st, &p.a_hi, &full_bar[stage], a_k, a_row, batch, rank);
-                    tma_load_3d(sb, &p.b_hi, &full_bar[stage], b_k, b_n0, b_z);
+                    tma_load_3d(sb, &p.b_hi, &full_bar[stage], b_k, b_n0, 0);
                 } else {
                     // planes: scheme 0 [A_hi A_lo W_hi W_lo]; scheme 1 pass 0 [A_l8 A_h8 W_h8 W_l8] (64-byte rows)
                     const CUtensorMap* ma0 = kScheme == 0 ? &p.a_hi : &p.a_l8;
@@ -132,8 +130,8 @@ __device__ __forceinline__ void produce(const GemmParams& p, uint8_t* smem, uint
                     const CUtensorMap* mb1 = kScheme == 0 ? &p.b_lo : &p.b_l8;
                     load_a<CN, Cfg::RB>(st, ma0, &full_bar[stage], a_k, a_row, batch, rank);
                     load_a<CN, Cfg::RB>(st + Cfg::kAPlane, ma1, &full_bar[stage], a_k, a_row, batch, rank);
-                    tma_load_3d(sb, mb0, &full_bar[stage], b_k, b_n0, b_z);
-                    tma_load_3d(sb + Cfg::kBPlane, mb1, &full_bar[stage], b_k, b_n0, b_z);
+                    tma_load_3d(sb, mb0, &full_bar[stage], b_k, b_n0, 0);
+                    tma_load_3d(sb + Cfg::kBPlane, mb1, &full_bar[stage], b_k, b_n0, 0);
                 }
                 if (++stage == Cfg::kStages) stage = 0, phase ^= 1u;
             }

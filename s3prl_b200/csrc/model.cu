@@ -187,15 +187,16 @@ struct LayerW {
     // ln1 = self_attn_layer_norm, ln2 = final_layer_norm; dw_w / dw_b the depthwise taps with BatchNorm folded in
     SplitBuf v, ffn1_w1, ffn1_w2, pw1, pw2;
     DevBuf ffn1_b1, ffn1_b2, ffn1_ln_g, ffn1_ln_b, ffn2_ln_g, ffn2_ln_b, conv_ln_g, conv_ln_b, dw_w, dw_b;
-    // APC GRU layer: wih = weight_ih_l0 [3H][K] (layer 0: K = 80 zero-padded to kDecoar2K), gru_b = bias_ih_l0 with
-    // bias_hh_l0's r and z thirds added (the input GEMM's bias), whh = weight_hh_l0 [3H][H] fp32, bhn = bias_hh_l0[2H:]
+    // APC GRU layer: wih = weight_ih_l0 [3H][K] (tap_weight_layout, k = 1; layer 0: K = 80 zero-padded to kDecoar2K),
+    // gru_b = bias_ih_l0 with bias_hh_l0's r and z thirds added (the input GEMM's bias), whh = weight_hh_l0 [3H][H]
+    // fp32, bhn = bias_hh_l0[2H:]
     // DeCoAR LSTM layer k, direction d (layers[2k + d]): wih = weight_ih_lk [4H][H], gru_b = bias_ih_lk + bias_hh_lk,
     // whh = weight_hh_lk [4H][H] fp32
     SplitBuf wih;
     DevBuf gru_b, whh, bhn;
-    // NPC block i (finalize_npc): fc1 = blocks.i.conv with bn1 folded in ([512][3 * Cp], tap-major, Cp = 128 for block
-    // 0's 80 channels, 512 after), fc2 = blocks.i.linear with bn2 folded in ([512][512]), out = masked_convs.i's
-    // unmasked taps ([512][u * 512]); fc1_b, fc2_b, out_b their biases
+    // NPC block i (finalize_npc), each weight in tap_weight_layout: fc1 = blocks.i.conv with bn1 folded in
+    // ([512][3 * Cp], Cp = 128 for block 0's 80 channels, 512 after), fc2 = blocks.i.linear with bn2 folded in
+    // ([512][512]), out = masked_convs.i's unmasked taps ([512][u * 512]); fc1_b, fc2_b, out_b their biases
 };
 
 // per-category device-time profile (CUDA events around each launch on the launching stream)
@@ -690,41 +691,36 @@ static int finalize_conformer_layer(s3b_model* m, int l) {
 }
 
 // ---- weight relayouts shared by s3b_model_finalize and the building-block entry points ----------------------------
-// conv 1..6: [out][in][tap] -> [out][tap*512 + in] (K index of the channels-last im2col row)
-static std::vector<float> conv_weight_layout(const float* w, int kw) {
-    const int C = kConvDim;
-    std::vector<float> r((size_t)C * C * kw);
-    for (int o = 0; o < C; ++o)
-        for (int ci = 0; ci < C; ++ci)
-            for (int j = 0; j < kw; ++j) r[((size_t)o * kw + j) * C + ci] = w[((size_t)o * C + ci) * kw + j];
+// Every GEMM reads its weight as one [N][K] K-major matrix. A convolution weight w [N][cin][k] becomes
+// [N][(k - mask) * Cp]: the taps outside the centred band of `mask` taps, in tap order, each zero-padded from cin to
+// Cp channels, so that the K index tap * Cp + channel is the channels-last im2col row the convolution builders walk.
+// k = 1 pads a linear's [N][cin] to [N][Cp]. T = double (NPC's BatchNorm folding) rounds each element to fp32 once.
+template <class T>
+static std::vector<float> tap_weight_layout(const T* w, int N, int cin, int k, int mask, int Cp) {
+    const int u = k - mask, head = u / 2;
+    std::vector<float> r((size_t)N * u * Cp, 0.f);
+    for (int o = 0; o < N; ++o)
+        for (int q = 0; q < u; ++q) {
+            const int tap = q < head ? q : q + mask;
+            for (int c = 0; c < cin; ++c) r[((size_t)o * u + q) * Cp + c] = (float)w[((size_t)o * cin + c) * k + tap];
+        }
     return r;
 }
-// grouped positional conv, folded weight w [D][cpg][Kp]. One tap per k-block, or per two k-blocks above 64 channels
-// per group (posconv_params): B operand [group*Kp + tap][n = cpg][Kc = cpg rounded up to 64 (zero padded)]
+// grouped positional conv, one tap per k-block (posconv_params): tap_weight_layout with each group's cpg channels
+// zero-padded to Cp = posconv_kc(cpg), whole 64-wide k-blocks
 static int posconv_kc(int cpg) { return (cpg + 63) / 64 * 64; }
-static std::vector<float> posconv_weight_layout(const float* w, int D, int G, int Kp) {
-    const int cpg = D / G, Kc = posconv_kc(cpg);
-    std::vector<float> wb((size_t)G * Kp * cpg * Kc, 0.0f);
+// grouped positional conv, four taps per k-block (tap = 4q + j, posconv4_params), folded weight w [D][cpg][Kp], the
+// tap count rounded up to K4 = a multiple of four with zero taps: [G * 4cpg][K4 / 4 * 64], row g * 4cpg + j * cpg + n,
+// column q * 64 + channel (zero padded to 64); cpg <= 64 (48 or 64 where it runs)
+static std::vector<float> posconv4_weight_layout(const float* w, int D, int G, int Kp) {
+    const int cpg = D / G, Kq = (Kp + 3) / 4;
+    std::vector<float> w4((size_t)D * 4 * Kq * 64, 0.0f);
     for (int g = 0; g < G; ++g)
         for (int k = 0; k < Kp; ++k)
             for (int n = 0; n < cpg; ++n)
                 for (int ci = 0; ci < cpg; ++ci)
-                    wb[(((size_t)g * Kp + k) * cpg + n) * Kc + ci] = w[((size_t)(g * cpg + n) * cpg + ci) * Kp + k];
-    return wb;
-}
-// four taps per k-block (tap = 4q + j, posconv4_params), the tap count rounded up to K4 = a multiple of four with zero
-// taps: B operand [group*K4/4 + q][n = j*cpg + co][64 (zero padded)]; cpg <= 64 (48 or 64 where it runs)
-static std::vector<float> posconv4_weight_layout(const float* w, int D, int G, int Kp) {
-    const int cpg = D / G, K4 = (Kp + 3) / 4 * 4;
-    std::vector<float> w4((size_t)G * K4 * cpg * 64, 0.0f);
-    for (int g = 0; g < G; ++g)
-        for (int k = 0; k < Kp; ++k)
-            for (int n = 0; n < cpg; ++n)
-                for (int ci = 0; ci < cpg; ++ci) {
-                    const int q = k / 4, j = k % 4;
-                    w4[((((size_t)g * (K4 / 4) + q) * 4 + j) * cpg + n) * 64 + ci] =
+                    w4[((size_t)(g * 4 + k % 4) * cpg + n) * Kq * 64 + (k / 4) * 64 + ci] =
                         w[((size_t)(g * cpg + n) * cpg + ci) * Kp + k];
-                }
     return w4;
 }
 
@@ -742,8 +738,7 @@ static int finalize_apc(s3b_model* m) {
         S3B_OK(need(m, p + "weight_hh_l0", {3 * H, H}, &whh));
         S3B_OK(need(m, p + "bias_ih_l0", {3 * H}, &bih));
         S3B_OK(need(m, p + "bias_hh_l0", {3 * H}, &bhh));
-        std::vector<float> w((size_t)3 * H * K, 0.f);
-        for (int o = 0; o < 3 * H; ++o) memcpy(&w[(size_t)o * K], &wih->data[(size_t)o * in], in * sizeof(float));
+        const std::vector<float> w = tap_weight_layout(wih->data.data(), 3 * H, in, 1, 0, K);
         S3B_OK(upload_split(L.wih, w.data(), w.size(), m->scheme));
         // b_hr, b_hz sit outside r * (.) and fold into the GEMM's bias; b_hn does not
         std::vector<float> b(bih->data);
@@ -758,19 +753,6 @@ static int finalize_apc(s3b_model* m) {
         return fail("the GRU recurrence kernel cannot run on this device: cudaOccupancyMaxActiveClusters reports 0 "
                     "clusters of %d CTAs with %zu bytes of shared memory each", kGruCtas, gru_smem_bytes());
     return 0;
-}
-
-// NPC tap conv weight w [512][cin][k] (fp64) -> the GEMM's B operand [512][u * Cp]: the u = k - mask taps outside the
-// centred band of `mask` taps, in tap order, each zero-padded from cin to Cp channels (tapconv_params)
-static std::vector<float> npc_weight_layout(const std::vector<double>& w, int cin, int k, int mask, int Cp) {
-    const int N = 512, u = k - mask, head = (k - mask) / 2;
-    std::vector<float> r((size_t)N * u * Cp, 0.f);
-    for (int o = 0; o < N; ++o)
-        for (int q = 0; q < u; ++q) {
-            const int tap = q < head ? q : q + mask;
-            for (int c = 0; c < cin; ++c) r[((size_t)o * u + q) * Cp + c] = (float)w[((size_t)o * cin + c) * k + tap];
-        }
-    return r;
 }
 
 // NPC (npc.py): per block i, ConvBlock conv [512][cin][3] -> bn1 -> act -> linear [512][512][1] -> bn2 (+ input) -> act,
@@ -804,7 +786,7 @@ static int finalize_npc(s3b_model* m) {
                     bd[o] = (bd[o] - (double)mu->data[o]) * sc + (double)be->data[o];
                 }
             }
-            const std::vector<float> wl = npc_weight_layout(wd, kin, kw, 0, j == 0 ? Cp : H);
+            const std::vector<float> wl = tap_weight_layout(wd.data(), H, kin, kw, 0, j == 0 ? Cp : H);
             const std::vector<float> bl(bd.begin(), bd.end());
             S3B_OK(upload_split(j == 0 ? L.fc1 : L.fc2, wl.data(), wl.size(), m->scheme));
             S3B_OK(upload_f32(j == 0 ? L.fc1_b : L.fc2_b, bl.data(), bl.size()));
@@ -823,7 +805,7 @@ static int finalize_npc(s3b_model* m) {
                             "%d (taps %d..%d): the checkpoint's mask is not the config's", mc.c_str(), tap, k,
                             c.mask_size, i, head, head + mw - 1);
         }
-        const std::vector<float> wl = npc_weight_layout(wd, H, k, mw, H);
+        const std::vector<float> wl = tap_weight_layout(wd.data(), H, H, k, mw, H);
         S3B_OK(upload_split(L.out, wl.data(), wl.size(), m->scheme));
         S3B_OK(upload_vec(m, mc + "conv.bias", H, L.out_b));
     }
@@ -835,8 +817,7 @@ static int finalize_npc(s3b_model* m) {
 static int upload_fbank_proj(s3b_model* m, int N) {
     const HostTensor* t;
     S3B_OK(need(m, "post_extract_proj.weight", {N, 80}, &t));
-    std::vector<float> wp((size_t)N * kDecoar2K, 0.f);
-    for (int o = 0; o < N; ++o) memcpy(&wp[(size_t)o * kDecoar2K], &t->data[(size_t)o * 80], 80 * sizeof(float));
+    const std::vector<float> wp = tap_weight_layout(t->data.data(), N, 80, 1, 0, kDecoar2K);
     S3B_OK(upload_split(m->proj_w, wp.data(), wp.size(), m->scheme));
     return upload_vec(m, "post_extract_proj.bias", N, m->proj_b);
 }
@@ -897,12 +878,12 @@ static int finalize_encoder(s3b_model* m) {
             S3B_OK(upload_vec(m, fe + "0.2.weight", C, m->norm0_g));
             S3B_OK(upload_vec(m, fe + "0.2.bias", C, m->norm0_b));
         }
-        // ---- conv 1..6: [out][in][tap] -> [out][tap*512 + in] (K index of the channels-last im2col row) ----
+        // ---- conv 1..6 ---------------------------------------------------------------------------------------
         for (int i = 1; i < kNumConv; ++i) {
             const std::string p = fe + std::to_string(i);
             const int kw = kConvK[i];
             S3B_OK(need(m, p + ".0.weight", {C, C, kw}, &t));
-            const std::vector<float> r = conv_weight_layout(t->data.data(), kw);
+            const std::vector<float> r = tap_weight_layout(t->data.data(), C, C, kw, 0, C);
             S3B_OK(upload_split(m->conv_w[i], r.data(), r.size(), m->scheme));
             if (c.conv_bias) S3B_OK(upload_vec(m, p + ".0.bias", C, m->conv_b[i]));
             if (c.extractor_layer_norm) {
@@ -957,7 +938,7 @@ static int finalize_encoder(s3b_model* m) {
             const std::vector<float> w4 = posconv4_weight_layout(wf.data(), D, G, Kp);
             S3B_OK(upload_split(m->pos_w4, w4.data(), w4.size()));
         } else {
-            const std::vector<float> wb = posconv_weight_layout(wf.data(), D, G, Kp);
+            const std::vector<float> wb = tap_weight_layout(wf.data(), D, cpg, Kp, 0, posconv_kc(cpg));
             S3B_OK(upload_split(m->pos_w, wb.data(), wb.size()));
         }
         S3B_OK(upload_vec(m, "encoder.pos_conv.0.bias", D, m->pos_b));
@@ -1246,6 +1227,28 @@ static int pick_cluster_n(int bn, int n_tiles, int preferred) {
         if (_r != 0) return fail("cuTensorMapEncodeTiled failed (%d) at %s:%d", _r, __FILE__, __LINE__); \
     } while (0)
 
+// The A and B tensor maps of one launch in its operand scheme, the one place they are encoded. A: the (k, row, batch)
+// view of [batches][rows][ka] from element a_off of A's planes, rows lda and batches bstride elements apart, boxes
+// {64, a_box}. W: the [N][K] K-major weight, boxes {64, bn}.
+static int gemm_tmaps(GemmParams& p, int scheme, const SplitBuf& A, size_t a_off, uint64_t ka, uint64_t rows,
+                      uint64_t batches, uint64_t lda, uint64_t bstride, uint32_t a_box, const SplitBuf& W, int N, int K,
+                      int bn) {
+    const uint64_t wn = (uint64_t)N * K;
+    TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h() + a_off, ka, rows, batches, lda, bstride, 64, a_box));
+    TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, wn, 64, bn));
+    if (scheme != 0) {
+        TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8() + a_off, ka, rows, batches, lda, bstride, 64, a_box));
+        TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8() + a_off, ka, rows, batches, lda, bstride, 64, a_box));
+        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, N, 1, K, wn, 64, bn));
+        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, N, 1, K, wn, 64, bn));
+    } else {
+        TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l() + a_off, ka, rows, batches, lda, bstride, 64, a_box));
+        TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, W.l(), K, N, 1, K, wn, 64, bn));
+    }
+    p.scheme = scheme;
+    return 0;
+}
+
 // out[M][N] = A[M][K] * W[N][K]^T with epilogue `e`, flat token-major A (hi/lo planes), K % 64 == 0
 // scheme 1: A and W are f16q8 operands (SplitBuf fmt 1), K % 128 == 0, tile width 128 or 256.
 // sm_count: SMs of the device the GEMM runs on (pick_bn's tile-width rule).
@@ -1258,107 +1261,46 @@ static int linear_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, in
     if (K % 64 != 0 || N % 16 != 0) return fail("linear: K %% 64 or N %% 16 violated (N=%d K=%d)", N, K);
     const int bn = pick_bn(M, N, K, scheme, sm_count, forced_bn);
     const int cn = pick_cluster_n(bn, N / bn, scheme != 0 ? 2 : 1);
-    const uint32_t a_box = 128 / cn;
-    if (scheme != 0) {
-        if ((bn != 128 && bn != 256) || K % 128 != 0)
-            return fail("f16q8 GEMM needs a tile width of 128 or 256 and K %% 128 == 0 (N=%d K=%d)", N, K);
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, a_box));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, a_box));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, a_box));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, (uint64_t)N * K, 64, bn));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, N, 1, K, (uint64_t)N * K, 64, bn));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, N, 1, K, (uint64_t)N * K, 64, bn));
-        p.scheme = 1;
-    } else {
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, a_box));
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l() + a_off, K, M, 1, lda, (uint64_t)M * lda, 64, a_box));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, (uint64_t)N * K, 64, bn));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, W.l(), K, N, 1, K, (uint64_t)N * K, 64, bn));
-    }
+    if (scheme != 0 && ((bn != 128 && bn != 256) || K % 128 != 0))
+        return fail("f16q8 GEMM needs a tile width of 128 or 256 and K %% 128 == 0 (N=%d K=%d)", N, K);
+    S3B_OK(gemm_tmaps(p, scheme, A, a_off, K, M, 1, lda, (uint64_t)M * lda, 128 / cn, W, N, K, bn));
     p.num_k_blocks = K / 64, p.kb_per_row = K / 64;
     p.batches = 1, p.rows_per_batch = (int)M, p.tiles_m_per_batch = (int)((M + 127) / 128);
     p.n_tiles = N / bn, p.bn = bn, p.cluster_n = cn;
-    p.a_row_step = 0, p.a_row_off = 0, p.a_k_per_ntile = 0, p.b_n_tiled = 1, p.b_z_per_ntile = 0;
     p.out_rows_per_batch = (int)M;
     p.alg_flops = 2.0 * (double)M * N * K;
     set_epi(p, e, N);
     return 0;
 }
 
-// conv i (k in {2,3}, stride 2) over channels-last [B][Lin][512] with epilogue `e`: row t of the [ceil(Lin/2)][1024]
-// view holds samples (2t, 2t+1); taps 0,1 come from view row t, tap 2 from the first half of view row t+1.
-static int conv_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int B, int64_t Lin, int64_t Lout, int kw,
-                       int scheme, const Epi& e) {
+// Convolution of k taps into 512 channels over channels-last operand planes A [B][Lin][Cp], with epilogue `e`, as one
+// implicit GEMM over W [512][u * Cp] (tap_weight_layout; u = k - mask taps). Output row t of utterance b takes tap j
+// from input row stride * t + j - pad of its own utterance, TMA zero-filling rows outside [0, Lin).
+//  - stride 1 (NPC): same padding, pad = (k - 1) / 2 and Lout = Lin. Only the taps outside the centred band of `mask`
+//    taps are contracted: one k-block row per tap (Cp / 64 k-blocks), and the rows after the left run of u / 2 taps
+//    skip the band (a_gap).
+//  - stride 2 (conv 1..6, k in {2, 3}, mask 0): no padding. Row t of the [ceil(Lin / 2)][2 Cp] view holds input rows
+//    (2t, 2t + 1): taps 0, 1 come from view row t, tap 2 from the first half of view row t + 1.
+// alg_flops counts cin, the channels before padding.
+static int conv_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int B, int64_t Lin, int64_t Lout,
+                       int stride, int cin, int Cp, int k, int mask, int scheme, const Epi& e) {
     memset(&p, 0, sizeof(p));
-    const int C = kConvDim, K = kw * C;
-    const uint64_t rows = (uint64_t)((Lin + 1) / 2);
+    const int N = kConvDim, u = k - mask, K = u * Cp, width = stride * Cp;
     // Tile: tools/gemm_shapes.py times the linear with conv i's M, N = 512 and K as a proxy (H100 80GB HBM3, 700 W,
     // hubert_base's conv stack at 32 x 10 s). f16q8 on 128-wide tiles in clusters of 4 (N = 512 is four tiles, which
     // then share each A tile) runs conv 1..6 in 6.96 ms, against 7.57 in clusters of 2, 7.97 on 256-wide tiles
     // (10-13% slower at every conv) and 9.49 on unclustered 128-wide tiles. bf16x3 stays on unclustered 128-wide
     // tiles: clusters of 2 and 4 are 2% and 10% slower there, and 256-wide tiles 70%.
     const int bn = 128;
-    const int cn = pick_cluster_n(bn, C / bn, scheme != 0 ? 4 : 1);
-    const uint32_t a_box = 128 / cn;
-    // weights [512][K], K index = tap*512 + channel, read linearly along K
-    if (scheme != 0) {
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, a_box));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, a_box));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, a_box));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, C, 1, K, (uint64_t)C * K, 64, bn));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, C, 1, K, (uint64_t)C * K, 64, bn));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, C, 1, K, (uint64_t)C * K, 64, bn));
-        p.scheme = 1;
-    } else {
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, a_box));
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l(), 2 * C, rows, B, 2 * C, (uint64_t)Lin * C, 64, a_box));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, C, 1, K, (uint64_t)C * K, 64, bn));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, W.l(), K, C, 1, K, (uint64_t)C * K, 64, bn));
-    }
-    p.num_k_blocks = K / 64, p.kb_per_row = (2 * C) / 64;
-    p.batches = B, p.rows_per_batch = (int)Lout, p.tiles_m_per_batch = (int)((Lout + 127) / 128);
-    p.n_tiles = C / bn, p.bn = bn, p.cluster_n = cn;
-    p.a_row_step = 1, p.a_row_off = 0, p.a_k_per_ntile = 0, p.b_n_tiled = 1, p.b_z_per_ntile = 0, p.b_k_linear = 1;
-    p.out_rows_per_batch = (int)Lout;
-    p.alg_flops = 2.0 * (double)B * Lout * C * K;
-    set_epi(p, e, C);
-    return 0;
-}
-
-// NPC's same-padded convolutions over channels-last operand planes A [B][T][Cp] (Cp = 128 or 512): output row t of
-// utterance b takes taps j of a k-wide kernel from input row t + j - (k - 1) / 2, TMA zero-filling rows outside
-// [0, T) of its own utterance (padding = (k - 1) / 2). Only the u = k - mask taps outside the centred band of `mask`
-// taps are contracted: one k-block row per tap (Cp / 64 k-blocks), and the rows after the left run of (k - mask) / 2
-// taps skip the band (a_gap). W: [512][u * Cp], npc_weight_layout. alg_flops counts cin, the channels before padding.
-static int tapconv_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int B, int T, int Cp, int cin, int k,
-                          int mask, int scheme, const Epi& e) {
-    memset(&p, 0, sizeof(p));
-    const int N = 512, u = k - mask, K = u * Cp;
-    // 128-wide tiles, clustered like conv_params: f16q8 in fours (N = 512 is four tiles sharing each A box), bf16x3 alone
-    const int bn = 128;
     const int cn = pick_cluster_n(bn, N / bn, scheme != 0 ? 4 : 1);
-    const uint32_t a_box = 128 / cn;
-    if (scheme != 0) {
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), Cp, T, B, Cp, (uint64_t)T * Cp, 64, a_box));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8(), Cp, T, B, Cp, (uint64_t)T * Cp, 64, a_box));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8(), Cp, T, B, Cp, (uint64_t)T * Cp, 64, a_box));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, (uint64_t)N * K, 64, bn));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, N, 1, K, (uint64_t)N * K, 64, bn));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, N, 1, K, (uint64_t)N * K, 64, bn));
-        p.scheme = 1;
-    } else {
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h(), Cp, T, B, Cp, (uint64_t)T * Cp, 64, a_box));
-        TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l(), Cp, T, B, Cp, (uint64_t)T * Cp, 64, a_box));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, (uint64_t)N * K, 64, bn));
-        TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, W.l(), K, N, 1, K, (uint64_t)N * K, 64, bn));
-    }
-    p.num_k_blocks = K / 64, p.kb_per_row = Cp / 64;
-    p.batches = B, p.rows_per_batch = T, p.tiles_m_per_batch = (T + 127) / 128;
+    S3B_OK(gemm_tmaps(p, scheme, A, 0, width, (uint64_t)((Lin + stride - 1) / stride), B, width, (uint64_t)Lin * Cp,
+                      128 / cn, W, N, K, bn));
+    p.num_k_blocks = K / 64, p.kb_per_row = width / 64;
+    p.batches = B, p.rows_per_batch = (int)Lout, p.tiles_m_per_batch = (int)((Lout + 127) / 128);
     p.n_tiles = N / bn, p.bn = bn, p.cluster_n = cn;
-    p.a_row_step = 1, p.a_row_off = -((k - 1) / 2), p.a_gap_at = (k - mask) / 2, p.a_gap = mask;
-    p.a_k_per_ntile = 0, p.b_n_tiled = 1, p.b_z_per_ntile = 0, p.b_k_linear = 1;
-    p.out_rows_per_batch = T;
-    p.alg_flops = 2.0 * (double)B * T * N * cin * u;
+    p.a_row_step = 1, p.a_row_off = stride == 1 ? -((k - 1) / 2) : 0, p.a_gap_at = u / 2, p.a_gap = mask;
+    p.out_rows_per_batch = (int)Lout;
+    p.alg_flops = 2.0 * (double)B * Lout * N * cin * u;
     set_epi(p, e, N);
     return 0;
 }
@@ -1370,21 +1312,19 @@ static int pos_taps(const s3b_config& c) {
 }
 static int pos_taps4(const s3b_config& c) { return (pos_taps(c) + 3) / 4 * 4; }
 
-// grouped positional conv: one k-block per tap; A row coordinate = t + tap - K/2 (TMA zero-fills t<0, t>=T).
-// Groups of 80 and 120 channels take two 64-wide k-blocks per tap: the A box of the second reads on into the next
-// group's channels (or, for the last group, past D: TMA zero fill), which meet the zero-padded weights of posconv_kc.
-// The tile is exactly the group's cpg columns wide, so no output column lands in a neighbouring group.
-static int posconv_params(GemmParams& p, const s3b_config& c, const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo,
-                          const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, int B, int T, const Epi& e) {
+// grouped positional conv over x [B][T][D]: one k-block per tap; A row coordinate = t + tap - K/2 (TMA zero-fills t<0,
+// t>=T). Groups of 80 and 120 channels take two 64-wide k-blocks per tap: the A box of the second reads on into the
+// next group's channels (or, for the last group, past D: TMA zero fill), which meet the zero-padded weights of
+// posconv_kc. The tile is exactly the group's cpg columns wide, so no output column lands in a neighbouring group, and
+// it reads its group's rows of W [D][Kp * Kc].
+static int posconv_params(GemmParams& p, const s3b_config& c, const SplitBuf& x, const SplitBuf& W, int B, int T,
+                          const Epi& e) {
     memset(&p, 0, sizeof(p));
     const int D = c.embed_dim, G = c.pos_conv_groups, cpg = D / G, Kp = c.pos_conv_kernel, Kc = posconv_kc(cpg);
-    TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, x_hi, D, T, B, D, (uint64_t)T * D, 64, 128));
-    TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, x_lo, D, T, B, D, (uint64_t)T * D, 64, 128));
-    TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, w_hi, Kc, cpg, (uint64_t)G * Kp, Kc, (uint64_t)cpg * Kc, 64, cpg));
-    TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, w_lo, Kc, cpg, (uint64_t)G * Kp, Kc, (uint64_t)cpg * Kc, 64, cpg));
+    S3B_OK(gemm_tmaps(p, 0, x, 0, D, T, B, D, (uint64_t)T * D, 128, W, D, Kp * Kc, cpg));
     p.batches = B, p.rows_per_batch = T, p.tiles_m_per_batch = (T + 127) / 128;
     p.n_tiles = G, p.bn = cpg, p.num_k_blocks = Kp * (Kc / 64), p.kb_per_row = Kc / 64;
-    p.a_row_step = 1, p.a_row_off = -(Kp / 2), p.a_k_per_ntile = cpg, p.b_n_tiled = 0, p.b_z_per_ntile = Kp;
+    p.a_row_step = 1, p.a_row_off = -(Kp / 2), p.a_k_per_ntile = cpg;
     p.out_rows_per_batch = T;
     p.alg_flops = 2.0 * (double)B * T * D * cpg * Kp;
     set_epi(p, e, D);
@@ -1396,23 +1336,21 @@ static int posconv_params(GemmParams& p, const s3b_config& c, const __nv_bfloat1
 // (4 KB per 24-cycle MMA). Writing tap = 4q + j,
 //     Z_j[u] = sum_q x[u + 4q - Kp/2] . W[4q + j],      conv[t] = sum_j Z_j[t + j]
 // gives one GEMM with N = 4*cpg (192 / 256) columns per group and Kp/4 k-blocks whose A rows advance by 4; the four
-// column blocks are re-aligned by posconv_combine_kernel (norm.cu). Rows u in [0, T+3) per utterance.
+// column blocks are re-aligned by posconv_combine_kernel (norm.cu). Rows u in [0, T+3) per utterance. W: the
+// [G * 4cpg][Kq * 64] matrix of posconv4_weight_layout, one group's rows per tile.
 static bool posconv4_ok(const s3b_config& c) {
     const int cpg = c.embed_dim / c.pos_conv_groups;
     if (c.pos_conv_depth > 1) return true;  // the only formulation of the data2vec blocks (checked at create)
     return c.pos_conv_kernel % 4 == 0 && (4 * cpg == 192 || 4 * cpg == 256);
 }
-static int posconv4_params(GemmParams& p, const s3b_config& c, const __nv_bfloat16* x_hi, const __nv_bfloat16* x_lo,
-                           const __nv_bfloat16* w_hi, const __nv_bfloat16* w_lo, int B, int T, const Epi& e) {
+static int posconv4_params(GemmParams& p, const s3b_config& c, const SplitBuf& x, const SplitBuf& W, int B, int T,
+                           const Epi& e) {
     memset(&p, 0, sizeof(p));
     const int D = c.embed_dim, G = c.pos_conv_groups, cpg = D / G, Kq = pos_taps4(c) / 4, bn = 4 * cpg;
-    TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, x_hi, D, T, B, D, (uint64_t)T * D, 64, 128));
-    TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, x_lo, D, T, B, D, (uint64_t)T * D, 64, 128));
-    TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, w_hi, 64, bn, (uint64_t)G * Kq, 64, (uint64_t)bn * 64, 64, bn));
-    TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, w_lo, 64, bn, (uint64_t)G * Kq, 64, (uint64_t)bn * 64, 64, bn));
+    S3B_OK(gemm_tmaps(p, 0, x, 0, D, T, B, D, (uint64_t)T * D, 128, W, 4 * D, Kq * 64, bn));
     p.batches = B, p.rows_per_batch = T + 3, p.tiles_m_per_batch = (T + 3 + 127) / 128;
     p.n_tiles = G, p.bn = bn, p.num_k_blocks = Kq, p.kb_per_row = 1;
-    p.a_row_step = 4, p.a_row_off = -(pos_taps(c) / 2), p.a_k_per_ntile = cpg, p.b_n_tiled = 0, p.b_z_per_ntile = Kq;
+    p.a_row_step = 4, p.a_row_off = -(pos_taps(c) / 2), p.a_k_per_ntile = cpg;
     p.out_rows_per_batch = T + 3;
     p.k_steps = (cpg + 15) / 16;  // 48 channels per group: the 4th k-step of every 64-wide box has zero weights
     p.alg_flops = 2.0 * (double)B * T * D * cpg * pos_taps(c);
@@ -1732,7 +1670,7 @@ static int add_conv_frontend(const Lane& lane, std::vector<Step>& steps) {
             else e.gelu = 1;
         }
         GemmParams p;
-        S3B_OK(conv_params(p, w->act[i - 1], m->conv_w[i], B, lane.L[i - 1], lane.L[i], kConvK[i], sch, e));
+        S3B_OK(conv_params(p, w->act[i - 1], m->conv_w[i], B, lane.L[i - 1], lane.L[i], 2, C, C, kConvK[i], 0, sch, e));
         const size_t rows = (size_t)B * lane.L[i];
         steps.push_back([=](Fwd& f) {
             S3B_OK(run_gemm(f, p));
@@ -1807,8 +1745,7 @@ static int add_pos_conv(const Lane& lane, std::vector<Step>& steps) {
         std::vector<GemmParams> conv(depth);
         for (int i = 0; i < depth; ++i) {
             x[i] = i == 0 ? &w->x_s : (i & 1) ? &w->x1_s : &w->ctx_s;
-            S3B_OK(posconv4_params(conv[i], c, x[i]->h(), x[i]->l(), m->posd_w4[i].h(), m->posd_w4[i].l(), B, T,
-                                   epi_f32(z)));
+            S3B_OK(posconv4_params(conv[i], c, *x[i], m->posd_w4[i], B, T, epi_f32(z)));
         }
         steps.push_back([=](Fwd& f) {
             for (int i = 0; i < depth; ++i) {
@@ -1825,7 +1762,7 @@ static int add_pos_conv(const Lane& lane, std::vector<Step>& steps) {
     } else if (posconv4_ok(c)) {
         // four taps per k-block into pos_z, then the combine kernel (+ LayerNorm)
         GemmParams p;
-        S3B_OK(posconv4_params(p, c, w->x_s.h(), w->x_s.l(), m->pos_w4.h(), m->pos_w4.l(), B, T, epi_f32(z)));
+        S3B_OK(posconv4_params(p, c, w->x_s, m->pos_w4, B, T, epi_f32(z)));
         steps.push_back([=](Fwd& f) {
             S3B_OK(run_gemm(f, p));
             KNORM(m, f.st, launch_posconv_combine(z, f.proj_out(), m->pos_b.as<float>(), B, T, D, cpg,
@@ -1839,7 +1776,7 @@ static int add_pos_conv(const Lane& lane, std::vector<Step>& steps) {
         Epi e = epi_f32(w->tmp_f32.as<float>(), m->pos_b.as<float>());
         e.gelu = 1;
         GemmParams p;
-        S3B_OK(posconv_params(p, c, w->x_s.h(), w->x_s.l(), m->pos_w.h(), m->pos_w.l(), B, T, e));
+        S3B_OK(posconv_params(p, c, w->x_s, m->pos_w, B, T, e));
         steps.push_back([=](Fwd& f) {
             GemmParams q = p;
             q.residual = f.proj_out();
@@ -2146,14 +2083,14 @@ static int add_npc_stack(const Lane& lane, std::vector<Step>& steps) {
         const LayerW& L = m->layers[i];
         const bool first = i == 0;
         GemmParams conv, lin, mc;
-        S3B_OK(tapconv_params(conv, first ? w->ln512_s : w->x_s, L.fc1, B, T, first ? kDecoar2K : H, first ? 80 : H, 3,
-                              0, sch, epi_planes(w->h_s.planes(sch), L.fc1_b.as<float>(), act)));
+        S3B_OK(conv_params(conv, first ? w->ln512_s : w->x_s, L.fc1, B, T, T, 1, first ? 80 : H, first ? kDecoar2K : H,
+                           3, 0, sch, epi_planes(w->h_s.planes(sch), L.fc1_b.as<float>(), act)));
         Epi el = epi_f32(nullptr, L.fc2_b.as<float>());
         el.op = w->x_s.planes(sch), el.gelu = act, el.res_first = 1;
-        S3B_OK(tapconv_params(lin, w->h_s, L.fc2, B, T, H, H, 1, 0, sch, el));
+        S3B_OK(conv_params(lin, w->h_s, L.fc2, B, T, T, 1, H, H, 1, 0, sch, el));
         Epi em = epi_f32(nullptr, L.out_b.as<float>());
         em.gelu = 4;
-        S3B_OK(tapconv_params(mc, w->x_s, L.out, B, T, H, H, c.kernel_size, npc_mask_width(c, i), sch, em));
+        S3B_OK(conv_params(mc, w->x_s, L.out, B, T, T, 1, H, H, c.kernel_size, npc_mask_width(c, i), sch, em));
         const bool residual = c.residual && !first;
         steps.push_back([=](Fwd& f) { return run_gemm(f, conv); });
         steps.push_back([=](Fwd& f) {
@@ -2729,7 +2666,7 @@ extern "C" int s3b_conv_gemm_f32(const float* x, const float* w, const float* bi
     SplitBuf xs, ws, os;
     std::vector<float> wh;
     S3B_OK(download_f32(w, (size_t)C * C * kw, st, wh));
-    const std::vector<float> wl = conv_weight_layout(wh.data(), kw);
+    const std::vector<float> wl = tap_weight_layout(wh.data(), C, C, kw, 0, C);
     S3B_OK(upload_split(ws, wl.data(), wl.size(), sch));
     S3B_OK(split_operand(x, xs, (size_t)B * Lin * C, sch, 0, st));
     Epi e;
@@ -2741,7 +2678,7 @@ extern "C" int s3b_conv_gemm_f32(const float* x, const float* w, const float* bi
         e.op = os.planes(out_fmt);
     }
     GemmParams p;
-    S3B_OK(conv_params(p, xs, ws, B, Lin, Lout, kw, sch, e));
+    S3B_OK(conv_params(p, xs, ws, B, Lin, Lout, 2, C, C, kw, 0, sch, e));
     CUDA_OK(launch_gemm(p, sms, st));
     if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), (size_t)B * Lout * C, out, st));
     CUDA_OK(cudaStreamSynchronize(st));
@@ -2780,8 +2717,8 @@ extern "C" int s3b_posconv_f32(const float* x, const float* w, const float* bias
     DevBuf z;
     std::vector<float> wh;
     S3B_OK(download_f32(w, (size_t)D * cpg * k, st, wh));
-    const std::vector<float> wl =
-        taps == 4 ? posconv4_weight_layout(wh.data(), D, G, k) : posconv_weight_layout(wh.data(), D, G, k);
+    const std::vector<float> wl = taps == 4 ? posconv4_weight_layout(wh.data(), D, G, k)
+                                            : tap_weight_layout(wh.data(), D, cpg, k, 0, posconv_kc(cpg));
     S3B_OK(upload_split(ws, wl.data(), wl.size()));
     S3B_OK(split_operand(x, xs, M * D, 0, 0, st));
     OutPlanes op = no_planes();
@@ -2794,7 +2731,7 @@ extern "C" int s3b_posconv_f32(const float* x, const float* w, const float* bias
     if (taps == 4) {
         // add_pos_conv: Z = the four-tap GEMM, then the combine kernel (+ LayerNorm)
         S3B_OK(z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
-        S3B_OK(posconv4_params(p, c, xs.h(), xs.l(), ws.h(), ws.l(), B, T, epi_f32(z.as<float>())));
+        S3B_OK(posconv4_params(p, c, xs, ws, B, T, epi_f32(z.as<float>())));
         CUDA_OK(launch_gemm(p, sms, st));
         CUDA_OK(launch_posconv_combine(z.as<float>(), x, bias, B, T, D, cpg, gamma, beta, gamma ? 1 : 0, mode,
                                        out_f32, op, st));
@@ -2803,7 +2740,7 @@ extern "C" int s3b_posconv_f32(const float* x, const float* w, const float* bias
         if (gamma != nullptr) S3B_OK(z.ensure(M * D * sizeof(float)));
         Epi e = epi_f32(gamma != nullptr ? z.as<float>() : out_f32, bias, x);
         e.gelu = 1;
-        S3B_OK(posconv_params(p, c, xs.h(), xs.l(), ws.h(), ws.l(), B, T, e));
+        S3B_OK(posconv_params(p, c, xs, ws, B, T, e));
         CUDA_OK(launch_gemm(p, sms, st));
         if (gamma != nullptr) CUDA_OK(launch_layernorm(z.as<float>(), M, D, gamma, beta, 0, out_f32, op, st));
     }
@@ -2832,7 +2769,7 @@ extern "C" int s3b_npc_conv_f32(const float* x, int32_t B, int32_t T, int32_t c_
     S3B_OK(device_sm_count(&sms));
     std::vector<float> wh;
     S3B_OK(download_f32(w, (size_t)N * c_in * k, st, wh));
-    const std::vector<float> wl = npc_weight_layout(std::vector<double>(wh.begin(), wh.end()), c_in, k, mask, Cp);
+    const std::vector<float> wl = tap_weight_layout(wh.data(), N, c_in, k, mask, Cp);
     SplitBuf xs, ws;
     S3B_OK(upload_split(ws, wl.data(), wl.size(), sch));
     DevBuf xpad;
@@ -2845,7 +2782,7 @@ extern "C" int s3b_npc_conv_f32(const float* x, int32_t B, int32_t T, int32_t c_
     Epi e = epi_f32(out, bias, residual);
     e.gelu = act == 0 ? 0 : act == 1 ? 3 : 4, e.res_first = res_first;
     GemmParams p;
-    S3B_OK(tapconv_params(p, xs, ws, B, T, Cp, c_in, k, mask, sch, e));
+    S3B_OK(conv_params(p, xs, ws, B, T, T, 1, c_in, Cp, k, mask, sch, e));
     p.out_pre = out_pre;
     CUDA_OK(launch_gemm(p, sms, st));
     CUDA_OK(cudaStreamSynchronize(st));
