@@ -34,6 +34,8 @@ int main(void) {
         (const void*)s3b_gru_f32,        (const void*)s3b_gru_max_active_clusters,
         (const void*)s3b_decoar_model_create, (const void*)s3b_lstm_f32, (const void*)s3b_lstm_fits,
         (const void*)s3b_npc_model_create, (const void*)s3b_npc_conv_f32,
+        (const void*)s3b_cpc_model_create, (const void*)s3b_cpc_conv_f32, (const void*)s3b_cpc_lstm_f32,
+        (const void*)s3b_cpc_lstm_max_active_clusters,
     };
     s3b_config cfg;
     int64_t lens[2] = {16000, 800};
@@ -115,6 +117,24 @@ int main(void) {
         }
         s3b_model_destroy(m);
         if (valid[0] != 98 || valid[1] != 3) return 13;
+    }
+    {
+        /* modified CPC: the padded conv chain (16000 -> 100, 800 -> 5); the encoder and the last LSTM layer */
+        s3b_cpc_config ccfg;
+        s3b_model* m = NULL;
+        memset(&ccfg, 0, sizeof(ccfg));
+        ccfg.struct_size = (int32_t)sizeof(ccfg), ccfg.hidden = 256, ccfg.num_layers = 1;
+        if (s3b_cpc_model_create(&ccfg, &m) != 0) {
+            printf("s3b_cpc_model_create: %s\n", s3b_last_error());
+            return 14;
+        }
+        if (s3b_valid_frames(m, lens, 2, 16000, valid) != 0 || s3b_num_outputs(m) != 2 ||
+            s3b_num_frames(m, 16000) != 100 || s3b_num_frames(m, 158) != -1) {
+            printf("CPC bookkeeping: %s\n", s3b_last_error());
+            return 15;
+        }
+        s3b_model_destroy(m);
+        if (valid[0] != 100 || valid[1] != 5) return 16;
     }
     return 0;
 }

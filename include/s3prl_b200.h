@@ -145,6 +145,25 @@ typedef struct s3b_npc_config {
     int32_t reserved[4]; /* 0 */
 } s3b_npc_config;
 int s3b_npc_model_create(const s3b_npc_config* cfg, s3b_model** out);
+/* Modified CPC (s3prl/upstream/cpc/{expert,model}.py): pad_sequence of the waveforms (no normalisation), then the
+ * encoder: five Conv1d(k = 2 s) with strides 5, 4, 2, 2, 2 and paddings 3, 2, 1, 1, 1 (1 -> 256 channels, then 256 ->
+ * 256), each followed by ChannelNorm (per frame over the 256 channels, unbiased variance, rsqrt(var + 1e-5)) and ReLU;
+ * then nn.LSTM(256, 256, num_layers) over the whole padded batch (no packing, h0 = c0 = 0, gate order i, f, g, o).
+ * T = the conv chain over max_len (159 samples -> 1 frame, 16000 -> 100); max_len < 159 yields no frame. Individual
+ * utterances may be shorter. Frames are not masked: the frames near and after an utterance's end hold the model's
+ * response to the zero samples, so the last frame of an utterance (and those after it) depend on max_len.
+ * Tensors (reference key names, CPCModel.state_dict()): gEncoder.conv{i}.{weight [256][1 or 256][2 s], bias [256]},
+ * gEncoder.batchNorm{i}.{weight, bias} [1][256][1] for i = 0..4; gAR.baseNet.{weight_ih_l{k} [1024][256],
+ * weight_hh_l{k} [1024][256], bias_ih_l{k}, bias_hh_l{k} [1024]} for k < num_layers.
+ * s3b_num_outputs = 2: hidden_out is [encoder output, last LSTM layer's output] [batch][T][256]. s3b_forward_ex refuses
+ * ffn_out and last_residual. Served: hidden 256, num_layers 1..8. */
+typedef struct s3b_cpc_config {
+    int32_t struct_size; /* sizeof(s3b_cpc_config) */
+    int32_t hidden;      /* hiddenEncoder = hiddenGar: 256 */
+    int32_t num_layers;  /* nLevelsGRU: LSTM layers, 1..8 */
+    int32_t reserved[4]; /* 0 */
+} s3b_cpc_config;
+int s3b_cpc_model_create(const s3b_cpc_config* cfg, s3b_model** out);
 int s3b_model_finalize(s3b_model* m);
 void s3b_model_destroy(s3b_model* m);
 
@@ -383,6 +402,21 @@ int s3b_posconv_f32(const float* x, const float* w, const float* bias, int32_t b
 int s3b_npc_conv_f32(const float* x, int32_t batch, int32_t t, int32_t c_in, const float* w, int32_t k, int32_t mask,
                      const float* bias, const float* residual, int32_t act, int32_t res_first, int32_t scheme,
                      float* out, float* out_pre, void* stream);
+/* One modified CPC conv + ChannelNorm + ReLU as the model runs it. layer 0: x is the padded waveform batch
+ * [batch][len], w [256][1][10] (stride 5, padding 3); the model writes conv 0's output as operand planes only, so out
+ * holds those planes (format of `scheme`) decoded to fp32. layer 1..4: x is channels-last [batch][len][256], w
+ * [256][256][2 s] (torch layout; s = 4, 2, 2, 2, padding s / 2), computed as the model computes it: x split into operand
+ * planes of `scheme` in the padded layout, one implicit GEMM (+ bias) in fp32, then the norm. bias, gamma, beta: [256];
+ * all pointers device. scheme -1 / 0 / 1 as s3b_linear_ex. out: [batch][T][256] fp32, T = the conv's output length. */
+int s3b_cpc_conv_f32(const float* x, int32_t batch, int32_t len, int32_t layer, const float* w, const float* bias,
+                     const float* gamma, const float* beta, int32_t scheme, float* out, void* stream);
+/* One modified CPC LSTM layer's recurrence as the model runs it: xg [batch][t][1024] = W_ih x + b_ih + b_hh (gate order
+ * i, f, g, o), whh [1024][256]; every utterance runs all t steps from h0 = c0 = 0. out [batch][t][256] fp32; out_fmt 0 /
+ * 1 also writes the same values as operand planes of that format, decoded into planes_out (-1: none). */
+int s3b_cpc_lstm_f32(const float* xg, const float* whh, int32_t batch, int32_t t, int32_t out_fmt, float* out,
+                     float* planes_out, void* stream);
+/* clusters of the CPC recurrence kernel (8 CTAs, 4 utterances each) that can be co-resident on the current device */
+int s3b_cpc_lstm_max_active_clusters(int32_t* out);
 /* micro-benchmark of the production GEMM kernel: `iters` back-to-back launches of [M][K] x [N][K]^T with the fc1-style
  * epilogue (gelu != 0: bias + GELU + bf16 hi/lo output) or the out_proj-style one (bias + residual + fp32 output).
  * force_un in {0 = the library's choice, 128, 256} forces the tile width (columns per output tile) wherever it divides

@@ -54,6 +54,8 @@ __device__ __forceinline__ float sigmoid_fast(float x) {
     return r;
 }
 __device__ __forceinline__ float silu(float x) { return x * sigmoid_fast(x); }
+// ReLU that keeps a NaN, as torch.relu does (fmaxf(NaN, 0) would return 0 and hide it)
+__device__ __forceinline__ float relu_nan(float x) { return x < 0.0f ? 0.0f : x; }
 
 // hi/lo split of an fp32 value into two bf16 values (round-to-nearest-even both times)
 __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {
@@ -282,6 +284,32 @@ __device__ __forceinline__ uint32_t peer_addr(const void* p, uint32_t rank) {
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(out) : "r"(smem_u32(p)), "r"(rank));
     return out;
 }
+// store to a peer_addr address (distributed shared memory)
+__device__ __forceinline__ void st_cluster_f4(uint32_t addr, float4 v) {
+    asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z),
+                 "f"(v.w)
+                 : "memory");
+}
+
+// ----------------------------------------------------------------------------------------------
+// the recurrences' dot products (gru.cu, lstm.cu, cpc_lstm.cu)
+// ----------------------------------------------------------------------------------------------
+// one butterfly level: lanes with bit kOff set keep values [kHalf, 2 kHalf), the others [0, kHalf); each adds its
+// partner's copy of what it keeps. The kept values move to [0, kHalf).
+template <int kOff, int kHalf, int kN>
+__device__ __forceinline__ void halve(float (&acc)[kN], int lane) {
+    static_assert(2 * kHalf <= kN, "halve: more values kept than held");
+    const bool upper = (lane & kOff) != 0;
+#pragma unroll
+    for (int v = 0; v < kHalf; ++v) {
+        const float send = upper ? acc[v] : acc[v + kHalf];
+        const float keep = upper ? acc[v + kHalf] : acc[v];
+        acc[v] = keep + __shfl_xor_sync(0xffffffffu, send, kOff);
+    }
+}
+
+// the recurrences' sigmoid: IEEE division and expf, the accuracy of PyTorch's CPU and cuDNN cells
+__device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
 // arrive on an mbarrier of any CTA of the cluster (a peer_addr address). The default .release.cta semantics: a
 // .cluster-scoped release compiles to a MEMBAR.ALL.GPU that waits for every outstanding store of the thread (the GEMM
 // epilogue's), and a consumer releasing a shared-memory stage that only wgmma read needs no such fence.

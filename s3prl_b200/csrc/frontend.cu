@@ -383,4 +383,87 @@ cudaError_t launch_conv0_layernorm(const float* x, int B, long long L, int L0, c
 
 size_t conv0_ws_part_bytes(int B, int L0) { return (size_t)B * ((L0 + kTCH - 1) / kTCH) * kNMom * sizeof(double); }
 
+// ------------------------------------------------------------------------------------------------
+// modified CPC's conv 0 (s3prl/upstream/cpc/model.py CPCEncoder): Conv1d(1, 256, 10, stride 5, padding 3) + bias,
+// ChannelNorm over the 256 channels of each frame (unbiased variance, eps inside the rsqrt), ReLU. One warp per
+// output row; lane l holds channels 4 l .. 4 l + 3 and 128 + 4 l .. + 3. The output is conv 1's padded operand
+// layout: utterance b owns rows [b R, b R + R), and row r holds frame r - pad when that is in [0, T0), zeros
+// otherwise (every row is written, so a reused workspace never leaks into the result).
+// ------------------------------------------------------------------------------------------------
+static constexpr int kCpcC = 256;
+static constexpr int kCpcK0 = 10;
+static constexpr int kCpcS0 = 5;
+static constexpr int kCpcP0 = 3;
+
+__global__ void __launch_bounds__(256) cpc_conv0_kernel(const float* __restrict__ x, int B, long long L, int T0,
+                                                        const float* __restrict__ w, const float* __restrict__ cbias,
+                                                        const float* __restrict__ gamma,
+                                                        const float* __restrict__ beta, int R, int pad,
+                                                        const OutPlanes op) {
+    const int lane = threadIdx.x & 31;
+    const size_t rows = (size_t)B * R;
+    const size_t warps = (size_t)gridDim.x * (blockDim.x >> 5);
+    float wr[2][4][kCpcK0], cb[2][4], g[2][4], be[2][4];
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int c = 128 * i + 4 * lane + e;
+#pragma unroll
+            for (int j = 0; j < kCpcK0; ++j) wr[i][e][j] = w[c * kCpcK0 + j];
+            cb[i][e] = cbias[c], g[i][e] = gamma[c], be[i][e] = beta[c];
+        }
+    for (size_t row = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); row < rows; row += warps) {
+        const int b = (int)(row / R), t = (int)(row - (size_t)b * R) - pad;
+        float4 y[2];
+        if (t < 0 || t >= T0) {
+            y[0] = y[1] = make_float4(0.f, 0.f, 0.f, 0.f);
+        } else {
+            const float* xb = x + (size_t)b * L;
+            const long long s0 = (long long)t * kCpcS0 - kCpcP0;
+            float xv[kCpcK0];
+#pragma unroll
+            for (int j = 0; j < kCpcK0; ++j) xv[j] = (s0 + j >= 0 && s0 + j < L) ? __ldg(xb + s0 + j) : 0.f;
+            float z[2][4], s = 0.f;
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    float a = 0.f;
+#pragma unroll
+                    for (int j = 0; j < kCpcK0; ++j) a = fmaf(wr[i][e][j], xv[j], a);
+                    z[i][e] = a + cb[i][e];
+                    s += z[i][e];
+                }
+            const float mean = warp_sum(s) * (1.0f / kCpcC);
+            float q = 0.f;
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) q += (z[i][e] - mean) * (z[i][e] - mean);
+            const float rstd = rsqrtf(warp_sum(q) * (1.0f / (kCpcC - 1)) + 1e-5f);
+            float o[2][4];
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int e = 0; e < 4; ++e) o[i][e] = relu_nan((z[i][e] - mean) * rstd * g[i][e] + be[i][e]);
+            y[0] = make_float4(o[0][0], o[0][1], o[0][2], o[0][3]);
+            y[1] = make_float4(o[1][0], o[1][1], o[1][2], o[1][3]);
+        }
+        store_planes4(op, y[0], row * kCpcC + 4 * lane);
+        store_planes4(op, y[1], row * kCpcC + 128 + 4 * lane);
+    }
+}
+
+cudaError_t launch_cpc_conv0(const float* x, int B, long long L, int T0, const float* w, const float* cbias,
+                             const float* gamma, const float* beta, int R, int pad, const OutPlanes& op,
+                             cudaStream_t s) {
+    const size_t rows = (size_t)B * R;
+    if (rows == 0) return cudaSuccess;
+    size_t blocks = (rows + 7) / 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
+    cpc_conv0_kernel<<<(unsigned)blocks, 256, 0, s>>>(x, B, L, T0, w, cbias, gamma, beta, R, pad, op);
+    return cudaGetLastError();
+}
+
 }  // namespace s3b

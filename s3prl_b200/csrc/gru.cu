@@ -42,27 +42,6 @@ struct GruSmem {
 // one CTA per SM with the opt-in maximum of dynamic shared memory (227 KB on sm_90)
 static_assert(sizeof(GruSmem) <= 227 * 1024, "the recurrence kernel's shared memory exceeds 227 KB");
 
-__device__ __forceinline__ void st_cluster_f4(uint32_t addr, float4 v) {
-    asm volatile("st.shared::cluster.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(v.x), "f"(v.y), "f"(v.z),
-                 "f"(v.w)
-                 : "memory");
-}
-
-// one butterfly level: lanes with bit kOff set keep values [kHalf, 2 kHalf), the others [0, kHalf); each adds its
-// partner's copy of what it keeps. The kept values move to [0, kHalf).
-template <int kOff, int kHalf>
-__device__ __forceinline__ void halve(float (&acc)[kVals], int lane) {
-    const bool upper = (lane & kOff) != 0;
-#pragma unroll
-    for (int v = 0; v < kHalf; ++v) {
-        const float send = upper ? acc[v] : acc[v + kHalf];
-        const float keep = upper ? acc[v + kHalf] : acc[v];
-        acc[v] = keep + __shfl_xor_sync(0xffffffffu, send, kOff);
-    }
-}
-
-__device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
-
 // grid: kCtas x number of groups, cluster (kCtas, 1, 1); block kThreads; dynamic smem sizeof(GruSmem)
 __global__ void __launch_bounds__(kThreads, 1) gru_cluster_kernel(GruParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];

@@ -21,12 +21,21 @@ cudaError_t launch_conv0_groupnorm(const float* x, int B, long long L, int L0, c
                                    cudaStream_t s);
 cudaError_t launch_conv0_layernorm(const float* x, int B, long long L, int L0, const float* w, const float* cbias,
                                    const float* gamma, const float* beta, const OutPlanes& op, cudaStream_t s);
+// modified CPC's conv 0 (w [256][10], stride 5, padding 3, + bias) + ChannelNorm + ReLU over x [B][L] into T0 frames
+// of conv 1's padded operand layout: R rows per utterance, row r = frame r - pad (zeros outside [0, T0))
+cudaError_t launch_cpc_conv0(const float* x, int B, long long L, int T0, const float* w, const float* cbias,
+                             const float* gamma, const float* beta, int R, int pad, const OutPlanes& op,
+                             cudaStream_t s);
 
 // ---- norm.cu -------------------------------------------------------------------------------------
 // y = LayerNorm_D(x) * gamma + beta (eps 1e-5, biased var), optional GELU; D in {512, 768, 1024, 1280, 1920}.
 // Any of out_f32 / (out_hi,out_lo) may be null. x and out_f32 may alias.
 cudaError_t launch_layernorm(const float* x, size_t M, int D, const float* gamma, const float* beta, int gelu,
                              float* out_f32, const OutPlanes& op, cudaStream_t s);
+// modified CPC: y = relu(ChannelNorm_256(x)) (unbiased var, eps 1e-5) of x [B][T][256] into op with R rows per
+// utterance, row r = frame r - pad (zeros outside [0, T)); out_f32 [B][T][256] only with R == T and pad == 0
+cudaError_t launch_channelnorm_relu(const float* x, int B, int T, int R, int pad, const float* gamma,
+                                    const float* beta, float* out_f32, const OutPlanes& op, cudaStream_t s);
 // Conformer: y = LayerNorm_D(x) -> op, rope(y) -> op_rope; frame t = row % T, cs [>= T][64] = cos | sin of the 32 angles
 cudaError_t launch_layernorm_rope(const float* x, size_t M, int T, int D, const float* gamma, const float* beta,
                                   const float* cs, const OutPlanes& op, const OutPlanes& op_rope, cudaStream_t s);
@@ -107,6 +116,21 @@ size_t lstm_smem_bytes();
 // ok = 1 when the device can host the grid: >= kLstmCtas SMs, enough opt-in shared memory, cooperative launch and one
 // CTA per SM; sms / smem_optin report the device's values for messages
 cudaError_t lstm_fits(int* ok, int* sms, int* smem_optin);
+
+// ---- cpc_lstm.cu: the LSTM recurrence of modified CPC (cluster-resident W_hh) -------------------------------------
+static constexpr int kCpcLstmHidden = 256;  // hidden size the kernel is built for
+static constexpr int kCpcLstmGroup = 4;     // utterances per cluster
+static constexpr int kCpcLstmCtas = 8;      // CTAs per cluster (portable cluster size), 32 hidden units each
+struct CpcLstmParams {
+    const float* xg;   // [B][T][4H]: W_ih x + b_ih + b_hh, gate order i, f, g, o
+    const float* whh;  // [4H][H] weight_hh_l{k}
+    int B, T;          // every utterance runs all T steps; cluster g runs utterances 4g .. 4g + 3
+    float* out;        // optional [B][T][H] layer output (fp32)
+    OutPlanes op;      // optional [B * T][H] operand planes of the same values (op.hi null: none)
+};
+cudaError_t launch_cpc_lstm(const CpcLstmParams& p, cudaStream_t s);
+// clusters of the recurrence kernel that can be co-resident on the current device (0: the kernel cannot run)
+cudaError_t cpc_lstm_max_active_clusters(int* n);
 
 // ---- peer.cu: fused weighted sum + push all-gather over peer memory --------------------------------------------------
 cudaError_t launch_weighted_sum_push(const float* hs, int NL, size_t n_per_layer, size_t layer_stride, const float* w,

@@ -49,21 +49,6 @@ struct LstmSmem {
 // one CTA per SM with the opt-in maximum of dynamic shared memory (227 KB on sm_90)
 static_assert(sizeof(LstmSmem) <= 227 * 1024, "the LSTM recurrence kernel's shared memory exceeds 227 KB");
 
-// lanes with bit kOff set keep values [kHalf, 2 kHalf), the others [0, kHalf); each adds its partner's copy of what
-// it keeps. The kept values move to [0, kHalf).
-template <int kOff, int kHalf>
-__device__ __forceinline__ void halve(float (&acc)[kVals], int lane) {
-    const bool upper = (lane & kOff) != 0;
-#pragma unroll
-    for (int v = 0; v < kHalf; ++v) {
-        const float send = upper ? acc[v] : acc[v + kHalf];
-        const float keep = upper ? acc[v + kHalf] : acc[v];
-        acc[v] = keep + __shfl_xor_sync(0xffffffffu, send, kOff);
-    }
-}
-
-__device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
-
 __device__ __forceinline__ void grid_arrive(unsigned int* counter) {
     asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(counter) : "memory");
 }

@@ -272,6 +272,7 @@ enum ModelKind {
     kGruStack,      // s3b_apc_model_create (APC / VQ-APC): fbank + CMVN into a GRU stack
     kLstmStack,     // s3b_decoar_model_create (DeCoAR): fbank + CMVN, post_extract_proj, bidirectional LSTM stack
     kNpcStack,      // s3b_npc_model_create (NPC): fbank + CMVN into ConvBlocks and masked convs
+    kCpcStack,      // s3b_cpc_model_create (modified CPC): padded strided conv stack with ChannelNorm into an LSTM stack
 };
 
 struct s3b_model {
@@ -283,6 +284,9 @@ struct s3b_model {
     int decoar_all_layers = 0;  // 1: decoar_layers (every layer's output), 0: decoar (the last one)
     // kNpcStack: cfg holds num_layers = n_blocks and embed_dim = hidden
     s3b_npc_config npc = {};
+    // kCpcStack: cfg holds num_layers = the LSTM levels and embed_dim = 256. Weights: conv0_w [256][10], conv0_b and
+    // norm0_g / norm0_b (conv 0's ChannelNorm), conv_w[1..4] [256][2 s * 256] (tap_weight_layout), conv_b[1..4] and
+    // conv_ln_g / conv_ln_b[1..4]; per LSTM layer wih [1024][256], gru_b = bias_ih + bias_hh, whh [1024][256] fp32
     std::map<std::string, HostTensor> host;
     bool finalized = false;
     int sm_count = 132;
@@ -372,15 +376,34 @@ static int64_t num_frames(int64_t L) {
 static const int64_t kDecoar2MinLen = 560;  // two fbank frames: the unbiased std of one frame is NaN
 static int64_t decoar2_frames(int64_t L) { return L < 400 ? 0 : (1 + (L - 400) / 160 + 1) / 2; }
 static int64_t fbank_frames(int64_t L) { return L < 400 ? 0 : 1 + (L - 400) / 160; }
-// frames of a batch padded to L for this model's front end (m NULL: the conv stack); on the fbank kinds also the
-// valid frames of one utterance of L samples
+// modified CPC's encoder (cpc/model.py CPCEncoder): five Conv1d with k = 2 s, strides 5, 4, 2, 2, 2 and paddings
+// 3, 2, 1, 1, 1, 256 channels each
+static const int kCpcConvs = 5;
+static const int kCpcStride[kCpcConvs] = {5, 4, 2, 2, 2};
+static const int kCpcPad[kCpcConvs] = {3, 2, 1, 1, 1};
+static const int kCpcDim = 256;
+static int64_t cpc_conv_len(int64_t L, int i) {
+    const int s = kCpcStride[i], k = 2 * s;
+    return L + 2 * kCpcPad[i] < k ? 0 : (L + 2 * kCpcPad[i] - k) / s + 1;
+}
+static int64_t cpc_frames(int64_t L) {
+    for (int i = 0; i < kCpcConvs; ++i) L = cpc_conv_len(L, i);
+    return L;
+}
+// rows per utterance of conv i's (i >= 1) padded operand, whose view rows t, t + 1 feed output frame t (conv_params):
+// pad zero rows, the Lout(i - 1) input frames (those that fit), zero rows up to s (Lout + 1)
+static int64_t cpc_rows(int64_t Lout, int i) { return kCpcStride[i] * (Lout + 1); }
+
+// frames of a batch padded to L for this model's front end (m NULL: the conv stack); on the fbank kinds and modified
+// CPC also the valid frames of one utterance of L samples
 static int64_t model_frames(const s3b_model* m, int64_t L) {
+    if (m != nullptr && m->kind == kCpcStack) return cpc_frames(L);
     if (m == nullptr || m->kind == kConvEncoder) return num_frames(L);
     return m->kind == kFbankEncoder ? decoar2_frames(L) : fbank_frames(L);  // the recurrent stacks keep every frame
 }
 static int fail_too_short(const s3b_model* m, int64_t max_len) {
     return fail("max_len %lld too short: the %s yields no frame", (long long)max_len,
-                m->kind == kConvEncoder ? "conv stack" : "fbank");
+                m->kind == kConvEncoder || m->kind == kCpcStack ? "conv stack" : "fbank");
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -536,6 +559,24 @@ extern "C" int s3b_npc_model_create(const s3b_npc_config* cfg, s3b_model** out) 
     memset(&m->cfg, 0, sizeof(m->cfg));
     m->cfg.num_layers = cfg->n_blocks, m->cfg.embed_dim = cfg->hidden;
     m->kind = kNpcStack, m->npc = *cfg;
+    m->scheme = default_scheme();
+    *out = m;
+    return 0;
+}
+
+extern "C" int s3b_cpc_model_create(const s3b_cpc_config* cfg, s3b_model** out) {
+    if (!cfg || !out) return fail("null argument");
+    if (cfg->struct_size != (int32_t)sizeof(s3b_cpc_config))
+        return fail("s3b_cpc_config.struct_size %d != %d (header / library mismatch)", cfg->struct_size,
+                    (int)sizeof(s3b_cpc_config));
+    if (cfg->hidden != kCpcDim) return fail("hidden %d: modified CPC is served with hidden size %d", cfg->hidden, kCpcDim);
+    if (cfg->num_layers < 1 || cfg->num_layers > 8) return fail("num_layers %d: must be 1..8", cfg->num_layers);
+    for (int i = 0; i < 4; ++i)
+        if (cfg->reserved[i] != 0) return fail("s3b_cpc_config.reserved[%d] must be 0", i);
+    s3b_model* m = new s3b_model();
+    memset(&m->cfg, 0, sizeof(m->cfg));
+    m->cfg.num_layers = cfg->num_layers, m->cfg.embed_dim = cfg->hidden;
+    m->kind = kCpcStack;
     m->scheme = default_scheme();
     *out = m;
     return 0;
@@ -812,6 +853,51 @@ static int finalize_npc(s3b_model* m) {
     return 0;
 }
 
+// modified CPC (cpc/model.py CPCModel): gEncoder.conv{i} [256][cin][2 s] + bias, gEncoder.batchNorm{i} (ChannelNorm,
+// affine [1][256][1]), then gAR.baseNet = nn.LSTM(256, 256, num_layers). Conv 1..4 become [256][2 s * 256] tap-major
+// GEMM weights; the LSTM's two biases are summed into the input GEMM's bias.
+static int finalize_cpc(s3b_model* m) {
+    const int C = kCpcDim, H = kCpcDim, NL = m->cfg.num_layers;
+    for (int i = 0; i < kCpcConvs; ++i) {
+        const std::string conv = "gEncoder.conv" + std::to_string(i) + ".";
+        const std::string bn = "gEncoder.batchNorm" + std::to_string(i) + ".";
+        const int k = 2 * kCpcStride[i], cin = i == 0 ? 1 : C;
+        const HostTensor *w, *g, *b;
+        S3B_OK(need(m, conv + "weight", {C, cin, k}, &w));
+        S3B_OK(need(m, bn + "weight", {1, C, 1}, &g));
+        S3B_OK(need(m, bn + "bias", {1, C, 1}, &b));
+        if (i == 0) {
+            S3B_OK(upload_f32(m->conv0_w, w->data.data(), (size_t)C * k));
+        } else {
+            const std::vector<float> wl = tap_weight_layout(w->data.data(), C, C, k, 0, C);
+            S3B_OK(upload_split(m->conv_w[i], wl.data(), wl.size(), m->scheme));
+        }
+        S3B_OK(upload_vec(m, conv + "bias", C, i == 0 ? m->conv0_b : m->conv_b[i]));
+        S3B_OK(upload_f32(i == 0 ? m->norm0_g : m->conv_ln_g[i], g->data.data(), C));
+        S3B_OK(upload_f32(i == 0 ? m->norm0_b : m->conv_ln_b[i], b->data.data(), C));
+    }
+    m->layers.resize(NL);
+    for (int l = 0; l < NL; ++l) {
+        LayerW& L = m->layers[l];
+        const std::string s = "gAR.baseNet.", sl = "_l" + std::to_string(l);
+        const HostTensor *wih, *whh, *bih, *bhh;
+        S3B_OK(need(m, s + "weight_ih" + sl, {4 * H, C}, &wih));
+        S3B_OK(need(m, s + "weight_hh" + sl, {4 * H, H}, &whh));
+        S3B_OK(need(m, s + "bias_ih" + sl, {4 * H}, &bih));
+        S3B_OK(need(m, s + "bias_hh" + sl, {4 * H}, &bhh));
+        S3B_OK(upload_split(L.wih, wih->data.data(), wih->numel(), m->scheme));
+        S3B_OK(upload_f32(L.whh, whh->data.data(), whh->numel()));
+        std::vector<float> bsum(4 * H);
+        for (int j = 0; j < 4 * H; ++j) bsum[j] = bih->data[j] + bhh->data[j];
+        S3B_OK(upload_f32(L.gru_b, bsum.data(), bsum.size()));
+    }
+    int clusters = 0;
+    CUDA_OK(cpc_lstm_max_active_clusters(&clusters));
+    if (clusters < 1)
+        return fail("the CPC LSTM recurrence kernel cannot run on this device (no cluster of %d CTAs fits)", kCpcLstmCtas);
+    return 0;
+}
+
 // post_extract_proj of DeCoAR and DeCoAR 2.0: [N][80] zero-padded to K = kDecoar2K, the width of the CMVN kernel's
 // operand planes
 static int upload_fbank_proj(s3b_model* m, int N) {
@@ -1033,10 +1119,11 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
     case kGruStack: S3B_OK(finalize_apc(m)); break;
     case kLstmStack: S3B_OK(finalize_decoar(m)); break;
     case kNpcStack: S3B_OK(finalize_npc(m)); break;
+    case kCpcStack: S3B_OK(finalize_cpc(m)); break;
     case kConvEncoder:
     case kFbankEncoder: S3B_OK(finalize_encoder(m)); break;
     }
-    if (m->kind != kConvEncoder) CUDA_OK(init_fbank_tables());  // built here, not in a forward
+    if (m->kind != kConvEncoder && m->kind != kCpcStack) CUDA_OK(init_fbank_tables());  // built here, not in a forward
     m->host.clear();
     m->finalized = true;
     return 0;
@@ -1056,6 +1143,7 @@ extern "C" int32_t s3b_num_outputs(const s3b_model* m) {
     case kGruStack: return m->cfg.num_layers;  // the output of every GRU layer (+ residual)
     case kLstmStack: return m->decoar_all_layers ? m->cfg.num_layers : 1;  // decoar_layers: every layer; decoar: the last
     case kNpcStack: return 2 * m->cfg.num_layers + 1;  // every block, every masked conv, then feat
+    case kCpcStack: return 2;                          // the encoder's output, then the last LSTM layer's
     default: return m->cfg.num_layers + 1 + m->cfg.pred_heads;
     }
 }
@@ -1081,7 +1169,8 @@ extern "C" int s3b_valid_frames(const s3b_model* m, const int64_t* lens, int32_t
     for (int b = 0; b < batch; ++b) {
         int64_t v;
         if (m->kind != kConvEncoder) {
-            // pad_sequence of the per-utterance features (apc/expert.py:47-51, decoar2/expert.py:81-92)
+            // pad_sequence of the per-utterance features (apc/expert.py:47-51, decoar2/expert.py:81-92); modified CPC:
+            // the frames of the utterance's own conv chain (0 below 159 samples), though every frame is computed
             v = model_frames(m, lens[b]);
         } else if (m->cfg.family == 1) {
             // wav2vec2: conv-length rule, only when the batch has any padding (wav2vec2_model.py:2652-2671). The
@@ -1273,26 +1362,32 @@ static int linear_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, in
     return 0;
 }
 
-// Convolution of k taps into 512 channels over channels-last operand planes A [B][Lin][Cp], with epilogue `e`, as one
-// implicit GEMM over W [512][u * Cp] (tap_weight_layout; u = k - mask taps). Output row t of utterance b takes tap j
-// from input row stride * t + j - pad of its own utterance, TMA zero-filling rows outside [0, Lin).
+// Convolution of k taps into N channels (a multiple of 128) over channels-last operand planes A [B][Lin][Cp], with
+// epilogue `e`, as one implicit GEMM over W [N][u * Cp] (tap_weight_layout; u = k - mask taps). Output row t of
+// utterance b takes tap j from input row stride * t + j - pad of its own utterance, TMA zero-filling rows outside
+// [0, Lin).
 //  - stride 1 (NPC): same padding, pad = (k - 1) / 2 and Lout = Lin. Only the taps outside the centred band of `mask`
 //    taps are contracted: one k-block row per tap (Cp / 64 k-blocks), and the rows after the left run of u / 2 taps
 //    skip the band (a_gap).
-//  - stride 2 (conv 1..6, k in {2, 3}, mask 0): no padding. Row t of the [ceil(Lin / 2)][2 Cp] view holds input rows
-//    (2t, 2t + 1): taps 0, 1 come from view row t, tap 2 from the first half of view row t + 1.
+//  - stride s >= 2, mask 0: no padding in the GEMM. Row t of the [ceil(Lin / s)][s Cp] view holds input rows
+//    s t .. s t + s - 1, so taps 0 .. s - 1 come from view row t and taps s .. k - 1 from view row t + 1 (k <= 2 s).
+//    conv 1..6 of the wav2vec 2.0 stack: s = 2, k in {2, 3}. Modified CPC's conv 1..4 (k = 2 s, padding p): A is the
+//    producer's padded layout, Lin = s (Lout + 1) rows per utterance with p zero rows in front, so that the padding is
+//    part of the operand and view rows t, t + 1 are exactly the output row's receptive field.
 // alg_flops counts cin, the channels before padding.
 static int conv_params(GemmParams& p, const SplitBuf& A, const SplitBuf& W, int B, int64_t Lin, int64_t Lout,
-                       int stride, int cin, int Cp, int k, int mask, int scheme, const Epi& e) {
+                       int stride, int N, int cin, int Cp, int k, int mask, int scheme, const Epi& e) {
     memset(&p, 0, sizeof(p));
-    const int N = kConvDim, u = k - mask, K = u * Cp, width = stride * Cp;
+    if (N % 128 != 0) return fail("conv: N %d must be a multiple of 128", N);
+    const int u = k - mask, K = u * Cp, width = stride * Cp;
     // Tile: tools/gemm_shapes.py times the linear with conv i's M, N = 512 and K as a proxy (H100 80GB HBM3, 700 W,
     // hubert_base's conv stack at 32 x 10 s). f16q8 on 128-wide tiles in clusters of 4 (N = 512 is four tiles, which
     // then share each A tile) runs conv 1..6 in 6.96 ms, against 7.57 in clusters of 2, 7.97 on 256-wide tiles
     // (10-13% slower at every conv) and 9.49 on unclustered 128-wide tiles. bf16x3 stays on unclustered 128-wide
     // tiles: clusters of 2 and 4 are 2% and 10% slower there, and 256-wide tiles 70%.
+    // N = 256 (modified CPC) has two tiles, which f16q8 clusters in twos.
     const int bn = 128;
-    const int cn = pick_cluster_n(bn, N / bn, scheme != 0 ? 4 : 1);
+    const int cn = pick_cluster_n(bn, N / bn, scheme != 0 ? std::min(4, N / bn) : 1);
     S3B_OK(gemm_tmaps(p, scheme, A, 0, width, (uint64_t)((Lin + stride - 1) / stride), B, width, (uint64_t)Lin * Cp,
                       128 / cn, W, N, K, bn));
     p.num_k_blocks = K / 64, p.kb_per_row = width / 64;
@@ -1470,11 +1565,13 @@ int Fwd::prepare() {
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, C = kConvDim;
     if (B < 1) return fail("empty batch");
-    const bool fb = m->kind != kConvEncoder;
+    const bool cpc = m->kind == kCpcStack;
+    const bool fb = m->kind != kConvEncoder && !cpc;
     const bool recurrent = m->kind == kGruStack || m->kind == kLstmStack;
     {
         int64_t cur = Lmax;
-        for (int i = 0; i < kNumConv; ++i) cur = L[i] = fb ? 0 : conv_out_len(cur, i);
+        for (int i = 0; i < kNumConv; ++i)
+            cur = L[i] = fb ? 0 : cpc ? (i < kCpcConvs ? cpc_conv_len(cur, i) : 0) : conv_out_len(cur, i);
     }
     const int64_t T64 = model_frames(m, Lmax);
     if (T64 < 1) return fail_too_short(m, Lmax);
@@ -1539,7 +1636,15 @@ int Fwd::prepare() {
     d_mask = reinterpret_cast<uint8_t*>(db + off_mask);
 
     // ---- workspace ------------------------------------------------------------------------------------------
-    if (fb) {
+    if (cpc) {
+        // conv i's input (i = 1..4) in its padded layout act[i - 1], conv i's fp32 output, the LSTM's operand planes
+        // (encoder output, then each layer's), the input GEMM's output
+        S3B_OK(w->wav_pad.ensure((size_t)B * Lmax * 4));
+        for (int i = 1; i < kCpcConvs; ++i) S3B_OK(w->act[i - 1].ensure((size_t)B * cpc_rows(L[i], i) * kCpcDim));
+        S3B_OK(w->conv_f32.ensure((size_t)B * L[1] * kCpcDim * 4));
+        S3B_OK(w->x_s.ensure((size_t)M * kCpcDim));
+        S3B_OK(w->xg_f32.ensure((size_t)M * 4 * kCpcDim * 4));
+    } else if (fb) {
         S3B_OK(w->fb_f32.ensure((size_t)B * fbank_frames(Lmax) * 80 * 4));
         // the CMVN kernel's planes: the A operand of post_extract_proj (APC: of layer 0's input GEMM)
         S3B_OK(w->ln512_s.ensure((size_t)M * kDecoar2K));
@@ -1565,7 +1670,7 @@ int Fwd::prepare() {
         S3B_OK(w->xg_f32.ensure((size_t)M * 4 * H * 4));
         S3B_OK(w->lstm_h.ensure(lstm_hbuf_floats(B) * 4));
         S3B_OK(w->lstm_sync.ensure(sizeof(unsigned int)));
-    } else {  // the encoder's buffers
+    } else if (!cpc) {  // the encoder's buffers
         S3B_OK(w->tmp_f32.ensure((size_t)M * D * 4));
         S3B_OK(w->x_f32.ensure((size_t)M * D * 4));
         S3B_OK(w->x1_f32.ensure((size_t)M * D * 4));
@@ -1670,7 +1775,7 @@ static int add_conv_frontend(const Lane& lane, std::vector<Step>& steps) {
             else e.gelu = 1;
         }
         GemmParams p;
-        S3B_OK(conv_params(p, w->act[i - 1], m->conv_w[i], B, lane.L[i - 1], lane.L[i], 2, C, C, kConvK[i], 0, sch, e));
+        S3B_OK(conv_params(p, w->act[i - 1], m->conv_w[i], B, lane.L[i - 1], lane.L[i], 2, C, C, C, kConvK[i], 0, sch, e));
         const size_t rows = (size_t)B * lane.L[i];
         steps.push_back([=](Fwd& f) {
             S3B_OK(run_gemm(f, p));
@@ -2083,14 +2188,14 @@ static int add_npc_stack(const Lane& lane, std::vector<Step>& steps) {
         const LayerW& L = m->layers[i];
         const bool first = i == 0;
         GemmParams conv, lin, mc;
-        S3B_OK(conv_params(conv, first ? w->ln512_s : w->x_s, L.fc1, B, T, T, 1, first ? 80 : H, first ? kDecoar2K : H,
+        S3B_OK(conv_params(conv, first ? w->ln512_s : w->x_s, L.fc1, B, T, T, 1, H, first ? 80 : H, first ? kDecoar2K : H,
                            3, 0, sch, epi_planes(w->h_s.planes(sch), L.fc1_b.as<float>(), act)));
         Epi el = epi_f32(nullptr, L.fc2_b.as<float>());
         el.op = w->x_s.planes(sch), el.gelu = act, el.res_first = 1;
-        S3B_OK(conv_params(lin, w->h_s, L.fc2, B, T, T, 1, H, H, 1, 0, sch, el));
+        S3B_OK(conv_params(lin, w->h_s, L.fc2, B, T, T, 1, H, H, H, 1, 0, sch, el));
         Epi em = epi_f32(nullptr, L.out_b.as<float>());
         em.gelu = 4;
-        S3B_OK(conv_params(mc, w->x_s, L.out, B, T, T, 1, H, H, c.kernel_size, npc_mask_width(c, i), sch, em));
+        S3B_OK(conv_params(mc, w->x_s, L.out, B, T, T, 1, H, H, H, c.kernel_size, npc_mask_width(c, i), sch, em));
         const bool residual = c.residual && !first;
         steps.push_back([=](Fwd& f) { return run_gemm(f, conv); });
         steps.push_back([=](Fwd& f) {
@@ -2113,6 +2218,61 @@ static int add_npc_stack(const Lane& lane, std::vector<Step>& steps) {
     return 0;
 }
 
+// Modified CPC (cpc/expert.py, model.py): the padded waveforms into conv 0 + ChannelNorm + ReLU, written straight into
+// conv 1's padded operand layout; conv 1..4 as implicit GEMMs (fp32 + bias) each followed by ChannelNorm + ReLU into
+// the next conv's padded layout, conv 4's into hidden state 0 and the dense operand planes of the LSTM. Per LSTM layer
+// the input GEMM x_g = x W_ih^T + (b_ih + b_hh), fp32 [M][1024], then the recurrence over all T frames of every
+// utterance (the reference runs the padded batch unpacked): the last layer writes hidden state 1, the others the next
+// layer's operand planes. Frames near and beyond an utterance's end hold the response to the zero samples, as in the
+// reference.
+static int add_cpc_stack(const Lane& lane, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    Workspace* w = lane.w;
+    const int B = lane.B, T = lane.T, C = kCpcDim, NL = m->cfg.num_layers, sch = m->scheme;
+    const int64_t M = lane.M;
+    steps.push_back([=](Fwd& f) {
+        S3B_OK(copy_book(lane, f.st));
+        KMISC(m, f.st, launch_wav_pack(lane.d_wavs, lane.d_lens, B, lane.Lmax, 0, nullptr, w->wav_pad.as<float>(), f.st));
+        KLAUNCH(m, f.st, CAT_CONV0, 1, 2.0 * 10 * C * (double)B * lane.L[0],
+                launch_cpc_conv0(w->wav_pad.as<float>(), B, lane.Lmax, (int)lane.L[0], m->conv0_w.as<float>(),
+                                 m->conv0_b.as<float>(), m->norm0_g.as<float>(), m->norm0_b.as<float>(),
+                                 (int)cpc_rows(lane.L[1], 1), kCpcPad[1], w->act[0].planes(sch), f.st));
+        return 0;
+    });
+    for (int i = 1; i < kCpcConvs; ++i) {
+        const bool last = i == kCpcConvs - 1;
+        GemmParams p;
+        S3B_OK(conv_params(p, w->act[i - 1], m->conv_w[i], B, cpc_rows(lane.L[i], i), lane.L[i], kCpcStride[i], C, C, C,
+                           2 * kCpcStride[i], 0, sch, epi_f32(w->conv_f32.as<float>(), m->conv_b[i].as<float>())));
+        const int Tout = (int)lane.L[i];
+        const int R = last ? Tout : (int)cpc_rows(lane.L[i + 1], i + 1), pad = last ? 0 : kCpcPad[i + 1];
+        const OutPlanes op = last ? w->x_s.planes(sch) : w->act[i].planes(sch);
+        steps.push_back([=](Fwd& f) {
+            S3B_OK(run_gemm(f, p));
+            KNORM(m, f.st, launch_channelnorm_relu(w->conv_f32.as<float>(), B, Tout, R, pad, m->conv_ln_g[i].as<float>(),
+                                                   m->conv_ln_b[i].as<float>(), last ? f.slot(0) : nullptr, op, f.st));
+            return last ? f.done(0) : 0;
+        });
+    }
+    for (int l = 0; l < NL; ++l) {
+        const bool last = l == NL - 1;
+        const LayerW& W = m->layers[l];
+        GemmParams in;
+        S3B_OK(lane.linear(in, w->x_s, W.wih, 4 * C, C, epi_f32(w->xg_f32.as<float>(), W.gru_b.as<float>())));
+        steps.push_back([=](Fwd& f) { return run_gemm(f, in); });
+        CpcLstmParams g;
+        g.xg = w->xg_f32.as<float>(), g.whh = W.whh.as<float>(), g.B = B, g.T = T;
+        g.out = nullptr, g.op = last ? no_planes() : w->x_s.planes(sch);
+        steps.push_back([=](Fwd& f) {
+            CpcLstmParams q = g;
+            if (last) q.out = f.slot(1);
+            KLAUNCH(m, f.st, CAT_GRU, 1, 8.0 * C * C * (double)M, launch_cpc_lstm(q, f.st));
+            return last ? f.done(1) : 0;
+        });
+    }
+    return 0;
+}
+
 // One lane's forward at the lane's shape, in enqueue order
 static int build_steps(const Lane& lane, std::vector<Step>& steps) {
     const s3b_model* m = lane.m;
@@ -2127,6 +2287,7 @@ static int build_steps(const Lane& lane, std::vector<Step>& steps) {
     case kNpcStack:
         S3B_OK(add_fbank_frontend(lane, steps));
         return add_npc_stack(lane, steps);
+    case kCpcStack: return add_cpc_stack(lane, steps);
     case kFbankEncoder:
         S3B_OK(add_fbank_frontend(lane, steps));
         // six empty steps where the conv stack would be: with two lanes they keep lane 1's steps enqueued next to the
@@ -2253,6 +2414,8 @@ extern "C" int s3b_forward_ex(s3b_model* m, const float* const* wavs, const int6
             m->kind == kGruStack    ? "an APC model is a GRU stack, it has no feed-forward blocks or layer results"
             : m->kind == kLstmStack ? "a DeCoAR model is an LSTM stack, it has no feed-forward blocks or layer results"
             : m->kind == kNpcStack  ? "an NPC model is a conv stack, it has no feed-forward blocks or layer results"
+            : m->kind == kCpcStack  ? "a modified CPC model is a conv stack and an LSTM, it has no feed-forward blocks or "
+                                      "layer results"
             : m->cfg.conformer      ? "a Conformer encoder collects no layer results (wav2vec2_model.py:3199-3200)"
                                     : nullptr;
         if (why != nullptr) return fail("ffn_out / last_residual: %s", why);
@@ -2678,7 +2841,7 @@ extern "C" int s3b_conv_gemm_f32(const float* x, const float* w, const float* bi
         e.op = os.planes(out_fmt);
     }
     GemmParams p;
-    S3B_OK(conv_params(p, xs, ws, B, Lin, Lout, 2, C, C, kw, 0, sch, e));
+    S3B_OK(conv_params(p, xs, ws, B, Lin, Lout, 2, C, C, C, kw, 0, sch, e));
     CUDA_OK(launch_gemm(p, sms, st));
     if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), (size_t)B * Lout * C, out, st));
     CUDA_OK(cudaStreamSynchronize(st));
@@ -2782,9 +2945,88 @@ extern "C" int s3b_npc_conv_f32(const float* x, int32_t B, int32_t T, int32_t c_
     Epi e = epi_f32(out, bias, residual);
     e.gelu = act == 0 ? 0 : act == 1 ? 3 : 4, e.res_first = res_first;
     GemmParams p;
-    S3B_OK(conv_params(p, xs, ws, B, T, T, 1, c_in, Cp, k, mask, sch, e));
+    S3B_OK(conv_params(p, xs, ws, B, T, T, 1, N, c_in, Cp, k, mask, sch, e));
     p.out_pre = out_pre;
     CUDA_OK(launch_gemm(p, sms, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+extern "C" int s3b_cpc_conv_f32(const float* x, int32_t B, int32_t L, int32_t layer, const float* w, const float* bias,
+                                const float* gamma, const float* beta, int32_t scheme, float* out, void* stream) {
+    if (!x || !w || !bias || !gamma || !beta || !out) return fail("null argument");
+    if (layer < 0 || layer >= kCpcConvs) return fail("layer %d: must be 0..%d", layer, kCpcConvs - 1);
+    if (B < 1 || L < 1) return fail("bad sizes (batch %d, length %d)", B, L);
+    const int C = kCpcDim, s = kCpcStride[layer], k = 2 * s;
+    const int64_t Tout = cpc_conv_len(L, layer);
+    if (Tout < 1) return fail("length %d too short for conv %d (kernel %d, padding %d)", L, layer, k, kCpcPad[layer]);
+    if ((int64_t)B * cpc_rows(Tout, layer) > 2000000000LL) return fail("batch too large for 32-bit indexing");
+    if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
+    int sch = 0;
+    S3B_OK(resolve_scheme(scheme, k * C, C, &sch));
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t M = (size_t)B * Tout;
+    SplitBuf os;
+    S3B_OK(os.ensure(M * C));
+    if (layer == 0) {
+        // conv 0 writes operand planes only (in the model: conv 1's); here the dense layout, decoded back to fp32
+        CUDA_OK(launch_cpc_conv0(x, B, L, (int)Tout, w, bias, gamma, beta, (int)Tout, 0, os.planes(sch), st));
+        CUDA_OK(launch_planes_to_f32(os.planes(sch), M * C, out, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+        return 0;
+    }
+    // x [B][L][256] into the padded layout the model's producers write: pad zero rows, the frames that fit, zero rows
+    const int64_t R = cpc_rows(Tout, layer), pad = kCpcPad[layer], n = std::min<int64_t>(L, R - pad);
+    int sms = 0;
+    S3B_OK(device_sm_count(&sms));
+    std::vector<float> wh;
+    S3B_OK(download_f32(w, (size_t)C * C * k, st, wh));
+    const std::vector<float> wl = tap_weight_layout(wh.data(), C, C, k, 0, C);
+    SplitBuf xs, ws;
+    S3B_OK(upload_split(ws, wl.data(), wl.size(), sch));
+    DevBuf xpad, z;
+    S3B_OK(xpad.ensure((size_t)B * R * C * 4));
+    CUDA_OK(cudaMemsetAsync(xpad.p, 0, (size_t)B * R * C * 4, st));
+    CUDA_OK(cudaMemcpy2DAsync(xpad.as<float>() + pad * C, (size_t)R * C * 4, x, (size_t)L * C * 4, (size_t)n * C * 4, B,
+                              cudaMemcpyDeviceToDevice, st));
+    S3B_OK(split_operand(xpad.as<float>(), xs, (size_t)B * R * C, sch, 0, st));
+    S3B_OK(z.ensure(M * C * 4));
+    GemmParams p;
+    S3B_OK(conv_params(p, xs, ws, B, R, Tout, s, C, C, C, k, 0, sch, epi_f32(z.as<float>(), bias)));
+    CUDA_OK(launch_gemm(p, sms, st));
+    CUDA_OK(launch_channelnorm_relu(z.as<float>(), B, (int)Tout, (int)Tout, 0, gamma, beta, out, os.planes(sch), st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+extern "C" int s3b_cpc_lstm_max_active_clusters(int32_t* out) {
+    if (!out) return fail("null argument");
+    if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
+    int n = 0;
+    CUDA_OK(cpc_lstm_max_active_clusters(&n));
+    *out = n;
+    return 0;
+}
+
+extern "C" int s3b_cpc_lstm_f32(const float* xg, const float* whh, int32_t B, int32_t T, int32_t out_fmt, float* out,
+                                float* planes_out, void* stream) {
+    // add_cpc_stack's recurrence on this call's buffers
+    if (!xg || !whh || !out) return fail("null argument");
+    if (B < 1 || T < 1) return fail("bad sizes (batch %d, t %d)", B, T);
+    if (out_fmt < -1 || out_fmt > 1) return fail("out_fmt must be -1 (none), 0 (bf16 hi/lo) or 1 (f16q8), not %d", out_fmt);
+    if (out_fmt >= 0 && planes_out == nullptr) return fail("out_fmt %d needs planes_out", out_fmt);
+    if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t M = (size_t)B * T;
+    SplitBuf os;
+    CpcLstmParams g;
+    g.xg = xg, g.whh = whh, g.B = B, g.T = T, g.out = out, g.op = no_planes();
+    if (out_fmt >= 0) {
+        S3B_OK(os.ensure(M * kCpcDim));
+        g.op = os.planes(out_fmt);
+    }
+    CUDA_OK(launch_cpc_lstm(g, st));
+    if (out_fmt >= 0) CUDA_OK(launch_planes_to_f32(g.op, M * kCpcDim, planes_out, st));
     CUDA_OK(cudaStreamSynchronize(st));
     return 0;
 }

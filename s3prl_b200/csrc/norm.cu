@@ -70,6 +70,69 @@ cudaError_t launch_layernorm(const float* x, size_t M, int D, const float* gamma
 }
 
 // ------------------------------------------------------------------------------------------------
+// modified CPC's ChannelNorm + ReLU after conv 1..4 (s3prl/upstream/cpc/model.py): per frame over the 256 channels,
+//   y = relu((x - mean) * rsqrt(var + 1e-5) * gamma + beta),  var unbiased (divided by 255)
+// x: [B][T][256] fp32 (the conv GEMM's output). Output rows follow the next conv's padded operand layout: utterance b
+// owns rows [b R, b R + R), and row r holds frame r - pad when that is in [0, T), zeros otherwise; every row is
+// written. R = T, pad = 0 is the dense layout, the only one with an fp32 copy (out_f32 [B][T][256], may be null).
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) channelnorm_relu_kernel(const float* __restrict__ x, int B, int T, int R,
+                                                               int pad, const float* __restrict__ gamma,
+                                                               const float* __restrict__ beta, float* out_f32,
+                                                               const OutPlanes op) {
+    constexpr int D = 256, V4 = D / 128;
+    const int lane = threadIdx.x & 31;
+    const size_t row = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= (size_t)B * R) return;
+    const int b = (int)(row / R), t = (int)(row - (size_t)b * R) - pad;
+    float4 y[V4];
+    if (t < 0 || t >= T) {
+#pragma unroll
+        for (int i = 0; i < V4; ++i) y[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    } else {
+        const size_t src = (size_t)b * T + t;
+        const float4* xr = reinterpret_cast<const float4*>(x + src * D);
+        float4 v[V4];
+        float s = 0.f;
+#pragma unroll
+        for (int i = 0; i < V4; ++i) {
+            v[i] = xr[lane + 32 * i];
+            s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
+        }
+        const float mean = warp_sum(s) * (1.0f / D);
+        float q = 0.f;
+#pragma unroll
+        for (int i = 0; i < V4; ++i) {
+            const float a = v[i].x - mean, bb = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
+            q += (a * a + bb * bb) + (c * c + d * d);
+        }
+        const float rstd = rsqrtf(warp_sum(q) * (1.0f / (D - 1)) + 1e-5f);
+#pragma unroll
+        for (int i = 0; i < V4; ++i) {
+            const int c4 = lane + 32 * i;
+            const float4 g = __ldg(reinterpret_cast<const float4*>(gamma) + c4);
+            const float4 be = __ldg(reinterpret_cast<const float4*>(beta) + c4);
+            y[i].x = relu_nan((v[i].x - mean) * rstd * g.x + be.x);
+            y[i].y = relu_nan((v[i].y - mean) * rstd * g.y + be.y);
+            y[i].z = relu_nan((v[i].z - mean) * rstd * g.z + be.z);
+            y[i].w = relu_nan((v[i].w - mean) * rstd * g.w + be.w);
+            if (out_f32 != nullptr) reinterpret_cast<float4*>(out_f32 + src * D)[c4] = y[i];
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < V4; ++i) store_planes4(op, y[i], row * D + 4 * (size_t)(lane + 32 * i));
+}
+
+cudaError_t launch_channelnorm_relu(const float* x, int B, int T, int R, int pad, const float* gamma,
+                                    const float* beta, float* out_f32, const OutPlanes& op, cudaStream_t s) {
+    const size_t rows = (size_t)B * R;
+    if (rows == 0) return cudaSuccess;
+    if (op.hi == nullptr || (out_f32 != nullptr && (R != T || pad != 0))) return cudaErrorInvalidValue;
+    channelnorm_relu_kernel<<<(unsigned)((rows + 7) / 8), 256, 0, s>>>(x, B, T, R, pad, gamma, beta, out_f32, op);
+    return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------
 // Conformer attention input (wav2vec2_model.py:255-310, 541): y = self_attn_layer_norm(x) and its rotary embedding
 //   rope(y)_t = y_t * cos_t + rotate_half(y_t) * sin_t,  rotate_half(u) = cat(-u[32:], u[:32]) per 64-wide head,
 // t = frame index in the padded batch (row % T). y feeds linear_v, rope(y) linear_q / linear_k; both are written as

@@ -17,6 +17,7 @@ from typing import Callable, Dict, List, Optional
 
 from .upstream.apc import ApcExpert
 from .upstream.configs import ALIASES, ARCHS
+from .upstream.cpc import CpcExpert
 from .upstream.decoar import DecoarExpert
 from .upstream.decoar2 import Decoar2Expert
 from .upstream.expert import UpstreamExpert
@@ -78,6 +79,9 @@ for _family, _all in (("decoar", False), ("decoar_layers", True)):
 for _name, _required in (("npc", False), ("npc_360hr", False), ("npc_960hr", False), ("npc_local", True),
                          ("npc_url", True)):
     ENTRIES[_name] = _entry(_name, partial(NpcExpert, name=_name), ckpt_required=_required)
+# modified CPC (cpc/hubconf.py): the fabricated checkpoint without ckpt, else the local {"config", "weights"} file
+for _name, _required in (("modified_cpc", False), ("cpc_local", True), ("cpc_url", True)):
+    ENTRIES[_name] = _entry(_name, partial(CpcExpert, name=_name), ckpt_required=_required)
 globals().update(ENTRIES)
 
 

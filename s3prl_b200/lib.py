@@ -26,6 +26,7 @@ EXPORTED_SYMBOLS = [
     "s3b_apc_model_create",
     "s3b_decoar_model_create",
     "s3b_npc_model_create",
+    "s3b_cpc_model_create",
     "s3b_num_frames",
     "s3b_valid_frames",
     "s3b_num_outputs",
@@ -67,6 +68,9 @@ EXPORTED_SYMBOLS = [
     "s3b_lstm_f32",
     "s3b_lstm_fits",
     "s3b_npc_conv_f32",
+    "s3b_cpc_conv_f32",
+    "s3b_cpc_lstm_f32",
+    "s3b_cpc_lstm_max_active_clusters",
     "s3b_layernorm_rope_f32",
     "s3b_fbank",
     "s3b_fbank_ex",
@@ -160,6 +164,21 @@ class S3BNpcConfig(C.Structure):
     def __init__(self, **kw):
         super().__init__(**kw)
         self.struct_size = C.sizeof(S3BNpcConfig)
+
+
+class S3BCpcConfig(C.Structure):
+    """Mirror of ``struct s3b_cpc_config``."""
+
+    _fields_ = [
+        ("struct_size", C.c_int32),
+        ("hidden", C.c_int32),
+        ("num_layers", C.c_int32),
+        ("reserved", C.c_int32 * 4),
+    ]
+
+    def __init__(self, **kw):
+        super().__init__(**kw)
+        self.struct_size = C.sizeof(S3BCpcConfig)
 
 
 class S3BForwardOpts(C.Structure):
@@ -269,6 +288,7 @@ def load() -> C.CDLL:
     lib.s3b_apc_model_create.argtypes = [C.POINTER(S3BApcConfig), C.POINTER(vp)]
     lib.s3b_decoar_model_create.argtypes = [C.POINTER(S3BDecoarConfig), C.POINTER(vp)]
     lib.s3b_npc_model_create.argtypes = [C.POINTER(S3BNpcConfig), C.POINTER(vp)]
+    lib.s3b_cpc_model_create.argtypes = [C.POINTER(S3BCpcConfig), C.POINTER(vp)]
     lib.s3b_model_finalize.argtypes = [vp]
     lib.s3b_model_destroy.argtypes = [vp]
     lib.s3b_model_destroy.restype = None
@@ -319,6 +339,9 @@ def load() -> C.CDLL:
     lib.s3b_gru_max_active_clusters.argtypes = [C.POINTER(i32)]
     lib.s3b_gru_f32.argtypes = [f32p, f32p, f32p, f32p, C.POINTER(i32), i32, i32, i32, i32, f32p, f32p, vp]
     lib.s3b_lstm_fits.argtypes = [C.POINTER(i32)]
+    lib.s3b_cpc_conv_f32.argtypes = [f32p, i32, i32, i32, f32p, f32p, f32p, f32p, i32, f32p, vp]
+    lib.s3b_cpc_lstm_f32.argtypes = [f32p, f32p, i32, i32, i32, f32p, f32p, vp]
+    lib.s3b_cpc_lstm_max_active_clusters.argtypes = [C.POINTER(i32)]
     lib.s3b_npc_conv_f32.argtypes = [f32p, i32, i32, i32, f32p, i32, i32, f32p, f32p, i32, i32, i32, f32p, f32p, vp]
     lib.s3b_lstm_f32.argtypes = [f32p, f32p, f32p, C.POINTER(i32), i32, i32, i32, i32, f32p, f32p, vp]
     lib.s3b_layernorm_rope_f32.argtypes = [f32p, i64, i32, i32, f32p, f32p, C.POINTER(C.c_float), i32, f32p, f32p, vp]

@@ -117,6 +117,7 @@ class NativeExpert(nn.Module):
     shared across ranks."""
 
     min_samples = 0  # per-utterance minimum length (0: none beyond the library's own rules)
+    min_batch_samples = 400  # the shortest padded batch the front end makes one frame of
     model_label = ""  # the model's name in the minimum-length message
 
     def __init__(self, state_dict: Dict[str, torch.Tensor]):
@@ -157,7 +158,8 @@ class NativeExpert(nn.Module):
         max_len = self.global_max_len or max(lens)
         T = self.num_frames(max_len)
         if T < 1:
-            raise ValueError(f"waveforms too short ({max_len} samples): the front end needs >= 400 samples")
+            raise ValueError(f"waveforms too short ({max_len} samples): the front end needs >= "
+                             f"{self.min_batch_samples} samples")
         return lens, max_len, T
 
     def _prepare(self, wavs: List[torch.Tensor]):
