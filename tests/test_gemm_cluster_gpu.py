@@ -3,14 +3,19 @@ load each A box once between them (TMA multicast). That changes where the operan
 every output must be bit-identical to the launch without clusters (S3B_GEMM_CLUSTER=1), whatever the cluster size
 (S3B_GEMM_CLUSTER=2 / 4, or the library's own choice with the variable unset).
 
-Cases: the encoder linears of hubert_base and wav2vec2_large and conv 1..6 in both operand schemes; M with a partial
-last row tile; conv batches whose per-utterance row count is not a multiple of 128; n_tiles equal to the cluster size;
-launches with fewer clusters of tiles than clusters that can be resident (M = 1, 129). Outputs start as NaN, so a tile
-that no cluster writes shows as well."""
+Cases: the encoder linears of hubert_base and wav2vec2_large, conv 1..6, NPC's tap convolutions (masked ones too) and
+modified CPC's conv 1 and 4 (N = 256) in both operand schemes; M with a partial last row tile; conv batches whose
+per-utterance row count is not a multiple of 128; n_tiles equal to the cluster size; launches with fewer clusters of
+tiles than clusters that can be resident (M = 1, 129). Outputs start as NaN, so a tile that no cluster writes shows as
+well."""
 import pytest
 import torch
 
+import cpc_oracle as CO
+from test_cpc_gpu import _cpc_conv
 from test_gemm_layouts_gpu import _conv, _linear
+from test_npc_gpu import _conv_inputs as _npc_inputs
+from test_npc_gpu import _npc_conv
 
 pytestmark = pytest.mark.gpu
 
@@ -81,3 +86,31 @@ def test_conv_clusters_bit_identical(s3b_lib, monkeypatch, scheme, kw, Lout):
     for out_fmt in (-1, scheme):
         _assert_identical(f"conv s{scheme} kw={kw} Lout={Lout} fmt={out_fmt}",
                           _runs(monkeypatch, lambda: _conv(x, w, bias, Lin, kw, True, scheme, out_fmt)))
+
+
+@pytest.mark.parametrize("T", [129, 999])
+@pytest.mark.parametrize("cin,k,mask", [(80, 3, 0), (512, 3, 0), (512, 1, 0), (512, 15, 7), (512, 15, 13)])
+@pytest.mark.parametrize("scheme", [0, 1])
+def test_npc_conv_clusters_bit_identical(s3b_lib, monkeypatch, scheme, cin, k, mask, T):
+    """NPC's same-padded tap convolutions (N = 512: four 128-wide tiles) over three utterances, with the masked
+    convs' skip over the band (a_gap), tanh and a residual added after it, as its blocks run them."""
+    x, w, bias, res = _npc_inputs(T, cin, k, mask, "unit", T + cin + k + mask + scheme)
+    _assert_identical(f"npc conv s{scheme} c_in={cin} k={k} mask={mask} T={T}",
+                      _runs(monkeypatch, lambda: _npc_conv(s3b_lib, x, w, k, mask, bias, res, 2, 0, scheme)[0]))
+
+
+@pytest.mark.parametrize("T", [129, 999])
+@pytest.mark.parametrize("layer", [1, 4])
+@pytest.mark.parametrize("scheme", [0, 1])
+def test_cpc_conv_clusters_bit_identical(s3b_lib, monkeypatch, scheme, layer, T):
+    """Modified CPC's strided conv 1 (k 8, stride 4) and conv 4 (k 4, stride 2) on the padded row layout, N = 256: two
+    128-wide tiles, which f16q8 runs as a cluster of 2; then the ChannelNorm."""
+    s, p = CO.STRIDES[layer], CO.PADDINGS[layer]
+    L = s * (T - 1) + 2 * s - 2 * p + s - 1
+    g = torch.Generator(device="cuda").manual_seed(T + layer + scheme)
+    x = torch.relu(torch.randn(3, L, 256, device="cuda", generator=g))
+    w = torch.randn(256, 256, 2 * s, device="cuda", generator=g) / (512 * s) ** 0.5
+    bias, gamma, beta = (0.1 * torch.randn(256, device="cuda", generator=g),
+                         0.5 + torch.rand(256, device="cuda", generator=g), 0.2 * torch.randn(256, device="cuda", generator=g))
+    _assert_identical(f"cpc conv {layer} s{scheme} T={T}",
+                      _runs(monkeypatch, lambda: _cpc_conv(s3b_lib, x, layer, w, bias, gamma, beta, scheme)))

@@ -1,9 +1,11 @@
-"""GPU tests of NPC (``npc``): the tap convolution at block level (``s3b_npc_conv_f32``) against fp64 ``conv1d`` in both
-GEMM operand schemes, the band of masked taps left out bit-exactly, the whole model against the executed-reference
+"""GPU tests of NPC (``npc``): the tap convolution at block level (``s3b_npc_conv_f32``) in both GEMM operand schemes,
+per element against fp64 ``conv1d`` and against the scheme's emulated operand decomposition, the band of masked taps
+left out bit-exactly, the neighbouring utterances of a batch never read, the whole model against the executed-reference
 goldens (tests/golden/npc_ref*.pt) and the fp64 CPU oracle (tests/npc_oracle.py), bit-identical results across batch
 composition, shards, lanes, ``forward_host``, repeated calls and a long-lived model, the launch counts, and the
 library's refusal of a checkpoint whose conv_mask is not its config's.
-Bounds: block 1e-4 relative Frobenius; model 2e-4 relative per hidden state. Every check prints measured / bound."""
+Bounds: block per element, derived from the operands as in tests/test_gemm_layouts_gpu.py (_gemm_refs); model 2e-4
+relative per hidden state. Every check prints measured / bound."""
 import ctypes as C
 import os
 import sys
@@ -18,11 +20,13 @@ GOLDEN = ROOT / "tests" / "golden"
 sys.path.insert(0, str(ROOT / "tests"))
 
 import npc_oracle as NO  # noqa: E402
+from test_gemm_layouts_gpu import _check, _epilogue, _gemm_refs, _operands  # noqa: E402
+from test_port_shapes_gpu import LONG_K, _dropped_steps  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
-BLOCK_REL = 1e-4
 REL_TOL = 2e-4
+TANH_ERR = 2.0**-22  # tanhf: at most 2 ulp of its result
 
 
 def _rel(a, b):
@@ -57,50 +61,121 @@ def _npc_conv(s3b_lib, x, w, k, mask, bias, res, act, res_first, scheme, pre=Fal
     return out, out_pre
 
 
-def _conv_ref(x, w, k, mask, bias, res, act, res_first):
-    """fp64 conv1d with the centred band of `mask` taps zeroed, then the epilogue in either order"""
-    w = w.double().clone()
-    if mask:
-        head = (k - mask) // 2
-        w[:, :, head:head + mask] = 0
-    y = F.conv1d(x.double().transpose(1, 2), w, bias.double() if bias is not None else None,
-                 padding=(k - 1) // 2).transpose(1, 2)
-    f = {0: lambda v: v, 1: torch.relu, 2: torch.tanh}[act]
+def _unmasked_taps(k, mask):
+    head = (k - mask) // 2
+    return [j for j in range(k) if not head <= j < head + mask]
+
+
+def _im2col(x, w, k, mask):
+    """The GEMM the kernel runs, as fp32 matrices: row (b, t) of A is the unmasked taps x[b, t + j - (k - 1) / 2], zero
+    outside [0, T), tap-major; W [512][u c_in] the same taps of w. Also which rows read a frame inside [0, T) for every
+    tap (interior) and for none (empty: the output is act(bias) there)."""
+    B, T, cin = x.shape
+    taps = torch.tensor(_unmasked_taps(k, mask), device="cuda")
+    h = (k - 1) // 2
+    xp = F.pad(x, (0, 0, h, h))  # [B][T + k - 1][cin]
+    idx = torch.arange(T, device="cuda")[:, None] + taps[None, :]  # padded frame of tap jj of output t
+    a = xp[:, idx, :].reshape(B * T, len(taps) * cin)
+    wk = w[:, :, taps].permute(0, 2, 1).reshape(512, len(taps) * cin)
+    inside = ((idx - h >= 0) & (idx - h < T)).repeat(B, 1)
+    return a, wk, inside.all(1), ~inside.any(1)
+
+
+def _separation(what, a, w, e1, e2, interior, scheme):
+    """The bounds' separation for _check. _gemm_refs counts every 16-wide k-step of K in the accumulation bound; rows
+    with taps outside the utterance run fewer MMAs on non-zero operands, so their bounds are closer than the kernel's
+    accumulation is, and the separation is taken over the interior rows (none: not checked). Where it is under 50x for
+    f16q8 at K >= 5120 (tests/test_port_shapes_gpu.py), _dropped_steps checks what it stands for instead.
+    Returns (gemm, apart_check) for _check."""
+    if not interior.any():
+        return (e1, e2), False
+    gemm = (e1[interior], e2[interior])
+    if scheme == 1 and a.shape[1] >= LONG_K and (gemm[0] / gemm[1]).median().item() < 50.0:
+        _dropped_steps(what, a[interior], w, gemm[1])
+        return gemm, False
+    return gemm, True
+
+
+def _act_epilogue(pre, e, bias, res, act, res_first):
+    """fp64 epilogue of the NPC conv: v = pre + bias (+ residual if res_first); act; out_pre; (+ residual) and the
+    propagated bounds (_epilogue: the fp32 bias and residual adds). ReLU is 1-Lipschitz and exact in fp32; tanh has
+    slope <= 1, and tanhf adds at most 2 ulp (CUDA's documented maximum), bounded by TANH_ERR |tanh(v)|.
+    Returns (out, bound, out_pre, bound_pre)."""
+    v, ev = _epilogue(pre, e, bias, res=res if res_first else None)
+    if act == 1:
+        v = torch.relu(v)
+    elif act == 2:
+        v = torch.tanh(v)
+        ev = ev + TANH_ERR * v.abs()
     if res_first:
-        return f(y + res.double() if res is not None else y), None
-    pre = f(y)
-    return (pre + res.double() if res is not None else pre), pre
+        return v, ev, None, None
+    out = v + res.double()
+    return out, ev + 2.0**-24 * out.abs(), v, ev
 
 
 # (c_in, k, mask): the served config's shapes — conv k = 3 on 80 and 512 channels, the 1x1 linear, the masked convs of
 # kernel 15 / mask 5 (bands of 7, 9, 11, 13 taps) — and a kernel without a mask
 _SHAPES = [(80, 3, 0), (512, 3, 0), (512, 1, 0), (512, 15, 7), (512, 15, 9), (512, 15, 11), (512, 15, 13),
            (512, 15, 0), (80, 9, 3)]
-_T = [1, 2, 127, 128, 998]
+_T = [1, 2, 7, 8, 127, 128, 129, 998]
+_UTT_SCALES = (1.0, 0.25, 0.5)  # per utterance of a batch of 3: a row read from the wrong utterance shows
+
+
+def _conv_inputs(T, cin, k, mask, mag, seed):
+    """x [3][T][c_in], w [512][c_in][k] at _operands' magnitudes (unit: w ~ 1 / sqrt(u c_in), the taps contracted;
+    small: x 1e-3 of that, the f16q8 residuals in e4m3's subnormals; large: |x| up to 3000, |w| up to 40, where A_h8
+    and W_h8 saturate, standing in for BatchNorm-folded weights and activations past fp8's range), the utterances at
+    different scales; bias and residual at the scale of the convolution's output."""
+    B, u = 3, k - mask
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    a, wr = _operands(B * T, 512 * k, cin, mag, g)  # x rows; one weight row per (tap, output channel)
+    x = a.view(B, T, cin) * torch.tensor(_UTT_SCALES, device="cuda")[:, None, None]
+    w = wr.view(k, 512, cin).permute(1, 2, 0).contiguous()
+    if mag != "large":
+        w = w / u**0.5  # _operands scales by 1 / sqrt(c_in); the conv contracts u taps of c_in
+    y = 1.0 if mag == "unit" else 1e-3**2 if mag == "small" else 700 * 10 * (u * cin) ** 0.5
+    bias = torch.randn(512, device="cuda", generator=g) * 0.1 * y
+    res = torch.randn(B, T, 512, device="cuda", generator=g) * y
+    return x, w, bias, res
 
 
 @pytest.mark.parametrize("scheme", [0, 1])
 @pytest.mark.parametrize("cin,k,mask", _SHAPES)
 def test_npc_conv_block_matches_fp64(s3b_lib, scheme, cin, k, mask):
-    worst = 0.0
-    for T in _T:
-        g = torch.Generator().manual_seed(T * 31 + k * 7 + mask + cin)
-        B = 3 if T < 998 else 2
-        x = torch.randn(B, T, cin, generator=g).cuda()
-        w = (torch.randn(512, cin, k, generator=g) / (cin * max(k - mask, 1)) ** 0.5).cuda()
-        bias = (0.1 * torch.randn(512, generator=g)).cuda()
-        res = torch.randn(B, T, 512, generator=g).cuda()
+    """The same-padded tap convolution of three utterances against two references per element (the module's bounds):
+    the exact product in fp64, and the scheme's operand decomposition emulated in torch. Both run on the im2col view
+    of the GEMM the kernel runs (_im2col), which must itself equal F.conv1d in fp64 with the band of masked taps
+    zeroed. Epilogue: activation none, ReLU or tanh, with the residual added after the activation (out_pre checked
+    too: the value before the add) or before it (res_first). At k = 15 and T <= 7 some frames have every unmasked tap
+    outside the utterance: there the output is act(bias) exactly (act(bias + residual) with res_first)."""
+    for mag, T in [(m, t) for m in ("unit", "small", "large") for t in _T]:
+        what = f"npc conv c_in={cin} k={k} mask={mask} s{scheme} {mag} T={T}"
+        x, w, bias, res = _conv_inputs(T, cin, k, mask, mag, T * 31 + k * 7 + mask + cin + 1000 * scheme + len(mag))
+        a, wk, interior, empty = _im2col(x, w, k, mask)
+        exact, emu, e1, e2 = _gemm_refs(a, wk, scheme)
+        wm = w.double().clone()
+        if mask:
+            wm[:, :, (k - mask) // 2 : (k + mask) // 2] = 0
+        conv = F.conv1d(x.double().transpose(1, 2), wm, padding=(k - 1) // 2).transpose(1, 2).reshape(-1, 512)
+        assert ((conv - exact).abs() <= 1e-6 * e1).all()  # the im2col view is the convolution (to fp64 rounding)
+        gemm, apart_check = _separation(what, a, wk, e1, e2, interior, scheme)
+        r = res.view(-1, 512)
         for act in (0, 1, 2):
-            for res_first, r, pre in ((0, None, False), (0, res, True), (1, res, False), (0, res, False)):
-                out, out_pre = _npc_conv(s3b_lib, x, w, k, mask, bias, r, act, res_first, scheme, pre)
-                ref, ref_pre = _conv_ref(x, w, k, mask, bias, r, act, res_first)
-                e = _rel(out, ref)
-                if pre:
-                    e = max(e, _rel(out_pre, ref_pre))
-                worst = max(worst, e)
-                assert e < BLOCK_REL, (T, act, res_first, pre, e)
-    print(f"npc conv c_in={cin} k={k} mask={mask} scheme={scheme}: worst relative error over T={_T}, 3 activations, "
-          f"both orders, residual and out_pre: {worst:.3e} (measured/bound {worst / BLOCK_REL:.3f})")
+            for res_first in (0, 1):
+                out, out_pre = _npc_conv(s3b_lib, x, w, k, mask, bias, res, act, res_first, scheme, pre=not res_first)
+                out, tag = out.view(-1, 512), f"{what} act={act} res_first={res_first}"
+                ref1, b1, pre1, bp1 = _act_epilogue(conv, e1, bias, r, act, res_first)
+                ref2, b2, pre2, bp2 = _act_epilogue(emu, e2, bias, r, act, res_first)
+                _check(tag, out, ref1, b1, ref2, b2, gemm, scheme, frob=mag == "unit", apart_check=apart_check)
+                if not res_first:
+                    _check(f"{tag} out_pre", out_pre.view(-1, 512), pre1, bp1, pre2, bp2, gemm, scheme,
+                           frob=mag == "unit", apart_check=apart_check)
+                    assert torch.equal(out, out_pre.view(-1, 512) + r), "out != out_pre + residual"
+                if empty.any() and act != 2:  # no tap inside the utterance: the accumulator is exactly zero
+                    v = bias.expand_as(r) + r if res_first else bias.expand_as(r)
+                    v = torch.relu(v) if act == 1 else v
+                    want = v if res_first else v + r
+                    assert torch.equal(out[empty], want[empty]), (tag, "frames without a tap in the utterance")
 
 
 @pytest.mark.parametrize("scheme", [0, 1])
@@ -121,6 +196,22 @@ def test_masked_band_is_left_out_bit_exactly(s3b_lib, scheme):
     assert torch.equal(a[:, t], b[:, t])
     assert not torch.equal(a[:, t + 1], b[:, t + 1])  # one frame on, the band has moved off a rewritten row
     print(f"masked band scheme={scheme}: row {t} bit-identical after rewriting rows {t - r}..{t + r}")
+
+
+@pytest.mark.parametrize("scheme", [0, 1])
+@pytest.mark.parametrize("cin,k,mask,T", [(80, 3, 0, 129), (512, 3, 0, 1), (512, 15, 7, 7), (512, 15, 13, 129),
+                                          (512, 15, 0, 8)])
+def test_neighbours_are_never_read(s3b_lib, cin, k, mask, scheme, T):
+    """Utterance 1 of a batch of 3 whose utterances 0 and 2 are all NaN is bit-identical to utterance 1 run alone: the
+    halo of same padding reaches past both ends of every utterance at these lengths, and must read zeros there."""
+    x, w, bias, res = _conv_inputs(T, cin, k, mask, "unit", T + k + mask + cin + scheme)
+    alone, _ = _npc_conv(s3b_lib, x[1:2].contiguous(), w, k, mask, bias, res[1:2].contiguous(), 2, 0, scheme)
+    x[0], x[2] = float("nan"), float("nan")
+    res[0], res[2] = float("nan"), float("nan")
+    out, _ = _npc_conv(s3b_lib, x, w, k, mask, bias, res, 2, 0, scheme)
+    assert torch.isfinite(alone).all()
+    assert torch.equal(out[1], alone[0])
+    print(f"npc conv c_in={cin} k={k} mask={mask} T={T} s{scheme}: utterance 1 between NaN neighbours bit-identical")
 
 
 def test_npc_conv_refusals(s3b_lib):
