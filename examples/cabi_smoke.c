@@ -136,5 +136,23 @@ int main(void) {
         s3b_model_destroy(m);
         if (valid[0] != 100 || valid[1] != 5) return 16;
     }
+    {
+        /* LightHuBERT small: 384 channels, 16 pos_conv groups of 24, hidden state 0 = post_extract_proj's output; the
+         * HuBERT frame rule */
+        s3b_model* m = NULL;
+        memset(&cfg, 0, sizeof(cfg));
+        cfg.family = 0, cfg.extractor_layer_norm = 1, cfg.normalize_wav = 1, cfg.num_layers = 12, cfg.embed_dim = 384;
+        cfg.ffn_dim = 1536, cfg.num_heads = 6, cfg.pos_conv_kernel = 128, cfg.pos_conv_groups = 16, cfg.proj_hidden0 = 1;
+        if (s3b_model_create(&cfg, &m) != 0) {
+            printf("s3b_model_create (LightHuBERT): %s\n", s3b_last_error());
+            return 17;
+        }
+        if (s3b_valid_frames(m, lens, 2, 16000, valid) != 0 || s3b_num_outputs(m) != 13) {
+            printf("LightHuBERT bookkeeping: %s\n", s3b_last_error());
+            return 18;
+        }
+        s3b_model_destroy(m);
+        if (valid[0] != 49 || valid[1] != 3) return 19;
+    }
     return 0;
 }

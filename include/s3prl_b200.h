@@ -56,7 +56,12 @@ typedef struct s3b_config {
      *    a transformer encoder with pos_conv_depth <= 1; the conv-stack fields (extractor_layer_norm, conv_bias,
      *    normalize_wav, no_feature_layer_norm) must be 0. Utterances need >= 560 samples (2 fbank frames). */
     int32_t frontend;
-    int32_t reserved[2];
+    /* 1: output slot 0 is the post_extract_proj output with its padded frames zeroed (LightHuBERT,
+     * s3prl/upstream/lighthubert/lighthubert.py:687-783: hidden_states[0] is `features`, which the encoder's in-place
+     * index_put zeroes), instead of the encoder's layer-0 input. Needs family 0, a post-LN transformer encoder and
+     * frontend 0. 0: the encoder's layer-0 input, as for every other model of the family. */
+    int32_t proj_hidden0;
+    int32_t reserved[1];
 } s3b_config;
 
 /* Library / error ------------------------------------------------------------------------------ */
@@ -383,7 +388,8 @@ int s3b_qkv_hd_f32(const float* x, const float* w, const float* b, int32_t batch
 int s3b_conv_gemm_f32(const float* x, const float* w, const float* bias, int32_t batch, int64_t lin, int32_t kw,
                       int32_t gelu, int32_t scheme, int32_t out_fmt, float* out, void* stream);
 /* The positional conv as the model runs it (bf16x3): x [batch][t][d], folded weight w [d][d / groups][k], bias [d].
- * d in {512, 768, 1024, 1280, 1920}; d / groups in {16, 32, 48, 64, 80, 120} (80 and 120: taps_per_kblock 1 only).
+ * d in {384, 512, 640, 768, 1024, 1280, 1920}; d / groups in {16, 24, 32, 40, 48, 64, 80, 120} (80 and 120:
+ * taps_per_kblock 1 only; 24 and 40: taps_per_kblock 4 only).
  *  taps_per_kblock 1: one k-block per tap (two above 64 channels per group), bias + GELU + residual in the GEMM epilogue, fp32 (then LayerNorm if gamma:
  *    as in the model, operand planes come only from that LayerNorm, so out_fmt >= 0 needs gamma);
  *  taps_per_kblock 4: four taps per k-block (zero taps appended up to a multiple of 4) + the combine kernel, mode
@@ -422,7 +428,7 @@ int s3b_cpc_lstm_max_active_clusters(int32_t* out);
  * force_un in {0 = the library's choice, 128, 256} forces the tile width (columns per output tile) wherever it divides
  * n. out[0] = ms per launch, out[1] = tile width used. (tools/gemm_shapes.py) */
 int s3b_gemm_bench(int64_t m, int32_t n, int32_t k, int32_t gelu, int32_t force_un, int32_t iters, float* out);
-/* y = LayerNorm_D(x) (eps 1e-5), optional GELU; D in {512,768,1024,1280,1920} */
+/* y = LayerNorm_D(x) (eps 1e-5), optional GELU; D in {384,512,640,768,1024,1280,1920} */
 int s3b_layernorm_f32(const float* x, int64_t m, int32_t d, const float* gamma, const float* beta, int32_t gelu,
                       float* out, void* stream);
 /* softmax(q k^T / 8 + key padding mask) v per (batch, head); q,k,v: [batch][T][heads*64] fp32; valid_frames: host,

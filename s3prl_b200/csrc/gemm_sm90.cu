@@ -285,13 +285,20 @@ __device__ __forceinline__ void store_plane_pair(const GemmParams& p, float x0, 
 // Per-row work (flat row, mask, offsets, QKV's b and t) is done once per row, the bias once per chunk of kCh column
 // pairs for all rows, and every load of a chunk is issued before any of its stores. Mode tests are uniform branches
 // around whole chunks, never per pair.
+// the largest divisor of kJ column pairs that is at most 8
+constexpr int chunk_pairs(int kJ) {
+    for (int c = 8; c > 1; --c)
+        if (kJ % c == 0) return c;
+    return 1;
+}
+
 template <int BN, int kEpi, int kHalves>
 __device__ __forceinline__ void epilogue_tile(const GemmParams& p, float (&acc)[kHalves][BN / 2], int batch,
                                               int row_base, int col0) {
     constexpr int kJ = BN / 8;               // column pairs per row
-    // pairs per chunk: 8, but 2 next to the 128 accumulators of a 256-wide cooperative tile (168 registers at most),
-    // and 5 at the pos_conv's 80- and 120-column tiles
-    constexpr int kCh = BN * kHalves >= 256 && kHalves == 1 ? 2 : (kJ < 8 ? kJ : (kJ % 8 == 0 ? 8 : 5));
+    // pairs per chunk: the largest divisor of kJ up to 8 (5 at the pos_conv's 80-, 120- and 160-column tiles, 6 at
+    // 96), but 2 next to the 128 accumulators of a 256-wide cooperative tile (168 registers at most)
+    constexpr int kCh = BN * kHalves >= 256 && kHalves == 1 ? 2 : chunk_pairs(kJ);
     constexpr int kRows = 2 * kHalves;       // rows per thread
     static_assert(kJ % kCh == 0, "chunking");
     bool ok[kRows];
@@ -687,8 +694,10 @@ cudaError_t launch_gemm(const GemmParams& p, int sm_count, cudaStream_t stream) 
     switch (p.bn) {
         case 256: return launch_n<256>(p, sm_count, stream);
         case 192: return launch_n<192>(p, sm_count, stream);
+        case 160: return launch_n<160>(p, sm_count, stream);
         case 128: return launch_n<128>(p, sm_count, stream);
         case 120: return launch_n<120>(p, sm_count, stream);
+        case 96: return launch_n<96>(p, sm_count, stream);
         case 80: return launch_n<80>(p, sm_count, stream);
         case 64: return launch_n<64>(p, sm_count, stream);
         case 48: return launch_n<48>(p, sm_count, stream);

@@ -28,7 +28,7 @@ cudaError_t launch_cpc_conv0(const float* x, int B, long long L, int T0, const f
                              cudaStream_t s);
 
 // ---- norm.cu -------------------------------------------------------------------------------------
-// y = LayerNorm_D(x) * gamma + beta (eps 1e-5, biased var), optional GELU; D in {512, 768, 1024, 1280, 1920}.
+// y = LayerNorm_D(x) * gamma + beta (eps 1e-5, biased var), optional GELU; D in {384, 512, 640, 768, 1024, 1280, 1920}.
 // Any of out_f32 / (out_hi,out_lo) may be null. x and out_f32 may alias.
 cudaError_t launch_layernorm(const float* x, size_t M, int D, const float* gamma, const float* beta, int gelu,
                              float* out_f32, const OutPlanes& op, cudaStream_t s);

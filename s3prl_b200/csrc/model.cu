@@ -429,9 +429,13 @@ static int default_scheme() {
 }
 
 // attention head widths the kernel is built for (attention.cu), and pos_conv group widths: multiples of 16 up to 64
-// (one 64-wide k-block per tap, or four taps per k-block), 80 and 120 (two k-blocks per tap, one tap per k-block)
+// (one 64-wide k-block per tap, or four taps per k-block), 80 and 120 (two k-blocks per tap, one tap per k-block),
+// 24 and 40 (four taps per k-block only: posconv4_only)
 static bool head_dim_ok(int hd) { return hd == 64 || hd == 80 || hd == 120; }
-static bool posconv_cpg_ok(int cpg) { return (cpg % 16 == 0 && cpg >= 16 && cpg <= 64) || cpg == 80 || cpg == 120; }
+static bool posconv4_only(int cpg) { return cpg == 24 || cpg == 40; }
+static bool posconv_cpg_ok(int cpg) {
+    return (cpg % 16 == 0 && cpg >= 16 && cpg <= 64) || cpg == 80 || cpg == 120 || posconv4_only(cpg);
+}
 static int head_dim(const s3b_config& c) { return c.embed_dim / c.num_heads; }
 
 // ------------------------------------------------------------------------------------------------
@@ -448,8 +452,12 @@ extern "C" int s3b_model_create(const s3b_config* cfg, s3b_model** out) {
         return fail("embed_dim %% pos_conv_groups != 0");
     const int cpg = cfg->embed_dim / cfg->pos_conv_groups;
     if (!posconv_cpg_ok(cpg))
-        return fail("channels per pos_conv group (embed_dim / pos_conv_groups = %d) must be 16, 32, 48, 64, 80 or 120", cpg);
+        return fail("channels per pos_conv group (embed_dim / pos_conv_groups = %d) must be 16, 32, 48, 64, 80 or 120 "
+                    "(or 24 or 40 with four taps per k-block)", cpg);
     if (cfg->pos_conv_depth < 0 || cfg->pos_conv_depth > 8) return fail("pos_conv_depth out of range (0..8)");
+    if (posconv4_only(cpg) && (cfg->pos_conv_depth > 1 || cfg->pos_conv_kernel % 4 != 0))
+        return fail("%d channels per pos_conv group need pos_conv_depth <= 1 and a pos_conv_kernel that is a multiple of 4 "
+                    "(four taps per k-block), not depth %d, kernel %d", cpg, cfg->pos_conv_depth, cfg->pos_conv_kernel);
     if (cfg->pos_conv_depth <= 1 && cfg->pos_conv_kernel % 2 != 0) return fail("pos_conv_kernel must be even");
     if (cfg->pos_conv_depth > 1 && (cfg->pos_conv_kernel < 3 || (4 * cpg != 192 && 4 * cpg != 256)))
         return fail("pos_conv_depth > 1 needs 48 or 64 channels per group");
@@ -477,6 +485,10 @@ extern "C" int s3b_model_create(const s3b_config* cfg, s3b_model** out) {
     } else if (cfg->depthwise_kernel != 0) {
         return fail("depthwise_kernel is a Conformer field (conformer = 0)");
     }
+    if (cfg->proj_hidden0 != 0 && cfg->proj_hidden0 != 1) return fail("proj_hidden0 must be 0 or 1");
+    if (cfg->proj_hidden0 && (cfg->family != 0 || cfg->conformer || cfg->layer_norm_first || cfg->frontend != 0))
+        return fail("proj_hidden0 = 1 (LightHuBERT) goes with the hubert family (0), a post-LN transformer encoder and the "
+                    "conv stack");
     if (cfg->frontend != 0 && cfg->frontend != 1) return fail("frontend must be 0 (conv stack) or 1 (DeCoAR 2.0 fbank)");
     if (cfg->frontend == 1) {
         // DeCoAR 2.0 = fbank features into the wav2vec 2.0 TransformerEncoder (decoar2/decoar2.py:27-59)
@@ -752,7 +764,7 @@ static std::vector<float> tap_weight_layout(const T* w, int N, int cin, int k, i
 static int posconv_kc(int cpg) { return (cpg + 63) / 64 * 64; }
 // grouped positional conv, four taps per k-block (tap = 4q + j, posconv4_params), folded weight w [D][cpg][Kp], the
 // tap count rounded up to K4 = a multiple of four with zero taps: [G * 4cpg][K4 / 4 * 64], row g * 4cpg + j * cpg + n,
-// column q * 64 + channel (zero padded to 64); cpg <= 64 (48 or 64 where it runs)
+// column q * 64 + channel (zero padded to 64); cpg <= 64 (24, 40, 48 or 64 where it runs)
 static std::vector<float> posconv4_weight_layout(const float* w, int D, int G, int Kp) {
     const int cpg = D / G, Kq = (Kp + 3) / 4;
     std::vector<float> w4((size_t)D * 4 * Kq * 64, 0.0f);
@@ -1430,13 +1442,14 @@ static int posconv_params(GemmParams& p, const s3b_config& c, const SplitBuf& x,
 // frame, so the one-tap formulation (N = cpg = 48 columns) is bound by the shared-memory reads of its A operand
 // (4 KB per 24-cycle MMA). Writing tap = 4q + j,
 //     Z_j[u] = sum_q x[u + 4q - Kp/2] . W[4q + j],      conv[t] = sum_j Z_j[t + j]
-// gives one GEMM with N = 4*cpg (192 / 256) columns per group and Kp/4 k-blocks whose A rows advance by 4; the four
-// column blocks are re-aligned by posconv_combine_kernel (norm.cu). Rows u in [0, T+3) per utterance. W: the
-// [G * 4cpg][Kq * 64] matrix of posconv4_weight_layout, one group's rows per tile.
+// gives one GEMM with N = 4*cpg (96, 160, 192 or 256) columns per group and Kp/4 k-blocks whose A rows advance by
+// 4; the four column blocks are re-aligned by posconv_combine_kernel (norm.cu). Rows u in [0, T+3) per utterance.
+// W: the [G * 4cpg][Kq * 64] matrix of posconv4_weight_layout, one group's rows per tile. At 24 and 40 channels per
+// group the one-tap formulation would be bound by its A reads even more than at 48, so those widths run four taps only.
 static bool posconv4_ok(const s3b_config& c) {
     const int cpg = c.embed_dim / c.pos_conv_groups;
     if (c.pos_conv_depth > 1) return true;  // the only formulation of the data2vec blocks (checked at create)
-    return c.pos_conv_kernel % 4 == 0 && (4 * cpg == 192 || 4 * cpg == 256);
+    return c.pos_conv_kernel % 4 == 0 && (posconv4_only(cpg) || cpg == 48 || cpg == 64);
 }
 static int posconv4_params(GemmParams& p, const s3b_config& c, const SplitBuf& x, const SplitBuf& W, int B, int T,
                            const Epi& e) {
@@ -1447,7 +1460,7 @@ static int posconv4_params(GemmParams& p, const s3b_config& c, const SplitBuf& x
     p.n_tiles = G, p.bn = bn, p.num_k_blocks = Kq, p.kb_per_row = 1;
     p.a_row_step = 4, p.a_row_off = -(pos_taps(c) / 2), p.a_k_per_ntile = cpg;
     p.out_rows_per_batch = T + 3;
-    p.k_steps = (cpg + 15) / 16;  // 48 channels per group: the 4th k-step of every 64-wide box has zero weights
+    p.k_steps = (cpg + 15) / 16;  // 24, 40 or 48 channels per group: the box's last k-steps hold zero weights
     p.alg_flops = 2.0 * (double)B * T * D * cpg * pos_taps(c);
     set_epi(p, e, 4 * D);
     return 0;
@@ -1545,15 +1558,16 @@ struct Fwd : Lane {
     void* user = nullptr;
     Plan* plan = nullptr;
 
-    bool distil() const { return m->cfg.family == 3; }
+    // slot 0 is the post_extract_proj output, padded frames zeroed: the distiller's feat_final, LightHuBERT's features
+    bool proj_slot0() const { return m->cfg.family == 3 || m->cfg.proj_hidden0; }
     // Output slot i of the caller's buffer. Hidden state l (the input of layer l / the encoder output) lives in slot l —
-    // except for the distiller, whose slot 0 is feat_final and whose layer-0 input is not exposed (internal scratch).
+    // except where proj_slot0(): the layer-0 input is then not exposed (internal scratch).
     float* slot(int i) const { return hidden + (size_t)i * layer_stride; }
     // post_extract_proj output; a pre-LN Conformer's hidden state 0 is that output itself (no pos_conv)
     float* proj_out() const {
-        return (distil() || (m->cfg.conformer && m->cfg.layer_norm_first)) ? slot(0) : w->x_f32.as<float>();
+        return (proj_slot0() || (m->cfg.conformer && m->cfg.layer_norm_first)) ? slot(0) : w->x_f32.as<float>();
     }
-    float* hs(int l) const { return (distil() && l == 0) ? w->hs0.as<float>() : slot(l); }
+    float* hs(int l) const { return (proj_slot0() && l == 0) ? w->hs0.as<float>() : slot(l); }
     // hidden state l has been enqueued completely
     int done(int l) const { return layer_done != nullptr ? layer_done(m, l, st, user) : 0; }
     int prepare();
@@ -1685,7 +1699,7 @@ int Fwd::prepare() {
         if (c.conformer) S3B_OK(w->glu_f32.ensure((size_t)M * 2 * D * sizeof(float)));
         else if (posconv4_ok(c)) S3B_OK(w->pos_z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
         if (c.relative_position) S3B_OK(w->gate.ensure((size_t)B * H * T * 4));
-        if (c.family == 3) S3B_OK(w->hs0.ensure((size_t)M * D * 4));
+        if (c.family == 3 || c.proj_hidden0) S3B_OK(w->hs0.ensure((size_t)M * D * 4));
     }
 
     // ---- launch plan (cached per (B, Lmax) while no buffer has been reallocated) --------------------------------
@@ -1826,7 +1840,7 @@ static int add_post_extract_proj(const Lane& lane, std::vector<Step>& steps) {
         GemmParams q = p;
         q.out_f32 = f.proj_out();
         S3B_OK(run_gemm(f, q));
-        return f.distil() ? f.done(0) : 0;
+        return f.proj_slot0() ? f.done(0) : 0;
     });
     return 0;
 }
@@ -1862,7 +1876,7 @@ static int add_pos_conv(const Lane& lane, std::vector<Step>& steps) {
                                                       last ? (ln ? w->xs_s.planes(sch) : no_planes()) : x[i + 1]->planes(0),
                                                       f.st));
             }
-            return f.distil() ? 0 : f.done(0);
+            return f.proj_slot0() ? 0 : f.done(0);
         });
     } else if (posconv4_ok(c)) {
         // four taps per k-block into pos_z, then the combine kernel (+ LayerNorm)
@@ -1873,7 +1887,7 @@ static int add_pos_conv(const Lane& lane, std::vector<Step>& steps) {
             KNORM(m, f.st, launch_posconv_combine(z, f.proj_out(), m->pos_b.as<float>(), B, T, D, cpg,
                                                   m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(), ln ? 1 : 0, 0,
                                                   f.hs(0), ln ? w->xs_s.planes(sch) : no_planes(), f.st));
-            return f.distil() ? 0 : f.done(0);
+            return f.proj_slot0() ? 0 : f.done(0);
         });
     } else {
         // one tap per k-block: x + GELU(conv + bias) in the epilogue (pre-LN: straight into hidden state 0), then the
@@ -1890,7 +1904,7 @@ static int add_pos_conv(const Lane& lane, std::vector<Step>& steps) {
             if (ln)
                 KNORM(m, f.st, launch_layernorm(w->tmp_f32.as<float>(), (size_t)M, D, m->enc_ln_g.as<float>(),
                                                 m->enc_ln_b.as<float>(), 0, f.hs(0), w->xs_s.planes(sch), f.st));
-            return f.distil() ? 0 : f.done(0);
+            return f.proj_slot0() ? 0 : f.done(0);
         });
     }
     return 0;
@@ -2853,17 +2867,21 @@ extern "C" int s3b_posconv_f32(const float* x, const float* w, const float* bias
                                int32_t out_fmt, float* out, void* stream) {
     if (!x || !w || !bias || !out || (gamma == nullptr) != (beta == nullptr)) return fail("null argument");
     if (B < 1 || T < 1) return fail("bad sizes");
-    if (D != 512 && D != 768 && D != 1024 && D != 1280 && D != 1920)
-        return fail("d must be 512, 768, 1024, 1280 or 1920, not %d", D);
+    if (D != 384 && D != 512 && D != 640 && D != 768 && D != 1024 && D != 1280 && D != 1920)
+        return fail("d must be 384, 512, 640, 768, 1024, 1280 or 1920, not %d", D);
     if (G < 1 || D % G != 0) return fail("d %d is not a multiple of groups %d", D, G);
     const int cpg = D / G;
-    if (!posconv_cpg_ok(cpg)) return fail("channels per group must be 16, 32, 48, 64, 80 or 120 (got %d)", cpg);
+    if (!posconv_cpg_ok(cpg))
+        return fail("channels per group must be 16, 32, 48, 64, 80 or 120, or 24 or 40 with four taps per k-block (got %d)",
+                    cpg);
     if (taps != 1 && taps != 4) return fail("taps_per_kblock must be 1 or 4, not %d", taps);
     if (mode < 0 || mode > 2) return fail("mode must be 0, 1 or 2, not %d", mode);
     if (k < 2) return fail("kernel size %d < 2", k);
     if (mode == 0 && k % (taps == 4 ? 4 : 2) != 0) return fail("conv_pos kernel %d: must be even (a multiple of 4 with "
                                                                "four taps per k-block)", k);
-    if (taps == 4 && 4 * cpg != 192 && 4 * cpg != 256) return fail("four taps per k-block need 48 or 64 channels per group");
+    if (taps == 4 && !posconv4_only(cpg) && cpg != 48 && cpg != 64)
+        return fail("four taps per k-block need 24, 40, 48 or 64 channels per group");
+    if (taps == 1 && posconv4_only(cpg)) return fail("%d channels per group run four taps per k-block only", cpg);
     if (taps == 1 && mode != 0) return fail("the data2vec blocks (mode 1, 2) run four taps per k-block only");
     if (taps == 1 && gamma == nullptr && out_fmt >= 0)  // add_pos_conv: the one-tap epilogue writes fp32 only
         return fail("one tap per k-block writes operand planes only through the LayerNorm (gamma)");

@@ -1,6 +1,6 @@
 // Row-wise HBM-bound kernels: LayerNorm (+GELU) with fp32 and bf16 hi/lo outputs, Featurizer weighted sum.
 //   LayerNorm(512) before post_extract_proj       hubert_model.py:338,483
-//   encoder / per-layer LayerNorms (D=768/1024)   wav2vec2_model.py:3069-3070,3260-3322,3049-3050
+//   encoder / per-layer LayerNorms (D=384..1920)   wav2vec2_model.py:3069-3070,3260-3322,3049-3050
 //   per-frame LayerNorm+GELU of "layer_norm" conv blocks  wav2vec2_model.py:2887-2897
 //   Featurizer._weighted_sum                      s3prl/upstream/interfaces.py:217-248
 #include "common.cuh"
@@ -59,7 +59,9 @@ cudaError_t launch_layernorm(const float* x, size_t M, int D, const float* gamma
     const unsigned blocks = (unsigned)((M + 7) / 8);
     cudaError_t e = cudaSuccess;
     switch (D) {
+        case 384: e = launch_pdl(layernorm_kernel<3>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
         case 512: e = launch_pdl(layernorm_kernel<4>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
+        case 640: e = launch_pdl(layernorm_kernel<5>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
         case 768: e = launch_pdl(layernorm_kernel<6>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
         case 1024: e = launch_pdl(layernorm_kernel<8>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
         case 1280: e = launch_pdl(layernorm_kernel<10>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
@@ -332,7 +334,9 @@ cudaError_t launch_posconv_combine(const float* z, const float* x, const float* 
     return launch_pdl(posconv_combine_kernel<V>, dim3(blocks), dim3(256), 0, s, z, x, bias, B, T, cpg, gamma, beta, \
                       do_ln, mode, out_f32, op)
     switch (D) {
+        case 384: S3B_PC(3);
         case 512: S3B_PC(4);
+        case 640: S3B_PC(5);
         case 768: S3B_PC(6);
         case 1024: S3B_PC(8);
         case 1280: S3B_PC(10);

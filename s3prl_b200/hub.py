@@ -21,6 +21,7 @@ from .upstream.cpc import CpcExpert
 from .upstream.decoar import DecoarExpert
 from .upstream.decoar2 import Decoar2Expert
 from .upstream.expert import UpstreamExpert
+from .upstream.lighthubert import LighthubertExpert
 from .upstream.npc import NpcExpert
 
 
@@ -82,6 +83,12 @@ for _name, _required in (("npc", False), ("npc_360hr", False), ("npc_960hr", Fal
 # modified CPC (cpc/hubconf.py): the fabricated checkpoint without ckpt, else the local {"config", "weights"} file
 for _name, _required in (("modified_cpc", False), ("cpc_local", True), ("cpc_url", True)):
     ENTRIES[_name] = _entry(_name, partial(CpcExpert, name=_name), ckpt_required=_required)
+# LightHuBERT (lighthubert/hubconf.py): the fabricated supernet of each released subnet without ckpt, else the local
+# {"cfg", "model"} file; lighthubert is lighthubert_small
+for _name, _kind, _required in (("lighthubert", "small", False), ("lighthubert_small", "small", False),
+                                ("lighthubert_base", "base", False), ("lighthubert_stage1", "stage1", False),
+                                ("lighthubert_local", "small", True), ("lighthubert_url", "small", True)):
+    ENTRIES[_name] = _entry(_name, partial(LighthubertExpert, name=_name, kind=_kind), ckpt_required=_required)
 globals().update(ENTRIES)
 
 

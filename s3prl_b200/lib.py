@@ -113,6 +113,15 @@ class S3BConfig(C.Structure):
         ("reserved", C.c_int32 * 2),
     ]
 
+    # the header's `proj_hidden0` is the first of the two ints this mirror has always named `reserved`
+    @property
+    def proj_hidden0(self) -> int:
+        return self.reserved[0]
+
+    @proj_hidden0.setter
+    def proj_hidden0(self, v: int) -> None:
+        self.reserved[0] = v
+
 
 class S3BApcConfig(C.Structure):
     """Mirror of ``struct s3b_apc_config``."""
