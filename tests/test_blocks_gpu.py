@@ -22,21 +22,21 @@ def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
-@pytest.mark.parametrize(
-    "M,N,K,bias,gelu,res",
-    [
-        (128, 256, 64, False, False, False),
-        (128, 256, 256, True, False, False),
-        (300, 768, 512, True, False, True),
-        (1000, 2304, 768, True, True, False),
-        (4099, 3072, 768, True, True, True),
-        (257, 128, 1024, False, False, False),
-        (130, 64, 128, True, False, False),
-        (64, 48, 192, True, True, False),
-        (2000, 768, 3072, True, False, True),
-        (300, 576, 256, True, True, True),  # N % 192 == 0, N % 128 != 0: the 192-wide tile
-    ],
-)
+LINEAR_CASES = [  # (M, N, K, bias, gelu, res)
+    (128, 256, 64, False, False, False),
+    (128, 256, 256, True, False, False),
+    (300, 768, 512, True, False, True),
+    (1000, 2304, 768, True, True, False),
+    (4099, 3072, 768, True, True, True),
+    (257, 128, 1024, False, False, False),
+    (130, 64, 128, True, False, False),
+    (64, 48, 192, True, True, False),
+    (2000, 768, 3072, True, False, True),
+    (300, 576, 256, True, True, True),  # N % 192 == 0, N % 128 != 0: the 192-wide tile
+]
+
+
+@pytest.mark.parametrize("M,N,K,bias,gelu,res", LINEAR_CASES)
 @pytest.mark.parametrize("scheme", [None, 0, 1])
 def test_linear(s3b_lib, scheme, M, N, K, bias, gelu, res):
     """Both operand schemes, requested explicitly (s3b_linear_ex); f16q8 needs K % 128 == 0 and N % 128 == 0, and a

@@ -3,8 +3,9 @@ load each A box once between them (TMA multicast). That changes where the operan
 every output must be bit-identical to the launch without clusters (S3B_GEMM_CLUSTER=1), whatever the cluster size
 (S3B_GEMM_CLUSTER=2 / 4, or the library's own choice with the variable unset).
 
-Cases: the encoder linears of hubert_base and wav2vec2_large, conv 1..6, NPC's tap convolutions (masked ones too) and
-modified CPC's conv 1 and 4 (N = 256) in both operand schemes; M with a partial last row tile; conv batches whose
+Cases: the encoder linears of hubert_base, wav2vec2_large and the LightHuBERT subnets (some of an odd number of tiles,
+where a forced cluster size falls back to 1), modified CPC's LSTM input GEMM, conv 1..6, NPC's tap convolutions (masked
+ones too) and modified CPC's conv 1 and 4 (N = 256) in both operand schemes; M with a partial last row tile; conv batches whose
 per-utterance row count is not a multiple of 128; n_tiles equal to the cluster size; launches with fewer clusters of
 tiles than clusters that can be resident (M = 1, 129). Outputs start as NaN, so a tile that no cluster writes shows as
 well."""
@@ -42,9 +43,13 @@ def _assert_identical(what, outs):
         assert torch.equal(out, base), f"{what}: S3B_GEMM_CLUSTER={cn} differs from 1"
 
 
-# (K, N): QKV, out_proj, fc1, fc2 of hubert_base and wav2vec2_large; N = 256 and 512 are n_tiles == 2 and 4
+# (K, N): QKV, out_proj, fc1, fc2 of hubert_base and wav2vec2_large; N = 256 and 512 are n_tiles == 2 and 4; the same of
+# LightHuBERT's 384-, 640- and 512-wide subnets, where N = 384, 1152, 640 and 1920 are an odd number of tiles (clusters
+# of 2 or 4 fall back to 1); modified CPC's LSTM input GEMM
 LINEAR_SHAPES = [(768, 2304), (768, 768), (768, 3072), (3072, 768), (1024, 3072), (1024, 1024), (1024, 4096),
-                 (4096, 1024), (768, 256), (512, 512)]
+                 (4096, 1024), (768, 256), (512, 512),
+                 (384, 384), (384, 1152), (384, 1536), (1536, 384), (640, 640), (640, 1920), (640, 2560), (2560, 640),
+                 (512, 1536), (512, 2048), (2048, 512), (256, 1024)]
 
 
 @pytest.mark.parametrize("M", [1, 129, 1000, 4099])

@@ -1,7 +1,7 @@
 """Block-level GPU tests of the GEMM's layouts in both operand schemes, through the entry points that build their launches
 with the model's own code: the flat linears (tile widths 128 / 256, operand-plane output, post_extract_proj's row mask,
-fc2's pre-residual output, the distiller's column slice), the QKV epilogue, conv 1..6 and the positional conv in both
-formulations with its combine kernel.
+fc2's pre-residual output, the distiller's and DeCoAR's column slices), the QKV epilogue, conv 1..6 and the positional
+conv in both formulations with its combine kernel.
 
 Every case is checked against two references, both in fp64 on the GPU:
 1. the exact operation on the fp32 inputs, within a per-element bound derived from the inputs (_gemm_refs: the
@@ -167,8 +167,8 @@ def _linear(a, w, bias=None, res=None, gelu=False, M=None, N=None, K=None, **opt
 # ------------------------------------------------------------------------------------------------
 # flat linears
 # ------------------------------------------------------------------------------------------------
-LINEAR_SHAPES = [(512, 768), (512, 1024), (768, 2304), (1024, 3072), (768, 3072), (3072, 768), (1024, 4096),
-                 (4096, 1024)]  # (K, N): post_extract_proj, QKV, fc1 / fc2 of base and large
+LINEAR_SHAPES = [(512, 768), (512, 1024), (768, 2304), (1024, 3072), (768, 768), (1024, 1024), (768, 3072), (3072, 768),
+                 (1024, 4096), (4096, 1024)]  # (K, N): post_extract_proj, QKV, out_proj, fc1 / fc2 of base and large
 
 
 def _operands(M, N, K, mag, g):
@@ -275,24 +275,34 @@ def test_linear_out_pre(s3b_lib, scheme):
     _check(f"fc2 s{scheme}", out, ref1, b1, ref2, b2, (e1, e2), scheme)
 
 
-@pytest.mark.parametrize("task", [0, 1, 2])
+SPLIT_SLICES = [  # (N, K, lda, a_off): A is the K-column slice at a_off of rows lda apart
+    (768, 768, 3 * 768, 0),  # the distiller's SplitLinear, tasks 0, 1, 2
+    (768, 768, 3 * 768, 768),
+    (768, 768, 3 * 768, 2 * 768),
+    (4096, 1024, 2048, 0),  # DeCoAR's LSTM input GEMM above layer 0: the forward direction's half of [2048]
+    (4096, 1024, 2048, 1024),  # the backward direction's half
+]
+
+
+@pytest.mark.parametrize("N,K,lda,a_off", SPLIT_SLICES, ids=["0", "1", "2", "decoar_fwd", "decoar_bwd"])
 @pytest.mark.parametrize("scheme", [0, 1])
-def test_linear_split_slice(s3b_lib, scheme, task):
-    """The distiller's SplitLinear: A is the D-column slice a_off = task * D of rows lda = 3 * D apart; the result is
-    bit-identical to the dense slice."""
-    M, D, heads = 499, 768, 3
-    g = torch.Generator(device="cuda").manual_seed(11 + task + 5 * scheme)
-    h = torch.randn(M, heads * D, device="cuda", generator=g)
-    w = torch.randn(D, D, device="cuda", generator=g) / D**0.5
-    b = torch.randn(D, device="cuda", generator=g)
-    out, _ = _linear(h, w, b, M=M, N=D, K=D, scheme=scheme, lda=heads * D, a_off=task * D)
-    a = h[:, task * D : (task + 1) * D].contiguous()
+def test_linear_split_slice(s3b_lib, scheme, N, K, lda, a_off):
+    """A strided column slice of A (the distiller's SplitLinear, DeCoAR's bidirectional layer input): bit-identical to
+    the dense slice. The columns outside the slice are NaN, so reading any of them shows."""
+    M = 499
+    g = torch.Generator(device="cuda").manual_seed(11 + a_off + N + 5 * scheme)
+    h = torch.full((M, lda), float("nan"), device="cuda")
+    h[:, a_off : a_off + K] = torch.randn(M, K, device="cuda", generator=g)
+    w = torch.randn(N, K, device="cuda", generator=g) / K**0.5
+    b = torch.randn(N, device="cuda", generator=g)
+    out, _ = _linear(h, w, b, M=M, N=N, K=K, scheme=scheme, lda=lda, a_off=a_off)
+    a = h[:, a_off : a_off + K].contiguous()
     dense, _ = _linear(a, w, b, scheme=scheme)
     assert torch.equal(out, dense)
     exact, emu, e1, e2 = _gemm_refs(a, w, scheme)
     ref1, b1 = _epilogue(exact, e1, b)
     ref2, b2 = _epilogue(emu, e2, b)
-    _check(f"split linear s{scheme} task {task}", out, ref1, b1, ref2, b2, (e1, e2), scheme)
+    _check(f"split linear s{scheme} N={N} K={K} lda={lda} a_off={a_off}", out, ref1, b1, ref2, b2, (e1, e2), scheme)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -1,8 +1,13 @@
-"""Block-level GPU tests of the existing GEMM, LayerNorm and Featurizer kernels at the shapes the XLS-R, DeCoAR 2.0 and
-APC ports run them at, where until now only whole-model parity (2e-4 per layer) looked:
-- the flat linears of XLS-R 1B / 2B (out_proj, fc1, fc2: K up to 7680, N = 1920 on 128-wide tiles only), DeCoAR 2.0's
-  post_extract_proj and APC's gate GEMMs (K = 128: the 80 fbank bins zero-padded, two k-blocks per tile, so the ring's
-  stage / phase wraps mid-tile), in both operand schemes, with the two references of tests/test_gemm_layouts_gpu.py;
+"""Block-level GPU tests of the existing GEMM, LayerNorm and Featurizer kernels at the shapes the ports run them at,
+where otherwise only whole-model parity (2e-4 per layer) would look:
+- the flat linears of XLS-R 1B / 2B (QKV, out_proj, fc1, fc2, post_extract_proj: K up to 7680, N = 1920 on 128-wide
+  tiles only), DeCoAR 2.0's post_extract_proj and APC's gate GEMMs (K = 128: the 80 fbank bins zero-padded, two
+  k-blocks per tile, so the ring's stage / phase wraps mid-tile), the encoder linears and post_extract_proj of the
+  384-, 512- and 640-wide LightHuBERT subnets, DeCoAR's proj, modified CPC's LSTM input GEMM (K = 256) and the
+  Conformer's [q | k] / pointwise_conv1 (N = 2048), in both operand schemes, with the two references of
+  tests/test_gemm_layouts_gpu.py; tests/test_port_coverage_cpu.py checks that every served shape has a row here or in
+  another block table;
+- pick_bn's choice between 128- and 256-wide tiles by the fill of the last round, at XLS-R 1B's and LightHuBERT's fc2;
 - LayerNorm at D = 1280 (XLS-R 1B, pre-LN) with partial 8-row blocks, LayerNorm + RoPE at D = 512 and 1280;
 - the Featurizer weighted sum and its backward against fp64 at every served layer count, up to kMaxLayers = 64, and at
   a size whose grid-stride loops wrap (forward: more float4 than the 132 x 8 x 256 capped grid; backward: past its
@@ -42,15 +47,38 @@ U = 2.0**-24  # fp32 unit roundoff
 # GEMMs at the ports' production shapes
 # ------------------------------------------------------------------------------------------------
 PORT_LINEARS = [  # (layer, N, K, epilogue)
+    ("xls_r_1b.qkv", 3840, 1280, "bias"),
     ("xls_r_1b.out_proj", 1280, 1280, "residual"),
     ("xls_r_1b.fc1", 5120, 1280, "gelu"),
     ("xls_r_1b.fc2", 1280, 5120, "out_pre"),
+    ("xls_r_1b.post_extract_proj", 1280, 512, "row_mask"),
+    ("xls_r_2b.qkv", 5760, 1920, "bias"),  # 45 tiles of 128: no clusters
     ("xls_r_2b.out_proj", 1920, 1920, "residual"),  # 1920 % 256 != 0: 128-wide tiles only
     ("xls_r_2b.fc1", 7680, 1920, "gelu"),
     ("xls_r_2b.fc2", 1920, 7680, "out_pre"),  # the project's longest contraction
+    ("xls_r_2b.post_extract_proj", 1920, 512, "row_mask"),
     ("decoar2.post_extract_proj", 768, 128, "row_mask"),
     ("apc.gate_l0", 1536, 128, "bias"),
-    ("apc.gate_l12", 1536, 512, "bias"),
+    ("apc.gate_l12", 1536, 512, "bias"),  # also the QKV of LightHuBERT's 512-wide subnet
+    # LightHuBERT subnets: 384 wide (6 heads, FFN 1536), 512 (8 heads, FFN 2048), 640 (10 heads, FFN 2560); under f16q8
+    # N = 384, 640, 1152 and 1920 are an odd number of 128-wide tiles, which run without clusters
+    ("lighthubert_small.qkv", 1152, 384, "bias"),
+    ("lighthubert_small.out_proj", 384, 384, "residual"),
+    ("lighthubert_small.fc1", 1536, 384, "gelu"),
+    ("lighthubert_small.fc2", 384, 1536, "out_pre"),
+    ("lighthubert_small.post_extract_proj", 384, 512, "row_mask"),
+    ("lighthubert_stage1_small.out_proj", 512, 512, "residual"),
+    ("lighthubert_stage1_small.fc1", 2048, 512, "gelu"),
+    ("lighthubert_stage1_small.fc2", 512, 2048, "out_pre"),  # tile width by M: test_lighthubert_fc2_tile_picker
+    ("lighthubert_stage1_small.post_extract_proj", 512, 512, "row_mask"),
+    ("lighthubert_base.qkv", 1920, 640, "bias"),
+    ("lighthubert_base.out_proj", 640, 640, "residual"),
+    ("lighthubert_base.fc1", 2560, 640, "gelu"),
+    ("lighthubert_base.fc2", 640, 2560, "out_pre"),
+    ("lighthubert_base.post_extract_proj", 640, 512, "row_mask"),
+    ("decoar.proj", 1024, 128, "bias_planes"),  # into the LSTM's operand planes
+    ("cpc.lstm_input", 1024, 256, "bias"),
+    ("conformer.qk_pw1", 2048, 1024, "bias"),  # [q | k] and pointwise_conv1 of wav2vec2_conformer_rope
 ]
 FBANK_BINS = 80  # K = 128 layers: columns 80.. of A (the CMVN kernel's planes) and W (the finalized weights) are zero
 LONG_K = 5120  # f16q8 from here on: _dropped_steps in place of the 50x proxy
@@ -115,7 +143,8 @@ def _per_tile(N, scheme, launch):
 def test_port_linear(s3b_lib, scheme, layer, N, K, epi, M):
     """The layer's epilogue at both tile widths where N allows (bit-identical), against fp64 and against the scheme's
     emulated operand decomposition: residual (out_proj), GELU as fp32 and as the scheme's operand planes (fc1), out_pre
-    before the residual (fc2), the row mask as fp32 and bf16 planes (post_extract_proj), bias only (APC gates)."""
+    before the residual (fc2), the row mask as fp32 and bf16 planes (post_extract_proj), bias only (QKV's GEMM, the
+    recurrent models' input GEMMs), bias as fp32 and as the scheme's operand planes (DeCoAR's proj)."""
     what = f"{layer} s{scheme} M={M} N={N} K={K}"
     a, w, g = _port_operands(M, N, K, "unit", M * 131 + K * 7 + N + scheme)
     b = torch.randn(N, device="cuda", generator=g) * 0.5
@@ -129,8 +158,12 @@ def test_port_linear(s3b_lib, scheme, layer, N, K, epi, M):
     if epi == "residual":
         r = torch.randn(M, N, device="cuda", generator=g)
         check("residual", _per_tile(N, scheme, lambda t: _linear(a, w, b, r, scheme=scheme, tile_n=t)), res=r)
-    elif epi == "bias":
-        check("bias", _per_tile(N, scheme, lambda t: _linear(a, w, b, scheme=scheme, tile_n=t)))
+    elif epi in ("bias", "bias_planes"):
+        free = _per_tile(N, scheme, lambda t: _linear(a, w, b, scheme=scheme, tile_n=t))
+        check("bias", free)
+        if epi == "bias_planes":
+            planes = _per_tile(N, scheme, lambda t: _linear(a, w, b, scheme=scheme, out_fmt=scheme, tile_n=t))
+            assert torch.equal(planes, _through_planes(free, scheme)), "operand planes != planes of the fp32 output"
     elif epi == "gelu":
         h32 = _per_tile(N, scheme, lambda t: _linear(a, w, b, gelu=True, scheme=scheme, tile_n=t))
         check("gelu", h32, gelu=True)
@@ -159,7 +192,7 @@ def test_port_linear(s3b_lib, scheme, layer, N, K, epi, M):
             assert torch.equal(out[keep], want[keep]), fmt
 
 
-PORT_SHAPES = [(N, K) for _, N, K, _ in PORT_LINEARS]
+PORT_SHAPES = list(dict.fromkeys((N, K) for _, N, K, _ in PORT_LINEARS))
 
 
 @pytest.mark.parametrize("mag", ["small", "large"])
@@ -198,6 +231,37 @@ def test_xls_r_fc2_tile_picker(s3b_lib):
         forced, of = _linear(a, w, b, r, scheme=1, tile_n=tile)
         assert of.tile_n_used == tile
         assert torch.equal(forced, auto), tile
+
+
+def _picked_bn(M, N, K, sms):
+    """pick_bn's width (model.cu) for an f16q8 linear whose N is a multiple of 256: 256 columns at K >= 2048 when the
+    last round of 256-wide tiles is empty or fills at least half of the SMs, 128 columns otherwise."""
+    if K < 2048:
+        return 128
+    last = -(-M // 128) * (N // 256) % sms
+    return 256 if last == 0 or last >= sms // 2 else 128
+
+
+def test_lighthubert_fc2_tile_picker(s3b_lib):
+    """fc2 of LightHuBERT's 512-wide subnet in f16q8 (N = 512, K = 2048), where the tile width depends on M and the SM
+    count: at 128 * (SMs // 2) rows (8448 on 132 SMs) the last round of 256-wide tiles is empty or at least half full,
+    at 1280 rows (20 tiles) it is under half full. The picked width is the rule's for this device, and forcing the
+    other width gives the same bits."""
+    N, K = 512, 2048
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    Ms = (128 * (sms // 2), 1280)
+    assert [_picked_bn(M, N, K, sms) for M in Ms] == [256, 128], sms
+    for M in Ms:
+        a, w, g = _port_operands(M, N, K, "unit", M + 3)
+        b = torch.randn(N, device="cuda", generator=g)
+        r = torch.randn(M, N, device="cuda", generator=g)
+        auto, o = _linear(a, w, b, r, scheme=1)
+        want = _picked_bn(M, N, K, sms)
+        print(f"lighthubert fc2 M={M}: tile_n {o.tile_n_used} picked on {sms} SMs, rule {want}")
+        assert (o.scheme_used, o.tile_n_used) == (1, want), M
+        forced, of = _linear(a, w, b, r, scheme=1, tile_n=384 - want)
+        assert of.tile_n_used == 384 - want
+        assert torch.equal(forced, auto), M
 
 
 # ------------------------------------------------------------------------------------------------
@@ -253,6 +317,9 @@ WS_SHAPES = [  # (NL, B, T, D): hidden states per upstream and width
     (3, 3, 37, 512),  # APC
     (3, 3, 37, 768),  # distilhubert
     (13, 3, 37, 768),  # base models, DeCoAR 2.0
+    (13, 3, 37, 384),  # LightHuBERT subnets
+    (13, 3, 37, 512),
+    (13, 3, 37, 640),
     (25, 2, 49, 1024),  # large models
     (49, 2, 49, 1280),  # XLS-R 1B
     (49, 2, 49, 1920),  # XLS-R 2B

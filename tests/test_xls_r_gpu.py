@@ -1,7 +1,8 @@
 """GPU tests of XLS-R 1B / 2B (80- and 120-wide attention heads, 1920-channel encoders): attention at head widths 64, 80
-and 120, the QKV scatter epilogue, the positional conv with 80- and 120-channel groups and LayerNorm(1920) at block level
-against fp64 torch, and the whole model against the executed-reference goldens (tests/golden/xls_r_*.pt) and the CPU
-oracle on ragged batches, with determinism across lanes, shards and a converted checkpoint.
+and 120 and at LightHuBERT's 6, 8 and 10 heads of 64, the QKV scatter epilogue at the same heads, the positional conv
+with 80- and 120-channel groups and LayerNorm(1920) at block level against fp64 torch, and the whole model against the
+executed-reference goldens (tests/golden/xls_r_*.pt) and the CPU oracle on ragged batches, with determinism across
+lanes, shards and a converted checkpoint.
 Bounds: blocks 1e-4 relative Frobenius and 2e-4 of the output scale elementwise (the operand planes carry ~16
 significant bits), as tests/test_blocks_gpu.py; the model the golden bars of tests/test_upstream_gpu.py (2e-4 per layer,
 1e-3 of the layer's abs max). Every check prints measured / bound."""
@@ -64,14 +65,19 @@ def _attention(q, k, v, valid, H, hd, ctx_format):
     return out
 
 
+HEADS = [(3, 64), (3, 80), (3, 120), (6, 64), (8, 64), (10, 64)]  # (H, hd); H = 6, 8, 10: the LightHuBERT subnets
+HEAD_IDS = ["64", "80", "120", "h6-64", "h8-64", "h10-64"]
+
+
 @pytest.mark.parametrize("fmt", [0, 1])
-@pytest.mark.parametrize("hd", [64, 80, 120])
+@pytest.mark.parametrize("H,hd", HEADS, ids=HEAD_IDS)
 @pytest.mark.parametrize("T", [1, 37, 63, 64, 65, 127, 128, 129, 999])
-def test_attention_head_widths(s3b_lib, T, hd, fmt):
-    H, B = 3, 3
-    valid = [T, max(1, (2 * T) // 3), 1]
+def test_attention_head_widths(s3b_lib, T, H, hd, fmt):
+    """Ragged valid lengths: T, about 2T / 3, T rounded down to a multiple of 64 (a whole number of key blocks), 1."""
+    B = 4
+    valid = [T, max(1, (2 * T) // 3), max(1, T - T % 64), 1]
     D = H * hd
-    g = torch.Generator(device="cuda").manual_seed(T * 10 + hd + fmt)
+    g = torch.Generator(device="cuda").manual_seed(T * 10 + hd + fmt + 1000 * H)
     q, k, v = (torch.randn(B, T, D, device="cuda", generator=g) for _ in range(3))
     out = _attention(q, k, v, valid, H, hd, fmt)
     qh, kh, vh = (t.double().view(B, T, H, hd).transpose(1, 2) for t in (q, k, v))
@@ -79,7 +85,7 @@ def test_attention_head_widths(s3b_lib, T, hd, fmt):
     mask = torch.arange(T, device="cuda")[None, :] >= torch.tensor(valid, device="cuda")[:, None]
     s = s.masked_fill(mask[:, None, None, :], float("-inf"))
     ref = (s.softmax(-1) @ vh).transpose(1, 2).reshape(B, T, D)
-    _check_block(out, ref, f"attention hd={hd} T={T} valid={valid} ctx_format={fmt}")
+    _check_block(out, ref, f"attention H={H} hd={hd} T={T} valid={valid} ctx_format={fmt}")
 
 
 def test_attention_refusals(s3b_lib):
@@ -103,16 +109,17 @@ def test_attention_refusals(s3b_lib):
 # QKV scatter epilogue
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("scheme", [0, 1])
-@pytest.mark.parametrize("hd", [80, 120])
+@pytest.mark.parametrize("H,hd", [(16, 80), (16, 120), (6, 64), (8, 64), (10, 64)],
+                         ids=["80", "120", "h6-64", "h8-64", "h10-64"])
 @pytest.mark.parametrize("T", [1, 37, 130])
-def test_qkv_scatter(s3b_lib, T, hd, scheme):
+def test_qkv_scatter(s3b_lib, T, H, hd, scheme):
     """q, k as [B][H][T][hd] (q scaled by hd^-0.5 * log2(e)) and v^T as [B][H][hd][Tp], Tp = T rounded up to 8; the
-    padding columns of v^T stay zero."""
+    padding columns of v^T stay zero. XLS-R's 16 heads of 80 and 120, LightHuBERT's 6, 8 and 10 heads of 64."""
     from s3prl_b200 import lib
 
-    B, H = 2, 16
+    B = 2
     D, Tp = H * hd, (T + 7) // 8 * 8
-    g = torch.Generator(device="cuda").manual_seed(T + hd + scheme)
+    g = torch.Generator(device="cuda").manual_seed(T + hd + scheme + 100 * H)
     x = torch.randn(B, T, D, device="cuda", generator=g)
     w = torch.randn(3 * D, D, device="cuda", generator=g) / D**0.5
     b = torch.randn(3 * D, device="cuda", generator=g) * 0.1
@@ -124,9 +131,9 @@ def test_qkv_scatter(s3b_lib, T, hd, scheme):
     torch.cuda.synchronize()
     y = (x.double() @ w.double().t() + b.double()).view(B, T, 3, H, hd)
     scale = float(torch.tensor(LOG2E / math.sqrt(hd), dtype=torch.float32))
-    _check_block(q, y[:, :, 0].transpose(1, 2) * scale, f"qkv q hd={hd} T={T} scheme={scheme}")
-    _check_block(k, y[:, :, 1].transpose(1, 2), f"qkv k hd={hd} T={T} scheme={scheme}")
-    _check_block(vt[..., :T], y[:, :, 2].permute(0, 2, 3, 1), f"qkv v^T hd={hd} T={T} scheme={scheme}")
+    _check_block(q, y[:, :, 0].transpose(1, 2) * scale, f"qkv q H={H} hd={hd} T={T} scheme={scheme}")
+    _check_block(k, y[:, :, 1].transpose(1, 2), f"qkv k H={H} hd={hd} T={T} scheme={scheme}")
+    _check_block(vt[..., :T], y[:, :, 2].permute(0, 2, 3, 1), f"qkv v^T H={H} hd={hd} T={T} scheme={scheme}")
     assert torch.equal(vt[..., T:], torch.zeros_like(vt[..., T:]))
 
 
