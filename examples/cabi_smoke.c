@@ -35,7 +35,9 @@ int main(void) {
         (const void*)s3b_decoar_model_create, (const void*)s3b_lstm_f32, (const void*)s3b_lstm_fits,
         (const void*)s3b_npc_model_create, (const void*)s3b_npc_conv_f32,
         (const void*)s3b_cpc_model_create, (const void*)s3b_cpc_conv_f32, (const void*)s3b_cpc_lstm_f32,
-        (const void*)s3b_cpc_lstm_max_active_clusters,
+        (const void*)s3b_cpc_lstm_max_active_clusters, (const void*)s3b_ssast_model_create,
+        (const void*)s3b_layernorm_eps_f32, (const void*)s3b_ssast_fbank_f32, (const void*)s3b_ssast_embed_f32,
+        (const void*)s3b_ssast_fold_f32,
     };
     s3b_config cfg;
     int64_t lens[2] = {16000, 800};
@@ -153,6 +155,25 @@ int main(void) {
         }
         s3b_model_destroy(m);
         if (valid[0] != 49 || valid[1] != 3) return 19;
+    }
+    {
+        /* SSAST frame model, 1 s windows: 99 frames per window, trimmed to ceil(max_len / 160); 12 block outputs */
+        s3b_ssast_config scfg;
+        s3b_model* m = NULL;
+        memset(&scfg, 0, sizeof(scfg));
+        scfg.struct_size = (int32_t)sizeof(scfg), scfg.patch = 0, scfg.window_samples = 16000;
+        scfg.embed_dim = 768, scfg.num_heads = 12, scfg.num_layers = 12;
+        if (s3b_ssast_model_create(&scfg, &m) != 0) {
+            printf("s3b_ssast_model_create: %s\n", s3b_last_error());
+            return 20;
+        }
+        if (s3b_valid_frames(m, lens, 2, 16000, valid) != 0 || s3b_num_outputs(m) != 12 ||
+            s3b_num_frames(m, 16000) != 99 || s3b_num_frames(m, 16001) != 101) {
+            printf("SSAST bookkeeping: %s\n", s3b_last_error());
+            return 21;
+        }
+        s3b_model_destroy(m);
+        if (valid[0] != 99 || valid[1] != 5) return 22;
     }
     return 0;
 }

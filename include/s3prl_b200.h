@@ -169,6 +169,34 @@ typedef struct s3b_cpc_config {
     int32_t reserved[4]; /* 0 */
 } s3b_cpc_config;
 int s3b_cpc_model_create(const s3b_cpc_config* cfg, s3b_model** out);
+/* SSAST (s3prl/upstream/ssast/{expert,audio,ast_models}.py): every utterance zero-padded to nseg = ceil(max_len / S)
+ * windows of S = window_samples samples; per window kaldi fbank (128 mel bins, 25 ms / 10 ms, hanning window,
+ * snip_edges), y = (y + 4.2677393) / 9.1379948, zero rows appended up to TL = S / 160 frames; the patch embedding
+ * Conv2d over x[f][t] (frame model: kernel (128, 2), stride (128, 1), P = TL - 1 patches; patch model: kernel (16, 16),
+ * stride (10, 10), P = 12 t_dim patches, t_dim = (TL - 16) / 10 + 1, in (f, t) row-major order); the sequence
+ * [cls_token, dist_token, patches] + pos_embed; 12 pre-LN DeiT blocks (LayerNorm eps 1e-6, 12 heads of 64, FFN 3072,
+ * exact GELU), every token of a window attending to the 2 + P tokens of its window. No final norm.
+ * Hidden state l is block l's output without the class tokens: frame model [batch][T][768], patch model
+ * [batch][T][12 * 768] with column block fi = frequency patch fi; T = min(nseg t_dim, ceil(max_len / rate)), rate 160
+ * (frame) or 1600 (patch), t_dim = P for the frame model. Frames are not masked: windows past an utterance's end hold
+ * the model's response to silence, as in the reference.
+ * Tensors (timm names of ASTModel.v): patch_embed.proj.weight [768][1][128][2] or [768][1][16][16], patch_embed.proj.bias,
+ * cls_token and dist_token [1][1][768], pos_embed [1][2 + P][768] (already re-gridded to the window, as the reference's
+ * fine-tuning constructor does), blocks.{l}.{norm1, norm2}.{weight, bias}, blocks.{l}.attn.qkv.{weight [2304][768],
+ * bias}, blocks.{l}.attn.proj.*, blocks.{l}.mlp.{fc1, fc2}.*; other keys are ignored.
+ * s3b_num_outputs = num_layers (12); s3b_valid_frames gives min(T, ceil(lens[b] / rate)); s3b_forward_ex refuses ffn_out
+ * and last_residual. Served: the base model only (embed_dim 768, num_heads 12, num_layers 12); window_samples from 400
+ * (frame) or 2560 (patch) to 160000 (10 s). */
+typedef struct s3b_ssast_config {
+    int32_t struct_size;    /* sizeof(s3b_ssast_config) */
+    int32_t patch;          /* 0 = frame model (base_f), 1 = patch model (base_p) */
+    int32_t window_samples; /* int(window_secs * 16000) */
+    int32_t embed_dim;      /* 768 */
+    int32_t num_heads;      /* 12 */
+    int32_t num_layers;     /* 12 */
+    int32_t reserved[4];    /* 0 */
+} s3b_ssast_config;
+int s3b_ssast_model_create(const s3b_ssast_config* cfg, s3b_model** out);
 int s3b_model_finalize(s3b_model* m);
 void s3b_model_destroy(s3b_model* m);
 
@@ -517,6 +545,28 @@ int s3b_conformer_conv_f32(const float* x, int32_t batch, int32_t t, int32_t d, 
  * x: [m][d] (m a multiple of t: rows of utterances of t frames); d in {512, 768, 1024, 1280}. */
 int s3b_layernorm_rope_f32(const float* x, int64_t m, int32_t t, int32_t d, const float* gamma, const float* beta,
                            const float* inv_freq, int32_t out_fmt, float* out, float* out_rope, void* stream);
+
+/* y = LayerNorm_D(x) with epsilon eps, otherwise s3b_layernorm_f32 (SSAST's blocks use 1e-6) */
+int s3b_layernorm_eps_f32(const float* x, int64_t m, int32_t d, const float* gamma, const float* beta, int32_t gelu,
+                          float eps, float* out, void* stream);
+/* SSAST's front end as a forward runs it: ragged DEVICE waveforms (host array of pointers, host lengths lens[b] in
+ * [1, max_len]), nseg = ceil(max_len / window_samples) windows each -> out DEVICE [batch * nseg][TL][128], row block
+ * b * nseg + s, TL = window_samples / 160 (the normalised fbank, zero rows appended). */
+int s3b_ssast_fbank_f32(const float* const* wavs, const int64_t* lens, int32_t batch, int64_t max_len,
+                        int32_t window_samples, float* out, void* stream);
+/* SSAST's patch embedding and token assembly as a forward runs them, on the features feat [segments][TL][128] (DEVICE):
+ * the patch operand (patch 0: the features, patch 1: the 16 x 16 / stride-10 gather) written as operand planes of
+ * `scheme` (-1 / 0 / 1 as s3b_linear_ex) and decoded into planes_out (optional; [segments][TL][128] or
+ * [segments][P][256]), the (768, 256) patch GEMM + bias, then [cls + pos[0], dist + pos[1], patch p + pos[2 + p]] into
+ * out [segments][2 + P][768]. w [768][1][128][2] or [768][1][16][16] (torch layout), bias, cls, dist [768],
+ * pos [2 + P][768]; all DEVICE. */
+int s3b_ssast_embed_f32(const float* feat, int32_t segments, int32_t tl, int32_t patch, const float* w,
+                        const float* bias, const float* cls, const float* dist, const float* pos, int32_t scheme,
+                        float* planes_out, float* out, void* stream);
+/* One SSAST hidden state from the residual stream x [batch * nseg][2 + P][768] (DEVICE) as a forward writes it:
+ * out [batch][t_out][768 or 12 * 768], class tokens dropped, frequency patches folded into channels; t_out <= nseg t_dim. */
+int s3b_ssast_fold_f32(const float* x, int32_t batch, int32_t nseg, int32_t tl, int32_t patch, int32_t t_out,
+                       float* out, void* stream);
 
 #ifdef __cplusplus
 }

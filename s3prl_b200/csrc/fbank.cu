@@ -8,7 +8,8 @@
 // memory, power spectrum, sparse triangular mel projection (the "matmul"), log. All fp32.
 // The same frame kernel with a hamming window is the front end of DeCoAR 2.0 (s3prl/upstream/decoar2/audio.py:41-86),
 // followed by decoar2_cmvn_kernel: per-utterance CMVN over all frames, every second frame kept, written as the
-// operand planes of post_extract_proj.
+// operand planes of post_extract_proj. With a hanning window and 128 bins, per fixed-length window of the waveform, it
+// is SSAST's front end (ssast_fbank_kernel).
 #include <math.h>
 
 #include <vector>
@@ -34,6 +35,43 @@ static bool g_tab_ready[64] = {false};
 // of its own: g_tab.window stays the povey window of the fbank baseline, and both models can live in one process.
 __device__ float g_hamming[kWin];
 static bool g_hamming_ready[64] = {false};
+// SSAST's front end: 128 mel bins and the hanning window, torch.hann_window(400, periodic=False) (kaldi.py _get_window),
+// in tables of their own next to the 80-bin ones, so that every fbank model can live in one process
+static constexpr int kSsastMel = 128;
+struct MelTable {
+    int start[kSsastMel], count[kSsastMel], off[kSsastMel];
+    float w[kMaxMelNnz];
+};
+__device__ MelTable g_mel128;
+__device__ float g_hann[kWin];
+static bool g_ssast_ready[64] = {false};
+
+// mel banks (kaldi.py:436-512): low 20 Hz, high = nyquist 8000 Hz, nbins bins over 256 fft bins, fp32 like torch
+static void build_mel(int nbins, int* mel_start, int* mel_count, int* mel_off, float* mel_w) {
+    const float low = 20.0f, high = 8000.0f, fft_bin_width = 16000.0f / kFft;
+    auto mel = [](float f) { return 1127.0f * logf(1.0f + f / 700.0f); };
+    const double mel_low = 1127.0 * log(1.0 + (double)low / 700.0), mel_high = 1127.0 * log(1.0 + (double)high / 700.0);
+    const double delta = (mel_high - mel_low) / (nbins + 1);
+    int off = 0;
+    for (int j = 0; j < nbins; ++j) {
+        const float left = (float)(mel_low + j * delta), center = (float)(mel_low + (j + 1.0) * delta),
+                    right = (float)(mel_low + (j + 2.0) * delta);
+        int start = -1, count = 0;
+        for (int i = 0; i < kFft / 2; ++i) {
+            const float m = mel(fft_bin_width * (float)i);
+            const float up = (m - left) / (center - left), down = (right - m) / (right - center);
+            const float w = fmaxf(0.0f, fminf(up, down));
+            if (w > 0.0f) {
+                if (start < 0) start = i;
+                // weights of one triangle are contiguous in i
+                if (off + count < kMaxMelNnz) mel_w[off + count] = w;
+                ++count;
+            }
+        }
+        mel_start[j] = start < 0 ? 0 : start, mel_count[j] = count, mel_off[j] = off;
+        off += count;
+    }
+}
 
 static void build_tables(FbankTables& t) {
     // povey window: hann(400, periodic=False) ** 0.85   (kaldi.py:98-100)
@@ -45,30 +83,7 @@ static void build_tables(FbankTables& t) {
         t.tw_re[k] = (float)cos(-2.0 * M_PI * k / kFft);
         t.tw_im[k] = (float)sin(-2.0 * M_PI * k / kFft);
     }
-    // mel banks (kaldi.py:436-512): low 20 Hz, high = nyquist 8000 Hz, 80 bins over 256 fft bins, fp32 like torch
-    const float low = 20.0f, high = 8000.0f, fft_bin_width = 16000.0f / kFft;
-    auto mel = [](float f) { return 1127.0f * logf(1.0f + f / 700.0f); };
-    const double mel_low = 1127.0 * log(1.0 + (double)low / 700.0), mel_high = 1127.0 * log(1.0 + (double)high / 700.0);
-    const double delta = (mel_high - mel_low) / (kMel + 1);
-    int off = 0;
-    for (int j = 0; j < kMel; ++j) {
-        const float left = (float)(mel_low + j * delta), center = (float)(mel_low + (j + 1.0) * delta),
-                    right = (float)(mel_low + (j + 2.0) * delta);
-        int start = -1, count = 0;
-        for (int i = 0; i < kFft / 2; ++i) {
-            const float m = mel(fft_bin_width * (float)i);
-            const float up = (m - left) / (center - left), down = (right - m) / (right - center);
-            const float w = fmaxf(0.0f, fminf(up, down));
-            if (w > 0.0f) {
-                if (start < 0) start = i;
-                // weights of one triangle are contiguous in i
-                if (off + count < kMaxMelNnz) t.mel_w[off + count] = w;
-                ++count;
-            }
-        }
-        t.mel_start[j] = start < 0 ? 0 : start, t.mel_count[j] = count, t.mel_off[j] = off;
-        off += count;
-    }
+    build_mel(kMel, t.mel_start, t.mel_count, t.mel_off, t.mel_w);
 }
 
 static cudaError_t ensure_tables(cudaStream_t s) {
@@ -85,50 +100,43 @@ static cudaError_t ensure_tables(cudaStream_t s) {
     return e;
 }
 
-// Synchronous: the shared tables and the hamming window of the current device, built once. DeCoAR 2.0 models call it
-// at finalize, so that their forwards (asynchronous, graph-capturable) never build tables.
+// Synchronous: the shared tables, the hamming window and SSAST's tables of the current device, built once. The fbank
+// models call it at finalize, so that their forwards (asynchronous, graph-capturable) never build tables.
 cudaError_t init_fbank_tables() {
     cudaError_t e = ensure_tables(0);
     if (e != cudaSuccess) return e;
     int dev = 0;
     e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
-    if (dev < 64 && g_hamming_ready[dev]) return cudaSuccess;
+    if (!(dev < 64 && g_hamming_ready[dev])) {
+        float h[kWin];
+        for (int n = 0; n < kWin; ++n) h[n] = (float)(0.54 - 0.46 * cos(2.0 * M_PI * n / (kWin - 1)));
+        e = cudaMemcpyToSymbol(g_hamming, h, sizeof(h));
+        if (e != cudaSuccess) return e;
+        if (dev < 64) g_hamming_ready[dev] = true;
+    }
+    if (dev < 64 && g_ssast_ready[dev]) return cudaSuccess;
     float h[kWin];
-    for (int n = 0; n < kWin; ++n) h[n] = (float)(0.54 - 0.46 * cos(2.0 * M_PI * n / (kWin - 1)));
-    e = cudaMemcpyToSymbol(g_hamming, h, sizeof(h));
-    if (e == cudaSuccess && dev < 64) g_hamming_ready[dev] = true;
+    for (int n = 0; n < kWin; ++n) h[n] = (float)(0.5 - 0.5 * cos(2.0 * M_PI * n / (kWin - 1)));
+    e = cudaMemcpyToSymbol(g_hann, h, sizeof(h));
+    if (e != cudaSuccess) return e;
+    static MelTable mt;
+    build_mel(kSsastMel, mt.start, mt.count, mt.off, mt.w);
+    e = cudaMemcpyToSymbol(g_mel128, &mt, sizeof(mt));
+    if (e == cudaSuccess && dev < 64) g_ssast_ready[dev] = true;
     return e;
 }
 
 __device__ __forceinline__ int bitrev9(int x) { return (int)(__brev((unsigned)x) >> 23); }
 
-// grid: (ceil(max_frames / 4), B); block: 128 threads = 4 warps = 4 frames. kHamming: hamming instead of povey window;
-// kLd: floats between consecutive frames of `out` (the log-mel goes to columns [0, 80))
-template <bool kHamming, int kLd>
-__global__ void __launch_bounds__(128) fbank_frames_kernel(const float* const* __restrict__ wavs,
-                                                           const long long* __restrict__ lens, int max_frames,
-                                                           float* __restrict__ out) {
-    __shared__ float s_re[4][kFft], s_im[4][kFft], s_pw[4][kBins + 3];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int b = blockIdx.y;
-    const int t = blockIdx.x * 4 + warp;
-    const long long L = lens[b];
-    const int m = L < kWin ? 0 : (int)(1 + (L - kWin) / kShift);  // snip_edges=True (kaldi.py:_get_strided)
-    if (t >= m) return;  // warp-uniform
-    const float* w = wavs[b] + (size_t)t * kShift;
-    float* re = s_re[warp];
-    float* im = s_im[warp];
-
-    // frame -> registers (13 samples per lane, last partial), DC removal
-    float x[13];
+// One 25 ms frame per warp, 13 samples per lane in x (lane + 32 i, zero past 400): DC removal, pre-emphasis (replicate
+// first sample), `window`, zero pad, 512-point radix-2 DIT FFT in re / im, power spectrum |X|^2 into pw[0, 257)
+// (use_power=True; kaldi.py computes abs() then pow(2)). re, im, pw: this warp's shared rows.
+__device__ __forceinline__ void frame_power(float (&x)[13], const float* __restrict__ window, float* re, float* im,
+                                            float* pw, int lane) {
     float sum = 0.f;
 #pragma unroll
-    for (int i = 0; i < 13; ++i) {
-        const int n = lane + 32 * i;
-        x[i] = n < kWin ? w[n] : 0.f;
-        sum += x[i];
-    }
+    for (int i = 0; i < 13; ++i) sum += x[i];
     const float mean = warp_sum(sum) / (float)kWin;
 #pragma unroll
     for (int i = 0; i < 13; ++i) {
@@ -136,13 +144,12 @@ __global__ void __launch_bounds__(128) fbank_frames_kernel(const float* const* _
         if (n < kWin) re[n] = x[i] - mean;
     }
     __syncwarp();
-    // pre-emphasis (replicate first sample), povey window, zero pad, bit-reversed placement for the DIT FFT
     float y[16];
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
         const int n = lane + 32 * i;
         float v = 0.f;
-        if (n < kWin) v = (re[n] - 0.97f * re[n > 0 ? n - 1 : 0]) * (kHamming ? g_hamming[n] : g_tab.window[n]);
+        if (n < kWin) v = (re[n] - 0.97f * re[n > 0 ? n - 1 : 0]) * window[n];
         y[i] = v;
     }
     __syncwarp();
@@ -172,13 +179,35 @@ __global__ void __launch_bounds__(128) fbank_frames_kernel(const float* const* _
         }
         __syncwarp();
     }
-    // power spectrum (use_power=True): |X|^2 ; kaldi.py computes abs() then pow(2)
-    float* pw = s_pw[warp];
     for (int k = lane; k < kBins; k += 32) {
         const float a = sqrtf(re[k] * re[k] + im[k] * im[k]);
         pw[k] = a * a;
     }
     __syncwarp();
+}
+
+// grid: (ceil(max_frames / 4), B); block: 128 threads = 4 warps = 4 frames. kHamming: hamming instead of povey window;
+// kLd: floats between consecutive frames of `out` (the log-mel goes to columns [0, 80))
+template <bool kHamming, int kLd>
+__global__ void __launch_bounds__(128) fbank_frames_kernel(const float* const* __restrict__ wavs,
+                                                           const long long* __restrict__ lens, int max_frames,
+                                                           float* __restrict__ out) {
+    __shared__ float s_re[4][kFft], s_im[4][kFft], s_pw[4][kBins + 3];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int b = blockIdx.y;
+    const int t = blockIdx.x * 4 + warp;
+    const long long L = lens[b];
+    const int m = L < kWin ? 0 : (int)(1 + (L - kWin) / kShift);  // snip_edges=True (kaldi.py:_get_strided)
+    if (t >= m) return;  // warp-uniform
+    const float* w = wavs[b] + (size_t)t * kShift;
+    float x[13];
+#pragma unroll
+    for (int i = 0; i < 13; ++i) {
+        const int n = lane + 32 * i;
+        x[i] = n < kWin ? w[n] : 0.f;
+    }
+    float* pw = s_pw[warp];
+    frame_power(x, kHamming ? g_hamming : g_tab.window, s_re[warp], s_im[warp], pw, lane);
     // mel projection + log(max(e, eps))
     float* o = out + ((size_t)b * max_frames + t) * kLd;
     for (int j = lane; j < kMel; j += 32) {
@@ -188,6 +217,51 @@ __global__ void __launch_bounds__(128) fbank_frames_kernel(const float* const* _
         for (int i = 0; i < cnt; ++i) acc = fmaf(pw[st + i], mw[i], acc);
         o[j] = logf(fmaxf(acc, 1.1920928955078125e-07f));
     }
+}
+
+// SSAST's FeatureExtractor (s3prl/upstream/ssast/audio.py, expert.py) per window: kaldi.fbank of window s of
+// utterance b, samples [s S, s S + S) of the waveform zero-padded past lens[b], with the hanning window and 128 mel
+// bins, then y = (y + 4.2677393) / (4.5689974 * 2) and zero rows appended up to TL = target_length.
+// out: [B * nseg][TL][128] fp32, row block b * nseg + s. grid (ceil(TL / 4), nseg, B); block 128 threads = 4 frames.
+__global__ void __launch_bounds__(128) ssast_fbank_kernel(const float* const* __restrict__ wavs,
+                                                          const long long* __restrict__ lens, int S, int TL,
+                                                          float* __restrict__ out) {
+    __shared__ float s_re[4][kFft], s_im[4][kFft], s_pw[4][kBins + 3];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int s = blockIdx.y, b = blockIdx.z;
+    const int t = blockIdx.x * 4 + warp;
+    if (t >= TL) return;  // warp-uniform
+    float* o = out + (((size_t)b * gridDim.y + s) * TL + t) * kSsastMel;
+    if (t >= 1 + (S - kWin) / kShift) {  // the appended rows (snip_edges: frames of the window that fit)
+        for (int j = lane; j < kSsastMel; j += 32) o[j] = 0.f;
+        return;
+    }
+    const long long L = lens[b], start = (long long)s * S + (long long)t * kShift;
+    const float* w = wavs[b];
+    float x[13];
+#pragma unroll
+    for (int i = 0; i < 13; ++i) {
+        const int n = lane + 32 * i;
+        x[i] = (n < kWin && start + n < L) ? w[start + n] : 0.f;
+    }
+    float* pw = s_pw[warp];
+    frame_power(x, g_hann, s_re[warp], s_im[warp], pw, lane);
+    const float shift = (float)4.2677393, scale = (float)(4.5689974 * 2);
+    for (int j = lane; j < kSsastMel; j += 32) {
+        const int st = g_mel128.start[j], cnt = g_mel128.count[j];
+        const float* mw = g_mel128.w + g_mel128.off[j];
+        float acc = 0.f;
+        for (int i = 0; i < cnt; ++i) acc = fmaf(pw[st + i], mw[i], acc);
+        o[j] = (logf(fmaxf(acc, 1.1920928955078125e-07f)) + shift) / scale;
+    }
+}
+
+cudaError_t launch_ssast_fbank(const float* const* wavs_dev, const long long* lens_dev, int B, int nseg, int S,
+                               int TL, float* out, cudaStream_t s) {
+    if (S < kWin || TL < 1 + (S - kWin) / kShift) return cudaErrorInvalidValue;
+    if (B <= 0 || nseg <= 0) return cudaSuccess;
+    ssast_fbank_kernel<<<dim3((TL + 3) / 4, nseg, B), 128, 0, s>>>(wavs_dev, lens_dev, S, TL, out);
+    return cudaGetLastError();
 }
 
 // ComputeDeltas(win_length=5, mode="replicate") applied to columns [src, src+80) -> [src+80, src+160)

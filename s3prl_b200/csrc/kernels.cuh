@@ -28,10 +28,10 @@ cudaError_t launch_cpc_conv0(const float* x, int B, long long L, int T0, const f
                              cudaStream_t s);
 
 // ---- norm.cu -------------------------------------------------------------------------------------
-// y = LayerNorm_D(x) * gamma + beta (eps 1e-5, biased var), optional GELU; D in {384, 512, 640, 768, 1024, 1280, 1920}.
-// Any of out_f32 / (out_hi,out_lo) may be null. x and out_f32 may alias.
+// y = LayerNorm_D(x) * gamma + beta (biased var; eps 1e-5, SSAST's DeiT blocks 1e-6), optional GELU; D in {384, 512,
+// 640, 768, 1024, 1280, 1920}. Any of out_f32 / (out_hi,out_lo) may be null. x and out_f32 may alias.
 cudaError_t launch_layernorm(const float* x, size_t M, int D, const float* gamma, const float* beta, int gelu,
-                             float* out_f32, const OutPlanes& op, cudaStream_t s);
+                             float* out_f32, const OutPlanes& op, cudaStream_t s, float eps = 1e-5f);
 // modified CPC: y = relu(ChannelNorm_256(x)) (unbiased var, eps 1e-5) of x [B][T][256] into op with R rows per
 // utterance, row r = frame r - pad (zeros outside [0, T)); out_f32 [B][T][256] only with R == T and pad == 0
 cudaError_t launch_channelnorm_relu(const float* x, int B, int T, int R, int pad, const float* gamma,
@@ -67,6 +67,30 @@ cudaError_t init_fbank_tables();
 // device first. m_b >= 2 (m_b == 1 gives NaN, as the reference's unbiased std).
 cudaError_t launch_decoar2_features(const float* const* wavs_dev, const long long* lens_dev, int B, int max_frames,
                                     int T, int frame_step, float* fb, const OutPlanes& op, cudaStream_t s);
+
+// ---- fbank.cu: SSAST's front end -------------------------------------------------------------------------------
+// kaldi fbank (hanning window, 128 mel bins) of each S-sample window of each utterance (zero past lens[b]), normalised
+// (y + 4.2677393) / 9.1379948, rows from 1 + (S - 400) / 160 up to TL zero: out [B * nseg][TL][128], row block
+// b * nseg + s. Needs init_fbank_tables() on this device first.
+cudaError_t launch_ssast_fbank(const float* const* wavs_dev, const long long* lens_dev, int B, int nseg, int S,
+                               int TL, float* out, cudaStream_t s);
+
+// ---- ssast.cu: SSAST's patch operand, tokens and output layout ----------------------------------------------------
+// The patch-embedding GEMM's A operand from the features feat [SB][TL][128]: frame model (patch_f 1) the features
+// themselves as operand planes [SB][TL][128] (the implicit GEMM reads rows t and t + 1 of a segment); patch model
+// (patch_f 12) the 16 x 16 patches at stride 10 gathered into planes [SB][12 * tdim][256], row fi * tdim + ti, column
+// kf * 16 + kt = feat[sb][10 ti + kt][10 fi + kf].
+cudaError_t launch_ssast_patches(const float* feat, int SB, int TL, int patch_f, int tdim, const OutPlanes& op,
+                                 cudaStream_t s);
+// x [SB][2 + P][D] holds the patch GEMM's output (+ bias) in rows 2..: row 0 = cls + pos[0], row 1 = dist + pos[1],
+// row 2 + p += pos[2 + p]
+cudaError_t launch_ssast_tokens(float* x, const float* cls, const float* dist, const float* pos, int SB, int P, int D,
+                                cudaStream_t s);
+// One hidden state from the residual stream x [B * nseg][2 + P][D]: out [B][T][patch_f * D], out[b][t][fi * D + d] =
+// x[b * nseg + t / tdim][2 + fi * tdim + t % tdim][d] (class tokens dropped, frequency patches folded into channels,
+// time trimmed to T <= nseg * tdim). D % 4 == 0.
+cudaError_t launch_ssast_fold(const float* x, int B, int nseg, int P, int tdim, int patch_f, int D, int T, float* out,
+                              cudaStream_t s);
 
 // ---- gru.cu: the GRU recurrence of APC / VQ-APC (cluster-resident W_hh) ------------------------------------------
 static constexpr int kGruHidden = 512;  // hidden size the kernel is built for

@@ -273,6 +273,7 @@ enum ModelKind {
     kLstmStack,     // s3b_decoar_model_create (DeCoAR): fbank + CMVN, post_extract_proj, bidirectional LSTM stack
     kNpcStack,      // s3b_npc_model_create (NPC): fbank + CMVN into ConvBlocks and masked convs
     kCpcStack,      // s3b_cpc_model_create (modified CPC): padded strided conv stack with ChannelNorm into an LSTM stack
+    kSsastEncoder,  // s3b_ssast_model_create (SSAST): windowed 128-bin fbank, patch embedding, pre-LN DeiT encoder
 };
 
 struct s3b_model {
@@ -287,6 +288,12 @@ struct s3b_model {
     // kCpcStack: cfg holds num_layers = the LSTM levels and embed_dim = 256. Weights: conv0_w [256][10], conv0_b and
     // norm0_g / norm0_b (conv 0's ChannelNorm), conv_w[1..4] [256][2 s * 256] (tap_weight_layout), conv_b[1..4] and
     // conv_ln_g / conv_ln_b[1..4]; per LSTM layer wih [1024][256], gru_b = bias_ih + bias_hh, whh [1024][256] fp32
+    // kSsastEncoder: cfg holds the pre-LN encoder (num_layers, embed_dim, ffn_dim, num_heads, layer_norm_first = 1).
+    // Weights: proj_w / proj_b the patch embedding ([768][256], tap_weight_layout for the frame model), cls_tok,
+    // dist_tok [768], pos_tab [2 + P][768]; the blocks in layers (ln1 = norm1, ln2 = norm2, out = attn.proj)
+    s3b_ssast_config ssast = {};
+    DevBuf cls_tok, dist_tok, pos_tab;
+    float ln_eps = 1e-5f;  // eps of the encoder layers' LayerNorms
     std::map<std::string, HostTensor> host;
     bool finalized = false;
     int sm_count = 132;
@@ -394,10 +401,32 @@ static int64_t cpc_frames(int64_t L) {
 // pad zero rows, the Lout(i - 1) input frames (those that fit), zero rows up to s (Lout + 1)
 static int64_t cpc_rows(int64_t Lout, int i) { return kCpcStride[i] * (Lout + 1); }
 
+// SSAST (ssast/expert.py, ast_models.py): S samples per window, TL = S / 160 feature rows, P = patch_f * tdim patches
+// per window (frame model: patch_f 1, tdim TL - 1; patch model: patch_f 12 frequency patches, tdim time patches) and
+// `rate` samples per output frame
+struct SsastGeom {
+    int S, TL, patch_f, tdim, P, rate;
+};
+static SsastGeom ssast_geom(const s3b_ssast_config& c) {
+    SsastGeom g;
+    g.S = c.window_samples, g.TL = g.S / 160;
+    g.patch_f = c.patch ? 12 : 1;
+    g.tdim = c.patch ? (g.TL - 16) / 10 + 1 : g.TL - 1;
+    g.P = g.patch_f * g.tdim;
+    g.rate = c.patch ? 1600 : 160;
+    return g;
+}
+static int64_t ssast_segments(const SsastGeom& g, int64_t L) { return (L + g.S - 1) / g.S; }
+// len(range(0, L, rate)) frames, at most the nseg * tdim the windows make
+static int64_t ssast_frames(const SsastGeom& g, int64_t L) {
+    return L < 1 ? 0 : std::min(ssast_segments(g, L) * g.tdim, (L + g.rate - 1) / g.rate);
+}
+
 // frames of a batch padded to L for this model's front end (m NULL: the conv stack); on the fbank kinds and modified
 // CPC also the valid frames of one utterance of L samples
 static int64_t model_frames(const s3b_model* m, int64_t L) {
     if (m != nullptr && m->kind == kCpcStack) return cpc_frames(L);
+    if (m != nullptr && m->kind == kSsastEncoder) return ssast_frames(ssast_geom(m->ssast), L);
     if (m == nullptr || m->kind == kConvEncoder) return num_frames(L);
     return m->kind == kFbankEncoder ? decoar2_frames(L) : fbank_frames(L);  // the recurrent stacks keep every frame
 }
@@ -589,6 +618,31 @@ extern "C" int s3b_cpc_model_create(const s3b_cpc_config* cfg, s3b_model** out) 
     memset(&m->cfg, 0, sizeof(m->cfg));
     m->cfg.num_layers = cfg->num_layers, m->cfg.embed_dim = cfg->hidden;
     m->kind = kCpcStack;
+    m->scheme = default_scheme();
+    *out = m;
+    return 0;
+}
+
+extern "C" int s3b_ssast_model_create(const s3b_ssast_config* cfg, s3b_model** out) {
+    if (!cfg || !out) return fail("null argument");
+    if (cfg->struct_size != (int32_t)sizeof(s3b_ssast_config))
+        return fail("s3b_ssast_config.struct_size %d != %d (header / library mismatch)", cfg->struct_size,
+                    (int)sizeof(s3b_ssast_config));
+    if (cfg->patch != 0 && cfg->patch != 1) return fail("patch must be 0 (frame model) or 1 (patch model), not %d", cfg->patch);
+    if (cfg->embed_dim != 768 || cfg->num_heads != 12 || cfg->num_layers != 12)
+        return fail("only SSAST base is served: embed_dim 768, num_heads 12, num_layers 12 (got %d, %d, %d)",
+                    cfg->embed_dim, cfg->num_heads, cfg->num_layers);
+    const int min_s = cfg->patch ? 2560 : 400;
+    if (cfg->window_samples < min_s || cfg->window_samples > 160000)
+        return fail("window_samples %d out of range: the %s model needs %d..160000 (one patch of %d frames .. 10 s)",
+                    cfg->window_samples, cfg->patch ? "patch" : "frame", min_s, cfg->patch ? 16 : 2);
+    for (int i = 0; i < 4; ++i)
+        if (cfg->reserved[i] != 0) return fail("s3b_ssast_config.reserved[%d] must be 0", i);
+    s3b_model* m = new s3b_model();
+    m->kind = kSsastEncoder, m->ssast = *cfg;
+    m->cfg.num_layers = cfg->num_layers, m->cfg.embed_dim = cfg->embed_dim, m->cfg.num_heads = cfg->num_heads;
+    m->cfg.ffn_dim = 4 * cfg->embed_dim, m->cfg.layer_norm_first = 1;
+    m->ln_eps = 1e-6f;
     m->scheme = default_scheme();
     *out = m;
     return 0;
@@ -955,6 +1009,52 @@ static int finalize_decoar(s3b_model* m) {
     return 0;
 }
 
+// SSAST (ast_models.py): the patch embedding, class tokens and positional table, then timm's DeiT blocks (norm1 ->
+// attn.qkv [3D][D] with q | k | v rows, 64 per head -> attn.proj; norm2 -> mlp.fc1 -> GELU -> mlp.fc2)
+static int finalize_ssast(s3b_model* m) {
+    const SsastGeom g = ssast_geom(m->ssast);
+    const int D = m->cfg.embed_dim, F = m->cfg.ffn_dim;
+    const HostTensor* t;
+    if (m->ssast.patch) {
+        S3B_OK(need(m, "patch_embed.proj.weight", {D, 1, 16, 16}, &t));
+        S3B_OK(upload_split(m->proj_w, t->data.data(), t->numel(), m->scheme));  // column kf * 16 + kt
+    } else {
+        // [D][1][128 f][2 dt] read as a conv of 2 taps over 128 channels: column dt * 128 + f
+        S3B_OK(need(m, "patch_embed.proj.weight", {D, 1, 128, 2}, &t));
+        const std::vector<float> w = tap_weight_layout(t->data.data(), D, 128, 2, 0, 128);
+        S3B_OK(upload_split(m->proj_w, w.data(), w.size(), m->scheme));
+    }
+    S3B_OK(upload_vec(m, "patch_embed.proj.bias", D, m->proj_b));
+    S3B_OK(need(m, "cls_token", {1, 1, D}, &t));
+    S3B_OK(upload_f32(m->cls_tok, t->data.data(), t->numel()));
+    S3B_OK(need(m, "dist_token", {1, 1, D}, &t));
+    S3B_OK(upload_f32(m->dist_tok, t->data.data(), t->numel()));
+    S3B_OK(need(m, "pos_embed", {1, 2 + g.P, D}, &t));
+    S3B_OK(upload_f32(m->pos_tab, t->data.data(), t->numel()));
+    m->layers.resize(m->cfg.num_layers);
+    for (int l = 0; l < m->cfg.num_layers; ++l) {
+        LayerW& L = m->layers[l];
+        const std::string p = "blocks." + std::to_string(l) + ".";
+        S3B_OK(need(m, p + "attn.qkv.weight", {3 * D, D}, &t));
+        S3B_OK(upload_split(L.qkv, t->data.data(), t->numel(), m->scheme));
+        S3B_OK(upload_vec(m, p + "attn.qkv.bias", 3 * D, L.qkv_b));
+        S3B_OK(need(m, p + "attn.proj.weight", {D, D}, &t));
+        S3B_OK(upload_split(L.out, t->data.data(), t->numel(), m->scheme));
+        S3B_OK(upload_vec(m, p + "attn.proj.bias", D, L.out_b));
+        S3B_OK(upload_vec(m, p + "norm1.weight", D, L.ln1_g));
+        S3B_OK(upload_vec(m, p + "norm1.bias", D, L.ln1_b));
+        S3B_OK(upload_vec(m, p + "norm2.weight", D, L.ln2_g));
+        S3B_OK(upload_vec(m, p + "norm2.bias", D, L.ln2_b));
+        S3B_OK(need(m, p + "mlp.fc1.weight", {F, D}, &t));
+        S3B_OK(upload_split(L.fc1, t->data.data(), t->numel(), m->scheme));
+        S3B_OK(upload_vec(m, p + "mlp.fc1.bias", F, L.fc1_b));
+        S3B_OK(need(m, p + "mlp.fc2.weight", {D, F}, &t));
+        S3B_OK(upload_split(L.fc2, t->data.data(), t->numel(), m->scheme));
+        S3B_OK(upload_vec(m, p + "mlp.fc2.bias", D, L.fc2_b));
+    }
+    return 0;
+}
+
 // The conv-stack and fbank encoders: front end, pos_conv, transformer or Conformer layers, prediction heads
 static int finalize_encoder(s3b_model* m) {
     const s3b_config& c = m->cfg;
@@ -1132,6 +1232,7 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
     case kLstmStack: S3B_OK(finalize_decoar(m)); break;
     case kNpcStack: S3B_OK(finalize_npc(m)); break;
     case kCpcStack: S3B_OK(finalize_cpc(m)); break;
+    case kSsastEncoder: S3B_OK(finalize_ssast(m)); break;
     case kConvEncoder:
     case kFbankEncoder: S3B_OK(finalize_encoder(m)); break;
     }
@@ -1156,6 +1257,7 @@ extern "C" int32_t s3b_num_outputs(const s3b_model* m) {
     case kLstmStack: return m->decoar_all_layers ? m->cfg.num_layers : 1;  // decoar_layers: every layer; decoar: the last
     case kNpcStack: return 2 * m->cfg.num_layers + 1;  // every block, every masked conv, then feat
     case kCpcStack: return 2;                          // the encoder's output, then the last LSTM layer's
+    case kSsastEncoder: return m->cfg.num_layers;      // every block's output
     default: return m->cfg.num_layers + 1 + m->cfg.pred_heads;
     }
 }
@@ -1180,7 +1282,11 @@ extern "C" int s3b_valid_frames(const s3b_model* m, const int64_t* lens, int32_t
     }
     for (int b = 0; b < batch; ++b) {
         int64_t v;
-        if (m->kind != kConvEncoder) {
+        if (m->kind == kSsastEncoder) {
+            // the frames of the utterance's own samples at the downsample rate; every frame is computed
+            const int rate = ssast_geom(m->ssast).rate;
+            v = (lens[b] + rate - 1) / rate;
+        } else if (m->kind != kConvEncoder) {
             // pad_sequence of the per-utterance features (apc/expert.py:47-51, decoar2/expert.py:81-92); modified CPC:
             // the frames of the utterance's own conv chain (0 below 159 samples), though every frame is computed
             v = model_frames(m, lens[b]);
@@ -1532,6 +1638,9 @@ struct Lane {
     int64_t L[kNumConv];
     int T = 0;
     int64_t M = 0;
+    // the encoder's attention batch: SB sequences of ST tokens, M = SB * ST rows. B and T for every model but SSAST,
+    // whose sequences are the B * nseg windows of 2 + P tokens (T is then its output frames).
+    int SB = 0, ST = 0;
     const float** d_wavs = nullptr;
     long long* d_lens = nullptr;
     int* d_kv = nullptr;
@@ -1567,7 +1676,11 @@ struct Fwd : Lane {
     float* proj_out() const {
         return (proj_slot0() || (m->cfg.conformer && m->cfg.layer_norm_first)) ? slot(0) : w->x_f32.as<float>();
     }
-    float* hs(int l) const { return (proj_slot0() && l == 0) ? w->hs0.as<float>() : slot(l); }
+    // SSAST: the residual stream is internal (hidden states are a fold of it), one buffer that every layer updates
+    float* hs(int l) const {
+        if (m->kind == kSsastEncoder) return w->x_f32.as<float>();
+        return (proj_slot0() && l == 0) ? w->hs0.as<float>() : slot(l);
+    }
     // hidden state l has been enqueued completely
     int done(int l) const { return layer_done != nullptr ? layer_done(m, l, st, user) : 0; }
     int prepare();
@@ -1579,7 +1692,7 @@ int Fwd::prepare() {
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, C = kConvDim;
     if (B < 1) return fail("empty batch");
-    const bool cpc = m->kind == kCpcStack;
+    const bool cpc = m->kind == kCpcStack, ssast = m->kind == kSsastEncoder;
     const bool fb = m->kind != kConvEncoder && !cpc;
     const bool recurrent = m->kind == kGruStack || m->kind == kLstmStack;
     {
@@ -1591,9 +1704,14 @@ int Fwd::prepare() {
     if (T64 < 1) return fail_too_short(m, Lmax);
     if ((int64_t)B * (fb ? fbank_frames(Lmax) : L[0]) > 2000000000LL) return fail("batch too large for 32-bit tile indexing");
     T = (int)T64;
-    M = (int64_t)B * T;
-    const int Tp = (T + 7) & ~7;
-    if (layer_stride == 0) layer_stride = (size_t)M * D;
+    SB = B, ST = T;
+    if (ssast) {
+        const SsastGeom g = ssast_geom(m->ssast);
+        SB = (int)(B * ssast_segments(g, Lmax)), ST = g.P + 2;
+    }
+    M = (int64_t)SB * ST;
+    const int STp = (ST + 7) & ~7;
+    if (layer_stride == 0) layer_stride = (size_t)B * T * D * (ssast ? ssast_geom(m->ssast).patch_f : 1);
     if (ffn_out != nullptr && ffn_stride == 0) ffn_stride = (size_t)M * D;
     if (c.relative_position && T > m->rel_table_T) S3B_OK(build_rel_table(m, 2 * T));
     if (c.conformer && T > m->rope_T) S3B_OK(build_rope_table(m, 2 * T));
@@ -1601,7 +1719,7 @@ int Fwd::prepare() {
     // ---- bookkeeping block: pinned host mirror -> one async copy ---------------------------------------------
     const size_t off_lens = (size_t)B * sizeof(void*);
     const size_t off_kv = off_lens + (size_t)B * sizeof(long long);
-    const size_t off_ord = off_kv + (size_t)B * sizeof(int);
+    const size_t off_ord = off_kv + (size_t)SB * sizeof(int);  // kv: the attention's valid keys per sequence
     const size_t off_mask = (off_ord + (recurrent ? (size_t)B * sizeof(int) : 0) + 15) & ~(size_t)15;
     const size_t book_bytes = off_mask + (size_t)M;
     S3B_OK(w->book.ensure(book_bytes));
@@ -1629,6 +1747,8 @@ int Fwd::prepare() {
         for (int b = 0; b < B; ++b) hl[b] = (long long)lens[b];
         for (int b = 0; b < B; ++b)
             for (int t = hk[b]; t < T; ++t) hm[(size_t)b * T + t] = 1;
+        if (ssast)  // no key mask: every token of a window attends to all 2 + P tokens of its window
+            for (int i = 0; i < SB; ++i) hk[i] = ST;
         if (recurrent) {  // group utterances of similar length: a recurrence group stops at its own longest
             int* ho = reinterpret_cast<int*>(hb + off_ord);
             std::vector<int> ord(B);
@@ -1650,7 +1770,12 @@ int Fwd::prepare() {
     d_mask = reinterpret_cast<uint8_t*>(db + off_mask);
 
     // ---- workspace ------------------------------------------------------------------------------------------
-    if (cpc) {
+    if (ssast) {
+        // the windows' features, then the patch GEMM's operand planes
+        const SsastGeom g = ssast_geom(m->ssast);
+        S3B_OK(w->fb_f32.ensure((size_t)SB * g.TL * 128 * 4));
+        S3B_OK(w->ln512_s.ensure(m->ssast.patch ? (size_t)SB * g.P * 256 : (size_t)SB * g.TL * 128));
+    } else if (cpc) {
         // conv i's input (i = 1..4) in its padded layout act[i - 1], conv i's fp32 output, the LSTM's operand planes
         // (encoder output, then each layer's), the input GEMM's output
         S3B_OK(w->wav_pad.ensure((size_t)B * Lmax * 4));
@@ -1694,10 +1819,10 @@ int Fwd::prepare() {
         S3B_OK(w->ctx_s.ensure((size_t)M * D));
         S3B_OK(w->q_s.ensure((size_t)M * D));
         S3B_OK(w->k_s.ensure((size_t)M * D));
-        S3B_OK(w->vt_s.ensure((size_t)D * B * Tp));
+        S3B_OK(w->vt_s.ensure((size_t)D * SB * STp));
         S3B_OK(w->h_s.ensure((size_t)M * F));
         if (c.conformer) S3B_OK(w->glu_f32.ensure((size_t)M * 2 * D * sizeof(float)));
-        else if (posconv4_ok(c)) S3B_OK(w->pos_z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
+        else if (!ssast && posconv4_ok(c)) S3B_OK(w->pos_z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
         if (c.relative_position) S3B_OK(w->gate.ensure((size_t)B * H * T * 4));
         if (c.family == 3 || c.proj_hidden0) S3B_OK(w->hs0.ensure((size_t)M * D * 4));
     }
@@ -1915,12 +2040,15 @@ static int add_transformer_layer(const Lane& lane, int l, std::vector<Step>& ste
     s3b_model* m = lane.m;
     Workspace* w = lane.w;
     const s3b_config& c = m->cfg;
-    const int B = lane.B, T = lane.T, D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, hd = head_dim(c);
+    const int B = lane.SB, T = lane.ST, D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, hd = head_dim(c);
     const int sch = m->scheme;
     const size_t M = (size_t)lane.M;
     const LayerW* W = &m->layers[l];
     const bool pre = c.layer_norm_first != 0, rel = c.relative_position != 0, gru_rel = c.gru_rel_pos != 0;
     const bool last = l == c.num_layers - 1, heads = c.pred_heads > 0;
+    // SSAST's encoder has no final norm on its outputs, and its hidden states are written by the fold step after the layer
+    const bool ssast = m->kind == kSsastEncoder, enc_ln = pre && last && !ssast;
+    const float eps = m->ln_eps;
     const double attn_flops = 4.0 * (double)T * T * D * B;
     float* x1 = w->x1_f32.as<float>();
     float* tmp = w->tmp_f32.as<float>();
@@ -1938,7 +2066,7 @@ static int add_transformer_layer(const Lane& lane, int l, std::vector<Step>& ste
     steps.push_back([=](Fwd& f) {
         if (pre)
             KNORM(m, f.st, launch_layernorm(f.hs(l), M, D, W->ln1_g.as<float>(), W->ln1_b.as<float>(), 0, nullptr,
-                                            w->xs_s.planes(sch), f.st));
+                                            w->xs_s.planes(sch), f.st, eps));
         S3B_OK(run_gemm(f, qkv));
         if (rel)
             KMISC(m, f.st, launch_wavlm_gate(w->xs_s.planes(sch), M, B, T, H, D, gru_rel ? W->grep_w.as<float>() : nullptr,
@@ -1956,7 +2084,7 @@ static int add_transformer_layer(const Lane& lane, int l, std::vector<Step>& ste
         S3B_OK(run_gemm(f, p));
         if (pre)
             KNORM(m, f.st, launch_layernorm(x1, M, D, W->ln2_g.as<float>(), W->ln2_b.as<float>(), 0, nullptr,
-                                            w->x1_s.planes(sch), f.st));
+                                            w->x1_s.planes(sch), f.st, eps));
         else
             KNORM(m, f.st, launch_layernorm(tmp, M, D, W->ln1_g.as<float>(), W->ln1_b.as<float>(), 0, x1,
                                             w->x1_s.planes(sch), f.st));
@@ -1968,18 +2096,18 @@ static int add_transformer_layer(const Lane& lane, int l, std::vector<Step>& ste
         GemmParams p = fc2;
         // pre-LN: the sum IS hidden state l+1 (un-normalised residual stream), except after the last layer
         float* unnorm = (last && f.last_res != nullptr) ? f.last_res : tmp;
-        if (pre) p.out_f32 = last ? unnorm : f.hs(l + 1);
+        if (pre) p.out_f32 = enc_ln ? unnorm : f.hs(l + 1);
         if (f.ffn_out != nullptr) p.out_pre = f.ffn_out + (size_t)l * f.ffn_stride;
         S3B_OK(run_gemm(f, p));
         if (pre) {
-            if (last)  // encoder.layer_norm on the final output (wav2vec2_model.py:3049-3050)
+            if (enc_ln)  // encoder.layer_norm on the final output (wav2vec2_model.py:3049-3050)
                 KNORM(m, f.st, launch_layernorm(unnorm, M, D, m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(), 0,
                                                 f.hs(l + 1), heads ? w->xs_s.planes(sch) : no_planes(), f.st));
         } else {
             KNORM(m, f.st, launch_layernorm(tmp, M, D, W->ln2_g.as<float>(), W->ln2_b.as<float>(), 0, f.hs(l + 1),
                                             !last || heads ? w->xs_s.planes(sch) : no_planes(), f.st));
         }
-        return f.done(l + 1);
+        return ssast ? 0 : f.done(l + 1);
     });
     return 0;
 }
@@ -2287,6 +2415,57 @@ static int add_cpc_stack(const Lane& lane, std::vector<Step>& steps) {
     return 0;
 }
 
+// The patch GEMM of SSAST's embedding over the operand planes A (ssast_patches_kernel), its output (+ bias) written
+// into rows 2.. of each window's 2 + P rows of x. Frame model: a convolution of 2 taps over the TL feature rows of a
+// window (row t reads rows t and t + 1, K = 2 * 128); patch model: a [P][256] x [768][256]^T GEMM per window.
+static int ssast_patch_params(GemmParams& p, const SsastGeom& g, const SplitBuf& A, const SplitBuf& W, int SB, int D,
+                              int scheme, float* x, const float* bias) {
+    const Epi e = epi_f32(x + 2 * (size_t)D, bias);
+    if (g.patch_f == 1) S3B_OK(conv_params(p, A, W, SB, g.TL, g.tdim, 1, D, 128, 128, 2, 0, scheme, e));
+    else S3B_OK(conv_params(p, A, W, SB, g.P, g.P, 1, D, 256, 256, 1, 0, scheme, e));
+    p.out_rows_per_batch = g.P + 2;
+    return 0;
+}
+
+// SSAST's front end (profile category 2): per window the normalised 128-bin fbank, the patch operand, the patch GEMM
+// (category 0) and the token assembly, which leaves layer 0's input in x_f32
+static int add_ssast_frontend(const Lane& lane, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    Workspace* w = lane.w;
+    const SsastGeom g = ssast_geom(m->ssast);
+    const int D = m->cfg.embed_dim, SB = lane.SB, sch = m->scheme;
+    const int nseg = SB / lane.B;
+    GemmParams p;
+    S3B_OK(ssast_patch_params(p, g, w->ln512_s, m->proj_w, SB, D, sch, w->x_f32.as<float>(), m->proj_b.as<float>()));
+    steps.push_back([=](Fwd& f) {
+        S3B_OK(copy_book(lane, f.st));
+        KLAUNCH(m, f.st, CAT_CONV0, 1, 0.0,
+                launch_ssast_fbank(lane.d_wavs, lane.d_lens, lane.B, nseg, g.S, g.TL, w->fb_f32.as<float>(), f.st));
+        KLAUNCH(m, f.st, CAT_CONV0, 1, 0.0,
+                launch_ssast_patches(w->fb_f32.as<float>(), SB, g.TL, g.patch_f, g.tdim, w->ln512_s.planes(sch), f.st));
+        S3B_OK(run_gemm(f, p));
+        KLAUNCH(m, f.st, CAT_CONV0, 1, 0.0,
+                launch_ssast_tokens(w->x_f32.as<float>(), m->cls_tok.as<float>(), m->dist_tok.as<float>(),
+                                    m->pos_tab.as<float>(), SB, g.P, D, f.st));
+        return 0;
+    });
+    return 0;
+}
+
+// after SSAST layer l: its output, class tokens dropped and frequency patches folded into channels, into hidden state
+// l (profile category 4: the only misc kernel of the model)
+static int add_ssast_output(const Lane& lane, int l, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    Workspace* w = lane.w;
+    const SsastGeom g = ssast_geom(m->ssast);
+    const int B = lane.B, nseg = lane.SB / lane.B, T = lane.T, D = m->cfg.embed_dim;
+    steps.push_back([=](Fwd& f) {
+        KMISC(m, f.st, launch_ssast_fold(w->x_f32.as<float>(), B, nseg, g.P, g.tdim, g.patch_f, D, T, f.slot(l), f.st));
+        return f.done(l);
+    });
+    return 0;
+}
+
 // One lane's forward at the lane's shape, in enqueue order
 static int build_steps(const Lane& lane, std::vector<Step>& steps) {
     const s3b_model* m = lane.m;
@@ -2302,6 +2481,13 @@ static int build_steps(const Lane& lane, std::vector<Step>& steps) {
         S3B_OK(add_fbank_frontend(lane, steps));
         return add_npc_stack(lane, steps);
     case kCpcStack: return add_cpc_stack(lane, steps);
+    case kSsastEncoder:
+        S3B_OK(add_ssast_frontend(lane, steps));
+        for (int l = 0; l < c.num_layers; ++l) {
+            S3B_OK(add_transformer_layer(lane, l, steps));
+            S3B_OK(add_ssast_output(lane, l, steps));
+        }
+        return 0;
     case kFbankEncoder:
         S3B_OK(add_fbank_frontend(lane, steps));
         // six empty steps where the conv stack would be: with two lanes they keep lane 1's steps enqueued next to the
@@ -2320,6 +2506,11 @@ static int build_steps(const Lane& lane, std::vector<Step>& steps) {
     for (int l = 0; l < c.num_layers; ++l) S3B_OK(add_transformer_layer(lane, l, steps));
     if (c.pred_heads > 0) S3B_OK(add_pred_heads(lane, steps));
     return 0;
+}
+
+// floats per frame of a hidden state: the encoder width, or SSAST's patch model's 12 frequency patches of it
+static int out_width(const s3b_model* m) {
+    return m->kind == kSsastEncoder ? ssast_geom(m->ssast).patch_f * m->cfg.embed_dim : m->cfg.embed_dim;
 }
 
 // Number of lanes for a batch: S3B_LANES overrides; otherwise two lanes when the batch can be split AND carries at
@@ -2358,7 +2549,7 @@ static int forward_lanes(s3b_model* m, const float* const* wavs, const int64_t* 
     if (T < 1) return fail_too_short(m, Lmax);
     int lanes = std::min((o && o->lanes > 0) ? (int)o->lanes : default_lanes(B, T), max_lanes(m));
     if (lanes > B) lanes = B;
-    const size_t frame = (size_t)T * c.embed_dim;
+    const size_t frame = (size_t)T * out_width(m);
     const size_t layer_stride = (o && o->layer_stride > 0) ? (size_t)o->layer_stride : (size_t)B * frame;
     float* ffn_out = o ? o->ffn_out : nullptr;
     const size_t ffn_stride = (o && o->ffn_layer_stride > 0) ? (size_t)o->ffn_layer_stride : (size_t)B * frame;
@@ -2430,6 +2621,7 @@ extern "C" int s3b_forward_ex(s3b_model* m, const float* const* wavs, const int6
             : m->kind == kNpcStack  ? "an NPC model is a conv stack, it has no feed-forward blocks or layer results"
             : m->kind == kCpcStack  ? "a modified CPC model is a conv stack and an LSTM, it has no feed-forward blocks or "
                                       "layer results"
+            : m->kind == kSsastEncoder ? "the SSAST expert returns only its blocks' outputs (ssast/expert.py)"
             : m->cfg.conformer      ? "a Conformer encoder collects no layer results (wav2vec2_model.py:3199-3200)"
                                     : nullptr;
         if (why != nullptr) return fail("ffn_out / last_residual: %s", why);
@@ -2444,7 +2636,7 @@ static int forward_host_impl(s3b_model* m, const float* const* wavs, const int64
     size_t total = 0;
     for (int b = 0; b < batch; ++b) total += (size_t)lens[b];
     S3B_OK(m->stage_wav.ensure(total * 4));
-    const size_t frame_elems = (size_t)T * m->cfg.embed_dim;
+    const size_t frame_elems = (size_t)T * out_width(m);
     const size_t layer_elems = (size_t)batch * frame_elems;
     if (hidden_dev == nullptr) {
         S3B_OK(m->stage_out.ensure((size_t)s3b_num_outputs(m) * layer_elems * 4));
@@ -3089,6 +3281,14 @@ extern "C" int s3b_gemm_bench(int64_t M, int32_t N, int32_t K, int32_t gelu, int
     return 0;
 }
 
+extern "C" int s3b_layernorm_eps_f32(const float* x, int64_t M, int32_t D, const float* gamma, const float* beta,
+                                     int32_t gelu, float eps, float* out, void* stream) {
+    if (!x || !gamma || !beta || !out) return fail("null argument");
+    if (!(eps > 0.0f)) return fail("eps must be positive");
+    CUDA_OK(launch_layernorm(x, (size_t)M, D, gamma, beta, gelu, out, no_planes(), (cudaStream_t)stream, eps));
+    return 0;
+}
+
 extern "C" int s3b_layernorm_f32(const float* x, int64_t M, int32_t D, const float* gamma, const float* beta,
                                  int32_t gelu, float* out, void* stream) {
     if (!x || !gamma || !beta || !out) return fail("null argument");
@@ -3284,6 +3484,77 @@ static int fbank_cmvn_features(const float* const* wavs, const int64_t* lens, in
     CUDA_OK(cudaMemcpy2DAsync(out, 80 * sizeof(float), dec.p, kDecoar2K * sizeof(float), 80 * sizeof(float), rows,
                               cudaMemcpyDeviceToDevice, st));
     CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+// SSAST's building blocks (add_ssast_frontend, add_ssast_output) on buffers of the call
+extern "C" int s3b_ssast_fbank_f32(const float* const* wavs, const int64_t* lens, int32_t B, int64_t max_len,
+                                   int32_t S, float* out, void* stream) {
+    if (!wavs || !lens || !out) return fail("null argument");
+    if (B < 1) return fail("bad batch %d", B);
+    if (S < 400 || S > 160000) return fail("window_samples %d out of range (400..160000)", S);
+    for (int b = 0; b < B; ++b) {
+        if (wavs[b] == nullptr) return fail("null argument: wavs[%d]", b);
+        if (lens[b] < 1 || lens[b] > max_len) return fail("lens[%d]=%lld out of range", b, (long long)lens[b]);
+    }
+    const int64_t nseg = (max_len + S - 1) / S;
+    if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
+    CUDA_OK(init_fbank_tables());
+    cudaStream_t st = (cudaStream_t)stream;
+    DevBuf book;
+    S3B_OK(book.ensure((size_t)B * (sizeof(void*) + sizeof(long long))));
+    std::vector<long long> hl(lens, lens + B);
+    CUDA_OK(cudaMemcpyAsync(book.p, wavs, (size_t)B * sizeof(void*), cudaMemcpyHostToDevice, st));
+    long long* d_lens = reinterpret_cast<long long*>(book.as<char>() + (size_t)B * sizeof(void*));
+    CUDA_OK(cudaMemcpyAsync(d_lens, hl.data(), (size_t)B * sizeof(long long), cudaMemcpyHostToDevice, st));
+    CUDA_OK(launch_ssast_fbank(book.as<const float*>(), d_lens, B, (int)nseg, S, S / 160, out, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+extern "C" int s3b_ssast_embed_f32(const float* feat, int32_t SB, int32_t TL, int32_t patch, const float* w,
+                                   const float* bias, const float* cls, const float* dist, const float* pos,
+                                   int32_t scheme, float* planes_out, float* out, void* stream) {
+    if (!feat || !w || !bias || !cls || !dist || !pos || !out) return fail("null argument");
+    if (patch != 0 && patch != 1) return fail("patch must be 0 or 1, not %d", patch);
+    if (SB < 1 || TL < (patch ? 16 : 2)) return fail("bad sizes (segments %d, tl %d)", SB, TL);
+    s3b_ssast_config c = {};
+    c.patch = patch, c.window_samples = 160 * TL;
+    const SsastGeom g = ssast_geom(c);
+    const int D = 768, K = 256;
+    int sch = 0;
+    S3B_OK(resolve_scheme(scheme, K, D, &sch));
+    cudaStream_t st = (cudaStream_t)stream;
+    int sms = 0;
+    S3B_OK(device_sm_count(&sms));
+    std::vector<float> wh;
+    S3B_OK(download_f32(w, (size_t)D * K, st, wh));
+    const std::vector<float> wl = patch ? wh : tap_weight_layout(wh.data(), D, 128, 2, 0, 128);
+    SplitBuf ws, as;
+    S3B_OK(upload_split(ws, wl.data(), wl.size(), sch));
+    const size_t an = patch ? (size_t)SB * g.P * K : (size_t)SB * TL * 128;
+    S3B_OK(as.ensure(an));
+    CUDA_OK(launch_ssast_patches(feat, SB, TL, g.patch_f, g.tdim, as.planes(sch), st));
+    if (planes_out != nullptr) CUDA_OK(launch_planes_to_f32(as.planes(sch), an, planes_out, st));
+    GemmParams p;
+    S3B_OK(ssast_patch_params(p, g, as, ws, SB, D, sch, out, bias));
+    CUDA_OK(launch_gemm(p, sms, st));
+    CUDA_OK(launch_ssast_tokens(out, cls, dist, pos, SB, g.P, D, st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+extern "C" int s3b_ssast_fold_f32(const float* x, int32_t B, int32_t nseg, int32_t TL, int32_t patch, int32_t T,
+                                  float* out, void* stream) {
+    if (!x || !out) return fail("null argument");
+    if (patch != 0 && patch != 1) return fail("patch must be 0 or 1, not %d", patch);
+    if (B < 1 || nseg < 1 || TL < (patch ? 16 : 2)) return fail("bad sizes (batch %d, nseg %d, tl %d)", B, nseg, TL);
+    s3b_ssast_config c = {};
+    c.patch = patch, c.window_samples = 160 * TL;
+    const SsastGeom g = ssast_geom(c);
+    if (T < 1 || T > nseg * g.tdim) return fail("t_out %d out of range (1..%d)", T, nseg * g.tdim);
+    CUDA_OK(launch_ssast_fold(x, B, nseg, g.P, g.tdim, g.patch_f, 768, T, out, (cudaStream_t)stream));
+    CUDA_OK(cudaStreamSynchronize((cudaStream_t)stream));
     return 0;
 }
 

@@ -12,8 +12,8 @@ namespace s3b {
 template <int V4>
 __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict__ x, size_t M,
                                                         const float* __restrict__ gamma,
-                                                        const float* __restrict__ beta, int gelu, float* out_f32,
-                                                        const OutPlanes op) {
+                                                        const float* __restrict__ beta, int gelu, float eps,
+                                                        float* out_f32, const OutPlanes op) {
     constexpr int D = V4 * 128;
     const int lane = threadIdx.x & 31;
     const size_t row = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -35,7 +35,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
         const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
         q += (a * a + b * b) + (c * c + d * d);
     }
-    const float rstd = rsqrtf(warp_sum(q) * (1.0f / D) + 1e-5f);
+    const float rstd = rsqrtf(warp_sum(q) * (1.0f / D) + eps);
     const float4* g4 = reinterpret_cast<const float4*>(gamma);
     const float4* b4 = reinterpret_cast<const float4*>(beta);
 #pragma unroll
@@ -54,18 +54,18 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
 }
 
 cudaError_t launch_layernorm(const float* x, size_t M, int D, const float* gamma, const float* beta, int gelu,
-                             float* out_f32, const OutPlanes& op, cudaStream_t s) {
+                             float* out_f32, const OutPlanes& op, cudaStream_t s, float eps) {
     if (M == 0) return cudaSuccess;
     const unsigned blocks = (unsigned)((M + 7) / 8);
     cudaError_t e = cudaSuccess;
     switch (D) {
-        case 384: e = launch_pdl(layernorm_kernel<3>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
-        case 512: e = launch_pdl(layernorm_kernel<4>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
-        case 640: e = launch_pdl(layernorm_kernel<5>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
-        case 768: e = launch_pdl(layernorm_kernel<6>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
-        case 1024: e = launch_pdl(layernorm_kernel<8>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
-        case 1280: e = launch_pdl(layernorm_kernel<10>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
-        case 1920: e = launch_pdl(layernorm_kernel<15>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, out_f32, op); break;
+        case 384: e = launch_pdl(layernorm_kernel<3>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, eps, out_f32, op); break;
+        case 512: e = launch_pdl(layernorm_kernel<4>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, eps, out_f32, op); break;
+        case 640: e = launch_pdl(layernorm_kernel<5>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, eps, out_f32, op); break;
+        case 768: e = launch_pdl(layernorm_kernel<6>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, eps, out_f32, op); break;
+        case 1024: e = launch_pdl(layernorm_kernel<8>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, eps, out_f32, op); break;
+        case 1280: e = launch_pdl(layernorm_kernel<10>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, eps, out_f32, op); break;
+        case 1920: e = launch_pdl(layernorm_kernel<15>, dim3(blocks), dim3(256), 0, s, x, M, gamma, beta, gelu, eps, out_f32, op); break;
         default: return cudaErrorInvalidValue;
     }
     return e;

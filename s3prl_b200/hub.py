@@ -23,6 +23,7 @@ from .upstream.decoar2 import Decoar2Expert
 from .upstream.expert import UpstreamExpert
 from .upstream.lighthubert import LighthubertExpert
 from .upstream.npc import NpcExpert
+from .upstream.ssast import SsastExpert
 
 
 def _entry(name: str, make: Callable, ckpt_required: bool = False, refuse_legacy: bool = False,
@@ -89,6 +90,10 @@ for _name, _kind, _required in (("lighthubert", "small", False), ("lighthubert_s
                                 ("lighthubert_base", "base", False), ("lighthubert_stage1", "stage1", False),
                                 ("lighthubert_local", "small", True), ("lighthubert_url", "small", True)):
     ENTRIES[_name] = _entry(_name, partial(LighthubertExpert, name=_name, kind=_kind), ckpt_required=_required)
+# SSAST (ssast/hubconf.py): the fabricated checkpoint of each model without ckpt, else the local DataParallel file;
+# window_secs as in the reference (1 s for speech commands, 10 s for speaker identification)
+for _name, _kind in (("ssast_frame_base", "frame"), ("ssast_patch_base", "patch")):
+    ENTRIES[_name] = _entry(_name, partial(SsastExpert, name=_name, kind=_kind), url_hint="pass a local checkpoint file")
 globals().update(ENTRIES)
 
 
