@@ -549,6 +549,10 @@ int s3b_layernorm_rope_f32(const float* x, int64_t m, int32_t t, int32_t d, cons
 /* y = LayerNorm_D(x) with epsilon eps, otherwise s3b_layernorm_f32 (SSAST's blocks use 1e-6) */
 int s3b_layernorm_eps_f32(const float* x, int64_t m, int32_t d, const float* gamma, const float* beta, int32_t gelu,
                           float eps, float* out, void* stream);
+/* The same LayerNorm as a pre-LN layer's LN1 / LN2 runs it (SSAST: eps 1e-6): written only as operand planes of fmt
+ * (0 bf16 hi/lo, 1 f16q8), decoded to out [m][d]. */
+int s3b_layernorm_eps_planes_f32(const float* x, int64_t m, int32_t d, const float* gamma, const float* beta, float eps,
+                                 int32_t fmt, float* out, void* stream);
 /* SSAST's front end as a forward runs it: ragged DEVICE waveforms (host array of pointers, host lengths lens[b] in
  * [1, max_len]), nseg = ceil(max_len / window_samples) windows each -> out DEVICE [batch * nseg][TL][128], row block
  * b * nseg + s, TL = window_samples / 160 (the normalised fbank, zero rows appended). */

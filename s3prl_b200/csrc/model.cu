@@ -3289,6 +3289,22 @@ extern "C" int s3b_layernorm_eps_f32(const float* x, int64_t M, int32_t D, const
     return 0;
 }
 
+extern "C" int s3b_layernorm_eps_planes_f32(const float* x, int64_t M, int32_t D, const float* gamma,
+                                            const float* beta, float eps, int32_t fmt, float* out, void* stream) {
+    // a pre-LN layer's LN1 / LN2 as add_transformer_layer launches it: operand planes only, no fp32 copy; decoded here
+    if (!x || !gamma || !beta || !out) return fail("null argument");
+    if (M < 1) return fail("m = %lld must be positive", (long long)M);
+    if (!(eps > 0.0f)) return fail("eps must be positive");
+    if (fmt != 0 && fmt != 1) return fail("fmt must be 0 (bf16 hi/lo) or 1 (f16q8), not %d", fmt);
+    cudaStream_t st = (cudaStream_t)stream;
+    SplitBuf ys;
+    S3B_OK(ys.ensure((size_t)M * D));
+    CUDA_OK(launch_layernorm(x, (size_t)M, D, gamma, beta, 0, nullptr, ys.planes(fmt), st, eps));
+    CUDA_OK(launch_planes_to_f32(ys.planes(fmt), (size_t)M * D, out, st));
+    CUDA_OK(cudaStreamSynchronize(st));  // before ys is freed
+    return 0;
+}
+
 extern "C" int s3b_layernorm_f32(const float* x, int64_t M, int32_t D, const float* gamma, const float* beta,
                                  int32_t gelu, float* out, void* stream) {
     if (!x || !gamma || !beta || !out) return fail("null argument");

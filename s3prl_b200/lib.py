@@ -74,6 +74,7 @@ EXPORTED_SYMBOLS = [
     "s3b_cpc_lstm_max_active_clusters",
     "s3b_layernorm_rope_f32",
     "s3b_layernorm_eps_f32",
+    "s3b_layernorm_eps_planes_f32",
     "s3b_ssast_fbank_f32",
     "s3b_ssast_embed_f32",
     "s3b_ssast_fold_f32",
@@ -379,6 +380,7 @@ def load() -> C.CDLL:
     lib.s3b_lstm_f32.argtypes = [f32p, f32p, f32p, C.POINTER(i32), i32, i32, i32, i32, f32p, f32p, vp]
     lib.s3b_layernorm_rope_f32.argtypes = [f32p, i64, i32, i32, f32p, f32p, C.POINTER(C.c_float), i32, f32p, f32p, vp]
     lib.s3b_layernorm_eps_f32.argtypes = [f32p, i64, i32, f32p, f32p, i32, C.c_float, f32p, vp]
+    lib.s3b_layernorm_eps_planes_f32.argtypes = [f32p, i64, i32, f32p, f32p, C.c_float, i32, f32p, vp]
     lib.s3b_ssast_fbank_f32.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i64, i32, f32p, vp]
     lib.s3b_ssast_embed_f32.argtypes = [f32p, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, i32, f32p, f32p, vp]
     lib.s3b_ssast_fold_f32.argtypes = [f32p, i32, i32, i32, i32, i32, f32p, vp]

@@ -4,18 +4,21 @@ first two also against the operand scheme's emulation). Whole-forward parity, 2e
 dropped k-step or a misplaced column at a shape no block test runs. test_gemm_cluster_gpu.LINEAR_SHAPES does not count:
 it checks bit-identity across cluster sizes, not the values.
 
-The shapes are formed from the served geometries themselves (configs.ARCHS, configs.XLS_R, decoar2.DECOAR2 and
-lighthubert.SUBNETS), so a new geometry fails here, without a GPU, until its shapes have a block test. The recurrent
+The shapes are formed from the served geometries themselves (configs.ARCHS, configs.XLS_R, decoar2.DECOAR2,
+lighthubert.SUBNETS and SSAST's embed / FFN widths and patch shapes), so a new geometry fails here, without a GPU, until
+its shapes have a block test; SSAST's patch GEMM counts as covered through test_ssast_blocks_gpu.PATCH_GEMMS, which
+must keep, for each model, its smallest window and the windows on each side of a 128-row tile. The recurrent
 models' GEMMs are fixed by those models and are stated with the model.cu function that builds each. Convolutions (the
 conv stack, positional conv, NPC, modified CPC's conv 1..4) have block tests of their own and are not listed."""
 from dataclasses import replace
 
-from s3prl_b200.upstream import apc, cpc, decoar, lighthubert
+from s3prl_b200.upstream import apc, cpc, decoar, lighthubert, ssast
 from s3prl_b200.upstream.configs import ARCHS, XLS_R
 from s3prl_b200.upstream.decoar2 import DECOAR2
 from test_blocks_gpu import LINEAR_CASES
 from test_gemm_layouts_gpu import LINEAR_SHAPES, SPLIT_SLICES
 from test_port_shapes_gpu import PORT_LINEARS
+from test_ssast_blocks_gpu import PATCH_GEMMS
 
 CONV_DIM = 512  # model.cu kConvDim: the conv stack's channels, post_extract_proj's K
 FBANK_K = 128  # model.cu kDecoar2K: the 80 fbank bins zero-padded to whole 64-wide k-blocks
@@ -64,9 +67,19 @@ def _linears(arch):
     return shapes
 
 
+def _ssast_linears():
+    """layer -> (N, K) of SSAST's GEMMs: add_transformer_layer's four at the served width, and per model the patch
+    GEMM that ssast_patch_params builds, [fshape x tshape] patch columns into the embedding width."""
+    D, F = ssast.EMBED, ssast.FFN
+    shapes = {"ssast.qkv": (3 * D, D), "ssast.out_proj": (D, D), "ssast.fc1": (F, D), "ssast.fc2": (D, F)}
+    for kind, ((fs, ts), _) in ssast.KINDS.items():
+        shapes[f"ssast_{kind}.patch_embed (model.cu ssast_patch_params)"] = (D, fs * ts)
+    return shapes
+
+
 def _covered():
     return ({(N, K) for _, N, K, _ in PORT_LINEARS} | {(N, K) for K, N in LINEAR_SHAPES}
-            | {(N, K) for _, N, K, *_ in LINEAR_CASES})
+            | {(N, K) for _, N, K, *_ in LINEAR_CASES} | {(N, K) for _, N, K, *_ in PATCH_GEMMS})
 
 
 def _served():
@@ -75,7 +88,7 @@ def _served():
     for gname, arch in _geometries().items():
         for layer, nk in _linears(arch).items():
             served.setdefault(nk, []).append(f"{gname}.{layer}")
-    for layer, nk in FIXED.items():
+    for layer, nk in list(FIXED.items()) + list(_ssast_linears().items()):
         served.setdefault(nk, []).append(layer)
     return served
 
@@ -117,3 +130,22 @@ def test_every_served_column_slice_has_a_block_test():
         have.setdefault((N, K, lda), set()).add(a_off)
     for layer, (N, K, lda) in want.items():
         assert have.get((N, K, lda), set()) == set(range(0, lda, K)), (layer, (N, K, lda))
+
+
+def test_ssast_patch_gemm_table_keeps_its_edges():
+    """test_ssast_blocks_gpu.PATCH_GEMMS runs, for each SSAST model, its smallest window (one time patch) and the
+    windows just below and just above a 128-row M tile (the patch GEMM's rows per window: t_dim for the frame model,
+    P = 12 t_dim for the patch model, which steps by 12), so that a change to the window rules cannot drop them."""
+    for kind in ssast.KINDS:
+        (_, ts), _ = ssast.KINDS[kind]
+        rows_of = {}
+        for _, N, K, k, secs in PATCH_GEMMS:
+            if k == kind:
+                g = ssast.geometry(kind, secs)
+                rows_of[secs] = g["P"]
+                assert (N, K) == (ssast.EMBED, 256)
+        step = ssast.geometry(kind, 10.0)["f_dim"]
+        smallest = ssast.geometry(kind, max(400, ts * 160) / 16000)
+        assert smallest["t_dim"] == 1 and smallest["P"] in rows_of.values(), kind
+        assert any(128 - step <= r < 128 for r in rows_of.values()), (kind, sorted(rows_of.values()))
+        assert any(128 < r <= 128 + step for r in rows_of.values()), (kind, sorted(rows_of.values()))

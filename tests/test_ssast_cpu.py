@@ -15,6 +15,7 @@ GOLDEN = ROOT / "tests" / "golden"
 sys.path.insert(0, str(ROOT / "tests"))
 
 import ssast_oracle as SO  # noqa: E402
+from test_ssast_blocks_gpu import LN_GEOMETRIES, PRETRAINED_T_DIM, SSAST_WINDOWS, TOKENS  # noqa: E402
 
 GOLDENS = ("ssast_frame", "ssast_patch", "ssast_frame_w10", "ssast_patch_w10")
 
@@ -28,6 +29,10 @@ def _reference():
         pytest.skip("the reference (s3prl) is not available")
     ref_runtime.activate()
     timm_shim.install()
+
+
+# every window of the GPU tests' table, with the ids the 1 s and 10 s windows have always had
+WINDOWS = [pytest.param(w.kind, w.secs, id=f"{w.secs!r}-{w.kind}") for w in SSAST_WINDOWS]
 
 
 def _wavs(lens, seed, scale=0.1):
@@ -66,8 +71,22 @@ def _reference_frames(kind, window_secs, max_len):
     return min(nseg * t_dim, len(range(0, max_len, 160 if kind == "frame" else 1600)))
 
 
-@pytest.mark.parametrize("kind", ["frame", "patch"])
-@pytest.mark.parametrize("window_secs", [1.0, 10.0])
+def test_window_table_is_the_geometry_it_claims():
+    """Every row of the GPU tests' window table has the geometry it is there for, read back from ssast.geometry (float
+    rounding in int(window_secs * 16000) can move S by a sample)."""
+    from s3prl_b200.upstream.ssast import geometry
+
+    for w in SSAST_WINDOWS:
+        g = geometry(w.kind, w.secs)
+        assert {k: g[k] for k in w.want} == w.want, (w, g)
+        if w.what == "off the hop":
+            assert g["S"] % 160 != 0, w
+    assert {w.kind for w in SSAST_WINDOWS if w.what == "regrid"} == {"frame", "patch"}
+    assert PRETRAINED_T_DIM == {"frame": 512, "patch": 64}
+    assert {st for _, st in LN_GEOMETRIES} <= set(TOKENS)
+
+
+@pytest.mark.parametrize("kind,window_secs", WINDOWS)
 def test_frame_and_segment_rules(s3b_lib, kind, window_secs):
     from s3prl_b200 import lib
     from s3prl_b200.upstream.ssast import geometry, num_frames, num_segments
@@ -78,7 +97,9 @@ def test_frame_and_segment_rules(s3b_lib, kind, window_secs):
     lib.check(s3b_lib.s3b_ssast_model_create(C.byref(cfg), C.byref(h)))
     try:
         assert s3b_lib.s3b_num_outputs(h) == 12
-        for L in (1, 2, 159, 160, 161, 1599, 1600, 1601, 15999, 16000, 16001, 40000, 159999, 160000, 160001, 480000):
+        S = g["S"]
+        for L in (1, 2, 159, 160, 161, 1599, 1600, 1601, 15999, 16000, 16001, 40000, 159999, 160000, 160001, 480000,
+                  S - 1, S, S + 1, 2 * S - 1, 2 * S, 2 * S + 1):
             T = _reference_frames(kind, window_secs, L)
             assert num_frames(kind, window_secs, L) == T == s3b_lib.s3b_num_frames(h, L), (L, T)
             assert num_segments(g["S"], L) == -(-L // g["S"])
@@ -98,11 +119,12 @@ def test_frame_and_segment_rules(s3b_lib, kind, window_secs):
                                                                                   max(case["lens"])), 768 * f_dim)
 
 
-@pytest.mark.parametrize("kind", ["frame", "patch"])
-@pytest.mark.parametrize("window_secs", [1.0, 10.0])
-def test_pos_embed_regrid_equals_reference(tmp_path, kind, window_secs):
-    """1 s: the time crop (t_dim < p_t_dim) for both models; 10 s: the (8, t_dim) interpolation (t_dim > p_t_dim).
-    The fabricated file loads into the reference's ASTModel, whose fine-tuning constructor re-grids its table."""
+@pytest.mark.parametrize("kind,window_secs", WINDOWS)
+def test_pos_embed_regrid_equals_reference(tmp_path, monkeypatch, kind, window_secs):
+    """Every window of the GPU tests' table: 1 s, the smallest windows and t_dim = p_t_dim - 1 take the time crop
+    (t_dim < p_t_dim); 10 s, t_dim = p_t_dim and p_t_dim + 1 the (8, t_dim) interpolation. The fabricated file loads
+    into the reference's ASTModel, whose fine-tuning constructor re-grids its table. The GPU tests' whole forwards
+    compare against an oracle that reads the same table, so this is what checks it at their windows."""
     _reference()
     from s3prl.upstream.ssast.ast_models import ASTModel
 
@@ -114,7 +136,11 @@ def test_pos_embed_regrid_equals_reference(tmp_path, kind, window_secs):
     (fs, ts), (fst, tst) = KINDS[kind]
     g = geometry(kind, window_secs)
     crop = g["t_dim"] < (1024 - ts) // ts + 1
-    assert crop == (window_secs == 1.0)
+    if window_secs in (1.0, 10.0):
+        assert crop == (window_secs == 1.0)
+    # the fine-tuning constructor loads the file onto CUDA when a device is present: held on the CPU, it re-grids the
+    # table as it does on a machine without one, where prepare_ssast_tensors runs too
+    monkeypatch.setattr(torch.cuda, "is_available", lambda: False)
     model = ASTModel(fshape=fs, tshape=ts, fstride=fst, tstride=tst, input_fdim=128, input_tdim=g["TL"],
                      model_size="base", pretrain_stage=False, load_pretrained_mdl_path=str(path))
     ours = prepare_ssast_tensors(sd, kind, window_secs)
