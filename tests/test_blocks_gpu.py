@@ -77,7 +77,10 @@ def test_linear(s3b_lib, scheme, M, N, K, bias, gelu, res):
     assert mx < 2e-4 * ref.abs().max().item() + 1e-5
 
 
-@pytest.mark.parametrize("D", [512, 768, 1024])
+LAYERNORM_DIMS = [512, 768, 1024]  # eps 1e-5
+
+
+@pytest.mark.parametrize("D", LAYERNORM_DIMS)
 @pytest.mark.parametrize("gelu", [0, 1])
 def test_layernorm(s3b_lib, D, gelu):
     from s3prl_b200 import lib
@@ -95,20 +98,20 @@ def test_layernorm(s3b_lib, D, gelu):
     assert _rel(out, ref) < 2e-6
 
 
-@pytest.mark.parametrize(
-    "B,T,H,valid",
-    [
-        (1, 64, 1, [64]),
-        (2, 200, 2, [200, 130]),
-        (3, 499, 12, [499, 250, 1]),
-        (2, 129, 4, [129, 65]),
-        # BASELINE C3 length (wav2vec2_large 20 s -> T = 999: 16 key blocks, V^T row stride Tp = 1000) and neighbours
-        (2, 999, 16, [999, 640]),
-        (2, 1000, 2, [1000, 961]),
-        (3, 1023, 2, [1023, 1, 513]),
-        (1, 1025, 1, [1025]),
-    ],
-)
+ATTENTION_CASES = [  # (B, T, H, valid frames), 64-wide heads, no bias
+    (1, 64, 1, [64]),
+    (2, 200, 2, [200, 130]),
+    (3, 499, 12, [499, 250, 1]),
+    (2, 129, 4, [129, 65]),
+    # BASELINE C3 length (wav2vec2_large 20 s -> T = 999: 16 key blocks, V^T row stride Tp = 1000) and neighbours
+    (2, 999, 16, [999, 640]),
+    (2, 1000, 2, [1000, 961]),
+    (3, 1023, 2, [1023, 1, 513]),
+    (1, 1025, 1, [1025]),
+]
+
+
+@pytest.mark.parametrize("B,T,H,valid", ATTENTION_CASES)
 def test_attention(s3b_lib, B, T, H, valid):
     from s3prl_b200 import lib
 
@@ -257,12 +260,13 @@ BIAS_CASES = {  # T -> ragged valid_frames (incl. 1, 64, 65 and T); 999 / 1025 r
     999: [999, 640, 65],
     1025: [1025, 64, 1],
 }
+BIAS_HEADS = [12, 16]  # WavLM base / large, 64-wide heads
 
 
 @pytest.mark.parametrize("emb_std", [0.5, 4.0])
 @pytest.mark.parametrize("gate_kind", ["none", "const", "random"])
 @pytest.mark.parametrize("T", sorted(BIAS_CASES))
-@pytest.mark.parametrize("H", [12, 16])
+@pytest.mark.parametrize("H", BIAS_HEADS)
 def test_attention_wavlm_bias(s3b_lib, H, T, gate_kind, emb_std):
     """WavLM relative-position bias through the model's table (launch_wavlm_rel_table, centre / stride as in the model's
     plans), gated per (b, h, q), for a table built for exactly T frames (centre T - 1) and for the model's 4096, with the

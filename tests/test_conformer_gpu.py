@@ -70,12 +70,17 @@ def _bn_params(D, g):
             torch.randn(D, device="cuda", generator=g) * 0.1, torch.rand(D, device="cuda", generator=g) + 0.5)
 
 
+DEPTHWISE_D = 256
+DEPTHWISE_KS = [3, 31]
+DEPTHWISE_TS = [1, 2, 15, 16, 31, 32, 129, 499]
+
+
 @pytest.mark.parametrize("fmt", [0, 1])
-@pytest.mark.parametrize("k", [3, 31])
-@pytest.mark.parametrize("T", [1, 2, 15, 16, 31, 32, 129, 499])
+@pytest.mark.parametrize("k", DEPTHWISE_KS)
+@pytest.mark.parametrize("T", DEPTHWISE_TS)
 def test_depthwise_block(s3b_lib, T, k, fmt):
     g = torch.Generator(device="cuda").manual_seed(T * 100 + k)
-    B, D = 2, 256
+    B, D = 2, DEPTHWISE_D
     x = torch.randn(B, T, 2 * D, device="cuda", generator=g)
     w = torch.randn(D, 1, k, device="cuda", generator=g) / k**0.5
     bn = _bn_params(D, g)
@@ -122,8 +127,11 @@ def _rope_ref(y, T, inv_freq):
     return (yh * cos[:, None, :] + rot * sin[:, None, :]).view(M, D)
 
 
+ROPE_CASES = [(3, 1, 1024), (2, 999, 1024), (1, 4096, 1024), (2, 130, 768)]  # (B, T, D)
+
+
 @pytest.mark.parametrize("fmt", [0, 1])
-@pytest.mark.parametrize("B,T,D", [(3, 1, 1024), (2, 999, 1024), (1, 4096, 1024), (2, 130, 768)])
+@pytest.mark.parametrize("B,T,D", ROPE_CASES)
 def test_layernorm_rope_block(s3b_lib, B, T, D, fmt):
     from s3prl_b200 import lib
 

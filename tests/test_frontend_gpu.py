@@ -255,8 +255,11 @@ def _batch(L0, sid, g):
     return max_len, names, wavs
 
 
+CONV0_BIAS = [False, True]  # conv_bias, in both extractor modes
+
+
 @pytest.mark.parametrize("L0", L0S)
-@pytest.mark.parametrize("bias", [False, True])
+@pytest.mark.parametrize("bias", CONV0_BIAS)
 @pytest.mark.parametrize("filters", ["kaiming", "bank"])
 @pytest.mark.parametrize("fmt", [0, 1])
 def test_groupnorm(s3b_lib, fmt, filters, bias, L0):
@@ -285,7 +288,7 @@ def _near_equal_filters(g):
 
 
 @pytest.mark.parametrize("L0", [1, 4, 5, 256, 257, 513, 3001])
-@pytest.mark.parametrize("bias", [False, True])
+@pytest.mark.parametrize("bias", CONV0_BIAS)
 @pytest.mark.parametrize("filters", ["kaiming", "bank", "near_equal"])
 @pytest.mark.parametrize("fmt", [0, 1])
 def test_layernorm(s3b_lib, fmt, filters, bias, L0):

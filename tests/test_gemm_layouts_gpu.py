@@ -464,8 +464,11 @@ POS_CONFIGS = [  # (D, groups, k, taps per k-block, mode)
     (768, 16, 128, 1, 0),
     (1024, 16, 128, 4, 0),  # large: 64 channels per group
     (1024, 16, 128, 1, 0),
+    (512, 16, 128, 1, 0),  # LightHuBERT student small: 32 channels per group, one tap per k-block (32-column tiles)
     (768, 16, 19, 4, 1),  # data2vec blocks: 19 taps -> 20 (one zero tap)
     (768, 16, 19, 4, 2),
+    (1024, 16, 19, 4, 1),  # data2vec large: five k-blocks of 64-channel groups
+    (1024, 16, 19, 4, 2),
     (1024, 16, 24, 4, 1),  # even k: SamePad drops the last frame
     (1024, 16, 24, 4, 2),
     (768, 16, 3, 4, 1),

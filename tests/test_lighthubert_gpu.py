@@ -35,8 +35,12 @@ def _wavs(lens, seed, scale=0.1):
     return [torch.randn(n, generator=g) * scale for n in lens]
 
 
+NARROW_POS_DIMS = [384, 640]  # D of 16 groups of 24 / 40 channels: the hubert_pruner subnets
+NARROW_LN_DIMS = [384, 640]
+
+
 @pytest.mark.parametrize("T", [1, 2, 127, 128, 998])
-@pytest.mark.parametrize("D", [384, 640])
+@pytest.mark.parametrize("D", NARROW_POS_DIMS)
 @pytest.mark.parametrize("ln", [False, True])
 def test_posconv_four_taps_narrow_groups(s3b_lib, D, T, ln):
     """x + GELU(grouped conv(k = 128) + b) (and the encoder LayerNorm) at 16 groups of 24 / 40 channels, four taps per
@@ -63,7 +67,7 @@ def test_posconv_narrow_groups_refuse_one_tap(s3b_lib):
     assert r != 0 and b"multiple of 4" in s3b_lib.s3b_last_error()
 
 
-@pytest.mark.parametrize("D", [384, 640])
+@pytest.mark.parametrize("D", NARROW_LN_DIMS)
 @pytest.mark.parametrize("gelu", [0, 1])
 def test_layernorm_narrow(s3b_lib, D, gelu):
     from s3prl_b200 import lib

@@ -271,12 +271,16 @@ def _ln_params(D, g):
     return 1.0 + 0.3 * torch.randn(D, device="cuda", generator=g), 0.3 * torch.randn(D, device="cuda", generator=g)
 
 
+LAYERNORM_WIDE_D = 1280  # XLS-R 1B's encoder LayerNorms (eps 1e-5)
+ROPE_WIDTHS = [512, 1280]
+
+
 @pytest.mark.parametrize("M", [1, 7, 8, 9, 1037])
 @pytest.mark.parametrize("gelu", [0, 1])
 def test_layernorm_1280(s3b_lib, gelu, M):
     """XLS-R 1B's pre-LN LayerNorm(1280): 8 rows per 256-thread block, so M % 8 != 0 leaves a partial last block whose
     idle warps must return without writing; the 8 rows after the output stay untouched."""
-    D = 1280
+    D = LAYERNORM_WIDE_D
     g = torch.Generator(device="cuda").manual_seed(M * 2 + gelu)
     x = torch.randn(M, D, device="cuda", generator=g) * 3 + 1
     gamma, beta = _ln_params(D, g)
@@ -291,7 +295,7 @@ def test_layernorm_1280(s3b_lib, gelu, M):
 
 @pytest.mark.parametrize("fmt", [0, 1])
 @pytest.mark.parametrize("B,T", [(3, 1), (2, 130)])
-@pytest.mark.parametrize("D", [512, 1280])
+@pytest.mark.parametrize("D", ROPE_WIDTHS)
 def test_layernorm_rope_widths(s3b_lib, D, B, T, fmt):
     """LayerNorm + RoPE at the two widths the kernel accepts besides 768 and 1024 (8 and 20 heads of 64), in both
     operand-plane formats."""

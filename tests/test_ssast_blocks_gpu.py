@@ -276,6 +276,7 @@ def _ln_eps(s3b_lib, x, gm, bt, eps, fmt=None):
     return out
 
 
+LN_EPS = 1e-6  # the DeiT blocks' LayerNorm eps
 # (windows SB, tokens ST): the smallest windows of both models, the longest short one and both models' 10 s windows
 LN_GEOMETRIES = [(_windows_for(st), st) for st in (3, 14, SHORT_ST, 1001, 1190)]
 
@@ -295,10 +296,10 @@ def test_layernorm_eps_1e6_planes(s3b_lib, SB, ST, fmt):
     x[:small] = 1e-3 * torch.randn(small, D, device="cuda", generator=g)  # variance ~ eps: eps decides the scale
     gm = 1 + 0.3 * torch.randn(D, device="cuda", generator=g)
     bt = 0.3 * torch.randn(D, device="cuda", generator=g)
-    f32 = _ln_eps(s3b_lib, x, gm, bt, 1e-6)
-    planes = _ln_eps(s3b_lib, x, gm, bt, 1e-6, fmt)
+    f32 = _ln_eps(s3b_lib, x, gm, bt, LN_EPS)
+    planes = _ln_eps(s3b_lib, x, gm, bt, LN_EPS, fmt)
     assert torch.equal(planes, _through_planes(f32, fmt)), "planes != planes of the fp32 output"
-    ref = F.layer_norm(x.double(), (D,), gm.double(), bt.double(), 1e-6)
+    ref = F.layer_norm(x.double(), (D,), gm.double(), bt.double(), LN_EPS)
     rep = 2.0**-16 * ref.abs() if fmt == 0 else 2.0**-15 * ref.abs() + 2.0**-21
     bound = 2e-6 * ref.abs().amax(-1, keepdim=True) + rep
     r = ((planes.double() - ref).abs() / bound).max().item()

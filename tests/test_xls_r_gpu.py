@@ -65,8 +65,9 @@ def _attention(q, k, v, valid, H, hd, ctx_format):
     return out
 
 
-HEADS = [(3, 64), (3, 80), (3, 120), (6, 64), (8, 64), (10, 64)]  # (H, hd); H = 6, 8, 10: the LightHuBERT subnets
-HEAD_IDS = ["64", "80", "120", "h6-64", "h8-64", "h10-64"]
+# (H, hd); H = 6, 8, 10: the LightHuBERT subnets; 16 heads of 80 / 120: XLS-R 1B / 2B as served
+HEADS = [(3, 64), (3, 80), (3, 120), (6, 64), (8, 64), (10, 64), (16, 80), (16, 120)]
+HEAD_IDS = ["64", "80", "120", "h6-64", "h8-64", "h10-64", "h16-80", "h16-120"]
 
 
 @pytest.mark.parametrize("fmt", [0, 1])
@@ -151,8 +152,11 @@ def _posconv(x, w, bias, G, k, gamma=None, beta=None, out_fmt=-1):
     return out
 
 
+WIDE_GROUP_DIMS = [1280, 1920]  # D of 16 groups of 80 / 120 channels: XLS-R 1B / 2B
+
+
 @pytest.mark.parametrize("T", [1, 37, 63, 130, 999])
-@pytest.mark.parametrize("D", [1280, 1920])
+@pytest.mark.parametrize("D", WIDE_GROUP_DIMS)
 def test_posconv_wide_groups(s3b_lib, D, T):
     """x + GELU(grouped conv(x) + b), 16 groups of 80 / 120 channels, k = 128 (SamePad drops the last frame), with and
     without the LayerNorm, in fp32 and in both operand-plane formats (planes only through the LayerNorm)."""
@@ -193,11 +197,14 @@ def test_posconv_groups_stay_apart(s3b_lib):
         _check_block(out[..., sl], ref[..., sl], f"posconv group {gi}")
 
 
+LAYERNORM_WIDE_D = 1920  # XLS-R 2B's encoder LayerNorms (eps 1e-5)
+
+
 @pytest.mark.parametrize("gelu", [0, 1])
 def test_layernorm_1920(s3b_lib, gelu):
     from s3prl_b200 import lib
 
-    M, D = 333, 1920
+    M, D = 333, LAYERNORM_WIDE_D
     g = torch.Generator(device="cuda").manual_seed(gelu)
     x = torch.randn(M, D, device="cuda", generator=g) * 3 + 1
     gamma = 1.0 + 0.3 * torch.randn(D, device="cuda", generator=g)
