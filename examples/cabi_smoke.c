@@ -37,7 +37,7 @@ int main(void) {
         (const void*)s3b_cpc_model_create, (const void*)s3b_cpc_conv_f32, (const void*)s3b_cpc_lstm_f32,
         (const void*)s3b_cpc_lstm_max_active_clusters, (const void*)s3b_ssast_model_create,
         (const void*)s3b_layernorm_eps_f32, (const void*)s3b_ssast_fbank_f32, (const void*)s3b_ssast_embed_f32,
-        (const void*)s3b_ssast_fold_f32, (const void*)s3b_layernorm_eps_planes_f32,
+        (const void*)s3b_ssast_fold_f32, (const void*)s3b_layernorm_eps_planes_f32, (const void*)s3b_fbank_cmvn_planes,
     };
     s3b_config cfg;
     int64_t lens[2] = {16000, 800};

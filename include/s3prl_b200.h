@@ -510,6 +510,14 @@ int s3b_decoar2_features_f32(const float* const* wavs, const int64_t* lens, int3
  * out [batch][T][80], T = 1 + (max(lens) - 400) / 160, rows t >= m_b zero; lens[b] >= 560. */
 int s3b_apc_features_f32(const float* const* wavs, const int64_t* lens, int32_t batch, int32_t out_fmt, float* out,
                          void* stream);
+/* The same front end (step 1: APC, DeCoAR, NPC; step 2: DeCoAR 2.0) written into the caller's DEVICE buffers instead of
+ * workspaces of the call, undecoded: logmel [batch][m][80] fp32, the frame kernel's log-mel, m = 1 + (max(lens) - 400)
+ * / 160 (rows past an utterance's frames are not written); planes: the operand planes of out_fmt as the first GEMM reads
+ * them, each [batch][T][128] with T as above, back to back (4 * batch * T * 128 bytes, 4-byte aligned): out_fmt 0 the
+ * bf16 hi plane then the bf16 lo plane, out_fmt 1 the fp16 plane, then the e4m3 plane of the fp16 values, then the
+ * e4m3 plane of the residuals scaled by 2^11. */
+int s3b_fbank_cmvn_planes(const float* const* wavs, const int64_t* lens, int32_t batch, int32_t step, int32_t out_fmt,
+                          float* logmel, void* planes, void* stream);
 /* One APC GRU layer's recurrence as a forward runs it (the model's kernel): xg [batch][t][3H] DEVICE = W_ih x + b_ih
  * (gate order r, z, n), whh [3H][H] and bhh [3H] DEVICE (weight_hh_l0, bias_hh_l0), optional residual [batch][t][H]
  * DEVICE added to the output, lens HOST [batch] valid frames in [0, t]. out [batch][t][H] DEVICE: h_t + residual for

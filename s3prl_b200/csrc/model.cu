@@ -3462,12 +3462,14 @@ extern "C" int s3b_frontend_f32(const float* const* wavs, const int64_t* lens, i
     return 0;
 }
 
-// add_fbank_frontend's step for a DeCoAR 2.0 (step 2) or APC (step 1) model on workspaces of this call; the operand
-// planes decoded, columns 0..79 kept
+// add_fbank_frontend's step for a DeCoAR 2.0 (step 2) or APC (step 1) model. The log-mel and the operand planes go to
+// the caller's logmel / planes when given (s3b_fbank_cmvn_planes), else to workspaces of this call; out (optional):
+// the operand planes decoded, columns 0..79 kept
 static int fbank_cmvn_features(const float* const* wavs, const int64_t* lens, int32_t B, int step, int32_t out_fmt,
-                               float* out, void* stream) {
-    if (!wavs || !lens || !out) return fail("null argument");
+                               float* out, float* logmel, void* planes, void* stream) {
+    if (!wavs || !lens || (!out && !planes)) return fail("null argument");
     if (B < 1) return fail("bad batch %d", B);
+    if (step != 1 && step != 2) return fail("step must be 1 (every frame) or 2 (every second frame), not %d", step);
     if (out_fmt != 0 && out_fmt != 1) return fail("out_fmt must be 0 (bf16 hi/lo) or 1 (f16q8), not %d", out_fmt);
     int64_t max_len = 0;
     for (int b = 0; b < B; ++b) {
@@ -3491,16 +3493,38 @@ static int fbank_cmvn_features(const float* const* wavs, const int64_t* lens, in
     CUDA_OK(cudaMemcpyAsync(book.p, wavs, (size_t)B * sizeof(void*), cudaMemcpyHostToDevice, st));
     long long* d_lens = reinterpret_cast<long long*>(book.as<char>() + (size_t)B * sizeof(void*));
     CUDA_OK(cudaMemcpyAsync(d_lens, hl.data(), (size_t)B * sizeof(long long), cudaMemcpyHostToDevice, st));
-    S3B_OK(fbuf.ensure((size_t)B * mf * 80 * 4));
-    S3B_OK(os.ensure(rows * kDecoar2K));
-    S3B_OK(dec.ensure(rows * kDecoar2K * 4));
-    CUDA_OK(launch_decoar2_features(book.as<const float*>(), d_lens, B, (int)mf, (int)T, step, fbuf.as<float>(),
-                                    os.planes(out_fmt), st));
-    CUDA_OK(launch_planes_to_f32(os.planes(out_fmt), rows * kDecoar2K, dec.as<float>(), st));
-    CUDA_OK(cudaMemcpy2DAsync(out, 80 * sizeof(float), dec.p, kDecoar2K * sizeof(float), 80 * sizeof(float), rows,
-                              cudaMemcpyDeviceToDevice, st));
+    if (logmel == nullptr) {
+        S3B_OK(fbuf.ensure((size_t)B * mf * 80 * 4));
+        logmel = fbuf.as<float>();
+    }
+    OutPlanes op;
+    const size_t elems = rows * kDecoar2K;
+    if (planes != nullptr) {  // the layout s3b_fbank_cmvn_planes documents: whole planes back to back
+        char* p = static_cast<char*>(planes);
+        __nv_bfloat16* p16 = reinterpret_cast<__nv_bfloat16*>(p);
+        op = out_fmt ? OutPlanes{p16, nullptr, reinterpret_cast<uint8_t*>(p + 2 * elems),
+                                 reinterpret_cast<uint8_t*>(p + 3 * elems), 1}
+                     : OutPlanes{p16, reinterpret_cast<__nv_bfloat16*>(p + 2 * elems), nullptr, nullptr, 0};
+    } else {
+        S3B_OK(os.ensure(elems));
+        op = os.planes(out_fmt);
+    }
+    CUDA_OK(launch_decoar2_features(book.as<const float*>(), d_lens, B, (int)mf, (int)T, step, logmel, op, st));
+    if (out != nullptr) {
+        S3B_OK(dec.ensure(elems * 4));
+        CUDA_OK(launch_planes_to_f32(op, elems, dec.as<float>(), st));
+        CUDA_OK(cudaMemcpy2DAsync(out, 80 * sizeof(float), dec.p, kDecoar2K * sizeof(float), 80 * sizeof(float), rows,
+                                  cudaMemcpyDeviceToDevice, st));
+    }
     CUDA_OK(cudaStreamSynchronize(st));
     return 0;
+}
+
+extern "C" int s3b_fbank_cmvn_planes(const float* const* wavs, const int64_t* lens, int32_t B, int32_t step,
+                                     int32_t out_fmt, float* logmel, void* planes, void* stream) {
+    if (!logmel || !planes) return fail("null argument");
+    if (reinterpret_cast<uintptr_t>(planes) % 4 != 0) return fail("planes must be 4-byte aligned");
+    return fbank_cmvn_features(wavs, lens, B, step, out_fmt, nullptr, logmel, planes, stream);
 }
 
 // SSAST's building blocks (add_ssast_frontend, add_ssast_output) on buffers of the call
@@ -3576,12 +3600,14 @@ extern "C" int s3b_ssast_fold_f32(const float* x, int32_t B, int32_t nseg, int32
 
 extern "C" int s3b_decoar2_features_f32(const float* const* wavs, const int64_t* lens, int32_t B, int32_t out_fmt,
                                         float* out, void* stream) {
-    return fbank_cmvn_features(wavs, lens, B, 2, out_fmt, out, stream);
+    if (!out) return fail("null argument");
+    return fbank_cmvn_features(wavs, lens, B, 2, out_fmt, out, nullptr, nullptr, stream);
 }
 
 extern "C" int s3b_apc_features_f32(const float* const* wavs, const int64_t* lens, int32_t B, int32_t out_fmt,
                                     float* out, void* stream) {
-    return fbank_cmvn_features(wavs, lens, B, 1, out_fmt, out, stream);
+    if (!out) return fail("null argument");
+    return fbank_cmvn_features(wavs, lens, B, 1, out_fmt, out, nullptr, nullptr, stream);
 }
 
 extern "C" int s3b_gru_max_active_clusters(int32_t* out) {

@@ -64,6 +64,7 @@ EXPORTED_SYMBOLS = [
     "s3b_conformer_conv_f32",
     "s3b_decoar2_features_f32",
     "s3b_apc_features_f32",
+    "s3b_fbank_cmvn_planes",
     "s3b_gru_f32",
     "s3b_gru_max_active_clusters",
     "s3b_lstm_f32",
@@ -370,6 +371,7 @@ def load() -> C.CDLL:
     lib.s3b_conformer_conv_f32.argtypes = [f32p, i32, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, i32, f32p, vp]
     lib.s3b_decoar2_features_f32.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i32, f32p, vp]
     lib.s3b_apc_features_f32.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i32, f32p, vp]
+    lib.s3b_fbank_cmvn_planes.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i32, i32, f32p, vp, vp]
     lib.s3b_gru_max_active_clusters.argtypes = [C.POINTER(i32)]
     lib.s3b_gru_f32.argtypes = [f32p, f32p, f32p, f32p, C.POINTER(i32), i32, i32, i32, i32, f32p, f32p, vp]
     lib.s3b_lstm_fits.argtypes = [C.POINTER(i32)]

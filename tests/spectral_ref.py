@@ -29,6 +29,8 @@ Bounds (u = 2^-24, one fp32 rounding). Stage by stage, each an absolute bound pe
            so where |E - floor| < dE either side of the max is accepted
   deltas : dD_t <= (2 df_t-2 + df_t-1 + df_t+1 + 2 df_t+2) / 10 + 6u (2|f_t-2| + |f_t-1| + |f_t+1| + 2|f_t+2|) / 10
            + u |D_t| with the replicate-clamped indices; then the same for delta-delta on (D, dD)
+  (DeCoAR 2.0 / APC / DeCoAR / NPC: the same stages up to the log-mel with the hamming window and no deltas, then the
+  CMVN below over all m frames, every step-th row kept: fbank_cmvn_forward, fbank_cmvn_bounds)
   CMVN   : with s the fp64 std and ds <= ||df||_2 / sqrt(m - 1) + 4u s, dmu <= mean(df) + 2u max|f|:
            dz_t <= (df_t + dmu + u |f_t - mu|) / (s - ds) + |z_t| ds / (s - ds) + 3u |z_t|,
            compared only where s >= KAPPA max_t df_t (KAPPA = 10); other columns get structural checks.
@@ -87,6 +89,8 @@ def structured_wav(kind: str, n: int, seed: int = 0) -> torch.Tensor:
         x = 0.5 + 1e-3 * torch.randn(n, generator=g, dtype=torch.float64)
     elif kind == "impulses":
         x = ((torch.arange(n) % 97) == 5).double()
+    elif kind == "clipped":  # a 440 Hz tone at 1.6x full scale, clipped to [-1, 1]
+        x = tone(440.0, 1.6).clamp(-1.0, 1.0)
     elif kind == "int16":  # full int16 scale
         x = structured_wav("chirp", n).double()
         x = torch.round(x / x.abs().max() * 32767.0)
@@ -130,6 +134,15 @@ def povey_window(dtype) -> torch.Tensor:
     return torch.hann_window(WIN, periodic=False, dtype=dtype).pow(0.85)
 
 
+def hamming_window(dtype) -> torch.Tensor:
+    """kaldi's "hamming" (kaldi.py _get_window): 0.54 - 0.46 cos(2 pi n / (N - 1)), evaluated in float64."""
+    n = torch.arange(WIN, dtype=torch.float64)
+    return (0.54 - 0.46 * torch.cos(2 * math.pi * n / (WIN - 1))).to(dtype)
+
+
+WINDOWS = {"povey": povey_window, "hamming": hamming_window}
+
+
 def kaldi_mel_banks(dtype) -> torch.Tensor:
     """get_mel_banks(80 bins, 512-point FFT, 16 kHz, low 20 Hz, high = Nyquist) in `dtype` -> [80, 257]."""
     mel_low, mel_high = 1127.0 * math.log(1.0 + 20.0 / 700.0), 1127.0 * math.log(1.0 + 8000.0 / 700.0)
@@ -141,14 +154,16 @@ def kaldi_mel_banks(dtype) -> torch.Tensor:
     return F.pad(w, (0, 1))
 
 
-def fbank_stages(wav: torch.Tensor, dtype=torch.float64) -> Dict[str, torch.Tensor]:
+def fbank_stages(wav: torch.Tensor, dtype=torch.float64, window: str = "povey",
+                 preemph: float = 0.97) -> Dict[str, torch.Tensor]:
     """Every stage of kaldi fbank + deltas for one utterance: frames [m, 400] after DC removal (d) and after
-    pre-emphasis and window (y), spectrum X [m, 257], power P, mel energies E [m, 80], log-mel f, deltas D and DD."""
+    pre-emphasis and window (y), spectrum X [m, 257], power P, mel energies E [m, 80], log-mel f, deltas D and DD.
+    window: a key of WINDOWS (the fbank baseline's povey, or the hamming of DeCoAR 2.0 / APC / DeCoAR / NPC)."""
     m = num_frames(len(wav))
     frames = wav.to(dtype).unfold(0, WIN, SHIFT)[:m]
     d = frames - frames.mean(dim=1, keepdim=True)
     prev = torch.cat([d[:, :1], d[:, :-1]], dim=1)
-    y = (d - 0.97 * prev) * povey_window(dtype)
+    y = (d - preemph * prev) * WINDOWS[window](dtype)
     X = torch.fft.rfft(F.pad(y, (0, NFFT - WIN)))
     P = X.abs().pow(2)
     E = P @ kaldi_mel_banks(dtype).T
@@ -169,6 +184,18 @@ def deltas(x: torch.Tensor, win_length: int = 5) -> torch.Tensor:
 def cmvn(f: torch.Tensor) -> torch.Tensor:
     """(f - mean) / (1e-10 + unbiased std) per column over dim 0 (NaN for one row, as torch.std)."""
     return (f - f.mean(dim=0, keepdim=True)) / (LOG_EPS + f.std(dim=0, keepdim=True))
+
+
+def cmvn_frames(f: torch.Tensor, step: int) -> torch.Tensor:
+    """DeCoAR 2.0 / APC CMVN (decoar2/audio.py CMVN, apc/audio.py): cmvn over all m frames, then every step-th frame,
+    f[::step] (step 2: DeCoAR 2.0's low frame rate; step 1: APC, DeCoAR and NPC keep every frame)."""
+    return cmvn(f)[::step]
+
+
+def fbank_cmvn_forward(wav: torch.Tensor, step: int, dtype=torch.float64) -> torch.Tensor:
+    """The front end of DeCoAR 2.0 (step 2) and APC / DeCoAR / NPC (step 1) for one utterance: kaldi fbank with the
+    hamming window and 80 bins, no deltas, then cmvn_frames -> [ceil(m / step), 80]."""
+    return cmvn_frames(fbank_stages(wav, dtype, "hamming")["f"], step)
 
 
 def fbank_forward(wavs: Sequence[torch.Tensor], use_cmvn: bool = True, dtype=torch.float64) -> torch.Tensor:
@@ -296,20 +323,35 @@ def cmvn_bound(f: torch.Tensor, df: torch.Tensor):
     return z, dz, cond
 
 
+def logmel_bounds(wav: torch.Tensor, eps_w: float, window: str = "povey") -> Dict[str, torch.Tensor]:
+    """fp64 stages of one utterance (fbank_stages with `window`) and lo/hi, df of an fp32 log-mel of them."""
+    s = fbank_stages(wav, torch.float64, window)
+    dX = frame_error(s["x"], s["d"], s["y"], WINDOWS[window](torch.float64), fbank=True)
+    dE = energy_error(s["X"], dX, kaldi_mel_banks(torch.float64).T, eps_w)
+    lo, hi = log_interval(s["E"], dE, fbank=True)
+    return {**s, "dE": dE, "lo": lo, "hi": hi, "df": torch.maximum(s["f"] - lo, hi - s["f"])}
+
+
+def fbank_cmvn_bounds(wav: torch.Tensor, eps_w: float, step: int) -> Dict[str, torch.Tensor]:
+    """The front end of fbank_cmvn_forward and its bounds: logmel_bounds with the hamming window, then cmvn_bound of
+    the log-mel over all m frames, carried through the decimation: z, dz [ceil(m / step), 80] are the rows t of frame
+    step * t, and the statistics (mean, std and their bounds) stay those of all m frames, so the per-element bound of a
+    kept row is that row's bound before decimation; cond [80] is the columns' conditioning over all m frames."""
+    s = logmel_bounds(wav, eps_w, "hamming")
+    z, dz, cond = cmvn_bound(s["f"], s["df"])
+    return {**s, "z": z[::step], "dz": dz[::step], "cond": cond}
+
+
 def fbank_bounds(wav: torch.Tensor, eps_w: float) -> Dict[str, torch.Tensor]:
     """fp64 stages of one utterance and the bounds of an fp32 implementation of them: lo/hi of the log-mel, df, dD,
     dDD, then the no-CMVN features F [m, 240] with dF, and z, dz, cond of CMVN."""
-    s = fbank_stages(wav, torch.float64)
-    dX = frame_error(s["x"], s["d"], s["y"], povey_window(torch.float64), fbank=True)
-    dE = energy_error(s["X"], dX, kaldi_mel_banks(torch.float64).T, eps_w)
-    lo, hi = log_interval(s["E"], dE, fbank=True)
-    df = torch.maximum(s["f"] - lo, hi - s["f"])
-    dD = delta_error(s["f"], df, s["D"])
+    s = logmel_bounds(wav, eps_w)
+    dD = delta_error(s["f"], s["df"], s["D"])
     dDD = delta_error(s["D"], dD, s["DD"])
     Fe = torch.cat([s["f"], s["D"], s["DD"]], -1)
-    dF = torch.cat([df, dD, dDD], -1)
+    dF = torch.cat([s["df"], dD, dDD], -1)
     z, dz, cond = cmvn_bound(Fe, dF)
-    return {**s, "dE": dE, "lo": lo, "hi": hi, "df": df, "F": Fe, "dF": dF, "z": z, "dz": dz, "cond": cond}
+    return {**s, "F": Fe, "dF": dF, "z": z, "dz": dz, "cond": cond}
 
 
 def stft_bounds(wavs: Sequence[torch.Tensor], feat: str, eps_w: float) -> Dict[str, object]:

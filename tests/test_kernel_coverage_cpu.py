@@ -14,14 +14,22 @@ dropped tap at a configuration no block test runs. Per kernel family:
 - LayerNorm + RoPE (D): test_conformer_gpu.ROPE_CASES, test_port_shapes_gpu.ROPE_WIDTHS;
 - the Conformer's depthwise conv (D, k): test_conformer_gpu.test_depthwise_block and
   test_kernel_coverage_gpu.DEPTHWISE_SERVED;
-- the conv front end (extractor_mode, conv_bias): test_frontend_gpu.test_groupnorm / test_layernorm at CONV0_BIAS.
+- the conv front end (extractor_mode, conv_bias): test_frontend_gpu.test_groupnorm / test_layernorm at CONV0_BIAS;
+- the fbank front end (window, mel bins, step, CMVN, operand format) of APC, VQ-APC, DeCoAR, DeCoAR 2.0 and NPC:
+  test_fbank_frontend_gpu.CONFIGS, formed from the hub entries whose expert is one of those kinds.
 
 The configurations are formed from the served geometries (test_port_coverage_cpu._geometries: configs.ARCHS,
 configs.XLS_R, decoar2.DECOAR2, the LightHuBERT subnets; plus SSAST), with the model.cu rules that pick a
 formulation restated below, so a new geometry fails here, without a GPU, until its configurations have a block test."""
-from s3prl_b200.upstream import lighthubert, ssast
+import inspect
+import sys
+
+from s3prl_b200 import hub
+from s3prl_b200.upstream import apc, decoar, decoar2, lighthubert, npc, ssast
 from test_blocks_gpu import ATTENTION_CASES, BIAS_HEADS, LAYERNORM_DIMS
 from test_conformer_gpu import DEPTHWISE_D, DEPTHWISE_KS, ROPE_CASES
+from test_fbank_frontend_gpu import CMVN_ALL_FRAMES
+from test_fbank_frontend_gpu import CONFIGS as FBANK_CONFIGS
 from test_frontend_gpu import CONV0_BIAS
 from test_gemm_layouts_gpu import POS_CONFIGS
 from test_kernel_coverage_gpu import DEPTHWISE_SERVED
@@ -36,6 +44,10 @@ from test_xls_r_gpu import HEADS, WIDE_GROUP_DIMS
 from test_xls_r_gpu import LAYERNORM_WIDE_D as LN_1920
 
 LN_EPS = 1e-5  # s3b_model's ln_eps and launch_layernorm's default
+# the model kinds add_fbank_frontend serves (model.cu kGruStack, kLstmStack, kFbankEncoder, kNpcStack), by the module
+# of their expert
+FBANK_MODULES = (apc, decoar, decoar2, npc)
+HOP = 160  # kaldi fbank's frame shift in samples
 
 
 # ------------------------------------------------------------------------------------------------
@@ -170,6 +182,33 @@ def _served_frontend():
     return served
 
 
+def _hub_expert(entry):
+    """The expert class a hub entry makes (hub._entry's `make`, unwrapped from its partial); None for the others."""
+    make = inspect.getclosurevars(entry).nonlocals.get("make")
+    return getattr(make, "func", make)
+
+
+def _fbank_step(mod):
+    """model.cu add_fbank_frontend: every second frame for kFbankEncoder (DeCoAR 2.0), else every frame; the
+    module's downsample rate over the hop."""
+    return mod.DOWNSAMPLE_RATE // HOP
+
+
+def _served_fbank_frontend():
+    """(window, mel bins, step, CMVN, operand format) -> hub entries. add_fbank_frontend runs launch_decoar2_features
+    for every fbank kind: fbank_frames_kernel<true> (the hamming window), the expert module's mel bins, CMVN over all
+    frames, written in the model's operand scheme, which S3B_GEMM_SCHEME selects at run time: both formats."""
+    served = {}
+    for name, entry in hub.ENTRIES.items():
+        mod = sys.modules.get(getattr(_hub_expert(entry), "__module__", ""))
+        if mod not in FBANK_MODULES:
+            continue
+        for fmt in (0, 1):
+            key = ("hamming", mod.NUM_MEL_BINS, _fbank_step(mod), CMVN_ALL_FRAMES, fmt)
+            served.setdefault(key, []).append(name)
+    return served
+
+
 FAMILIES = {  # name -> (served, covered)
     "positional conv (D, groups, k, taps per k-block, mode, post-LN)": (_served_posconv, _covered_posconv),
     "attention (H, head dim, bias)": (_served_attention, _covered_attention),
@@ -179,6 +218,7 @@ FAMILIES = {  # name -> (served, covered)
                               lambda: {(DEPTHWISE_D, k) for k in DEPTHWISE_KS} | set(DEPTHWISE_SERVED)),
     "conv front end (extractor_mode, conv_bias)": (
         _served_frontend, lambda: {(m, b) for m in ("default", "layer_norm") for b in CONV0_BIAS}),
+    "fbank front end (window, mel bins, step, CMVN, operand format)": (_served_fbank_frontend, lambda: set(FBANK_CONFIGS)),
 }
 
 
@@ -208,6 +248,10 @@ def test_served_set_is_formed():
     assert (1024, 31) in _served_depthwise()
     assert (ssast.EMBED, 1e-6, 0) in _served_layernorm()
     assert len(lighthubert.SUBNETS) == sum(1 for n in _geometries() if n.startswith("lighthubert."))
+    fb = _served_fbank_frontend()
+    names = {n for models in fb.values() for n in models}
+    assert {"apc", "vq_apc", "decoar", "decoar_layers", "decoar2", "npc", "npc_360hr", "npc_960hr"} <= names
+    assert "decoar2" in fb[("hamming", 80, 2, CMVN_ALL_FRAMES, 1)] and "npc" in fb[("hamming", 80, 1, CMVN_ALL_FRAMES, 0)]
 
 
 def test_posconv_rules_match_the_model():
@@ -231,6 +275,20 @@ def test_every_served_posconv_has_a_block_test():
 
 def test_every_served_attention_has_a_block_test():
     _assert_covered("attention (H, head dim, bias)")
+
+
+def test_fbank_step_rule_matches_the_models():
+    """The step restated from each kind's downsample rate is the decimation its expert's frame count implies:
+    num_frames(n) = ceil(m / step) with m = 1 + (n - 400) // 160 kaldi frames, at lengths on frame edges."""
+    for mod in FBANK_MODULES:
+        step = _fbank_step(mod)
+        for n in (560, 561, 719, 720, 879, 880, 16000, 16001, 328000):
+            assert mod.num_frames(n) == -(-(1 + (n - 400) // HOP) // step), (mod.__name__, n)
+    assert [_fbank_step(mod) for mod in FBANK_MODULES] == [1, 1, 2, 1]
+
+
+def test_every_served_fbank_frontend_has_a_block_test():
+    _assert_covered("fbank front end (window, mel bins, step, CMVN, operand format)")
 
 
 def test_every_served_layernorm_has_a_block_test():

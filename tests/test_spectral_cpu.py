@@ -125,3 +125,87 @@ def test_spectrogram_plan_lengths_match_reference(fx):
         assert t_out == ref.shape[1]
         for b, n in enumerate(final_len):
             assert torch.count_nonzero(ref[b, n:]) == 0
+
+
+# ---- the hamming-window front end of APC, DeCoAR, DeCoAR 2.0 and NPC (tests/test_fbank_frontend_gpu.py) ------------------
+def _frontend_inputs():
+    from test_fbank_frontend_gpu import batches
+
+    return [(kind, w) for items in batches().values() for kind, w in items]
+
+
+def _torch_cmvn(f, step):
+    """The reference's CMVN module on its [1, D, T] layout ((x - mean) / (eps + std) over dim 2), then y[::step]."""
+    y = f.T.unsqueeze(0)
+    y = (y - y.mean(2, keepdim=True)) / (1e-10 + y.std(2, keepdim=True))
+    return y.squeeze(0).T[::step]
+
+
+def test_hamming_frontend_matches_torchaudio_fp64(monkeypatch):
+    """fbank_cmvn_forward against torchaudio's kaldi.fbank(window_type="hamming", 80 bins) plus the reference's CMVN,
+    all in float64, on every input of the GPU test. kaldi.fbank builds its mel banks in fp32 whatever the input dtype;
+    they are checked against kaldi_mel_banks within bank_eps and then replaced by the fp64 banks, so what remains to
+    compare is framing, DC removal, pre-emphasis, the window, the FFT, the floor and the log. The log-mel agrees to
+    1e-10 (the fp32 bounds start near 1e-7), and CMVN to 2e-10 / (1e-10 + std) per column."""
+    from torchaudio.compliance import kaldi
+
+    banks64 = R.kaldi_mel_banks(torch.float64)[:, :-1]
+    get_mel_banks = kaldi.get_mel_banks
+
+    def fp64_banks(*args, **kwargs):
+        b, centers = get_mel_banks(*args, **kwargs)
+        assert b.shape == banks64.shape and (b.double() - banks64).abs().max() <= R.bank_eps("kaldi")
+        return banks64, centers
+
+    monkeypatch.setattr(kaldi, "get_mel_banks", fp64_banks)
+    worst_f = worst_z = 0.0
+    for kind, w in _frontend_inputs():
+        ta = kaldi.fbank(w.double().unsqueeze(0), num_mel_bins=R.NMEL, sample_frequency=R.SR, window_type="hamming")
+        assert ta.dtype == torch.float64
+        f = R.fbank_stages(w, torch.float64, "hamming")["f"]
+        worst_f = max(worst_f, (ta - f).abs().max().item())
+        scale = 1e-10 + f.std(dim=0)
+        for step in (1, 2):
+            z = R.fbank_cmvn_forward(w, step)
+            assert z.shape == (-(-len(f) // step), R.NMEL), kind
+            worst_z = max(worst_z, ((_torch_cmvn(ta, step) - z).abs() * scale).max().item())
+    print(f"hamming front end vs torchaudio fp64: log-mel {worst_f:.2e}, CMVN x (1e-10 + std) {worst_z:.2e}")
+    assert worst_f <= 1e-10 and worst_z <= 2e-10
+
+
+def _biased_std_cmvn(f, step):
+    return ((f - f.mean(dim=0, keepdim=True)) / (R.LOG_EPS + f.std(dim=0, unbiased=False, keepdim=True)))[::step]
+
+
+FRONTEND_MISTAKES = {  # name -> (steps it applies to, the wrong front end from the fp64 stages and the waveform)
+    "biased std": ((1, 2), lambda f, w, step: _biased_std_cmvn(f, step)),
+    "y[1::2] for y[::2]": ((2,), lambda f, w, step: R.cmvn(f)[1::2]),
+    "statistics over the kept frames only": ((2,), lambda f, w, step: R.cmvn(f[::step])),
+    "povey window": ((1, 2), lambda f, w, step: R.cmvn_frames(R.fbank_stages(w, torch.float64, "povey")["f"], step)),
+    "no pre-emphasis": ((1, 2), lambda f, w, step: R.cmvn_frames(
+        R.fbank_stages(w, torch.float64, "hamming", preemph=0.0)["f"], step)),
+}
+
+
+def test_frontend_bounds_reject_plausible_mistakes():
+    """Each plausible wrong formula of the front end lands at least 100 times outside the per-element bound that
+    test_fbank_frontend_gpu holds the kernels to (dz on the conditioned columns), at some element of that test's
+    inputs: a kernel that made one of these mistakes fails there."""
+    eps_w = R.bank_eps("kaldi")
+    worst = {name: (0.0, None) for name in FRONTEND_MISTAKES}
+    for kind, w in _frontend_inputs():
+        s = R.fbank_cmvn_bounds(w, eps_w, 1)
+        for name, (steps, wrong) in FRONTEND_MISTAKES.items():
+            for step in steps:
+                z, dz, cond = s["z"][::step], s["dz"][::step], s["cond"]
+                if len(s["f"][::step]) < 2 or not cond.any():
+                    continue
+                zw = wrong(s["f"], w, step)
+                n = min(len(zw), len(z))
+                r = ((zw[:n] - z[:n]).abs() / dz[:n])[:, cond].max().item()
+                if r > worst[name][0]:
+                    worst[name] = (r, f"{kind} step {step}")
+    print("\nwrong front ends, largest |wrong - fp64| / dz:")
+    for name, (r, where) in worst.items():
+        print(f"  {name:38s} {r:12.1f}  ({where})")
+    assert all(r >= 100 for r, _ in worst.values()), worst
