@@ -38,6 +38,7 @@ int main(void) {
         (const void*)s3b_cpc_lstm_max_active_clusters, (const void*)s3b_ssast_model_create,
         (const void*)s3b_layernorm_eps_f32, (const void*)s3b_ssast_fbank_f32, (const void*)s3b_ssast_embed_f32,
         (const void*)s3b_ssast_fold_f32, (const void*)s3b_layernorm_eps_planes_f32, (const void*)s3b_fbank_cmvn_planes,
+        (const void*)s3b_mae_ast_model_create, (const void*)s3b_mae_ast_fbank_f32, (const void*)s3b_mae_ast_embed_f32,
     };
     s3b_config cfg;
     int64_t lens[2] = {16000, 800};
@@ -174,6 +175,24 @@ int main(void) {
         }
         s3b_model_destroy(m);
         if (valid[0] != 99 || valid[1] != 5) return 22;
+    }
+    {
+        /* MAE-AST frame model: 99 fbank frames -> 49 patches of 2; 800 samples = 3 frames -> 2 valid patches */
+        s3b_mae_ast_config mcfg;
+        s3b_model* m = NULL;
+        memset(&mcfg, 0, sizeof(mcfg));
+        mcfg.struct_size = (int32_t)sizeof(mcfg), mcfg.patch = 0, mcfg.embed_dim = 768, mcfg.num_heads = 12;
+        mcfg.ffn_dim = 3072, mcfg.num_layers = 12, mcfg.sine_pos = 1, mcfg.max_tokens = 48000;
+        if (s3b_mae_ast_model_create(&mcfg, &m) != 0) {
+            printf("s3b_mae_ast_model_create: %s\n", s3b_last_error());
+            return 23;
+        }
+        if (s3b_valid_frames(m, lens, 2, 16000, valid) != 0 || s3b_num_outputs(m) != 12 || s3b_num_frames(m, 16000) != 49) {
+            printf("MAE-AST bookkeeping: %s\n", s3b_last_error());
+            return 24;
+        }
+        s3b_model_destroy(m);
+        if (valid[0] != 49 || valid[1] != 2) return 25;
     }
     return 0;
 }

@@ -197,6 +197,34 @@ typedef struct s3b_ssast_config {
     int32_t reserved[4];    /* 0 */
 } s3b_ssast_config;
 int s3b_ssast_model_create(const s3b_ssast_config* cfg, s3b_model** out);
+/* MAE-AST (s3prl/upstream/mae_ast/{expert,mae_ast}.py): per utterance kaldi fbank (128 mel bins, povey window,
+ * 25 ms / 10 ms, snip_edges), zero-padded to the batch's F = 1 + (max_len - 400) / 160 frames; y = (x - running_mean)
+ * * rsqrt(running_var + 1e-5) * 0.5 on every element (padded frames too); unfold into (kt, kc) patches, (2, 128) for
+ * the frame model and (16, 16) for the patch model: T' = F / kt time patches of nv = 128 / kc frequency patches, token
+ * t * nv + fi, column i * kc + j; post_extract_proj Linear(256, 768); with sine_pos, rows 0 .. T' nv - 1 of the
+ * checkpoint's sinusoid table added to the valid tokens; then num_layers wav2vec 2.0 encoder layers (12 heads of 64,
+ * FFN 3072, exact GELU), post-LN with encoder.layer_norm on their input, or pre-LN without any encoder norm. Keys of
+ * utterance b are valid for its first valid_b = min(ceil(n_b / kt), T') nv tokens, n_b its own fbank frames.
+ * Hidden state l is layer l's output, [batch][T'][nv * 768]. s3b_num_outputs = num_layers; s3b_valid_frames gives
+ * min(ceil(n_b / kt), T'), and refuses lens[b] < 400; s3b_forward_ex refuses ffn_out and last_residual, and a batch of
+ * more than max_tokens tokens when sine_pos is set.
+ * Tensors: post_extract_proj.{weight [768][256], bias}, batch_norm.running_mean [1], batch_norm.running_var [1],
+ * enc_sine_pos_embed.pe [1][max_tokens][768] (sine_pos), encoder.layer_norm.* (post-LN), and per layer
+ * encoder.layers.{l}.self_attn.{q,k,v,out}_proj.*, self_attn_layer_norm.*, fc1.*, fc2.*, final_layer_norm.*; other
+ * keys are ignored. */
+typedef struct s3b_mae_ast_config {
+    int32_t struct_size;      /* sizeof(s3b_mae_ast_config) */
+    int32_t patch;            /* 0 = frame model (2 x 128 patches), 1 = patch model (16 x 16) */
+    int32_t embed_dim;        /* 768 */
+    int32_t num_heads;        /* 12 */
+    int32_t ffn_dim;          /* 3072 */
+    int32_t num_layers;       /* encoder_layers, 1..63 */
+    int32_t layer_norm_first; /* 0 = post-LN, 1 = pre-LN */
+    int32_t sine_pos;         /* enc_sine_pos: 0 or 1 */
+    int32_t max_tokens;       /* rows of enc_sine_pos_embed.pe (sine_pos 1), else 0 */
+    int32_t reserved[4];      /* 0 */
+} s3b_mae_ast_config;
+int s3b_mae_ast_model_create(const s3b_mae_ast_config* cfg, s3b_model** out);
 int s3b_model_finalize(s3b_model* m);
 void s3b_model_destroy(s3b_model* m);
 
@@ -579,6 +607,20 @@ int s3b_ssast_embed_f32(const float* feat, int32_t segments, int32_t tl, int32_t
  * out [batch][t_out][768 or 12 * 768], class tokens dropped, frequency patches folded into channels; t_out <= nseg t_dim. */
 int s3b_ssast_fold_f32(const float* x, int32_t batch, int32_t nseg, int32_t tl, int32_t patch, int32_t t_out,
                        float* out, void* stream);
+/* MAE-AST's front end as a forward runs it: ragged DEVICE waveforms (host array of pointers, host lengths lens[b] in
+ * [400, max_len]), the batch-normalised 128-bin fbank unfolded into the patch operand [batch * T' nv][256] (T' =
+ * (1 + (max_len - 400) / 160) / kt), with y = log-mel * (0.5 / sqrt(running_var + 1e-5)) - running_mean * that.
+ * out (optional): fp32, as the kernel computes it; planes_out (optional): the operand planes of `fmt` (0 bf16 hi/lo,
+ * 1 f16q8) decoded. Both DEVICE. */
+int s3b_mae_ast_fbank_f32(const float* const* wavs, const int64_t* lens, int32_t batch, int64_t max_len, int32_t patch,
+                          float running_mean, float running_var, int32_t fmt, float* out, float* planes_out,
+                          void* stream);
+/* MAE-AST's positions and input norm as a forward runs them, in place on x [batch][n_tok][768] (DEVICE, the
+ * projection's output): x[b][t] += pe[t] for t < valid[b] (host array; pe [>= n_tok][768] DEVICE, or NULL); with
+ * gamma / beta (DEVICE, post-LN) then LayerNorm(eps 1e-5) into x and, when planes_out is given, its operand planes of
+ * `fmt` decoded into planes_out [batch][n_tok][768] (DEVICE). */
+int s3b_mae_ast_embed_f32(float* x, int32_t batch, int32_t n_tok, const int32_t* valid, const float* pe,
+                          const float* gamma, const float* beta, int32_t fmt, float* planes_out, void* stream);
 
 #ifdef __cplusplus
 }

@@ -9,7 +9,8 @@
 // The same frame kernel with a hamming window is the front end of DeCoAR 2.0 (s3prl/upstream/decoar2/audio.py:41-86),
 // followed by decoar2_cmvn_kernel: per-utterance CMVN over all frames, every second frame kept, written as the
 // operand planes of post_extract_proj. With a hanning window and 128 bins, per fixed-length window of the waveform, it
-// is SSAST's front end (ssast_fbank_kernel).
+// is SSAST's front end (ssast_fbank_kernel). With the povey window and 128 bins, batch-normalised and stored straight
+// into spectrogram patches, it is MAE-AST's (mae_ast_fbank_kernel).
 #include <math.h>
 
 #include <vector>
@@ -261,6 +262,67 @@ cudaError_t launch_ssast_fbank(const float* const* wavs_dev, const long long* le
     if (S < kWin || TL < 1 + (S - kWin) / kShift) return cudaErrorInvalidValue;
     if (B <= 0 || nseg <= 0) return cudaSuccess;
     ssast_fbank_kernel<<<dim3((TL + 3) / 4, nseg, B), 128, 0, s>>>(wavs_dev, lens_dev, S, TL, out);
+    return cudaGetLastError();
+}
+
+// MAE-AST's front end (s3prl/upstream/mae_ast/{expert,mae_ast}.py): kaldi fbank of utterance b (povey window, 128 mel
+// bins), y = log-mel * bn_a + bn_c (eval BatchNorm2d(1, affine=False) times 0.5), stored at its unfolded position:
+// frame t, bin j -> row b * T' nv + (t / kt) nv + j / kc, column (t % kt) kc + j % kc of the [B T' nv][kt kc] patch
+// operand. Frames in [n_b, T' kt) hold the batch norm of the zero padding, bn_c; frames from T' kt on are not
+// computed. Written as operand planes `op`, or as fp32 into out_f32 when that is given. grid (T' kt / 4, B), block
+// 128 threads = 4 frames; each lane stores the bin pairs (2 p, 2 p + 1), p = lane, lane + 32.
+__global__ void __launch_bounds__(128) mae_ast_fbank_kernel(const float* const* __restrict__ wavs,
+                                                            const long long* __restrict__ lens, int Tp, int kt,
+                                                            int kc, float bn_a, float bn_c, float* out_f32,
+                                                            OutPlanes op) {
+    __shared__ float s_re[4][kFft], s_im[4][kFft], s_pw[4][kBins + 3];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int b = blockIdx.y;
+    const int t = blockIdx.x * 4 + warp;
+    if (t >= Tp * kt) return;  // warp-uniform
+    const long long L = lens[b];
+    const int n = L < kWin ? 0 : (int)(1 + (L - kWin) / kShift);
+    const int nv = kSsastMel / kc, K = kt * kc;
+    const size_t row0 = (size_t)b * Tp * nv + (size_t)(t / kt) * nv;
+    const int col0 = (t % kt) * kc;
+    float* pw = s_pw[warp];
+    if (t < n) {
+        const float* w = wavs[b] + (size_t)t * kShift;
+        float x[13];
+#pragma unroll
+        for (int i = 0; i < 13; ++i) {
+            const int k = lane + 32 * i;
+            x[i] = k < kWin ? w[k] : 0.f;
+        }
+        frame_power(x, g_tab.window, s_re[warp], s_im[warp], pw, lane);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int j = 2 * (lane + 32 * h);
+        float y[2] = {bn_c, bn_c};
+        if (t < n) {
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+                const int st = g_mel128.start[j + u], cnt = g_mel128.count[j + u];
+                const float* mw = g_mel128.w + g_mel128.off[j + u];
+                float acc = 0.f;
+                for (int i = 0; i < cnt; ++i) acc = fmaf(pw[st + i], mw[i], acc);
+                y[u] = fmaf(logf(fmaxf(acc, 1.1920928955078125e-07f)), bn_a, bn_c);
+            }
+        }
+        const size_t e = (row0 + j / kc) * K + col0 + j % kc;
+        if (out_f32 != nullptr) *reinterpret_cast<float2*>(out_f32 + e) = make_float2(y[0], y[1]);
+        else store_planes2(op, y[0], y[1], e);
+    }
+}
+
+cudaError_t launch_mae_ast_fbank(const float* const* wavs_dev, const long long* lens_dev, int B, int Tp, int kt,
+                                 int kc, float bn_a, float bn_c, float* out_f32, const OutPlanes& op, cudaStream_t s) {
+    if (!((kt == 2 && kc == 128) || (kt == 16 && kc == 16)) || (out_f32 == nullptr && op.hi == nullptr))
+        return cudaErrorInvalidValue;
+    if (B <= 0 || Tp <= 0) return cudaSuccess;
+    mae_ast_fbank_kernel<<<dim3((Tp * kt + 3) / 4, B), 128, 0, s>>>(wavs_dev, lens_dev, Tp, kt, kc, bn_a, bn_c,
+                                                                     out_f32, op);
     return cudaGetLastError();
 }
 

@@ -75,6 +75,20 @@ cudaError_t launch_decoar2_features(const float* const* wavs_dev, const long lon
 cudaError_t launch_ssast_fbank(const float* const* wavs_dev, const long long* lens_dev, int B, int nseg, int S,
                                int TL, float* out, cudaStream_t s);
 
+// ---- fbank.cu: MAE-AST's front end -------------------------------------------------------------------------------
+// kaldi fbank (povey window, 128 mel bins) of each utterance's frames t < T' kt, y = log-mel * bn_a + bn_c (frames
+// t >= n_b: bn_c), unfolded into (kt, kc) patches (kt, kc) = (2, 128) or (16, 16): frame t, bin j -> row
+// b T' nv + (t / kt) nv + j / kc, column (t % kt) kc + j % kc of [B T' nv][kt kc], nv = 128 / kc. Into out_f32 when it
+// is given, else operand planes op. Needs init_fbank_tables() on this device first.
+cudaError_t launch_mae_ast_fbank(const float* const* wavs_dev, const long long* lens_dev, int B, int Tp, int kt,
+                                 int kc, float bn_a, float bn_c, float* out_f32, const OutPlanes& op, cudaStream_t s);
+
+// ---- mae_ast.cu: MAE-AST's positions and input LayerNorm --------------------------------------------------------
+// x [B][N][D] (D = 768) in place: row (b, tok) += pe[tok] where tok < valid[b] (pe [>= N][D], or null: no positions);
+// ln = 1: then LayerNorm(eps 1e-5, gamma, beta) into x and operand planes op (op.hi may be null)
+cudaError_t launch_mae_ast_embed(float* x, int B, int N, int D, const int* valid, const float* pe, int ln,
+                                 const float* gamma, const float* beta, const OutPlanes& op, cudaStream_t s);
+
 // ---- ssast.cu: SSAST's patch operand, tokens and output layout ----------------------------------------------------
 // The patch-embedding GEMM's A operand from the features feat [SB][TL][128]: frame model (patch_f 1) the features
 // themselves as operand planes [SB][TL][128] (the implicit GEMM reads rows t and t + 1 of a segment); patch model

@@ -274,6 +274,7 @@ enum ModelKind {
     kNpcStack,      // s3b_npc_model_create (NPC): fbank + CMVN into ConvBlocks and masked convs
     kCpcStack,      // s3b_cpc_model_create (modified CPC): padded strided conv stack with ChannelNorm into an LSTM stack
     kSsastEncoder,  // s3b_ssast_model_create (SSAST): windowed 128-bin fbank, patch embedding, pre-LN DeiT encoder
+    kMaeAstEncoder,  // s3b_mae_ast_model_create (MAE-AST): 128-bin fbank patches into the wav2vec 2.0 encoder
 };
 
 struct s3b_model {
@@ -293,6 +294,11 @@ struct s3b_model {
     // dist_tok [768], pos_tab [2 + P][768]; the blocks in layers (ln1 = norm1, ln2 = norm2, out = attn.proj)
     s3b_ssast_config ssast = {};
     DevBuf cls_tok, dist_tok, pos_tab;
+    // kMaeAstEncoder: cfg holds the encoder (num_layers, embed_dim, ffn_dim, num_heads, layer_norm_first). Weights:
+    // proj_w / proj_b post_extract_proj [768][256]; pos_tab enc_sine_pos_embed.pe [max_tokens][768] (sine_pos); enc_ln_*
+    // (post-LN); the layers as the wav2vec 2.0 encoder's. The eval batch norm times 0.5 is y = x * mae_bn_a + mae_bn_c.
+    s3b_mae_ast_config mae = {};
+    float mae_bn_a = 0.f, mae_bn_c = 0.f;
     float ln_eps = 1e-5f;  // eps of the encoder layers' LayerNorms
     std::map<std::string, HostTensor> host;
     bool finalized = false;
@@ -422,11 +428,24 @@ static int64_t ssast_frames(const SsastGeom& g, int64_t L) {
     return L < 1 ? 0 : std::min(ssast_segments(g, L) * g.tdim, (L + g.rate - 1) / g.rate);
 }
 
+// MAE-AST (mae_ast/expert.py, mae_ast.py): (kt, kc) patches over the [F][128] fbank image, nv = 128 / kc per time patch;
+// T' = F / kt output frames (time patches) of nv * 768 floats
+struct MaeAstGeom {
+    int kt, kc, nv;
+};
+static MaeAstGeom mae_ast_geom(const s3b_mae_ast_config& c) {
+    MaeAstGeom g;
+    g.kt = c.patch ? 16 : 2, g.kc = c.patch ? 16 : 128;
+    g.nv = 128 / g.kc;
+    return g;
+}
+
 // frames of a batch padded to L for this model's front end (m NULL: the conv stack); on the fbank kinds and modified
 // CPC also the valid frames of one utterance of L samples
 static int64_t model_frames(const s3b_model* m, int64_t L) {
     if (m != nullptr && m->kind == kCpcStack) return cpc_frames(L);
     if (m != nullptr && m->kind == kSsastEncoder) return ssast_frames(ssast_geom(m->ssast), L);
+    if (m != nullptr && m->kind == kMaeAstEncoder) return fbank_frames(L) / mae_ast_geom(m->mae).kt;
     if (m == nullptr || m->kind == kConvEncoder) return num_frames(L);
     return m->kind == kFbankEncoder ? decoar2_frames(L) : fbank_frames(L);  // the recurrent stacks keep every frame
 }
@@ -643,6 +662,33 @@ extern "C" int s3b_ssast_model_create(const s3b_ssast_config* cfg, s3b_model** o
     m->cfg.num_layers = cfg->num_layers, m->cfg.embed_dim = cfg->embed_dim, m->cfg.num_heads = cfg->num_heads;
     m->cfg.ffn_dim = 4 * cfg->embed_dim, m->cfg.layer_norm_first = 1;
     m->ln_eps = 1e-6f;
+    m->scheme = default_scheme();
+    *out = m;
+    return 0;
+}
+
+extern "C" int s3b_mae_ast_model_create(const s3b_mae_ast_config* cfg, s3b_model** out) {
+    if (!cfg || !out) return fail("null argument");
+    if (cfg->struct_size != (int32_t)sizeof(s3b_mae_ast_config))
+        return fail("s3b_mae_ast_config.struct_size %d != %d (header / library mismatch)", cfg->struct_size,
+                    (int)sizeof(s3b_mae_ast_config));
+    if (cfg->patch != 0 && cfg->patch != 1) return fail("patch must be 0 (frame model) or 1 (patch model), not %d", cfg->patch);
+    if (cfg->embed_dim != 768 || cfg->num_heads != 12 || cfg->ffn_dim != 3072)
+        return fail("embed_dim %d, num_heads %d, ffn_dim %d: MAE-AST is served with 768, 12 and 3072", cfg->embed_dim,
+                    cfg->num_heads, cfg->ffn_dim);
+    if (cfg->num_layers < 1 || cfg->num_layers > 63) return fail("num_layers %d: must be 1..63", cfg->num_layers);
+    if (cfg->layer_norm_first != 0 && cfg->layer_norm_first != 1)
+        return fail("layer_norm_first must be 0 or 1, not %d", cfg->layer_norm_first);
+    if (cfg->sine_pos != 0 && cfg->sine_pos != 1) return fail("sine_pos must be 0 or 1, not %d", cfg->sine_pos);
+    if (cfg->sine_pos ? cfg->max_tokens < 1 : cfg->max_tokens != 0)
+        return fail("max_tokens %d: the rows of enc_sine_pos_embed.pe (>= 1) with sine_pos, 0 without", cfg->max_tokens);
+    for (int i = 0; i < 4; ++i)
+        if (cfg->reserved[i] != 0) return fail("s3b_mae_ast_config.reserved[%d] must be 0", i);
+    s3b_model* m = new s3b_model();
+    memset(&m->cfg, 0, sizeof(m->cfg));
+    m->kind = kMaeAstEncoder, m->mae = *cfg;
+    m->cfg.num_layers = cfg->num_layers, m->cfg.embed_dim = cfg->embed_dim, m->cfg.num_heads = cfg->num_heads;
+    m->cfg.ffn_dim = cfg->ffn_dim, m->cfg.layer_norm_first = cfg->layer_norm_first;
     m->scheme = default_scheme();
     *out = m;
     return 0;
@@ -1055,10 +1101,74 @@ static int finalize_ssast(s3b_model* m) {
     return 0;
 }
 
+// A wav2vec 2.0 TransformerSentenceEncoderLayer's weights (q | k | v stacked into one [3D][D] QKV matrix) from
+// encoder.layers.{l}.* into m->layers[l]
+static int upload_encoder_layer(s3b_model* m, int l) {
+    const int D = m->cfg.embed_dim, F = m->cfg.ffn_dim;
+    LayerW& L = m->layers[l];
+    const std::string p = "encoder.layers." + std::to_string(l) + ".";
+    const HostTensor *t, *wq, *wk, *wv, *bq, *bk, *bv;
+    S3B_OK(need(m, p + "self_attn.q_proj.weight", {D, D}, &wq));
+    S3B_OK(need(m, p + "self_attn.k_proj.weight", {D, D}, &wk));
+    S3B_OK(need(m, p + "self_attn.v_proj.weight", {D, D}, &wv));
+    S3B_OK(need(m, p + "self_attn.q_proj.bias", {D}, &bq));
+    S3B_OK(need(m, p + "self_attn.k_proj.bias", {D}, &bk));
+    S3B_OK(need(m, p + "self_attn.v_proj.bias", {D}, &bv));
+    std::vector<float> w((size_t)3 * D * D), b((size_t)3 * D);
+    memcpy(w.data(), wq->data.data(), (size_t)D * D * 4);
+    memcpy(w.data() + (size_t)D * D, wk->data.data(), (size_t)D * D * 4);
+    memcpy(w.data() + (size_t)2 * D * D, wv->data.data(), (size_t)D * D * 4);
+    memcpy(b.data(), bq->data.data(), D * 4), memcpy(b.data() + D, bk->data.data(), D * 4);
+    memcpy(b.data() + 2 * D, bv->data.data(), D * 4);
+    S3B_OK(upload_split(L.qkv, w.data(), w.size(), m->scheme));
+    S3B_OK(upload_f32(L.qkv_b, b.data(), b.size()));
+    S3B_OK(need(m, p + "self_attn.out_proj.weight", {D, D}, &t));
+    S3B_OK(upload_split(L.out, t->data.data(), t->numel(), m->scheme));
+    S3B_OK(upload_vec(m, p + "self_attn.out_proj.bias", D, L.out_b));
+    S3B_OK(upload_vec(m, p + "self_attn_layer_norm.weight", D, L.ln1_g));
+    S3B_OK(upload_vec(m, p + "self_attn_layer_norm.bias", D, L.ln1_b));
+    S3B_OK(need(m, p + "fc1.weight", {F, D}, &t));
+    S3B_OK(upload_split(L.fc1, t->data.data(), t->numel(), m->scheme));
+    S3B_OK(upload_vec(m, p + "fc1.bias", F, L.fc1_b));
+    S3B_OK(need(m, p + "fc2.weight", {D, F}, &t));
+    S3B_OK(upload_split(L.fc2, t->data.data(), t->numel(), m->scheme));
+    S3B_OK(upload_vec(m, p + "fc2.bias", D, L.fc2_b));
+    S3B_OK(upload_vec(m, p + "final_layer_norm.weight", D, L.ln2_g));
+    S3B_OK(upload_vec(m, p + "final_layer_norm.bias", D, L.ln2_b));
+    return 0;
+}
+
+// MAE-AST (mae_ast.py): post_extract_proj over the unfolded patches, the eval batch norm folded into one affine map,
+// the checkpoint's own sinusoid table (a persistent buffer that strict loading reads from the file), and the wav2vec 2.0
+// encoder layers; encoder.layer_norm on the input of a post-LN encoder
+static int finalize_mae_ast(s3b_model* m) {
+    const int D = m->cfg.embed_dim;
+    const HostTensor* t;
+    S3B_OK(need(m, "post_extract_proj.weight", {D, 256}, &t));
+    S3B_OK(upload_split(m->proj_w, t->data.data(), t->numel(), m->scheme));
+    S3B_OK(upload_vec(m, "post_extract_proj.bias", D, m->proj_b));
+    const HostTensor *rm, *rv;
+    S3B_OK(need(m, "batch_norm.running_mean", {1}, &rm));
+    S3B_OK(need(m, "batch_norm.running_var", {1}, &rv));
+    const double a = 0.5 / sqrt((double)rv->data[0] + 1e-5);
+    m->mae_bn_a = (float)a, m->mae_bn_c = (float)(-(double)rm->data[0] * a);
+    if (m->mae.sine_pos) {
+        S3B_OK(need(m, "enc_sine_pos_embed.pe", {1, m->mae.max_tokens, D}, &t));
+        S3B_OK(upload_f32(m->pos_tab, t->data.data(), t->numel()));
+    }
+    if (!m->cfg.layer_norm_first) {
+        S3B_OK(upload_vec(m, "encoder.layer_norm.weight", D, m->enc_ln_g));
+        S3B_OK(upload_vec(m, "encoder.layer_norm.bias", D, m->enc_ln_b));
+    }
+    m->layers.resize(m->cfg.num_layers);
+    for (int l = 0; l < m->cfg.num_layers; ++l) S3B_OK(upload_encoder_layer(m, l));
+    return 0;
+}
+
 // The conv-stack and fbank encoders: front end, pos_conv, transformer or Conformer layers, prediction heads
 static int finalize_encoder(s3b_model* m) {
     const s3b_config& c = m->cfg;
-    const int D = c.embed_dim, F = c.ffn_dim, C = kConvDim;
+    const int D = c.embed_dim, C = kConvDim;
     const HostTensor* t;
     const std::string fe = "feature_extractor.conv_layers.";
 
@@ -1153,34 +1263,7 @@ static int finalize_encoder(s3b_model* m) {
     for (int l = 0; l < c.num_layers && !c.conformer; ++l) {
         LayerW& L = m->layers[l];
         const std::string p = "encoder.layers." + std::to_string(l) + ".";
-        const HostTensor *wq, *wk, *wv, *bq, *bk, *bv;
-        S3B_OK(need(m, p + "self_attn.q_proj.weight", {D, D}, &wq));
-        S3B_OK(need(m, p + "self_attn.k_proj.weight", {D, D}, &wk));
-        S3B_OK(need(m, p + "self_attn.v_proj.weight", {D, D}, &wv));
-        S3B_OK(need(m, p + "self_attn.q_proj.bias", {D}, &bq));
-        S3B_OK(need(m, p + "self_attn.k_proj.bias", {D}, &bk));
-        S3B_OK(need(m, p + "self_attn.v_proj.bias", {D}, &bv));
-        std::vector<float> w((size_t)3 * D * D), b((size_t)3 * D);
-        memcpy(w.data(), wq->data.data(), (size_t)D * D * 4);
-        memcpy(w.data() + (size_t)D * D, wk->data.data(), (size_t)D * D * 4);
-        memcpy(w.data() + (size_t)2 * D * D, wv->data.data(), (size_t)D * D * 4);
-        memcpy(b.data(), bq->data.data(), D * 4), memcpy(b.data() + D, bk->data.data(), D * 4);
-        memcpy(b.data() + 2 * D, bv->data.data(), D * 4);
-        S3B_OK(upload_split(L.qkv, w.data(), w.size(), m->scheme));
-        S3B_OK(upload_f32(L.qkv_b, b.data(), b.size()));
-        S3B_OK(need(m, p + "self_attn.out_proj.weight", {D, D}, &t));
-        S3B_OK(upload_split(L.out, t->data.data(), t->numel(), m->scheme));
-        S3B_OK(upload_vec(m, p + "self_attn.out_proj.bias", D, L.out_b));
-        S3B_OK(upload_vec(m, p + "self_attn_layer_norm.weight", D, L.ln1_g));
-        S3B_OK(upload_vec(m, p + "self_attn_layer_norm.bias", D, L.ln1_b));
-        S3B_OK(need(m, p + "fc1.weight", {F, D}, &t));
-        S3B_OK(upload_split(L.fc1, t->data.data(), t->numel(), m->scheme));
-        S3B_OK(upload_vec(m, p + "fc1.bias", F, L.fc1_b));
-        S3B_OK(need(m, p + "fc2.weight", {D, F}, &t));
-        S3B_OK(upload_split(L.fc2, t->data.data(), t->numel(), m->scheme));
-        S3B_OK(upload_vec(m, p + "fc2.bias", D, L.fc2_b));
-        S3B_OK(upload_vec(m, p + "final_layer_norm.weight", D, L.ln2_g));
-        S3B_OK(upload_vec(m, p + "final_layer_norm.bias", D, L.ln2_b));
+        S3B_OK(upload_encoder_layer(m, l));
         if (c.relative_position && c.gru_rel_pos) {
             S3B_OK(need(m, p + "self_attn.grep_linear.weight", {8, 64}, &t));
             S3B_OK(upload_f32(L.grep_w, t->data.data(), t->numel()));
@@ -1233,6 +1316,7 @@ extern "C" int s3b_model_finalize(s3b_model* m) {
     case kNpcStack: S3B_OK(finalize_npc(m)); break;
     case kCpcStack: S3B_OK(finalize_cpc(m)); break;
     case kSsastEncoder: S3B_OK(finalize_ssast(m)); break;
+    case kMaeAstEncoder: S3B_OK(finalize_mae_ast(m)); break;
     case kConvEncoder:
     case kFbankEncoder: S3B_OK(finalize_encoder(m)); break;
     }
@@ -1258,6 +1342,7 @@ extern "C" int32_t s3b_num_outputs(const s3b_model* m) {
     case kNpcStack: return 2 * m->cfg.num_layers + 1;  // every block, every masked conv, then feat
     case kCpcStack: return 2;                          // the encoder's output, then the last LSTM layer's
     case kSsastEncoder: return m->cfg.num_layers;      // every block's output
+    case kMaeAstEncoder: return m->cfg.num_layers;     // every layer's output
     default: return m->cfg.num_layers + 1 + m->cfg.pred_heads;
     }
 }
@@ -1278,6 +1363,8 @@ extern "C" int s3b_valid_frames(const s3b_model* m, const int64_t* lens, int32_t
         if (fbank_model != nullptr && lens[b] < kDecoar2MinLen)
             return fail("lens[%d]=%lld: %s needs >= %lld samples (2 fbank frames; the CMVN std of one frame is NaN)", b,
                         (long long)lens[b], fbank_model, (long long)kDecoar2MinLen);
+        if (m->kind == kMaeAstEncoder && lens[b] < 400)
+            return fail("lens[%d]=%lld: MAE-AST needs >= 400 samples (one fbank frame)", b, (long long)lens[b]);
         any_pad |= lens[b] < max_len;
     }
     for (int b = 0; b < batch; ++b) {
@@ -1286,6 +1373,11 @@ extern "C" int s3b_valid_frames(const s3b_model* m, const int64_t* lens, int32_t
             // the frames of the utterance's own samples at the downsample rate; every frame is computed
             const int rate = ssast_geom(m->ssast).rate;
             v = (lens[b] + rate - 1) / rate;
+        } else if (m->kind == kMaeAstEncoder) {
+            // the reference's key mask (mae_ast.py forward_padding_mask): ceil(n_b / kt) patches; a partly padded last
+            // patch is valid
+            const int kt = mae_ast_geom(m->mae).kt;
+            v = (fbank_frames(lens[b]) + kt - 1) / kt;
         } else if (m->kind != kConvEncoder) {
             // pad_sequence of the per-utterance features (apc/expert.py:47-51, decoar2/expert.py:81-92); modified CPC:
             // the frames of the utterance's own conv chain (0 below 159 samples), though every frame is computed
@@ -1677,8 +1769,10 @@ struct Fwd : Lane {
         return (proj_slot0() || (m->cfg.conformer && m->cfg.layer_norm_first)) ? slot(0) : w->x_f32.as<float>();
     }
     // SSAST: the residual stream is internal (hidden states are a fold of it), one buffer that every layer updates
+    // MAE-AST: hidden state l is layer l's output, slot l; the layers' input (the embedding) is internal
     float* hs(int l) const {
         if (m->kind == kSsastEncoder) return w->x_f32.as<float>();
+        if (m->kind == kMaeAstEncoder) return l == 0 ? w->x_f32.as<float>() : slot(l - 1);
         return (proj_slot0() && l == 0) ? w->hs0.as<float>() : slot(l);
     }
     // hidden state l has been enqueued completely
@@ -1687,12 +1781,13 @@ struct Fwd : Lane {
 };
 
 static int build_steps(const Lane& lane, std::vector<Step>& steps);
+static int out_width(const s3b_model* m);
 
 int Fwd::prepare() {
     const s3b_config& c = m->cfg;
     const int D = c.embed_dim, F = c.ffn_dim, H = c.num_heads, C = kConvDim;
     if (B < 1) return fail("empty batch");
-    const bool cpc = m->kind == kCpcStack, ssast = m->kind == kSsastEncoder;
+    const bool cpc = m->kind == kCpcStack, ssast = m->kind == kSsastEncoder, mae = m->kind == kMaeAstEncoder;
     const bool fb = m->kind != kConvEncoder && !cpc;
     const bool recurrent = m->kind == kGruStack || m->kind == kLstmStack;
     {
@@ -1709,9 +1804,15 @@ int Fwd::prepare() {
         const SsastGeom g = ssast_geom(m->ssast);
         SB = (int)(B * ssast_segments(g, Lmax)), ST = g.P + 2;
     }
+    if (mae) {
+        ST = T * mae_ast_geom(m->mae).nv;
+        if (m->mae.sine_pos && ST > m->mae.max_tokens)
+            return fail("max_len %lld gives %d tokens: enc_sine_pos_embed.pe has %d rows (max_token_length)",
+                        (long long)Lmax, ST, m->mae.max_tokens);
+    }
     M = (int64_t)SB * ST;
     const int STp = (ST + 7) & ~7;
-    if (layer_stride == 0) layer_stride = (size_t)B * T * D * (ssast ? ssast_geom(m->ssast).patch_f : 1);
+    if (layer_stride == 0) layer_stride = (size_t)B * T * out_width(m);
     if (ffn_out != nullptr && ffn_stride == 0) ffn_stride = (size_t)M * D;
     if (c.relative_position && T > m->rel_table_T) S3B_OK(build_rel_table(m, 2 * T));
     if (c.conformer && T > m->rope_T) S3B_OK(build_rope_table(m, 2 * T));
@@ -1749,6 +1850,8 @@ int Fwd::prepare() {
             for (int t = hk[b]; t < T; ++t) hm[(size_t)b * T + t] = 1;
         if (ssast)  // no key mask: every token of a window attends to all 2 + P tokens of its window
             for (int i = 0; i < SB; ++i) hk[i] = ST;
+        if (mae)  // valid_b time patches of nv tokens each
+            for (int b = 0; b < B; ++b) hk[b] *= mae_ast_geom(m->mae).nv;
         if (recurrent) {  // group utterances of similar length: a recurrence group stops at its own longest
             int* ho = reinterpret_cast<int*>(hb + off_ord);
             std::vector<int> ord(B);
@@ -1775,6 +1878,8 @@ int Fwd::prepare() {
         const SsastGeom g = ssast_geom(m->ssast);
         S3B_OK(w->fb_f32.ensure((size_t)SB * g.TL * 128 * 4));
         S3B_OK(w->ln512_s.ensure(m->ssast.patch ? (size_t)SB * g.P * 256 : (size_t)SB * g.TL * 128));
+    } else if (mae) {
+        S3B_OK(w->ln512_s.ensure((size_t)M * 256));  // the front end's patch operand planes
     } else if (cpc) {
         // conv i's input (i = 1..4) in its padded layout act[i - 1], conv i's fp32 output, the LSTM's operand planes
         // (encoder output, then each layer's), the input GEMM's output
@@ -1822,7 +1927,7 @@ int Fwd::prepare() {
         S3B_OK(w->vt_s.ensure((size_t)D * SB * STp));
         S3B_OK(w->h_s.ensure((size_t)M * F));
         if (c.conformer) S3B_OK(w->glu_f32.ensure((size_t)M * 2 * D * sizeof(float)));
-        else if (!ssast && posconv4_ok(c)) S3B_OK(w->pos_z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
+        else if (!ssast && !mae && posconv4_ok(c)) S3B_OK(w->pos_z.ensure((size_t)B * (T + 3) * 4 * D * sizeof(float)));
         if (c.relative_position) S3B_OK(w->gate.ensure((size_t)B * H * T * 4));
         if (c.family == 3 || c.proj_hidden0) S3B_OK(w->hs0.ensure((size_t)M * D * 4));
     }
@@ -2046,8 +2151,9 @@ static int add_transformer_layer(const Lane& lane, int l, std::vector<Step>& ste
     const LayerW* W = &m->layers[l];
     const bool pre = c.layer_norm_first != 0, rel = c.relative_position != 0, gru_rel = c.gru_rel_pos != 0;
     const bool last = l == c.num_layers - 1, heads = c.pred_heads > 0;
-    // SSAST's encoder has no final norm on its outputs, and its hidden states are written by the fold step after the layer
-    const bool ssast = m->kind == kSsastEncoder, enc_ln = pre && last && !ssast;
+    // SSAST's and MAE-AST's encoders have no final norm on their outputs. SSAST's hidden states are written by the fold
+    // step after the layer; MAE-AST's layer l writes hidden state l itself.
+    const bool ssast = m->kind == kSsastEncoder, mae = m->kind == kMaeAstEncoder, enc_ln = pre && last && !ssast && !mae;
     const float eps = m->ln_eps;
     const double attn_flops = 4.0 * (double)T * T * D * B;
     float* x1 = w->x1_f32.as<float>();
@@ -2107,7 +2213,7 @@ static int add_transformer_layer(const Lane& lane, int l, std::vector<Step>& ste
             KNORM(m, f.st, launch_layernorm(tmp, M, D, W->ln2_g.as<float>(), W->ln2_b.as<float>(), 0, f.hs(l + 1),
                                             !last || heads ? w->xs_s.planes(sch) : no_planes(), f.st));
         }
-        return ssast ? 0 : f.done(l + 1);
+        return ssast ? 0 : f.done(mae ? l : l + 1);
     });
     return 0;
 }
@@ -2466,6 +2572,33 @@ static int add_ssast_output(const Lane& lane, int l, std::vector<Step>& steps) {
     return 0;
 }
 
+// MAE-AST's input to layer 0 (mae_ast.py forward), left in x_f32 (hidden state 0 of the layers): the batch-normalised
+// fbank patches (profile category 2) as post_extract_proj's operand, the projection, then the positions of the valid
+// tokens and, post-LN, encoder.layer_norm with layer 0's operand planes (category 3)
+static int add_mae_ast_input(const Lane& lane, std::vector<Step>& steps) {
+    s3b_model* m = lane.m;
+    Workspace* w = lane.w;
+    const MaeAstGeom g = mae_ast_geom(m->mae);
+    const int D = m->cfg.embed_dim, sch = m->scheme;
+    const bool post = !m->cfg.layer_norm_first, pos = m->mae.sine_pos != 0;
+    GemmParams p;
+    S3B_OK(lane.linear(p, w->ln512_s, m->proj_w, D, 256, epi_f32(w->x_f32.as<float>(), m->proj_b.as<float>())));
+    steps.push_back([=](Fwd& f) {
+        S3B_OK(copy_book(lane, f.st));
+        KLAUNCH(m, f.st, CAT_CONV0, 1, 0.0,
+                launch_mae_ast_fbank(lane.d_wavs, lane.d_lens, lane.B, lane.T, g.kt, g.kc, m->mae_bn_a, m->mae_bn_c,
+                                     nullptr, w->ln512_s.planes(sch), f.st));
+        S3B_OK(run_gemm(f, p));
+        if (post || pos)
+            KNORM(m, f.st, launch_mae_ast_embed(w->x_f32.as<float>(), lane.B, lane.ST, D, lane.d_kv,
+                                                pos ? m->pos_tab.as<float>() : nullptr, post ? 1 : 0,
+                                                m->enc_ln_g.as<float>(), m->enc_ln_b.as<float>(),
+                                                post ? w->xs_s.planes(sch) : no_planes(), f.st));
+        return 0;
+    });
+    return 0;
+}
+
 // One lane's forward at the lane's shape, in enqueue order
 static int build_steps(const Lane& lane, std::vector<Step>& steps) {
     const s3b_model* m = lane.m;
@@ -2488,6 +2621,10 @@ static int build_steps(const Lane& lane, std::vector<Step>& steps) {
             S3B_OK(add_ssast_output(lane, l, steps));
         }
         return 0;
+    case kMaeAstEncoder:
+        S3B_OK(add_mae_ast_input(lane, steps));
+        for (int l = 0; l < c.num_layers; ++l) S3B_OK(add_transformer_layer(lane, l, steps));
+        return 0;
     case kFbankEncoder:
         S3B_OK(add_fbank_frontend(lane, steps));
         // six empty steps where the conv stack would be: with two lanes they keep lane 1's steps enqueued next to the
@@ -2508,8 +2645,10 @@ static int build_steps(const Lane& lane, std::vector<Step>& steps) {
     return 0;
 }
 
-// floats per frame of a hidden state: the encoder width, or SSAST's patch model's 12 frequency patches of it
+// floats per frame of a hidden state: the encoder width, or SSAST's patch model's 12 (MAE-AST's nv) frequency patches
+// of it
 static int out_width(const s3b_model* m) {
+    if (m->kind == kMaeAstEncoder) return mae_ast_geom(m->mae).nv * m->cfg.embed_dim;
     return m->kind == kSsastEncoder ? ssast_geom(m->ssast).patch_f * m->cfg.embed_dim : m->cfg.embed_dim;
 }
 
@@ -2622,6 +2761,7 @@ extern "C" int s3b_forward_ex(s3b_model* m, const float* const* wavs, const int6
             : m->kind == kCpcStack  ? "a modified CPC model is a conv stack and an LSTM, it has no feed-forward blocks or "
                                       "layer results"
             : m->kind == kSsastEncoder ? "the SSAST expert returns only its blocks' outputs (ssast/expert.py)"
+            : m->kind == kMaeAstEncoder ? "the MAE-AST expert returns only its layers' outputs (mae_ast/expert.py)"
             : m->cfg.conformer      ? "a Conformer encoder collects no layer results (wav2vec2_model.py:3199-3200)"
                                     : nullptr;
         if (why != nullptr) return fail("ffn_out / last_residual: %s", why);
@@ -3595,6 +3735,76 @@ extern "C" int s3b_ssast_fold_f32(const float* x, int32_t B, int32_t nseg, int32
     if (T < 1 || T > nseg * g.tdim) return fail("t_out %d out of range (1..%d)", T, nseg * g.tdim);
     CUDA_OK(launch_ssast_fold(x, B, nseg, g.P, g.tdim, g.patch_f, 768, T, out, (cudaStream_t)stream));
     CUDA_OK(cudaStreamSynchronize((cudaStream_t)stream));
+    return 0;
+}
+
+// MAE-AST's building blocks (add_mae_ast_input) on buffers of the call
+extern "C" int s3b_mae_ast_fbank_f32(const float* const* wavs, const int64_t* lens, int32_t B, int64_t max_len,
+                                     int32_t patch, float running_mean, float running_var, int32_t fmt, float* out,
+                                     float* planes_out, void* stream) {
+    if (!wavs || !lens || (!out && !planes_out)) return fail("null argument");
+    if (B < 1) return fail("bad batch %d", B);
+    if (patch != 0 && patch != 1) return fail("patch must be 0 or 1, not %d", patch);
+    if (fmt != 0 && fmt != 1) return fail("fmt must be 0 (bf16 hi/lo) or 1 (f16q8), not %d", fmt);
+    for (int b = 0; b < B; ++b) {
+        if (wavs[b] == nullptr) return fail("null argument: wavs[%d]", b);
+        if (lens[b] < 400 || lens[b] > max_len) return fail("lens[%d]=%lld out of range (400..max_len)", b, (long long)lens[b]);
+    }
+    s3b_mae_ast_config c = {};
+    c.patch = patch;
+    const MaeAstGeom g = mae_ast_geom(c);
+    const int64_t Tp = fbank_frames(max_len) / g.kt;
+    if (Tp < 1) return fail("max_len %lld too short: no %d-frame patch", (long long)max_len, g.kt);
+    if ((int64_t)B * Tp * g.kt > 2000000000LL) return fail("batch too large for 32-bit indexing");
+    if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
+    CUDA_OK(init_fbank_tables());
+    cudaStream_t st = (cudaStream_t)stream;
+    const double a = 0.5 / sqrt((double)running_var + 1e-5);
+    const float bn_a = (float)a, bn_c = (float)(-(double)running_mean * a);
+    DevBuf book;
+    S3B_OK(book.ensure((size_t)B * (sizeof(void*) + sizeof(long long))));
+    std::vector<long long> hl(lens, lens + B);
+    CUDA_OK(cudaMemcpyAsync(book.p, wavs, (size_t)B * sizeof(void*), cudaMemcpyHostToDevice, st));
+    long long* d_lens = reinterpret_cast<long long*>(book.as<char>() + (size_t)B * sizeof(void*));
+    CUDA_OK(cudaMemcpyAsync(d_lens, hl.data(), (size_t)B * sizeof(long long), cudaMemcpyHostToDevice, st));
+    const size_t elems = (size_t)B * Tp * g.nv * 256;
+    if (out != nullptr)
+        CUDA_OK(launch_mae_ast_fbank(book.as<const float*>(), d_lens, B, (int)Tp, g.kt, g.kc, bn_a, bn_c, out,
+                                     no_planes(), st));
+    if (planes_out != nullptr) {
+        SplitBuf os;
+        S3B_OK(os.ensure(elems));
+        CUDA_OK(launch_mae_ast_fbank(book.as<const float*>(), d_lens, B, (int)Tp, g.kt, g.kc, bn_a, bn_c, nullptr,
+                                     os.planes(fmt), st));
+        CUDA_OK(launch_planes_to_f32(os.planes(fmt), elems, planes_out, st));
+        CUDA_OK(cudaStreamSynchronize(st));
+    }
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
+}
+
+extern "C" int s3b_mae_ast_embed_f32(float* x, int32_t B, int32_t N, const int32_t* valid, const float* pe,
+                                     const float* gamma, const float* beta, int32_t fmt, float* planes_out,
+                                     void* stream) {
+    if (!x || !valid) return fail("null argument");
+    if (B < 1 || N < 1) return fail("bad sizes (batch %d, n_tok %d)", B, N);
+    if ((gamma == nullptr) != (beta == nullptr)) return fail("gamma and beta go together (post-LN) or are both null");
+    if (planes_out != nullptr && gamma == nullptr) return fail("planes_out needs the LayerNorm (gamma, beta)");
+    if (fmt != 0 && fmt != 1) return fail("fmt must be 0 (bf16 hi/lo) or 1 (f16q8), not %d", fmt);
+    for (int b = 0; b < B; ++b)
+        if (valid[b] < 0 || valid[b] > N) return fail("valid[%d]=%d out of range (0..%d)", b, valid[b], N);
+    cudaStream_t st = (cudaStream_t)stream;
+    const int D = 768;
+    const size_t elems = (size_t)B * N * D;
+    DevBuf kv;
+    SplitBuf os;
+    S3B_OK(kv.ensure((size_t)B * sizeof(int)));
+    CUDA_OK(cudaMemcpyAsync(kv.p, valid, (size_t)B * sizeof(int), cudaMemcpyHostToDevice, st));
+    if (planes_out != nullptr) S3B_OK(os.ensure(elems));
+    CUDA_OK(launch_mae_ast_embed(x, B, N, D, kv.as<int>(), pe, gamma != nullptr, gamma, beta,
+                                 planes_out != nullptr ? os.planes(fmt) : no_planes(), st));
+    if (planes_out != nullptr) CUDA_OK(launch_planes_to_f32(os.planes(fmt), elems, planes_out, st));
+    CUDA_OK(cudaStreamSynchronize(st));
     return 0;
 }
 

@@ -5,10 +5,11 @@
 //   Featurizer._weighted_sum                      s3prl/upstream/interfaces.py:217-248
 #include "common.cuh"
 #include "kernels.cuh"
+#include "norm.cuh"
 
 namespace s3b {
 
-// one warp per row; V4 = D / 128 float4 per lane; two-pass statistics held in registers
+// one warp per row; V4 = D / 128 float4 per lane; two-pass statistics held in registers (layernorm_row)
 template <int V4>
 __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict__ x, size_t M,
                                                         const float* __restrict__ gamma,
@@ -22,35 +23,9 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
     if (row >= M) return;
     const float4* xr = reinterpret_cast<const float4*>(x + row * D);
     float4 v[V4];
-    float s = 0.f;
 #pragma unroll
-    for (int i = 0; i < V4; ++i) {
-        v[i] = xr[lane + 32 * i];
-        s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
-    }
-    const float mean = warp_sum(s) * (1.0f / D);
-    float q = 0.f;
-#pragma unroll
-    for (int i = 0; i < V4; ++i) {
-        const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, d = v[i].w - mean;
-        q += (a * a + b * b) + (c * c + d * d);
-    }
-    const float rstd = rsqrtf(warp_sum(q) * (1.0f / D) + eps);
-    const float4* g4 = reinterpret_cast<const float4*>(gamma);
-    const float4* b4 = reinterpret_cast<const float4*>(beta);
-#pragma unroll
-    for (int i = 0; i < V4; ++i) {
-        const int c4 = lane + 32 * i;
-        const float4 g = __ldg(g4 + c4), b = __ldg(b4 + c4);
-        float4 y;
-        y.x = (v[i].x - mean) * rstd * g.x + b.x;
-        y.y = (v[i].y - mean) * rstd * g.y + b.y;
-        y.z = (v[i].z - mean) * rstd * g.z + b.z;
-        y.w = (v[i].w - mean) * rstd * g.w + b.w;
-        if (gelu) y.x = gelu_erf(y.x), y.y = gelu_erf(y.y), y.z = gelu_erf(y.z), y.w = gelu_erf(y.w);
-        if (out_f32 != nullptr) reinterpret_cast<float4*>(out_f32 + row * D)[c4] = y;
-        if (op.hi != nullptr) store_planes4(op, y, row * D + 4 * (size_t)c4);
-    }
+    for (int i = 0; i < V4; ++i) v[i] = xr[lane + 32 * i];
+    layernorm_row<V4>(v, lane, gamma, beta, gelu, eps, out_f32 != nullptr ? out_f32 + row * D : nullptr, op, row * D);
 }
 
 cudaError_t launch_layernorm(const float* x, size_t M, int D, const float* gamma, const float* beta, int gelu,

@@ -22,6 +22,7 @@ from .upstream.decoar import DecoarExpert
 from .upstream.decoar2 import Decoar2Expert
 from .upstream.expert import UpstreamExpert
 from .upstream.lighthubert import LighthubertExpert
+from .upstream.mae_ast import MaeAstExpert
 from .upstream.npc import NpcExpert
 from .upstream.ssast import SsastExpert
 
@@ -94,6 +95,12 @@ for _name, _kind, _required in (("lighthubert", "small", False), ("lighthubert_s
 # window_secs as in the reference (1 s for speech commands, 10 s for speaker identification)
 for _name, _kind in (("ssast_frame_base", "frame"), ("ssast_patch_base", "patch")):
     ENTRIES[_name] = _entry(_name, partial(SsastExpert, name=_name, kind=_kind), url_hint="pass a local checkpoint file")
+# MAE-AST (mae_ast/hubconf.py): the fabricated checkpoint of each model without ckpt, else the local {"cfg", "model"}
+# file; mae_ast_local and mae_ast_url take the file's own patch shape
+for _name, _kind, _required in (("mae_ast_frame", "frame", False), ("mae_ast_patch", "patch", False),
+                                ("mae_ast_local", None, True), ("mae_ast_url", None, True)):
+    ENTRIES[_name] = _entry(_name, partial(MaeAstExpert, name=_name, kind=_kind), ckpt_required=_required,
+                            url_hint="pass a local checkpoint file")
 globals().update(ENTRIES)
 
 

@@ -28,6 +28,7 @@ EXPORTED_SYMBOLS = [
     "s3b_npc_model_create",
     "s3b_cpc_model_create",
     "s3b_ssast_model_create",
+    "s3b_mae_ast_model_create",
     "s3b_num_frames",
     "s3b_valid_frames",
     "s3b_num_outputs",
@@ -79,6 +80,8 @@ EXPORTED_SYMBOLS = [
     "s3b_ssast_fbank_f32",
     "s3b_ssast_embed_f32",
     "s3b_ssast_fold_f32",
+    "s3b_mae_ast_fbank_f32",
+    "s3b_mae_ast_embed_f32",
     "s3b_fbank",
     "s3b_fbank_ex",
     "s3b_fbank_num_frames",
@@ -215,6 +218,27 @@ class S3BSsastConfig(C.Structure):
         self.struct_size = C.sizeof(S3BSsastConfig)
 
 
+class S3BMaeAstConfig(C.Structure):
+    """Mirror of ``struct s3b_mae_ast_config``."""
+
+    _fields_ = [
+        ("struct_size", C.c_int32),
+        ("patch", C.c_int32),
+        ("embed_dim", C.c_int32),
+        ("num_heads", C.c_int32),
+        ("ffn_dim", C.c_int32),
+        ("num_layers", C.c_int32),
+        ("layer_norm_first", C.c_int32),
+        ("sine_pos", C.c_int32),
+        ("max_tokens", C.c_int32),
+        ("reserved", C.c_int32 * 4),
+    ]
+
+    def __init__(self, **kw):
+        super().__init__(**kw)
+        self.struct_size = C.sizeof(S3BMaeAstConfig)
+
+
 class S3BForwardOpts(C.Structure):
     """Mirror of ``struct s3b_forward_opts``."""
 
@@ -324,6 +348,7 @@ def load() -> C.CDLL:
     lib.s3b_npc_model_create.argtypes = [C.POINTER(S3BNpcConfig), C.POINTER(vp)]
     lib.s3b_cpc_model_create.argtypes = [C.POINTER(S3BCpcConfig), C.POINTER(vp)]
     lib.s3b_ssast_model_create.argtypes = [C.POINTER(S3BSsastConfig), C.POINTER(vp)]
+    lib.s3b_mae_ast_model_create.argtypes = [C.POINTER(S3BMaeAstConfig), C.POINTER(vp)]
     lib.s3b_model_finalize.argtypes = [vp]
     lib.s3b_model_destroy.argtypes = [vp]
     lib.s3b_model_destroy.restype = None
@@ -386,6 +411,9 @@ def load() -> C.CDLL:
     lib.s3b_ssast_fbank_f32.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i64, i32, f32p, vp]
     lib.s3b_ssast_embed_f32.argtypes = [f32p, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, i32, f32p, f32p, vp]
     lib.s3b_ssast_fold_f32.argtypes = [f32p, i32, i32, i32, i32, i32, f32p, vp]
+    lib.s3b_mae_ast_fbank_f32.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i64, i32, C.c_float, C.c_float, i32, f32p,
+                                          f32p, vp]
+    lib.s3b_mae_ast_embed_f32.argtypes = [f32p, i32, i32, C.POINTER(i32), f32p, f32p, f32p, i32, f32p, vp]
     lib.s3b_fbank_num_frames.argtypes = [i64]
     lib.s3b_fbank_num_frames.restype = i64
     lib.s3b_fbank.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, f32p, vp]
