@@ -39,6 +39,7 @@ int main(void) {
         (const void*)s3b_layernorm_eps_f32, (const void*)s3b_ssast_fbank_f32, (const void*)s3b_ssast_embed_f32,
         (const void*)s3b_ssast_fold_f32, (const void*)s3b_layernorm_eps_planes_f32, (const void*)s3b_fbank_cmvn_planes,
         (const void*)s3b_mae_ast_model_create, (const void*)s3b_mae_ast_fbank_f32, (const void*)s3b_mae_ast_embed_f32,
+        (const void*)s3b_ssast_patch_planes, (const void*)s3b_mae_ast_fbank_planes,
     };
     s3b_config cfg;
     int64_t lens[2] = {16000, 800};

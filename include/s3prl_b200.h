@@ -603,6 +603,12 @@ int s3b_ssast_fbank_f32(const float* const* wavs, const int64_t* lens, int32_t b
 int s3b_ssast_embed_f32(const float* feat, int32_t segments, int32_t tl, int32_t patch, const float* w,
                         const float* bias, const float* cls, const float* dist, const float* pos, int32_t scheme,
                         float* planes_out, float* out, void* stream);
+/* The patch operand of s3b_ssast_embed_f32 (the features, or the 16 x 16 / stride-10 gather) as a forward writes it
+ * from feat [segments][TL][128] (DEVICE), undecoded, into the caller's DEVICE buffer `planes`: the operand planes of
+ * fmt (0 bf16 hi/lo, 1 f16q8), each [segments][TL][128] (patch 0) or [segments][P][256] (patch 1), back to back in
+ * the layout of s3b_fbank_cmvn_planes (4 bytes per element, 4-byte aligned). */
+int s3b_ssast_patch_planes(const float* feat, int32_t segments, int32_t tl, int32_t patch, int32_t fmt, void* planes,
+                           void* stream);
 /* One SSAST hidden state from the residual stream x [batch * nseg][2 + P][768] (DEVICE) as a forward writes it:
  * out [batch][t_out][768 or 12 * 768], class tokens dropped, frequency patches folded into channels; t_out <= nseg t_dim. */
 int s3b_ssast_fold_f32(const float* x, int32_t batch, int32_t nseg, int32_t tl, int32_t patch, int32_t t_out,
@@ -615,6 +621,12 @@ int s3b_ssast_fold_f32(const float* x, int32_t batch, int32_t nseg, int32_t tl, 
 int s3b_mae_ast_fbank_f32(const float* const* wavs, const int64_t* lens, int32_t batch, int64_t max_len, int32_t patch,
                           float running_mean, float running_var, int32_t fmt, float* out, float* planes_out,
                           void* stream);
+/* The same front end with the forward's batch-norm constants, undecoded, into the caller's DEVICE buffer `planes`:
+ * the operand planes of fmt, each [batch * T' nv][256], back to back in the layout of s3b_fbank_cmvn_planes (4 bytes
+ * per element, 4-byte aligned). */
+int s3b_mae_ast_fbank_planes(const float* const* wavs, const int64_t* lens, int32_t batch, int64_t max_len,
+                             int32_t patch, float running_mean, float running_var, int32_t fmt, void* planes,
+                             void* stream);
 /* MAE-AST's positions and input norm as a forward runs them, in place on x [batch][n_tok][768] (DEVICE, the
  * projection's output): x[b][t] += pe[t] for t < valid[b] (host array; pe [>= n_tok][768] DEVICE, or NULL); with
  * gamma / beta (DEVICE, post-LN) then LayerNorm(eps 1e-5) into x and, when planes_out is given, its operand planes of

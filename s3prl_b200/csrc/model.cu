@@ -1138,6 +1138,13 @@ static int upload_encoder_layer(s3b_model* m, int l) {
     return 0;
 }
 
+// MAE-AST's eval BatchNorm2d(1, affine=False) times 0.5 as the affine map y = x * a + c its fbank kernel applies:
+// a = 0.5 / sqrt(running_var + 1e-5), c = -running_mean * a, in double, each rounded once to fp32
+static void mae_ast_bn_fold(float running_mean, float running_var, float* a, float* c) {
+    const double ad = 0.5 / sqrt((double)running_var + 1e-5);
+    *a = (float)ad, *c = (float)(-(double)running_mean * ad);
+}
+
 // MAE-AST (mae_ast.py): post_extract_proj over the unfolded patches, the eval batch norm folded into one affine map,
 // the checkpoint's own sinusoid table (a persistent buffer that strict loading reads from the file), and the wav2vec 2.0
 // encoder layers; encoder.layer_norm on the input of a post-LN encoder
@@ -1150,8 +1157,7 @@ static int finalize_mae_ast(s3b_model* m) {
     const HostTensor *rm, *rv;
     S3B_OK(need(m, "batch_norm.running_mean", {1}, &rm));
     S3B_OK(need(m, "batch_norm.running_var", {1}, &rv));
-    const double a = 0.5 / sqrt((double)rv->data[0] + 1e-5);
-    m->mae_bn_a = (float)a, m->mae_bn_c = (float)(-(double)rm->data[0] * a);
+    mae_ast_bn_fold(rm->data[0], rv->data[0], &m->mae_bn_a, &m->mae_bn_c);
     if (m->mae.sine_pos) {
         S3B_OK(need(m, "enc_sine_pos_embed.pe", {1, m->mae.max_tokens, D}, &t));
         S3B_OK(upload_f32(m->pos_tab, t->data.data(), t->numel()));
@@ -3602,6 +3608,17 @@ extern "C" int s3b_frontend_f32(const float* const* wavs, const int64_t* lens, i
     return 0;
 }
 
+// The operand planes of fmt over `elems` elements in a caller's buffer, in the layout the *_planes entry points
+// document: whole planes back to back, 4 bytes per element (bf16 hi, bf16 lo; or fp16, e4m3 of the fp16, e4m3 of the
+// residual x 2^11)
+static OutPlanes caller_planes(void* planes, size_t elems, int fmt) {
+    char* p = static_cast<char*>(planes);
+    __nv_bfloat16* p16 = reinterpret_cast<__nv_bfloat16*>(p);
+    return fmt ? OutPlanes{p16, nullptr, reinterpret_cast<uint8_t*>(p + 2 * elems),
+                           reinterpret_cast<uint8_t*>(p + 3 * elems), 1}
+               : OutPlanes{p16, reinterpret_cast<__nv_bfloat16*>(p + 2 * elems), nullptr, nullptr, 0};
+}
+
 // add_fbank_frontend's step for a DeCoAR 2.0 (step 2) or APC (step 1) model. The log-mel and the operand planes go to
 // the caller's logmel / planes when given (s3b_fbank_cmvn_planes), else to workspaces of this call; out (optional):
 // the operand planes decoded, columns 0..79 kept
@@ -3639,12 +3656,8 @@ static int fbank_cmvn_features(const float* const* wavs, const int64_t* lens, in
     }
     OutPlanes op;
     const size_t elems = rows * kDecoar2K;
-    if (planes != nullptr) {  // the layout s3b_fbank_cmvn_planes documents: whole planes back to back
-        char* p = static_cast<char*>(planes);
-        __nv_bfloat16* p16 = reinterpret_cast<__nv_bfloat16*>(p);
-        op = out_fmt ? OutPlanes{p16, nullptr, reinterpret_cast<uint8_t*>(p + 2 * elems),
-                                 reinterpret_cast<uint8_t*>(p + 3 * elems), 1}
-                     : OutPlanes{p16, reinterpret_cast<__nv_bfloat16*>(p + 2 * elems), nullptr, nullptr, 0};
+    if (planes != nullptr) {
+        op = caller_planes(planes, elems, out_fmt);
     } else {
         S3B_OK(os.ensure(elems));
         op = os.planes(out_fmt);
@@ -3724,6 +3737,23 @@ extern "C" int s3b_ssast_embed_f32(const float* feat, int32_t SB, int32_t TL, in
     return 0;
 }
 
+extern "C" int s3b_ssast_patch_planes(const float* feat, int32_t SB, int32_t TL, int32_t patch, int32_t fmt,
+                                      void* planes, void* stream) {
+    if (!feat || !planes) return fail("null argument");
+    if (reinterpret_cast<uintptr_t>(planes) % 4 != 0) return fail("planes must be 4-byte aligned");
+    if (patch != 0 && patch != 1) return fail("patch must be 0 or 1, not %d", patch);
+    if (fmt != 0 && fmt != 1) return fail("fmt must be 0 (bf16 hi/lo) or 1 (f16q8), not %d", fmt);
+    if (SB < 1 || TL < (patch ? 16 : 2)) return fail("bad sizes (segments %d, tl %d)", SB, TL);
+    s3b_ssast_config c = {};
+    c.patch = patch, c.window_samples = 160 * TL;
+    const SsastGeom g = ssast_geom(c);
+    const size_t an = patch ? (size_t)SB * g.P * 256 : (size_t)SB * TL * 128;
+    cudaStream_t st = (cudaStream_t)stream;
+    CUDA_OK(launch_ssast_patches(feat, SB, TL, g.patch_f, g.tdim, caller_planes(planes, an, fmt), st));
+    CUDA_OK(cudaStreamSynchronize(st));
+    return 0;
+}
+
 extern "C" int s3b_ssast_fold_f32(const float* x, int32_t B, int32_t nseg, int32_t TL, int32_t patch, int32_t T,
                                   float* out, void* stream) {
     if (!x || !out) return fail("null argument");
@@ -3738,11 +3768,12 @@ extern "C" int s3b_ssast_fold_f32(const float* x, int32_t B, int32_t nseg, int32
     return 0;
 }
 
-// MAE-AST's building blocks (add_mae_ast_input) on buffers of the call
-extern "C" int s3b_mae_ast_fbank_f32(const float* const* wavs, const int64_t* lens, int32_t B, int64_t max_len,
-                                     int32_t patch, float running_mean, float running_var, int32_t fmt, float* out,
-                                     float* planes_out, void* stream) {
-    if (!wavs || !lens || (!out && !planes_out)) return fail("null argument");
+// MAE-AST's front end step (add_mae_ast_input) on buffers of the call: out (fp32), planes_out (the operand planes
+// decoded) and raw (the operand planes themselves, caller_planes' layout), each optional
+static int mae_ast_fbank(const float* const* wavs, const int64_t* lens, int32_t B, int64_t max_len, int32_t patch,
+                         float running_mean, float running_var, int32_t fmt, float* out, float* planes_out, void* raw,
+                         void* stream) {
+    if (!wavs || !lens || (!out && !planes_out && !raw)) return fail("null argument");
     if (B < 1) return fail("bad batch %d", B);
     if (patch != 0 && patch != 1) return fail("patch must be 0 or 1, not %d", patch);
     if (fmt != 0 && fmt != 1) return fail("fmt must be 0 (bf16 hi/lo) or 1 (f16q8), not %d", fmt);
@@ -3759,8 +3790,8 @@ extern "C" int s3b_mae_ast_fbank_f32(const float* const* wavs, const int64_t* le
     if (s3b_device_count() == 0) return fail("no CUDA device: s3prl_b200 has no CPU fallback");
     CUDA_OK(init_fbank_tables());
     cudaStream_t st = (cudaStream_t)stream;
-    const double a = 0.5 / sqrt((double)running_var + 1e-5);
-    const float bn_a = (float)a, bn_c = (float)(-(double)running_mean * a);
+    float bn_a, bn_c;
+    mae_ast_bn_fold(running_mean, running_var, &bn_a, &bn_c);
     DevBuf book;
     S3B_OK(book.ensure((size_t)B * (sizeof(void*) + sizeof(long long))));
     std::vector<long long> hl(lens, lens + B);
@@ -3779,8 +3810,27 @@ extern "C" int s3b_mae_ast_fbank_f32(const float* const* wavs, const int64_t* le
         CUDA_OK(launch_planes_to_f32(os.planes(fmt), elems, planes_out, st));
         CUDA_OK(cudaStreamSynchronize(st));
     }
+    if (raw != nullptr)
+        CUDA_OK(launch_mae_ast_fbank(book.as<const float*>(), d_lens, B, (int)Tp, g.kt, g.kc, bn_a, bn_c, nullptr,
+                                     caller_planes(raw, elems, fmt), st));
     CUDA_OK(cudaStreamSynchronize(st));
     return 0;
+}
+
+extern "C" int s3b_mae_ast_fbank_f32(const float* const* wavs, const int64_t* lens, int32_t B, int64_t max_len,
+                                     int32_t patch, float running_mean, float running_var, int32_t fmt, float* out,
+                                     float* planes_out, void* stream) {
+    return mae_ast_fbank(wavs, lens, B, max_len, patch, running_mean, running_var, fmt, out, planes_out, nullptr,
+                         stream);
+}
+
+extern "C" int s3b_mae_ast_fbank_planes(const float* const* wavs, const int64_t* lens, int32_t B, int64_t max_len,
+                                        int32_t patch, float running_mean, float running_var, int32_t fmt,
+                                        void* planes, void* stream) {
+    if (!planes) return fail("null argument");
+    if (reinterpret_cast<uintptr_t>(planes) % 4 != 0) return fail("planes must be 4-byte aligned");
+    return mae_ast_fbank(wavs, lens, B, max_len, patch, running_mean, running_var, fmt, nullptr, nullptr, planes,
+                         stream);
 }
 
 extern "C" int s3b_mae_ast_embed_f32(float* x, int32_t B, int32_t N, const int32_t* valid, const float* pe,

@@ -80,7 +80,9 @@ EXPORTED_SYMBOLS = [
     "s3b_ssast_fbank_f32",
     "s3b_ssast_embed_f32",
     "s3b_ssast_fold_f32",
+    "s3b_ssast_patch_planes",
     "s3b_mae_ast_fbank_f32",
+    "s3b_mae_ast_fbank_planes",
     "s3b_mae_ast_embed_f32",
     "s3b_fbank",
     "s3b_fbank_ex",
@@ -411,8 +413,11 @@ def load() -> C.CDLL:
     lib.s3b_ssast_fbank_f32.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i64, i32, f32p, vp]
     lib.s3b_ssast_embed_f32.argtypes = [f32p, i32, i32, i32, f32p, f32p, f32p, f32p, f32p, i32, f32p, f32p, vp]
     lib.s3b_ssast_fold_f32.argtypes = [f32p, i32, i32, i32, i32, i32, f32p, vp]
+    lib.s3b_ssast_patch_planes.argtypes = [f32p, i32, i32, i32, i32, vp, vp]
     lib.s3b_mae_ast_fbank_f32.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i64, i32, C.c_float, C.c_float, i32, f32p,
                                           f32p, vp]
+    lib.s3b_mae_ast_fbank_planes.argtypes = [C.POINTER(vp), C.POINTER(i64), i32, i64, i32, C.c_float, C.c_float, i32,
+                                             vp, vp]
     lib.s3b_mae_ast_embed_f32.argtypes = [f32p, i32, i32, C.POINTER(i32), f32p, f32p, f32p, i32, f32p, vp]
     lib.s3b_fbank_num_frames.argtypes = [i64]
     lib.s3b_fbank_num_frames.restype = i64

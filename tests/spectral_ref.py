@@ -29,6 +29,8 @@ Bounds (u = 2^-24, one fp32 rounding). Stage by stage, each an absolute bound pe
            so where |E - floor| < dE either side of the max is accepted
   deltas : dD_t <= (2 df_t-2 + df_t-1 + df_t+1 + 2 df_t+2) / 10 + 6u (2|f_t-2| + |f_t-1| + |f_t+1| + 2|f_t+2|) / 10
            + u |D_t| with the replicate-clamped indices; then the same for delta-delta on (D, dD)
+  (SSAST / MAE-AST: the same stages up to the log-mel with 128 bins and the hanning / povey window, then an affine map
+  whose fp32 constants' error and roundings ssast_interval / mae_ast_bounds carry)
   (DeCoAR 2.0 / APC / DeCoAR / NPC: the same stages up to the log-mel with the hamming window and no deltas, then the
   CMVN below over all m frames, every step-th row kept: fbank_cmvn_forward, fbank_cmvn_bounds)
   CMVN   : with s the fp64 std and ds <= ||df||_2 / sqrt(m - 1) + 4u s, dmu <= mean(df) + 2u max|f|:
@@ -140,33 +142,40 @@ def hamming_window(dtype) -> torch.Tensor:
     return (0.54 - 0.46 * torch.cos(2 * math.pi * n / (WIN - 1))).to(dtype)
 
 
-WINDOWS = {"povey": povey_window, "hamming": hamming_window}
+def hanning_window(dtype) -> torch.Tensor:
+    """kaldi's "hanning" (SSAST's window): torch.hann_window(400, periodic=False)."""
+    return torch.hann_window(WIN, periodic=False, dtype=dtype)
 
 
-def kaldi_mel_banks(dtype) -> torch.Tensor:
-    """get_mel_banks(80 bins, 512-point FFT, 16 kHz, low 20 Hz, high = Nyquist) in `dtype` -> [80, 257]."""
+WINDOWS = {"povey": povey_window, "hamming": hamming_window, "hanning": hanning_window}
+
+
+def kaldi_mel_banks(dtype, nmel: int = NMEL) -> torch.Tensor:
+    """get_mel_banks(nmel bins, 512-point FFT, 16 kHz, low 20 Hz, high = Nyquist) in `dtype` -> [nmel, 257]."""
     mel_low, mel_high = 1127.0 * math.log(1.0 + 20.0 / 700.0), 1127.0 * math.log(1.0 + 8000.0 / 700.0)
-    delta = (mel_high - mel_low) / (NMEL + 1)
-    b = torch.arange(NMEL, dtype=dtype).unsqueeze(1)
+    delta = (mel_high - mel_low) / (nmel + 1)
+    b = torch.arange(nmel, dtype=dtype).unsqueeze(1)
     left, center, right = mel_low + b * delta, mel_low + (b + 1.0) * delta, mel_low + (b + 2.0) * delta
     mel = 1127.0 * (1.0 + (SR / NFFT) * torch.arange(NFFT // 2, dtype=dtype) / 700.0).log()
     w = torch.min((mel - left) / (center - left), (right - mel) / (right - center)).clamp(min=0.0)
     return F.pad(w, (0, 1))
 
 
-def fbank_stages(wav: torch.Tensor, dtype=torch.float64, window: str = "povey",
-                 preemph: float = 0.97) -> Dict[str, torch.Tensor]:
+def fbank_stages(wav: torch.Tensor, dtype=torch.float64, window: str = "povey", preemph: float = 0.97,
+                 nmel: int = NMEL, replicate_first: bool = True) -> Dict[str, torch.Tensor]:
     """Every stage of kaldi fbank + deltas for one utterance: frames [m, 400] after DC removal (d) and after
-    pre-emphasis and window (y), spectrum X [m, 257], power P, mel energies E [m, 80], log-mel f, deltas D and DD.
-    window: a key of WINDOWS (the fbank baseline's povey, or the hamming of DeCoAR 2.0 / APC / DeCoAR / NPC)."""
+    pre-emphasis and window (y), spectrum X [m, 257], power P, mel energies E [m, nmel], log-mel f, deltas D and DD.
+    window: a key of WINDOWS (the fbank baseline's and MAE-AST's povey, the hamming of DeCoAR 2.0 / APC / DeCoAR / NPC,
+    SSAST's hanning); nmel: 80, or SSAST's and MAE-AST's 128. replicate_first=False pre-emphasises the first sample
+    against 0 instead of itself (kaldi replicates it; only a window that is not 0 at n = 0 sees the difference)."""
     m = num_frames(len(wav))
     frames = wav.to(dtype).unfold(0, WIN, SHIFT)[:m]
     d = frames - frames.mean(dim=1, keepdim=True)
-    prev = torch.cat([d[:, :1], d[:, :-1]], dim=1)
+    prev = torch.cat([d[:, :1] if replicate_first else torch.zeros_like(d[:, :1]), d[:, :-1]], dim=1)
     y = (d - preemph * prev) * WINDOWS[window](dtype)
     X = torch.fft.rfft(F.pad(y, (0, NFFT - WIN)))
     P = X.abs().pow(2)
-    E = P @ kaldi_mel_banks(dtype).T
+    E = P @ kaldi_mel_banks(dtype, nmel).T
     f = E.clamp(min=FLOOR).log()
     D = deltas(f)
     return {"x": frames, "d": d, "y": y, "X": X, "P": P, "E": E, "f": f, "D": D, "DD": deltas(D)}
@@ -258,9 +267,9 @@ def spectrogram_forward(wavs: Sequence[torch.Tensor], feat: str, use_cmvn: bool 
 
 
 # ---- bounds ---------------------------------------------------------------------------------------------------------
-def bank_eps(which: str) -> float:
-    """Twice the largest |fp32 bank weight - fp64 bank weight|, at least 2u."""
-    fn = kaldi_mel_banks if which == "kaldi" else htk_mel_banks
+def bank_eps(which: str, nmel: int = NMEL) -> float:
+    """Twice the largest |fp32 bank weight - fp64 bank weight|, at least 2u (nmel: kaldi banks only)."""
+    fn = (lambda dt: kaldi_mel_banks(dt, nmel)) if which == "kaldi" else htk_mel_banks
     return max(2.0 * (fn(torch.float32).double() - fn(torch.float64)).abs().max().item(), 2 * U)
 
 
@@ -323,11 +332,12 @@ def cmvn_bound(f: torch.Tensor, df: torch.Tensor):
     return z, dz, cond
 
 
-def logmel_bounds(wav: torch.Tensor, eps_w: float, window: str = "povey") -> Dict[str, torch.Tensor]:
-    """fp64 stages of one utterance (fbank_stages with `window`) and lo/hi, df of an fp32 log-mel of them."""
-    s = fbank_stages(wav, torch.float64, window)
+def logmel_bounds(wav: torch.Tensor, eps_w: float, window: str = "povey", nmel: int = NMEL) -> Dict[str, torch.Tensor]:
+    """fp64 stages of one utterance (fbank_stages with `window` and nmel bins) and lo/hi, df of an fp32 log-mel of
+    them. eps_w: bank_eps("kaldi", nmel)."""
+    s = fbank_stages(wav, torch.float64, window, nmel=nmel)
     dX = frame_error(s["x"], s["d"], s["y"], WINDOWS[window](torch.float64), fbank=True)
-    dE = energy_error(s["X"], dX, kaldi_mel_banks(torch.float64).T, eps_w)
+    dE = energy_error(s["X"], dX, kaldi_mel_banks(torch.float64, nmel).T, eps_w)
     lo, hi = log_interval(s["E"], dE, fbank=True)
     return {**s, "dE": dE, "lo": lo, "hi": hi, "df": torch.maximum(s["f"] - lo, hi - s["f"])}
 
@@ -340,6 +350,51 @@ def fbank_cmvn_bounds(wav: torch.Tensor, eps_w: float, step: int) -> Dict[str, t
     s = logmel_bounds(wav, eps_w, "hamming")
     z, dz, cond = cmvn_bound(s["f"], s["df"])
     return {**s, "z": z[::step], "dz": dz[::step], "cond": cond}
+
+
+def _f32(v: float) -> float:
+    return torch.tensor(v, dtype=torch.float64).float().item()
+
+
+def bn_fold(rm: float, rv: float):
+    """MAE-AST's eval batch norm times 0.5 as y = x a + c: (a, c) in fp64 and as the library rounds them to fp32
+    (a = fp32(0.5 / sqrt(rv + 1e-5)), c = fp32(-rm a) with a in fp64)."""
+    a = 0.5 / math.sqrt(rv + 1e-5)
+    return a, -rm * a, _f32(a), _f32(-rm * a)
+
+
+def mae_ast_bounds(wav: torch.Tensor, eps_w: float, rm: float, rv: float) -> Dict[str, torch.Tensor]:
+    """MAE-AST's normalised fbank of one utterance (povey window, 128 bins, y = f a + c) in fp64 and the interval an
+    fp32 fma(f32, a32, c32) of the kernel's log-mel f32 lies in: f32 in [lo, hi], so f32 a32 + c32 is within
+    a (f32 - f) + |a32 - a| |f32| + |c32 - c| of y, plus the fma's one rounding u |y|."""
+    s = logmel_bounds(wav, eps_w, "povey", 128)
+    a, c, a32, c32 = bn_fold(rm, rv)
+    e = abs(a32 - a) * torch.maximum(s["lo"].abs(), s["hi"].abs()) + abs(c32 - c)
+    lo, hi = a * s["lo"] + c - e, a * s["hi"] + c + e
+    r = U * torch.maximum(lo.abs(), hi.abs())
+    return {**s, "y": a * s["f"] + c, "ylo": lo - r, "yhi": hi + r}
+
+
+SSAST_SHIFT, SSAST_SCALE = 4.2677393, 4.5689974 * 2  # (f + shift) / scale (ssast/audio.py)
+
+
+def ssast_interval(lo: torch.Tensor, hi: torch.Tensor):
+    """The interval of fp32 (f32 + shift32) / scale32 for f32 in [lo, hi]: the sum and the quotient each rounded once
+    (u |.|), with the fp32 constants' error carried (the interval holds both the fp32 and the fp64 constants' value)."""
+    sh, sc = (SSAST_SHIFT, _f32(SSAST_SHIFT)), (SSAST_SCALE, _f32(SSAST_SCALE))
+    glo, ghi = lo + min(sh), hi + max(sh)
+    glo, ghi = glo - U * glo.abs(), ghi + U * ghi.abs()
+    qlo = torch.minimum(glo / sc[0], glo / sc[1])
+    qhi = torch.maximum(ghi / sc[0], ghi / sc[1])
+    return qlo - U * qlo.abs(), qhi + U * qhi.abs()
+
+
+def ssast_bounds(seg: torch.Tensor, eps_w: float) -> Dict[str, torch.Tensor]:
+    """SSAST's normalised fbank of one zero-padded window of S samples (hanning window, 128 bins) in fp64, y = (f +
+    shift) / scale [m, 128], and the interval ssast_interval gives the kernel's value from the log-mel's [lo, hi]."""
+    s = logmel_bounds(seg, eps_w, "hanning", 128)
+    ylo, yhi = ssast_interval(s["lo"], s["hi"])
+    return {**s, "y": (s["f"] + SSAST_SHIFT) / SSAST_SCALE, "ylo": ylo, "yhi": yhi}
 
 
 def fbank_bounds(wav: torch.Tensor, eps_w: float) -> Dict[str, torch.Tensor]:

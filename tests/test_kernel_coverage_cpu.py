@@ -16,7 +16,9 @@ dropped tap at a configuration no block test runs. Per kernel family:
   test_kernel_coverage_gpu.DEPTHWISE_SERVED;
 - the conv front end (extractor_mode, conv_bias): test_frontend_gpu.test_groupnorm / test_layernorm at CONV0_BIAS;
 - the fbank front end (window, mel bins, step, CMVN, operand format) of APC, VQ-APC, DeCoAR, DeCoAR 2.0 and NPC:
-  test_fbank_frontend_gpu.CONFIGS, formed from the hub entries whose expert is one of those kinds.
+  test_fbank_frontend_gpu.CONFIGS, formed from the hub entries whose expert is one of those kinds;
+- the 128-bin fbank front end (window, mel bins, normalisation, operand layout, operand format) of SSAST and MAE-AST:
+  test_fbank128_frontend_gpu.CONFIGS, formed from the hub entries whose expert module is ssast or mae_ast.
 
 The configurations are formed from the served geometries (test_port_coverage_cpu._geometries: configs.ARCHS,
 configs.XLS_R, decoar2.DECOAR2, the LightHuBERT subnets; plus SSAST), with the model.cu rules that pick a
@@ -25,9 +27,11 @@ import inspect
 import sys
 
 from s3prl_b200 import hub
-from s3prl_b200.upstream import apc, decoar, decoar2, lighthubert, npc, ssast
+from s3prl_b200.upstream import apc, decoar, decoar2, lighthubert, mae_ast, npc, ssast
 from test_blocks_gpu import ATTENTION_CASES, BIAS_HEADS, LAYERNORM_DIMS
 from test_conformer_gpu import DEPTHWISE_D, DEPTHWISE_KS, ROPE_CASES
+from test_fbank128_frontend_gpu import CONFIGS as FBANK128_CONFIGS
+from test_fbank128_frontend_gpu import MAE_AST_NORM, SSAST_NORM
 from test_fbank_frontend_gpu import CMVN_ALL_FRAMES
 from test_fbank_frontend_gpu import CONFIGS as FBANK_CONFIGS
 from test_frontend_gpu import CONV0_BIAS
@@ -209,6 +213,27 @@ def _served_fbank_frontend():
     return served
 
 
+# the 128-bin front ends (fbank.cu ssast_fbank_kernel + ssast_patches_kernel, mae_ast_fbank_kernel) by the module of
+# their expert: (window, normalisation)
+FBANK128_MODULES = {ssast: ("hanning", SSAST_NORM), mae_ast: ("povey", MAE_AST_NORM)}
+
+
+def _served_fbank128_frontend():
+    """(window, mel bins, normalisation, operand layout, operand format) -> hub entries whose expert module is ssast or
+    mae_ast: the layout is the module's KINDS entry of every kind the entry can serve (mae_ast_local / _url take the
+    file's own), both operand formats (S3B_GEMM_SCHEME selects one at run time)."""
+    served = {}
+    for name, entry in hub.ENTRIES.items():
+        mod = sys.modules.get(getattr(_hub_expert(entry), "__module__", ""))
+        if mod not in FBANK128_MODULES:
+            continue
+        window, norm = FBANK128_MODULES[mod]
+        for layout in mod.KINDS.values():
+            for fmt in (0, 1):
+                served.setdefault((window, mod.NUM_BINS, norm, layout, fmt), []).append(name)
+    return served
+
+
 FAMILIES = {  # name -> (served, covered)
     "positional conv (D, groups, k, taps per k-block, mode, post-LN)": (_served_posconv, _covered_posconv),
     "attention (H, head dim, bias)": (_served_attention, _covered_attention),
@@ -219,6 +244,8 @@ FAMILIES = {  # name -> (served, covered)
     "conv front end (extractor_mode, conv_bias)": (
         _served_frontend, lambda: {(m, b) for m in ("default", "layer_norm") for b in CONV0_BIAS}),
     "fbank front end (window, mel bins, step, CMVN, operand format)": (_served_fbank_frontend, lambda: set(FBANK_CONFIGS)),
+    "128-bin fbank front end (window, mel bins, normalisation, operand layout, operand format)": (
+        _served_fbank128_frontend, lambda: set(FBANK128_CONFIGS)),
 }
 
 
@@ -252,6 +279,12 @@ def test_served_set_is_formed():
     names = {n for models in fb.values() for n in models}
     assert {"apc", "vq_apc", "decoar", "decoar_layers", "decoar2", "npc", "npc_360hr", "npc_960hr"} <= names
     assert "decoar2" in fb[("hamming", 80, 2, CMVN_ALL_FRAMES, 1)] and "npc" in fb[("hamming", 80, 1, CMVN_ALL_FRAMES, 0)]
+    fb128 = _served_fbank128_frontend()
+    names = {n for models in fb128.values() for n in models}
+    assert {"ssast_frame_base", "ssast_patch_base", "mae_ast_frame", "mae_ast_patch", "mae_ast_local",
+            "mae_ast_url"} <= names
+    assert "mae_ast_patch" in fb128[("povey", 128, MAE_AST_NORM, (16, 16), 1)]
+    assert "ssast_frame_base" in fb128[("hanning", 128, SSAST_NORM, ((128, 2), (128, 1)), 0)]
 
 
 def test_posconv_rules_match_the_model():
@@ -289,6 +322,10 @@ def test_fbank_step_rule_matches_the_models():
 
 def test_every_served_fbank_frontend_has_a_block_test():
     _assert_covered("fbank front end (window, mel bins, step, CMVN, operand format)")
+
+
+def test_every_served_fbank128_frontend_has_a_block_test():
+    _assert_covered("128-bin fbank front end (window, mel bins, normalisation, operand layout, operand format)")
 
 
 def test_every_served_layernorm_has_a_block_test():

@@ -335,11 +335,12 @@ def test_fbank_at_new_windows(s3b_lib, secs):
     """s3b_ssast_fbank_f32 against ssast_oracle.fbank_windows on structured audio: the smallest windows of both
     models (one and 14 fbank frames), the largest, and a window of 16015 samples, whose windows start off the
     160-sample hop. Windows that start past an utterance's end are silent: exactly the floor.
-    Bound per element, in normalised units: test_ssast_gpu's 1e-4, plus the fp32 spectrum's own error in a bin far
-    below its frame. The FFT's error in a bin is on the order of u times the frame's total amplitude, so the bin's log
-    energy is off by up to 2 u sqrt(E_frame / E_bin). Past 4.3 s the chirp of _structured aliases, and its frames'
-    lowest mel bins sit 1e-10 under their peak. There the error reaches 2.5e-4, at the same sample whatever the
-    window length: it is the frame's content, not the window's geometry."""
+    Bound per element: spectral_ref.ssast_bounds' interval on each zero-padded window (the fp64 log-mel's stage-by-
+    stage interval through (f + 4.2677393) / 9.1379948 with its roundings). Its FFT bound is absolute per frame, so a
+    bin far below its frame's peak (past 4.3 s the chirp of _structured aliases, and its frames' lowest mel bins sit
+    1e-10 under their peak) gets the wide interval its fp32 spectrum needs."""
+    import spectral_ref as R
+
     from s3prl_b200 import lib
 
     S = geometry("frame", secs)["S"]
@@ -361,14 +362,20 @@ def test_fbank_at_new_windows(s3b_lib, secs):
     silent = torch.tensor([s * S >= n for n in lens for s in range(nseg)])
     assert silent.any() and ref[silent][:, :m].eq(floor).all()
     assert (got[silent][:, :m] - floor).abs().max().item() < 1e-6
-    scale = 4.5689974 * 2
-    energy = torch.exp(ref[:, :m] * scale - 4.2677393)  # the mel energies, un-normalised
-    bound = 1e-4 + 2 * U * (energy.sum(-1, keepdim=True) / energy).sqrt() / scale
+    eps_w = R.bank_eps("kaldi", 128)
+    r = 0.0
+    for b, w in enumerate(wavs):
+        x = torch.zeros(nseg * S)
+        x[:len(w)] = w
+        for s in range(nseg):
+            if s * S < len(w):
+                sb = R.ssast_bounds(x[s * S:(s + 1) * S], eps_w)
+                assert (sb["y"] - ref[b * nseg + s, :m]).abs().max() <= 1e-12
+                r = max(r, R.interval_ratio(got[b * nseg + s, :m], sb["y"], sb["ylo"], sb["yhi"]).max().item())
     d = (got[:, :m] - ref[:, :m]).abs()
-    r = (d / bound).max().item()
     print(f"ssast fbank S={S} ({nseg} windows of {m} frames): max |err| {d.max().item():.2e} (normalised units), "
           f"measured/bound {r:.3f}")
-    assert r < 1.0
+    assert r <= 1.0
 
 
 # ------------------------------------------------------------------------------------------------
