@@ -104,32 +104,41 @@ __device__ __forceinline__ void split_q8_pack2(float a, float b, uint32_t& h16, 
     const float sc = (float)(1 << kQ8ShiftA);
     asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(l8) : "f"(rb * sc), "f"(ra * sc));
 }
-// four consecutive elements -> one 8-byte fp16 store + two 4-byte e4m3 stores
-__device__ __forceinline__ void store_q8x4(const float4& y, __nv_bfloat16* p16, uint8_t* ph8, uint8_t* pl8, size_t elem) {
+// The two e4m3 planes of an operand are stored as ONE interleaved q8 plane of 2 bytes per element: every 32-element
+// chunk of the flat element order is 64 bytes [l8 x 32 | h8 x 32]. A 64-element k-block of a row whose width is a
+// multiple of 64 is then one 128-byte row [l8 k0..31 | h8 k0..31 | l8 k32..63 | h8 k32..63], which the GEMM loads as
+// one box with the 128-byte swizzle. Byte offset of element `elem`, plane p (0 = l8, 1 = h8):
+//   2 elem - (elem & 31) + 32 p  =  elem + (elem & ~31) + 32 p
+__host__ __device__ __forceinline__ size_t q8_off(size_t elem, int p) { return elem + (elem & ~(size_t)31) + 32 * (size_t)p; }
+// bytes of the q8 plane of n elements: the last chunk is whole
+__host__ __device__ __forceinline__ size_t q8_bytes(size_t n) { return 2 * ((n + 31) & ~(size_t)31); }
+
+// four consecutive elements (elem % 4 == 0, so inside one chunk) -> one 8-byte fp16 store + two 4-byte e4m3 stores
+__device__ __forceinline__ void store_q8x4(const float4& y, __nv_bfloat16* p16, uint8_t* q8, size_t elem) {
     uint32_t h0, h1;
     uint16_t a0, a1, b0, b1;
     split_q8_pack2(y.x, y.y, h0, a0, b0);
     split_q8_pack2(y.z, y.w, h1, a1, b1);
+    uint8_t* q = q8 + q8_off(elem, 0);
     *reinterpret_cast<uint2*>(p16 + elem) = make_uint2(h0, h1);
-    *reinterpret_cast<uint32_t*>(ph8 + elem) = (uint32_t)a0 | ((uint32_t)a1 << 16);
-    *reinterpret_cast<uint32_t*>(pl8 + elem) = (uint32_t)b0 | ((uint32_t)b1 << 16);
+    *reinterpret_cast<uint32_t*>(q + 32) = (uint32_t)a0 | ((uint32_t)a1 << 16);
+    *reinterpret_cast<uint32_t*>(q) = (uint32_t)b0 | ((uint32_t)b1 << 16);
 }
 
 // GEMM-operand output of a producer kernel (LayerNorm, conv-0, GEMM epilogues, attention, pos_conv combine):
-// fmt 0 = bf16 hi / lo planes (bf16x3 scheme), fmt 1 = fp16 plane + two e4m3 planes (f16q8 scheme).
+// fmt 0 = bf16 hi / lo planes (bf16x3 scheme), fmt 1 = fp16 plane + the interleaved q8 plane (f16q8 scheme).
 struct OutPlanes {
     __nv_bfloat16* hi;
     __nv_bfloat16* lo;
-    uint8_t* h8;
-    uint8_t* l8;
+    uint8_t* q8;
     int fmt;
 };
-__host__ __device__ inline OutPlanes no_planes() { return OutPlanes{nullptr, nullptr, nullptr, nullptr, 0}; }
+__host__ __device__ inline OutPlanes no_planes() { return OutPlanes{nullptr, nullptr, nullptr, 0}; }
 
 // four consecutive elements starting at element index `elem` (elem % 4 == 0)
 __device__ __forceinline__ void store_planes4(const OutPlanes& o, const float4& y, size_t elem) {
     if (o.fmt != 0) {
-        store_q8x4(y, o.hi, o.h8, o.l8, elem);
+        store_q8x4(y, o.hi, o.q8, elem);
     } else {
         uint32_t h0, l0, h1, l1;
         split_pack2(y.x, y.y, h0, l0);
@@ -145,10 +154,11 @@ __device__ __forceinline__ void store_planes8(const OutPlanes& o, const float (&
         uint16_t a[4], b[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) split_q8_pack2(y[2 * e], y[2 * e + 1], h[e], a[e], b[e]);
+        uint8_t* q = o.q8 + q8_off(elem, 0);
         *reinterpret_cast<uint4*>(o.hi + elem) = make_uint4(h[0], h[1], h[2], h[3]);
-        *reinterpret_cast<uint2*>(o.h8 + elem) =
+        *reinterpret_cast<uint2*>(q + 32) =
             make_uint2((uint32_t)a[0] | ((uint32_t)a[1] << 16), (uint32_t)a[2] | ((uint32_t)a[3] << 16));
-        *reinterpret_cast<uint2*>(o.l8 + elem) =
+        *reinterpret_cast<uint2*>(q) =
             make_uint2((uint32_t)b[0] | ((uint32_t)b[1] << 16), (uint32_t)b[2] | ((uint32_t)b[3] << 16));
     } else {
         uint32_t h[4], l[4];
@@ -164,9 +174,10 @@ __device__ __forceinline__ void store_planes2(const OutPlanes& o, float y0, floa
         uint32_t h;
         uint16_t a, b;
         split_q8_pack2(y0, y1, h, a, b);
+        uint8_t* q = o.q8 + q8_off(elem, 0);
         *reinterpret_cast<uint32_t*>(o.hi + elem) = h;
-        *reinterpret_cast<uint16_t*>(o.h8 + elem) = a;
-        *reinterpret_cast<uint16_t*>(o.l8 + elem) = b;
+        *reinterpret_cast<uint16_t*>(q + 32) = a;
+        *reinterpret_cast<uint16_t*>(q) = b;
     } else {
         uint32_t h, l;
         split_pack2(y0, y1, h, l);
@@ -178,7 +189,7 @@ __device__ __forceinline__ void store_planes2(const OutPlanes& o, float y0, floa
 __device__ __forceinline__ float2 load_planes2(const OutPlanes& o, size_t elem) {
     const uint32_t h = *reinterpret_cast<const uint32_t*>(o.hi + elem);
     if (o.fmt != 0) {
-        const uint16_t l = *reinterpret_cast<const uint16_t*>(o.l8 + elem);
+        const uint16_t l = *reinterpret_cast<const uint16_t*>(o.q8 + q8_off(elem, 0));
         float h0, h1;
         asm("{ .reg .b16 lo, hi; mov.b32 {lo, hi}, %2; cvt.f32.f16 %0, lo; cvt.f32.f16 %1, hi; }"
             : "=f"(h0), "=f"(h1)

@@ -34,9 +34,9 @@ cudaError_t launch_split(const float* x, __nv_bfloat16* hi, __nv_bfloat16* lo, s
 }
 
 // fp32 -> f16q8 planes (common.cuh): activations (weight == 0) or weights (weight != 0: wh8 = e4m3(w * 2^ShiftB),
-// wl8 = e4m3((w - w16) * 2^ShiftD))
+// wl8 = e4m3((w - w16) * 2^ShiftD)), the e4m3 pairs into the interleaved q8 plane
 __global__ void split_q8_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ p16,
-                                uint8_t* __restrict__ h8, uint8_t* __restrict__ l8, size_t n2, int weight) {
+                                uint8_t* __restrict__ q8, size_t n2, int weight) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     for (; i < n2; i += stride) {
@@ -56,19 +56,37 @@ __global__ void split_q8_kernel(const float* __restrict__ x, __nv_bfloat16* __re
             asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(q_l) : "f"((b - hb) * sd), "f"((a - ha) * sd));
         }
         reinterpret_cast<uint32_t*>(p16)[i] = h;
-        reinterpret_cast<uint16_t*>(h8)[i] = q_h;
-        reinterpret_cast<uint16_t*>(l8)[i] = q_l;
+        *reinterpret_cast<uint16_t*>(q8 + q8_off(2 * i, 1)) = q_h;
+        *reinterpret_cast<uint16_t*>(q8 + q8_off(2 * i, 0)) = q_l;
     }
 }
 
-cudaError_t launch_split_q8(const float* x, __nv_bfloat16* p16, uint8_t* h8, uint8_t* l8, size_t n, int weight,
+cudaError_t launch_split_q8(const float* x, __nv_bfloat16* p16, uint8_t* q8, size_t n, int weight,
                             cudaStream_t s) {
     if (n == 0) return cudaSuccess;
     if (n & 1) return cudaErrorInvalidValue;
     const size_t n2 = n / 2;
     size_t blocks = (n2 + 255) / 256;
     if (blocks > 132 * 16) blocks = 132 * 16;
-    split_q8_kernel<<<(unsigned)blocks, 256, 0, s>>>(x, p16, h8, l8, n2, weight);
+    split_q8_kernel<<<(unsigned)blocks, 256, 0, s>>>(x, p16, q8, n2, weight);
+    return cudaGetLastError();
+}
+
+// the interleaved q8 plane of n elements -> separate h8 and l8 planes (the C ABI's back-to-back plane layout)
+__global__ void q8_deinterleave_kernel(const uint8_t* __restrict__ q8, size_t n, uint8_t* __restrict__ h8,
+                                       uint8_t* __restrict__ l8) {
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        h8[i] = q8[q8_off(i, 1)];
+        l8[i] = q8[q8_off(i, 0)];
+    }
+}
+
+cudaError_t launch_q8_deinterleave(const uint8_t* q8, size_t n, uint8_t* h8, uint8_t* l8, cudaStream_t s) {
+    if (n == 0) return cudaSuccess;
+    size_t blocks = (n + 255) / 256;
+    if (blocks > 132 * 16) blocks = 132 * 16;
+    q8_deinterleave_kernel<<<(unsigned)blocks, 256, 0, s>>>(q8, n, h8, l8);
     return cudaGetLastError();
 }
 

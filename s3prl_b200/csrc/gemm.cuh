@@ -17,11 +17,12 @@ struct GemmParams {
     CUtensorMap b_hi, b_lo;
 
     // scheme 1 ("f16q8", bn 128 or 256 only): fp16 main product + two e4m3 correction products.
-    //   a_hi / b_hi are the fp16 planes (box {64, rows}, SWIZZLE_128B), a_h8 / a_l8 / b_h8 / b_l8 the e4m3 planes
-    //   (box {64, rows}, SWIZZLE_64B); a_lo / b_lo are unused. K % 128 == 0, and the kernel walks the 64-wide
-    //   k-blocks twice: num_k_blocks stages of e4m3 corrections, then num_k_blocks of fp16 products.
+    //   a_hi / b_hi are the fp16 planes (box {64, rows}, SWIZZLE_128B), a_q8 / b_q8 the interleaved e4m3 planes
+    //   (common.cuh: q8_off) as byte maps of 2 K bytes per row (box {128, rows}, SWIZZLE_128B: one 64-wide k-block);
+    //   a_lo / b_lo are unused. K % 128 == 0, and the kernel walks the 64-wide k-blocks twice: num_k_blocks stages of
+    //   e4m3 corrections, then num_k_blocks of fp16 products.
     int scheme;
-    CUtensorMap a_h8, a_l8, b_h8, b_l8;
+    CUtensorMap a_q8, b_q8;
 
     // ---- tiling: every k-block is 64 elements of K wide --------------------------------------------------------
     int batches;            // extent of A's 3rd dim that is tiled over
@@ -63,11 +64,10 @@ struct GemmParams {
     float* out_f32;
     __nv_bfloat16* out_hi;
     __nv_bfloat16* out_lo;
-    // out_fmt 1: out_hi is an fp16 plane and out_h8 / out_l8 the two e4m3 planes of the f16q8 operand format;
+    // out_fmt 1: out_hi is an fp16 plane and out_q8 the interleaved e4m3 plane of the f16q8 operand format;
     // out_fmt 0: out_hi / out_lo are the bf16 hi / lo planes.
     int out_fmt;
-    uint8_t* out_h8;
-    uint8_t* out_l8;
+    uint8_t* out_q8;
     float* out_pre;  // optional: v BEFORE the residual add (fc2 output, "fairseq_layers_before_residual"), same layout
 
     // ---- epilogue, QKV scatter mode (qkv_mode != 0): columns [0,D) -> q*scale, [D,2D) -> k, [2D,3D) -> v
@@ -99,7 +99,7 @@ cudaError_t launch_gemm(const GemmParams& p, int sm_count, cudaStream_t stream);
 // Returns 0 on success, else a CUresult / -1 (driver entry point missing).
 int encode_tmap_bf16_3d(CUtensorMap* out, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1,
                         uint64_t stride2, uint32_t box0, uint32_t box1);
-// Same for a 1-byte (e4m3) plane: box0 is 128 elements (SWIZZLE_128B) or 64 elements (SWIZZLE_64B), one swizzle row.
+// Same for a byte plane (the interleaved e4m3 plane): box0 is 128 bytes, one SWIZZLE_128B row. Strides in bytes.
 int encode_tmap_u8_3d(CUtensorMap* out, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1,
                       uint64_t stride2, uint32_t box0, uint32_t box1);
 

@@ -33,16 +33,17 @@ static constexpr int kThreads = 288;
 static constexpr int kPingPongThreads = 384;
 static constexpr int kSmemBudget = 220 * 1024;
 
-// RB: bytes of one K row of a stage plane = the swizzle span. bf16x3: 128 (64 bf16 elements). f16q8: 64, with 64
-// elements of K per stage: pass 0 fills the four planes with 64-byte e4m3 rows [A_l8 A_h8 W_h8 W_l8], pass 1 fills
-// [A16 | W16] with 128-byte fp16 rows (each spanning two planes). Both are 48 KB at BN = 256, which makes the ring
-// four deep there (six at BN = 128).
+// A stage holds 64 elements of K of A (128 rows) and W (BN rows) in rows of 128 bytes with the 128-byte swizzle.
+// bf16x3: four planes [A_hi A_lo W_hi W_lo] of 64 bf16 elements per row. f16q8: one A box and one W box per stage,
+// pass 0 of interleaved e4m3 rows [l8 k0..31 | h8 k0..31 | l8 k32..63 | h8 k32..63] (common.cuh: q8_off), pass 1 of
+// fp16 rows [A16 | W16]. f16q8 stages are 48 KB at BN = 256, which makes the ring four deep there (six at BN = 128).
 template <int BN, int kScheme>
 struct GemmCfg {
-    static constexpr int RB = kScheme == 0 ? 128 : 64;
-    static constexpr int kAPlane = kBlockM * RB;
-    static constexpr int kBPlane = BN * RB;
-    static constexpr int kStageBytes = 2 * kAPlane + 2 * kBPlane;
+    static constexpr int RB = 128;                        // bytes of one box row = the swizzle span
+    static constexpr int kAPlane = kBlockM * RB;          // one A box
+    static constexpr int kBPlane = BN * RB;               // one W box
+    static constexpr int kBoxes = kScheme == 0 ? 2 : 1;   // boxes of A and of W per stage
+    static constexpr int kStageBytes = kBoxes * (kAPlane + kBPlane);
     static constexpr int kStages = (kSmemBudget - 2048) / kStageBytes > 6 ? 6 : (kSmemBudget - 2048) / kStageBytes;
     static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
     static_assert(kStages >= 2, "tile too large for the shared-memory ring");
@@ -113,25 +114,24 @@ __device__ __forceinline__ void produce(const GemmParams& p, uint8_t* smem, uint
                 const int kr = kb - kq * p.kb_per_row;
                 mbar_wait(&empty_bar[stage], phase ^ 1u);
                 uint8_t* st = smem + stage * Cfg::kStageBytes;
-                uint8_t* sb = st + 2 * Cfg::kAPlane;
+                uint8_t* sb = st + Cfg::kBoxes * Cfg::kAPlane;
                 mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)Cfg::kStageBytes);
                 const int a_row = row0 + kq * p.a_row_step + p.a_row_off + (kq >= p.a_gap_at ? p.a_gap : 0);
                 const int a_k = a_k0 + kr * kBlockK;
                 const int b_k = kb * kBlockK;
-                if (kScheme == 1 && pass == 1) {
-                    // [A16 | W16]: one fp16 box of 128-byte rows each, spanning both planes of the stage
-                    load_a<CN, 128>(st, &p.a_hi, &full_bar[stage], a_k, a_row, batch, rank);
-                    tma_load_3d(sb, &p.b_hi, &full_bar[stage], b_k, b_n0, 0);
+                if constexpr (kScheme == 1) {
+                    // one A box and one W box of 128-byte rows: pass 0 the q8 planes (2 bytes per element of K, so
+                    // at twice the fp16 column), pass 1 the fp16 planes
+                    const CUtensorMap* ma = pass == 0 ? &p.a_q8 : &p.a_hi;
+                    const CUtensorMap* mb = pass == 0 ? &p.b_q8 : &p.b_hi;
+                    const int q = pass == 0 ? 2 : 1;
+                    load_a<CN, Cfg::RB>(st, ma, &full_bar[stage], q * a_k, a_row, batch, rank);
+                    tma_load_3d(sb, mb, &full_bar[stage], q * b_k, b_n0, 0);
                 } else {
-                    // planes: scheme 0 [A_hi A_lo W_hi W_lo]; scheme 1 pass 0 [A_l8 A_h8 W_h8 W_l8] (64-byte rows)
-                    const CUtensorMap* ma0 = kScheme == 0 ? &p.a_hi : &p.a_l8;
-                    const CUtensorMap* ma1 = kScheme == 0 ? &p.a_lo : &p.a_h8;
-                    const CUtensorMap* mb0 = kScheme == 0 ? &p.b_hi : &p.b_h8;
-                    const CUtensorMap* mb1 = kScheme == 0 ? &p.b_lo : &p.b_l8;
-                    load_a<CN, Cfg::RB>(st, ma0, &full_bar[stage], a_k, a_row, batch, rank);
-                    load_a<CN, Cfg::RB>(st + Cfg::kAPlane, ma1, &full_bar[stage], a_k, a_row, batch, rank);
-                    tma_load_3d(sb, mb0, &full_bar[stage], b_k, b_n0, 0);
-                    tma_load_3d(sb + Cfg::kBPlane, mb1, &full_bar[stage], b_k, b_n0, 0);
+                    load_a<CN, Cfg::RB>(st, &p.a_hi, &full_bar[stage], a_k, a_row, batch, rank);
+                    load_a<CN, Cfg::RB>(st + Cfg::kAPlane, &p.a_lo, &full_bar[stage], a_k, a_row, batch, rank);
+                    tma_load_3d(sb, &p.b_hi, &full_bar[stage], b_k, b_n0, 0);
+                    tma_load_3d(sb + Cfg::kBPlane, &p.b_lo, &full_bar[stage], b_k, b_n0, 0);
                 }
                 if (++stage == Cfg::kStages) stage = 0, phase ^= 1u;
             }
@@ -203,10 +203,10 @@ __device__ __forceinline__ void mma_tile(const GemmParams& p, uint8_t* smem, uin
         for (int kb = 0; kb < p.num_k_blocks; ++kb) {
             mbar_wait(&full_bar[stage], phase);
             const uint32_t st = smem_u32(smem + stage * Cfg::kStageBytes);
-            const uint32_t b0 = st + 2 * Cfg::kAPlane, b1 = b0 + Cfg::kBPlane;
-            const uint64_t db0 = make_wgmma_desc<RB>(b0), db1 = make_wgmma_desc<RB>(b1);
+            const uint32_t b0 = st + Cfg::kBoxes * Cfg::kAPlane;
             wgmma_fence();
             if constexpr (kScheme == 0) {
+                const uint64_t db0 = make_wgmma_desc<RB>(b0), db1 = make_wgmma_desc<RB>(b0 + Cfg::kBPlane);
 #pragma unroll
                 for (int k = 0; k < RB / 32; ++k) {
                     if (k < k_steps) {
@@ -223,23 +223,23 @@ __device__ __forceinline__ void mma_tile(const GemmParams& p, uint8_t* smem, uin
                         first = false;
                     }
                 }
-            } else if (pass == 0) {  // (kScheme == 1 from here on, RB == 64)
-                // A_l8 x W_h8 and A_h8 x W_l8, K = 32 per MMA (32 bytes), two k-steps per 64-byte row
+            } else if (pass == 0) {  // (kScheme == 1 from here on: one A and one W box of 128-byte rows)
+                // e4m3 MMAs of K = 32 (32 bytes) at byte 32 i of the rows: A chunk i x W chunk i ^ 1 gives
+                // A_l8 x W_h8, A_h8 x W_l8 for k 0..31, then the same for k 32..63 (a half's 64 A rows start
+                // 64 * 128 bytes apart)
+                const uint64_t db = make_wgmma_desc<128>(b0);
 #pragma unroll
-                for (int k = 0; k < 2; ++k) {
-                    const uint64_t ko = (uint64_t)(k * 2);
+                for (int i = 0; i < 4; ++i) {
 #pragma unroll
                     for (int h = 0; h < kHalves; ++h) {
-                        const uint32_t a0 = st + (half0 + h) * 64 * RB, a1 = a0 + Cfg::kAPlane;
-                        const uint64_t da0 = make_wgmma_desc<RB>(a0), da1 = make_wgmma_desc<RB>(a1);
-                        Wgmma<BN, 2>::ss(acc[h], da0 + ko, db0 + ko, first ? 0u : 1u);
-                        Wgmma<BN, 2>::ss(acc[h], da1 + ko, db1 + ko, 1u);
+                        const uint64_t da = make_wgmma_desc<128>(st + (half0 + h) * 64 * 128);
+                        Wgmma<BN, 2>::ss(acc[h], da + (uint64_t)(2 * i), db + (uint64_t)(2 * (i ^ 1)),
+                                         first ? 0u : 1u);
                     }
                     first = false;
                 }
             } else {
-                // A16[k..k+64) x W16[k..k+64), K = 16 per MMA: one box of 128-byte rows each, spanning both
-                // 64-byte planes of the stage (a half's 64 A rows start 64 * 128 bytes apart)
+                // A16[k..k+64) x W16[k..k+64), K = 16 per MMA
                 const uint64_t db = make_wgmma_desc<128>(b0);
 #pragma unroll
                 for (int k = 0; k < 4; ++k) {
@@ -269,9 +269,10 @@ __device__ __forceinline__ void store_plane_pair(const GemmParams& p, float x0, 
         uint32_t h;
         uint16_t a, b;
         split_q8_pack2(x0, x1, h, a, b);
+        uint8_t* q = p.out_q8 + q8_off(off, 0);
         *reinterpret_cast<uint32_t*>(p.out_hi + off) = h;
-        *reinterpret_cast<uint16_t*>(p.out_h8 + off) = a;
-        *reinterpret_cast<uint16_t*>(p.out_l8 + off) = b;
+        *reinterpret_cast<uint16_t*>(q + 32) = a;
+        *reinterpret_cast<uint16_t*>(q) = b;
     } else {
         uint32_t h, l;
         split_pack2(x0, x1, h, l);
@@ -485,10 +486,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_sm90_kernel(const __grid_con
     if (warp == 8 && elect_one()) {
         tma_prefetch_desc(&p.a_hi);
         tma_prefetch_desc(&p.b_hi);
-        if (kScheme == 0) {
-            tma_prefetch_desc(&p.a_lo);
-            tma_prefetch_desc(&p.b_lo);
-        }
+        tma_prefetch_desc(kScheme == 0 ? &p.a_lo : &p.a_q8);
+        tma_prefetch_desc(kScheme == 0 ? &p.b_lo : &p.b_q8);
         for (int s = 0; s < kStages; ++s) {
             mbar_init(&full_bar[s], 1);
             mbar_init(&empty_bar[s], 8);  // one arrive per consumer warp
@@ -540,10 +539,8 @@ __global__ void __launch_bounds__(kPingPongThreads, 1) gemm_sm90_pingpong_kernel
     if (warp == 8 && elect_one()) {
         tma_prefetch_desc(&p.a_hi);
         tma_prefetch_desc(&p.b_hi);
-        if (kScheme == 0) {
-            tma_prefetch_desc(&p.a_lo);
-            tma_prefetch_desc(&p.b_lo);
-        }
+        tma_prefetch_desc(kScheme == 0 ? &p.a_lo : &p.a_q8);
+        tma_prefetch_desc(kScheme == 0 ? &p.b_lo : &p.b_q8);
         for (int s = 0; s < kStages; ++s) {
             mbar_init(&full_bar[s], 1);
             // each stage is consumed by ONE warpgroup of each CTA of the cluster: one arrive per warp
@@ -689,7 +686,7 @@ static cudaError_t launch_n(const GemmParams& p, int sm_count, cudaStream_t stre
 cudaError_t launch_gemm(const GemmParams& p, int sm_count, cudaStream_t stream) {
     if (p.scheme != 0 && p.k_steps != 0) return cudaErrorInvalidValue;
     if (p.gelu < 0 || p.gelu > 4 || (p.res_first != 0 && p.out_pre != nullptr)) return cudaErrorInvalidValue;
-    if (p.out_fmt != 0 && (p.qkv_mode || (p.out_hi != nullptr && (p.out_h8 == nullptr || p.out_l8 == nullptr))))
+    if (p.out_fmt != 0 && (p.qkv_mode || (p.out_hi != nullptr && p.out_q8 == nullptr)))
         return cudaErrorInvalidValue;
     switch (p.bn) {
         case 256: return launch_n<256>(p, sm_count, stream);
@@ -750,15 +747,14 @@ int encode_tmap_u8_3d(CUtensorMap* out, const void* base, uint64_t d0, uint64_t 
                       uint64_t stride2, uint32_t box0, uint32_t box1) {
     PFN_encodeTiled fn = get_encode_fn();
     if (fn == nullptr) return -1;
-    // the swizzle span equals the box row: 128 e4m3 elements -> 128 B, 64 elements -> 64 B
-    if (box0 != 128 && box0 != 64) return -2;
-    const CUtensorMapSwizzle sw = box0 == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+    // the swizzle span equals the box row: 128 bytes
+    if (box0 != 128) return -2;
     cuuint64_t dims[3] = {d0, d1, d2};
-    cuuint64_t strides[2] = {stride1, stride2};  // bytes == elements
+    cuuint64_t strides[2] = {stride1, stride2};  // bytes
     cuuint32_t box[3] = {box0, box1, 1};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<void*>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return (int)r;
 }

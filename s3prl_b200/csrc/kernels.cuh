@@ -14,8 +14,9 @@ cudaError_t launch_split(const float* x, __nv_bfloat16* hi, __nv_bfloat16* lo, s
 cudaError_t launch_wav_pack(const float* const* wavs, const long long* lens, int B, long long Lpad, int normalize,
                             float* mean_rstd_ws, float* out, cudaStream_t s);
 size_t conv0_ws_part_bytes(int B, int L0);
-cudaError_t launch_split_q8(const float* x, __nv_bfloat16* p16, uint8_t* h8, uint8_t* l8, size_t n, int weight,
+cudaError_t launch_split_q8(const float* x, __nv_bfloat16* p16, uint8_t* q8, size_t n, int weight,
                             cudaStream_t s);
+cudaError_t launch_q8_deinterleave(const uint8_t* q8, size_t n, uint8_t* h8, uint8_t* l8, cudaStream_t s);
 cudaError_t launch_conv0_groupnorm(const float* x, int B, long long L, int L0, const float* w, const float* gamma,
                                    const float* beta, double* ws_part, float* ws_scale_shift, const OutPlanes& op,
                                    cudaStream_t s);

@@ -113,22 +113,18 @@ static_assert(!std::is_copy_constructible<DevBuf>::value, "DevBuf owns its alloc
 
 // One GEMM operand in HBM, 4 bytes per element in either format:
 //   fmt 0 (bf16x3 scheme): `hi` = bf16 hi plane, `lo` = bf16 lo plane
-//   fmt 1 (f16q8 scheme) : `hi` = fp16 plane, `lo` holds the two e4m3 planes back to back (h8 at 0, l8 at l8_off)
+//   fmt 1 (f16q8 scheme) : `hi` = fp16 plane, `lo` = the interleaved plane of both e4m3 values (common.cuh: q8_off)
 struct SplitBuf {
     DevBuf hi, lo;
-    size_t l8_off = 0;
     int ensure(size_t elems) {
         S3B_OK(hi.ensure(elems * 2));
-        const size_t before = lo.bytes;
-        S3B_OK(lo.ensure(elems * 2));
-        if (lo.bytes != before) l8_off = (elems + 255) & ~(size_t)255;
+        S3B_OK(lo.ensure(q8_bytes(elems)));
         return 0;
     }
     __nv_bfloat16* h() const { return hi.as<__nv_bfloat16>(); }
     __nv_bfloat16* l() const { return lo.as<__nv_bfloat16>(); }
-    uint8_t* h8() const { return lo.as<uint8_t>(); }
-    uint8_t* l8() const { return lo.as<uint8_t>() + l8_off; }
-    OutPlanes planes(int fmt) const { return OutPlanes{h(), fmt ? nullptr : l(), fmt ? h8() : nullptr, fmt ? l8() : nullptr, fmt}; }
+    uint8_t* q8() const { return lo.as<uint8_t>(); }
+    OutPlanes planes(int fmt) const { return OutPlanes{h(), fmt ? nullptr : l(), fmt ? q8() : nullptr, fmt}; }
 };
 
 // Streams, events and pinned host memory, released on destruction
@@ -346,7 +342,7 @@ static int upload_split(SplitBuf& dst, const float* src, size_t n, int fmt = 0) 
     DevBuf tmp;
     S3B_OK(upload_f32(tmp, src, n));
     S3B_OK(dst.ensure(n));
-    if (fmt != 0) CUDA_OK(launch_split_q8(tmp.as<float>(), dst.h(), dst.h8(), dst.l8(), n, 1, 0));
+    if (fmt != 0) CUDA_OK(launch_split_q8(tmp.as<float>(), dst.h(), dst.q8(), n, 1, 0));
     else CUDA_OK(launch_split(tmp.as<float>(), dst.h(), dst.l(), n, 0));
     CUDA_OK(cudaDeviceSynchronize());
     return 0;
@@ -1459,7 +1455,7 @@ static Epi epi_planes(const OutPlanes& op, const float* bias = nullptr, int gelu
 
 static void set_epi(GemmParams& p, const Epi& e, int ldo) {
     p.bias = e.bias, p.residual = e.residual, p.row_mask = e.row_mask, p.gelu = e.gelu, p.res_first = e.res_first;
-    p.out_f32 = e.out_f32, p.out_hi = e.op.hi, p.out_lo = e.op.lo, p.out_h8 = e.op.h8, p.out_l8 = e.op.l8;
+    p.out_f32 = e.out_f32, p.out_hi = e.op.hi, p.out_lo = e.op.lo, p.out_q8 = e.op.q8;
     p.out_fmt = e.op.fmt, p.ldo = ldo;
     p.qkv_mode = 0;
 }
@@ -1534,7 +1530,9 @@ static int pick_cluster_n(int bn, int n_tiles, int preferred) {
 
 // The A and B tensor maps of one launch in its operand scheme, the one place they are encoded. A: the (k, row, batch)
 // view of [batches][rows][ka] from element a_off of A's planes, rows lda and batches bstride elements apart, boxes
-// {64, a_box}. W: the [N][K] K-major weight, boxes {64, bn}.
+// {64, a_box}. W: the [N][K] K-major weight, boxes {64, bn}. f16q8's q8 planes are the byte views of twice the
+// width (boxes of 128 bytes = 64 elements of K), which hold whole 64-element k-blocks only where ka, lda, bstride and
+// a_off are multiples of 64 (common.cuh: q8_off).
 static int gemm_tmaps(GemmParams& p, int scheme, const SplitBuf& A, size_t a_off, uint64_t ka, uint64_t rows,
                       uint64_t batches, uint64_t lda, uint64_t bstride, uint32_t a_box, const SplitBuf& W, int N, int K,
                       int bn) {
@@ -1542,10 +1540,14 @@ static int gemm_tmaps(GemmParams& p, int scheme, const SplitBuf& A, size_t a_off
     TMAP_OK(encode_tmap_bf16_3d(&p.a_hi, A.h() + a_off, ka, rows, batches, lda, bstride, 64, a_box));
     TMAP_OK(encode_tmap_bf16_3d(&p.b_hi, W.h(), K, N, 1, K, wn, 64, bn));
     if (scheme != 0) {
-        TMAP_OK(encode_tmap_u8_3d(&p.a_h8, A.h8() + a_off, ka, rows, batches, lda, bstride, 64, a_box));
-        TMAP_OK(encode_tmap_u8_3d(&p.a_l8, A.l8() + a_off, ka, rows, batches, lda, bstride, 64, a_box));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_h8, W.h8(), K, N, 1, K, wn, 64, bn));
-        TMAP_OK(encode_tmap_u8_3d(&p.b_l8, W.l8(), K, N, 1, K, wn, 64, bn));
+        if (ka % 64 != 0 || lda % 64 != 0 || bstride % 64 != 0 || a_off % 64 != 0)
+            return fail("f16q8 GEMM: the A operand view (width %llu, rows %llu and batches %llu elements apart, from "
+                        "element %zu) is not 64-aligned", (unsigned long long)ka, (unsigned long long)lda,
+                        (unsigned long long)bstride, a_off);
+        if (K % 64 != 0) return fail("f16q8 GEMM: the weight's K = %d is not a multiple of 64", K);
+        TMAP_OK(encode_tmap_u8_3d(&p.a_q8, A.q8() + 2 * a_off, 2 * ka, rows, batches, 2 * lda, 2 * bstride, 128,
+                                  a_box));
+        TMAP_OK(encode_tmap_u8_3d(&p.b_q8, W.q8(), 2 * (uint64_t)K, N, 1, 2 * (uint64_t)K, 2 * wn, 128, bn));
     } else {
         TMAP_OK(encode_tmap_bf16_3d(&p.a_lo, A.l() + a_off, ka, rows, batches, lda, bstride, 64, a_box));
         TMAP_OK(encode_tmap_bf16_3d(&p.b_lo, W.l(), K, N, 1, K, wn, 64, bn));
@@ -3060,7 +3062,7 @@ static int resolve_scheme(int scheme, int K, int N, int* out) {
 // fp32 -> operand planes of `scheme`, on the stream (weight != 0: the weight split of the f16q8 format)
 static int split_operand(const float* x, SplitBuf& s, size_t n, int scheme, int weight, cudaStream_t st) {
     S3B_OK(s.ensure(n));
-    if (scheme != 0) CUDA_OK(launch_split_q8(x, s.h(), s.h8(), s.l8(), n, weight, st));
+    if (scheme != 0) CUDA_OK(launch_split_q8(x, s.h(), s.q8(), n, weight, st));
     else CUDA_OK(launch_split(x, s.h(), s.l(), n, st));
     return 0;
 }
@@ -3097,14 +3099,22 @@ extern "C" int s3b_linear_ex(const float* a, const float* w, const float* bias, 
     if (gelu < 0 || gelu > 2) return fail("gelu must be 0 (none), 1 (GELU) or 2 (SiLU), not %d", gelu);
     if (o.tile_n != 0 && o.tile_n != 128 && o.tile_n != 256) return fail("tile_n must be 0, 128 or 256, not %d", o.tile_n);
     if (o.tile_n != 0 && N % o.tile_n != 0) return fail("tile_n %d does not divide N = %d", o.tile_n, N);
-    const int64_t lda = o.lda != 0 ? o.lda : K;
-    if (o.a_off < 0 || o.a_off + K > lda || (o.lda != 0 && (lda % 16 != 0 || o.a_off % 16 != 0)))
+    int64_t lda = o.lda != 0 ? o.lda : K, a_off = o.a_off;
+    if (a_off < 0 || a_off + K > lda || (o.lda != 0 && (lda % 16 != 0 || a_off % 16 != 0)))
         return fail("A slice [%lld, %lld) of rows of %lld elements: out of range or not a multiple of 16",
-                    (long long)o.a_off, (long long)(o.a_off + K), (long long)lda);
+                    (long long)a_off, (long long)(a_off + K), (long long)lda);
     cudaStream_t st = (cudaStream_t)stream;
     int sms = 0;
     S3B_OK(device_sm_count(&sms));
     SplitBuf as, ws, os;
+    DevBuf dense;
+    if (scheme != 0 && (lda % 64 != 0 || a_off % 64 != 0)) {
+        // f16q8 reads A's q8 plane in whole 64-element k-blocks: a slice off that grid is split as dense rows
+        S3B_OK(dense.ensure((size_t)M * K * 4));
+        CUDA_OK(cudaMemcpy2DAsync(dense.p, (size_t)K * 4, a + a_off, (size_t)lda * 4, (size_t)K * 4, (size_t)M,
+                                  cudaMemcpyDeviceToDevice, st));
+        a = dense.as<float>(), lda = K, a_off = 0;
+    }
     S3B_OK(split_operand(a, as, (size_t)M * lda, scheme, 0, st));
     S3B_OK(split_operand(w, ws, (size_t)N * K, scheme, 1, st));
     Epi e;
@@ -3116,7 +3126,7 @@ extern "C" int s3b_linear_ex(const float* a, const float* w, const float* bias, 
         e.op = os.planes(o.out_fmt);
     }
     GemmParams p;
-    S3B_OK(linear_params(p, as, ws, M, N, K, scheme, sms, e, lda, (size_t)o.a_off, o.tile_n));
+    S3B_OK(linear_params(p, as, ws, M, N, K, scheme, sms, e, lda, (size_t)a_off, o.tile_n));
     if (o.tile_n != 0 && p.bn != o.tile_n) return fail("tile_n %d requested, %d chosen", o.tile_n, p.bn);
     p.out_pre = o.out_pre;
     CUDA_OK(launch_gemm(p, sms, st));
@@ -3555,7 +3565,7 @@ extern "C" int s3b_wavlm_gate_f32(const float* x, int32_t B, int32_t T, int32_t 
     const size_t M = (size_t)B * T;
     SplitBuf xs;
     S3B_OK(xs.ensure(M * D));
-    if (x_format != 0) CUDA_OK(launch_split_q8(x, xs.h(), xs.h8(), xs.l8(), M * D, 0, st));
+    if (x_format != 0) CUDA_OK(launch_split_q8(x, xs.h(), xs.q8(), M * D, 0, st));
     else CUDA_OK(launch_split(x, xs.h(), xs.l(), M * D, st));
     CUDA_OK(launch_wavlm_gate(xs.planes(x_format), M, B, T, H, D, grep_w, grep_b, grep_a, gate_out, st));
     const cudaError_t se = cudaStreamSynchronize(st);  // before xs is freed
@@ -3608,15 +3618,18 @@ extern "C" int s3b_frontend_f32(const float* const* wavs, const int64_t* lens, i
     return 0;
 }
 
-// The operand planes of fmt over `elems` elements in a caller's buffer, in the layout the *_planes entry points
-// document: whole planes back to back, 4 bytes per element (bf16 hi, bf16 lo; or fp16, e4m3 of the fp16, e4m3 of the
-// residual x 2^11)
-static OutPlanes caller_planes(void* planes, size_t elems, int fmt) {
+// The operand planes of fmt over `elems` elements of `s`, copied into a caller's buffer in the layout the *_planes
+// entry points document: whole planes back to back, 4 bytes per element (bf16 hi, bf16 lo; or fp16, e4m3 of the fp16,
+// e4m3 of the residual x 2^11). The f16q8 q8 plane is de-interleaved on the way.
+static int copy_caller_planes(const SplitBuf& s, size_t elems, int fmt, void* planes, cudaStream_t st) {
     char* p = static_cast<char*>(planes);
-    __nv_bfloat16* p16 = reinterpret_cast<__nv_bfloat16*>(p);
-    return fmt ? OutPlanes{p16, nullptr, reinterpret_cast<uint8_t*>(p + 2 * elems),
-                           reinterpret_cast<uint8_t*>(p + 3 * elems), 1}
-               : OutPlanes{p16, reinterpret_cast<__nv_bfloat16*>(p + 2 * elems), nullptr, nullptr, 0};
+    CUDA_OK(cudaMemcpyAsync(p, s.hi.p, 2 * elems, cudaMemcpyDeviceToDevice, st));
+    if (fmt != 0)
+        CUDA_OK(launch_q8_deinterleave(s.q8(), elems, reinterpret_cast<uint8_t*>(p + 2 * elems),
+                                       reinterpret_cast<uint8_t*>(p + 3 * elems), st));
+    else
+        CUDA_OK(cudaMemcpyAsync(p + 2 * elems, s.lo.p, 2 * elems, cudaMemcpyDeviceToDevice, st));
+    return 0;
 }
 
 // add_fbank_frontend's step for a DeCoAR 2.0 (step 2) or APC (step 1) model. The log-mel and the operand planes go to
@@ -3654,15 +3667,11 @@ static int fbank_cmvn_features(const float* const* wavs, const int64_t* lens, in
         S3B_OK(fbuf.ensure((size_t)B * mf * 80 * 4));
         logmel = fbuf.as<float>();
     }
-    OutPlanes op;
     const size_t elems = rows * kDecoar2K;
-    if (planes != nullptr) {
-        op = caller_planes(planes, elems, out_fmt);
-    } else {
-        S3B_OK(os.ensure(elems));
-        op = os.planes(out_fmt);
-    }
+    S3B_OK(os.ensure(elems));
+    const OutPlanes op = os.planes(out_fmt);
     CUDA_OK(launch_decoar2_features(book.as<const float*>(), d_lens, B, (int)mf, (int)T, step, logmel, op, st));
+    if (planes != nullptr) S3B_OK(copy_caller_planes(os, elems, out_fmt, planes, st));
     if (out != nullptr) {
         S3B_OK(dec.ensure(elems * 4));
         CUDA_OK(launch_planes_to_f32(op, elems, dec.as<float>(), st));
@@ -3749,7 +3758,10 @@ extern "C" int s3b_ssast_patch_planes(const float* feat, int32_t SB, int32_t TL,
     const SsastGeom g = ssast_geom(c);
     const size_t an = patch ? (size_t)SB * g.P * 256 : (size_t)SB * TL * 128;
     cudaStream_t st = (cudaStream_t)stream;
-    CUDA_OK(launch_ssast_patches(feat, SB, TL, g.patch_f, g.tdim, caller_planes(planes, an, fmt), st));
+    SplitBuf as;
+    S3B_OK(as.ensure(an));
+    CUDA_OK(launch_ssast_patches(feat, SB, TL, g.patch_f, g.tdim, as.planes(fmt), st));
+    S3B_OK(copy_caller_planes(as, an, fmt, planes, st));
     CUDA_OK(cudaStreamSynchronize(st));
     return 0;
 }
@@ -3769,7 +3781,7 @@ extern "C" int s3b_ssast_fold_f32(const float* x, int32_t B, int32_t nseg, int32
 }
 
 // MAE-AST's front end step (add_mae_ast_input) on buffers of the call: out (fp32), planes_out (the operand planes
-// decoded) and raw (the operand planes themselves, caller_planes' layout), each optional
+// decoded) and raw (the operand planes themselves, copy_caller_planes' layout), each optional
 static int mae_ast_fbank(const float* const* wavs, const int64_t* lens, int32_t B, int64_t max_len, int32_t patch,
                          float running_mean, float running_var, int32_t fmt, float* out, float* planes_out, void* raw,
                          void* stream) {
@@ -3802,17 +3814,15 @@ static int mae_ast_fbank(const float* const* wavs, const int64_t* lens, int32_t 
     if (out != nullptr)
         CUDA_OK(launch_mae_ast_fbank(book.as<const float*>(), d_lens, B, (int)Tp, g.kt, g.kc, bn_a, bn_c, out,
                                      no_planes(), st));
-    if (planes_out != nullptr) {
+    if (planes_out != nullptr || raw != nullptr) {
         SplitBuf os;
         S3B_OK(os.ensure(elems));
         CUDA_OK(launch_mae_ast_fbank(book.as<const float*>(), d_lens, B, (int)Tp, g.kt, g.kc, bn_a, bn_c, nullptr,
                                      os.planes(fmt), st));
-        CUDA_OK(launch_planes_to_f32(os.planes(fmt), elems, planes_out, st));
-        CUDA_OK(cudaStreamSynchronize(st));
+        if (planes_out != nullptr) CUDA_OK(launch_planes_to_f32(os.planes(fmt), elems, planes_out, st));
+        if (raw != nullptr) S3B_OK(copy_caller_planes(os, elems, fmt, raw, st));
+        CUDA_OK(cudaStreamSynchronize(st));  // before os is freed
     }
-    if (raw != nullptr)
-        CUDA_OK(launch_mae_ast_fbank(book.as<const float*>(), d_lens, B, (int)Tp, g.kt, g.kc, bn_a, bn_c, nullptr,
-                                     caller_planes(raw, elems, fmt), st));
     CUDA_OK(cudaStreamSynchronize(st));
     return 0;
 }

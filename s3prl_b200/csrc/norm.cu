@@ -203,7 +203,10 @@ cudaError_t launch_layernorm_rope(const float* x, size_t M, int T, int D, const 
 // z: [B][T + 3][G][4][cpg] fp32
 // ------------------------------------------------------------------------------------------------
 template <int V4>
-__global__ void __launch_bounds__(256) posconv_combine_kernel(const float* __restrict__ z, const float* __restrict__ x,
+// 640 channels: left to itself, ptxas picks 48 registers for this instantiation and spills there since the f16q8
+// plane stores (store_planes4) compute the interleaved q8 offset; a bound of 4 blocks per SM lets it take 64. The
+// kernel writes the encoder's operand planes, which is why the operand layout reaches it.
+__global__ void __launch_bounds__(256, V4 == 5 ? 4 : 0) posconv_combine_kernel(const float* __restrict__ z, const float* __restrict__ x,
                                                               const float* __restrict__ bias, int B, int T, int cpg,
                                                               const float* __restrict__ gamma,
                                                               const float* __restrict__ beta, int do_ln, int mode,
